@@ -5,9 +5,9 @@ Numba-CUDA path on 1 GPU ... in the same run").
 
 Runs in its OWN process (bench.py spawns it before it touches CUDA itself) so that numba's CUDA context, its JIT
 cache and the reference's import-time GPU query never share a process with the engine.  The reference is used
-UNMODIFIED through its public API, imported from where it lies: /root/reference (build container) or the
-git-ignored scratch copy baseline/_ref/ that travels with the snapshot to the GPU box; nothing of it is copied into
-the repository.  One shim: ``np.float = float`` (mppi_numba/mppi.py:32-33 uses the alias numpy removed).
+UNMODIFIED through its public API, imported from the git-ignored bytecode build() compiled under oracle/_ref/
+(oracle/ref_build.py); nothing of it is copied into the repository.  One shim: ``np.float = float``
+(mppi_numba/mppi.py:32-33 uses the alias numpy removed).
 
     python baseline/numba_cuda_leg.py c5 [c3 c2 c4]      ->  ONE JSON line on stdout
 
@@ -28,22 +28,17 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 
 
-def locate():
-    for cand in ("/root/reference", os.path.join(HERE, "_ref")):
-        if os.path.isdir(os.path.join(cand, "mppi_numba")):
-            return cand
-    return None
-
-
 def main():
     real_stdout = os.dup(1)
     os.dup2(2, 1)                                   # the reference prints; keep stdout for the one JSON line
 
     def emit(obj):
         os.write(real_stdout, (json.dumps(obj) + "\n").encode())
-    ref_root = locate()
+    sys.path.insert(0, ROOT)
+    from oracle.ref_build import compiled_reference
+    ref_root = compiled_reference()
     if ref_root is None:
-        return emit({"unavailable": "reference package not found (/root/reference, baseline/_ref)"})
+        return emit({"unavailable": "compiled reference not found (oracle/_ref)"})
     try:
         import numpy as np
         np.float = float

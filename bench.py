@@ -1,8 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- rollouts/s (N*M*T state-steps per solve / time) of the MPPI hot path on B200.
+"""bench.py -- rollouts/s (N*M*T state-steps per solve / time) of the MPPI hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload c5|c3|c2|c4]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
+
+The K timed solves start from the planner's state right after set-up (the warm-up solves are rolled back), so the
+same arguments give the same inputs in every run; --dump-outputs DIR writes what the last of them computed.
 
 A "step" is one MPPI_Numba.solve() (num_opt = 1): control noise, both traction-distribution maps sampled (M maps
 each), N x M x T rollouts with cost accumulation, CVaR over M, softmax update, D2H of the T x 2 control sequence.
@@ -16,9 +20,11 @@ own peer-memory kernels over NVLink (B200MPPI_EXCHANGE=nccl: by two NCCL collect
 `e2e`    : the same metric through the public Python API from HOST buffers -- every step does
            shift_and_update(x0, u) (H2D of the T x 2 warm start + the params POD) and solve()
            (D2H of the T x 2 result), wall-clock, max over ranks.
-`roofline`: the dominant kernel's algorithmic bytes / its CUDA-event time vs the measured HBM peak, and -- because
-           ncu shows both dominant kernels bound by instruction issue, not by HBM -- its warp instructions
-           (ncu, profiles/) / its time vs the SM issue peak (148 SMs x 4 schedulers x the SM clock sampled here).
+`roofline`: the dominant kernel's algorithmic bytes / its CUDA-event time vs the measured (or data-sheet) HBM peak.
+           Only when an ncu capture summary is stored in profiles/kernel_metrics.json (tools/ncu_target.py,
+           tools/ncu_summary.py) for this workload: `bound`, the resource the capture shows saturated, and `issue`,
+           its warp instructions / its time vs the SM issue peak (the device's SMs x 4 schedulers x the SM clock
+           sampled here); otherwise both are null.
 `parity_check` (N > 1): before the timed region the sharded solve is checked on the real GPUs against a 1-rank
            solve of the same scenario and seed run by rank 0: u identical on all ranks, u vs 1-rank within 1e-5,
            every rank's CVaR-cost slice bit-identical to the 1-rank costs.  A failure exits non-zero.
@@ -204,7 +210,7 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3, not measured)"
 
 
 # ----------------------------------------------------------------------------- algorithmic bytes (DESIGN.md)
@@ -239,9 +245,10 @@ def algorithmic_bytes(sc, cfg, n_local, m_local, box=None):
 
 
 def kernel_metrics(workload):
-    """ncu figures of the dominant kernels (per launch: DRAM bytes, warp instructions) from the committed capture
-    summary profiles/kernel_metrics.json -- written from an `ncu --set full` capture of tools/ncu_target.py; the
-    live part of the roofline (kernel time, SM clock) is measured here."""
+    """ncu figures of the dominant kernels (per launch: DRAM bytes, warp instructions) from a capture summary stored
+    as profiles/kernel_metrics.json (tools/ncu_summary.py of an `ncu --set full` capture of tools/ncu_target.py), or
+    None when there is none for this workload (none is committed); the live part of the roofline (kernel time, SM
+    clock) is measured here."""
     try:
         with open(os.path.join(ROOT, "profiles", "kernel_metrics.json")) as f:
             j = json.load(f)
@@ -301,6 +308,15 @@ def workload_name_of(name):
     mode, N, M, T, H, res, B, da = WORKLOADS[name]
     return "%s: %s MPPI N=%d M=%d T=%d, %dx%d PMF grid (%d bins, res %.1f m), num_opt=1" % (
         name, {"tdm": "CVaR-cost", "det": "CVaR-dynamics"}[mode], N, M, T, H, H, B, res)
+
+
+def dump_outputs(out_dir, **arrays):
+    """--dump-outputs: what the last timed solve() computed, one DIR/<name>.npy per array: `u`, the (T, 2)
+    control sequence solve() returns, and `costs`, the (N,) per-rollout costs the update weighed (all ranks' slices in
+    n order), so that dumps compare output for output whatever the number of GPUs."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def _quiet():
@@ -445,7 +461,7 @@ def run_b200(args, sc):
     if world != args.gpus:
         raise SystemExit("--gpus %d but WORLD_SIZE=%d: launch with torch.distributed.run" % (args.gpus, world))
     import __graft_entry__
-    __graft_entry__.build()
+    __graft_entry__.build_engine()
     import mppi_numba_b200 as E
     torch.cuda.set_device(local)
     pg = None
@@ -496,6 +512,9 @@ def run_b200(args, sc):
             raise SystemExit(3)
 
     # ---- device-timed region: K solves, inputs resident
+    # The warm-up and settle solves run a wall-clock-dependent number of times; the planner is put back to this
+    # checkpoint (warm start + RNG streams) before the timed solves, so that those see the same inputs in every run.
+    st0 = pl.get_state()
     clocks = ClockSampler(local)          # started before the warm-up: nvidia-smi needs ~0.3 s to produce a sample
     t_w = time.perf_counter()
     for _ in range(args.warmup):
@@ -507,6 +526,7 @@ def run_b200(args, sc):
     n_settle = int(max_over_ranks(float(min(5000, int(0.5 / per_solve) + 1))))
     for _ in range(n_settle):
         pl.solve()
+    pl.set_state(st0)
     barrier()
     clocks.lines.clear()
     l0 = pl.launch_count()          # includes the TDM kernels launched inside solve()
@@ -517,6 +537,15 @@ def run_b200(args, sc):
             u = pl.solve()
         e1.record(stream)
     barrier()
+    if args.dump_outputs:
+        costs = pl.costs_d.copy_to_host()
+        if world > 1:                        # every rank holds the costs of its block of control sequences
+            import torch.distributed as dist
+            parts = [None] * world
+            dist.all_gather_object(parts, costs)
+            costs = np.concatenate(parts)    # rank slices in rank order = n order
+        if rank == 0:
+            dump_outputs(args.dump_outputs, u=u, costs=costs)
     ms = max_over_ranks(e0.elapsed_time(e1)) / args.steps
     launches = pl.launch_count() - l0      # kernels launched in the timed region
     # very short timed region: extend the load for the clock sampler only (same count on every rank)
@@ -562,22 +591,23 @@ def run_b200(args, sc):
     km = kernel_metrics(args.workload) if world == 1 else None
     kd = (km or {}).get("kernels", {}).get(dom)
     if dom == "sample_grids" and not box[0]:
-        kd = None                         # the committed capture is of the boxed launch
+        kd = None                         # a stored capture is of the boxed launch
     traffic = kd.get("dram_bytes") if kd else None
-    sm_hz = (clk.get("sm_mhz") or 1965.0) * 1e6
-    issue_peak = 148 * 4 * sm_hz
+    sm_hz = (clk.get("sm_mhz") or 1980.0) * 1e6                     # fallback: the H100 SXM's maximum SM clock
+    issue_peak = torch.cuda.get_device_properties(dev).multi_processor_count * 4 * sm_hz
     issue = None
     if kd and kd.get("warp_inst"):
         rate = kd["warp_inst"] / (dom_ms * 1e-3)
         issue = {"warp_inst": kd["warp_inst"], "peak_warp_inst_per_s": issue_peak, "achieved_warp_inst_per_s": rate,
                  "frac": rate / issue_peak, "sm_mhz": sm_hz / 1e6,
                  "source": "smsp__inst_executed.sum of %s (%s), live kernel time and SM clock" % (kd.get("kernel", dom), km.get("capture"))}
-    roofline = {"bound": (kd or {}).get("bound", "issue" if sc["mode"] == "tdm" else "latency"),
+    roofline = {"bound": (kd or {}).get("bound"),
                 "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
                 "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": dom_bytes, "kernel_ms": dom_ms,
-                "note": "achieved/peak/frac are the HBM figures of the contract; `bound` is the resource ncu shows "
-                        "saturated for this kernel (profiles/), `issue` its instruction-issue roofline",
+                "note": "achieved/peak/frac are the HBM figures of the contract; `bound` (the resource an ncu capture "
+                        "shows saturated) and `issue` (the instruction-issue roofline) are null without a stored capture "
+                        "for this workload (profiles/kernel_metrics.json)",
                 "issue": issue,
                 "solve_algorithmic_bytes": ab["total"],
                 "solve_frac_of_hbm_roofline": (ab["total"] / (ms * 1e-3) / 1e9) / peak,
@@ -661,7 +691,13 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-numba", action="store_true", help="skip the reference's Numba-CUDA leg (N = 1)")
     ap.add_argument("--no-others", action="store_true", help="skip the other BASELINE configs (N = 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed solve as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl != "b200":
+        ap.error("--dump-outputs needs --impl b200")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     sc = build_scenario(args.workload)
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * b200mppi.h -- C-ABI of the B200-native MPPI rollout-and-reduction engine.
+ * b200mppi.h -- C-ABI of the H100-native MPPI rollout-and-reduction engine.
  *
  * This is the drop-in boundary for the ONE hot path of mit-acl/mppi_numba:
  *   MPPI_Numba.solve()  (reference mppi_numba/mppi.py:186-211)  =

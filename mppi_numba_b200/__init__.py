@@ -1,8 +1,8 @@
-"""mppi_numba_b200 -- B200-native drop-in for the hot path of mit-acl/mppi_numba.
+"""mppi_numba_b200 -- H100-native drop-in for the hot path of mit-acl/mppi_numba.
 
     from mppi_numba_b200 import Config, TDM_Numba, MPPI_Numba        # same names as the reference
 
-Python (this package) -> ctypes -> libb200mppi.so (include/b200mppi.h) -> hand-written sm_100a CUDA.
+Python (this package) -> ctypes -> libb200mppi.so (include/b200mppi.h) -> hand-written sm_90a CUDA.
 Importing the package needs the built library (``python mppi_numba_b200/build.py``); creating a
 planner or TDM needs a CUDA device.  There is no CPU fallback.
 """

@@ -45,7 +45,7 @@ def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             "mppi_numba_b200: %s is missing. Build it with `python mppi_numba_b200/build.py` "
-            "(nvcc, sm_100a). There is no CPU fallback." % LIB_PATH)
+            "(nvcc, sm_90a). There is no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     P, I32, I64, F, D, SZ = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_double, C.c_size_t
     sigs = {

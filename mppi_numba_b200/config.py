@@ -6,7 +6,7 @@ touch a GPU (the reference queries the device at import, config.py:9-12, SURVEY.
 limits it used to read from the device are the constants every CUDA device since sm_30 reports.
 """
 
-# Limits the reference read from the device (identical on a B200).
+# Limits the reference read from the device (identical on an H100).
 max_threads_per_block = 1024
 max_square_block_dim = (32, 32)          # (int(1024**0.5),) * 2
 max_blocks = 2 ** 31 - 1

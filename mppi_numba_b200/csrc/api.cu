@@ -111,9 +111,8 @@ static int tdm_prepare_jump(b200mppi_tdm* t, cudaStream_t st) {
   const int tx = t->cfg.tdm_thread_x, ty = t->cfg.tdm_thread_y;
   const int nrow = (t->rows + tx - 1) / tx, ncol = (t->cols + ty - 1) / ty;
   const int groups = (t->num_maps + 7) / 8;
-  // enough CTAs (~4k, i.e. several waves of the 5 resident CTAs per SM) to keep 148 SMs busy through the
-  // tail; measured on config 5: 1 / 2 / 4 / 8 segments -> 1.63 / 1.50 / 1.37 / 1.32 ms.  A rank holding M/8 = 32
-  // maps (8 GPUs) needs 2-row segments (33 of them): 0.183 ms against 0.208 ms with 16 (tools/sampler_segs.py)
+  // enough CTAs (~4k, i.e. several waves of the 5 resident CTAs per SM) to keep every SM busy through the
+  // tail; a rank holding M/8 = 32 maps (8 GPUs) gets 2-row segments (33 of them; sweep: tools/sampler_segs.py)
   int segs = (4096 + tx * groups - 1) / (tx * groups);
   if (const char* e = getenv("B200MPPI_SAMPLE_SEGS")) segs = atoi(e);      // tuning / test hook
   if (segs > SAMPLE_MAX_SEGS) segs = SAMPLE_MAX_SEGS;
@@ -149,9 +148,10 @@ static int tdm_prepare_jump(b200mppi_tdm* t, cudaStream_t st) {
   int rc = upload_set(t->jump_d, segs, seg_rows);
   if (rc) return rc;
   // a boxed launch covers a few tile rows only: finer row segments keep every SM busy through several waves
-  // (measured on config 5 with whole-map segment sizes: 24 % of the SM-cycles idle in the tail, profiles/)
-  // ~3 waves of the ~6 resident CTAs per SM, for a box of ~8 tile rows sampled ~14 maps per CTA
-  int bsegs = (3 * 6 * 148 + 8 * ((t->num_maps + 13) / 14) - 1) / (8 * ((t->num_maps + 13) / 14));
+  // (with whole-map segment sizes a large share of the SM-cycles sits idle in the tail)
+  // ~3 waves of the ~6 resident CTAs per SM, for a box of ~8 tile rows sampled ~14 maps per CTA (the segment count
+  // only splits the work: every segment starts from its generator's jumped state, the draws are the same)
+  int bsegs = (3 * 6 * device_sm_count() + 8 * ((t->num_maps + 13) / 14) - 1) / (8 * ((t->num_maps + 13) / 14));
   if (const char* e = getenv("B200MPPI_SAMPLE_BOX_SEGS")) bsegs = atoi(e);
   if (bsegs > SAMPLE_BOX_MAX_SEGS) bsegs = SAMPLE_BOX_MAX_SEGS;
   if (bsegs > nrow) bsegs = nrow;
@@ -1039,8 +1039,8 @@ static int stage_rollout(b200mppi_planner* p) {
       w.WW = WW; w.WH = WH;
       const int xi0 = (int)std::floor(((double)p->prm.x0[0] - (double)l->pxl[0]) / (double)l->res);
       const int yi0 = (int)std::floor(((double)p->prm.x0[1] - (double)l->pyl[0]) / (double)l->res);
-      // TMA: the inner (x) start coordinate must be 16-byte aligned for 1-byte elements (probed on B200:
-      // an unaligned c0 raises 'illegal instruction'); floor to a multiple of 16, also for negatives
+      // TMA: the inner (x) start coordinate is kept 16-byte aligned for 1-byte elements (an unaligned c0 faulted
+      // with 'illegal instruction' when probed); floor to a multiple of 16, also for negatives
       // The window is kept INSIDE the map (origin clamped, extents cut): a staged cell is then always a map cell, and
       // every index outside the map takes the global-memory path with the generic kernel's wrap + clamp.
       int cx = xi0 - WW / 2, cy = yi0 - WH / 2;

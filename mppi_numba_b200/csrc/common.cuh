@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the B200 MPPI engine (sm_100a only).
+// common.cuh -- shared device helpers of the MPPI engine (sm_90a, H100).
 //
 // The arithmetic helpers mirror, instruction for instruction, what NVVM emits for the reference's
 // Numba kernels with fastmath=True (PTX census: SURVEY.md 2.3; re-derived with
@@ -57,7 +57,7 @@ __device__ __forceinline__ float d2f(double a) {          // cvt.rn.ftz.f32.f64
 // (numba/cpython/numbers.py real_divmod -> abs, div.rn, floor, remainder, div.full, sign fix, floor,
 // snap-to-nearest, cvt.rzi).  NVVM emits the remainder as `mul.ftz.f32` + `sub.ftz.f32` WITHOUT a
 // rounding modifier, which ptxas contracts into one FFMA (verified in the SASS of the reference's
-// PTX and by state traces against the reference on a B200: profiles/r01_*): the remainder is exact,
+// PTX and by state traces against the reference on the GPU): the remainder is exact,
 // so the sequence yields the true floor of a/res.  `a` is already the float32 difference x - lo.
 // [emu:begin cell_index]
 static __device__ __noinline__ int cell_index_exact(float a, float r) {

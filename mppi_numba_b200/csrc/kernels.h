@@ -152,6 +152,7 @@ void launch_noise_prepare(uint64_t* states, float* noise, const float* u_cur, fl
 bool make_u8_tensor_map(void* out_map, const void* base, int rank, int cols, int rows, int maps, int pitch,
                         int WW, int WH);
 void rollout_win_geometry(int T, int* WW, int* WH, size_t* smem);
+int device_sm_count();                          // SMs of the current device (cached per device)
 void rollout_win_set_debug(long long* dev);    // device buffer of 4 int64 per CTA (<= 1024 CTAs) or null
 cudaError_t launch_rollout_win(const RolloutWinArgs& a, const void* tm_lin, const void* tm_ang, const void* tm_obs,
                                const void* tm_unk, cudaStream_t st);

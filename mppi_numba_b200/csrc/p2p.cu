@@ -1,7 +1,7 @@
 // Peer-memory (NVLink / NVSwitch) exchange for the sharded solve: the two collectives of a multi-rank
 // solve() -- the all-to-all of per-(n,m) rollout costs and the all-gather of the (2T+2)-float softmax
 // partials -- done by this library's own kernels with plain stores into the peers' memory plus epoch flags,
-// instead of two NCCL calls (about 52 + 17 us of fixed latency at 8 GPUs against a 0.65 ms solve).
+// instead of two NCCL calls, whose fixed latency is a large part of a sharded solve (tools/nccl_latency.py).
 //
 // Protocol (one "exchange" = one epoch e, a counter that only grows):
 //   producer rank r:  data stores into peer d's buffer -> __threadfence_system() -> flags_d[r] = e (st.release.sys)

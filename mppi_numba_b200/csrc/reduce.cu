@@ -57,7 +57,8 @@ __device__ __forceinline__ float softmax_weight(float c, float beta, float lambd
 constexpr int UPD_THREADS = 256;
 
 int update_num_ctas(int N) {
-  // slabs of >= 32 rollouts; at most 2 CTAs per SM of a B200 (148 SMs)
+  // slabs of >= 32 rollouts, at most 296 CTAs (~2 per SM of an H100).  A constant, not the device's SM count:
+  // the CTA partition fixes the summation order of u, which must not depend on the GPU it runs on
   int ctas = (N + 31) / 32;
   if (ctas > 296) ctas = 296;
   if (ctas < 1) ctas = 1;

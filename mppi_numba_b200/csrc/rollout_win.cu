@@ -1,4 +1,4 @@
-// rollout_win.cu -- the stochastic ("CVaR-cost") rollout kernel as it is meant to run on a B200:
+// rollout_win.cu -- the stochastic ("CVaR-cost") rollout kernel as it is meant to run on an H100 (sm_90a):
 // a persistent CTA per SM works on ONE sampled traction map at a time; the window of that map around the robot
 // (linear and angular traction planes of map m, plus the obstacle / unknown planes shared by all maps) is staged
 // into shared memory with four TMA tensor loads (cp.async.bulk.tensor), after which every per-step lookup of the
@@ -186,7 +186,7 @@ void launch_prepare_rollout(const float* noise, const float* u_cur, float* noise
 }
 
 // ---------------------------------------------------------------------------------------------
-// TMA plumbing (sm_90+/sm_100a): mbarrier + cp.async.bulk.tensor
+// TMA plumbing (sm_90a): mbarrier + cp.async.bulk.tensor
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -253,8 +253,8 @@ __constant__ double k_veltkamp_c = 536870913.0;
 // WIN_ROUND_FP64 = 1 (default): Veltkamp's splitting on the FP64 pipe -- g = RN(a * (2^29 + 1)), hi = RN(g + RN(a - g))
 // is a rounded to 53 - 29 = 24 significant bits, ties to even (three round-to-nearest operations that must not be
 // contracted into an FMA: hence the intrinsics; pinned against the float32 conversion on 10^7 near-tie values in
-// tests/test_rollout_win_emulated_cpu.py).  Three FP64-pipe instructions (that pipe is ~10 % busy) instead of the five
-// integer instructions of the bit-level version below (ncu: the integer pipe is where this kernel's warps queue).
+// tests/test_rollout_win_emulated_cpu.py).  Three FP64-pipe instructions (a lightly used pipe in this kernel) instead of
+// the five integer instructions of the bit-level version below (the integer pipe is the busier one).
 // A zero loses its sign (-0 -> +0), which no later operation of the step can see.
 __device__ __forceinline__ double round_to_f32_precision(double a) {
 #if WIN_ROUND_FP64
@@ -270,9 +270,8 @@ __device__ __forceinline__ double round_to_f32_precision(double a) {
 // obstacle / unknown penalties (mppi.py:700-701), inside a branch taken when either mask byte is non-zero (a tenth of the
 // warp-steps at BASELINE config 5, up to half for the control sequences that graze obstacles).  Inline and off the XU
 // pipe: float(v) of the int8 mask value by the magic-number trick (exact for |v| < 2^22) instead of I2F -- as an
-// out-of-line call with two conversions queued behind the other warps' MUFU / F2F work the branch cost ~700 cycles per
-// visit (measured with the per-CTA debug hook), which made the CTAs whose rollouts cross obstacles the stragglers of
-// the grid.
+// out-of-line call with two conversions queued behind the other warps' MUFU / F2F work the branch was expensive
+// enough to make the CTAs whose rollouts cross obstacles the stragglers of the grid.
 static __device__ __forceinline__ float add_penalties(float cost, int ob, int un, float obs_cost, float unk_cost) {
   const float fo = fsub(__int_as_float(0x4B400000 + ob), 12582912.0f);
   const float fu = fsub(__int_as_float(0x4B400000 + un), 12582912.0f);
@@ -349,7 +348,7 @@ constexpr int WIN_WW = 240;       // window width in cells (inner TMA box extent
 // Work distribution: PERSISTENT grid, one CTA per SM.  The work list is the map-major sequence of 32-rollout chunks
 // (map m, control sequences [32c, 32c + 32)); CTA b owns the contiguous share [b*total/G, (b+1)*total/G) of it --
 // every SM gets the same number of chunks whatever M and N are (a (tiles, M) grid of one-tile CTAs quantises: 256
-// tile units on 148 SMs at 8 GPUs = two rounds where 1.73 would do).  A share spans one to a few maps: per map the
+// tile units on 132 SMs = two rounds where 1.94 would do).  A share spans one to a few maps: per map the
 // CTA stages that map's window once (thread 0 issues the TMA loads after the CTA has left the previous window), then
 // its warps pull chunks from a shared-memory counter until the map's part of the share is done -- warps whose
 // rollouts reached the goal early simply take the next chunk.  Short shares (a rank of a 4- or 8-GPU solve): see
@@ -386,12 +385,11 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
   const long long total = (long long)p.M * cpm;
   // share boundaries are multiples of a.unit chunks (32 = one chunk per warp of the CTA when the shares are long
   // enough: every map segment is then a whole number of passes and all warps reach the end-of-segment barrier
-  // together -- ncu showed 0.8 of 7.8 warps parked there with chunk-granular shares; 1 for short shares)
+  // together, where chunk-granular shares leave warps parked at that barrier; 1 for short shares)
   //
   // a.unit == 0 (short shares and at least one CTA per map: the 8-GPU regime): shares never cross a map.  Map m gets q
   // or q + 1 of the CTAs (q = CTAs / maps) and its chunks are split evenly among them.  A share that crosses a map
-  // boundary costs a second window and, worse, two partial passes (a handful of warps running alone twice): measured
-  // at 32 maps on 148 CTAs, such CTAs took 81-145 us against 57 us for the others.
+  // boundary costs a second window and, worse, two partial passes (a handful of warps running alone twice).
   long long w_lo, w_hi;
   if (a.unit == 0) {
     const int G = (int)gridDim.x, b = ((int)blockIdx.x + a.rotate) % (int)gridDim.x, q = G / p.M, r = G - q * p.M;    // the first r maps get q + 1 CTAs
@@ -535,7 +533,7 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
       const double dv = lds_f64(sb_lutL + (uint32_t)(ql * 8)) * c2.x;
       const float cs = cos_approx(th);
       const float sn = sin_approx(th);
-      // float64 copies of the float32-rounded state, without a second XU-pipe conversion (widen(narrow(.)) measured
+      // float64 copies of the float32-rounded state, without a second XU-pipe conversion (widen(narrow(.)) was
       // slower: the XU pipe is this kernel's busiest)
       const double x64 = round_to_f32_precision(rx);
       const double y64 = round_to_f32_precision(ry);
@@ -586,7 +584,7 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
   if (a.sig.ws > 0) {
     // one fence per CTA: the barrier orders every thread's cost stores before thread 0, whose (cumulative) system-scope
     // fence then orders them before its ticket -- the pattern of a cooperative grid barrier.  (A fence by each of the
-    // 1024 threads, as in the first version, costs the kernel ~10 us with stores in flight over NVLink.)
+    // 1024 threads, as in the first version, is slower with stores in flight over NVLink.)
     if (a.stagger == -1) __threadfence_system();            // A/B hook: the first version
     __syncthreads();
     if (tid == 0) {
@@ -641,12 +639,12 @@ static long long* win_debug_buffer = nullptr;   // b200mppi_debug_rollout_cta_ti
                                                 // lane-steps on the slow path, of which outside the window)
 void rollout_win_set_debug(long long* dev) { win_debug_buffer = dev; }
 constexpr int WIN_SYNC_MAX_PASSES = 0;    // shares of at most this many passes are run pass by pass (see the kernel);
-                                          // 0 = never: measured on a rank of an 8-GPU solve (2 passes per CTA) 0.207 ms
-                                          // against 0.186 ms with the shared counter -- a pass started in lockstep ends
+                                          // 0 = never: slower than the shared counter even at 2 passes per CTA (a rank
+                                          // of an 8-GPU solve) -- a pass started in lockstep ends
                                           // with its low-priority warps alone, the counter keeps the favoured warps busy
 constexpr int WIN_STAGGER_DEFAULT = 0;    // cycles between the warps of a scheduler after a window barrier (B200MPPI_WIN_STAGGER)
 static int win_grid_override = 0;         // B200MPPI_WIN_GRID (tuning / test hook): number of persistent CTAs
-constexpr int WIN_MAX_SMEM = 232448;      // 227 KB: per-block opt-in limit on sm_100
+constexpr int WIN_MAX_SMEM = 232448;      // 227 KB: per-block opt-in limit on sm_90 (H100)
 
 void rollout_win_geometry(int T, int* WW, int* WH, size_t* smem) {
   // 4 byte planes + tables must fit 227 KB; inner box extent a multiple of 16 B and <= 256; plane size a
@@ -657,6 +655,17 @@ void rollout_win_geometry(int T, int* WW, int* WH, size_t* smem) {
 }
 
 int rollout_win_threads() { return WIN_THREADS; }
+
+int device_sm_count() {
+  int dev = 0, sms = 132;                                   // H100 SXM
+  cudaGetDevice(&dev);
+  static int sm_count[64] = {};
+  if (dev >= 0 && dev < 64) {
+    if (!sm_count[dev]) cudaDeviceGetAttribute(&sm_count[dev], cudaDevAttrMultiProcessorCount, dev);
+    if (sm_count[dev] > 0) sms = sm_count[dev];
+  }
+  return sms;
+}
 
 cudaError_t launch_rollout_win(const RolloutWinArgs& a, const void* tm_lin, const void* tm_ang, const void* tm_obs,
                                const void* tm_unk, cudaStream_t st) {
@@ -681,13 +690,7 @@ cudaError_t launch_rollout_win(const RolloutWinArgs& a, const void* tm_lin, cons
   }
   if (a.WW != WIN_WW || (a.WH != 232 && a.WH != 224) || L.total > WIN_MAX_SMEM) return cudaErrorInvalidValue;
   // persistent: one CTA per SM (1024 threads and 222 KB of shared memory fill an SM), never more CTAs than chunks
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  static int sm_count[64] = {};
-  if (dev >= 0 && dev < 64) {
-    if (!sm_count[dev]) cudaDeviceGetAttribute(&sm_count[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (sm_count[dev] > 0) sms = sm_count[dev];
-  }
+  const int sms = device_sm_count();
   static bool env_read = false;
   if (!env_read) {
     if (const char* e = getenv("B200MPPI_WIN_GRID")) win_grid_override = atoi(e);
@@ -716,8 +719,8 @@ cudaError_t launch_rollout_win(const RolloutWinArgs& a, const void* tm_lin, cons
     sync_read = true;
   }
   // whole passes (32 chunks) per share once a share is at least 4 passes long (no end-of-segment stragglers); shorter
-  // shares stay chunk-granular: rounding 3.46 passes per CTA (a rank of a 4-GPU solve) to 3 or 4 costs more than it
-  // saves (measured 0.387 against 0.308 ms)
+  // shares stay chunk-granular: rounding a fractional pass count per CTA (a rank of a 4-GPU solve) to a whole one costs
+  // more than it saves
   b.unit = (total / (32LL * grid.x) >= 4) ? 32 : ((int)grid.x >= a.p.M ? 0 : 1);
   static int unit_override = -1;                            // B200MPPI_WIN_UNIT = 0 | 1 | 32 (A/B hook)
   static bool unit_read = false;

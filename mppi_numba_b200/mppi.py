@@ -1,5 +1,5 @@
 """``MPPI_Numba`` -- the planner object, kept API-compatible with the reference class of the same
-name (mppi_numba/mppi.py:39-608) but backed by libb200mppi.so (hand-written sm_100a CUDA behind the
+name (mppi_numba/mppi.py:39-608) but backed by libb200mppi.so (hand-written sm_90a CUDA behind the
 C-ABI of include/b200mppi.h) instead of Numba-JIT kernels.
 
 What a reference user keeps: ``MPPI_Numba(cfg)``, ``reset()``, ``setup(params, lin_tdm, ang_tdm)``,

@@ -1,4 +1,4 @@
-"""Traction-distribution maps for the B200 MPPI engine.
+"""Traction-distribution maps for the H100 MPPI engine.
 
 ``TDM_Numba`` keeps the public surface of the reference class of the same name
 (mppi_numba/terrain.py:69-628): the two setters, ``sample_grids``, the padded-limit attributes the

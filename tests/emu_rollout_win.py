@@ -211,7 +211,7 @@ extern "C" void emu_cell_between(const float* a, int n, float res, int* out_new,
   }
 }
 
-// ctas: number of persistent CTAs (0: launch_rollout_win's own rule for a 148-SM device).
+// ctas: number of persistent CTAs (0: launch_rollout_win's own rule for a 132-SM device, an H100 SXM).
 // dst_blocks: 1 = one map-major (M, N) destination; ws > 1 = the sharded layout, ws separate (ws*M, N/ws) "receive
 // buffers" written at the rows of "rank" 1 (fill_cost_dst with direct = true) plus the epoch flags of CostSignal --
 // checked here; costs_nm always comes back as the logical (N, M) array.
@@ -262,7 +262,7 @@ extern "C" int emu_rollout_win(const float* f, const int* g, const double* ratio
   const CUtensorMap t_unk{(const unsigned char*)unk, p.g.cols, p.g.rows, 1, p.g.mask_pitch, WW, WH};
   if (ctas <= 0) {                                            // launch_rollout_win (rollout_win.cu)
     const long long total = (long long)p.M * (npad / 32);
-    ctas = (int)std::min<long long>(std::max<long long>(total / 8, 1), 148);
+    ctas = (int)std::min<long long>(std::max<long long>(total / 8, 1), 132);
   }
   w.unit = ((long long)p.M * (npad / 32) / (32LL * ctas) >= 1) ? 32 : 1;     // launch_rollout_win
   if (unit_override > 0) w.unit = unit_override;

@@ -14,7 +14,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 @pytest.fixture(scope="module")
 def libmod():
     import __graft_entry__
-    __graft_entry__.build()
+    __graft_entry__.build_engine()
     from mppi_numba_b200 import _lib
     return _lib
 
@@ -29,10 +29,12 @@ def test_every_declared_symbol_is_exported(libmod):
     assert set(libmod.EXPORTS) == declared, set(libmod.EXPORTS) ^ declared
 
 
-def test_library_has_sm100a_code(libmod):
+def test_library_has_sm90a_code(libmod):
     import subprocess
-    out = subprocess.run(["/usr/local/cuda/bin/cuobjdump", "-lelf", libmod.LIB_PATH], capture_output=True, text=True)
-    assert "sm_100a" in out.stdout
+    from mppi_numba_b200 import build
+    cuobjdump = os.path.join(os.path.dirname(build.NVCC), "cuobjdump")
+    out = subprocess.run([cuobjdump, "-lelf", libmod.LIB_PATH], capture_output=True, text=True)
+    assert "sm_90a" in out.stdout
 
 
 def test_pod_layouts_match_header(libmod, tmp_path):

@@ -1,4 +1,4 @@
-"""GPU parity tests proper (run with ``-m gpu`` on the B200 box): the CUDA engine, called through the
+"""GPU parity tests proper (run with ``-m gpu`` on an H100): the CUDA engine, called through the
 C-ABI / the drop-in Python API, against (1) the committed golden vectors produced by the reference's
 own kernels and (2) the oracle on identical seeded inputs, plus size-independent properties.
 
@@ -26,7 +26,7 @@ from tests.scenarios import make_scenario, oracle_rollout_costs   # noqa: E402
 @pytest.fixture(scope="module")
 def eng():
     import __graft_entry__
-    __graft_entry__.build()
+    __graft_entry__.build_engine()
     import mppi_numba_b200 as E
     assert E.device_count() >= 1, "GPU tests need a CUDA device"
     return E

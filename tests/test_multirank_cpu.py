@@ -36,7 +36,7 @@ def _rank_main(rank, port, out_dir):
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=WS)
     import __graft_entry__
-    __graft_entry__.build()
+    __graft_entry__.build_engine()
     from mppi_numba_b200 import _lib
     costs, noise, u0 = _inputs()
     lam = np.float32(1.0)
@@ -96,7 +96,7 @@ def _peer_main(rank, port, out_dir):
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=WS)
     import __graft_entry__
-    __graft_entry__.build()
+    __graft_entry__.build_engine()
     import mppi_numba_b200 as E
     import mppi_numba_b200.mppi as M
     import mppi_numba_b200.terrain as Tm

@@ -16,7 +16,7 @@ def emu(request, tmp_path_factory):
     """The kernel as built, and with its compile-time A/B switches flipped (value lookup through a register table;
     the bytes >= q counted with shifts + one POPC instead of one POPC per word)."""
     import __graft_entry__
-    __graft_entry__.build()
+    __graft_entry__.build_engine()
     d = str(tmp_path_factory.mktemp("emu"))
     if request.param == "values-in-registers":
         return build(d, values_in_registers=True)

@@ -1,5 +1,5 @@
 #!/bin/bash
-# A/B on one box (box-to-box spread is a few %): library variants built beforehand into mppi_numba_b200/ab/lib_<name>.so
+# A/B on one machine (the spread between machines is larger than the differences of interest): library variants built beforehand into mppi_numba_b200/ab/lib_<name>.so
 # (e.g. B200MPPI_NVCC_FLAGS=-DWIN_ROUND_FP64=0 python mppi_numba_b200/build.py --force; cp mppi_numba_b200/libb200mppi.so
 # mppi_numba_b200/ab/lib_intround.so), each timed twice, interleaved: bench stage times + one rank of 8 / 4 alone.
 #   tools/ab_libs.sh <name> <name> ...

@@ -1,8 +1,10 @@
-// Which SM resource is shared between SMs?  One CTA (one SM busy) against 148 CTAs (all SMs busy) of the same
+// Which SM resource is shared between SMs?  One CTA (one SM busy) against one CTA per SM (all SMs busy) of the same
 // per-thread loop of ONE instruction type: if the per-SM rate drops when the neighbours work, the unit is shared.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/pair_probe tools/pair_probe.cu && /tmp/pair_probe
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/pair_probe tools/pair_probe.cu && /tmp/pair_probe
 #include <cstdio>
 #include <cuda_runtime.h>
+
+static int g_sms = 0;   // SMs of device 0 (main)
 
 template <int OP>
 __global__ void __launch_bounds__(1024) probe(float* out, int iters, float seed) {
@@ -35,7 +37,7 @@ __global__ void __launch_bounds__(1024) probe(float* out, int iters, float seed)
 }
 
 // L2-resident stream: every thread loads 16 B per iteration, coalesced (512 B per warp), from an 8 MB buffer, with
-// `pad` FFMA per load in between (the rollout kernel: ~74 instructions per 512 B)
+// `pad` FFMA per load in between (the rollout kernel's mix of streamed controls and arithmetic)
 template <int PAD>
 __global__ void __launch_bounds__(1024) stream(const double2* __restrict__ src, float* out, int iters, int words) {
   const int gt = blockIdx.x * 1024 + threadIdx.x;
@@ -86,9 +88,9 @@ void run_stream_smem(const char* name, int iters, int bcast) {
   const int words = 1 << 20;                                        // 16 MB of double2
   double2* src; cudaMalloc(&src, (size_t)words * 16); cudaMemset(src, 0, (size_t)words * 16);
   float* out; cudaMalloc(&out, 4);
-  long long* dur; cudaMalloc(&dur, 148 * 8);
+  long long* dur; cudaMalloc(&dur, g_sms * 8);
   cudaFuncSetAttribute(stream_smem<PAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, 222 * 1024);
-  const int grids[2] = {1, 148};
+  const int grids[2] = {1, g_sms};
   printf("%-34s", name);
   for (int k = 0; k < 2; ++k) {
     stream_smem<PAD><<<grids[k], 1024, 222 * 1024>>>(src, out, iters, words, bcast, dur);
@@ -111,7 +113,7 @@ void run_stream(const char* name, int iters) {
   float* out; cudaMalloc(&out, 4);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   float ms[3];
-  const int grids[3] = {1, 74, 148};
+  const int grids[3] = {1, g_sms / 2, g_sms};
   for (int k = 0; k < 3; ++k) {
     stream<PAD><<<grids[k], 1024>>>(src, out, iters, words);
     cudaEventRecord(e0);
@@ -120,8 +122,8 @@ void run_stream(const char* name, int iters) {
     cudaEventElapsedTime(&ms[k], e0, e1);
   }
   const double gb = 1024.0 * 16 * iters / 1e6;                      // MB per CTA
-  printf("%-28s 1 CTA %.3f ms (%.0f GB/s/SM) | 74 CTAs %.3f ms (x%.2f) | 148 CTAs %.3f ms (x%.2f, %.0f GB/s/SM, %.2f TB/s)\n", name, ms[0],
-         gb / ms[0], ms[1], ms[1] / ms[0], ms[2], ms[2] / ms[0], gb / ms[2], gb * 148 / ms[2] / 1e3);
+  printf("%-28s 1 CTA %.3f ms (%.0f GB/s/SM) | %d CTAs %.3f ms (x%.2f) | %d CTAs %.3f ms (x%.2f, %.0f GB/s/SM, %.2f TB/s)\n", name, ms[0],
+         gb / ms[0], grids[1], ms[1], ms[1] / ms[0], grids[2], ms[2], ms[2] / ms[0], gb / ms[2], gb * g_sms / ms[2] / 1e3);
   cudaFree(src); cudaFree(out);
 }
 
@@ -130,7 +132,7 @@ void run(const char* name, int iters) {
   float* out; cudaMalloc(&out, 4);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   float ms[3];
-  const int grids[3] = {1, 74, 148};
+  const int grids[3] = {1, g_sms / 2, g_sms};
   for (int k = 0; k < 3; ++k) {
     probe<OP><<<grids[k], 1024>>>(out, iters, 1.0f);            // warm-up
     cudaEventRecord(e0);
@@ -138,11 +140,13 @@ void run(const char* name, int iters) {
     cudaEventRecord(e1); cudaEventSynchronize(e1);
     cudaEventElapsedTime(&ms[k], e0, e1);
   }
-  printf("%-28s 1 CTA %.3f ms | 74 CTAs %.3f ms (x%.2f) | 148 CTAs %.3f ms (x%.2f)\n", name, ms[0], ms[1], ms[1] / ms[0], ms[2], ms[2] / ms[0]);
+  printf("%-28s 1 CTA %.3f ms | %d CTAs %.3f ms (x%.2f) | %d CTAs %.3f ms (x%.2f)\n", name, ms[0], grids[1], ms[1], ms[1] / ms[0], grids[2],
+         ms[2], ms[2] / ms[0]);
   cudaFree(out);
 }
 
 int main() {
+  cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0);
   const int it = 20000;
   run<3>("FFMA", it);
   run<4>("IADD/LOP3", it);

@@ -25,17 +25,19 @@ def solve():
     else:
         check(lib.b200mppi_planner_solve_local(pl._handle, 1)); check(lib.b200mppi_planner_synchronize(pl._handle))
 for _ in range(6): solve()
-raw = np.zeros((256 + 99, 6), np.int64)        # 148 x 6 per-CTA slots, then (from word 1536) 148 x 4 extra counters
+import torch
+SMS = torch.cuda.get_device_properties(0).multi_processor_count
+raw = np.zeros((256 + 99, 6), np.int64)        # SMS x 6 per-CTA slots, then (from word 1536) SMS x 4 extra counters
 check(lib.b200mppi_debug_rollout_cta_times(1, None, 0))
 solve()
 check(lib.b200mppi_debug_rollout_cta_times(0, raw.ctypes.data_as(C.c_void_p), 256 + 99))
-out = raw[:148].copy()
-extra = raw.reshape(-1)[1536:1536 + 148 * 4].reshape(148, 4)
+out = raw[:SMS].copy()
+extra = raw.reshape(-1)[1536:1536 + SMS * 4].reshape(SMS, 4)
 if not out[:, 1].any():
     sys.exit("no data: build the library with -DB200MPPI_WIN_DEBUG_HOOK (see the docstring)")
 ran = out[:, 1] > 0
 extra = extra[ran]
-out = out[ran]                                # the CTAs that ran (B200MPPI_WIN_GRID < 148)
+out = out[ran]                                # the CTAs that ran (B200MPPI_WIN_GRID < SMS)
 smid = out[:, 2] >> 40
 out[:, 2] &= (1 << 40) - 1
 wsteps = out[:, 5] >> 40

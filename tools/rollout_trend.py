@@ -1,5 +1,5 @@
-import io, contextlib, numpy as np, sys
-sys.path.insert(0, "/root/repo")
+import io, contextlib, numpy as np, os, sys
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import mppi_numba_b200 as E
 from bench import build_scenario
 sc = build_scenario("c5")
