@@ -299,6 +299,31 @@ int b200mppi_planner_launch_count(b200mppi_planner* pl, int64_t* out);
  * out[5] = { mode used by the last solve (0 whole maps, 1 static, 2 dynamic), row_lo, row_hi, col_lo, col_hi }. */
 int b200mppi_planner_sample_box(b200mppi_planner* pl, int32_t out[5]);
 
+/* ------------------------------------------------------------------ batched one-map solves
+ * K independent planners of the same shape solved with ONE launch per stage for the whole batch (noise, map sampling,
+ * rollout, update; plus one descriptor upload and one D2H of all K control sequences), instead of K solve() calls of
+ * four small launches, two copies and a host synchronisation each.  The planners are BORROWED (they must outlive the
+ * batch) and keep every per-planner call (set_params, set_u, shift_u, copy_out, get_state_rollout, ...).
+ *   create: planners on one device, world_size 1, one mode among MODE_DET_DYN / MODE_SPEED_MAP / MODE_BAREBONE (the
+ *           stochastic MODE_TDM is not batched: its windowed rollout kernel already fills the GPU), equal num_steps and
+ *           num_control_rollouts, no planner listed twice.  Anything else: B200MPPI_EINVAL naming the planner's index.
+ *   solve : == b200mppi_planner_solve on planners[0], planners[1], ... in that order, bit for bit: u, u_prev, noise,
+ *           costs, weights, the planners' and their TDMs' RNG states and the sampled maps all end up identical.  Needs
+ *           equal params.num_opt and no TDM shared between two planners of the batch (B200MPPI_EINVAL; a planner whose
+ *           lin == ang is fine); every planner must be ready to solve (the first that is not is reported with its
+ *           index).  Rejections are decided before any work is issued.  The batch's work starts after all work already
+ *           issued on the members' streams and has finished when the call returns.  Pairs of TDMs whose maps cannot
+ *           be sampled with the batch's one sampler launch (other map geometry, ill-formed PMF, ...) are sampled by
+ *           their own launches -- same results, more launches.
+ *           u_out: float32 (count, T, 2), may be NULL.
+ *   launch_count: kernel launches issued by this batch (per-planner launch counts and stage timings are not touched). */
+typedef struct b200mppi_batch b200mppi_batch;
+int b200mppi_batch_create(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out);
+int b200mppi_batch_destroy(b200mppi_batch* b);
+int b200mppi_batch_set_stream(b200mppi_batch* b, void* cuda_stream);
+int b200mppi_batch_solve(b200mppi_batch* b, float* u_out);
+int b200mppi_batch_launch_count(b200mppi_batch* b, int64_t* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,6 +9,7 @@ planner or TDM needs a CUDA device.  There is no CPU fallback.
 from .config import Config
 from .terrain import TDM_Numba, TractionGrid, Terrain
 from .mppi import MPPI_Numba
+from .batch import MPPI_Batch
 from ._lib import B200MPPIError, device_count
 
-__all__ = ["Config", "TDM_Numba", "TractionGrid", "Terrain", "MPPI_Numba", "B200MPPIError", "device_count"]
+__all__ = ["Config", "TDM_Numba", "TractionGrid", "Terrain", "MPPI_Numba", "MPPI_Batch", "B200MPPIError", "device_count"]

@@ -104,6 +104,11 @@ def _load():
         "b200mppi_planner_launch_count": (C.c_int, [P, C.POINTER(I64)]),
         "b200mppi_planner_sample_box": (C.c_int, [P, C.POINTER(I32 * 5)]),
         "b200mppi_debug_rollout_cta_times": (C.c_int, [I32, P, I32]),
+        "b200mppi_batch_create": (C.c_int, [C.POINTER(P), I32, C.POINTER(P)]),
+        "b200mppi_batch_destroy": (C.c_int, [P]),
+        "b200mppi_batch_set_stream": (C.c_int, [P, P]),
+        "b200mppi_batch_solve": (C.c_int, [P, P]),
+        "b200mppi_batch_launch_count": (C.c_int, [P, C.POINTER(I64)]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)          # AttributeError here == ABI drift, fail loudly

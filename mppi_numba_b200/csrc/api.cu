@@ -235,6 +235,23 @@ static int tdm_sample_on(b200mppi_tdm* t, double alpha_dyn, cudaStream_t st, con
   return B200MPPI_OK;
 }
 
+// Two distinct TDMs whose generators are in identical states over identical tiles: one stream of draws samples both.
+static bool tdm_same_stream(const b200mppi_tdm* l, const b200mppi_tdm* g) {
+  return l != g && l->sig == g->sig && l->rows == g->rows && l->cols == g->cols && l->num_maps == g->num_maps &&
+         l->pitch == g->pitch && l->cfg.tdm_thread_x == g->cfg.tdm_thread_x &&
+         l->cfg.tdm_thread_y == g->cfg.tdm_thread_y && l->cfg.max_map_rows == g->cfg.max_map_rows;
+}
+
+// Bookkeeping of a fused whole-map pair sampling (launched by the caller): advanced states, fresh signatures.
+static void tdm_pair_sampled_whole(b200mppi_tdm* l, b200mppi_tdm* g, double alpha_dyn) {
+  std::swap(l->states, l->states_alt);
+  std::swap(g->states, g->states_alt);
+  l->grid_partial = g->grid_partial = false;
+  l->partial_alpha = g->partial_alpha = alpha_dyn;
+  tdm_advance_sig(l);
+  tdm_advance_sig(g);
+}
+
 // Both TDMs of a planner.  When their generator states are identical (same seed, same history: the
 // reference seeds both with cfg.seed) ONE pass draws each uniform once and samples both maps.
 // The state advance of a boxed pair sampling does not depend on the box: solve() launches it while the host still waits
@@ -243,10 +260,7 @@ static int tdm_sample_on(b200mppi_tdm* t, double alpha_dyn, cudaStream_t st, con
 static void tdm_pair_advance_early(b200mppi_tdm* l, b200mppi_tdm* g, double alpha_dyn, cudaStream_t st, int64_t* launches) {
   if (!l->pmf_set || !g->pmf_set || l == g) return;
   if (tdm_prepare_thresholds(l, alpha_dyn, st) || tdm_prepare_thresholds(g, alpha_dyn, st)) return;
-  const bool same_stream = l->sig == g->sig && l->rows == g->rows && l->cols == g->cols &&
-                           l->num_maps == g->num_maps && l->pitch == g->pitch &&
-                           l->cfg.tdm_thread_x == g->cfg.tdm_thread_x && l->cfg.tdm_thread_y == g->cfg.tdm_thread_y &&
-                           l->cfg.max_map_rows == g->cfg.max_map_rows;
+  const bool same_stream = tdm_same_stream(l, g);
   if (!same_stream || !l->thr_ok || !g->thr_ok || tdm_prepare_jump(l, st)) return;
   SampleGridsV2Args v2{};
   fill_v2(l, v2, 0);
@@ -265,10 +279,7 @@ static int tdm_sample_pair_on(b200mppi_tdm* l, b200mppi_tdm* g, double alpha_dyn
   int rc = tdm_prepare_thresholds(l, alpha_dyn, st);
   if (rc) return rc;
   if ((rc = tdm_prepare_thresholds(g, alpha_dyn, st))) return rc;
-  const bool same_stream = l != g && l->sig == g->sig && l->rows == g->rows && l->cols == g->cols &&
-                           l->num_maps == g->num_maps && l->pitch == g->pitch &&
-                           l->cfg.tdm_thread_x == g->cfg.tdm_thread_x && l->cfg.tdm_thread_y == g->cfg.tdm_thread_y &&
-                           l->cfg.max_map_rows == g->cfg.max_map_rows;
+  const bool same_stream = tdm_same_stream(l, g);
   if ((rc = tdm_prepare_jump(l, st))) return rc;
   SampleGridsV2Args v2{};
   fill_v2(l, v2, 0);
@@ -359,6 +370,9 @@ static int tdm_init(b200mppi_tdm* t, const b200mppi_config* cfg) {
   CU(cudaMalloc(&t->states, h.size() * sizeof(uint64_t)));
   CU(cudaMalloc(&t->states_alt, h.size() * sizeof(uint64_t)));
   CU(cudaMemcpyAsync(t->states, h.data(), h.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, t->stream));
+  // both halves of the double buffer start alike: a whole-map sampling writes only the generators whose tile holds map
+  // cells, the others (tiles below / right of the map) keep their states across the swap, as in the reference
+  CU(cudaMemcpyAsync(t->states_alt, h.data(), h.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, t->stream));
   CU(cudaStreamSynchronize(t->stream));
   return B200MPPI_OK;
 }
@@ -663,6 +677,7 @@ extern "C" int b200mppi_tdm_set_rng_states(b200mppi_tdm* t, const uint64_t* in, 
   CU(cudaSetDevice(t->cfg.device));
   { const int rc = tdm_complete_grid(t, t->stream); if (rc) return rc; }   // completion needs the states it replaces
   CU(cudaMemcpyAsync(t->states, in, bytes, cudaMemcpyHostToDevice, t->stream));
+  CU(cudaMemcpyAsync(t->states_alt, in, bytes, cudaMemcpyHostToDevice, t->stream));   // see tdm_init
   CU(cudaStreamSynchronize(t->stream));
   // content-derived signature: two TDMs given identical states compare equal again
   uint64_t h = 0x1234567ULL;
@@ -1008,8 +1023,8 @@ static void fill_cost_dst(b200mppi_planner* p, CostDst& d, bool direct) {
     d.base[r] = direct ? (float*)p->peer_x[r] : p->costs_nm + (size_t)r * p->M * p->n_red;
 }
 
-static int stage_rollout(b200mppi_planner* p) {
-  RolloutArgs a{};
+static void fill_rollout_args(b200mppi_planner* p, RolloutArgs& a) {
+  a = RolloutArgs{};
   fill_rollout_params(p, a.p);
   a.mode = p->cfg.mode;
   if (p->cfg.mode != B200MPPI_MODE_BAREBONE) {
@@ -1019,6 +1034,11 @@ static int stage_rollout(b200mppi_planner* p) {
   a.obstacles = p->obstacles; a.num_obstacles = p->num_obstacles;
   a.noise = p->noise; a.u_cur = p->u_cur; a.costs = p->costs;
   fill_cost_dst(p, a.dst, false);
+}
+
+static int stage_rollout(b200mppi_planner* p) {
+  RolloutArgs a;
+  fill_rollout_args(p, a);
   p->pushed_direct = false;
   bool done = false;
   if (planner_uses_window(p)) {
@@ -1705,5 +1725,265 @@ extern "C" int b200mppi_planner_sample_box(b200mppi_planner* p, int32_t out[5]) 
 extern "C" int b200mppi_planner_launch_count(b200mppi_planner* p, int64_t* out) {
   if (!p || !out) return fail(B200MPPI_EINVAL, "null argument");
   *out = p->launches + (p->lin ? 0 : 0);
+  return B200MPPI_OK;
+}
+
+// --------------------------------------------------------------------------------------------- batch
+// K independent one-map planners of equal N and T solved with one launch per stage (noise, map sampling, rollout,
+// update) for the whole batch.  The per-planner kernel arguments travel as descriptor arrays in device memory (a
+// grid coordinate selects the planner): rebuilt every solve -- params, maps and TDM buffers may change in between --
+// and uploaded with ONE copy from pinned staging.  Every kernel of a planner computes exactly what it computes in that
+// planner's own solve(), in the same order, so the results are those of K solve() calls, bit for bit.
+struct b200mppi_batch {
+  std::vector<b200mppi_planner*> pl;
+  int device = 0, mode = 0, T = 0, N = 0;
+  cudaStream_t stream = nullptr;
+  bool own_stream = false;
+  cudaEvent_t ev = nullptr;            // orders the batch after the work already issued on a member's stream
+  // descriptor arrays, one allocation: [NoiseDesc K | SampleGridsV2Args K | RolloutArgs K | UpdateBatchDesc K]
+  size_t off_sample = 0, off_roll = 0, off_upd = 0, desc_bytes = 0;
+  unsigned char* h_desc = nullptr;     // pinned staging
+  unsigned char* d_desc = nullptr;
+  float* u_d = nullptr;                // (K, T, 2): every planner's new u, written by its update's last CTA
+  float* h_u = nullptr;                // pinned (K, T, 2)
+  int64_t launches = 0;
+};
+
+static size_t align256(size_t v) { return (v + 255) / 256 * 256; }
+
+extern "C" int b200mppi_batch_destroy(b200mppi_batch* b) {
+  if (!b) return B200MPPI_OK;
+  cudaSetDevice(b->device);
+  if (b->stream) cudaStreamSynchronize(b->stream);
+  cudaFree(b->d_desc); cudaFree(b->u_d);
+  if (b->h_desc) cudaFreeHost(b->h_desc);
+  if (b->h_u) cudaFreeHost(b->h_u);
+  if (b->ev) cudaEventDestroy(b->ev);
+  if (b->own_stream && b->stream) cudaStreamDestroy(b->stream);
+  delete b;
+  return B200MPPI_OK;
+}
+
+static int batch_init(b200mppi_batch* b) {
+  const size_t K = b->pl.size();
+  b->off_sample = align256(K * sizeof(NoiseDesc));
+  b->off_roll = b->off_sample + align256(K * sizeof(SampleGridsV2Args));
+  b->off_upd = b->off_roll + align256(K * sizeof(RolloutArgs));
+  b->desc_bytes = b->off_upd + align256(K * sizeof(UpdateBatchDesc));
+  CU(cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
+  b->own_stream = true;
+  CU(cudaEventCreateWithFlags(&b->ev, cudaEventDisableTiming));
+  CU(cudaMallocHost(&b->h_desc, b->desc_bytes));
+  CU(cudaMalloc(&b->d_desc, b->desc_bytes));
+  const size_t ubytes = K * (size_t)b->T * 2 * sizeof(float);
+  CU(cudaMallocHost(&b->h_u, ubytes));
+  CU(cudaMalloc(&b->u_d, ubytes));
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_batch_create(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out) {
+  if (!planners || !out) return fail(B200MPPI_EINVAL, "batch_create: null argument");
+  if (count < 1) return fail(B200MPPI_EINVAL, "batch_create: count < 1");
+  if (count > 65535) return fail(B200MPPI_EINVAL, "batch_create: more than 65535 planners");
+  for (int i = 0; i < count; ++i) {
+    const b200mppi_planner* p = planners[i];
+    const std::string who = "batch_create: planner " + std::to_string(i);
+    if (!p) return fail(B200MPPI_EINVAL, who + " is null");
+    for (int j = 0; j < i; ++j)
+      if (planners[j] == p) return fail(B200MPPI_EINVAL, who + " is planner " + std::to_string(j) + " again");
+    if (p->cfg.world_size != 1)
+      return fail(B200MPPI_EINVAL, who + " has world_size " + std::to_string(p->cfg.world_size) +
+                                       " (a batch holds single-rank planners)");
+    if (p->cfg.mode == B200MPPI_MODE_TDM)
+      return fail(B200MPPI_EINVAL, who + " is MODE_TDM: the stochastic mode is not batched (batches hold "
+                                         "MODE_DET_DYN, MODE_SPEED_MAP or MODE_BAREBONE planners)");
+    const b200mppi_planner* q = planners[0];
+    if (p->cfg.device != q->cfg.device)
+      return fail(B200MPPI_EINVAL, who + " is on device " + std::to_string(p->cfg.device) + ", planner 0 on device " +
+                                       std::to_string(q->cfg.device));
+    if (p->cfg.mode != q->cfg.mode)
+      return fail(B200MPPI_EINVAL, who + " has mode " + std::to_string(p->cfg.mode) + ", planner 0 mode " +
+                                       std::to_string(q->cfg.mode) + " (modes cannot be mixed)");
+    if (p->T != q->T) return fail(B200MPPI_EINVAL, who + " has num_steps " + std::to_string(p->T) + ", planner 0 " +
+                                                      std::to_string(q->T) + " (T must be equal)");
+    if (p->n_local != q->n_local)
+      return fail(B200MPPI_EINVAL, who + " has num_control_rollouts " + std::to_string(p->n_local) + ", planner 0 " +
+                                       std::to_string(q->n_local) + " (N must be equal)");
+  }
+  CU(cudaSetDevice(planners[0]->cfg.device));
+  b200mppi_batch* b = new b200mppi_batch();
+  b->pl.assign(planners, planners + count);
+  b->device = planners[0]->cfg.device; b->mode = planners[0]->cfg.mode;
+  b->T = planners[0]->T; b->N = planners[0]->n_local;
+  const int rc = batch_init(b);
+  if (rc) {
+    const std::string keep = g_err;
+    b200mppi_batch_destroy(b);
+    g_err = keep;
+    return rc;
+  }
+  *out = b;
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_batch_set_stream(b200mppi_batch* b, void* s) {
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  if (b->own_stream && b->stream) { cudaStreamSynchronize(b->stream); cudaStreamDestroy(b->stream); }
+  b->stream = (cudaStream_t)s;
+  b->own_stream = false;
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_batch_launch_count(b200mppi_batch* b, int64_t* out) {
+  if (!b || !out) return fail(B200MPPI_EINVAL, "null argument");
+  *out = b->launches;
+  return B200MPPI_OK;
+}
+
+// Everything a batch solve checks before it issues any work.
+static int batch_validate(b200mppi_batch* b) {
+  const int K = (int)b->pl.size();
+  for (int i = 0; i < K; ++i) {
+    const int rc = planner_check_ready(b->pl[i]);
+    if (rc) return fail(rc, "batch_solve: planner " + std::to_string(i) + ": " + g_err);
+  }
+  for (int i = 0; i < K; ++i) {
+    const b200mppi_planner* p = b->pl[i];
+    if (p->prm.num_opt != b->pl[0]->prm.num_opt)
+      return fail(B200MPPI_EINVAL, "batch_solve: planner " + std::to_string(i) + " has num_opt " +
+                                       std::to_string(p->prm.num_opt) + ", planner 0 num_opt " +
+                                       std::to_string(b->pl[0]->prm.num_opt) + " (must be equal)");
+  }
+  if (b->mode == B200MPPI_MODE_BAREBONE) return B200MPPI_OK;
+  // sequential solves would sample a TDM shared by two planners twice, one after the other: those planners are not
+  // independent, so the batch refuses them (one planner's lin == ang is fine: its own solve samples it twice too)
+  for (int i = 0; i < K; ++i)
+    for (int j = 0; j < i; ++j) {
+      const b200mppi_planner* p = b->pl[i]; const b200mppi_planner* q = b->pl[j];
+      if (p->lin == q->lin || p->lin == q->ang || p->ang == q->lin || p->ang == q->ang)
+        return fail(B200MPPI_EINVAL, "batch_solve: planners " + std::to_string(j) + " and " + std::to_string(i) +
+                                         " share a TDM (batched planners must be independent)");
+    }
+  return B200MPPI_OK;
+}
+
+// The maps of every planner, as its solve() samples them: the pairs its solve() would sample with the fused whole-map
+// launch and whose launch geometry equals the first such pair's go into ONE launch; every other pair takes its own
+// path (tdm_sample_pair_on), in planner order.  One-map modes never sample a reach box.
+// Planning (host tables, the fused pairs' descriptors) comes before the solve's one upload, the launches after the noise.
+constexpr double BATCH_ALPHA = 1.0;   // det / speed-map solves sample with the default alpha_dyn (stage_sample_tdms)
+
+static int batch_plan_sample(b200mppi_batch* b, SampleGridsV2Args* h_sg, std::vector<char>& fused, int* nfused) {
+  const double alpha = BATCH_ALPHA;
+  cudaStream_t st = b->stream;
+  const int K = (int)b->pl.size();
+  fused.assign(K, 0);
+  int nf = 0, rc;
+  for (int i = 0; i < K; ++i) {
+    b200mppi_planner* p = b->pl[i];
+    b200mppi_tdm* l = p->lin; b200mppi_tdm* g = p->ang;
+    l->advance_done = false;
+    if ((rc = tdm_prepare_thresholds(l, alpha, st)) || (rc = tdm_prepare_thresholds(g, alpha, st))) return rc;
+    if ((rc = tdm_prepare_jump(l, st))) return rc;
+    SampleGridsV2Args v2{};
+    fill_v2(l, v2, 0);
+    fill_v2(g, v2, 1);
+    if (!(tdm_same_stream(l, g) && l->thr_ok && g->thr_ok && sample_grids_v2_fits(v2, 2))) continue;
+    if (nf > 0 && !sample_grids_v2_same_launch(h_sg[0], v2)) continue;
+    h_sg[nf++] = v2;
+    fused[i] = 1;
+  }
+  *nfused = nf;
+  return B200MPPI_OK;
+}
+
+static int batch_run_sample(b200mppi_batch* b, const SampleGridsV2Args* h_sg, const SampleGridsV2Args* d_sg,
+                            const std::vector<char>& fused, int nf) {
+  const double alpha = BATCH_ALPHA;
+  cudaStream_t st = b->stream;
+  const int K = (int)b->pl.size();
+  int rc;
+  if (nf > 0) {
+    launch_sample_grids_v2_batch(h_sg[0], d_sg, nf, st);
+    b->launches++;
+    CHECK_LAUNCH();
+  }
+  for (int i = 0; i < K; ++i) {
+    b200mppi_planner* p = b->pl[i];
+    if (fused[i]) tdm_pair_sampled_whole(p->lin, p->ang, alpha);
+    else if ((rc = tdm_sample_pair_on(p->lin, p->ang, alpha, st, &b->launches, nullptr))) return rc;
+    p->last_box[0] = 0; p->last_box[1] = 0; p->last_box[2] = p->lin->rows; p->last_box[3] = 0; p->last_box[4] = p->lin->cols;
+  }
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  int rc = batch_validate(b);
+  if (rc) return rc;
+  CU(cudaSetDevice(b->device));
+  const int K = (int)b->pl.size(), T = b->T;
+  cudaStream_t st = b->stream;
+  // start after everything already issued on the members' streams (idle streams need no event)
+  for (b200mppi_planner* p : b->pl) {
+    if (p->stream == st) continue;
+    const cudaError_t q = cudaStreamQuery(p->stream);
+    if (q == cudaSuccess) continue;
+    if (q != cudaErrorNotReady) CU(q);
+    CU(cudaEventRecord(b->ev, p->stream));
+    CU(cudaStreamWaitEvent(st, b->ev, 0));
+  }
+  // descriptors, built on the host for this solve and uploaded with ONE copy before the first launch (the sampler's
+  // are decided here too: its host-side preparation may synchronise the stream)
+  NoiseDesc* hn = reinterpret_cast<NoiseDesc*>(b->h_desc);
+  SampleGridsV2Args* hs = reinterpret_cast<SampleGridsV2Args*>(b->h_desc + b->off_sample);
+  RolloutArgs* hr = reinterpret_cast<RolloutArgs*>(b->h_desc + b->off_roll);
+  UpdateBatchDesc* hu = reinterpret_cast<UpdateBatchDesc*>(b->h_desc + b->off_upd);
+  for (int i = 0; i < K; ++i) {
+    b200mppi_planner* p = b->pl[i];
+    hn[i] = NoiseDesc{p->states, p->noise, p->prm.u_std[0], p->prm.u_std[1]};
+    fill_rollout_args(p, hr[i]);
+    fill_update_args(p, hu[i].a, nullptr);
+    hu[i].tl = UpdateTail{};
+    hu[i].tl.counter = p->upd_counter_d;
+    hu[i].tl.mode = UPD_TAIL_APPLY;
+    hu[i].tl.u_prev = p->u_prev;                       // self.u_prev_d = self.u_cur_d (alias, mppi.py:292,362)
+    hu[i].tl.u_out = b->u_d + (size_t)i * T * 2;
+  }
+  const NoiseDesc* dn = reinterpret_cast<const NoiseDesc*>(b->d_desc);
+  const SampleGridsV2Args* ds = reinterpret_cast<const SampleGridsV2Args*>(b->d_desc + b->off_sample);
+  const RolloutArgs* dr = reinterpret_cast<const RolloutArgs*>(b->d_desc + b->off_roll);
+  const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(b->d_desc + b->off_upd);
+  const bool maps = b->mode != B200MPPI_MODE_BAREBONE;
+  std::vector<char> fused;
+  int nf = 0;
+  if (maps && (rc = batch_plan_sample(b, hs, fused, &nf))) return rc;
+  CU(cudaMemcpyAsync(b->d_desc, b->h_desc, b->desc_bytes, cudaMemcpyHostToDevice, st));
+  const int num_opt = b->pl[0]->prm.num_opt;
+  if (num_opt <= 0) {                                  // the reference samples before its (empty) loop; u unchanged
+    if (maps && (rc = batch_run_sample(b, hs, ds, fused, nf))) return rc;
+    for (int i = 0; i < K; ++i)
+      CU(cudaMemcpyAsync(b->u_d + (size_t)i * T * 2, b->pl[i]->u_cur, (size_t)T * 2 * sizeof(float),
+                         cudaMemcpyDeviceToDevice, st));
+  }
+  // solve(): num_opt x (noise, [first iteration: maps], rollout, update)
+  for (int k = 0; k < num_opt; ++k) {
+    launch_sample_noise_batch(dn, K, b->N, T, st);
+    b->launches++;
+    CHECK_LAUNCH();
+    for (b200mppi_planner* p : b->pl) p->prepared = false;
+    if (k == 0 && maps && (rc = batch_run_sample(b, hs, ds, fused, nf))) return rc;
+    launch_rollout_batch(dr, K, b->mode, b->N, T, st);
+    b->launches++;
+    CHECK_LAUNCH();
+    for (b200mppi_planner* p : b->pl) p->pushed_direct = false;
+    launch_update_partial_batch(du, K, b->pl[0]->num_ctas, st);
+    b->launches++;
+    CHECK_LAUNCH();
+  }
+  CU(cudaMemcpyAsync(b->h_u, b->u_d, (size_t)K * T * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  // the host waits for the whole batch: work issued afterwards on any member's stream sees its results
+  CU(cudaStreamSynchronize(st));
+  if (u_out) std::memcpy(u_out, b->h_u, (size_t)K * T * 2 * sizeof(float));
   return B200MPPI_OK;
 }

@@ -55,6 +55,11 @@ constexpr int SAMPLE_TABLE_WORDS = 256 + 256 / 8;
 bool build_sample_thresholds(double alpha, int q_cap, uint64_t* table /*[SAMPLE_TABLE_WORDS]*/);
 bool sample_grids_v2_fits(const SampleGridsV2Args& a, int nt);
 void launch_sample_grids_v2(const SampleGridsV2Args& a, int nt, cudaStream_t st);
+// batched one-map solves: equal launch configuration (grid, threads, shared memory, kernel variant)
+bool sample_grids_v2_same_launch(const SampleGridsV2Args& a, const SampleGridsV2Args& b);
+// ONE fused (nt = 2) launch for `count` pairs: descs = device array of their args, geom = any of them (host)
+void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs, int count,
+                                  cudaStream_t st);
 // tile classes of a generator: (full | last) tile height x (full | last) tile width -> draws per whole-map walk
 void sample_tile_draws(int rows, int cols, int tx, int ty, int64_t ks[4]);
 // states_out[g] = states[g] advanced by the draws of a whole-map walk of generator g's tile (GF(2) jump with
@@ -73,6 +78,15 @@ void launch_collapse_pad(const int8_t* raw, int8_t* out, int8_t* risk, int* bad_
 // `reach` (may be null): a device float the kernel zeroes for the prepare kernel's max-reduction
 void launch_sample_noise(uint64_t* states, float* noise, int n_local, int T, float std_v,
                          float std_w, float* reach, cudaStream_t st);
+// batched one-map solves: one launch samples the noise of `count` planners of equal N and T (planner = blockIdx.y)
+// [emu:begin noise_desc]
+struct NoiseDesc {
+  uint64_t* states;         // (N*T, 2)
+  float* noise;             // (N, T, 2)
+  float std_v, std_w;
+};
+// [emu:end noise_desc]
+void launch_sample_noise_batch(const NoiseDesc* descs, int count, int n_local, int T, cudaStream_t st);
 
 // Where the per-(map, control sequence) cost of a stochastic rollout goes.  Layout is MAP-MAJOR: row m holds the
 // costs of the control sequences on sampled map m, so the 32 lanes of a warp (consecutive n, same map) store one
@@ -119,6 +133,8 @@ struct RolloutArgs {
 };
 // [emu:end rollout_args]
 void launch_rollout(const RolloutArgs& a, cudaStream_t st);
+// batched one-map solves (mode 1, 2, 3): descs = device array of `count` RolloutArgs of equal N and T (blockIdx.y)
+void launch_rollout_batch(const RolloutArgs* descs, int count, int mode, int N, int T, cudaStream_t st);
 // windowed (TMA-staged) stochastic rollout kernel -- rollout_win.cu
 // [emu:begin win_args]
 struct RolloutWinArgs {
@@ -189,10 +205,20 @@ struct UpdateTail {
   uint32_t* peer_flags[P2P_MAX_PEERS];  // peer d's partial flags [ws]
   int ws, rank;
   uint32_t epoch;
+  float* u_prev;                        // UPD_TAIL_APPLY, when set: the new u is also stored here (T,2) ...
+  float* u_out;                         // ... and here (batched solves: u_prev alias, contiguous (K,T,2) result)
 };
 // [emu:end update_tail]
+// [emu:begin update_desc]
+struct UpdateBatchDesc {               // one planner of a batched update launch (blockIdx.y)
+  UpdateArgs a;
+  UpdateTail tl;
+};
+// [emu:end update_desc]
 int update_num_ctas(int N);
 void launch_update_partial(const UpdateArgs& a, const UpdateTail& tl, cudaStream_t st);
+// batched one-map solves: `count` planners of equal N (hence equal num_ctas), UPD_TAIL_APPLY each
+void launch_update_partial_batch(const UpdateBatchDesc* descs, int count, int num_ctas, cudaStream_t st);
 // combine `count` partials (each 2T+2 floats; this rank's own partial is entry `self`) into u and weights
 void launch_update_finish(const UpdateArgs& a, const float* gathered, int count, const FlagWait& fw, cudaStream_t st);
 

@@ -21,9 +21,8 @@ namespace b200 {
 
 // one thread per generator g = n*T + t (mppi.py:1367); generator and noise accesses are both
 // contiguous in g, so loads/stores are fully coalesced 16 B / 8 B per lane.
-__global__ void __launch_bounds__(256) sample_noise_kernel(uint64_t* __restrict__ states,
-                                                           float2* __restrict__ noise, int64_t count,
-                                                           float std_v, float std_w, float* __restrict__ reach) {
+__device__ __forceinline__ void sample_noise_body(uint64_t* __restrict__ states, float2* __restrict__ noise,
+                                                  int64_t count, float std_v, float std_w, float* __restrict__ reach) {
   const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= count) return;
   if (g == 0 && reach) *reach = 0.0f;          // the prepare kernel that follows max-reduces into it
@@ -37,7 +36,20 @@ __global__ void __launch_bounds__(256) sample_noise_kernel(uint64_t* __restrict_
   *sp = make_ulonglong2(s.s0, s.s1);
 }
 
+__global__ void __launch_bounds__(256) sample_noise_kernel(uint64_t* __restrict__ states,
+                                                           float2* __restrict__ noise, int64_t count,
+                                                           float std_v, float std_w, float* __restrict__ reach) {
+  sample_noise_body(states, noise, count, std_v, std_w, reach);
+}
+
 // [emu:end noise]
+// [emu:begin noise_batch]
+// batched one-map solves: planner blockIdx.y, its generators / noise / u_std from the descriptor array
+__global__ void __launch_bounds__(256) sample_noise_batch_kernel(const NoiseDesc* __restrict__ descs, int64_t count) {
+  const NoiseDesc& d = descs[blockIdx.y];
+  sample_noise_body(d.states, reinterpret_cast<float2*>(d.noise), count, d.std_v, d.std_w, nullptr);
+}
+// [emu:end noise_batch]
 
 void launch_sample_noise(uint64_t* states, float* noise, int n_local, int T, float std_v, float std_w,
                          float* reach, cudaStream_t st) {
@@ -45,6 +57,12 @@ void launch_sample_noise(uint64_t* states, float* noise, int n_local, int T, flo
   const int threads = 256;
   sample_noise_kernel<<<(unsigned)((count + threads - 1) / threads), threads, 0, st>>>(
       states, reinterpret_cast<float2*>(noise), count, std_v, std_w, reach);
+}
+
+void launch_sample_noise_batch(const NoiseDesc* descs, int count, int n_local, int T, cudaStream_t st) {
+  const int64_t per = (int64_t)n_local * T;
+  const int threads = 256;
+  sample_noise_batch_kernel<<<dim3((unsigned)((per + threads - 1) / threads), (unsigned)count), threads, 0, st>>>(descs, per);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -135,7 +153,8 @@ __device__ void apply_update(const UpdateArgs& a, const float* __restrict__ part
 //   UPD_TAIL_APPLY  one rank: applies the update (u_cur, normalised weights) -- the whole update is ONE launch,
 //   UPD_TAIL_BCAST  stores the partial into slot `rank` of every peer's gather buffer and raises its epoch flag
 //                   (the all-gather of the peer-memory exchange, p2p.cu has the protocol).
-__global__ void __launch_bounds__(UPD_THREADS) update_partial_kernel(const UpdateArgs a, const UpdateTail tl) {
+// UPD_TAIL_APPLY also stores the new u into tl.u_prev / tl.u_out where those are set (batched solves).
+__device__ __forceinline__ void update_partial_body(const UpdateArgs& a, const UpdateTail& tl) {
   __shared__ float s_red[UPD_THREADS / 32];
   __shared__ float s_w[64];
   __shared__ float s_beta;
@@ -246,7 +265,10 @@ __global__ void __launch_bounds__(UPD_THREADS) update_partial_kernel(const Updat
       const float u = a.u_cur[j] + v / W;
       const float lo = (j & 1) ? a.wrange[0] : a.vrange[0];
       const float hi = (j & 1) ? a.wrange[1] : a.vrange[1];
-      a.u_cur[j] = fmaxf(lo, fminf(hi, u));
+      const float un = fmaxf(lo, fminf(hi, u));
+      a.u_cur[j] = un;
+      if (tl.u_prev) tl.u_prev[j] = un;
+      if (tl.u_out) tl.u_out[j] = un;
     }
   }
   if (tid == 0) { a.rank_partial[0] = s_bS[0]; a.rank_partial[1] = W; }
@@ -269,6 +291,10 @@ __global__ void __launch_bounds__(UPD_THREADS) update_partial_kernel(const Updat
   }
 }
 
+__global__ void __launch_bounds__(UPD_THREADS) update_partial_kernel(const UpdateArgs a, const UpdateTail tl) {
+  update_partial_body(a, tl);
+}
+
 // gathered rank partials -> u_cur (clipped), plus this rank's normalised weights.  wait_flags != null: the partials
 // arrive through the peer-memory exchange -- every CTA first waits (bounded) until all ranks' epoch flags are up.
 __global__ void __launch_bounds__(UPD_THREADS) update_apply_kernel(const UpdateArgs a,
@@ -282,9 +308,20 @@ __global__ void __launch_bounds__(UPD_THREADS) update_apply_kernel(const UpdateA
 }
 
 // [emu:end update]
+// [emu:begin update_batch]
+// batched one-map solves: planner blockIdx.y, each with its own CTA partials, ticket counter, weights and u
+__global__ void __launch_bounds__(UPD_THREADS) update_partial_batch_kernel(const UpdateBatchDesc* __restrict__ descs) {
+  const UpdateBatchDesc& d = descs[blockIdx.y];
+  update_partial_body(d.a, d.tl);
+}
+// [emu:end update_batch]
 
 void launch_update_partial(const UpdateArgs& a, const UpdateTail& tl, cudaStream_t st) {
   update_partial_kernel<<<a.num_ctas, UPD_THREADS, 0, st>>>(a, tl);
+}
+
+void launch_update_partial_batch(const UpdateBatchDesc* descs, int count, int num_ctas, cudaStream_t st) {
+  update_partial_batch_kernel<<<dim3((unsigned)num_ctas, (unsigned)count), UPD_THREADS, 0, st>>>(descs);
 }
 
 void launch_update_finish(const UpdateArgs& a, const float* gathered, int count, const FlagWait& fw, cudaStream_t st) {

@@ -75,7 +75,7 @@ __device__ __forceinline__ float ctrl_term(float u0, float u1, float e0, float e
 // Generic rollout kernel: one thread per (n, m); lanes of a warp = consecutive n on the SAME map.
 // MODE 0: stochastic (per-(m,n) cost -> a.dst);  MODE 1: det dynamics;  MODE 2: nominal + speed map.
 template <int MODE>
-__global__ void __launch_bounds__(128) rollout_kernel(const RolloutArgs a) {
+__device__ __forceinline__ void rollout_body(const RolloutArgs& a) {
   const RolloutParams& p = a.p;
   extern __shared__ float s_u[];           // u_cur (T,2)
   for (int i = threadIdx.x; i < 2 * p.T; i += blockDim.x) s_u[i] = a.u_cur[i];
@@ -142,12 +142,17 @@ __global__ void __launch_bounds__(128) rollout_kernel(const RolloutArgs a) {
   }
 }
 
+template <int MODE>
+__global__ void __launch_bounds__(128) rollout_kernel(const RolloutArgs a) {
+  rollout_body<MODE>(a);
+}
+
 // ---------------------------------------------------------------------------------------------
 // MODE 3: the map-free "barebone" MPPI of the reference's barebone_mppi_numba.ipynb (cell 3, rollout_numba):
 // nominal float32 unicycle, stage cost w*d^2, circular obstacles, terminal cost (1-reached)*d^2.
 // Contractions follow the SASS of the compiled notebook kernel (dv = FMUL(v, dt); x = FFMA(dv, cos, x);
 // theta = FFMA(w, dt, theta); d^2 - r^2 as one FFMA; the obstacle indicator enters through a float64 FMA).
-__global__ void __launch_bounds__(128) rollout_barebone_kernel(const RolloutArgs a) {
+__device__ __forceinline__ void rollout_barebone_body(const RolloutArgs& a) {
   const RolloutParams& p = a.p;
   extern __shared__ float s_u[];
   for (int i = threadIdx.x; i < 2 * p.T; i += blockDim.x) s_u[i] = a.u_cur[i];
@@ -189,7 +194,20 @@ __global__ void __launch_bounds__(128) rollout_barebone_kernel(const RolloutArgs
   a.costs[n] = cost;
 }
 
+__global__ void __launch_bounds__(128) rollout_barebone_kernel(const RolloutArgs a) {
+  rollout_barebone_body(a);
+}
+
 // [emu:end rollout]
+// [emu:begin rollout_batch]
+// batched one-map solves (modes 1, 2, 3): planner blockIdx.y, its full RolloutArgs (geometry, maps, noise, u, costs)
+// from the descriptor array; N and T are the batch's, so the grid and the 2T floats of shared memory are too
+template <int MODE>
+__global__ void __launch_bounds__(128) rollout_batch_kernel(const RolloutArgs* __restrict__ descs) {
+  if constexpr (MODE == 3) rollout_barebone_body(descs[blockIdx.y]);
+  else rollout_body<MODE>(descs[blockIdx.y]);
+}
+// [emu:end rollout_batch]
 void launch_rollout(const RolloutArgs& a, cudaStream_t st) {
   const int threads = 128;
   if (a.mode == 3) {
@@ -201,6 +219,15 @@ void launch_rollout(const RolloutArgs& a, cudaStream_t st) {
   if (a.mode == 0) rollout_kernel<0><<<grid, threads, smem, st>>>(a);
   else if (a.mode == 1) rollout_kernel<1><<<grid, threads, smem, st>>>(a);
   else rollout_kernel<2><<<grid, threads, smem, st>>>(a);
+}
+
+void launch_rollout_batch(const RolloutArgs* descs, int count, int mode, int N, int T, cudaStream_t st) {
+  const int threads = 128;
+  const dim3 grid((N + threads - 1) / threads, count);
+  const size_t smem = (size_t)2 * T * sizeof(float);
+  if (mode == 1) rollout_batch_kernel<1><<<grid, threads, smem, st>>>(descs);
+  else if (mode == 2) rollout_batch_kernel<2><<<grid, threads, smem, st>>>(descs);
+  else rollout_batch_kernel<3><<<grid, threads, smem, st>>>(descs);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -207,7 +207,7 @@ constexpr bool SG_VALUES_IN_REGISTERS = false;
 constexpr bool SG_POPC_PER_WORD = SG_POPC_VARIANT;
 
 template <int NT, int NW>
-__global__ void __launch_bounds__(256) sample_grids_v2_kernel(const SampleGridsV2Args a) {
+__device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int nw = (NW > 0) ? NW : a.t[0].bpad / 4;
   const int bpad = nw * 4;
@@ -411,6 +411,11 @@ __global__ void __launch_bounds__(256) sample_grids_v2_kernel(const SampleGridsV
   }
 }
 
+template <int NT, int NW>
+__global__ void __launch_bounds__(256) sample_grids_v2_kernel(const SampleGridsV2Args a) {
+  sample_grids_v2_body<NT, NW>(a);
+}
+
 // whole-tile advance of every generator (box mode: the sampler walks only part of each tile, so the states a
 // whole-map walk would leave behind are produced by ONE GF(2) jump per generator).  Tile classes as sample_tile_draws.
 __global__ void __launch_bounds__(128) advance_states_kernel(const ulonglong2* __restrict__ in, ulonglong2* __restrict__ out0,
@@ -434,6 +439,15 @@ __global__ void __launch_bounds__(128) advance_states_kernel(const ulonglong2* _
 }
 
 // [emu:end sampler_v2]
+// [emu:begin sampler_batch]
+// batched one-map solves: one fused lin + ang whole-map launch for every pair of the batch, pair blockIdx.z.  The
+// launch geometry (rows, cols, bins, pitch, thread tiles, segments) is the batch's; each descriptor brings its own
+// TDM buffers, threshold table and jump matrices.
+template <int NT, int NW>
+__global__ void __launch_bounds__(256) sample_grids_v2_batch_kernel(const SampleGridsV2Args* __restrict__ descs) {
+  sample_grids_v2_body<NT, NW>(descs[blockIdx.z]);
+}
+// [emu:end sampler_batch]
 
 void launch_advance_states(const uint64_t* states, uint64_t* out0, uint64_t* out1, const uint64_t* mats, int rows,
                            int cols, int tx, int ty, int num_maps, cudaStream_t st) {
@@ -496,6 +510,31 @@ bool sample_grids_v2_fits(const SampleGridsV2Args& a, int nt) {
 
 void launch_sample_grids_v2(const SampleGridsV2Args& a, int nt, cudaStream_t st) {
   if (nt == 2) launch_v2_nt<2>(a, st); else launch_v2_nt<1>(a, st);
+}
+
+bool sample_grids_v2_same_launch(const SampleGridsV2Args& a, const SampleGridsV2Args& b) {
+  return a.rows == b.rows && a.cols == b.cols && a.grid_rows == b.grid_rows && a.pitch == b.pitch && a.tx == b.tx &&
+         a.ty == b.ty && a.num_maps == b.num_maps && a.segs == b.segs && a.seg_rows == b.seg_rows && a.gm == b.gm &&
+         a.tix_lo == b.tix_lo && a.tiy_lo == b.tiy_lo && a.nact == b.nact && a.row_lo == b.row_lo &&
+         a.row_hi == b.row_hi && a.t[0].bpad == b.t[0].bpad && a.t[1].bpad == b.t[1].bpad;
+}
+
+void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs, int count,
+                                  cudaStream_t st) {
+  const int nrow = (geom.rows + geom.tx - 1) / geom.tx;
+  const int tix_hi = std::min(geom.tx - 1, (std::max(geom.row_hi, geom.row_lo + 1) - 1) / nrow);
+  const dim3 grid((tix_hi - geom.tix_lo + 1) * geom.segs, (geom.num_maps + geom.gm - 1) / geom.gm, count);
+  const int threads = v2_threads(geom);
+  const size_t smem = sample_grids_v2_smem(geom, 2);
+  const int nw = geom.t[0].bpad / 4;
+  auto go = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    kern<<<grid, threads, smem, st>>>(descs);
+  };
+  if (nw == 3) go(sample_grids_v2_batch_kernel<2, 3>);
+  else if (nw == 8) go(sample_grids_v2_batch_kernel<2, 8>);
+  else if (nw == 1) go(sample_grids_v2_batch_kernel<2, 1>);
+  else go(sample_grids_v2_batch_kernel<2, 0>);
 }
 
 static inline void next_h(uint64_t& s0, uint64_t& s1);
