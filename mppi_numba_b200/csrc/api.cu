@@ -149,9 +149,10 @@ static int tdm_prepare_jump(b200mppi_tdm* t, cudaStream_t st) {
   if (rc) return rc;
   // a boxed launch covers a few tile rows only: finer row segments keep every SM busy through several waves
   // (with whole-map segment sizes a large share of the SM-cycles sits idle in the tail)
-  // ~3 waves of the ~6 resident CTAs per SM, for a box of ~8 tile rows sampled ~14 maps per CTA (the segment count
-  // only splits the work: every segment starts from its generator's jumped state, the draws are the same)
-  int bsegs = (3 * 6 * device_sm_count() + 8 * ((t->num_maps + 13) / 14) - 1) / (8 * ((t->num_maps + 13) / 14));
+  // ~6 waves of the ~6 resident CTAs per SM, for a box of ~8 tile rows sampled ~14 maps per CTA (the segment count
+  // only splits the work: every segment starts from its generator's jumped state, the draws are the same).  At
+  // config 5 on an H100 that is 32 segments; 16 (3 waves) left the boxed kernel ~5 % slower, 64 ~4 % slower.
+  int bsegs = (6 * 6 * device_sm_count() + 8 * ((t->num_maps + 13) / 14) - 1) / (8 * ((t->num_maps + 13) / 14));
   if (const char* e = getenv("B200MPPI_SAMPLE_BOX_SEGS")) bsegs = atoi(e);
   if (bsegs > SAMPLE_BOX_MAX_SEGS) bsegs = SAMPLE_BOX_MAX_SEGS;
   if (bsegs > nrow) bsegs = nrow;
@@ -620,8 +621,7 @@ extern "C" int b200mppi_debug_sample_threshold(double alpha_dyn, int32_t q_cap, 
   if (!build_sample_thresholds(alpha_dyn, q_cap, T))
     return fail(B200MPPI_ESTATE, "debug_sample_threshold: alpha_dyn / q_cap not representable by the bucket table "
                                  "(the sampler falls back to its generic kernel)");
-  const unsigned char* Q = reinterpret_cast<const unsigned char*>(T + 256);
-  for (int64_t i = 0; i < n; ++i) q_out[i] = (uint8_t)sample_threshold_q(draws[i], T, Q);
+  for (int64_t i = 0; i < n; ++i) q_out[i] = (uint8_t)sample_threshold_q(draws[i], T);
   return B200MPPI_OK;
 }
 

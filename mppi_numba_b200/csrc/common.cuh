@@ -128,13 +128,14 @@ __device__ __forceinline__ float xoro_normal(Xoro& s) {
 // Threshold of sample_grids_numba, q(r) = int8(ceil(f64(f32((r >> 11) * 2^-53)) * 100 * alpha)) (terrain.py:682-684),
 // as a lookup on the RAW 64-bit draw r: q is a monotone step function of r; bucket = top 8 bits of r; inside a
 // bucket q rises at most once, at the raw value thr[bucket] (thr = 0 with qbase = q - 1: "already risen").
+// One 64-bit entry per bucket: thr | qbase.  The breakpoints are (53-bit draw) << 11, so the low 11 bits of thr are
+// free and hold qbase (<= 127); r >= thr  <=>  (r | 0x7ff) >= (thr | qbase).
 // Tables come from build_sample_thresholds (sample.cu), which verifies that alpha is representable this way.
 // Shared by the sampler kernel and the host-side check b200mppi_debug_sample_threshold.
 // [emu:begin threshold]
-__host__ __device__ __forceinline__ uint32_t sample_threshold_q(uint64_t r, const uint64_t* thr,
-                                                                const unsigned char* qbase) {
-  const uint32_t b = (uint32_t)(r >> 56);
-  return (uint32_t)qbase[b] + (r >= thr[b] ? 1u : 0u);
+__host__ __device__ __forceinline__ uint32_t sample_threshold_q(uint64_t r, const uint64_t* table) {
+  const uint64_t e = table[r >> 56];
+  return ((uint32_t)e & 0x7ffu) + ((r | 0x7ffULL) >= e ? 1u : 0u);
 }
 // [emu:end threshold]
 

@@ -27,7 +27,7 @@ struct SampleTdm {
 };
 struct SampleGridsV2Args {
   SampleTdm t[2];
-  const uint64_t* thresholds;   // device, SAMPLE_TABLE_WORDS u64: thr[256] then the 256 qbase bytes (sample_threshold_q)
+  const uint64_t* thresholds;   // device, SAMPLE_TABLE_WORDS u64: thr | qbase per bucket (sample_threshold_q)
   const uint64_t* jump;         // device, [(segs-1)*2][128][2]: A^(s*seg_rows*width) for width class 0 / 1
   int rows, cols, grid_rows, pitch, tx, ty, num_maps;
   int segs, seg_rows;           // row segments per generator tile (jump-ahead split), rows per segment
@@ -48,9 +48,9 @@ inline void sample_box_full(SampleGridsV2Args& a) {
 }
 void build_jump_matrices(const int64_t* ks, int count, uint64_t* out);
 void build_jump_series(int64_t k0, int64_t k1, int segs, uint64_t* out);     // (s-1)*2 + c -> A^(s * k_c), s = 1 .. segs-1
-// q(r) of a RAW 64-bit draw r as a two-table lookup over its top 8 bits (see sample_threshold_q in common.cuh):
-// table = thr[256] (u64) followed by qbase[256] (u8).  false if alpha is not representable that way.
-constexpr int SAMPLE_TABLE_WORDS = 256 + 256 / 8;
+// q(r) of a RAW 64-bit draw r as a table lookup over its top 8 bits (see sample_threshold_q in common.cuh):
+// table = thr[256] | qbase[256] (u64, qbase in the low 11 bits).  false if alpha is not representable that way.
+constexpr int SAMPLE_TABLE_WORDS = 256;
 // [emu:end sampler_args]
 bool build_sample_thresholds(double alpha, int q_cap, uint64_t* table /*[SAMPLE_TABLE_WORDS]*/);
 bool sample_grids_v2_fits(const SampleGridsV2Args& a, int nt);

@@ -150,7 +150,8 @@ void launch_sample_grids(const SampleGridsArgs& a, cudaStream_t st) {
 //     conversion (XU-pipe) instructions: q(v) is a monotone step function of the 53-bit draw v, so the
 //     host tabulates its breakpoints T[k] = min{v : q(v) >= k} with the exact float arithmetic and folds
 //     them into a 256-entry table over the top 8 bits of v: (q at the bucket start, the one breakpoint
-//     inside the bucket) -- one shared-memory load and one 64-bit compare per draw (the host verifies that
+//     inside the bucket, packed into one 64-bit word) -- one shared-memory load and one 64-bit compare per
+//     draw (the host verifies that
 //     no bucket holds two breakpoints, otherwise the generic kernel is used);
 //   * the first bin whose cumulative mass reaches q is found with a SIMD-in-register byte compare and
 //     one POPC instead of a loop;
@@ -251,8 +252,7 @@ __device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a)
   const int gm = a.gm;
   unsigned char* s_cum = smem;                               // [NT][row_bytes_al]
   unsigned char* s_stage = s_cum + NT * row_bytes_al;        // [NT][gm][stage_pitch]
-  uint64_t* s_T = reinterpret_cast<uint64_t*>(s_stage + max(NT * gm * stage_pitch, 2 * 128 * 16));   // [256] bucket thresholds
-  const unsigned char* s_Q = reinterpret_cast<const unsigned char*>(s_T + 256);      // [256] q at bucket start
+  uint64_t* s_T = reinterpret_cast<uint64_t*>(s_stage + max(NT * gm * stage_pitch, 2 * 128 * 16));   // [256] thr | qbase
   unsigned char* s_q = reinterpret_cast<unsigned char*>(s_T + SAMPLE_TABLE_WORDS);   // [NT][128]
   // [2][128] segment-start jump matrices: they live in the (not yet used) output stage -- every thread has applied
   // them before the row loop's first barrier, after which the stage is written
@@ -263,7 +263,7 @@ __device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a)
   const int m = blockIdx.y * gm + mloc;
   const bool active = (mloc < gm) && (m < a.num_maps);
 
-  for (int i = tid; i < SAMPLE_TABLE_WORDS; i += nthreads) s_T[i] = a.thresholds[i];   // thresholds + the qbase bytes
+  for (int i = tid; i < SAMPLE_TABLE_WORDS; i += nthreads) s_T[i] = a.thresholds[i];
   // value table indexed by ge = number of cumulative bytes >= q (the SIMD compare yields that count directly):
   // bin = 4*nw - ge, so the table is stored reversed and the lookup is one byte load at s_q[ge]
   for (int i = tid; i < 128; i += nthreads) {
@@ -287,6 +287,20 @@ __device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a)
   const int wc = c1 - c0;
   const int last_seg = (t1 > t0 && wc > 0) ? (t1 - t0 - 1) / a.seg_rows : 0;     // owner of the final state
 
+  // one cumulative-table row of the window -> shared memory, with the guard bits of cell()
+  auto stage_cum_row = [&](int ri) {
+#pragma unroll
+    for (int k = 0; k < NT; ++k) {
+      const uint32_t* src = reinterpret_cast<const uint32_t*>(a.t[k].cum + ((size_t)ri * a.cols + cs0) * bpad);
+      uint32_t* dst = reinterpret_cast<uint32_t*>(s_cum + k * row_bytes_al);
+#pragma unroll 8
+      for (int i = tid; i < row_bytes / 4; i += nthreads) dst[i] = __ldg(src + i) | 0x80808080u;
+    }
+  };
+  // the first row is staged before the jump-ahead below, whose arithmetic then hides the loads' latency (the jump
+  // matrices overlay the output stage, not the cumulative rows)
+  if (rs0 < rs1) stage_cum_row(rs0);
+
   const int64_t gen = (int64_t)tix * ((int64_t)a.ty * a.num_maps) + (int64_t)m * a.ty + tiy;
   if (seg > 0) {                                            // both width classes of this segment's jump (CTA-uniform)
     const ulonglong2* src = reinterpret_cast<const ulonglong2*>(a.jump) + (size_t)(seg - 1) * 2 * 128;
@@ -307,15 +321,9 @@ __device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a)
   if (active && rs0 < rs1)
     for (int64_t i = (int64_t)(rs0 - r0) * wc; i > 0; --i) xoro_next(s);
 
+  // two barriers per row: row ri's cumulative slice is staged (and the previous row's output stage drained) before
+  // the cells; after them, the write-back of row ri and the staging of row ri + 1 run together
   for (int ri = rs0; ri < rs1; ++ri) {
-    __syncthreads();                                          // previous row's stage fully drained
-#pragma unroll
-    for (int k = 0; k < NT; ++k) {
-      const uint32_t* src = reinterpret_cast<const uint32_t*>(a.t[k].cum + ((size_t)ri * a.cols + cs0) * bpad);
-      uint32_t* dst = reinterpret_cast<uint32_t*>(s_cum + k * row_bytes_al);
-#pragma unroll 8
-      for (int i = tid; i < row_bytes / 4; i += nthreads) dst[i] = __ldg(src + i) | 0x80808080u;   // guard bits, see cell()
-    }
     __syncthreads();
     if (active) {
       // one cell: threshold from the 53-bit draw, then the first bin whose cumulative mass reaches it.
@@ -323,7 +331,7 @@ __device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a)
       // the shared-memory loads of the whole group are independent of the byte stores (ILP).
       auto cell = [&](int ci, uint64_t r, uint32_t (&outv)[NT]) {
         // bucket of the raw draw's top 8 bits: q at the bucket start and the single breakpoint inside it
-        const uint32_t q = sample_threshold_q(r, s_T, s_Q);
+        const uint32_t q = sample_threshold_q(r, s_T);
         const uint32_t qq = q * 0x01010101u;
 #pragma unroll
         for (int k = 0; k < NT; ++k) {
@@ -384,7 +392,8 @@ __device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a)
         if (NT == 2) st1[ci] = (unsigned char)o[NT - 1];
       }
     }
-    __syncthreads();
+    __syncthreads();                                          // every cell of row ri read s_cum and wrote the stage
+    if (ri + 1 < rs1) stage_cum_row(ri + 1);
     // coalesced write-back of the gm x NT staged rows: 16-byte chunks, bytes at the ragged ends of the window
     const int chunks = (wcols + 15) / 16;
     const int maps_here = min(gm, a.num_maps - (int)blockIdx.y * gm);
@@ -411,8 +420,10 @@ __device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a)
   }
 }
 
+// four CTAs of 256 threads per SM: a budget of 64 registers, with which every single-planner variant but <2,8> runs
+// without spills (left to itself ptxas picks 40-48 and spills in some of them)
 template <int NT, int NW>
-__global__ void __launch_bounds__(256) sample_grids_v2_kernel(const SampleGridsV2Args a) {
+__global__ void __launch_bounds__(256, 4) sample_grids_v2_kernel(const SampleGridsV2Args a) {
   sample_grids_v2_body<NT, NW>(a);
 }
 
@@ -625,7 +636,7 @@ bool build_sample_thresholds(double alpha, int q_cap, uint64_t* B /*[SAMPLE_TABL
   // bucket b covers the 53-bit draws v in [b << 45, (b+1) << 45), i.e. the RAW draws r = v << 11 | (11 low bits) in
   // [b << 56, (b+1) << 56): v >= T[k]  <=>  r >= T[k] << 11.  Valid iff at most one breakpoint lies strictly inside
   // each bucket and it raises q by exactly one.  No breakpoint inside: thr = 0 ("r >= thr" always true), qbase = q-1.
-  unsigned char* Q = reinterpret_cast<unsigned char*>(B + 256);
+  // The entry is thr | qbase (sample_threshold_q): thr has its low 11 bits clear, qbase <= 127.
   for (int b = 0; b < 256; ++b) {
     const uint64_t start = (uint64_t)b << 45, end = start + (1ULL << 45);
     const int qb = q_of_v(start, alpha);
@@ -636,17 +647,15 @@ bool build_sample_thresholds(double alpha, int q_cap, uint64_t* B /*[SAMPLE_TABL
     if (inside > 1 || qb < 0 || qb > 127) return false;
     if (inside == 1) {
       if (q_of_v(next, alpha) != qb + 1) return false;
-      B[b] = next << 11;
-      Q[b] = (unsigned char)qb;
+      B[b] = (next << 11) | (uint64_t)qb;
     } else if (qb > 0) {
-      B[b] = 0;
-      Q[b] = (unsigned char)(qb - 1);
+      B[b] = (uint64_t)(qb - 1);
     } else {
       // q = 0 over a whole bucket: only v = 0 has q = 0 for alpha > 0 (bucket 0 then holds the breakpoint v = 1),
-      // so this is alpha = 0; "never" needs thr > every r of the bucket, which bucket 255 cannot offer
+      // so this is alpha = 0; "never" needs thr > every r of the bucket (the next bucket's start), which bucket 255
+      // cannot offer
       if (b == 255) return false;
-      B[b] = ~0ULL;
-      Q[b] = 0;
+      B[b] = (uint64_t)(b + 1) << 56;
     }
   }
   return true;
