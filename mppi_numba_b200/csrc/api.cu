@@ -55,7 +55,6 @@ struct b200mppi_tdm {
   // stale ones outside; states_alt still holds the pre-solve generator states, so the whole maps of that very
   // sampling call can be produced on demand (tdm_complete_grid) -- every reader of `grid` outside solve() does
   bool grid_partial = false;
-  bool advance_done = false;        // advance_states already launched for the coming boxed sampling (tdm_pair_advance_early)
   double partial_alpha = 1.0;
   float tr_abs_max = 0.0f;          // max |traction| a sampled byte can decode to: max_b |lo + 0.01*(hi-lo)*q_b|
   int64_t num_gen = 0;
@@ -70,7 +69,6 @@ struct b200mppi_tdm {
   bool masks01 = true;            // every obstacle / unknown byte is 0 or 1 (b200mppi_tdm_set_masks checks the host arrays)
   size_t mask_cap = 0, risk_cap = 0;
   int mask_rows = 0, mask_cols = 0, mask_pitch = 0;
-  int64_t launches = 0;
   // fast sampler eligibility (sample.cu v2): entries in [0,127], monotone sums <= 127
   bool pmf_valid = false;
   int min_total = 0;            // smallest column total (q above it would leave a cell unwritten)
@@ -200,42 +198,6 @@ static void apply_box(const b200mppi_tdm* t, SampleGridsV2Args& a, const SampleB
   a.disc_cx = b.cx; a.disc_cy = b.cy; a.disc_r = b.r;
 }
 
-// One TDM.  Fast staged sampler when the PMF is well-formed, else the generic per-generator kernel.
-// box != null (solve() only): sample just that part of every map; generator states advance as for whole maps.
-static int tdm_sample_on(b200mppi_tdm* t, double alpha_dyn, cudaStream_t st, const SampleBox* box = nullptr) {
-  if (!t->pmf_set) return fail(B200MPPI_ESTATE, "sample_grids: PMF grid not set");
-  int rc = tdm_prepare_thresholds(t, alpha_dyn, st);
-  if (rc) return rc;
-  if ((rc = tdm_prepare_jump(t, st))) return rc;
-  SampleGridsV2Args v2{};
-  fill_v2(t, v2, 0);
-  bool boxed = false;
-  if (t->thr_ok && sample_grids_v2_fits(v2, 1)) {
-    if (box) {
-      SampleGridsV2Args bx = v2;
-      apply_box(t, bx, *box);
-      if (sample_grids_v2_fits(bx, 1)) { v2 = bx; boxed = true; }
-    }
-    launch_sample_grids_v2(v2, 1, st);
-    if (boxed) launch_advance_states(t->states, t->states_alt, nullptr, t->jump_tile_d, t->rows, t->cols, v2.tx, v2.ty,
-                                     t->num_maps, st);
-  } else {
-    SampleGridsArgs a{};
-    a.grid = t->grid; a.cum = t->cum; a.states = t->states; a.qvals = t->qvals;
-    a.num_bins = t->B; a.bpad = t->bpad; a.rows = t->rows; a.cols = t->cols;
-    a.grid_rows = t->cfg.max_map_rows; a.pitch = t->pitch;
-    a.tx = t->cfg.tdm_thread_x; a.ty = t->cfg.tdm_thread_y; a.num_maps = t->num_maps;
-    a.alpha_dyn = alpha_dyn;
-    launch_sample_grids(a, st);
-  }
-  CHECK_LAUNCH();
-  if (t->thr_ok && sample_grids_v2_fits(v2, 1)) std::swap(t->states, t->states_alt);   // advanced states: other buffer
-  t->launches += boxed ? 2 : 1;
-  t->grid_partial = boxed; t->partial_alpha = alpha_dyn;
-  tdm_advance_sig(t);
-  return B200MPPI_OK;
-}
-
 // Two distinct TDMs whose generators are in identical states over identical tiles: one stream of draws samples both.
 static bool tdm_same_stream(const b200mppi_tdm* l, const b200mppi_tdm* g) {
   return l != g && l->sig == g->sig && l->rows == g->rows && l->cols == g->cols && l->num_maps == g->num_maps &&
@@ -243,74 +205,101 @@ static bool tdm_same_stream(const b200mppi_tdm* l, const b200mppi_tdm* g) {
          l->cfg.tdm_thread_y == g->cfg.tdm_thread_y && l->cfg.max_map_rows == g->cfg.max_map_rows;
 }
 
-// Bookkeeping of a fused whole-map pair sampling (launched by the caller): advanced states, fresh signatures.
-static void tdm_pair_sampled_whole(b200mppi_tdm* l, b200mppi_tdm* g, double alpha_dyn) {
-  std::swap(l->states, l->states_alt);
-  std::swap(g->states, g->states_alt);
-  l->grid_partial = g->grid_partial = false;
-  l->partial_alpha = g->partial_alpha = alpha_dyn;
-  tdm_advance_sig(l);
-  tdm_advance_sig(g);
-}
+// How one sampling call samples one TDM or a lin/ang pair.  Fused: the pair's generator states are identical (same
+// seed, same history: the reference seeds both with cfg.seed), so ONE staged launch (nt = 2, args a[0]) draws each
+// uniform once and samples both maps.  Otherwise each TDM on its own, one after the other: the staged sampler (nt = 1,
+// args a[i]) when its PMF is well-formed at this alpha and the launch fits, else the generic per-generator kernel.
+// boxed[i]: a[i] samples only the reach box (plan_box); generator states still advance as for whole maps.
+struct SamplePlan {
+  b200mppi_tdm* t[2] = {};
+  int nt = 1;
+  bool fused = false;
+  bool v2[2] = {};
+  bool boxed[2] = {};
+  double alpha = 1.0;
+  SampleGridsV2Args a[2] = {};
+};
 
-// Both TDMs of a planner.  When their generator states are identical (same seed, same history: the
-// reference seeds both with cfg.seed) ONE pass draws each uniform once and samples both maps.
-// The state advance of a boxed pair sampling does not depend on the box: solve() launches it while the host still waits
-// for the reach read-back (the GPU would idle), tdm_sample_pair_on then skips its own.  If the sampling falls back to
-// whole maps after all, that launch stores the very same states again.
-static void tdm_pair_advance_early(b200mppi_tdm* l, b200mppi_tdm* g, double alpha_dyn, cudaStream_t st, int64_t* launches) {
-  if (!l->pmf_set || !g->pmf_set || l == g) return;
-  if (tdm_prepare_thresholds(l, alpha_dyn, st) || tdm_prepare_thresholds(g, alpha_dyn, st)) return;
-  const bool same_stream = tdm_same_stream(l, g);
-  if (!same_stream || !l->thr_ok || !g->thr_ok || tdm_prepare_jump(l, st)) return;
-  SampleGridsV2Args v2{};
-  fill_v2(l, v2, 0);
-  fill_v2(g, v2, 1);
-  if (!sample_grids_v2_fits(v2, 2)) return;
-  launch_advance_states(l->states, l->states_alt, g->states_alt, l->jump_tile_d, l->rows, l->cols, v2.tx, v2.ty,
-                        l->num_maps, st);
-  if (cudaGetLastError() != cudaSuccess) return;
-  l->advance_done = true;
-  *launches += 1;
-}
-
-static int tdm_sample_pair_on(b200mppi_tdm* l, b200mppi_tdm* g, double alpha_dyn, cudaStream_t st, int64_t* launches,
-                              const SampleBox* box = nullptr) {
-  if (!l->pmf_set || !g->pmf_set) return fail(B200MPPI_ESTATE, "sample_grids: PMF grid not set");
-  int rc = tdm_prepare_thresholds(l, alpha_dyn, st);
-  if (rc) return rc;
-  if ((rc = tdm_prepare_thresholds(g, alpha_dyn, st))) return rc;
-  const bool same_stream = tdm_same_stream(l, g);
-  if ((rc = tdm_prepare_jump(l, st))) return rc;
-  SampleGridsV2Args v2{};
-  fill_v2(l, v2, 0);
-  fill_v2(g, v2, 1);
-  if (same_stream && l->thr_ok && g->thr_ok && sample_grids_v2_fits(v2, 2)) {
-    bool boxed = false;
-    if (box) {
-      SampleGridsV2Args bx = v2;
-      apply_box(l, bx, *box);
-      if (sample_grids_v2_fits(bx, 2)) { v2 = bx; boxed = true; }
-    }
-    launch_sample_grids_v2(v2, 2, st);
-    const bool early = l->advance_done;
-    l->advance_done = false;
-    if (boxed && !early) launch_advance_states(l->states, l->states_alt, g->states_alt, l->jump_tile_d, l->rows, l->cols,
-                                               v2.tx, v2.ty, l->num_maps, st);
-    CHECK_LAUNCH();
-    std::swap(l->states, l->states_alt);
-    std::swap(g->states, g->states_alt);
-    l->grid_partial = g->grid_partial = boxed;
-    l->partial_alpha = g->partial_alpha = alpha_dyn;
-    tdm_advance_sig(l);
-    tdm_advance_sig(g);
-    *launches += (boxed && !early) ? 2 : 1;
-    return B200MPPI_OK;
+// Host preparation (threshold tables; jump tables where the staged sampler may run) and the whole-map plan of TDM l,
+// or of the pair l, g.  g may be l: that TDM is then sampled twice.
+static int plan_sampling(b200mppi_tdm* l, b200mppi_tdm* g, double alpha, cudaStream_t st, SamplePlan* pl) {
+  *pl = SamplePlan{};
+  pl->t[0] = l; pl->t[1] = g; pl->nt = g ? 2 : 1; pl->alpha = alpha;
+  int rc;
+  for (int i = 0; i < pl->nt; ++i) {
+    if (!pl->t[i]->pmf_set) return fail(B200MPPI_ESTATE, "sample_grids: PMF grid not set");
+    if ((rc = tdm_prepare_thresholds(pl->t[i], alpha, st))) return rc;
   }
-  l->advance_done = false;
-  if ((rc = tdm_sample_on(l, alpha_dyn, st, box))) return rc;
-  if ((rc = tdm_sample_on(g, alpha_dyn, st, box))) return rc;
-  *launches += (l->grid_partial ? 2 : 1) + (g->grid_partial ? 2 : 1);
+  if (l->thr_ok && (rc = tdm_prepare_jump(l, st))) return rc;
+  if (g && tdm_same_stream(l, g) && l->thr_ok && g->thr_ok) {      // the fused launch runs on l's jump tables
+    fill_v2(l, pl->a[0], 0);
+    fill_v2(g, pl->a[0], 1);
+    if (sample_grids_v2_fits(pl->a[0], 2)) { pl->fused = pl->v2[0] = pl->v2[1] = true; return B200MPPI_OK; }
+    pl->a[0] = SampleGridsV2Args{};
+  }
+  if (g && g->thr_ok && (rc = tdm_prepare_jump(g, st))) return rc;
+  for (int i = 0; i < pl->nt; ++i) {
+    if (!pl->t[i]->thr_ok) continue;
+    fill_v2(pl->t[i], pl->a[i], 0);
+    pl->v2[i] = sample_grids_v2_fits(pl->a[i], 1);
+  }
+  return B200MPPI_OK;
+}
+
+// Narrow a plan's staged launches to `b` where the narrowed launch fits; the others (and the generic kernel) keep
+// sampling whole maps.
+static void plan_box(SamplePlan* pl, const SampleBox& b) {
+  for (int i = 0; i < (pl->fused ? 1 : pl->nt); ++i) {
+    if (!pl->v2[i]) continue;
+    SampleGridsV2Args bx = pl->a[i];
+    apply_box(pl->t[i], bx, b);
+    if (sample_grids_v2_fits(bx, pl->fused ? 2 : 1)) { pl->a[i] = bx; pl->boxed[i] = true; }
+  }
+  if (pl->fused) pl->boxed[1] = pl->boxed[0];
+}
+
+// The state advance of a boxed staged launch (which stores no states) for TDM i, or for the fused pair: every generator
+// jumped over its whole tile into the other buffer.  It does not depend on the box.
+static void launch_plan_advance(const SamplePlan& pl, int i, cudaStream_t st) {
+  const b200mppi_tdm* t = pl.t[i];
+  launch_advance_states(t->states, t->states_alt, pl.fused ? pl.t[1]->states_alt : nullptr, t->jump_tile_d, t->rows,
+                        t->cols, t->cfg.tdm_thread_x, t->cfg.tdm_thread_y, t->num_maps, st);
+}
+
+// After TDM i's sampling: the staged sampler left the advanced states in the other buffer (the generic kernel advances
+// them in place), the maps are fresh inside the box only, if boxed, and the signature moves on.
+static void plan_commit(const SamplePlan& pl, int i) {
+  b200mppi_tdm* t = pl.t[i];
+  if (pl.v2[i]) std::swap(t->states, t->states_alt);
+  t->grid_partial = pl.boxed[i];
+  t->partial_alpha = pl.alpha;
+  tdm_advance_sig(t);
+}
+
+// Issue a plan's launches -- each sampler launch followed, if boxed, by its state advance unless `advanced` (the fused
+// pair's advance is already queued: stage_sample_tdms) -- add their number to *launches, and commit every TDM.
+static int plan_launch(SamplePlan& pl, bool advanced, cudaStream_t st, int64_t* launches) {
+  for (int i = 0; i < (pl.fused ? 1 : pl.nt); ++i) {
+    b200mppi_tdm* t = pl.t[i];
+    if (pl.v2[i]) {
+      // the states as they are now: when lin == ang the first sampling has swapped the buffers
+      pl.a[i].t[0].states = t->states; pl.a[i].t[0].states_out = t->states_alt;
+      launch_sample_grids_v2(pl.a[i], pl.fused ? 2 : 1, st);
+      if (pl.boxed[i] && !advanced) launch_plan_advance(pl, i, st);
+    } else {
+      SampleGridsArgs a{};
+      a.grid = t->grid; a.cum = t->cum; a.states = t->states; a.qvals = t->qvals;
+      a.num_bins = t->B; a.bpad = t->bpad; a.rows = t->rows; a.cols = t->cols;
+      a.grid_rows = t->cfg.max_map_rows; a.pitch = t->pitch;
+      a.tx = t->cfg.tdm_thread_x; a.ty = t->cfg.tdm_thread_y; a.num_maps = t->num_maps;
+      a.alpha_dyn = pl.alpha;
+      launch_sample_grids(a, st);
+    }
+    CHECK_LAUNCH();
+    *launches += pl.boxed[i] && !advanced ? 2 : 1;
+    plan_commit(pl, i);
+    if (pl.fused) plan_commit(pl, 1);
+  }
   return B200MPPI_OK;
 }
 
@@ -318,16 +307,13 @@ static int tdm_sample_pair_on(b200mppi_tdm* l, b200mppi_tdm* g, double alpha_dyn
 // double buffer still holds; the advanced states the walk stores are the ones `states` already holds.
 static int tdm_complete_grid(b200mppi_tdm* t, cudaStream_t st) {
   if (!t->grid_partial) return B200MPPI_OK;
-  int rc = tdm_prepare_thresholds(t, t->partial_alpha, st);
+  SamplePlan pl;
+  const int rc = plan_sampling(t, nullptr, t->partial_alpha, st, &pl);
   if (rc) return rc;
-  if ((rc = tdm_prepare_jump(t, st))) return rc;
-  SampleGridsV2Args v2{};
-  fill_v2(t, v2, 0);
-  v2.t[0].states = t->states_alt; v2.t[0].states_out = t->states;
-  if (!t->thr_ok || !sample_grids_v2_fits(v2, 1)) return fail(B200MPPI_ESTATE, "complete_grid: sampler state changed");
-  launch_sample_grids_v2(v2, 1, st);
+  if (!pl.v2[0]) return fail(B200MPPI_ESTATE, "complete_grid: sampler state changed");
+  pl.a[0].t[0].states = t->states_alt; pl.a[0].t[0].states_out = t->states;
+  launch_sample_grids_v2(pl.a[0], 1, st);
   CHECK_LAUNCH();
-  t->launches++;
   t->grid_partial = false;
   return B200MPPI_OK;
 }
@@ -468,7 +454,6 @@ extern "C" int b200mppi_tdm_set_pmf(b200mppi_tdm* t, const int8_t* pmf, int32_t 
   }
   t->grid_partial = false;                                // a new PMF: nothing left to complete
   launch_build_cum(t->pmf, t->cum, B, bpad, rows, cols, t->stream);
-  t->launches++;
   CHECK_LAUNCH();
   CU(cudaStreamSynchronize(t->stream));
   t->B = B; t->bpad = bpad; t->rows = rows; t->cols = cols;
@@ -516,7 +501,6 @@ extern "C" int b200mppi_tdm_set_pmf_collapsed(b200mppi_tdm* t, const int8_t* raw
     cudaMemsetAsync(bad_d, 0, sizeof(int), t->stream);
     launch_collapse_pad(raw_d, t->pmf, speed ? t->risk : nullptr, bad_d, bv_d, B, H, W, keep_r, keep_c, pad, rpitch, alpha,
                         bounds[0], bounds[1] - bounds[0], t->cfg.mode, t->stream);
-    t->launches++;
     int bad = 0;
     cudaMemcpyAsync(&bad, bad_d, sizeof(int), cudaMemcpyDeviceToHost, t->stream);
     cudaMemcpyAsync(host_out.data(), t->pmf, out_bytes, cudaMemcpyDeviceToHost, t->stream);
@@ -628,8 +612,10 @@ extern "C" int b200mppi_debug_sample_threshold(double alpha_dyn, int32_t q_cap, 
 extern "C" int b200mppi_tdm_sample_grids(b200mppi_tdm* t, double alpha_dyn) {
   if (!t) return fail(B200MPPI_EINVAL, "null tdm");
   CU(cudaSetDevice(t->cfg.device));
-  int rc = tdm_sample_on(t, alpha_dyn, t->stream);
-  if (rc) return rc;
+  SamplePlan pl;
+  int64_t launches = 0;                       // a TDM keeps no launch count
+  int rc = plan_sampling(t, nullptr, alpha_dyn, t->stream, &pl);
+  if (rc || (rc = plan_launch(pl, false, t->stream, &launches))) return rc;
   CU(cudaStreamSynchronize(t->stream));
   return B200MPPI_OK;
 }
@@ -734,7 +720,7 @@ struct b200mppi_planner {
   bool params_set = false;
   bool profiling = false;
   cudaEvent_t ev[8] = {};
-  cudaEvent_t ev_reach = nullptr;   // after the reach read-back copy (planner_reach_box)
+  cudaEvent_t ev_reach = nullptr;   // after the reach read-back copy (stage_sample_tdms)
   float last_ms[B200MPPI_T_COUNT] = {};
   int64_t launches = 0;
 };
@@ -1169,32 +1155,19 @@ extern "C" int b200mppi_planner_set_obstacles(b200mppi_planner* p, const float* 
 
 // Cells the rollouts of this solve can read.  A rollout moves at most |traction| * |v| * dt per step, so it stays
 // within R = dt * max|traction| * S of x0, S = sum_t |v_t| -- bounded by T * max|vrange| (static box) or, when the maps
-// are sampled once for ONE set of controls (num_opt = 1), by the max over the N control sequences actually drawn
-// (reach_d, reduced by the prepare kernel: one 4-byte read-back + stream sync per solve buys the smaller box).
+// are sampled once for ONE set of controls (num_opt = 1), by `reach`: the max over the N control sequences actually
+// drawn (reach_d, reduced by the prepare kernel and read back by stage_sample_tdms; null: the static bound).
 // False (whole maps) whenever the bound is not airtight: the box would leave the map (out-of-map indices wrap),
 // traction bytes not under the sampler's control, non-finite inputs.
-static bool planner_reach_box(b200mppi_planner* p, SampleBox* box, int* how, int* err) {
-  *err = B200MPPI_OK;
+static bool planner_reach_box(const b200mppi_planner* p, const float* reach, SampleBox* box, int* how) {
   *how = 1;
-  if (p->lin) p->lin->advance_done = false;                // (set below, only for the sampling call that follows)
   if (p->box_mode == 0 || !planner_uses_window(p)) return false;
   const b200mppi_tdm* l = p->lin;
   const b200mppi_params& q = p->prm;
   double S = (double)p->T * std::fmax(std::fabs((double)q.vrange[0]), std::fabs((double)q.vrange[1]));
-  if (p->box_mode == 2 && q.num_opt == 1 && p->prepared && p->reach_valid) {
-    float* h = p->h_u + (size_t)p->T * 2 + 2;
-    // the host waits for the 4 bytes only (an event, not the stream): the state advance queued behind the copy runs
-    // while the host wakes up, sizes the box and launches the sampler
-    const double alpha = p->cfg.mode == B200MPPI_MODE_TDM ? q.alpha_dyn : 1.0;
-    bool ok = cudaMemcpyAsync(h, p->reach_d + p->reach_slot, sizeof(float), cudaMemcpyDeviceToHost, p->stream) == cudaSuccess &&
-              cudaEventRecord(p->ev_reach, p->stream) == cudaSuccess;
-    if (ok) tdm_pair_advance_early(p->lin, p->ang, alpha, p->stream, &p->launches);
-    if (!ok || cudaEventSynchronize(p->ev_reach) != cudaSuccess) {
-      *err = fail(B200MPPI_ECUDA, std::string("reach read-back: ") + cudaGetErrorString(cudaGetLastError()));
-      return false;
-    }
-    if (!((double)*h <= S)) return false;              // NaN or beyond the speed limit: not a usable bound
-    S = (double)*h;
+  if (reach) {
+    if (!((double)*reach <= S)) return false;          // NaN or beyond the speed limit: not a usable bound
+    S = (double)*reach;
     *how = 2;
   }
   // 1.0002: cos/sin.approx may exceed 1 by ~1e-6, float32 rounding of the state adds ~1e-7 per step; + one cell below
@@ -1218,13 +1191,33 @@ static int stage_sample_tdms(b200mppi_planner* p) {
   if (p->cfg.mode == B200MPPI_MODE_BAREBONE) return B200MPPI_OK;      // no maps
   // det / speed-map solves call sample_grids() with the default alpha_dyn = 1.0 (mppi.py:248-249,322-323)
   const double alpha = p->cfg.mode == B200MPPI_MODE_TDM ? p->prm.alpha_dyn : 1.0;
-  SampleBox box;
-  int err;
+  SamplePlan plan;
+  int rc = plan_sampling(p->lin, p->ang, alpha, p->stream, &plan);
+  if (rc) return rc;
+  // a box from this solve's own controls: the host waits for their 4-byte reach statistic only (an event, not the
+  // stream).  A fused pair's state advance does not depend on the box: queued behind the copy, it runs while the host
+  // wakes up, sizes the box and launches the sampler.  Should the sampling take whole maps after all, that launch
+  // stores the very same states again.
+  const float* reach = nullptr;
+  bool advanced = false;
+  if (p->box_mode == 2 && p->prm.num_opt == 1 && p->prepared && p->reach_valid && planner_uses_window(p)) {
+    float* h = p->h_u + (size_t)p->T * 2 + 2;
+    CU(cudaMemcpyAsync(h, p->reach_d + p->reach_slot, sizeof(float), cudaMemcpyDeviceToHost, p->stream));
+    CU(cudaEventRecord(p->ev_reach, p->stream));
+    if (plan.fused) {
+      launch_plan_advance(plan, 0, p->stream);
+      CHECK_LAUNCH();
+      p->launches++;
+      advanced = true;
+    }
+    CU(cudaEventSynchronize(p->ev_reach));
+    reach = h;
+  }
+  SampleBox box{};
   int how = 0;
-  const bool boxed = planner_reach_box(p, &box, &how, &err);
-  if (err) return err;
-  const int rc = tdm_sample_pair_on(p->lin, p->ang, alpha, p->stream, &p->launches, boxed ? &box : nullptr);
-  const bool used = boxed && p->lin->grid_partial;        // the sampler may still have fallen back to whole maps
+  if (planner_reach_box(p, reach, &box, &how)) plan_box(&plan, box);
+  rc = plan_launch(plan, advanced, p->stream, &p->launches);
+  const bool used = plan.boxed[0];                        // the box may not fit the sampler's launch: whole maps
   p->last_box[0] = used ? how : 0;
   p->last_box[1] = used ? box.row_lo : 0; p->last_box[2] = used ? box.row_hi : p->lin->rows;
   p->last_box[3] = used ? box.col_lo : 0; p->last_box[4] = used ? box.col_hi : p->lin->cols;
@@ -1724,7 +1717,7 @@ extern "C" int b200mppi_planner_sample_box(b200mppi_planner* p, int32_t out[5]) 
 
 extern "C" int b200mppi_planner_launch_count(b200mppi_planner* p, int64_t* out) {
   if (!p || !out) return fail(B200MPPI_EINVAL, "null argument");
-  *out = p->launches + (p->lin ? 0 : 0);
+  *out = p->launches;
   return B200MPPI_OK;
 }
 
@@ -1867,51 +1860,45 @@ static int batch_validate(b200mppi_batch* b) {
   return B200MPPI_OK;
 }
 
-// The maps of every planner, as its solve() samples them: the pairs its solve() would sample with the fused whole-map
-// launch and whose launch geometry equals the first such pair's go into ONE launch; every other pair takes its own
-// path (tdm_sample_pair_on), in planner order.  One-map modes never sample a reach box.
-// Planning (host tables, the fused pairs' descriptors) comes before the solve's one upload, the launches after the noise.
+// The maps of every planner, as its solve() samples them: the pairs whose plan is fused and whose launch equals the
+// first such pair's go into ONE launch; every other pair runs its own plan, in planner order.  One-map modes never
+// sample a reach box.
+// Planning (host tables, the batched pairs' descriptors) comes before the solve's one upload, the launches after the noise.
 constexpr double BATCH_ALPHA = 1.0;   // det / speed-map solves sample with the default alpha_dyn (stage_sample_tdms)
 
-static int batch_plan_sample(b200mppi_batch* b, SampleGridsV2Args* h_sg, std::vector<char>& fused, int* nfused) {
-  const double alpha = BATCH_ALPHA;
-  cudaStream_t st = b->stream;
+static int batch_plan_sample(b200mppi_batch* b, SampleGridsV2Args* h_sg, std::vector<SamplePlan>& plans,
+                             std::vector<char>& joined, int* njoined) {
   const int K = (int)b->pl.size();
-  fused.assign(K, 0);
-  int nf = 0, rc;
+  plans.resize(K);
+  joined.assign(K, 0);
+  int nj = 0;
   for (int i = 0; i < K; ++i) {
-    b200mppi_planner* p = b->pl[i];
-    b200mppi_tdm* l = p->lin; b200mppi_tdm* g = p->ang;
-    l->advance_done = false;
-    if ((rc = tdm_prepare_thresholds(l, alpha, st)) || (rc = tdm_prepare_thresholds(g, alpha, st))) return rc;
-    if ((rc = tdm_prepare_jump(l, st))) return rc;
-    SampleGridsV2Args v2{};
-    fill_v2(l, v2, 0);
-    fill_v2(g, v2, 1);
-    if (!(tdm_same_stream(l, g) && l->thr_ok && g->thr_ok && sample_grids_v2_fits(v2, 2))) continue;
-    if (nf > 0 && !sample_grids_v2_same_launch(h_sg[0], v2)) continue;
-    h_sg[nf++] = v2;
-    fused[i] = 1;
+    const int rc = plan_sampling(b->pl[i]->lin, b->pl[i]->ang, BATCH_ALPHA, b->stream, &plans[i]);
+    if (rc) return rc;
+    if (!plans[i].fused || (nj > 0 && !sample_grids_v2_same_launch(h_sg[0], plans[i].a[0]))) continue;
+    h_sg[nj++] = plans[i].a[0];
+    joined[i] = 1;
   }
-  *nfused = nf;
+  *njoined = nj;
   return B200MPPI_OK;
 }
 
 static int batch_run_sample(b200mppi_batch* b, const SampleGridsV2Args* h_sg, const SampleGridsV2Args* d_sg,
-                            const std::vector<char>& fused, int nf) {
-  const double alpha = BATCH_ALPHA;
-  cudaStream_t st = b->stream;
-  const int K = (int)b->pl.size();
-  int rc;
-  if (nf > 0) {
-    launch_sample_grids_v2_batch(h_sg[0], d_sg, nf, st);
+                            std::vector<SamplePlan>& plans, const std::vector<char>& joined, int nj) {
+  if (nj > 0) {
+    launch_sample_grids_v2_batch(h_sg[0], d_sg, nj, b->stream);
     b->launches++;
     CHECK_LAUNCH();
   }
-  for (int i = 0; i < K; ++i) {
+  for (size_t i = 0; i < plans.size(); ++i) {
     b200mppi_planner* p = b->pl[i];
-    if (fused[i]) tdm_pair_sampled_whole(p->lin, p->ang, alpha);
-    else if ((rc = tdm_sample_pair_on(p->lin, p->ang, alpha, st, &b->launches, nullptr))) return rc;
+    if (joined[i]) {
+      plan_commit(plans[i], 0);
+      plan_commit(plans[i], 1);
+    } else {
+      const int rc = plan_launch(plans[i], false, b->stream, &b->launches);
+      if (rc) return rc;
+    }
     p->last_box[0] = 0; p->last_box[1] = 0; p->last_box[2] = p->lin->rows; p->last_box[3] = 0; p->last_box[4] = p->lin->cols;
   }
   return B200MPPI_OK;
@@ -1955,13 +1942,14 @@ extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
   const RolloutArgs* dr = reinterpret_cast<const RolloutArgs*>(b->d_desc + b->off_roll);
   const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(b->d_desc + b->off_upd);
   const bool maps = b->mode != B200MPPI_MODE_BAREBONE;
-  std::vector<char> fused;
-  int nf = 0;
-  if (maps && (rc = batch_plan_sample(b, hs, fused, &nf))) return rc;
+  std::vector<SamplePlan> plans;
+  std::vector<char> joined;
+  int nj = 0;
+  if (maps && (rc = batch_plan_sample(b, hs, plans, joined, &nj))) return rc;
   CU(cudaMemcpyAsync(b->d_desc, b->h_desc, b->desc_bytes, cudaMemcpyHostToDevice, st));
   const int num_opt = b->pl[0]->prm.num_opt;
   if (num_opt <= 0) {                                  // the reference samples before its (empty) loop; u unchanged
-    if (maps && (rc = batch_run_sample(b, hs, ds, fused, nf))) return rc;
+    if (maps && (rc = batch_run_sample(b, hs, ds, plans, joined, nj))) return rc;
     for (int i = 0; i < K; ++i)
       CU(cudaMemcpyAsync(b->u_d + (size_t)i * T * 2, b->pl[i]->u_cur, (size_t)T * 2 * sizeof(float),
                          cudaMemcpyDeviceToDevice, st));
@@ -1972,7 +1960,7 @@ extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
     b->launches++;
     CHECK_LAUNCH();
     for (b200mppi_planner* p : b->pl) p->prepared = false;
-    if (k == 0 && maps && (rc = batch_run_sample(b, hs, ds, fused, nf))) return rc;
+    if (k == 0 && maps && (rc = batch_run_sample(b, hs, ds, plans, joined, nj))) return rc;
     launch_rollout_batch(dr, K, b->mode, b->N, T, st);
     b->launches++;
     CHECK_LAUNCH();

@@ -79,7 +79,7 @@ static void run(const SampleGridsV2Args& a, int threads, unsigned gx, unsigned g
 // cum: (nt)(rows, cols, bpad) int8 running sums; grids: (nt)(M, grid_rows, pitch); qvals: (nt)(128).
 // disc = {cx, cy, r} (cells) or null: the reach disc inside the box (per-CTA narrowing of the tile columns).
 // box = {row_lo, row_hi, col_lo, col_hi} (cells) or null: with a box the launch is restricted as apply_box (api.cu)
-// does it and the states come from advance_states_kernel -- what tdm_sample_pair_on does for a boxed solve.
+// does it and the states come from advance_states_kernel -- what plan_launch does for a boxed solve.
 extern "C" int emu_sample_v2(int nt, int8_t* grid0, int8_t* grid1, const int8_t* cum0, const int8_t* cum1,
                              const uint64_t* states, uint64_t* states_out, const int8_t* qv0, const int8_t* qv1, int bpad,
                              int rows, int cols, int grid_rows, int pitch, int tx, int ty, int num_maps, int segs,

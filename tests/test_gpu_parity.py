@@ -984,29 +984,40 @@ def _tdm_planner(eng, sc, monkeypatch, box):
     return cfg, lin, ang, pl
 
 
-@pytest.mark.parametrize("N,M,T,H,res,warm,tdim", [
-    (1024, 64, 64, 512, 0.1, False, (16, 16)),     # BASELINE config 3
-    (512, 40, 64, 420, 0.1, True, (7, 5)),         # ragged tiles, warm start (longer reach), 40 maps: partial map groups
-    (256, 16, 16, 200, 0.05, True, (4, 12)),       # the speed-limit box (4.8 m) leaves the 10 m map, the actual reach does not
+@pytest.mark.parametrize("N,M,T,H,res,warm,tdim,diverge", [
+    # BASELINE config 3
+    pytest.param(1024, 64, 64, 512, 0.1, False, (16, 16), False, id="1024-64-64-512-0.1-False-tdim0"),
+    # ragged tiles, warm start (longer reach), 40 maps: partial map groups
+    pytest.param(512, 40, 64, 420, 0.1, True, (7, 5), False, id="512-40-64-420-0.1-True-tdim1"),
+    # the speed-limit box (4.8 m) leaves the 10 m map, the actual reach does not
+    pytest.param(256, 16, 16, 200, 0.05, True, (4, 12), False, id="256-16-16-200-0.05-True-tdim2"),
+    # lin's stream ahead of ang's: each TDM sampled (and boxed) on its own
+    pytest.param(512, 40, 64, 420, 0.1, True, (7, 5), True, id="512-40-64-420-0.1-True-tdim1-diverged"),
 ])
-def test_boxed_solve_identical_to_whole_map_solve(eng, monkeypatch, N, M, T, H, res, warm, tdim):
+def test_boxed_solve_identical_to_whole_map_solve(eng, monkeypatch, N, M, T, H, res, warm, tdim, diverge):
     """solve() samples only the cells its rollouts can reach (include/b200mppi.h, b200mppi_planner_sample_box).
     Against whole-map sampling (what the reference does, terrain.py:610-694) over a closed loop with a moving
     robot: u, CVaR costs, per-(n,m) costs, noise and EVERY generator state bit-identical; afterwards the sampled
-    maps read through the public handle are the whole maps of that sampling call (completed on demand)."""
+    maps read through the public handle are the whole maps of that sampling call (completed on demand).
+    With `diverge`, one public lin.sample_grids() before the loop leaves the two TDMs in different generator states,
+    so the maps are not sampled from one stream but one TDM at a time."""
     sc = make_scenario("tdm", N=N, M=M, T=T, H=H, W=H, res=res, B=12, seed=11, warm_start=warm, thread_dim=tdim)
     runs = {}
     for box in ("off", "static", "dynamic"):
         cfg, lin, ang, pl = _tdm_planner(eng, sc, monkeypatch, box)
+        if diverge:
+            lin.sample_grids(sc["params"]["alpha_dyn"])
         x0 = sc["params"]["x0"].copy()
-        hist, modes = [], []
+        hist, modes, launches = [], [], []
         for k in range(4):
+            l0 = pl.launch_count()
             u = pl.solve()
+            launches.append(pl.launch_count() - l0)
             modes.append(pl.sample_box())
             hist.append((u.copy(), pl.costs_d.copy_to_host(), pl.costs_nm_d.copy_to_host()))
             x0 = x0 + np.array([0.37, -0.21, 0.05])
             pl.shift_and_update(x0, u, 1)
-        runs[box] = dict(hist=hist, modes=modes, lin_rng=lin.rng_states_d.copy_to_host(),
+        runs[box] = dict(hist=hist, modes=modes, launches=launches, lin_rng=lin.rng_states_d.copy_to_host(),
                          ang_rng=ang.rng_states_d.copy_to_host(), rng=pl.rng_states_d.copy_to_host(),
                          noise=pl.noise_samples_d.copy_to_host(), lin_grid=lin.sample_grid_batch_d.copy_to_host(),
                          ang_grid=ang.sample_grid_batch_d.copy_to_host())
@@ -1021,6 +1032,14 @@ def test_boxed_solve_identical_to_whole_map_solve(eng, monkeypatch, N, M, T, H, 
     assert runs["static"]["modes"][0][0] == (1 if static_fits else 0), runs["static"]["modes"]
     assert all(m[0] in (0, 1) for m in runs["static"]["modes"])
     assert all(m[0] == 2 for m in runs["dynamic"]["modes"]), runs["dynamic"]["modes"]
+    # launches per solve: noise + controls, rollout, CVaR, update, and the sampler -- one launch for both maps when the
+    # TDMs share a stream, one per TDM otherwise -- each followed, when boxed, by its generator-state advance
+    samplers = 2 if diverge else 1
+    for box in ("off", "static", "dynamic"):
+        r = runs[box]
+        assert r["launches"] == [4 + samplers * (2 if m[0] else 1) for m in r["modes"]], (box, r["launches"])
+    if not diverge:
+        assert runs["dynamic"]["launches"] == [6] * 4                 # README: a stochastic solve is 6 launches
     Hp = H + 2 * int(np.ceil(5.0 * 0.1 / res))
     for box in ("static", "dynamic"):
         r = runs[box]
