@@ -1,0 +1,166 @@
+#!/usr/bin/env python
+"""bench_trials.py -- closed-loop episodes of K one-map planners: the host-driven loop against MPPI_Batch.run_trials.
+
+    python bench_trials.py --workload c2|c4 --batch K --closed-loop S [--rounds R]
+
+K planners of the workload (bench.py's WORKLOADS, seeds 1..K: different maps, start poses and warm starts), each with
+a seeded ground-truth TractionGrid over its map; every other planner has its goal 1.5 m away (reached within S steps),
+the others the workload's distant goal (they run all S steps).  First the parity check: run_trials on one set of
+planners, and on identical twins the host loop replayed with the device's trajectory -- u[0] of every solve and the
+final planner state (u, u_prev, noise, costs, weights, RNG states, sampled maps, params['x0']) bit for bit; a mismatch
+exits non-zero.  Then R rounds of each, alternating, every round from the same start (params, warm start):
+  host: the best host loop available -- MPPI_Batch.solve() of all K, then per running planner a numpy plant step and
+        shift_and_update, until every planner has stopped;
+  device: one MPPI_Batch.run_trials(grids, S).
+Wall clock per round (each ends in a host synchronisation); control steps/s (planner-steps run), episodes/s, kernel
+launches per round.  Prints one JSON line with the card's name and power limit; writes nothing to the tree.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+from bench import WORKLOADS, make_planner, workload_name_of   # noqa: E402
+
+
+def run(args, emit):
+    import torch
+    import __graft_entry__
+    __graft_entry__.build_engine()
+    import mppi_numba_b200 as E
+    from tests.scenarios import make_scenario
+    from tests.trial_loop import plant_step, within
+    K, S = args.batch, args.closed_loop
+    mode, N, M, T, H, res, B, da = WORKLOADS[args.workload]
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    scs = []
+    for k in range(K):
+        sc = make_scenario(mode, N=N, M=M, T=T, H=H, W=H, res=res, B=B, seed=k + 1, det_alpha=da, warm_start=True)
+        if k % 2 == 0:
+            sc["params"]["xgoal"] = sc["params"]["x0"][:2] + np.array([1.2, -0.9])
+        scs.append(sc)
+    rng = np.random.default_rng(7)
+    grids = [E.TractionGrid(rng.uniform(0.3, 1.0, (H, H)), rng.uniform(0.3, 1.0, (H, H)), res=res) for _ in range(K)]
+    A, Bs = [[make_planner(E, sc, 0)[3] for sc in scs] for _ in range(2)]
+
+    def reset(pls):
+        for p, sc in zip(pls, scs):
+            p.params["x0"] = sc["params"]["x0"].copy()
+            p.u_cur_d.copy_to_device(sc["u0"])
+
+    reset(A), reset(Bs)
+    ba, bb = E.MPPI_Batch(A), E.MPPI_Batch(Bs)
+
+    # ---- parity: run_trials == the host loop replayed with the device's trajectory
+    out = ba.run_trials(grids, S)
+    ok_u = True
+    for k, p in enumerate(Bs):
+        for t in range(int(out["steps"][k])):
+            useq = p.solve()
+            ok_u &= bool(np.array_equal(useq[0], out["uhist"][k, t]))
+            p.shift_and_update(out["xhist"][k, t + 1], useq, 1)
+
+    def state(p):
+        d = [p.u_cur_d, p.u_prev_d, p.costs_d, p.weights_d, p.noise_samples_d, p.rng_states_d, p.lin_tdm.rng_states_d,
+             p.ang_tdm.rng_states_d, p.lin_tdm.sample_grid_batch_d, p.ang_tdm.sample_grid_batch_d]
+        return [a.copy_to_host() for a in d] + [p.params["x0"]]
+    ok_state = all(all(np.array_equal(x, y) for x, y in zip(state(a), state(b))) for a, b in zip(A, Bs))
+    parity = {"passed": ok_u and ok_state, "u_bitwise": ok_u, "state_bitwise": ok_state, "planners": K,
+              "steps": out["steps"].tolist(), "status": out["status"],
+              "against": "the host loop replayed with the device's trajectory on identical twins"}
+    if not parity["passed"]:
+        sys.stderr.write("bench_trials.py: PARITY CHECK FAILED: %s\n" % json.dumps(parity))
+        emit(json.dumps({"metric": "closed-loop trials", "error": "parity_check failed", "parity_check": parity}))
+        raise SystemExit(3)
+
+    def host_round():
+        reset(Bs)
+        x = [np.asarray(p.params["x0"], dtype=np.float64) for p in Bs]
+        running, steps = list(range(K)), 0
+        for t in range(S):
+            u = bb.solve()
+            still = []
+            for k in running:
+                p = Bs[k]
+                xn = plant_step(grids[k], x[k], u[k, 0], float(p.params["dt"]))
+                p.shift_and_update(xn, u[k], 1)
+                x[k] = xn
+                steps += 1
+                d = np.linalg.norm(xn[:2] - p.params["xgoal"]) - p.params["goal_tolerance"]
+                if d > 0 and within(p, xn):
+                    still.append(k)
+            running = still
+            if not running:
+                break
+        torch.cuda.synchronize(dev)
+        return steps
+
+    def device_round():
+        reset(A)
+        o = ba.run_trials(grids, S)
+        torch.cuda.synchronize(dev)
+        return int(o["steps"].sum())
+
+    host_round(), device_round()                          # warm-up of both paths
+    res = {"host": [], "device": []}
+    launches = {}
+    for _ in range(args.rounds):
+        for name, fn, b in (("host", host_round, bb), ("device", device_round, ba)):
+            l0 = b.launch_count()
+            t0 = time.perf_counter()
+            steps = fn()
+            res[name].append((time.perf_counter() - t0, steps))
+            launches[name] = b.launch_count() - l0
+
+    def summary(name):
+        wall = [r[0] for r in res[name]]
+        med = float(np.median(wall))
+        return {"s_per_round_wall": med, "s_per_round_wall_runs": wall, "control_steps_per_round": res[name][0][1],
+                "control_steps_per_s": res[name][0][1] / med, "episodes_per_s": K / med,
+                "kernel_launches_per_round": launches[name]}
+    host, devr = summary("host"), summary("device")
+    gpu = {"name": torch.cuda.get_device_name(dev)}
+    try:
+        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+        gpu["power_limit_and_max_sm_clock"] = q
+    except Exception as e:                               # noqa: BLE001
+        gpu["power_limit_and_max_sm_clock"] = "unavailable (%r)" % e
+    emit(json.dumps({"metric": "closed-loop trials: host-driven loop vs MPPI_Batch.run_trials",
+                     "unit": "episodes/s", "value": devr["episodes_per_s"], "higher_is_better": True,
+                     "config": {"workload": workload_name_of(args.workload), "batch": K, "max_steps": S,
+                                "planners": "seeds 1..K, warm started; even k: goal 1.5 m away, odd k: distant goal"},
+                     "rounds": args.rounds, "gpu": gpu, "parity_check": parity, "host": host, "device": devr,
+                     "speedup_wall": host["s_per_round_wall"] / devr["s_per_round_wall"]}))
+
+
+def main():
+    # one JSON line on stdout: everything else (the engine's allocation notices, ...) goes to stderr
+    real_stdout = os.dup(1)
+    os.dup2(2, 1)
+    sys.stdout = os.fdopen(os.dup(2), "w", buffering=1)
+
+    def emit(line):
+        os.write(real_stdout, (line + "\n").encode())
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[1])
+    ap.add_argument("--workload", default="c2", choices=["c2", "c4"])
+    ap.add_argument("--batch", type=int, default=64, metavar="K", help="planners in the batch")
+    ap.add_argument("--closed-loop", type=int, default=150, metavar="S", help="max control steps per episode")
+    ap.add_argument("--rounds", type=int, default=3, help="timed rounds of each loop")
+    args = ap.parse_args()
+    if args.batch < 1 or args.closed_loop < 1 or args.rounds < 1:
+        ap.error("--batch, --closed-loop and --rounds must be at least 1")
+    run(args, emit)
+
+
+if __name__ == "__main__":
+    main()

@@ -324,6 +324,45 @@ int b200mppi_batch_set_stream(b200mppi_batch* b, void* cuda_stream);
 int b200mppi_batch_solve(b200mppi_batch* b, float* u_out);
 int b200mppi_batch_launch_count(b200mppi_batch* b, int64_t* out);
 
+/* ------------------------------------------------------------------ closed-loop trials of a batch
+ * Every planner of a MODE_DET_DYN or MODE_SPEED_MAP batch drives a unicycle through one receding-horizon episode on
+ * its own ground-truth traction grid, entirely on the device: per step ONE launch each of noise, map sampling, rollout
+ * and update for the whole batch (num_opt = 1; num_opt > 1 repeats noise, rollout and update), then the plant step.
+ * The plant step is the benchmark loop's: u = u_cur[0]; (lt, at) = grid value of the cell holding (x, y), (0, 0)
+ * outside the grid; x += dt*lt*cos(theta)*v, y += dt*lt*sin(theta)*v, theta += dt*at*w in float64; u_cur shifted by
+ * one (the last row kept); d = |(x, y) - xgoal| - goal_tolerance, cum_obj += dt + d, cum_dist_to_goal += d.  A planner
+ * stops once d <= 0 (GOAL), once its pose leaves the padded map limits (LEFT_MAP: its next solve would be refused) or
+ * after max_steps steps (MAX_STEPS).  Stopped planners' CTAs return at once; the host polls the count of running
+ * planners every few steps and issues nothing more once it is zero.
+ * Afterwards every planner, its TDMs (RNG states, sampled maps) and its params are exactly as `steps` rounds of
+ * solve() -> plant step -> set_u(shifted u) -> set_params(x0 = float32(new pose)) would leave them, except that the
+ * C-side params keep the x0 of the last solve (as in that loop, where the new pose is uploaded by the next solve).
+ * Refused (B200MPPI_EINVAL naming the planner) before any work is issued: what batch_solve refuses, MODE_BAREBONE,
+ * max_steps < 1, num_opt < 1, a grid or limit that is not usable, a start pose outside the padded limits, and a batch
+ * whose TDM pairs cannot all be sampled by the one batched sampler launch.
+ *   trials  : count descriptors, in planner order; the grids are uploaded and freed by the call.
+ *   xhist   : float64 (count, max_steps+1, 3), NaN after a planner's last step;  uhist: float32 (count, max_steps, 2),
+ *             NaN after it;  results: count records;  steps_issued (may be NULL): steps the batch issued. */
+enum { B200MPPI_TRIAL_GOAL = 1, B200MPPI_TRIAL_MAX_STEPS = 2, B200MPPI_TRIAL_LEFT_MAP = 3 };
+typedef struct {
+  const double* lin;            /* ground-truth linear traction, (height, width) row-major, host */
+  const double* ang;            /* ground-truth angular traction, same shape */
+  int32_t height, width;
+  double xlo, ylo, res;         /* the grid's xlimits[0], ylimits[0] and cell size: cell = floor((x - xlo) / res) */
+  double x0[3];                 /* start pose */
+  double xgoal[2];
+  double goal_tolerance, v_post_rollout, dt;
+  double pxlim[2], pylim[2];    /* the planner's padded map limits */
+} b200mppi_trial_desc;
+typedef struct {
+  double cum_obj;               /* sum over steps of dt + d (the caller adds the benchmark's d / v_post_rollout tail) */
+  double cum_dist_to_goal;      /* sum over steps of d */
+  double dist_to_goal;          /* d of the last step */
+  int32_t steps, status;        /* steps run, B200MPPI_TRIAL_* */
+} b200mppi_trial_result;
+int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps, double* xhist,
+                              float* uhist, b200mppi_trial_result* results, int32_t* steps_issued);
+
 #ifdef __cplusplus
 }
 #endif

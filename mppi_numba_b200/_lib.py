@@ -41,6 +41,23 @@ class ParamsPOD(C.Structure):
                 ("dist_weight", C.c_float), ("num_opt", C.c_int32), ("alpha_dyn", C.c_double)]
 
 
+class TrialDesc(C.Structure):
+    """b200mppi_trial_desc: one planner's closed-loop trial (ground-truth grid, start, goal, padded limits)."""
+    _fields_ = [("lin", C.c_void_p), ("ang", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32),
+                ("xlo", C.c_double), ("ylo", C.c_double), ("res", C.c_double), ("x0", C.c_double * 3),
+                ("xgoal", C.c_double * 2), ("goal_tolerance", C.c_double), ("v_post_rollout", C.c_double),
+                ("dt", C.c_double), ("pxlim", C.c_double * 2), ("pylim", C.c_double * 2)]
+
+
+class TrialResult(C.Structure):
+    """b200mppi_trial_result"""
+    _fields_ = [("cum_obj", C.c_double), ("cum_dist_to_goal", C.c_double), ("dist_to_goal", C.c_double),
+                ("steps", C.c_int32), ("status", C.c_int32)]
+
+
+TRIAL_GOAL, TRIAL_MAX_STEPS, TRIAL_LEFT_MAP = 1, 2, 3
+
+
 def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
@@ -109,6 +126,8 @@ def _load():
         "b200mppi_batch_set_stream": (C.c_int, [P, P]),
         "b200mppi_batch_solve": (C.c_int, [P, P]),
         "b200mppi_batch_launch_count": (C.c_int, [P, C.POINTER(I64)]),
+        "b200mppi_batch_run_trials": (C.c_int, [P, C.POINTER(TrialDesc), I32, P, P, C.POINTER(TrialResult),
+                                                C.POINTER(I32)]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)          # AttributeError here == ABI drift, fail loudly

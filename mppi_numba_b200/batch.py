@@ -10,12 +10,19 @@
 Each planner keeps its own params, TDMs, warm start and RNG streams; ``solve()`` leaves every one of them exactly as
 ``planner.solve()`` called on planners[0], planners[1], ... in that order would (include/b200mppi.h, batched one-map
 solves).  The planners must share N, T, the device and the mode; their TDMs must not be shared between planners.
+
+``run_trials(traction_grids, max_steps)`` runs the benchmark's closed-loop episode (solve, plant step on a ground-truth
+``TractionGrid``, shift_and_update, stop at the goal) for every det-dynamics or speed-map planner at once on the GPU,
+without a host round trip per step (include/b200mppi.h, closed-loop trials).
 """
 import ctypes as C
 
 import numpy as np
 
+from . import _lib
 from ._lib import check, lib, ptr
+
+TRIAL_STATUS = {_lib.TRIAL_GOAL: "goal", _lib.TRIAL_MAX_STEPS: "max_steps", _lib.TRIAL_LEFT_MAP: "left_map"}
 
 
 def _kind(p):
@@ -95,3 +102,85 @@ class MPPI_Batch(object):
         check(lib.b200mppi_batch_launch_count(self._handle, C.byref(n)))
         return int(n.value)
 
+
+    def run_trials(self, traction_grids, max_steps, dt=None):
+        """One closed-loop episode per planner, on the GPU: up to ``max_steps`` rounds of ``u = solve()``, a plant step
+        on ``traction_grids[k]`` (a ``TractionGrid``, float or ``use_int8``) with ``u[0]`` and ``shift_and_update``,
+        stopping once the planner is within ``goal_tolerance`` of its goal -- the loop of the benchmark's ``trial()``,
+        whose ``dt`` argument (default: each planner's ``params['dt']``) is used as a float64.  A planner also stops when
+        its pose leaves the padded map limits, where its next ``solve()`` would be refused.
+
+        Afterwards every planner (controls, noise, costs, weights, RNG streams, its TDMs' streams and sampled maps, and
+        ``params['x0']``) is exactly as after that host loop.  Returns a dict:
+          ``logs``: per planner, the trial log of ``trial()`` (time_to_goal, success, dist_to_goal, cum_dist_to_goal,
+                    avg_dist_to_goal, cum_obj) with its NaN conventions; a planner that left the map is logged as one
+                    that did not reach its goal;
+          ``xhist`` float64 (K, max_steps+1, 3) and ``uhist`` float32 (K, max_steps, 2), NaN after a planner's last
+          step; ``steps`` (K,) int; ``status`` (K,) of "goal" | "max_steps" | "left_map".
+        Raises ValueError (naming the planner) for barebone batches, a grid count other than K, max_steps < 1,
+        num_opt < 1, a grid of another dtype than float64 or integer, or a planner that cannot solve (e.g. its start
+        pose is outside the padded map limits); B200MPPIError when the planners' maps cannot all be sampled by the
+        batch's one sampler launch.  Nothing is issued when the call is refused."""
+        K = len(self.planners)
+        if self.kind not in ("det", "spd"):
+            raise ValueError("MPPI_Batch.run_trials: planner 0 is a %s planner (trials need det-dynamics or speed-map "
+                             "planners)" % self.kind)
+        grids = list(traction_grids)
+        if len(grids) != K:
+            raise ValueError("MPPI_Batch.run_trials: %d traction grids for %d planners" % (len(grids), K))
+        max_steps = int(max_steps)
+        if max_steps < 1:
+            raise ValueError("MPPI_Batch.run_trials: max_steps %d < 1" % max_steps)
+        descs = (_lib.TrialDesc * K)()
+        keep = []
+        for i, (p, g) in enumerate(zip(self.planners, grids)):
+            if not p.check_solve_conditions():
+                raise ValueError("MPPI_Batch.run_trials: planner %d cannot solve (reason printed above)" % i)
+            if int(p.params["num_opt"]) < 1:
+                raise ValueError("MPPI_Batch.run_trials: planner %d has num_opt %d < 1" % (i, int(p.params["num_opt"])))
+            lin, ang = np.asarray(g.lin_traction), np.asarray(g.ang_traction)
+            for a in (lin, ang):
+                if a.dtype != np.float64 and not np.issubdtype(a.dtype, np.integer):
+                    raise ValueError("MPPI_Batch.run_trials: planner %d: traction grid of dtype %s (float64 or integer "
+                                     "grids only: the plant step is float64)" % (i, a.dtype))
+            if lin.ndim != 2 or lin.shape != ang.shape:
+                raise ValueError("MPPI_Batch.run_trials: planner %d: lin / ang traction grids of shapes %s / %s"
+                                 % (i, lin.shape, ang.shape))
+            lin = np.ascontiguousarray(lin, dtype=np.float64)
+            ang = np.ascontiguousarray(ang, dtype=np.float64)
+            keep += [lin, ang]
+            d, q = descs[i], p.params
+            d.lin, d.ang = lin.ctypes.data, ang.ctypes.data
+            d.height, d.width = lin.shape
+            d.xlo, d.ylo, d.res = float(g.xlimits[0]), float(g.ylimits[0]), float(g.res)
+            d.x0[:] = [float(v) for v in np.asarray(q["x0"], dtype=np.float64)[:3]]
+            d.xgoal[:] = [float(v) for v in np.asarray(q["xgoal"], dtype=np.float64)[:2]]
+            d.goal_tolerance, d.v_post_rollout = float(q["goal_tolerance"]), float(q["v_post_rollout"])
+            d.dt = float(q["dt"] if dt is None else dt)
+            d.pxlim[:] = [float(v) for v in p.lin_tdm.padded_xlimits]
+            d.pylim[:] = [float(v) for v in p.lin_tdm.padded_ylimits]
+        for p in self.planners:
+            p.move_mppi_task_vars_to_device()
+        xhist = np.empty((K, max_steps + 1, 3), dtype=np.float64)
+        uhist = np.empty((K, max_steps, 2), dtype=np.float32)
+        res = (_lib.TrialResult * K)()
+        issued = C.c_int32()
+        check(lib.b200mppi_batch_run_trials(self._handle, descs, max_steps, ptr(xhist), ptr(uhist), res,
+                                            C.byref(issued)))
+        self.steps_issued = int(issued.value)
+        steps = np.array([r.steps for r in res], dtype=np.int64)
+        status = [TRIAL_STATUS[r.status] for r in res]
+        logs = []
+        for i, p in enumerate(self.planners):
+            p.u_prev_d = p._u_prev_buf                 # as each planner's own solve() does (mppi.py:292,362)
+            p.params["x0"] = xhist[i, steps[i]].copy()  # shift_and_update(x_next, ...)
+            r, n, reached = res[i], int(steps[i]), status[i] == "goal"
+            cum_obj, dist = r.cum_obj, r.dist_to_goal
+            if reached:
+                dist = np.nan
+            else:
+                cum_obj += dist / descs[i].v_post_rollout
+            logs.append(dict(time_to_goal=n * descs[i].dt if reached else np.nan, success=reached, dist_to_goal=dist,
+                             cum_dist_to_goal=r.cum_dist_to_goal, avg_dist_to_goal=r.cum_dist_to_goal / n,
+                             cum_obj=cum_obj))
+        return dict(logs=logs, xhist=xhist, uhist=uhist, steps=steps, status=status)

@@ -1886,7 +1886,7 @@ static int batch_plan_sample(b200mppi_batch* b, SampleGridsV2Args* h_sg, std::ve
 static int batch_run_sample(b200mppi_batch* b, const SampleGridsV2Args* h_sg, const SampleGridsV2Args* d_sg,
                             std::vector<SamplePlan>& plans, const std::vector<char>& joined, int nj) {
   if (nj > 0) {
-    launch_sample_grids_v2_batch(h_sg[0], d_sg, nj, b->stream);
+    launch_sample_grids_v2_batch(h_sg[0], d_sg, nj, nullptr, b->stream);
     b->launches++;
     CHECK_LAUNCH();
   }
@@ -1956,16 +1956,16 @@ extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
   }
   // solve(): num_opt x (noise, [first iteration: maps], rollout, update)
   for (int k = 0; k < num_opt; ++k) {
-    launch_sample_noise_batch(dn, K, b->N, T, st);
+    launch_sample_noise_batch(dn, K, b->N, T, nullptr, st);
     b->launches++;
     CHECK_LAUNCH();
     for (b200mppi_planner* p : b->pl) p->prepared = false;
     if (k == 0 && maps && (rc = batch_run_sample(b, hs, ds, plans, joined, nj))) return rc;
-    launch_rollout_batch(dr, K, b->mode, b->N, T, st);
+    launch_rollout_batch(dr, K, b->mode, b->N, T, nullptr, st);
     b->launches++;
     CHECK_LAUNCH();
     for (b200mppi_planner* p : b->pl) p->pushed_direct = false;
-    launch_update_partial_batch(du, K, b->pl[0]->num_ctas, st);
+    launch_update_partial_batch(du, K, b->pl[0]->num_ctas, nullptr, st);
     b->launches++;
     CHECK_LAUNCH();
   }
@@ -1973,5 +1973,214 @@ extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
   // the host waits for the whole batch: work issued afterwards on any member's stream sees its results
   CU(cudaStreamSynchronize(st));
   if (u_out) std::memcpy(u_out, b->h_u, (size_t)K * T * 2 * sizeof(float));
+  return B200MPPI_OK;
+}
+
+// --------------------------------------------------------------------------------------------- closed-loop trials
+// A batch's planners run whole receding-horizon episodes on the device.  Only x0 (written by the plant kernel into the
+// rollout descriptors) and the parity of the TDMs' generator-state double buffers change from step to step: every
+// running planner has sampled its maps exactly s times before step s, so two sampler descriptor sets, one per parity,
+// serve all steps.  Stopped planners are gated out of every launch by `active`; the host polls the count of running
+// planners through pinned memory POLL steps behind the GPU and stops issuing once it reads zero.
+constexpr int TRIAL_POLL = 4;
+
+static int trial_validate(b200mppi_batch* b, const b200mppi_trial_desc* tr, int32_t max_steps) {
+  const int K = (int)b->pl.size();
+  if (!tr) return fail(B200MPPI_EINVAL, "run_trials: null trial descriptors");
+  if (max_steps < 1) return fail(B200MPPI_EINVAL, "run_trials: max_steps < 1");
+  if (b->mode == B200MPPI_MODE_BAREBONE)
+    return fail(B200MPPI_EINVAL, "run_trials: planner 0 is MODE_BAREBONE (trials need traction maps: MODE_DET_DYN or "
+                                 "MODE_SPEED_MAP batches)");
+  int rc = batch_validate(b);
+  if (rc) return rc;
+  for (int i = 0; i < K; ++i) {
+    const std::string who = "run_trials: planner " + std::to_string(i);
+    const b200mppi_trial_desc& d = tr[i];
+    if (b->pl[i]->prm.num_opt < 1) return fail(B200MPPI_EINVAL, who + " has num_opt < 1");
+    if (!d.lin || !d.ang || d.height < 1 || d.width < 1)
+      return fail(B200MPPI_EINVAL, who + ": empty or missing traction grid");
+    if (!(d.res > 0.0) || !std::isfinite(d.res) || !std::isfinite(d.xlo) || !std::isfinite(d.ylo) || !(d.dt > 0.0) ||
+        !std::isfinite(d.dt))
+      return fail(B200MPPI_EINVAL, who + ": grid res / limits or dt not finite and positive");
+    if (!(d.x0[0] >= d.pxlim[0] && d.x0[0] <= d.pxlim[1] && d.x0[1] >= d.pylim[0] && d.x0[1] <= d.pylim[1]) ||
+        !std::isfinite(d.x0[2]))
+      return fail(B200MPPI_EINVAL, who + ": start pose outside the padded map limits");
+  }
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps,
+                                         double* xhist, float* uhist, b200mppi_trial_result* results,
+                                         int32_t* steps_issued) {
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  int rc = trial_validate(b, trials, max_steps);
+  if (rc) return rc;
+  if (!xhist || !uhist || !results) return fail(B200MPPI_EINVAL, "run_trials: null output buffer");
+  CU(cudaSetDevice(b->device));
+  const int K = (int)b->pl.size(), T = b->T, S = max_steps;
+  cudaStream_t st = b->stream;
+  // the sampler plans first (their host preparation may synchronise the stream): every pair must join the one launch
+  std::vector<unsigned char> hd(b->desc_bytes + align256((size_t)K * sizeof(SampleGridsV2Args)));
+  SampleGridsV2Args* hs0 = reinterpret_cast<SampleGridsV2Args*>(hd.data() + b->off_sample);
+  std::vector<SamplePlan> plans;
+  std::vector<char> joined;
+  int nj = 0;
+  if ((rc = batch_plan_sample(b, hs0, plans, joined, &nj))) return rc;
+  for (int i = 0; i < K; ++i)
+    if (!joined[i])
+      return fail(B200MPPI_EINVAL, "run_trials: planner " + std::to_string(i) + ": its TDM pair cannot join the batch's "
+                                   "one sampler launch (map geometry, PMF or generator streams differ from planner 0's)");
+  for (b200mppi_planner* p : b->pl) {
+    if (p->stream == st) continue;
+    const cudaError_t q = cudaStreamQuery(p->stream);
+    if (q == cudaSuccess) continue;
+    if (q != cudaErrorNotReady) CU(q);
+    CU(cudaEventRecord(b->ev, p->stream));
+    CU(cudaStreamWaitEvent(st, b->ev, 0));
+  }
+  // device buffers of this call: [descriptors + the parity-1 sampler set | trials | states | active K + count | grids
+  // | xhist | uhist]
+  const size_t off_s1 = b->desc_bytes;
+  const size_t off_tr = off_s1 + align256((size_t)K * sizeof(SampleGridsV2Args));
+  const size_t off_state = off_tr + align256((size_t)K * sizeof(TrialDev));
+  const size_t off_act = off_state + align256((size_t)K * sizeof(TrialState));
+  size_t off = off_act + align256((size_t)(K + 1) * sizeof(int));
+  std::vector<size_t> off_grid(K);
+  for (int i = 0; i < K; ++i) {
+    off_grid[i] = off;
+    off += align256((size_t)2 * trials[i].height * trials[i].width * sizeof(double));
+  }
+  const size_t off_xh = off, off_uh = off_xh + align256((size_t)K * (S + 1) * 3 * sizeof(double));
+  const size_t total = off_uh + align256((size_t)K * S * 2 * sizeof(float));
+  const size_t head = off_xh;                         // uploaded part
+  unsigned char* d = nullptr;
+  unsigned char* h = nullptr;
+  CU(cudaMalloc(&d, total));
+  if (cudaMallocHost(&h, total) != cudaSuccess) { cudaFree(d); return fail(B200MPPI_ECUDA, "run_trials: cudaMallocHost"); }
+  struct Free {
+    unsigned char *d, *h;
+    ~Free() { cudaFree(d); cudaFreeHost(h); }
+  } guard{d, h};
+  std::memcpy(h, hd.data(), b->desc_bytes);
+  NoiseDesc* hn = reinterpret_cast<NoiseDesc*>(h);
+  SampleGridsV2Args* hs[2] = {reinterpret_cast<SampleGridsV2Args*>(h + b->off_sample),
+                              reinterpret_cast<SampleGridsV2Args*>(h + off_s1)};
+  RolloutArgs* hr = reinterpret_cast<RolloutArgs*>(h + b->off_roll);
+  UpdateBatchDesc* hu = reinterpret_cast<UpdateBatchDesc*>(h + b->off_upd);
+  TrialDev* ht = reinterpret_cast<TrialDev*>(h + off_tr);
+  TrialState* hst = reinterpret_cast<TrialState*>(h + off_state);
+  int* hact = reinterpret_cast<int*>(h + off_act);
+  RolloutArgs* dr = reinterpret_cast<RolloutArgs*>(d + b->off_roll);
+  for (int i = 0; i < K; ++i) {
+    b200mppi_planner* p = b->pl[i];
+    hn[i] = NoiseDesc{p->states, p->noise, p->prm.u_std[0], p->prm.u_std[1]};
+    fill_rollout_args(p, hr[i]);
+    fill_update_args(p, hu[i].a, nullptr);
+    hu[i].tl = UpdateTail{};
+    hu[i].tl.counter = p->upd_counter_d;
+    hu[i].tl.mode = UPD_TAIL_APPLY;
+    hu[i].tl.u_prev = p->u_prev;                       // self.u_prev_d = self.u_cur_d (alias, mppi.py:292,362)
+    hu[i].tl.u_out = b->u_d + (size_t)i * T * 2;
+    // parity 1: the pair samples from the buffers parity 0 wrote into
+    hs[1][i] = hs[0][i];
+    for (SampleTdm& td : hs[1][i].t) {
+      uint64_t* in = td.states_out;
+      td.states_out = const_cast<uint64_t*>(td.states);
+      td.states = in;
+    }
+    const b200mppi_trial_desc& q = trials[i];
+    const size_t cells = (size_t)q.height * q.width;
+    double* g = reinterpret_cast<double*>(h + off_grid[i]);
+    std::memcpy(g, q.lin, cells * sizeof(double));
+    std::memcpy(g + cells, q.ang, cells * sizeof(double));
+    const double* dg = reinterpret_cast<const double*>(d + off_grid[i]);
+    TrialDev& t = ht[i];
+    t.lin = dg; t.ang = dg + cells; t.H = q.height; t.W = q.width;
+    t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res; t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1];
+    t.tol = q.goal_tolerance;
+    t.pxlim[0] = q.pxlim[0]; t.pxlim[1] = q.pxlim[1]; t.pylim[0] = q.pylim[0]; t.pylim[1] = q.pylim[1];
+    t.u_cur = p->u_cur;
+    t.x0_out = dr[i].p.x0;
+    hst[i] = TrialState{};
+    for (int c = 0; c < 3; ++c) hst[i].x[c] = q.x0[c];
+    hact[i] = 1;
+  }
+  hact[K] = K;
+  CU(cudaMemcpyAsync(d, h, head, cudaMemcpyHostToDevice, st));
+  const NoiseDesc* dn = reinterpret_cast<const NoiseDesc*>(d);
+  const SampleGridsV2Args* ds[2] = {reinterpret_cast<const SampleGridsV2Args*>(d + b->off_sample),
+                                    reinterpret_cast<const SampleGridsV2Args*>(d + off_s1)};
+  const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(d + b->off_upd);
+  int* dact = reinterpret_cast<int*>(d + off_act);
+  PlantArgs pa{};
+  pa.trials = reinterpret_cast<const TrialDev*>(d + off_tr);
+  pa.state = reinterpret_cast<TrialState*>(d + off_state);
+  pa.active = dact; pa.active_count = dact + K;
+  pa.xhist = reinterpret_cast<double*>(d + off_xh);
+  pa.uhist = reinterpret_cast<float*>(d + off_uh);
+  pa.K = K; pa.T = T; pa.max_steps = S;
+  // the polled counts live in the (no longer needed) head of the pinned staging, one slot per step in flight
+  CU(cudaStreamSynchronize(st));                      // the staging is read by the upload above
+  int* hcount = reinterpret_cast<int*>(h);
+  cudaEvent_t ev[TRIAL_POLL] = {};
+  struct Events {
+    cudaEvent_t* e;
+    ~Events() { for (int i = 0; i < TRIAL_POLL; ++i) if (e[i]) cudaEventDestroy(e[i]); }
+  } evguard{ev};
+  for (auto& e : ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  const int num_opt = b->pl[0]->prm.num_opt;
+  int issued = 0;
+  for (int s = 0; s < S; ++s) {
+    if (s >= TRIAL_POLL) {                            // the count after step s - POLL
+      CU(cudaEventSynchronize(ev[s % TRIAL_POLL]));
+      if (hcount[s % TRIAL_POLL] == 0) break;
+    }
+    for (int k = 0; k < num_opt; ++k) {
+      launch_sample_noise_batch(dn, K, b->N, T, dact, st);
+      CHECK_LAUNCH();
+      if (k == 0) {
+        launch_sample_grids_v2_batch(hs[0][0], ds[s & 1], K, dact, st);
+        CHECK_LAUNCH();
+      }
+      launch_rollout_batch(dr, K, b->mode, b->N, T, dact, st);
+      CHECK_LAUNCH();
+      launch_update_partial_batch(du, K, b->pl[0]->num_ctas, dact, st);
+      CHECK_LAUNCH();
+    }
+    pa.step = s;
+    launch_plant_step(pa, st);
+    CHECK_LAUNCH();
+    b->launches += 3 * num_opt + 2;
+    ++issued;
+    CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, dact + K, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(ev[s % TRIAL_POLL], st));
+  }
+  CU(cudaMemcpyAsync(h + off_state, d + off_state, off_act - off_state, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(h + off_xh, d + off_xh, total - off_xh, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const double* hx = reinterpret_cast<const double*>(h + off_xh);
+  const float* hu_h = reinterpret_cast<const float*>(h + off_uh);
+  const double dnan = std::nan("");
+  const float fnan = std::nanf("");
+  for (int i = 0; i < K; ++i) {
+    const TrialState& r = hst[i];
+    const int n = r.steps;
+    double* xo = xhist + (size_t)i * (S + 1) * 3;
+    float* uo = uhist + (size_t)i * S * 2;
+    for (int c = 0; c < 3; ++c) xo[c] = trials[i].x0[c];
+    std::memcpy(xo + 3, hx + ((size_t)i * (S + 1) + 1) * 3, (size_t)n * 3 * sizeof(double));
+    for (size_t j = (size_t)(n + 1) * 3; j < (size_t)(S + 1) * 3; ++j) xo[j] = dnan;
+    std::memcpy(uo, hu_h + (size_t)i * S * 2, (size_t)n * 2 * sizeof(float));
+    for (size_t j = (size_t)n * 2; j < (size_t)S * 2; ++j) uo[j] = fnan;
+    results[i] = b200mppi_trial_result{r.cum_obj, r.cum_dist, r.dist, n, r.status};
+    // host state as after n rounds of the host loop: n samplings of the pair, the last solve's x0 in the params
+    b200mppi_planner* p = b->pl[i];
+    for (int s = 0; s < n; ++s) { plan_commit(plans[i], 0); plan_commit(plans[i], 1); }
+    p->prepared = false;
+    p->pushed_direct = false;
+    p->last_box[0] = 0; p->last_box[1] = 0; p->last_box[2] = p->lin->rows; p->last_box[3] = 0; p->last_box[4] = p->lin->cols;
+    for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)xo[(size_t)(n - 1) * 3 + c];
+  }
+  if (steps_issued) *steps_issued = issued;
   return B200MPPI_OK;
 }

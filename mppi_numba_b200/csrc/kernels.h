@@ -58,8 +58,9 @@ void launch_sample_grids_v2(const SampleGridsV2Args& a, int nt, cudaStream_t st)
 // batched one-map solves: equal launch configuration (grid, threads, shared memory, kernel variant)
 bool sample_grids_v2_same_launch(const SampleGridsV2Args& a, const SampleGridsV2Args& b);
 // ONE fused (nt = 2) launch for `count` pairs: descs = device array of their args, geom = any of them (host)
+// active (device, may be null): active[pair] == 0 -> that pair's CTAs return at once (closed-loop trials)
 void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs, int count,
-                                  cudaStream_t st);
+                                  const int* active, cudaStream_t st);
 // tile classes of a generator: (full | last) tile height x (full | last) tile width -> draws per whole-map walk
 void sample_tile_draws(int rows, int cols, int tx, int ty, int64_t ks[4]);
 // states_out[g] = states[g] advanced by the draws of a whole-map walk of generator g's tile (GF(2) jump with
@@ -86,7 +87,8 @@ struct NoiseDesc {
   float std_v, std_w;
 };
 // [emu:end noise_desc]
-void launch_sample_noise_batch(const NoiseDesc* descs, int count, int n_local, int T, cudaStream_t st);
+void launch_sample_noise_batch(const NoiseDesc* descs, int count, int n_local, int T, const int* active,
+                               cudaStream_t st);
 
 // Where the per-(map, control sequence) cost of a stochastic rollout goes.  Layout is MAP-MAJOR: row m holds the
 // costs of the control sequences on sampled map m, so the 32 lanes of a warp (consecutive n, same map) store one
@@ -134,7 +136,8 @@ struct RolloutArgs {
 // [emu:end rollout_args]
 void launch_rollout(const RolloutArgs& a, cudaStream_t st);
 // batched one-map solves (mode 1, 2, 3): descs = device array of `count` RolloutArgs of equal N and T (blockIdx.y)
-void launch_rollout_batch(const RolloutArgs* descs, int count, int mode, int N, int T, cudaStream_t st);
+void launch_rollout_batch(const RolloutArgs* descs, int count, int mode, int N, int T, const int* active,
+                          cudaStream_t st);
 // windowed (TMA-staged) stochastic rollout kernel -- rollout_win.cu
 // [emu:begin win_args]
 struct RolloutWinArgs {
@@ -218,11 +221,36 @@ struct UpdateBatchDesc {               // one planner of a batched update launch
 int update_num_ctas(int N);
 void launch_update_partial(const UpdateArgs& a, const UpdateTail& tl, cudaStream_t st);
 // batched one-map solves: `count` planners of equal N (hence equal num_ctas), UPD_TAIL_APPLY each
-void launch_update_partial_batch(const UpdateBatchDesc* descs, int count, int num_ctas, cudaStream_t st);
+void launch_update_partial_batch(const UpdateBatchDesc* descs, int count, int num_ctas, const int* active,
+                                 cudaStream_t st);
 // combine `count` partials (each 2T+2 floats; this rank's own partial is entry `self`) into u and weights
 void launch_update_finish(const UpdateArgs& a, const float* gathered, int count, const FlagWait& fw, cudaStream_t st);
 
 void launch_shift_u(float* u, int T, int shifts, cudaStream_t st);
+
+// closed-loop trials of a batch (b200mppi_batch_run_trials): the plant step of every running planner, one warp each
+// [emu:begin trial_args]
+enum { TRIAL_RUNNING = 0, TRIAL_GOAL = 1, TRIAL_MAX_STEPS = 2, TRIAL_LEFT_MAP = 3 };
+struct TrialDev {
+  const double* lin; const double* ang;   // ground-truth traction (H, W), float64
+  int H, W;
+  double xlo, ylo, res, dt, xgoal[2], tol, pxlim[2], pylim[2];
+  float* u_cur;                           // (T, 2): u_cur[0] is applied, then the sequence is shifted by one
+  float* x0_out;                          // RolloutArgs::p.x0 of this planner in the batch's device descriptors
+};
+struct TrialState {
+  double x[3], cum_obj, cum_dist, dist;
+  int steps, status;
+};
+struct PlantArgs {
+  const TrialDev* trials; TrialState* state;
+  int* active; int* active_count;
+  double* xhist;                          // (K, max_steps+1, 3)
+  float* uhist;                           // (K, max_steps, 2)
+  int K, T, max_steps, step;
+};
+// [emu:end trial_args]
+void launch_plant_step(const PlantArgs& a, cudaStream_t st);
 
 // visualisation rollouts (mppi.py:1194-1351)
 // [emu:begin vis_args]

@@ -44,8 +44,11 @@ __global__ void __launch_bounds__(256) sample_noise_kernel(uint64_t* __restrict_
 
 // [emu:end noise]
 // [emu:begin noise_batch]
-// batched one-map solves: planner blockIdx.y, its generators / noise / u_std from the descriptor array
-__global__ void __launch_bounds__(256) sample_noise_batch_kernel(const NoiseDesc* __restrict__ descs, int64_t count) {
+// batched one-map solves: planner blockIdx.y, its generators / noise / u_std from the descriptor array; a planner with
+// active[y] == 0 is left untouched (active null: every planner runs)
+__global__ void __launch_bounds__(256) sample_noise_batch_kernel(const NoiseDesc* __restrict__ descs, int64_t count,
+                                                                 const int* __restrict__ active = nullptr) {
+  if (active && !active[blockIdx.y]) return;
   const NoiseDesc& d = descs[blockIdx.y];
   sample_noise_body(d.states, reinterpret_cast<float2*>(d.noise), count, d.std_v, d.std_w, nullptr);
 }
@@ -59,10 +62,12 @@ void launch_sample_noise(uint64_t* states, float* noise, int n_local, int T, flo
       states, reinterpret_cast<float2*>(noise), count, std_v, std_w, reach);
 }
 
-void launch_sample_noise_batch(const NoiseDesc* descs, int count, int n_local, int T, cudaStream_t st) {
+void launch_sample_noise_batch(const NoiseDesc* descs, int count, int n_local, int T, const int* active,
+                               cudaStream_t st) {
   const int64_t per = (int64_t)n_local * T;
   const int threads = 256;
-  sample_noise_batch_kernel<<<dim3((unsigned)((per + threads - 1) / threads), (unsigned)count), threads, 0, st>>>(descs, per);
+  sample_noise_batch_kernel<<<dim3((unsigned)((per + threads - 1) / threads), (unsigned)count), threads, 0, st>>>(
+      descs, per, active);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -309,8 +314,11 @@ __global__ void __launch_bounds__(UPD_THREADS) update_apply_kernel(const UpdateA
 
 // [emu:end update]
 // [emu:begin update_batch]
-// batched one-map solves: planner blockIdx.y, each with its own CTA partials, ticket counter, weights and u
-__global__ void __launch_bounds__(UPD_THREADS) update_partial_batch_kernel(const UpdateBatchDesc* __restrict__ descs) {
+// batched one-map solves: planner blockIdx.y, each with its own CTA partials, ticket counter, weights and u; a planner
+// with active[y] == 0 is left untouched, its ticket counter included (active null: every planner runs)
+__global__ void __launch_bounds__(UPD_THREADS) update_partial_batch_kernel(const UpdateBatchDesc* __restrict__ descs,
+                                                                           const int* __restrict__ active = nullptr) {
+  if (active && !active[blockIdx.y]) return;
   const UpdateBatchDesc& d = descs[blockIdx.y];
   update_partial_body(d.a, d.tl);
 }
@@ -320,8 +328,9 @@ void launch_update_partial(const UpdateArgs& a, const UpdateTail& tl, cudaStream
   update_partial_kernel<<<a.num_ctas, UPD_THREADS, 0, st>>>(a, tl);
 }
 
-void launch_update_partial_batch(const UpdateBatchDesc* descs, int count, int num_ctas, cudaStream_t st) {
-  update_partial_batch_kernel<<<dim3((unsigned)num_ctas, (unsigned)count), UPD_THREADS, 0, st>>>(descs);
+void launch_update_partial_batch(const UpdateBatchDesc* descs, int count, int num_ctas, const int* active,
+                                 cudaStream_t st) {
+  update_partial_batch_kernel<<<dim3((unsigned)num_ctas, (unsigned)count), UPD_THREADS, 0, st>>>(descs, active);
 }
 
 void launch_update_finish(const UpdateArgs& a, const float* gathered, int count, const FlagWait& fw, cudaStream_t st) {
@@ -341,6 +350,90 @@ __global__ void shift_u_kernel(float* u, int T, int shifts) {
 void launch_shift_u(float* u, int T, int shifts, cudaStream_t st) {
   if (shifts <= 0 || shifts >= T) return;
   shift_u_kernel<<<1, 256, (size_t)2 * T * sizeof(float), st>>>(u, T, shifts);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Plant step of a closed-loop trial, as the benchmark's trial() computes it in float64 (no contraction: every product
+// and sum is rounded on its own, in the loop's order).
+// [emu:begin trial]
+// CPython's float `//` (float_floor_div): fmod, subtract, divide, floor, with its sign and snap-to-nearest corrections
+__device__ __forceinline__ double py_floordiv(double vx, double wx) {
+  double mod = fmod(vx, wx);
+  double div = __ddiv_rn(__dsub_rn(vx, mod), wx);
+  if (mod != 0.0) {
+    if ((wx < 0.0) != (mod < 0.0)) div = __dsub_rn(div, 1.0);
+  }
+  if (div != 0.0) {
+    double fl = floor(div);
+    if (__dsub_rn(div, fl) > 0.5) fl = __dadd_rn(fl, 1.0);
+    return fl;
+  }
+  return copysign(0.0, __ddiv_rn(vx, wx));
+}
+
+// One warp per planner (warp k of the grid = planner k): apply u_cur[0], shift u_cur by one row (the last row kept),
+// record the step, and stop the planner on the goal, on leaving the padded map or after max_steps steps.
+__device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int lane) {
+  if (k >= a.K || !a.active[k]) return;
+  const TrialDev& d = a.trials[k];
+  float* u = d.u_cur;
+  float v = 0.0f, w = 0.0f;
+  if (lane == 0) { v = u[0]; w = u[1]; }
+  __syncwarp();
+  // u[:-1] = u[1:] in place: chunk c reads floats [c+2, c+34) before any lane writes [c, c+32)
+  const int n = 2 * (a.T - 1);
+  for (int c = 0; c < n; c += 32) {
+    const int i = c + lane;
+    const float x = i < n ? u[i + 2] : 0.0f;
+    __syncwarp();
+    if (i < n) u[i] = x;
+  }
+  if (lane != 0) return;
+  TrialState& s = a.state[k];
+  const int t = a.step;
+  float* uh = a.uhist + ((size_t)k * a.max_steps + t) * 2;
+  uh[0] = v; uh[1] = w;
+  const double x = s.x[0], y = s.x[1], th = s.x[2];
+  // TractionGrid.get: int((x - xlo) // res), (0, 0) outside [0, W) x [0, H)
+  const double fx = py_floordiv(__dsub_rn(x, d.xlo), d.res), fy = py_floordiv(__dsub_rn(y, d.ylo), d.res);
+  double lt = 0.0, at = 0.0;
+  if (fx >= 0.0 && fx < (double)d.W && fy >= 0.0 && fy < (double)d.H) {
+    const size_t cell = (size_t)fy * (size_t)d.W + (size_t)fx;
+    lt = d.lin[cell]; at = d.ang[cell];
+  }
+  const double dtl = __dmul_rn(d.dt, lt);
+  const double xn = __dadd_rn(x, __dmul_rn(__dmul_rn(dtl, cos(th)), (double)v));
+  const double yn = __dadd_rn(y, __dmul_rn(__dmul_rn(dtl, sin(th)), (double)v));
+  const double thn = __dadd_rn(th, __dmul_rn(__dmul_rn(d.dt, at), (double)w));
+  s.x[0] = xn; s.x[1] = yn; s.x[2] = thn;
+  double* xh = a.xhist + ((size_t)k * (a.max_steps + 1) + t + 1) * 3;
+  xh[0] = xn; xh[1] = yn; xh[2] = thn;
+  // the next rollout starts from float32(x_next), as set_params would pass it
+  d.x0_out[0] = __double2float_rn(xn); d.x0_out[1] = __double2float_rn(yn); d.x0_out[2] = __double2float_rn(thn);
+  const double dx = __dsub_rn(xn, d.xgoal[0]), dy = __dsub_rn(yn, d.xgoal[1]);
+  const double dist = __dsub_rn(__dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy))), d.tol);
+  s.cum_obj = __dadd_rn(s.cum_obj, __dadd_rn(d.dt, dist));
+  s.cum_dist = __dadd_rn(s.cum_dist, dist);
+  s.dist = dist;
+  s.steps = t + 1;
+  int status = TRIAL_RUNNING;
+  if (dist <= 0.0) status = TRIAL_GOAL;
+  else if (!(xn >= d.pxlim[0] && xn <= d.pxlim[1] && yn >= d.pylim[0] && yn <= d.pylim[1])) status = TRIAL_LEFT_MAP;
+  else if (t + 1 >= a.max_steps) status = TRIAL_MAX_STEPS;
+  if (status != TRIAL_RUNNING) {
+    s.status = status;
+    a.active[k] = 0;
+    atomicSub(a.active_count, 1);
+  }
+}
+
+__global__ void __launch_bounds__(128) plant_step_kernel(const PlantArgs a) {
+  plant_step_body(a, (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), (int)(threadIdx.x & 31));
+}
+// [emu:end trial]
+
+void launch_plant_step(const PlantArgs& a, cudaStream_t st) {
+  plant_step_kernel<<<(unsigned)((a.K + 3) / 4), 128, 0, st>>>(a);
 }
 
 }  // namespace b200

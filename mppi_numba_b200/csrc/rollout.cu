@@ -201,9 +201,12 @@ __global__ void __launch_bounds__(128) rollout_barebone_kernel(const RolloutArgs
 // [emu:end rollout]
 // [emu:begin rollout_batch]
 // batched one-map solves (modes 1, 2, 3): planner blockIdx.y, its full RolloutArgs (geometry, maps, noise, u, costs)
-// from the descriptor array; N and T are the batch's, so the grid and the 2T floats of shared memory are too
+// from the descriptor array; N and T are the batch's, so the grid and the 2T floats of shared memory are too.  A
+// planner with active[y] == 0 is left untouched (active null: every planner runs)
 template <int MODE>
-__global__ void __launch_bounds__(128) rollout_batch_kernel(const RolloutArgs* __restrict__ descs) {
+__global__ void __launch_bounds__(128) rollout_batch_kernel(const RolloutArgs* __restrict__ descs,
+                                                            const int* __restrict__ active = nullptr) {
+  if (active && !active[blockIdx.y]) return;
   if constexpr (MODE == 3) rollout_barebone_body(descs[blockIdx.y]);
   else rollout_body<MODE>(descs[blockIdx.y]);
 }
@@ -221,13 +224,14 @@ void launch_rollout(const RolloutArgs& a, cudaStream_t st) {
   else rollout_kernel<2><<<grid, threads, smem, st>>>(a);
 }
 
-void launch_rollout_batch(const RolloutArgs* descs, int count, int mode, int N, int T, cudaStream_t st) {
+void launch_rollout_batch(const RolloutArgs* descs, int count, int mode, int N, int T, const int* active,
+                          cudaStream_t st) {
   const int threads = 128;
   const dim3 grid((N + threads - 1) / threads, count);
   const size_t smem = (size_t)2 * T * sizeof(float);
-  if (mode == 1) rollout_batch_kernel<1><<<grid, threads, smem, st>>>(descs);
-  else if (mode == 2) rollout_batch_kernel<2><<<grid, threads, smem, st>>>(descs);
-  else rollout_batch_kernel<3><<<grid, threads, smem, st>>>(descs);
+  if (mode == 1) rollout_batch_kernel<1><<<grid, threads, smem, st>>>(descs, active);
+  else if (mode == 2) rollout_batch_kernel<2><<<grid, threads, smem, st>>>(descs, active);
+  else rollout_batch_kernel<3><<<grid, threads, smem, st>>>(descs, active);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -453,9 +453,12 @@ __global__ void __launch_bounds__(128) advance_states_kernel(const ulonglong2* _
 // [emu:begin sampler_batch]
 // batched one-map solves: one fused lin + ang whole-map launch for every pair of the batch, pair blockIdx.z.  The
 // launch geometry (rows, cols, bins, pitch, thread tiles, segments) is the batch's; each descriptor brings its own
-// TDM buffers, threshold table and jump matrices.
+// TDM buffers, threshold table and jump matrices.  A pair with active[z] == 0 is left untouched (active null: every
+// pair runs).
 template <int NT, int NW>
-__global__ void __launch_bounds__(256) sample_grids_v2_batch_kernel(const SampleGridsV2Args* __restrict__ descs) {
+__global__ void __launch_bounds__(256) sample_grids_v2_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
+                                                                    const int* __restrict__ active = nullptr) {
+  if (active && !active[blockIdx.z]) return;
   sample_grids_v2_body<NT, NW>(descs[blockIdx.z]);
 }
 // [emu:end sampler_batch]
@@ -531,7 +534,7 @@ bool sample_grids_v2_same_launch(const SampleGridsV2Args& a, const SampleGridsV2
 }
 
 void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs, int count,
-                                  cudaStream_t st) {
+                                  const int* active, cudaStream_t st) {
   const int nrow = (geom.rows + geom.tx - 1) / geom.tx;
   const int tix_hi = std::min(geom.tx - 1, (std::max(geom.row_hi, geom.row_lo + 1) - 1) / nrow);
   const dim3 grid((tix_hi - geom.tix_lo + 1) * geom.segs, (geom.num_maps + geom.gm - 1) / geom.gm, count);
@@ -540,7 +543,7 @@ void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGri
   const int nw = geom.t[0].bpad / 4;
   auto go = [&](auto kern) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    kern<<<grid, threads, smem, st>>>(descs);
+    kern<<<grid, threads, smem, st>>>(descs, active);
   };
   if (nw == 3) go(sample_grids_v2_batch_kernel<2, 3>);
   else if (nw == 8) go(sample_grids_v2_batch_kernel<2, 8>);
