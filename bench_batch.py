@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench_batch.py -- K one-map planners: K sequential solve() calls against one batched MPPI_Batch.solve().
+"""bench_batch.py -- K planners: K sequential solve() calls against one batched MPPI_Batch / MPPI_StochasticBatch solve().
 
-    python bench_batch.py --workload c2|c4 --batch K [--steps S] [--warmup W]
+    python bench_batch.py --workload c2|c3|c4 --batch K [--steps S] [--warmup W] [--profile]
 
 K planners of the workload (bench.py's WORKLOADS, seeds 1..K: different maps, start poses and goals; num_opt = 1).
 First one MPPI_Batch.solve() is checked against K solve() calls on identical twins, bit for bit (u, u_prev, costs,
@@ -10,6 +10,9 @@ sequential solve() calls and one batch solve are timed, alternating (sequential,
 events on the one stream all planners and the batch use, and the wall clock (each round ends in a host
 synchronisation); solves/s, state-steps/s and kernel launches per round.  Prints one JSON line; writes nothing to the
 tree (the library is built by build() beforehand).
+c3 (stochastic, use_tdm) runs MPPI_StochasticBatch; its parity check also compares the per-(m, n) costs and the reach
+box of every planner.  --profile adds a torch.profiler split of one batched round's kernel time into map sampler,
+rollout and the rest (a separate run after the timings).
 """
 import argparse
 import json
@@ -44,12 +47,16 @@ def run(args, emit):
     stream = torch.cuda.Stream(device=dev)
     for p in A + S:
         check(lib.b200mppi_planner_set_stream(p._handle, C.c_void_p(stream.cuda_stream)))
-    batch = E.MPPI_Batch(A)
+    stochastic = mode == "tdm"
+    batch = E.MPPI_StochasticBatch(A) if stochastic else E.MPPI_Batch(A)
     batch.set_stream(stream.cuda_stream)
 
     def state(p):
         d = [p.u_cur_d, p.u_prev_d, p.costs_d, p.weights_d, p.noise_samples_d, p.rng_states_d, p.lin_tdm.rng_states_d,
              p.ang_tdm.rng_states_d, p.lin_tdm.sample_grid_batch_d, p.ang_tdm.sample_grid_batch_d]
+        if stochastic:
+            d.append(p.costs_nm_d)
+            return [np.asarray(p.sample_box())] + [a.copy_to_host() for a in d]
         return [a.copy_to_host() for a in d]
 
     # ---- parity: one batch solve == K sequential solves, bit for bit
@@ -59,6 +66,9 @@ def run(args, emit):
     same_state = all(all(np.array_equal(x, y) for x, y in zip(state(a), state(s))) for a, s in zip(A, S))
     parity = {"passed": same_u and same_state, "u_bitwise": same_u, "state_bitwise": same_state, "planners": K,
               "against": "K solve() calls on identical twins (u, u_prev, costs, weights, noise, RNG states, sampled maps)"}
+    if stochastic:
+        parity["against"] = ("K solve() calls on identical twins (u, u_prev, costs, per-(m, n) costs, weights, noise, RNG "
+                             "states, sampled maps, reach box)")
     if not parity["passed"]:
         sys.stderr.write("bench_batch.py: PARITY CHECK FAILED: %s\n" % json.dumps(parity))
         emit(json.dumps({"metric": "batched one-map solves", "error": "parity_check failed", "parity_check": parity}))
@@ -112,14 +122,46 @@ def run(args, emit):
         gpu["power_limit_and_max_sm_clock"] = q
     except Exception as e:                               # noqa: BLE001
         gpu["power_limit_and_max_sm_clock"] = "unavailable (%r)" % e
-    emit(json.dumps({"metric": "batched one-map solves: K sequential solve() calls vs one MPPI_Batch.solve()",
+    out = {"metric": "batched one-map solves: K sequential solve() calls vs one MPPI_Batch.solve()",
                      "unit": "solves/s", "value": bat["solves_per_s"], "higher_is_better": True,
                      "config": {"workload": workload_name_of(args.workload), "batch": K,
                                 "planners": "seeds 1..K (different maps, start poses and goals), num_opt=1"},
                      "steps": args.steps, "warmup": args.warmup, "gpu": gpu, "parity_check": parity,
                      "sequential": seq, "batched": bat,
                      "speedup_wall": seq["ms_per_round_wall"] / bat["ms_per_round_wall"],
-                     "speedup_events": seq["ms_per_round_events"] / bat["ms_per_round_events"]}))
+                     "speedup_events": seq["ms_per_round_events"] / bat["ms_per_round_events"]}
+    if stochastic:
+        out["metric"] = "batched stochastic solves: K sequential solve() calls vs one MPPI_StochasticBatch.solve()"
+        out["config"]["planners"] = "seeds 1..K (different maps, start poses and goals), use_tdm, num_opt=1"
+    if args.profile:
+        out["profile_batched_round"] = profile_round(batch_round, dev, stream)
+    emit(json.dumps(out))
+
+
+def profile_round(fn, dev, stream, rounds=5):
+    """Kernel time per batched round by group (torch.profiler, CUDA activities), over `rounds` rounds."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize(dev)
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(rounds):
+            fn()
+        torch.cuda.synchronize(dev)
+    groups = {"sampler": 0.0, "rollout": 0.0, "rest": 0.0}
+    kernels = {}
+    for ev in prof.events():
+        if ev.device_type != torch.autograd.DeviceType.CUDA or "memcpy" in ev.name.lower() or "memset" in ev.name.lower():
+            continue
+        us = ev.device_time if hasattr(ev, "device_time") else ev.cuda_time
+        name = ev.name
+        g = "sampler" if ("sample_grids" in name or "advance_states" in name) else (
+            "rollout" if "rollout_win" in name else "rest")
+        groups[g] += us
+        short = name.split("(")[0][-60:]
+        kernels[short] = kernels.get(short, 0.0) + us
+    return {"kernel_ms_per_round": {k: v / rounds / 1e3 for k, v in groups.items()},
+            "kernel_ms_per_round_by_kernel": {k: v / rounds / 1e3 for k, v in sorted(kernels.items())},
+            "rounds": rounds}
 
 
 def main():
@@ -131,10 +173,11 @@ def main():
     def emit(line):
         os.write(real_stdout, (line + "\n").encode())
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[1])
-    ap.add_argument("--workload", default="c2", choices=["c2", "c4"])
+    ap.add_argument("--workload", default="c2", choices=["c2", "c3", "c4"])
     ap.add_argument("--batch", type=int, default=64, metavar="K", help="planners in the batch")
     ap.add_argument("--steps", type=int, default=20, help="timed rounds per measurement")
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--profile", action="store_true", help="add a torch.profiler kernel-time split of a batched round")
     args = ap.parse_args()
     if args.batch < 1 or args.steps < 1:
         ap.error("--batch and --steps must be at least 1")

@@ -304,8 +304,8 @@ int b200mppi_planner_sample_box(b200mppi_planner* pl, int32_t out[5]);
  * rollout, update; plus one descriptor upload and one D2H of all K control sequences), instead of K solve() calls of
  * four small launches, two copies and a host synchronisation each.  The planners are BORROWED (they must outlive the
  * batch) and keep every per-planner call (set_params, set_u, shift_u, copy_out, get_state_rollout, ...).
- *   create: planners on one device, world_size 1, one mode among MODE_DET_DYN / MODE_SPEED_MAP / MODE_BAREBONE (the
- *           stochastic MODE_TDM is not batched: its windowed rollout kernel already fills the GPU), equal num_steps and
+ *   create: planners on one device, world_size 1, one mode among MODE_DET_DYN / MODE_SPEED_MAP / MODE_BAREBONE
+ *           (MODE_TDM planners: b200mppi_batch_create_stochastic below), equal num_steps and
  *           num_control_rollouts, no planner listed twice.  Anything else: B200MPPI_EINVAL naming the planner's index.
  *   solve : == b200mppi_planner_solve on planners[0], planners[1], ... in that order, bit for bit: u, u_prev, noise,
  *           costs, weights, the planners' and their TDMs' RNG states and the sampled maps all end up identical.  Needs
@@ -323,6 +323,22 @@ int b200mppi_batch_destroy(b200mppi_batch* b);
 int b200mppi_batch_set_stream(b200mppi_batch* b, void* cuda_stream);
 int b200mppi_batch_solve(b200mppi_batch* b, float* u_out);
 int b200mppi_batch_launch_count(b200mppi_batch* b, int64_t* out);
+
+/* ------------------------------------------------------------------ batched stochastic solves
+ * K independent MODE_TDM (CVaR-cost) planners of one shape solved together: per optimisation iteration ONE launch each
+ * of noise + controls, windowed rollout (all K*M (planner, map) units on the persistent grid), CVaR and update.  The map
+ * sampling of the first iteration stays per planner (each planner's reach box is its own: 1 or 2 launches each), with
+ * one host wait for all K reach statistics.  The result is a b200mppi_batch: batch_solve, set_stream, launch_count and
+ * destroy work on it as above; b200mppi_batch_run_trials refuses it.
+ *   create: planners on one device, MODE_TDM, world_size 1, equal num_steps, num_control_rollouts and
+ *           num_grid_samples (at most 1024), no planner listed twice.  Anything else: B200MPPI_EINVAL naming the planner.
+ *   solve : == b200mppi_planner_solve on planners[0], planners[1], ... in that order, bit for bit: u, noise, per-(m, n)
+ *           costs, costs, weights, the planners' and their TDMs' RNG states, the sampled maps (boxed or whole), the
+ *           reach-box decisions (b200mppi_planner_sample_box) and the host-side solve state.  Refused before any work is
+ *           issued (B200MPPI_EINVAL or the planner's own error, naming the planner): what batch_solve refuses, and a
+ *           planner that would not take the windowed rollout kernel (B200MPPI_NO_WINDOW, a window that does not fit,
+ *           tensor maps that cannot be encoded).  u_prev is not touched (a stochastic solve does not alias it). */
+int b200mppi_batch_create_stochastic(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out);
 
 /* ------------------------------------------------------------------ closed-loop trials of a batch
  * Every planner of a MODE_DET_DYN or MODE_SPEED_MAP batch drives a unicycle through one receding-horizon episode on

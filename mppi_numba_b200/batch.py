@@ -11,6 +11,10 @@ Each planner keeps its own params, TDMs, warm start and RNG streams; ``solve()``
 ``planner.solve()`` called on planners[0], planners[1], ... in that order would (include/b200mppi.h, batched one-map
 solves).  The planners must share N, T, the device and the mode; their TDMs must not be shared between planners.
 
+``MPPI_StochasticBatch(planners)`` does the same for use_tdm (CVaR-cost) planners of equal N, T and
+num_grid_samples (at most 1024): one launch per stage for noise, rollout, CVaR and update, the map sampling per planner
+(include/b200mppi.h, batched stochastic solves).
+
 ``run_trials(traction_grids, max_steps)`` runs the benchmark's closed-loop episode (solve, plant step on a ground-truth
 ``TractionGrid``, shift_and_update, stop at the goal) for every det-dynamics or speed-map planner at once on the GPU,
 without a host round trip per step (include/b200mppi.h, closed-loop trials).
@@ -80,16 +84,21 @@ class MPPI_Batch(object):
     def solve(self):
         """One solve() of every planner.  Returns np.float32 (K, T, 2), or None (with the planner's index and the
         reason printed) when a planner's preconditions fail -- then nothing is solved."""
+        u = self._solve("MPPI_Batch")
+        if u is not None:
+            for p in self.planners:                    # as each planner's own solve() does (mppi.py:292,362)
+                p.u_prev_d = p._u_prev_buf
+        return u
+
+    def _solve(self, name):
         for i, p in enumerate(self.planners):
             if not p.check_solve_conditions():
-                print("MPPI_Batch: planner {}: MPPI solve condition not met. Cannot solve. Return".format(i))
+                print("{}: planner {}: MPPI solve condition not met. Cannot solve. Return".format(name, i))
                 return None
         for p in self.planners:
             p.move_mppi_task_vars_to_device()          # each planner's params POD (and TDMs / obstacles)
         u = np.empty((len(self.planners), self.num_steps, 2), dtype=np.float32)
         check(lib.b200mppi_batch_solve(self._handle, ptr(u)))
-        for p in self.planners:                        # as each planner's own solve() does (mppi.py:292,362)
-            p.u_prev_d = p._u_prev_buf
         return u
 
     def set_stream(self, cuda_stream):
@@ -184,3 +193,40 @@ class MPPI_Batch(object):
                              cum_dist_to_goal=r.cum_dist_to_goal, avg_dist_to_goal=r.cum_dist_to_goal / n,
                              cum_obj=cum_obj))
         return dict(logs=logs, xhist=xhist, uhist=uhist, steps=steps, status=status)
+
+
+class MPPI_StochasticBatch(MPPI_Batch):
+    """Borrows use_tdm ``planners`` (keeps them alive) and solves them with one launch per stage: noise, windowed
+    rollout, CVaR and update; each planner's map sampling keeps its own launches.  ``solve()``, ``set_stream`` and
+    ``launch_count`` as in MPPI_Batch; closed-loop trials are not offered."""
+
+    def __init__(self, planners):
+        planners = list(planners)
+        if not planners:
+            raise ValueError("MPPI_StochasticBatch: no planners")
+        for i, p in enumerate(planners):
+            kind, ws = _kind(p)
+            if kind != "tdm":
+                raise ValueError("MPPI_StochasticBatch: planner %d is a %s planner (a stochastic batch holds use_tdm "
+                                 "planners; MPPI_Batch takes the others)" % (i, kind))
+            if ws != 1:
+                raise ValueError("MPPI_StochasticBatch: planner %d has world_size %d (a batch holds single-rank planners)"
+                                 % (i, ws))
+        self.planners = planners
+        self.kind = "tdm"
+        self.num_steps = planners[0].num_steps
+        self._handle = None
+        handles = (C.c_void_p * len(planners))(*[p._handle.value for p in planners])
+        h = C.c_void_p()
+        check(lib.b200mppi_batch_create_stochastic(handles, len(planners), C.byref(h)))
+        self._handle = h
+
+    def solve(self):
+        """One solve() of every planner.  Returns np.float32 (K, T, 2), or None (with the planner's index and the
+        reason printed) when a planner's preconditions fail -- then nothing is solved.  u_prev_d is left alone, as a
+        stochastic planner's own solve() leaves it."""
+        return self._solve("MPPI_StochasticBatch")
+
+    def run_trials(self, traction_grids, max_steps, dt=None):
+        raise ValueError("MPPI_StochasticBatch.run_trials: closed-loop trials run det-dynamics or speed-map batches "
+                         "(a stochastic solve sizes each planner's map-sampling box on the host)")

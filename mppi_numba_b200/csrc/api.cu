@@ -1022,6 +1022,29 @@ static void fill_rollout_args(b200mppi_planner* p, RolloutArgs& a) {
   fill_cost_dst(p, a.dst, false);
 }
 
+// The planner's part of the windowed rollout's arguments: window (centred on the robot's cell) and buffers.
+static void fill_win_args(const b200mppi_planner* p, int WW, int WH, RolloutWinArgs& w) {
+  const b200mppi_tdm* l = p->lin; const b200mppi_tdm* g = p->ang;
+  w.WW = WW; w.WH = WH;
+  const int xi0 = (int)std::floor(((double)p->prm.x0[0] - (double)l->pxl[0]) / (double)l->res);
+  const int yi0 = (int)std::floor(((double)p->prm.x0[1] - (double)l->pyl[0]) / (double)l->res);
+  // TMA: the inner (x) start coordinate is kept 16-byte aligned for 1-byte elements (an unaligned c0 faulted
+  // with 'illegal instruction' when probed); floor to a multiple of 16, also for negatives
+  // The window is kept INSIDE the map (origin clamped, extents cut): a staged cell is then always a map cell, and
+  // every index outside the map takes the global-memory path with the generic kernel's wrap + clamp.
+  int cx = xi0 - WW / 2, cy = yi0 - WH / 2;
+  cx = std::max(0, std::min(cx, l->cols - WW));
+  cy = std::max(0, std::min(cy, l->rows - WH));
+  w.wx0 = cx & ~15;
+  w.wy0 = cy;
+  w.ww = std::min(WW, l->cols - w.wx0);
+  w.wh = std::min(WH, l->rows - w.wy0);
+  w.npad = p->npad;
+  w.masks01 = l->masks01 ? 1 : 0;
+  w.lin_grid = l->grid; w.ang_grid = g->grid; w.obstacle = l->obstacle; w.unknown = l->unknown;
+  w.noiseT = p->noiseT; w.ctrl = p->ctrl; w.u_cur = p->u_cur;
+}
+
 static int stage_rollout(b200mppi_planner* p) {
   RolloutArgs a;
   fill_rollout_args(p, a);
@@ -1031,7 +1054,6 @@ static int stage_rollout(b200mppi_planner* p) {
     // stochastic mode: TMA-staged map windows (rollout_win.cu); window centred on the robot's cell
     int WW, WH; size_t smem;
     rollout_win_geometry(p->T, &WW, &WH, &smem);
-    const b200mppi_tdm* l = p->lin; const b200mppi_tdm* g = p->ang;
     if (planner_tensor_maps(p, WW, WH)) {
       if (!p->prepared) {                       // noise came from outside (set_noise): derive the controls now
         launch_prepare_rollout(p->noise, p->u_cur, p->noiseT, p->ctrl, nullptr, p->n_local, p->T, p->npad,
@@ -1042,24 +1064,7 @@ static int stage_rollout(b200mppi_planner* p) {
       p->prepared = false;                      // u_cur changes with the update that follows
       RolloutWinArgs w{};
       w.p = a.p;
-      w.WW = WW; w.WH = WH;
-      const int xi0 = (int)std::floor(((double)p->prm.x0[0] - (double)l->pxl[0]) / (double)l->res);
-      const int yi0 = (int)std::floor(((double)p->prm.x0[1] - (double)l->pyl[0]) / (double)l->res);
-      // TMA: the inner (x) start coordinate is kept 16-byte aligned for 1-byte elements (an unaligned c0 faulted
-      // with 'illegal instruction' when probed); floor to a multiple of 16, also for negatives
-      // The window is kept INSIDE the map (origin clamped, extents cut): a staged cell is then always a map cell, and
-      // every index outside the map takes the global-memory path with the generic kernel's wrap + clamp.
-      int cx = xi0 - WW / 2, cy = yi0 - WH / 2;
-      cx = std::max(0, std::min(cx, l->cols - WW));
-      cy = std::max(0, std::min(cy, l->rows - WH));
-      w.wx0 = cx & ~15;
-      w.wy0 = cy;
-      w.ww = std::min(WW, l->cols - w.wx0);
-      w.wh = std::min(WH, l->rows - w.wy0);
-      w.npad = p->npad;
-      w.masks01 = l->masks01 ? 1 : 0;
-      w.lin_grid = l->grid; w.ang_grid = g->grid; w.obstacle = l->obstacle; w.unknown = l->unknown;
-      w.noiseT = p->noiseT; w.ctrl = p->ctrl; w.u_cur = p->u_cur;
+      fill_win_args(p, WW, WH, w);
       // sharded + peers connected: the all-to-all is this kernel's epilogue (stores into the peers, then the flags)
       const bool direct = p->shard_maps && p->p2p_ready;
       fill_cost_dst(p, w.dst, direct);
@@ -1187,21 +1192,46 @@ static bool planner_reach_box(const b200mppi_planner* p, const float* reach, Sam
   return true;
 }
 
+// A solve's map sampling in three steps, shared by solve() (stage_sample_tdms) and the stochastic batch:
+//   plan_sampling with sample_alpha; then, if sample_reads_reach, the 4-byte reach statistic is copied to the host
+//   (sample_reach_host) behind an event, a fused pair's state advance is queued (it does not depend on the box: it runs
+//   while the host wakes up, and should the sampling take whole maps after all, that launch stores the very same states
+//   again), and the host waits for the event; finally sample_finish sizes the box and launches the sampler.
+// det / speed-map solves call sample_grids() with the default alpha_dyn = 1.0 (mppi.py:248-249,322-323)
+static double sample_alpha(const b200mppi_planner* p) {
+  return p->cfg.mode == B200MPPI_MODE_TDM ? p->prm.alpha_dyn : 1.0;
+}
+
+// a box from this solve's own controls: the host waits for their reach statistic only (an event, not the stream)
+static bool sample_reads_reach(const b200mppi_planner* p) {
+  return p->box_mode == 2 && p->prm.num_opt == 1 && p->prepared && p->reach_valid && planner_uses_window(p);
+}
+
+static float* sample_reach_host(b200mppi_planner* p) { return p->h_u + (size_t)p->T * 2 + 2; }
+
+// reach: the read-back statistic or null (static box); advanced: a fused pair's state advance is already queued
+static int sample_finish(b200mppi_planner* p, SamplePlan& plan, const float* reach, bool advanced, cudaStream_t st,
+                         int64_t* launches) {
+  SampleBox box{};
+  int how = 0;
+  if (planner_reach_box(p, reach, &box, &how)) plan_box(&plan, box);
+  const int rc = plan_launch(plan, advanced, st, launches);
+  const bool used = plan.boxed[0];                        // the box may not fit the sampler's launch: whole maps
+  p->last_box[0] = used ? how : 0;
+  p->last_box[1] = used ? box.row_lo : 0; p->last_box[2] = used ? box.row_hi : p->lin->rows;
+  p->last_box[3] = used ? box.col_lo : 0; p->last_box[4] = used ? box.col_hi : p->lin->cols;
+  return rc;
+}
+
 static int stage_sample_tdms(b200mppi_planner* p) {
   if (p->cfg.mode == B200MPPI_MODE_BAREBONE) return B200MPPI_OK;      // no maps
-  // det / speed-map solves call sample_grids() with the default alpha_dyn = 1.0 (mppi.py:248-249,322-323)
-  const double alpha = p->cfg.mode == B200MPPI_MODE_TDM ? p->prm.alpha_dyn : 1.0;
   SamplePlan plan;
-  int rc = plan_sampling(p->lin, p->ang, alpha, p->stream, &plan);
+  int rc = plan_sampling(p->lin, p->ang, sample_alpha(p), p->stream, &plan);
   if (rc) return rc;
-  // a box from this solve's own controls: the host waits for their 4-byte reach statistic only (an event, not the
-  // stream).  A fused pair's state advance does not depend on the box: queued behind the copy, it runs while the host
-  // wakes up, sizes the box and launches the sampler.  Should the sampling take whole maps after all, that launch
-  // stores the very same states again.
   const float* reach = nullptr;
   bool advanced = false;
-  if (p->box_mode == 2 && p->prm.num_opt == 1 && p->prepared && p->reach_valid && planner_uses_window(p)) {
-    float* h = p->h_u + (size_t)p->T * 2 + 2;
+  if (sample_reads_reach(p)) {
+    float* h = sample_reach_host(p);
     CU(cudaMemcpyAsync(h, p->reach_d + p->reach_slot, sizeof(float), cudaMemcpyDeviceToHost, p->stream));
     CU(cudaEventRecord(p->ev_reach, p->stream));
     if (plan.fused) {
@@ -1213,15 +1243,7 @@ static int stage_sample_tdms(b200mppi_planner* p) {
     CU(cudaEventSynchronize(p->ev_reach));
     reach = h;
   }
-  SampleBox box{};
-  int how = 0;
-  if (planner_reach_box(p, reach, &box, &how)) plan_box(&plan, box);
-  rc = plan_launch(plan, advanced, p->stream, &p->launches);
-  const bool used = plan.boxed[0];                        // the box may not fit the sampler's launch: whole maps
-  p->last_box[0] = used ? how : 0;
-  p->last_box[1] = used ? box.row_lo : 0; p->last_box[2] = used ? box.row_hi : p->lin->rows;
-  p->last_box[3] = used ? box.col_lo : 0; p->last_box[4] = used ? box.col_hi : p->lin->cols;
-  return rc;
+  return sample_finish(p, plan, reach, advanced, p->stream, &p->launches);
 }
 
 static void collect_timings(b200mppi_planner* p) {
@@ -1740,6 +1762,11 @@ struct b200mppi_batch {
   float* u_d = nullptr;                // (K, T, 2): every planner's new u, written by its update's last CTA
   float* h_u = nullptr;                // pinned (K, T, 2)
   int64_t launches = 0;
+  // stochastic batch (b200mppi_batch_create_stochastic): MODE_TDM planners, windowed rollouts.  Descriptors:
+  // [NoisePrepDesc K | RolloutWinArgs K | CUtensorMap 4K (64-byte aligned) | CvarDesc K | UpdateBatchDesc K]
+  bool stochastic = false;
+  int M = 0;
+  size_t off_win = 0, off_tm = 0, off_cvar = 0;
 };
 
 static size_t align256(size_t v) { return (v + 255) / 256 * 256; }
@@ -1759,9 +1786,16 @@ extern "C" int b200mppi_batch_destroy(b200mppi_batch* b) {
 
 static int batch_init(b200mppi_batch* b) {
   const size_t K = b->pl.size();
-  b->off_sample = align256(K * sizeof(NoiseDesc));
-  b->off_roll = b->off_sample + align256(K * sizeof(SampleGridsV2Args));
-  b->off_upd = b->off_roll + align256(K * sizeof(RolloutArgs));
+  if (b->stochastic) {
+    b->off_win = align256(K * sizeof(NoisePrepDesc));
+    b->off_tm = b->off_win + align256(K * sizeof(RolloutWinArgs));
+    b->off_cvar = b->off_tm + align256(K * sizeof(b200mppi_planner::tmaps));
+    b->off_upd = b->off_cvar + align256(K * sizeof(CvarDesc));
+  } else {
+    b->off_sample = align256(K * sizeof(NoiseDesc));
+    b->off_roll = b->off_sample + align256(K * sizeof(SampleGridsV2Args));
+    b->off_upd = b->off_roll + align256(K * sizeof(RolloutArgs));
+  }
   b->desc_bytes = b->off_upd + align256(K * sizeof(UpdateBatchDesc));
   CU(cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
   b->own_stream = true;
@@ -1808,6 +1842,58 @@ extern "C" int b200mppi_batch_create(b200mppi_planner* const* planners, int32_t 
   b->pl.assign(planners, planners + count);
   b->device = planners[0]->cfg.device; b->mode = planners[0]->cfg.mode;
   b->T = planners[0]->T; b->N = planners[0]->n_local;
+  const int rc = batch_init(b);
+  if (rc) {
+    const std::string keep = g_err;
+    b200mppi_batch_destroy(b);
+    g_err = keep;
+    return rc;
+  }
+  *out = b;
+  return B200MPPI_OK;
+}
+
+// K independent MODE_TDM planners of equal N, T and M solved with one launch per stage (noise + controls, windowed
+// rollout, CVaR, update); the map sampling stays per planner (each planner's reach box is its own).  The results are
+// those of K solve() calls in planner order, bit for bit (include/b200mppi.h).
+extern "C" int b200mppi_batch_create_stochastic(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out) {
+  if (!planners || !out) return fail(B200MPPI_EINVAL, "batch_create_stochastic: null argument");
+  if (count < 1) return fail(B200MPPI_EINVAL, "batch_create_stochastic: count < 1");
+  if (count > 65535) return fail(B200MPPI_EINVAL, "batch_create_stochastic: more than 65535 planners");
+  for (int i = 0; i < count; ++i) {
+    const b200mppi_planner* p = planners[i];
+    const std::string who = "batch_create_stochastic: planner " + std::to_string(i);
+    if (!p) return fail(B200MPPI_EINVAL, who + " is null");
+    for (int j = 0; j < i; ++j)
+      if (planners[j] == p) return fail(B200MPPI_EINVAL, who + " is planner " + std::to_string(j) + " again");
+    if (p->cfg.mode != B200MPPI_MODE_TDM)
+      return fail(B200MPPI_EINVAL, who + " has mode " + std::to_string(p->cfg.mode) +
+                                       " (a stochastic batch holds MODE_TDM planners)");
+    if (p->cfg.world_size != 1)
+      return fail(B200MPPI_EINVAL, who + " has world_size " + std::to_string(p->cfg.world_size) +
+                                       " (a batch holds single-rank planners)");
+    const b200mppi_planner* q = planners[0];
+    if (p->cfg.device != q->cfg.device)
+      return fail(B200MPPI_EINVAL, who + " is on device " + std::to_string(p->cfg.device) + ", planner 0 on device " +
+                                       std::to_string(q->cfg.device));
+    if (p->T != q->T) return fail(B200MPPI_EINVAL, who + " has num_steps " + std::to_string(p->T) + ", planner 0 " +
+                                                      std::to_string(q->T) + " (T must be equal)");
+    if (p->n_local != q->n_local)
+      return fail(B200MPPI_EINVAL, who + " has num_control_rollouts " + std::to_string(p->n_local) + ", planner 0 " +
+                                       std::to_string(q->n_local) + " (N must be equal)");
+    if (p->M != q->M)
+      return fail(B200MPPI_EINVAL, who + " has num_grid_samples " + std::to_string(p->M) + ", planner 0 " +
+                                       std::to_string(q->M) + " (M must be equal)");
+    if (p->M > cvar_warp_max_maps())
+      return fail(B200MPPI_EINVAL, who + " has num_grid_samples " + std::to_string(p->M) + " (a stochastic batch takes " +
+                                       "at most " + std::to_string(cvar_warp_max_maps()) + " maps)");
+  }
+  CU(cudaSetDevice(planners[0]->cfg.device));
+  b200mppi_batch* b = new b200mppi_batch();
+  b->pl.assign(planners, planners + count);
+  b->device = planners[0]->cfg.device; b->mode = B200MPPI_MODE_TDM;
+  b->T = planners[0]->T; b->N = planners[0]->n_local; b->M = planners[0]->M;
+  b->stochastic = true;
   const int rc = batch_init(b);
   if (rc) {
     const std::string keep = g_err;
@@ -1904,22 +1990,30 @@ static int batch_run_sample(b200mppi_batch* b, const SampleGridsV2Args* h_sg, co
   return B200MPPI_OK;
 }
 
+// start after everything already issued on the members' streams (idle streams need no event)
+static int batch_wait_members(b200mppi_batch* b) {
+  for (b200mppi_planner* p : b->pl) {
+    if (p->stream == b->stream) continue;
+    const cudaError_t q = cudaStreamQuery(p->stream);
+    if (q == cudaSuccess) continue;
+    if (q != cudaErrorNotReady) CU(q);
+    CU(cudaEventRecord(b->ev, p->stream));
+    CU(cudaStreamWaitEvent(b->stream, b->ev, 0));
+  }
+  return B200MPPI_OK;
+}
+
+static int batch_solve_stochastic(b200mppi_batch* b, float* u_out);
+
 extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  if (b->stochastic) return batch_solve_stochastic(b, u_out);
   int rc = batch_validate(b);
   if (rc) return rc;
   CU(cudaSetDevice(b->device));
   const int K = (int)b->pl.size(), T = b->T;
   cudaStream_t st = b->stream;
-  // start after everything already issued on the members' streams (idle streams need no event)
-  for (b200mppi_planner* p : b->pl) {
-    if (p->stream == st) continue;
-    const cudaError_t q = cudaStreamQuery(p->stream);
-    if (q == cudaSuccess) continue;
-    if (q != cudaErrorNotReady) CU(q);
-    CU(cudaEventRecord(b->ev, p->stream));
-    CU(cudaStreamWaitEvent(st, b->ev, 0));
-  }
+  if ((rc = batch_wait_members(b))) return rc;
   // descriptors, built on the host for this solve and uploaded with ONE copy before the first launch (the sampler's
   // are decided here too: its host-side preparation may synchronise the stream)
   NoiseDesc* hn = reinterpret_cast<NoiseDesc*>(b->h_desc);
@@ -1976,6 +2070,123 @@ extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
   return B200MPPI_OK;
 }
 
+// The stochastic batch's solve: per iteration ONE noise + controls launch, [first iteration: every planner's map
+// sampling, in planner order, with the decisions of stage_sample_tdms], ONE windowed rollout launch over all (planner,
+// map) units, ONE CVaR launch and ONE update launch.  The reach statistics of all planners are read back behind one
+// event, so the host waits once.
+static int batch_solve_stochastic(b200mppi_batch* b, float* u_out) {
+  int rc = batch_validate(b);
+  if (rc) return rc;
+  const int K = (int)b->pl.size(), T = b->T, N = b->N;
+  int WW, WH; size_t smem;
+  rollout_win_geometry(T, &WW, &WH, &smem);
+  WH = rollout_win_batch_height(T);
+  CU(cudaSetDevice(b->device));
+  for (int i = 0; i < K; ++i) {
+    b200mppi_planner* p = b->pl[i];
+    const std::string who = "batch_solve: planner " + std::to_string(i);
+    // the generic rollout kernel's costs differ from the windowed kernel's in the last bit: no stand-in
+    if (!planner_uses_window(p))
+      return fail(B200MPPI_EINVAL, who + " does not take the windowed rollout kernel (B200MPPI_NO_WINDOW is set or its "
+                                         "window does not fit shared memory)");
+    if (!planner_tensor_maps(p, WW, WH))
+      return fail(B200MPPI_EINVAL, who + ": the tensor maps of its sampled maps / masks could not be encoded");
+  }
+  cudaStream_t st = b->stream;
+  if ((rc = batch_wait_members(b))) return rc;
+  NoisePrepDesc* hn = reinterpret_cast<NoisePrepDesc*>(b->h_desc);
+  RolloutWinArgs* hw = reinterpret_cast<RolloutWinArgs*>(b->h_desc + b->off_win);
+  unsigned char* ht = b->h_desc + b->off_tm;
+  CvarDesc* hc = reinterpret_cast<CvarDesc*>(b->h_desc + b->off_cvar);
+  UpdateBatchDesc* hu = reinterpret_cast<UpdateBatchDesc*>(b->h_desc + b->off_upd);
+  bool masks01 = true;
+  for (int i = 0; i < K; ++i) {
+    b200mppi_planner* p = b->pl[i];
+    const b200mppi_params& q = p->prm;
+    hn[i] = NoisePrepDesc{p->states, p->noise, p->u_cur, p->noiseT, p->ctrl, p->reach_d, p->reach_slot ^ 1,
+                          q.u_std[0], q.u_std[1], q.lambda_weight, q.u_std[0] * q.u_std[0], q.u_std[1] * q.u_std[1],
+                          q.vrange[0], q.vrange[1], q.wrange[0], q.wrange[1]};
+    hw[i] = RolloutWinArgs{};
+    fill_rollout_params(p, hw[i].p);
+    fill_win_args(p, WW, WH, hw[i]);
+    fill_cost_dst(p, hw[i].dst, false);
+    masks01 = masks01 && hw[i].masks01;
+    std::memcpy(ht + (size_t)i * sizeof(b200mppi_planner::tmaps), p->tmaps, sizeof(b200mppi_planner::tmaps));
+    hc[i] = CvarDesc{p->costs_nm, p->costs, p->n_local, p->n_local, p->M, cvar_numel(p->M, q.cvar_alpha)};
+    fill_update_args(p, hu[i].a, nullptr);
+    hu[i].tl = UpdateTail{};
+    hu[i].tl.counter = p->upd_counter_d;
+    hu[i].tl.mode = UPD_TAIL_APPLY;
+    hu[i].tl.u_out = b->u_d + (size_t)i * T * 2;        // u_prev stays null: a stochastic solve does not alias it
+  }
+  // the sampler plans (their host preparation may synchronise the stream) before the one upload
+  std::vector<SamplePlan> plans(K);
+  for (int i = 0; i < K; ++i)
+    if ((rc = plan_sampling(b->pl[i]->lin, b->pl[i]->ang, sample_alpha(b->pl[i]), st, &plans[i]))) return rc;
+  CU(cudaMemcpyAsync(b->d_desc, b->h_desc, b->desc_bytes, cudaMemcpyHostToDevice, st));
+  const NoisePrepDesc* dn = reinterpret_cast<const NoisePrepDesc*>(b->d_desc);
+  const RolloutWinArgs* dw = reinterpret_cast<const RolloutWinArgs*>(b->d_desc + b->off_win);
+  const void* dt = b->d_desc + b->off_tm;
+  const CvarDesc* dc = reinterpret_cast<const CvarDesc*>(b->d_desc + b->off_cvar);
+  const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(b->d_desc + b->off_upd);
+  const int num_opt = b->pl[0]->prm.num_opt;
+  if (num_opt <= 0) {                                  // the reference samples before its (empty) loop; u unchanged
+    for (int i = 0; i < K; ++i) {
+      if ((rc = sample_finish(b->pl[i], plans[i], nullptr, false, st, &b->launches))) return rc;
+      CU(cudaMemcpyAsync(b->u_d + (size_t)i * T * 2, b->pl[i]->u_cur, (size_t)T * 2 * sizeof(float),
+                         cudaMemcpyDeviceToDevice, st));
+    }
+  }
+  for (int k = 0; k < num_opt; ++k) {
+    launch_noise_prepare_batch(dn, K, N, T, b->pl[0]->npad, k, st);
+    b->launches++;
+    CHECK_LAUNCH();
+    for (b200mppi_planner* p : b->pl) {                // stage_noise
+      p->reach_slot ^= 1;
+      p->prepared = true;
+      p->reach_valid = true;
+    }
+    if (k == 0) {                                      // stage_sample_tdms of every planner, one host wait
+      std::vector<char> reads(K), advanced(K);
+      bool any = false;
+      for (int i = 0; i < K; ++i) {
+        b200mppi_planner* p = b->pl[i];
+        if (!(reads[i] = sample_reads_reach(p))) continue;
+        CU(cudaMemcpyAsync(sample_reach_host(p), p->reach_d + p->reach_slot, sizeof(float), cudaMemcpyDeviceToHost, st));
+        any = true;
+      }
+      if (any) CU(cudaEventRecord(b->ev, st));
+      for (int i = 0; i < K; ++i) {
+        if (!reads[i] || !plans[i].fused) continue;
+        launch_plan_advance(plans[i], 0, st);
+        CHECK_LAUNCH();
+        b->launches++;
+        advanced[i] = 1;
+      }
+      if (any) CU(cudaEventSynchronize(b->ev));
+      for (int i = 0; i < K; ++i) {
+        b200mppi_planner* p = b->pl[i];
+        if ((rc = sample_finish(p, plans[i], reads[i] ? sample_reach_host(p) : nullptr, advanced[i] != 0, st,
+                                &b->launches)))
+          return rc;
+      }
+    }
+    CU(launch_rollout_win_batch(hw[0], dw, dt, K, masks01, st));
+    b->launches++;
+    for (b200mppi_planner* p : b->pl) { p->prepared = false; p->pushed_direct = false; }
+    launch_cvar_batch(dc, K, N, b->M, st);
+    b->launches++;
+    CHECK_LAUNCH();
+    launch_update_partial_batch(du, K, b->pl[0]->num_ctas, nullptr, st);
+    b->launches++;
+    CHECK_LAUNCH();
+  }
+  CU(cudaMemcpyAsync(b->h_u, b->u_d, (size_t)K * T * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (u_out) std::memcpy(u_out, b->h_u, (size_t)K * T * 2 * sizeof(float));
+  return B200MPPI_OK;
+}
+
 // --------------------------------------------------------------------------------------------- closed-loop trials
 // A batch's planners run whole receding-horizon episodes on the device.  Only x0 (written by the plant kernel into the
 // rollout descriptors) and the parity of the TDMs' generator-state double buffers change from step to step: every
@@ -2013,6 +2224,9 @@ extern "C" int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial
                                          double* xhist, float* uhist, b200mppi_trial_result* results,
                                          int32_t* steps_issued) {
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  if (b->stochastic)
+    return fail(B200MPPI_EINVAL, "run_trials: planner 0 is MODE_TDM (trials run det-dynamics or speed-map batches: a "
+                                 "stochastic solve sizes each planner's map-sampling box on the host)");
   int rc = trial_validate(b, trials, max_steps);
   if (rc) return rc;
   if (!xhist || !uhist || !results) return fail(B200MPPI_EINVAL, "run_trials: null output buffer");

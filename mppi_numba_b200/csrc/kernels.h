@@ -168,6 +168,21 @@ void launch_prepare_rollout(const float* noise, const float* u_cur, float* noise
 void launch_noise_prepare(uint64_t* states, float* noise, const float* u_cur, float* noiseT, float* ctrl, float* reach,
                           int slot, int N, int T, int npad, float lambda, float std_v, float std_w, const float vrange[2],
                           const float wrange[2], cudaStream_t st);
+// batched stochastic solves: one noise + prepare launch for `count` planners of equal N, T (planner = blockIdx.y)
+// [emu:begin noise_prep_desc]
+struct NoisePrepDesc {
+  uint64_t* states;         // (N*T, 2)
+  float* noise;             // (N, T, 2)
+  const float* u_cur;       // (T, 2)
+  float* noiseT;            // [T + 1][npad] double2
+  float* ctrl;              // [npad]
+  float* reach;             // the planner's two reach slots
+  int slot;                 // slot of the solve's first iteration
+  float std_v, std_w, lambda, sv2, sw2, v_lo, v_hi, w_lo, w_hi;
+};
+// [emu:end noise_prep_desc]
+void launch_noise_prepare_batch(const NoisePrepDesc* descs, int count, int N, int T, int npad, int iter,
+                                cudaStream_t st);
 bool make_u8_tensor_map(void* out_map, const void* base, int rank, int cols, int rows, int maps, int pitch,
                         int WW, int WH);
 void rollout_win_geometry(int T, int* WW, int* WH, size_t* smem);
@@ -175,6 +190,13 @@ int device_sm_count();                          // SMs of the current device (ca
 void rollout_win_set_debug(long long* dev);    // device buffer of 4 int64 per CTA (<= 1024 CTAs) or null
 cudaError_t launch_rollout_win(const RolloutWinArgs& a, const void* tm_lin, const void* tm_ang, const void* tm_obs,
                                const void* tm_unk, cudaStream_t st);
+// batched stochastic solves: the window height of a batched launch (its shared memory also holds one planner record)
+int rollout_win_batch_height(int T);
+// ONE persistent launch over the (planner, map) units of `count` planners of equal N, M, T: g = the launch-wide fields
+// (p.N, p.M, p.T, npad, WH), descs = device array of each planner's own RolloutWinArgs, tmaps = device array (64-byte
+// aligned) of 4 encoded tensor maps per planner (lin, ang, obstacle, unknown); masks01: every planner's masks are 0/1
+cudaError_t launch_rollout_win_batch(const RolloutWinArgs& g, const RolloutWinArgs* descs, const void* tmaps, int count,
+                                     bool masks01, cudaStream_t st);
 // CVaR over M (mppi.py:718-755): costs[n] = mean of the ceil(M*alpha) largest of costs_mn[:, n]
 // costs_mn is map-major: (M, n_cnt) with row stride ld -- the local buffer of a one-rank solve, or the receive buffer
 // of a map-sharded solve (rows g*M/ws .. = rank g's maps): the same kernel, the same values per lane, hence
@@ -183,6 +205,17 @@ int cvar_max_maps();   // largest M the CVaR kernels accept
 // fw: flags to wait for before the costs are read (sharded solve, peer-memory exchange); FlagWait{} = none
 void launch_cvar(const float* costs_mn, float* costs, int n_cnt, int ld, int M, float cvar_alpha, const FlagWait& fw,
                  cudaStream_t st);
+int cvar_warp_max_maps();   // largest M of the warp kernel (the one the batched launch runs)
+// batched stochastic solves: one warp-kernel launch for `count` planners of equal n_cnt and M (planner = blockIdx.y)
+// [emu:begin cvar_desc]
+struct CvarDesc {
+  const float* costs_mn;    // map-major (M, ld)
+  float* costs;             // (n_cnt)
+  int n_cnt, ld, M, numel;  // numel = ceil(M * cvar_alpha) clamped to [1, M], as launch_cvar computes it
+};
+// [emu:end cvar_desc]
+int cvar_numel(int M, float cvar_alpha);
+void launch_cvar_batch(const CvarDesc* descs, int count, int n_cnt, int M, cudaStream_t st);
 
 // update_useq_numba (mppi.py:1113-1191) as an online-softmax two-level reduction
 // [emu:begin update_args]

@@ -266,11 +266,9 @@ __host__ __device__ inline int cvar_block_n(int M) {
 // PER = values held per lane (compile time: the select loop is fully unrolled over them); value j = map j sits in
 // slot j / 32 of lane j % 32 whatever the number of ranks the maps came from.
 template <int PER>
-__global__ void __launch_bounds__(CVAR_THREADS) cvar_kernel(const float* __restrict__ costs_mn,
-                                                            float* __restrict__ costs, int n_cnt, int ld, int M, int numel,
-                                                            const FlagWait fw) {
+__device__ __forceinline__ void cvar_body(const float* __restrict__ costs_mn, float* __restrict__ costs, int n_cnt, int ld,
+                                          int M, int numel) {
   __shared__ float s_tile[CVAR_TILE_FLOATS];
-  flag_wait(fw);                                              // sharded solve: the peers' costs have arrived
   const int NB = cvar_block_n(M);
   const int n0 = blockIdx.x * NB;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -332,6 +330,14 @@ __global__ void __launch_bounds__(CVAR_THREADS) cvar_kernel(const float* __restr
   }
 }
 
+template <int PER>
+__global__ void __launch_bounds__(CVAR_THREADS) cvar_kernel(const float* __restrict__ costs_mn,
+                                                            float* __restrict__ costs, int n_cnt, int ld, int M, int numel,
+                                                            const FlagWait fw) {
+  flag_wait(fw);                                              // sharded solve: the peers' costs have arrived
+  cvar_body<PER>(costs_mn, costs, n_cnt, ld, M, numel);
+}
+
 // M > 1024 (the reference switches to rollout_oversized_numba, mppi.py:199-203, 760-913, whose "sort" swaps
 // unconditionally, so only its alpha = 1 mean is meaningful; this kernel computes the INTENDED statistic, the
 // mean of the ceil(M*alpha) largest costs, for any M that fits shared memory).  One CTA per control
@@ -384,13 +390,39 @@ __global__ void __launch_bounds__(CVAR_LARGE_THREADS) cvar_large_kernel(const fl
 }
 
 // [emu:end cvar]
+// batched stochastic solves: planner blockIdx.y; every planner has the batch's n_cnt and M (hence PER and the grid)
+// [emu:begin cvar_batch]
+template <int PER>
+__global__ void __launch_bounds__(CVAR_THREADS) cvar_batch_kernel(const CvarDesc* __restrict__ descs) {
+  const CvarDesc& d = descs[blockIdx.y];
+  cvar_body<PER>(d.costs_mn, d.costs, d.n_cnt, d.ld, d.M, d.numel);
+}
+// [emu:end cvar_batch]
 int cvar_max_maps() { return CVAR_LARGE_MAX_MAPS; }
+int cvar_warp_max_maps() { return 32 * CVAR_MAX_PER_LANE; }
 
-void launch_cvar(const float* costs_mn, float* costs, int n_cnt, int ld, int M, float cvar_alpha, const FlagWait& fw,
-                 cudaStream_t st) {
+int cvar_numel(int M, float cvar_alpha) {
   int numel = (int)ceil((double)M * (double)cvar_alpha);    // mppi.py:744 (float32 alpha, f64 product)
   if (numel < 1) numel = 1;
   if (numel > M) numel = M;
+  return numel;
+}
+
+void launch_cvar_batch(const CvarDesc* descs, int count, int n_cnt, int M, cudaStream_t st) {
+  const int nb = cvar_block_n(M);
+  const dim3 grid((unsigned)((n_cnt + nb - 1) / nb), (unsigned)count);
+  const int per = (M + 31) / 32;
+  if (per <= 1) cvar_batch_kernel<1><<<grid, CVAR_THREADS, 0, st>>>(descs);
+  else if (per <= 2) cvar_batch_kernel<2><<<grid, CVAR_THREADS, 0, st>>>(descs);
+  else if (per <= 4) cvar_batch_kernel<4><<<grid, CVAR_THREADS, 0, st>>>(descs);
+  else if (per <= 8) cvar_batch_kernel<8><<<grid, CVAR_THREADS, 0, st>>>(descs);
+  else if (per <= 16) cvar_batch_kernel<16><<<grid, CVAR_THREADS, 0, st>>>(descs);
+  else cvar_batch_kernel<32><<<grid, CVAR_THREADS, 0, st>>>(descs);
+}
+
+void launch_cvar(const float* costs_mn, float* costs, int n_cnt, int ld, int M, float cvar_alpha, const FlagWait& fw,
+                 cudaStream_t st) {
+  const int numel = cvar_numel(M, cvar_alpha);
   if (M > 32 * CVAR_MAX_PER_LANE) {
     const size_t smem = (size_t)M * sizeof(uint32_t);
     cudaFuncSetAttribute(cvar_large_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,   // per device

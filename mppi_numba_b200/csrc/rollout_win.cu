@@ -105,12 +105,11 @@ __global__ void __launch_bounds__(256) prepare_rollout_kernel(const float2* __re
 // [emu:begin noise_prepare]
 constexpr int NP_NB = 8;            // control sequences per CTA: 1024 CTAs of 8 x 32 threads at config 5 (occupancy; the
                                     // Box-Muller chains are long and latency-bound)
-__global__ void __launch_bounds__(256) noise_prepare_kernel(uint64_t* __restrict__ states, float2* __restrict__ noise,
-                                                            const float* __restrict__ u_cur, double2* __restrict__ noiseT,
-                                                            float* __restrict__ ctrl, float* __restrict__ reach, int slot,
-                                                            int N, int T, int npad, float std_v, float std_w, float lambda,
-                                                            float sv2, float sw2, float v_lo, float v_hi, float w_lo,
-                                                            float w_hi) {
+__device__ __forceinline__ void noise_prepare_body(uint64_t* __restrict__ states, float2* __restrict__ noise,
+                                                   const float* __restrict__ u_cur, double2* __restrict__ noiseT,
+                                                   float* __restrict__ ctrl, float* __restrict__ reach, int slot, int N,
+                                                   int T, int npad, float std_v, float std_w, float lambda, float sv2,
+                                                   float sw2, float v_lo, float v_hi, float w_lo, float w_hi) {
   __shared__ float2 tile[NP_NB][33];
   const int n0 = blockIdx.x * NP_NB;
   const int tx = threadIdx.x & 31, r = threadIdx.x >> 5;       // generation: row r = control sequence, lane = time step
@@ -167,7 +166,29 @@ __global__ void __launch_bounds__(256) noise_prepare_kernel(uint64_t* __restrict
   }
 }
 
+__global__ void __launch_bounds__(256) noise_prepare_kernel(uint64_t* __restrict__ states, float2* __restrict__ noise,
+                                                            const float* __restrict__ u_cur, double2* __restrict__ noiseT,
+                                                            float* __restrict__ ctrl, float* __restrict__ reach, int slot,
+                                                            int N, int T, int npad, float std_v, float std_w, float lambda,
+                                                            float sv2, float sw2, float v_lo, float v_hi, float w_lo,
+                                                            float w_hi) {
+  noise_prepare_body(states, noise, u_cur, noiseT, ctrl, reach, slot, N, T, npad, std_v, std_w, lambda, sv2, sw2, v_lo,
+                     v_hi, w_lo, w_hi);
+}
+
 // [emu:end noise_prepare]
+// batched stochastic solves: planner blockIdx.y, its buffers and scalars from the descriptor array; N, T and npad are
+// the batch's.  Iteration `iter` of a solve uses reach slot d.slot ^ (iter & 1): each planner's slot toggles once per
+// iteration, as in its own solve()
+// [emu:begin noise_prepare_batch]
+__global__ void __launch_bounds__(256) noise_prepare_batch_kernel(const NoisePrepDesc* __restrict__ descs, int N, int T,
+                                                                  int npad, int iter) {
+  const NoisePrepDesc& d = descs[blockIdx.y];
+  noise_prepare_body(d.states, reinterpret_cast<float2*>(d.noise), d.u_cur, reinterpret_cast<double2*>(d.noiseT), d.ctrl,
+                     d.reach, d.slot ^ (iter & 1), N, T, npad, d.std_v, d.std_w, d.lambda, d.sv2, d.sw2, d.v_lo, d.v_hi,
+                     d.w_lo, d.w_hi);
+}
+// [emu:end noise_prepare_batch]
 void launch_noise_prepare(uint64_t* states, float* noise, const float* u_cur, float* noiseT, float* ctrl, float* reach,
                           int slot, int N, int T, int npad, float lambda, float std_v, float std_w, const float vrange[2],
                           const float wrange[2], cudaStream_t st) {
@@ -175,6 +196,10 @@ void launch_noise_prepare(uint64_t* states, float* noise, const float* u_cur, fl
                                                  reinterpret_cast<double2*>(noiseT), ctrl, reach, slot, N, T, npad, std_v,
                                                  std_w, lambda, std_v * std_v, std_w * std_w, vrange[0], vrange[1],
                                                  wrange[0], wrange[1]);
+}
+void launch_noise_prepare_batch(const NoisePrepDesc* descs, int count, int N, int T, int npad, int iter,
+                                cudaStream_t st) {
+  noise_prepare_batch_kernel<<<dim3((unsigned)(npad / NP_NB), (unsigned)count), 256, 0, st>>>(descs, N, T, npad, iter);
 }
 void launch_prepare_rollout(const float* noise, const float* u_cur, float* noiseT, float* ctrl, float* reach, int N,
                             int T, int npad, float lambda, float std_v, float std_w, const float vrange[2],
@@ -363,17 +388,25 @@ constexpr int WIN_WW = 240;       // window width in cells (inner TMA box extent
 #endif
 // MASK01: every byte of the obstacle / unknown masks is 0 or 1 (checked on the host when they are set): the penalty of a
 // step is then two additions of `c` or +0.0 (selected by an integer multiply) instead of the general multiply-adds
-template <int THREADS, int WH, bool MASK01>
-__global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWinArgs a,
-                                                                 const __grid_constant__ CUtensorMap tm_lin,
-                                                                 const __grid_constant__ CUtensorMap tm_ang,
-                                                                 const __grid_constant__ CUtensorMap tm_obs,
-                                                                 const __grid_constant__ CUtensorMap tm_unk) {
+//
+// BATCH (batched stochastic solves, rollout_win_batch_kernel): the work list is the planner-major, then map-major
+// sequence of chunks over the count * M (planner, map) units, and the share logic above reads "map" as "unit".  `g` holds
+// the launch-wide fields (p.N, p.M, p.T, npad and the share settings); whenever a CTA reaches a unit of another planner it
+// copies that planner's RolloutWinArgs from `descs` into shared memory behind the window (per-step scalars are then
+// shared-memory loads, never global ones) and rebuilds the traction tables, s_u and the derived registers from it.
+// Single launch: `g` is the planner's own RolloutWinArgs and the tensor maps are kernel parameters.
+template <int THREADS, int WH, bool MASK01, bool BATCH>
+__device__ __forceinline__ void rollout_win_body(const RolloutWinArgs& g, const CUtensorMap* tm_lin,
+                                                 const CUtensorMap* tm_ang, const CUtensorMap* tm_obs,
+                                                 const CUtensorMap* tm_unk, const RolloutWinArgs* descs,
+                                                 const CUtensorMap* tmaps, int count) {
   extern __shared__ __align__(128) unsigned char smem[];
-  const RolloutParams& p = a.p;
   constexpr int WW = WIN_WW;
   constexpr int PLANE = WW * WH;
-  const WinSmem L = win_smem_layout(WW, WH, p.T);
+  const WinSmem L = win_smem_layout(WW, WH, g.p.T);
+  RolloutWinArgs* s_rec = reinterpret_cast<RolloutWinArgs*>(smem + L.total);     // BATCH: the current planner's record
+  const RolloutWinArgs& a = BATCH ? *s_rec : g;
+  const RolloutParams& p = a.p;
   double* s_lutL = reinterpret_cast<double*>(smem + L.off_lut);
   double* s_lutA = s_lutL + 256;
   float* s_u = reinterpret_cast<float*>(smem + L.off_u);
@@ -381,8 +414,9 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
   int* s_next = reinterpret_cast<int*>(bar + 1);             // chunk counter of the current map
 
   const int tid = threadIdx.x, lane = tid & 31;
-  const int cpm = a.npad >> 5;                               // chunks per map
-  const long long total = (long long)p.M * cpm;
+  const int cpm = g.npad >> 5;                               // chunks per map
+  const int units_n = BATCH ? count * g.p.M : g.p.M;         // maps, or (planner, map) units
+  const long long total = (long long)units_n * cpm;
   // share boundaries are multiples of a.unit chunks (32 = one chunk per warp of the CTA when the shares are long
   // enough: every map segment is then a whole number of passes and all warps reach the end-of-segment barrier
   // together, where chunk-granular shares leave warps parked at that barrier; 1 for short shares)
@@ -391,76 +425,104 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
   // or q + 1 of the CTAs (q = CTAs / maps) and its chunks are split evenly among them.  A share that crosses a map
   // boundary costs a second window and, worse, two partial passes (a handful of warps running alone twice).
   long long w_lo, w_hi;
-  if (a.unit == 0) {
-    const int G = (int)gridDim.x, b = ((int)blockIdx.x + a.rotate) % (int)gridDim.x, q = G / p.M, r = G - q * p.M;    // the first r maps get q + 1 CTAs
+  if (g.unit == 0) {
+    const int G = (int)gridDim.x, b = ((int)blockIdx.x + g.rotate) % (int)gridDim.x, q = G / units_n, r = G - q * units_n;    // the first r maps get q + 1 CTAs
     int m, j, k;
     if (b < r * (q + 1)) { m = b / (q + 1); j = b - m * (q + 1); k = q + 1; }
     else { const int b2 = b - r * (q + 1); m = r + b2 / q; j = b2 - (m - r) * q; k = q; }
     w_lo = (long long)m * cpm + (long long)cpm * j / k;
     w_hi = (long long)m * cpm + (long long)cpm * (j + 1) / k;
   } else {
-    const long long units = (total + a.unit - 1) / a.unit;
-    w_lo = min(total, units * blockIdx.x / gridDim.x * a.unit);
-    w_hi = min(total, units * (blockIdx.x + 1) / gridDim.x * a.unit);
+    const long long units = (total + g.unit - 1) / g.unit;
+    w_lo = min(total, units * blockIdx.x / gridDim.x * g.unit);
+    w_hi = min(total, units * (blockIdx.x + 1) / gridDim.x * g.unit);
   }
   if (tid == 0) {
     mbar_init(bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  // traction tables: (lo + ratio*q) * dt exactly as the reference evaluates it (fma.rn.f64, mul.f64)
-  const double dt64 = f2d(p.dt);
-  for (int i = tid; i < 256; i += THREADS) {
-    const double q = (double)(i - 128);
-    s_lutL[i] = fma(p.lin_ratio, q, f2d(p.lin_lo)) * dt64;
-    s_lutA[i] = fma(p.ang_ratio, q, f2d(p.ang_lo)) * dt64;
-  }
-  for (int i = tid; i < 2 * p.T; i += THREADS) s_u[i] = a.u_cur[i];
-
-  uint32_t sb_win = smem_u32(smem);
-  uint32_t sb_lutL = smem_u32(s_lutL) + 128 * 8;     // index by the signed int8 value directly
-  uint32_t sb_lutA = smem_u32(s_lutA) + 128 * 8;
-  uint32_t sb_u = smem_u32(s_u);
-  // keep the shared-window addresses in registers (opaque to the optimiser, which would otherwise
-  // re-derive them from SR_CgaCtaId with S2UR/ULEA inside the loop)
-  asm volatile("" : "+r"(sb_win), "+r"(sb_lutL), "+r"(sb_lutA), "+r"(sb_u));
-  const float xlo = p.g.xlo, ylo = p.g.ylo, res = p.g.res, inv_res = p.g.inv_res;
-  const float gx = p.xgoal[0], gy = p.xgoal[1];
+  uint32_t sb_win, sb_lutL, sb_lutA, sb_u;
+  float xlo, ylo, res, inv_res, gx, gy, inv_lo, inv_hi;
+  int magic_wx, magic_wy;
+  unsigned uww, uwh;
   const float MAGIC = 12582912.0f;                          // 1.5 * 2^23
-  int magic_wx = 0x4B400000 + a.wx0, magic_wy = 0x4B400000 + a.wy0;
-  asm volatile("" : "+r"(magic_wx), "+r"(magic_wy));       // keep the folded constants (else re-derived per step)
-  // interval half-width 2.4e-7 (relative): the exact quotient q = a/res satisfies |fl(a*fl(inv*(1-+d))) - q(1-+d)| <=
-  // 3 * 2^-24 |q| = 1.79e-7 |q| (roundings of 1/res, of the scaled reciprocal, of the FMA), so d = 2.4e-7 keeps q inside
-  // [lower end, upper end] with a third to spare; a wider interval only sends more steps to the exact sequence
-  float inv_lo = inv_res * (1.0f - 2.4e-7f), inv_hi = inv_res * (1.0f + 2.4e-7f);
-  keep_in_registers(inv_lo, inv_hi);                       // (else re-derived from inv_res on every step)
-  const unsigned uww = (unsigned)a.ww, uwh = (unsigned)a.wh;     // staged AND inside the map (<= WW, WH)
+  // everything the CTA derives from its planner's arguments (once; BATCH: at every planner switch)
+  auto stage_planner = [&]() {
+    // traction tables: (lo + ratio*q) * dt exactly as the reference evaluates it (fma.rn.f64, mul.f64)
+    const double dt64 = f2d(p.dt);
+    for (int i = tid; i < 256; i += THREADS) {
+      const double q = (double)(i - 128);
+      s_lutL[i] = fma(p.lin_ratio, q, f2d(p.lin_lo)) * dt64;
+      s_lutA[i] = fma(p.ang_ratio, q, f2d(p.ang_lo)) * dt64;
+    }
+    for (int i = tid; i < 2 * g.p.T; i += THREADS) s_u[i] = a.u_cur[i];
 
-  const long long dbg_t0 = WIN_DBG(a) ? (long long)globaltimer_ns() : 0;
+    sb_win = smem_u32(smem);
+    sb_lutL = smem_u32(s_lutL) + 128 * 8;     // index by the signed int8 value directly
+    sb_lutA = smem_u32(s_lutA) + 128 * 8;
+    sb_u = smem_u32(s_u);
+    // keep the shared-window addresses in registers (opaque to the optimiser, which would otherwise
+    // re-derive them from SR_CgaCtaId with S2UR/ULEA inside the loop)
+    asm volatile("" : "+r"(sb_win), "+r"(sb_lutL), "+r"(sb_lutA), "+r"(sb_u));
+    xlo = p.g.xlo; ylo = p.g.ylo; res = p.g.res; inv_res = p.g.inv_res;
+    gx = p.xgoal[0]; gy = p.xgoal[1];
+    magic_wx = 0x4B400000 + a.wx0; magic_wy = 0x4B400000 + a.wy0;
+    asm volatile("" : "+r"(magic_wx), "+r"(magic_wy));       // keep the folded constants (else re-derived per step)
+    // interval half-width 2.4e-7 (relative): the exact quotient q = a/res satisfies |fl(a*fl(inv*(1-+d))) - q(1-+d)| <=
+    // 3 * 2^-24 |q| = 1.79e-7 |q| (roundings of 1/res, of the scaled reciprocal, of the FMA), so d = 2.4e-7 keeps q
+    // inside [lower end, upper end] with a third to spare; a wider interval only sends more steps to the exact sequence
+    inv_lo = inv_res * (1.0f - 2.4e-7f); inv_hi = inv_res * (1.0f + 2.4e-7f);
+    keep_in_registers(inv_lo, inv_hi);                       // (else re-derived from inv_res on every step)
+    uww = (unsigned)a.ww; uwh = (unsigned)a.wh;              // staged AND inside the map (<= WW, WH)
+  };
+  int cur = -1;                                              // BATCH: the planner staged in s_rec
+  if (!BATCH) stage_planner();
+
+  const long long dbg_t0 = WIN_DBG(g) ? (long long)globaltimer_ns() : 0;
   uint32_t phase = 0;
   for (long long w = w_lo; w < w_hi;) {
-    const int m = (int)(w / cpm);
-    const int c_lo = (int)(w - (long long)m * cpm);
-    const int c_hi = (int)min((long long)cpm, w_hi - (long long)m * cpm);       // this map's part of the share
+    const int u = (int)(w / cpm);
+    const int m = BATCH ? u % g.p.M : u;
+    const int c_lo = (int)(w - (long long)u * cpm);
+    const int c_hi = (int)min((long long)cpm, w_hi - (long long)u * cpm);       // this map's part of the share
     w += c_hi - c_lo;
     __syncthreads();                                        // every warp has left the previous window (and the tables are written)
+    if constexpr (BATCH) {
+      const int k = u / g.p.M;                              // CTA-uniform
+      if (k != cur) {
+        cur = k;
+        const unsigned* src = reinterpret_cast<const unsigned*>(descs + k);
+        unsigned* dst = reinterpret_cast<unsigned*>(s_rec);
+        for (int i = tid; i < (int)(sizeof(RolloutWinArgs) / 4); i += THREADS) dst[i] = src[i];
+        tm_lin = tmaps + 4 * k; tm_ang = tm_lin + 1; tm_obs = tm_lin + 2; tm_unk = tm_lin + 3;
+        if (tid == 0) {
+          // tensor maps in global memory, written by a host copy: acquire them for the tensor-map proxy before use
+          // (CUDA Programming Guide, tensor maps passed in global memory)
+          for (int i = 0; i < 4; ++i)
+            asm volatile ("fence.proxy.tensormap::generic.acquire.sys [%0], 128;" ::"l"(tm_lin + i) : "memory");
+        }
+        __syncthreads();                                    // the record is in shared memory
+        stage_planner();                                    // the barrier after the TMA issue below publishes the tables
+      }
+    }
     if (tid == 0) {
       *s_next = c_lo;
       // order the CTA's generic-proxy reads of the previous window before the async-proxy writes of the next one
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       mbar_expect_tx(bar, 4u * (uint32_t)PLANE);
-      tma_load_3d(smem, &tm_lin, bar, a.wx0, a.wy0, m);
-      tma_load_3d(smem + PLANE, &tm_ang, bar, a.wx0, a.wy0, m);
-      tma_load_2d(smem + 2 * PLANE, &tm_obs, bar, a.wx0, a.wy0);
-      tma_load_2d(smem + 3 * PLANE, &tm_unk, bar, a.wx0, a.wy0);
+      tma_load_3d(smem, tm_lin, bar, a.wx0, a.wy0, m);
+      tma_load_3d(smem + PLANE, tm_ang, bar, a.wx0, a.wy0, m);
+      tma_load_2d(smem + 2 * PLANE, tm_obs, bar, a.wx0, a.wy0);
+      tma_load_2d(smem + 3 * PLANE, tm_unk, bar, a.wx0, a.wy0);
     }
     __syncthreads();                                        // s_next visible
     mbar_wait(bar, phase);
     phase ^= 1u;
     // the barrier above releases all 32 warps in lockstep: they would hit the XU / LSU / FP64 sections of the step
     // together, pass after pass.  Spread the warps of a scheduler over one step period (a.stagger cycles per slot)
-    if (a.stagger > 0) {
+    if (g.stagger > 0) {
       const long long t0 = clock64();
-      const long long wait = (long long)(tid >> 7) * a.stagger;
+      const long long wait = (long long)(tid >> 7) * g.stagger;
       while (clock64() - t0 < wait) { }
     }
     const int8_t* __restrict__ g_lin = a.lin_grid + (size_t)m * p.g.grid_rows * p.g.grid_pitch;
@@ -473,7 +535,7 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
     // ends with its low-priority warps running alone at a fraction of the issue rate.
     for (int pass = 0;; ++pass) {
       int c;
-      if (a.sync_passes) {
+      if (g.sync_passes) {
         if (c_lo + pass * (THREADS / 32) >= c_hi) break;    // CTA-uniform
         if (pass > 0) __syncthreads();
         c = c_lo + pass * (THREADS / 32) + (tid >> 5);
@@ -485,8 +547,8 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
       }
       const bool has = c < c_hi;                            // pass mode: no chunk left for this warp in the last pass
       const int n = has ? (c << 5) + lane : lane;
-      const bool live = has && n < p.N;                     // ragged last chunk (n is padded to whole warps): such lanes
-      const int Tn = live ? p.T : 0;                        // run zero steps and store nothing, but stay with their warp
+      const bool live = has && n < g.p.N;                   // ragged last chunk (n is padded to whole warps): such lanes
+      const int Tn = live ? g.p.T : 0;                      // run zero steps and store nothing, but stay with their warp
     const double2* __restrict__ ep = reinterpret_cast<const double2*>(a.noiseT) + n;
     float x = p.x0[0], y = p.x0[1], th = p.x0[2];
     // the float64 state is carried UNROUNDED across the back edge (rx, ry, rt: the float64 FMA results, initially the
@@ -497,7 +559,7 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
     double2 c2 = __ldg(ep);                                 // controls of step t (loaded during step t-1, see below)
     int t = 0;
     for (; t < Tn; ++t) {
-      ep += a.npad;
+      ep += g.npad;
       // ---- cell index of both axes: floor(a/res) by round-down magic-number addition on the FP32 pipe, taken
       //      at BOTH ends of an interval that contains the exact quotient a/res (relative half-width 2.4e-7,
       //      1.34x the worst accumulated rounding error, see inv_lo / inv_hi; the +-1e-30 covers a == 0 and flushed
@@ -518,10 +580,10 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
         const uint32_t ad = sb_win + (uint32_t)(wy * WW + wx);
         ql = lds_s8(ad, 0); qa = lds_s8(ad, PLANE); ob = lds_s8(ad, 2 * PLANE); un = lds_s8(ad, 3 * PLANE);
       } else {
-        if (WIN_DBG(a)) {                                   // debug hook: lane-steps on the slow path / outside the window
-          atomicAdd(reinterpret_cast<unsigned long long*>(a.dbg) + 6 * blockIdx.x + 4, 1ull);
+        if (WIN_DBG(g)) {                                   // debug hook: lane-steps on the slow path / outside the window
+          atomicAdd(reinterpret_cast<unsigned long long*>(g.dbg) + 6 * blockIdx.x + 4, 1ull);
           if (!(((unsigned)wx < uww) & ((unsigned)wy < uwh)))
-            atomicAdd(reinterpret_cast<unsigned long long*>(a.dbg) + 6 * blockIdx.x + 5, 1ull);
+            atomicAdd(reinterpret_cast<unsigned long long*>(g.dbg) + 6 * blockIdx.x + 5, 1ull);
         }
         const int pk = lookup_slow(ax, ay, res, inv_lo, inv_hi, sb_win, uww, uwh, WW, PLANE, a.wx0, a.wy0, p.g.rows, p.g.cols, p.g.grid_rows,
                                    p.g.grid_cols, p.g.grid_pitch, p.g.mask_pitch, g_lin, g_ang, a.obstacle, a.unknown);
@@ -561,9 +623,9 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
     }
     // the loop is left early exactly when d2 <= tol2 and otherwise ends with d2 > tol2 (d2 = 1e9 for T = 0), so the
     // reference's goal_reached flag is recovered from d2 -- no flag register (and no constant) inside the loop
-    if (WIN_DBG(a)) {                                       // debug hook: steps this warp ran for the chunk (its slowest lane)
+    if (WIN_DBG(g)) {                                       // debug hook: steps this warp ran for the chunk (its slowest lane)
       const int steps = __reduce_max_sync(0xffffffffu, t < Tn ? t + 1 : t);
-      if (lane == 0) atomicAdd(reinterpret_cast<unsigned long long*>(a.dbg) + 6 * blockIdx.x + 5, (unsigned long long)steps << 40);
+      if (lane == 0) atomicAdd(reinterpret_cast<unsigned long long*>(g.dbg) + 6 * blockIdx.x + 5, (unsigned long long)steps << 40);
     }
     const float not_reached = (d2 <= p.tol2) ? 0.0f : 1.0f;
     cost = fadd(cost, a.ctrl[n]);                                           // control cost (mppi.py:708-710)
@@ -572,34 +634,51 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
     if (live) *cost_ptr(a.dst, m, n) = cost;                // map-major: the warp's 32 lanes store one 128-byte line
     }
   }
-  if (WIN_DBG(a)) __syncthreads();                          // the CTA's end, not the end of thread 0's warp
-  if (WIN_DBG(a) && tid == 0) {                                // per-CTA wall time (tools/rollout_cta_times.py)
-    a.dbg[6 * blockIdx.x + 0] = dbg_t0;
-    a.dbg[6 * blockIdx.x + 1] = (long long)globaltimer_ns();
-    a.dbg[6 * blockIdx.x + 2] = w_lo | ((long long)sm_id() << 40);           // SM id in the upper bits
-    a.dbg[6 * blockIdx.x + 3] = w_hi;
+  if (WIN_DBG(g)) __syncthreads();                          // the CTA's end, not the end of thread 0's warp
+  if (WIN_DBG(g) && tid == 0) {                                // per-CTA wall time (tools/rollout_cta_times.py)
+    g.dbg[6 * blockIdx.x + 0] = dbg_t0;
+    g.dbg[6 * blockIdx.x + 1] = (long long)globaltimer_ns();
+    g.dbg[6 * blockIdx.x + 2] = w_lo | ((long long)sm_id() << 40);           // SM id in the upper bits
+    g.dbg[6 * blockIdx.x + 3] = w_hi;
   }
   // sharded solve, peer-memory exchange: the costs above went straight into the receive buffers of the ranks that
   // reduce them; the LAST CTA to get here raises this rank's epoch flag in every peer (p2p.cu has the protocol)
-  if (a.sig.ws > 0) {
+  if (g.sig.ws > 0) {
     // one fence per CTA: the barrier orders every thread's cost stores before thread 0, whose (cumulative) system-scope
     // fence then orders them before its ticket -- the pattern of a cooperative grid barrier.  (A fence by each of the
     // 1024 threads, as in the first version, is slower with stores in flight over NVLink.)
-    if (a.stagger == -1) __threadfence_system();            // A/B hook: the first version
+    if (g.stagger == -1) __threadfence_system();            // A/B hook: the first version
     __syncthreads();
     if (tid == 0) {
       __threadfence_system();
-      const unsigned prev = atomicAdd(a.sig.counter, 1u);
+      const unsigned prev = atomicAdd(g.sig.counter, 1u);
       if (prev == gridDim.x - 1) {
-        *a.sig.counter = 0;
+        *g.sig.counter = 0;
         __threadfence_system();
-        for (int q = 0; q < a.sig.ws; ++q) st_flag_sys(a.sig.peer_flags[q] + a.sig.rank, a.sig.epoch);
+        for (int q = 0; q < g.sig.ws; ++q) st_flag_sys(g.sig.peer_flags[q] + g.sig.rank, g.sig.epoch);
       }
     }
   }
 }
 
+template <int THREADS, int WH, bool MASK01>
+__global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWinArgs a,
+                                                                 const __grid_constant__ CUtensorMap tm_lin,
+                                                                 const __grid_constant__ CUtensorMap tm_ang,
+                                                                 const __grid_constant__ CUtensorMap tm_obs,
+                                                                 const __grid_constant__ CUtensorMap tm_unk) {
+  rollout_win_body<THREADS, WH, MASK01, false>(a, &tm_lin, &tm_ang, &tm_obs, &tm_unk, nullptr, nullptr, 1);
+}
+
 // [emu:end win_kernel]
+// [emu:begin win_batch]
+template <int THREADS, int WH, bool MASK01>
+__global__ void __launch_bounds__(THREADS, 1) rollout_win_batch_kernel(const RolloutWinArgs g,
+                                                                       const RolloutWinArgs* __restrict__ descs,
+                                                                       const CUtensorMap* __restrict__ tmaps, int count) {
+  rollout_win_body<THREADS, WH, MASK01, true>(g, nullptr, nullptr, nullptr, nullptr, descs, tmaps, count);
+}
+// [emu:end win_batch]
 // ---------------------------------------------------------------------------------------------
 // host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -736,6 +815,48 @@ cudaError_t launch_rollout_win(const RolloutWinArgs& a, const void* tm_lin, cons
   const CUtensorMap& t2 = *reinterpret_cast<const CUtensorMap*>(tm_obs);
   const CUtensorMap& t3 = *reinterpret_cast<const CUtensorMap*>(tm_unk);
   kernels[a.WH == 232 ? 0 : 1][a.masks01 ? 1 : 0]<<<grid, WIN_THREADS, L.total, st>>>(b, t0, t1, t2, t3);
+  return cudaGetLastError();
+}
+
+// the planner record the batched kernel keeps behind the window
+static size_t win_batch_smem(int WH, int T) {
+  return (size_t)win_smem_layout(WIN_WW, WH, T).total + sizeof(RolloutWinArgs);
+}
+
+int rollout_win_batch_height(int T) { return win_batch_smem(232, T) <= (size_t)WIN_MAX_SMEM ? 232 : 224; }
+
+// The launch-wide choices of launch_rollout_win (persistent CTAs, share unit) over units = count * M; its tuning hooks
+// (B200MPPI_WIN_*) and the debug hook are not applied to batched launches.
+cudaError_t launch_rollout_win_batch(const RolloutWinArgs& g, const RolloutWinArgs* descs, const void* tmaps, int count,
+                                     bool masks01, cudaStream_t st) {
+  typedef void (*WinBatchKernel)(const RolloutWinArgs, const RolloutWinArgs*, const CUtensorMap*, int);
+  static const WinBatchKernel kernels[2][2] = {
+      {rollout_win_batch_kernel<WIN_THREADS, 232, false>, rollout_win_batch_kernel<WIN_THREADS, 232, true>},
+      {rollout_win_batch_kernel<WIN_THREADS, 224, false>, rollout_win_batch_kernel<WIN_THREADS, 224, true>}};
+  {
+    static bool attr_set[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
+      for (int i = 0; i < 2; ++i)
+        for (int j = 0; j < 2; ++j) {
+          const cudaError_t e = cudaFuncSetAttribute(kernels[i][j], cudaFuncAttributeMaxDynamicSharedMemorySize, WIN_MAX_SMEM);
+          if (e != cudaSuccess) return e;
+        }
+      if (dev >= 0 && dev < 64) attr_set[dev] = true;
+    }
+  }
+  const size_t smem = win_batch_smem(g.WH, g.p.T);
+  if (g.WW != WIN_WW || (g.WH != 232 && g.WH != 224) || smem > (size_t)WIN_MAX_SMEM || count < 1) return cudaErrorInvalidValue;
+  const int units = count * g.p.M;
+  const long long total = (long long)units * (g.npad / 32);
+  const dim3 grid((unsigned)std::min<long long>(std::max<long long>(total / 8, 1), device_sm_count()));
+  RolloutWinArgs b = g;
+  b.unit = (total / (32LL * grid.x) >= 4) ? 32 : ((int)grid.x >= units ? 0 : 1);
+  b.sync_passes = (total + 32LL * grid.x - 1) / (32LL * grid.x) <= WIN_SYNC_MAX_PASSES;
+  b.stagger = WIN_STAGGER_DEFAULT; b.rotate = 0; b.dbg = nullptr; b.sig = CostSignal{};
+  kernels[g.WH == 232 ? 0 : 1][masks01 ? 1 : 0]<<<grid, WIN_THREADS, smem, st>>>(
+      b, descs, reinterpret_cast<const CUtensorMap*>(tmaps), count);
   return cudaGetLastError();
 }
 
