@@ -1,7 +1,11 @@
 #!/usr/bin/env python
-"""bench_trials.py -- closed-loop episodes of K one-map planners: the host-driven loop against MPPI_Batch.run_trials.
+"""bench_trials.py -- closed-loop episodes of K planners: the host-driven loop against the batch's device episodes.
 
-    python bench_trials.py --workload c2|c4 --batch K --closed-loop S [--rounds R]
+    python bench_trials.py --workload c2|c4|c3|ref --batch K --closed-loop S [--rounds R] [--profile]
+
+c2 and c4 are one-map workloads (MPPI_Batch.run_trials); c3 and ref are stochastic (use_tdm, CVaR cost:
+MPPI_StochasticBatch.run_stochastic_trials).  ref is the reference benchmark's noisy_dyn trial shape (N 1024, M 1024,
+T 100, a 9 x 9-cell map at 1 m), defined here: every reach box leaves that map, so every step samples whole maps.
 
 K planners of the workload (bench.py's WORKLOADS, seeds 1..K: different maps, start poses and warm starts), each with
 a seeded ground-truth TractionGrid over its map; every other planner has its goal 1.5 m away (reached within S steps),
@@ -9,9 +13,9 @@ the others the workload's distant goal (they run all S steps).  First the parity
 planners, and on identical twins the host loop replayed with the device's trajectory -- u[0] of every solve and the
 final planner state (u, u_prev, noise, costs, weights, RNG states, sampled maps, params['x0']) bit for bit; a mismatch
 exits non-zero.  Then R rounds of each, alternating, every round from the same start (params, warm start):
-  host: the best host loop available -- MPPI_Batch.solve() of all K, then per running planner a numpy plant step and
+  host: the best host loop available -- the batch's solve() of all K, then per running planner a numpy plant step and
         shift_and_update, until every planner has stopped;
-  device: one MPPI_Batch.run_trials(grids, S).
+  device: one run_trials(grids, S) (run_stochastic_trials for c3 and ref).
 Wall clock per round (each ends in a host synchronisation); control steps/s (planner-steps run), episodes/s, kernel
 launches per round.  Prints one JSON line with the card's name and power limit; writes nothing to the tree.
 """
@@ -30,6 +34,9 @@ if ROOT not in sys.path:
 
 from bench import WORKLOADS, make_planner, workload_name_of   # noqa: E402
 
+# the reference benchmark's noisy_dyn trial: N 1024, M 1024, T 100 on a 9 x 9-cell map at 1 m (c3's bins)
+LOCAL_WORKLOADS = {"ref": ("tdm", 1024, 1024, 100, 9, 1.0) + tuple(WORKLOADS["c3"][6:])}
+
 
 def run(args, emit):
     import torch
@@ -39,7 +46,10 @@ def run(args, emit):
     from tests.scenarios import make_scenario
     from tests.trial_loop import plant_step, within
     K, S = args.batch, args.closed_loop
-    mode, N, M, T, H, res, B, da = WORKLOADS[args.workload]
+    mode, N, M, T, H, res, B, da = LOCAL_WORKLOADS.get(args.workload) or WORKLOADS[args.workload]
+    stochastic = mode == "tdm"
+    Batch = E.MPPI_StochasticBatch if stochastic else E.MPPI_Batch
+    trials = (lambda b, g, s: b.run_stochastic_trials(g, s)) if stochastic else (lambda b, g, s: b.run_trials(g, s))
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     scs = []
@@ -58,21 +68,24 @@ def run(args, emit):
             p.u_cur_d.copy_to_device(sc["u0"])
 
     reset(A), reset(Bs)
-    ba, bb = E.MPPI_Batch(A), E.MPPI_Batch(Bs)
+    ba, bb = Batch(A), Batch(Bs)
 
-    # ---- parity: run_trials == the host loop replayed with the device's trajectory
-    out = ba.run_trials(grids, S)
+    # ---- parity: the device episodes == the host loop replayed with the device's trajectory
+    out = trials(ba, grids, S)
     ok_u = True
     for k, p in enumerate(Bs):
+        one = Batch([p])
         for t in range(int(out["steps"][k])):
-            useq = p.solve()
+            useq = one.solve()[0]
             ok_u &= bool(np.array_equal(useq[0], out["uhist"][k, t]))
             p.shift_and_update(out["xhist"][k, t + 1], useq, 1)
 
     def state(p):
         d = [p.u_cur_d, p.u_prev_d, p.costs_d, p.weights_d, p.noise_samples_d, p.rng_states_d, p.lin_tdm.rng_states_d,
              p.ang_tdm.rng_states_d, p.lin_tdm.sample_grid_batch_d, p.ang_tdm.sample_grid_batch_d]
-        return [a.copy_to_host() for a in d] + [p.params["x0"]]
+        if stochastic:
+            d.append(p.costs_nm_d)
+        return [a.copy_to_host() for a in d] + [p.params["x0"], np.asarray(p.sample_box())]
     ok_state = all(all(np.array_equal(x, y) for x, y in zip(state(a), state(b))) for a, b in zip(A, Bs))
     parity = {"passed": ok_u and ok_state, "u_bitwise": ok_u, "state_bitwise": ok_state, "planners": K,
               "steps": out["steps"].tolist(), "status": out["status"],
@@ -106,7 +119,7 @@ def run(args, emit):
 
     def device_round():
         reset(A)
-        o = ba.run_trials(grids, S)
+        o = trials(ba, grids, S)
         torch.cuda.synchronize(dev)
         return int(o["steps"].sum())
 
@@ -128,6 +141,17 @@ def run(args, emit):
                 "control_steps_per_s": res[name][0][1] / med, "episodes_per_s": K / med,
                 "kernel_launches_per_round": launches[name]}
     host, devr = summary("host"), summary("device")
+    split = None
+    if args.profile:                                     # a separate run: tracing slows the host
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            device_round()
+        split = {}
+        for ev in prof.key_averages():
+            if ev.device_type.name == "CUDA" and ev.count:
+                t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0.0)
+                split[ev.key] = {"ms": t / 1e3, "launches": ev.count}
+        split = dict(sorted(split.items(), key=lambda kv: -kv[1]["ms"]))
     gpu = {"name": torch.cuda.get_device_name(dev)}
     try:
         q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -135,12 +159,15 @@ def run(args, emit):
         gpu["power_limit_and_max_sm_clock"] = q
     except Exception as e:                               # noqa: BLE001
         gpu["power_limit_and_max_sm_clock"] = "unavailable (%r)" % e
-    emit(json.dumps({"metric": "closed-loop trials: host-driven loop vs MPPI_Batch.run_trials",
+    emit(json.dumps({"metric": "closed-loop trials: host-driven loop vs " +
+                     ("MPPI_StochasticBatch.run_stochastic_trials" if stochastic else "MPPI_Batch.run_trials"),
                      "unit": "episodes/s", "value": devr["episodes_per_s"], "higher_is_better": True,
-                     "config": {"workload": workload_name_of(args.workload), "batch": K, "max_steps": S,
+                     "config": {"workload": (args.workload if args.workload in LOCAL_WORKLOADS else
+                                             workload_name_of(args.workload)), "batch": K, "max_steps": S,
                                 "planners": "seeds 1..K, warm started; even k: goal 1.5 m away, odd k: distant goal"},
                      "rounds": args.rounds, "gpu": gpu, "parity_check": parity, "host": host, "device": devr,
-                     "speedup_wall": host["s_per_round_wall"] / devr["s_per_round_wall"]}))
+                     "speedup_wall": host["s_per_round_wall"] / devr["s_per_round_wall"],
+                     "device_kernel_split_one_round": split}))
 
 
 def main():
@@ -152,10 +179,11 @@ def main():
     def emit(line):
         os.write(real_stdout, (line + "\n").encode())
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[1])
-    ap.add_argument("--workload", default="c2", choices=["c2", "c4"])
+    ap.add_argument("--workload", default="c2", choices=["c2", "c4", "c3", "ref"])
     ap.add_argument("--batch", type=int, default=64, metavar="K", help="planners in the batch")
     ap.add_argument("--closed-loop", type=int, default=150, metavar="S", help="max control steps per episode")
     ap.add_argument("--rounds", type=int, default=3, help="timed rounds of each loop")
+    ap.add_argument("--profile", action="store_true", help="then one device round under torch.profiler: kernel split")
     args = ap.parse_args()
     if args.batch < 1 or args.closed_loop < 1 or args.rounds < 1:
         ap.error("--batch, --closed-loop and --rounds must be at least 1")

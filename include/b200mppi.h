@@ -329,7 +329,8 @@ int b200mppi_batch_launch_count(b200mppi_batch* b, int64_t* out);
  * of noise + controls, windowed rollout (all K*M (planner, map) units on the persistent grid), CVaR and update.  The map
  * sampling of the first iteration stays per planner (each planner's reach box is its own: 1 or 2 launches each), with
  * one host wait for all K reach statistics.  The result is a b200mppi_batch: batch_solve, set_stream, launch_count and
- * destroy work on it as above; b200mppi_batch_run_trials refuses it.
+ * destroy work on it as above; b200mppi_batch_run_trials refuses it (b200mppi_batch_run_stochastic_trials below runs
+ * its closed-loop trials).
  *   create: planners on one device, MODE_TDM, world_size 1, equal num_steps, num_control_rollouts and
  *           num_grid_samples (at most 1024), no planner listed twice.  Anything else: B200MPPI_EINVAL naming the planner.
  *   solve : == b200mppi_planner_solve on planners[0], planners[1], ... in that order, bit for bit: u, noise, per-(m, n)
@@ -378,6 +379,25 @@ typedef struct {
 } b200mppi_trial_result;
 int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps, double* xhist,
                               float* uhist, b200mppi_trial_result* results, int32_t* steps_issued);
+
+/* ------------------------------------------------------------------ closed-loop trials of a stochastic batch
+ * The same episodes, plant step, stop rules, descriptors and results as b200mppi_batch_run_trials, for a batch made by
+ * b200mppi_batch_create_stochastic (MODE_TDM, CVaR cost).  Each planner's map-sampling reach box is decided on the device
+ * by the function the host-side solve uses, from the pose the plant step wrote and the reach of the controls just drawn,
+ * so no step waits for the host.  Per step 4*num_opt + 3 launches for the whole batch: num_opt x (noise + controls,
+ * windowed rollout, CVaR, update), one boxed map sampling of every pair, one state advance of every pair and the plant
+ * step, which also moves each planner's rollout window.
+ * Afterwards every planner is exactly as `steps` rounds of batch_solve (b200mppi_batch_solve on this batch) -> plant step
+ * -> set_u(shifted u) -> set_params(x0 = float32(new pose)) would leave it, bit for bit: u, noise, per-(m, n) costs,
+ * costs, weights, the planners' and their TDMs' RNG states, the sampled maps, b200mppi_planner_sample_box and the host-side
+ * solve state; the C-side params keep the x0 of the last solve.
+ * Refused (B200MPPI_EINVAL naming the planner) before any work is issued: what b200mppi_batch_run_trials and the
+ * stochastic batch_solve refuse, and a TDM pair that cannot join the one batched sampler launch (lin == ang, diverged
+ * lin / ang streams, a PMF the staged sampler cannot take, a geometry that differs from planner 0's).  A batch made by
+ * b200mppi_batch_create is refused, naming planner 0's mode. */
+int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps,
+                                         double* xhist, float* uhist, b200mppi_trial_result* results,
+                                         int32_t* steps_issued);
 
 #ifdef __cplusplus
 }

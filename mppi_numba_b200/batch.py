@@ -17,7 +17,8 @@ num_grid_samples (at most 1024): one launch per stage for noise, rollout, CVaR a
 
 ``run_trials(traction_grids, max_steps)`` runs the benchmark's closed-loop episode (solve, plant step on a ground-truth
 ``TractionGrid``, shift_and_update, stop at the goal) for every det-dynamics or speed-map planner at once on the GPU,
-without a host round trip per step (include/b200mppi.h, closed-loop trials).
+without a host round trip per step (include/b200mppi.h, closed-loop trials); ``MPPI_StochasticBatch.
+run_stochastic_trials`` does the same for use_tdm planners.
 """
 import ctypes as C
 
@@ -130,31 +131,36 @@ class MPPI_Batch(object):
         num_opt < 1, a grid of another dtype than float64 or integer, or a planner that cannot solve (e.g. its start
         pose is outside the padded map limits); B200MPPIError when the planners' maps cannot all be sampled by the
         batch's one sampler launch.  Nothing is issued when the call is refused."""
-        K = len(self.planners)
         if self.kind not in ("det", "spd"):
             raise ValueError("MPPI_Batch.run_trials: planner 0 is a %s planner (trials need det-dynamics or speed-map "
                              "planners)" % self.kind)
+        return self._trials("MPPI_Batch.run_trials", lib.b200mppi_batch_run_trials, traction_grids, max_steps, dt)
+
+    def _trials(self, name, entry, traction_grids, max_steps, dt):
+        """The marshalling of a closed-loop trial call through the C entry point ``entry`` and the logs built from its
+        results (run_trials, MPPI_StochasticBatch.run_stochastic_trials); ``name`` prefixes the refusals."""
+        K = len(self.planners)
         grids = list(traction_grids)
         if len(grids) != K:
-            raise ValueError("MPPI_Batch.run_trials: %d traction grids for %d planners" % (len(grids), K))
+            raise ValueError("%s: %d traction grids for %d planners" % (name, len(grids), K))
         max_steps = int(max_steps)
         if max_steps < 1:
-            raise ValueError("MPPI_Batch.run_trials: max_steps %d < 1" % max_steps)
+            raise ValueError("%s: max_steps %d < 1" % (name, max_steps))
         descs = (_lib.TrialDesc * K)()
         keep = []
         for i, (p, g) in enumerate(zip(self.planners, grids)):
             if not p.check_solve_conditions():
-                raise ValueError("MPPI_Batch.run_trials: planner %d cannot solve (reason printed above)" % i)
+                raise ValueError("%s: planner %d cannot solve (reason printed above)" % (name, i))
             if int(p.params["num_opt"]) < 1:
-                raise ValueError("MPPI_Batch.run_trials: planner %d has num_opt %d < 1" % (i, int(p.params["num_opt"])))
+                raise ValueError("%s: planner %d has num_opt %d < 1" % (name, i, int(p.params["num_opt"])))
             lin, ang = np.asarray(g.lin_traction), np.asarray(g.ang_traction)
             for a in (lin, ang):
                 if a.dtype != np.float64 and not np.issubdtype(a.dtype, np.integer):
-                    raise ValueError("MPPI_Batch.run_trials: planner %d: traction grid of dtype %s (float64 or integer "
-                                     "grids only: the plant step is float64)" % (i, a.dtype))
+                    raise ValueError("%s: planner %d: traction grid of dtype %s (float64 or integer "
+                                     "grids only: the plant step is float64)" % (name, i, a.dtype))
             if lin.ndim != 2 or lin.shape != ang.shape:
-                raise ValueError("MPPI_Batch.run_trials: planner %d: lin / ang traction grids of shapes %s / %s"
-                                 % (i, lin.shape, ang.shape))
+                raise ValueError("%s: planner %d: lin / ang traction grids of shapes %s / %s"
+                                 % (name, i, lin.shape, ang.shape))
             lin = np.ascontiguousarray(lin, dtype=np.float64)
             ang = np.ascontiguousarray(ang, dtype=np.float64)
             keep += [lin, ang]
@@ -174,14 +180,14 @@ class MPPI_Batch(object):
         uhist = np.empty((K, max_steps, 2), dtype=np.float32)
         res = (_lib.TrialResult * K)()
         issued = C.c_int32()
-        check(lib.b200mppi_batch_run_trials(self._handle, descs, max_steps, ptr(xhist), ptr(uhist), res,
-                                            C.byref(issued)))
+        check(entry(self._handle, descs, max_steps, ptr(xhist), ptr(uhist), res, C.byref(issued)))
         self.steps_issued = int(issued.value)
         steps = np.array([r.steps for r in res], dtype=np.int64)
         status = [TRIAL_STATUS[r.status] for r in res]
         logs = []
         for i, p in enumerate(self.planners):
-            p.u_prev_d = p._u_prev_buf                 # as each planner's own solve() does (mppi.py:292,362)
+            if self.kind != "tdm":
+                p.u_prev_d = p._u_prev_buf             # as each planner's own solve() does (mppi.py:292,362)
             p.params["x0"] = xhist[i, steps[i]].copy()  # shift_and_update(x_next, ...)
             r, n, reached = res[i], int(steps[i]), status[i] == "goal"
             cum_obj, dist = r.cum_obj, r.dist_to_goal
@@ -198,7 +204,7 @@ class MPPI_Batch(object):
 class MPPI_StochasticBatch(MPPI_Batch):
     """Borrows use_tdm ``planners`` (keeps them alive) and solves them with one launch per stage: noise, windowed
     rollout, CVaR and update; each planner's map sampling keeps its own launches.  ``solve()``, ``set_stream`` and
-    ``launch_count`` as in MPPI_Batch; closed-loop trials are not offered."""
+    ``launch_count`` as in MPPI_Batch; closed-loop trials through ``run_stochastic_trials``."""
 
     def __init__(self, planners):
         planners = list(planners)
@@ -229,4 +235,17 @@ class MPPI_StochasticBatch(MPPI_Batch):
 
     def run_trials(self, traction_grids, max_steps, dt=None):
         raise ValueError("MPPI_StochasticBatch.run_trials: closed-loop trials run det-dynamics or speed-map batches "
-                         "(a stochastic solve sizes each planner's map-sampling box on the host)")
+                         "(a stochastic batch runs them with run_stochastic_trials)")
+
+    def run_stochastic_trials(self, traction_grids, max_steps, dt=None):
+        """MPPI_Batch.run_trials for use_tdm planners: the same arguments, episode, stop rules, returned dict and NaN
+        conventions, one episode per planner on the GPU without a host round trip per step (each planner's
+        map-sampling reach box is decided on the device).  Afterwards every planner is exactly as after ``steps[k]``
+        rounds of ``u = batch.solve()``, the plant step on ``traction_grids[k]`` and ``shift_and_update(x_next, u[k])``:
+        controls, noise, per-(m, n) and CVaR costs, weights, RNG streams, its TDMs' streams and sampled maps,
+        ``sample_box()`` and ``params['x0']``.  u_prev_d is left alone, as a stochastic solve leaves it.
+        Raises ValueError (naming the planner) as run_trials does; B200MPPIError when a planner cannot take the windowed
+        rollout or its TDM pair cannot join the batch's one sampler launch.  Nothing is issued when the call is
+        refused."""
+        return self._trials("MPPI_StochasticBatch.run_stochastic_trials", lib.b200mppi_batch_run_stochastic_trials,
+                            traction_grids, max_steps, dt)

@@ -178,11 +178,9 @@ static void fill_v2(const b200mppi_tdm* t, SampleGridsV2Args& a, int slot) {
   }
 }
 
-// Cells [row_lo, row_hi) x [col_lo, col_hi) that the rollouts of the coming solve can read (planner: reach_box).
-struct SampleBox { int row_lo, row_hi, col_lo, col_hi; float cx, cy, r; };   // + the reach disc in cells (r = 0: none)
-
-// Restrict a whole-map launch description to the tile rows / row range / tile columns covering `b`.
-static void apply_box(const b200mppi_tdm* t, SampleGridsV2Args& a, const SampleBox& b) {
+// Restrict a whole-map launch description to the tile rows / row range / tile columns covering the reach box `b`
+// (reach_box_decide, kernels.h).
+static void apply_box(const b200mppi_tdm* t, SampleGridsV2Args& a, const ReachBox& b) {
   const int nrow = (a.rows + a.tx - 1) / a.tx, ncol = (a.cols + a.ty - 1) / a.ty;
   a.segs = t->box_segs; a.seg_rows = t->box_seg_rows; a.jump = t->jump_box_d;
   a.row_lo = b.row_lo; a.row_hi = b.row_hi;
@@ -248,7 +246,7 @@ static int plan_sampling(b200mppi_tdm* l, b200mppi_tdm* g, double alpha, cudaStr
 
 // Narrow a plan's staged launches to `b` where the narrowed launch fits; the others (and the generic kernel) keep
 // sampling whole maps.
-static void plan_box(SamplePlan* pl, const SampleBox& b) {
+static void plan_box(SamplePlan* pl, const ReachBox& b) {
   for (int i = 0; i < (pl->fused ? 1 : pl->nt); ++i) {
     if (!pl->v2[i]) continue;
     SampleGridsV2Args bx = pl->a[i];
@@ -1023,22 +1021,19 @@ static void fill_rollout_args(b200mppi_planner* p, RolloutArgs& a) {
 }
 
 // The planner's part of the windowed rollout's arguments: window (centred on the robot's cell) and buffers.
+// win_origin (kernels.h), shared with the plant step of stochastic trials, takes the six window fields from WW on
+static_assert(offsetof(RolloutWinArgs, WH) == offsetof(RolloutWinArgs, WW) + 4 &&
+              offsetof(RolloutWinArgs, wx0) == offsetof(RolloutWinArgs, WW) + 8 &&
+              offsetof(RolloutWinArgs, wy0) == offsetof(RolloutWinArgs, WW) + 12 &&
+              offsetof(RolloutWinArgs, ww) == offsetof(RolloutWinArgs, WW) + 16 &&
+              offsetof(RolloutWinArgs, wh) == offsetof(RolloutWinArgs, WW) + 20, "RolloutWinArgs window fields");
+
 static void fill_win_args(const b200mppi_planner* p, int WW, int WH, RolloutWinArgs& w) {
   const b200mppi_tdm* l = p->lin; const b200mppi_tdm* g = p->ang;
   w.WW = WW; w.WH = WH;
-  const int xi0 = (int)std::floor(((double)p->prm.x0[0] - (double)l->pxl[0]) / (double)l->res);
-  const int yi0 = (int)std::floor(((double)p->prm.x0[1] - (double)l->pyl[0]) / (double)l->res);
   // TMA: the inner (x) start coordinate is kept 16-byte aligned for 1-byte elements (an unaligned c0 faulted
-  // with 'illegal instruction' when probed); floor to a multiple of 16, also for negatives
-  // The window is kept INSIDE the map (origin clamped, extents cut): a staged cell is then always a map cell, and
-  // every index outside the map takes the global-memory path with the generic kernel's wrap + clamp.
-  int cx = xi0 - WW / 2, cy = yi0 - WH / 2;
-  cx = std::max(0, std::min(cx, l->cols - WW));
-  cy = std::max(0, std::min(cy, l->rows - WH));
-  w.wx0 = cx & ~15;
-  w.wy0 = cy;
-  w.ww = std::min(WW, l->cols - w.wx0);
-  w.wh = std::min(WH, l->rows - w.wy0);
+  // with 'illegal instruction' when probed)
+  win_origin(p->prm.x0[0], p->prm.x0[1], l->pxl[0], l->pyl[0], l->res, l->cols, l->rows, &w.WW);
   w.npad = p->npad;
   w.masks01 = l->masks01 ? 1 : 0;
   w.lin_grid = l->grid; w.ang_grid = g->grid; w.obstacle = l->obstacle; w.unknown = l->unknown;
@@ -1158,38 +1153,21 @@ extern "C" int b200mppi_planner_set_obstacles(b200mppi_planner* p, const float* 
   return B200MPPI_OK;
 }
 
-// Cells the rollouts of this solve can read.  A rollout moves at most |traction| * |v| * dt per step, so it stays
-// within R = dt * max|traction| * S of x0, S = sum_t |v_t| -- bounded by T * max|vrange| (static box) or, when the maps
-// are sampled once for ONE set of controls (num_opt = 1), by `reach`: the max over the N control sequences actually
-// drawn (reach_d, reduced by the prepare kernel and read back by stage_sample_tdms; null: the static bound).
-// False (whole maps) whenever the bound is not airtight: the box would leave the map (out-of-map indices wrap),
-// traction bytes not under the sampler's control, non-finite inputs.
-static bool planner_reach_box(const b200mppi_planner* p, const float* reach, SampleBox* box, int* how) {
-  *how = 1;
-  if (p->box_mode == 0 || !planner_uses_window(p)) return false;
+// The constants of a planner's reach-box decision (reach_box_decide, kernels.h) for the plan of its pair: the box is
+// sized from the speed limit or, when the maps are sampled once for ONE set of controls (num_opt = 1, box_mode 2), from
+// the reach statistic of the controls actually drawn (reach_d, reduced by the prepare kernel).
+static void fill_reach_const(const b200mppi_planner* p, const SamplePlan& pl, ReachBoxConst* c) {
   const b200mppi_tdm* l = p->lin;
   const b200mppi_params& q = p->prm;
-  double S = (double)p->T * std::fmax(std::fabs((double)q.vrange[0]), std::fabs((double)q.vrange[1]));
-  if (reach) {
-    if (!((double)*reach <= S)) return false;          // NaN or beyond the speed limit: not a usable bound
-    S = (double)*reach;
-    *how = 2;
-  }
-  // 1.0002: cos/sin.approx may exceed 1 by ~1e-6, float32 rounding of the state adds ~1e-7 per step; + one cell below
-  const double R = (double)q.dt * (double)l->tr_abs_max * S * 1.0002;
-  if (!(R >= 0.0) || !std::isfinite(R)) return false;
-  const double res = (double)l->res;
-  const double fx0 = ((double)q.x0[0] - R - (double)l->pxl[0]) / res, fx1 = ((double)q.x0[0] + R - (double)l->pxl[0]) / res;
-  const double fy0 = ((double)q.x0[1] - R - (double)l->pyl[0]) / res, fy1 = ((double)q.x0[1] + R - (double)l->pyl[0]) / res;
-  if (!(fx0 > 2.0 && fy0 > 2.0 && fx1 < (double)l->cols - 3.0 && fy1 < (double)l->rows - 3.0)) return false;
-  box->col_lo = (int)std::floor(fx0) - 1; box->col_hi = (int)std::floor(fx1) + 3;      // [lo, hi)
-  box->row_lo = (int)std::floor(fy0) - 1; box->row_hi = (int)std::floor(fy1) + 3;
-  // the same bound as a disc: a rollout stays within Euclidean distance R of x0, so the cell it reads lies within
-  // R/res + sqrt(2) cells of the robot's (fractional) cell position; + 1.5 for float32 effects, rounded up
-  box->cx = (float)(((double)q.x0[0] - (double)l->pxl[0]) / res);
-  box->cy = (float)(((double)q.x0[1] - (double)l->pyl[0]) / res);
-  box->r = p->disc ? (float)(R / res + 3.0) * 1.0001f : 0.0f;
-  return true;
+  *c = ReachBoxConst{};
+  c->mode = (p->box_mode == 0 || !planner_uses_window(p)) ? 0 : (p->box_mode == 2 && q.num_opt == 1) ? 2 : 1;
+  c->disc = p->disc ? 1 : 0;
+  c->T = p->T;
+  c->vr0 = q.vrange[0]; c->vr1 = q.vrange[1]; c->dt = q.dt; c->tr_abs_max = l->tr_abs_max;
+  c->res = l->res; c->pxl = l->pxl[0]; c->pyl = l->pyl[0]; c->rows = l->rows; c->cols = l->cols;
+  const SampleGridsV2Args& a = pl.a[0];
+  c->nt = !pl.v2[0] ? 0 : pl.fused ? 2 : 1;
+  c->tx = a.tx; c->ty = a.ty; c->num_maps = a.num_maps; c->bpad0 = a.t[0].bpad; c->bpad1 = a.t[1].bpad;
 }
 
 // A solve's map sampling in three steps, shared by solve() (stage_sample_tdms) and the stochastic batch:
@@ -1212,9 +1190,11 @@ static float* sample_reach_host(b200mppi_planner* p) { return p->h_u + (size_t)p
 // reach: the read-back statistic or null (static box); advanced: a fused pair's state advance is already queued
 static int sample_finish(b200mppi_planner* p, SamplePlan& plan, const float* reach, bool advanced, cudaStream_t st,
                          int64_t* launches) {
-  SampleBox box{};
-  int how = 0;
-  if (planner_reach_box(p, reach, &box, &how)) plan_box(&plan, box);
+  ReachBoxConst c;
+  fill_reach_const(p, plan, &c);
+  ReachBox box;
+  const int how = reach_box_decide(c, p->prm.x0[0], p->prm.x0[1], reach, &box);
+  if (box.geo) plan_box(&plan, box);                      // an unfused pair's TDM 1 may take the box on its own
   const int rc = plan_launch(plan, advanced, st, launches);
   const bool used = plan.boxed[0];                        // the box may not fit the sampler's launch: whole maps
   p->last_box[0] = used ? how : 0;
@@ -2074,32 +2054,36 @@ extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
 // sampling, in planner order, with the decisions of stage_sample_tdms], ONE windowed rollout launch over all (planner,
 // map) units, ONE CVaR launch and ONE update launch.  The reach statistics of all planners are read back behind one
 // event, so the host waits once.
-static int batch_solve_stochastic(b200mppi_batch* b, float* u_out) {
-  int rc = batch_validate(b);
-  if (rc) return rc;
-  const int K = (int)b->pl.size(), T = b->T, N = b->N;
-  int WW, WH; size_t smem;
-  rollout_win_geometry(T, &WW, &WH, &smem);
-  WH = rollout_win_batch_height(T);
+// The windowed rollout of every planner of a stochastic batch (its kernel and its encoded tensor maps at the batch's
+// window geometry WW x WH), checked before any work is issued; `fn` prefixes the messages.
+static int stochastic_validate(b200mppi_batch* b, const char* fn, int* WW, int* WH) {
+  size_t smem;
+  rollout_win_geometry(b->T, WW, WH, &smem);
+  *WH = rollout_win_batch_height(b->T);
   CU(cudaSetDevice(b->device));
-  for (int i = 0; i < K; ++i) {
+  for (int i = 0; i < (int)b->pl.size(); ++i) {
     b200mppi_planner* p = b->pl[i];
-    const std::string who = "batch_solve: planner " + std::to_string(i);
+    const std::string who = std::string(fn) + ": planner " + std::to_string(i);
     // the generic rollout kernel's costs differ from the windowed kernel's in the last bit: no stand-in
     if (!planner_uses_window(p))
       return fail(B200MPPI_EINVAL, who + " does not take the windowed rollout kernel (B200MPPI_NO_WINDOW is set or its "
                                          "window does not fit shared memory)");
-    if (!planner_tensor_maps(p, WW, WH))
+    if (!planner_tensor_maps(p, *WW, *WH))
       return fail(B200MPPI_EINVAL, who + ": the tensor maps of its sampled maps / masks could not be encoded");
   }
-  cudaStream_t st = b->stream;
-  if ((rc = batch_wait_members(b))) return rc;
-  NoisePrepDesc* hn = reinterpret_cast<NoisePrepDesc*>(b->h_desc);
-  RolloutWinArgs* hw = reinterpret_cast<RolloutWinArgs*>(b->h_desc + b->off_win);
-  unsigned char* ht = b->h_desc + b->off_tm;
-  CvarDesc* hc = reinterpret_cast<CvarDesc*>(b->h_desc + b->off_cvar);
-  UpdateBatchDesc* hu = reinterpret_cast<UpdateBatchDesc*>(b->h_desc + b->off_upd);
-  bool masks01 = true;
+  return B200MPPI_OK;
+}
+
+// The per-planner descriptors of a stochastic batch's noise + controls, windowed rollout (+ tensor maps), CVaR and update
+// launches at byte offset 0 of `h` (the layout of b->h_desc); *masks01: every planner's masks are 0 / 1.
+static void stochastic_descs(b200mppi_batch* b, unsigned char* h, int WW, int WH, bool* masks01) {
+  const int K = (int)b->pl.size(), T = b->T;
+  NoisePrepDesc* hn = reinterpret_cast<NoisePrepDesc*>(h);
+  RolloutWinArgs* hw = reinterpret_cast<RolloutWinArgs*>(h + b->off_win);
+  unsigned char* ht = h + b->off_tm;
+  CvarDesc* hc = reinterpret_cast<CvarDesc*>(h + b->off_cvar);
+  UpdateBatchDesc* hu = reinterpret_cast<UpdateBatchDesc*>(h + b->off_upd);
+  *masks01 = true;
   for (int i = 0; i < K; ++i) {
     b200mppi_planner* p = b->pl[i];
     const b200mppi_params& q = p->prm;
@@ -2110,15 +2094,28 @@ static int batch_solve_stochastic(b200mppi_batch* b, float* u_out) {
     fill_rollout_params(p, hw[i].p);
     fill_win_args(p, WW, WH, hw[i]);
     fill_cost_dst(p, hw[i].dst, false);
-    masks01 = masks01 && hw[i].masks01;
+    *masks01 = *masks01 && hw[i].masks01;
     std::memcpy(ht + (size_t)i * sizeof(b200mppi_planner::tmaps), p->tmaps, sizeof(b200mppi_planner::tmaps));
-    hc[i] = CvarDesc{p->costs_nm, p->costs, p->n_local, p->n_local, p->M, cvar_numel(p->M, q.cvar_alpha)};
+    hc[i] = CvarDesc{p->costs_nm, p->costs, p->n_local, p->n_local, p->M, cvar_numel(p->M, q.cvar_alpha), nullptr};
     fill_update_args(p, hu[i].a, nullptr);
     hu[i].tl = UpdateTail{};
     hu[i].tl.counter = p->upd_counter_d;
     hu[i].tl.mode = UPD_TAIL_APPLY;
     hu[i].tl.u_out = b->u_d + (size_t)i * T * 2;        // u_prev stays null: a stochastic solve does not alias it
   }
+}
+
+static int batch_solve_stochastic(b200mppi_batch* b, float* u_out) {
+  int rc = batch_validate(b);
+  if (rc) return rc;
+  const int K = (int)b->pl.size(), T = b->T, N = b->N;
+  int WW, WH;
+  if ((rc = stochastic_validate(b, "batch_solve", &WW, &WH))) return rc;
+  cudaStream_t st = b->stream;
+  if ((rc = batch_wait_members(b))) return rc;
+  const RolloutWinArgs* hw = reinterpret_cast<const RolloutWinArgs*>(b->h_desc + b->off_win);
+  bool masks01 = true;
+  stochastic_descs(b, b->h_desc, WW, WH, &masks01);
   // the sampler plans (their host preparation may synchronise the stream) before the one upload
   std::vector<SamplePlan> plans(K);
   for (int i = 0; i < K; ++i)
@@ -2138,7 +2135,7 @@ static int batch_solve_stochastic(b200mppi_batch* b, float* u_out) {
     }
   }
   for (int k = 0; k < num_opt; ++k) {
-    launch_noise_prepare_batch(dn, K, N, T, b->pl[0]->npad, k, st);
+    launch_noise_prepare_batch(dn, K, N, T, b->pl[0]->npad, k, nullptr, st);
     b->launches++;
     CHECK_LAUNCH();
     for (b200mppi_planner* p : b->pl) {                // stage_noise
@@ -2171,7 +2168,7 @@ static int batch_solve_stochastic(b200mppi_batch* b, float* u_out) {
           return rc;
       }
     }
-    CU(launch_rollout_win_batch(hw[0], dw, dt, K, masks01, st));
+    CU(launch_rollout_win_batch(hw[0], dw, dt, K, masks01, nullptr, st));
     b->launches++;
     for (b200mppi_planner* p : b->pl) { p->prepared = false; p->pushed_direct = false; }
     launch_cvar_batch(dc, K, N, b->M, st);
@@ -2195,17 +2192,18 @@ static int batch_solve_stochastic(b200mppi_batch* b, float* u_out) {
 // planners through pinned memory POLL steps behind the GPU and stops issuing once it reads zero.
 constexpr int TRIAL_POLL = 4;
 
-static int trial_validate(b200mppi_batch* b, const b200mppi_trial_desc* tr, int32_t max_steps) {
+static int trial_validate(b200mppi_batch* b, const b200mppi_trial_desc* tr, int32_t max_steps,
+                          const char* fn = "run_trials") {
   const int K = (int)b->pl.size();
-  if (!tr) return fail(B200MPPI_EINVAL, "run_trials: null trial descriptors");
-  if (max_steps < 1) return fail(B200MPPI_EINVAL, "run_trials: max_steps < 1");
+  if (!tr) return fail(B200MPPI_EINVAL, std::string(fn) + ": null trial descriptors");
+  if (max_steps < 1) return fail(B200MPPI_EINVAL, std::string(fn) + ": max_steps < 1");
   if (b->mode == B200MPPI_MODE_BAREBONE)
     return fail(B200MPPI_EINVAL, "run_trials: planner 0 is MODE_BAREBONE (trials need traction maps: MODE_DET_DYN or "
                                  "MODE_SPEED_MAP batches)");
   int rc = batch_validate(b);
   if (rc) return rc;
   for (int i = 0; i < K; ++i) {
-    const std::string who = "run_trials: planner " + std::to_string(i);
+    const std::string who = std::string(fn) + ": planner " + std::to_string(i);
     const b200mppi_trial_desc& d = tr[i];
     if (b->pl[i]->prm.num_opt < 1) return fail(B200MPPI_EINVAL, who + " has num_opt < 1");
     if (!d.lin || !d.ang || d.height < 1 || d.width < 1)
@@ -2309,6 +2307,7 @@ extern "C" int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial
     std::memcpy(g + cells, q.ang, cells * sizeof(double));
     const double* dg = reinterpret_cast<const double*>(d + off_grid[i]);
     TrialDev& t = ht[i];
+    t = TrialDev{};                                   // win stays null: one-map rollouts have no window
     t.lin = dg; t.ang = dg + cells; t.H = q.height; t.W = q.width;
     t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res; t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1];
     t.tol = q.goal_tolerance;
@@ -2393,6 +2392,256 @@ extern "C" int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial
     p->prepared = false;
     p->pushed_direct = false;
     p->last_box[0] = 0; p->last_box[1] = 0; p->last_box[2] = p->lin->rows; p->last_box[3] = 0; p->last_box[4] = p->lin->cols;
+    for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)xo[(size_t)(n - 1) * 3 + c];
+  }
+  if (steps_issued) *steps_issued = issued;
+  return B200MPPI_OK;
+}
+
+// Closed-loop trials of a stochastic batch.  As for one-map batches, only x0 and the parity of the generator-state
+// double buffers change from step to step -- plus each planner's reach box, which moves with the robot and, with
+// box_mode 2 and num_opt 1, depends on the controls drawn: the batched boxed sampler decides it on the device
+// (reach_box_decide, the function sample_finish calls), so a step needs no host round trip.  Per step: num_opt x (noise +
+// controls, [first iteration: boxed sampler, state advance], windowed rollout, CVaR, update) and the plant step, which
+// also moves each planner's rollout window.
+extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials,
+                                                    int32_t max_steps, double* xhist, float* uhist,
+                                                    b200mppi_trial_result* results, int32_t* steps_issued) {
+  static const char* FN = "run_stochastic_trials";
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  if (!b->stochastic)
+    return fail(B200MPPI_EINVAL, std::string(FN) + ": planner 0 is " +
+                                     (b->mode == B200MPPI_MODE_DET_DYN ? "MODE_DET_DYN" :
+                                      b->mode == B200MPPI_MODE_SPEED_MAP ? "MODE_SPEED_MAP" : "MODE_BAREBONE") +
+                                     " (stochastic trials run MODE_TDM batches; b200mppi_batch_run_trials runs the others)");
+  int rc = trial_validate(b, trials, max_steps, FN);
+  if (rc) return rc;
+  if (!xhist || !uhist || !results) return fail(B200MPPI_EINVAL, std::string(FN) + ": null output buffer");
+  int WW, WH;
+  if ((rc = stochastic_validate(b, FN, &WW, &WH))) return rc;
+  const int K = (int)b->pl.size(), T = b->T, N = b->N, S = max_steps;
+  cudaStream_t st = b->stream;
+  // every pair must join the one boxed sampler launch: a fused plan (identical generator streams, well-formed PMF at
+  // its alpha, lin != ang) whose launch and box segments equal planner 0's
+  std::vector<SamplePlan> plans(K);
+  for (int i = 0; i < K; ++i) {
+    b200mppi_planner* p = b->pl[i];
+    if ((rc = plan_sampling(p->lin, p->ang, sample_alpha(p), st, &plans[i]))) return rc;
+    const b200mppi_tdm* l = p->lin; const b200mppi_tdm* l0 = b->pl[0]->lin;
+    if (!plans[i].fused || !sample_grids_v2_same_launch(plans[0].a[0], plans[i].a[0]) || l->box_segs != l0->box_segs ||
+        l->box_seg_rows != l0->box_seg_rows)
+      return fail(B200MPPI_EINVAL, std::string(FN) + ": planner " + std::to_string(i) + ": its TDM pair cannot join the "
+                                   "batch's one sampler launch (lin == ang, or map geometry, PMF or generator streams "
+                                   "differ from planner 0's)");
+  }
+  // the one sampler launch is sized for the largest box the static bound allows (reach_box_decide: at most 2 R / res + 5
+  // cells a side) over all planners that sample a box: mrows tile rows x ncact tile columns with the boxed launch's maps
+  // per CTA.  Whole-map steps loop over such groups.
+  const SampleGridsV2Args& sg = plans[0].a[0];
+  const int nrow = (sg.rows + sg.tx - 1) / sg.tx, ncol = (sg.cols + sg.ty - 1) / sg.ty;
+  double span = 0.0;                                  // cells a side, + margin
+  bool any_box = false;
+  for (int i = 0; i < K; ++i) {
+    ReachBoxConst c;
+    fill_reach_const(b->pl[i], plans[i], &c);
+    if (c.mode == 0) continue;
+    any_box = true;
+    const double R = (double)c.dt * (double)c.tr_abs_max * ((double)c.T * std::fmax(std::fabs((double)c.vr0),
+                                                                                       std::fabs((double)c.vr1))) * 1.0002;
+    span = std::fmax(span, 2.0 * R / (double)c.res + 8.0);
+  }
+  int mrows = sg.tx, ncact = sg.ty;
+  if (any_box && span < (double)(sg.rows + sg.cols)) {
+    mrows = std::min(sg.tx, (int)span / nrow + 2);
+    ncact = std::min(sg.ty, (int)span / ncol + 2);
+  }
+  int gm_b = 128 / ncact;                             // apply_box's maps per CTA for that many tile columns
+  gm_b = std::max(1, std::min(std::min(gm_b, SG_GM_MAX), sg.num_maps));
+  {
+    SampleGridsV2Args geom = sg;
+    geom.gm = gm_b;
+    if (!sample_box_batch_fits(geom, ncact))
+      return fail(B200MPPI_EINVAL, std::string(FN) + ": planner 0: the batched sampler launch (" + std::to_string(ncact) +
+                                   " tile columns x " + std::to_string(gm_b) + " maps per CTA) does not fit a CTA");
+  }
+  if ((rc = batch_wait_members(b))) return rc;
+  // device buffers of this call: [descriptors | sampler sets of parity 0, 1 | box descriptors | box records | trials |
+  // states | active K + count | grids | xhist | uhist]
+  const size_t off_s0 = b->desc_bytes;
+  const size_t off_s1 = off_s0 + align256((size_t)K * sizeof(SampleGridsV2Args));
+  const size_t off_box = off_s1 + align256((size_t)K * sizeof(SampleGridsV2Args));
+  const size_t off_rec = off_box + align256((size_t)K * sizeof(SampleBoxDesc));
+  const size_t off_tr = off_rec + align256((size_t)K * 5 * sizeof(int));
+  const size_t off_state = off_tr + align256((size_t)K * sizeof(TrialDev));
+  const size_t off_act = off_state + align256((size_t)K * sizeof(TrialState));
+  size_t off = off_act + align256((size_t)(K + 1) * sizeof(int));
+  std::vector<size_t> off_grid(K);
+  for (int i = 0; i < K; ++i) {
+    off_grid[i] = off;
+    off += align256((size_t)2 * trials[i].height * trials[i].width * sizeof(double));
+  }
+  const size_t off_xh = off, off_uh = off_xh + align256((size_t)K * (S + 1) * 3 * sizeof(double));
+  const size_t total = off_uh + align256((size_t)K * S * 2 * sizeof(float));
+  // pinned staging holds the head and the histories only: the ground-truth grids (float64, tens of MB for a batch of
+  // large maps) go to the device straight from the caller's arrays
+  const size_t head = off_grid.empty() ? off : off_grid[0];
+  const size_t h_xh = head, h_uh = head + (off_uh - off_xh);
+  unsigned char* d = nullptr;
+  unsigned char* h = nullptr;
+  CU(cudaMalloc(&d, total));
+  if (cudaMallocHost(&h, head + (total - off_xh)) != cudaSuccess) {
+    cudaFree(d);
+    return fail(B200MPPI_ECUDA, std::string(FN) + ": cudaMallocHost");
+  }
+  struct Free {
+    unsigned char *d, *h;
+    ~Free() { cudaFree(d); cudaFreeHost(h); }
+  } guard{d, h};
+  bool masks01 = true;
+  stochastic_descs(b, h, WW, WH, &masks01);
+  const RolloutWinArgs* hw = reinterpret_cast<const RolloutWinArgs*>(h + b->off_win);
+  CvarDesc* hc = reinterpret_cast<CvarDesc*>(h + b->off_cvar);
+  SampleGridsV2Args* hs[2] = {reinterpret_cast<SampleGridsV2Args*>(h + off_s0),
+                              reinterpret_cast<SampleGridsV2Args*>(h + off_s1)};
+  SampleBoxDesc* hb = reinterpret_cast<SampleBoxDesc*>(h + off_box);
+  TrialDev* ht = reinterpret_cast<TrialDev*>(h + off_tr);
+  TrialState* hst = reinterpret_cast<TrialState*>(h + off_state);
+  int* hact = reinterpret_cast<int*>(h + off_act);
+  RolloutWinArgs* dw = reinterpret_cast<RolloutWinArgs*>(d + b->off_win);
+  int* dact = reinterpret_cast<int*>(d + off_act);
+  int* drec = reinterpret_cast<int*>(d + off_rec);
+  for (int i = 0; i < K; ++i) {
+    b200mppi_planner* p = b->pl[i];
+    const b200mppi_tdm* l = p->lin;
+    hc[i].active = dact + i;
+    // the boxed launch's row segments over the whole-map plan; parity 1 samples from the buffers parity 0 wrote into
+    hs[0][i] = plans[i].a[0];
+    hs[0][i].segs = l->box_segs; hs[0][i].seg_rows = l->box_seg_rows; hs[0][i].jump = l->jump_box_d;
+    hs[0][i].write_states = 0;
+    hs[0][i].gm = gm_b;
+    hs[1][i] = hs[0][i];
+    for (SampleTdm& td : hs[1][i].t) {
+      uint64_t* in = td.states_out;
+      td.states_out = const_cast<uint64_t*>(td.states);
+      td.states = in;
+    }
+    hb[i] = SampleBoxDesc{};
+    fill_reach_const(p, plans[i], &hb[i].c);
+    hb[i].x0 = dw[i].p.x0;
+    hb[i].reach = p->reach_d;
+    hb[i].slot = p->reach_slot ^ 1;
+    hb[i].record = drec + 5 * i;
+    hb[i].jump_tile = l->jump_tile_d;
+    const b200mppi_trial_desc& q = trials[i];
+    const size_t cells = (size_t)q.height * q.width;
+    const double* dg = reinterpret_cast<const double*>(d + off_grid[i]);
+    TrialDev& t = ht[i];
+    t = TrialDev{};
+    t.lin = dg; t.ang = dg + cells; t.H = q.height; t.W = q.width;
+    t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res; t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1];
+    t.tol = q.goal_tolerance;
+    t.pxlim[0] = q.pxlim[0]; t.pxlim[1] = q.pxlim[1]; t.pylim[0] = q.pylim[0]; t.pylim[1] = q.pylim[1];
+    t.u_cur = p->u_cur;
+    t.x0_out = dw[i].p.x0;
+    t.win = &dw[i].WW;
+    t.win_pxl = l->pxl[0]; t.win_pyl = l->pyl[0]; t.win_res = l->res; t.win_rows = l->rows; t.win_cols = l->cols;
+    hst[i] = TrialState{};
+    for (int c = 0; c < 3; ++c) hst[i].x[c] = q.x0[c];
+    hact[i] = 1;
+  }
+  hact[K] = K;
+  CU(cudaMemcpyAsync(d, h, head, cudaMemcpyHostToDevice, st));
+  for (int i = 0; i < K; ++i) {                       // pageable sources: staged by the driver before the call returns
+    const size_t bytes = (size_t)trials[i].height * trials[i].width * sizeof(double);
+    CU(cudaMemcpyAsync(d + off_grid[i], trials[i].lin, bytes, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d + off_grid[i] + bytes, trials[i].ang, bytes, cudaMemcpyHostToDevice, st));
+  }
+  const NoisePrepDesc* dn = reinterpret_cast<const NoisePrepDesc*>(d);
+  const void* dtm = d + b->off_tm;
+  const CvarDesc* dc = reinterpret_cast<const CvarDesc*>(d + b->off_cvar);
+  const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(d + b->off_upd);
+  const SampleGridsV2Args* ds[2] = {reinterpret_cast<const SampleGridsV2Args*>(d + off_s0),
+                                    reinterpret_cast<const SampleGridsV2Args*>(d + off_s1)};
+  const SampleBoxDesc* db = reinterpret_cast<const SampleBoxDesc*>(d + off_box);
+  PlantArgs pa{};
+  pa.trials = reinterpret_cast<const TrialDev*>(d + off_tr);
+  pa.state = reinterpret_cast<TrialState*>(d + off_state);
+  pa.active = dact; pa.active_count = dact + K;
+  pa.xhist = reinterpret_cast<double*>(d + off_xh);
+  pa.uhist = reinterpret_cast<float*>(d + off_uh);
+  pa.K = K; pa.T = T; pa.max_steps = S;
+  const SampleGridsV2Args geom = hs[0][0];
+  const RolloutWinArgs g0 = hw[0];
+  CU(cudaStreamSynchronize(st));                      // the staging is read by the upload above
+  int* hcount = reinterpret_cast<int*>(h);             // the polled counts, in the no longer needed head of the staging
+  cudaEvent_t ev[TRIAL_POLL] = {};
+  struct Events {
+    cudaEvent_t* e;
+    ~Events() { for (int i = 0; i < TRIAL_POLL; ++i) if (e[i]) cudaEventDestroy(e[i]); }
+  } evguard{ev};
+  for (auto& e : ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  const int num_opt = b->pl[0]->prm.num_opt, npad = b->pl[0]->npad;
+  int issued = 0;
+  for (int s = 0; s < S; ++s) {
+    if (s >= TRIAL_POLL) {                            // the count after step s - POLL
+      CU(cudaEventSynchronize(ev[s % TRIAL_POLL]));
+      if (hcount[s % TRIAL_POLL] == 0) break;
+    }
+    for (int k = 0; k < num_opt; ++k) {
+      const int iter = s * num_opt + k;               // every planner's reach slot toggles once per iteration
+      launch_noise_prepare_batch(dn, K, N, T, npad, iter, dact, st);
+      CHECK_LAUNCH();
+      if (k == 0) {
+        launch_sample_grids_v2_box_batch(geom, ds[s & 1], db, K, dact, iter, mrows, ncact, st);
+        CHECK_LAUNCH();
+        launch_advance_states_batch(ds[s & 1], db, K, geom.rows, geom.cols, geom.tx, geom.ty, geom.num_maps, dact, st);
+        CHECK_LAUNCH();
+      }
+      CU(launch_rollout_win_batch(g0, dw, dtm, K, masks01, dact, st));
+      launch_cvar_batch(dc, K, N, b->M, st);
+      CHECK_LAUNCH();
+      launch_update_partial_batch(du, K, b->pl[0]->num_ctas, dact, st);
+      CHECK_LAUNCH();
+    }
+    pa.step = s;
+    launch_plant_step(pa, st);
+    CHECK_LAUNCH();
+    b->launches += 4 * num_opt + 3;
+    ++issued;
+    CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, dact + K, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(ev[s % TRIAL_POLL], st));
+  }
+  CU(cudaMemcpyAsync(h + off_rec, d + off_rec, off_tr - off_rec, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(h + off_state, d + off_state, off_act - off_state, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(h + h_xh, d + off_xh, total - off_xh, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const int* hrec = reinterpret_cast<const int*>(h + off_rec);
+  const double* hx = reinterpret_cast<const double*>(h + h_xh);
+  const float* hu_h = reinterpret_cast<const float*>(h + h_uh);
+  const double dnan = std::nan("");
+  const float fnan = std::nanf("");
+  for (int i = 0; i < K; ++i) {
+    const TrialState& r = hst[i];
+    const int n = r.steps;
+    double* xo = xhist + (size_t)i * (S + 1) * 3;
+    float* uo = uhist + (size_t)i * S * 2;
+    for (int c = 0; c < 3; ++c) xo[c] = trials[i].x0[c];
+    std::memcpy(xo + 3, hx + ((size_t)i * (S + 1) + 1) * 3, (size_t)n * 3 * sizeof(double));
+    for (size_t j = (size_t)(n + 1) * 3; j < (size_t)(S + 1) * 3; ++j) xo[j] = dnan;
+    std::memcpy(uo, hu_h + (size_t)i * S * 2, (size_t)n * 2 * sizeof(float));
+    for (size_t j = (size_t)n * 2; j < (size_t)S * 2; ++j) uo[j] = fnan;
+    results[i] = b200mppi_trial_result{r.cum_obj, r.cum_dist, r.dist, n, r.status};
+    // host state as after n rounds of the host loop: n boxed or whole-map samplings of the pair (the last one's kind
+    // in grid_partial), the reach slot toggled once per iteration, the last solve's box and x0
+    b200mppi_planner* p = b->pl[i];
+    const int* rec = hrec + 5 * i;
+    plans[i].boxed[0] = plans[i].boxed[1] = rec[0] != 0;
+    for (int s = 0; s < n; ++s) { plan_commit(plans[i], 0); plan_commit(plans[i], 1); }
+    p->reach_slot ^= (n * num_opt) & 1;
+    p->reach_valid = true;
+    p->prepared = false;
+    p->pushed_direct = false;
+    for (int c = 0; c < 5; ++c) p->last_box[c] = rec[c];
     for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)xo[(size_t)(n - 1) * 3 + c];
   }
   if (steps_issued) *steps_issued = issued;

@@ -51,6 +51,103 @@ void build_jump_series(int64_t k0, int64_t k1, int segs, uint64_t* out);     // 
 // q(r) of a RAW 64-bit draw r as a table lookup over its top 8 bits (see sample_threshold_q in common.cuh):
 // table = thr[256] | qbase[256] (u64, qbase in the low 11 bits).  false if alpha is not representable that way.
 constexpr int SAMPLE_TABLE_WORDS = 256;
+// shared memory / fit of a staged launch over tile columns [tiy_lo, tiy_lo + nact) with gm maps per CTA (nt TDMs)
+__host__ __device__ inline size_t sample_v2_smem_hd(int tiy_lo, int nact, int ty, int cols, int bpad, int gm, int nt) {
+  const int ncol = (cols + ty - 1) / ty;
+  const int cfirst = tiy_lo * ncol < cols ? tiy_lo * ncol : cols;
+  const int cs1 = (tiy_lo + nact) * ncol < cols ? (tiy_lo + nact) * ncol : cols;
+  const int wcols = cs1 - (cfirst & ~15);
+  const int row_bytes_al = (wcols * bpad + 15) & ~15;
+  const int stage_pitch = (wcols + 15) & ~15;
+  size_t stage = (size_t)nt * gm * stage_pitch;
+  if (stage < (size_t)2 * 128 * 16) stage = (size_t)2 * 128 * 16;           // the jump matrices overlay it
+  return (size_t)nt * row_bytes_al + stage + SAMPLE_TABLE_WORDS * 8 + (size_t)nt * 128;
+}
+__host__ __device__ inline bool sample_v2_fits_hd(int tiy_lo, int nact, int ty, int cols, int bpad0, int bpad1, int gm,
+                                                  int nt) {
+  return gm >= 1 && gm <= SG_GM_MAX && nact >= 1 && tiy_lo >= 0 && tiy_lo + nact <= ty &&
+         ((nact * gm + 31) / 32) * 32 <= 256 && bpad0 <= 32 &&
+         sample_v2_smem_hd(tiy_lo, nact, ty, cols, bpad0, gm, nt) <= 200 * 1024 && (nt == 1 || bpad0 == bpad1);
+}
+
+// The reach box of a solve's map sampling (planner_reach_box + plan_box in api.cu; the batched trial sampler decides it
+// on the device with the same function).  A rollout moves at most |traction| * |v| * dt per step, so it stays within
+// R = dt * max|traction| * S of x0, S = sum_t |v_t| -- bounded by T * max|vrange| (static box) or by `reach`, the max
+// over the N control sequences actually drawn.  Whole maps (0) whenever the bound is not airtight: the box would leave
+// the map (out-of-map indices wrap), non-finite inputs, a reach beyond the speed limit.  Float64 operations are
+// explicitly rounded on the device, so host and device decide alike.
+#ifdef __CUDA_ARCH__
+#define RB_MUL(a, b) __dmul_rn(a, b)
+#define RB_ADD(a, b) __dadd_rn(a, b)
+#define RB_SUB(a, b) __dsub_rn(a, b)
+#define RB_DIV(a, b) __ddiv_rn(a, b)
+#else
+#define RB_MUL(a, b) ((a) * (b))
+#define RB_ADD(a, b) ((a) + (b))
+#define RB_SUB(a, b) ((a) - (b))
+#define RB_DIV(a, b) ((a) / (b))
+#endif
+struct ReachBoxConst {          // a planner's constants of the decision
+  int mode;                     // 0: whole maps (box off or no windowed rollout), 1: static bound, 2: reach statistic
+                                //    (box_mode 2 with num_opt 1: the device path then reads the statistic)
+  int disc;                     // narrow to the reach disc (B200MPPI_SAMPLE_DISC)
+  int T;
+  float vr0, vr1, dt, tr_abs_max, res, pxl, pyl;
+  int rows, cols;
+  // the staged launch of TDM 0 (apply_box, sample_grids_v2_fits): nt = 2 fused pair, 1 one TDM, 0 generic kernel
+  int nt, tx, ty, num_maps, bpad0, bpad1;
+};
+struct ReachBox {
+  int geo;                      // the box exists (inside the map, finite bound) -- TDM 1 of an unfused pair may use it
+  int how;                      // the decision for TDM 0: 0 whole maps, 1 static box, 2 box from the reach statistic
+  int row_lo, row_hi, col_lo, col_hi;     // cells [row_lo, row_hi) x [col_lo, col_hi) (whole map when how = 0)
+  float cx, cy, r;              // reach disc in cells (r = 0: none)
+  int tiy_lo, nact, gm;         // the boxed launch's tile columns and maps per CTA (how != 0)
+};
+__host__ __device__ inline int reach_box_decide(const ReachBoxConst& c, float x0x, float x0y, const float* reach,
+                                                ReachBox* b) {
+  b->geo = 0; b->how = 0;
+  b->row_lo = 0; b->row_hi = c.rows; b->col_lo = 0; b->col_hi = c.cols;
+  b->cx = b->cy = b->r = 0.0f;
+  b->tiy_lo = 0; b->nact = c.ty; b->gm = 0;
+  if (c.mode == 0) return 0;
+  double S = RB_MUL((double)c.T, fmax(fabs((double)c.vr0), fabs((double)c.vr1)));
+  int how = 1;
+  if (reach) {
+    if (!((double)*reach <= S)) return 0;               // NaN or beyond the speed limit: not a usable bound
+    S = (double)*reach;
+    how = 2;
+  }
+  // 1.0002: cos/sin.approx may exceed 1 by ~1e-6, float32 rounding of the state adds ~1e-7 per step; + one cell below
+  const double R = RB_MUL(RB_MUL(RB_MUL((double)c.dt, (double)c.tr_abs_max), S), 1.0002);
+  if (!(R >= 0.0 && R <= 1.7976931348623157e308)) return 0;      // negative, NaN or infinite
+  const double res = (double)c.res, x = (double)x0x, y = (double)x0y;
+  const double fx0 = RB_DIV(RB_SUB(RB_SUB(x, R), (double)c.pxl), res);
+  const double fx1 = RB_DIV(RB_SUB(RB_ADD(x, R), (double)c.pxl), res);
+  const double fy0 = RB_DIV(RB_SUB(RB_SUB(y, R), (double)c.pyl), res);
+  const double fy1 = RB_DIV(RB_SUB(RB_ADD(y, R), (double)c.pyl), res);
+  if (!(fx0 > 2.0 && fy0 > 2.0 && fx1 < RB_SUB((double)c.cols, 3.0) && fy1 < RB_SUB((double)c.rows, 3.0))) return 0;
+  b->geo = 1;
+  b->col_lo = (int)floor(fx0) - 1; b->col_hi = (int)floor(fx1) + 3;      // [lo, hi)
+  b->row_lo = (int)floor(fy0) - 1; b->row_hi = (int)floor(fy1) + 3;
+  // the same bound as a disc: a rollout stays within Euclidean distance R of x0, so the cell it reads lies within
+  // R/res + sqrt(2) cells of the robot's (fractional) cell position; + 1.5 for float32 effects, rounded up
+  b->cx = (float)RB_DIV(RB_SUB(x, (double)c.pxl), res);
+  b->cy = (float)RB_DIV(RB_SUB(y, (double)c.pyl), res);
+  b->r = c.disc ? (float)RB_ADD(RB_DIV(R, res), 3.0) * 1.0001f : 0.0f;
+  // apply_box's narrowing of TDM 0's staged launch; a box whose launch does not fit samples whole maps
+  const int ncol = (c.cols + c.ty - 1) / c.ty;
+  b->tiy_lo = b->col_lo / ncol;
+  b->nact = (b->col_hi - 1) / ncol - b->tiy_lo + 1;
+  int gm = 128 / b->nact;                                // ~4 warps per CTA whatever the number of active tile columns
+  if (gm > SG_GM_MAX) gm = SG_GM_MAX;
+  if (gm > c.num_maps) gm = c.num_maps;
+  if (gm < 1) gm = 1;
+  b->gm = gm;
+  if (c.nt == 0 || !sample_v2_fits_hd(b->tiy_lo, b->nact, c.ty, c.cols, c.bpad0, c.bpad1, gm, c.nt)) return 0;
+  b->how = how;
+  return how;
+}
 // [emu:end sampler_args]
 bool build_sample_thresholds(double alpha, int q_cap, uint64_t* table /*[SAMPLE_TABLE_WORDS]*/);
 bool sample_grids_v2_fits(const SampleGridsV2Args& a, int nt);
@@ -61,6 +158,31 @@ bool sample_grids_v2_same_launch(const SampleGridsV2Args& a, const SampleGridsV2
 // active (device, may be null): active[pair] == 0 -> that pair's CTAs return at once (closed-loop trials)
 void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs, int count,
                                   const int* active, cudaStream_t st);
+// closed-loop trials of a stochastic batch: each pair's reach box decided on the device, from the x0 the plant step
+// wrote and the reach statistic of the step's first iteration (slot ^ (iter & 1)).  The decision goes to `record`:
+// [how, row_lo, row_hi, col_lo, col_hi] as b200mppi_planner_sample_box reports it.
+// [emu:begin box_desc]
+struct SampleBoxDesc {
+  ReachBoxConst c;
+  const float* x0;              // RolloutWinArgs::p.x0 of the pair's planner in the batch's device descriptors
+  const float* reach;           // the planner's two reach slots
+  int slot;                     // slot of the call's first iteration
+  int* record;                  // [5]
+  const uint64_t* jump_tile;    // [4][128][2] whole-tile advance matrices (advance_states_batch_kernel)
+};
+// [emu:end box_desc]
+// ONE launch for `count` fused pairs of equal geometry (geom: a whole-map plan with the boxed launch's segs / seg_rows /
+// jump and maps per CTA gm): mrows tile rows x the row segments x ncact tile columns, sized for the largest box of the
+// static bound; every CTA narrows to its pair's box and disc, whole maps loop over row and column groups.  No state
+// stores: launch_advance_states_batch advances the states.
+void launch_sample_grids_v2_box_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
+                                      const SampleBoxDesc* boxes, int count, const int* active, int iter, int mrows,
+                                      int ncact, cudaStream_t st);
+// the launch above holds ncact tile columns with geom.gm maps per CTA (threads, shared memory)
+bool sample_box_batch_fits(const SampleGridsV2Args& geom, int ncact);
+// launch_advance_states for `count` pairs (pair blockIdx.y): descs[y].t[0].states -> both TDMs' states_out
+void launch_advance_states_batch(const SampleGridsV2Args* descs, const SampleBoxDesc* boxes, int count, int rows,
+                                 int cols, int tx, int ty, int num_maps, const int* active, cudaStream_t st);
 // tile classes of a generator: (full | last) tile height x (full | last) tile width -> draws per whole-map walk
 void sample_tile_draws(int rows, int cols, int tx, int ty, int64_t ks[4]);
 // states_out[g] = states[g] advanced by the draws of a whole-map walk of generator g's tile (GF(2) jump with
@@ -181,8 +303,9 @@ struct NoisePrepDesc {
   float std_v, std_w, lambda, sv2, sw2, v_lo, v_hi, w_lo, w_hi;
 };
 // [emu:end noise_prep_desc]
+// active (device, may be null): active[y] == 0 -> that planner is left untouched (closed-loop trials)
 void launch_noise_prepare_batch(const NoisePrepDesc* descs, int count, int N, int T, int npad, int iter,
-                                cudaStream_t st);
+                                const int* active, cudaStream_t st);
 bool make_u8_tensor_map(void* out_map, const void* base, int rank, int cols, int rows, int maps, int pitch,
                         int WW, int WH);
 void rollout_win_geometry(int T, int* WW, int* WH, size_t* smem);
@@ -195,8 +318,9 @@ int rollout_win_batch_height(int T);
 // ONE persistent launch over the (planner, map) units of `count` planners of equal N, M, T: g = the launch-wide fields
 // (p.N, p.M, p.T, npad, WH), descs = device array of each planner's own RolloutWinArgs, tmaps = device array (64-byte
 // aligned) of 4 encoded tensor maps per planner (lin, ang, obstacle, unknown); masks01: every planner's masks are 0/1
+// active (device, may be null): the units of a planner with active[k] == 0 are skipped (closed-loop trials)
 cudaError_t launch_rollout_win_batch(const RolloutWinArgs& g, const RolloutWinArgs* descs, const void* tmaps, int count,
-                                     bool masks01, cudaStream_t st);
+                                     bool masks01, const int* active, cudaStream_t st);
 // CVaR over M (mppi.py:718-755): costs[n] = mean of the ceil(M*alpha) largest of costs_mn[:, n]
 // costs_mn is map-major: (M, n_cnt) with row stride ld -- the local buffer of a one-rank solve, or the receive buffer
 // of a map-sharded solve (rows g*M/ws .. = rank g's maps): the same kernel, the same values per lane, hence
@@ -212,6 +336,7 @@ struct CvarDesc {
   const float* costs_mn;    // map-major (M, ld)
   float* costs;             // (n_cnt)
   int n_cnt, ld, M, numel;  // numel = ceil(M * cvar_alpha) clamped to [1, M], as launch_cvar computes it
+  const int* active;        // may be null: *active == 0 -> the planner is left untouched (closed-loop trials)
 };
 // [emu:end cvar_desc]
 int cvar_numel(int M, float cvar_alpha);
@@ -264,12 +389,41 @@ void launch_shift_u(float* u, int T, int shifts, cudaStream_t st);
 // closed-loop trials of a batch (b200mppi_batch_run_trials): the plant step of every running planner, one warp each
 // [emu:begin trial_args]
 enum { TRIAL_RUNNING = 0, TRIAL_GOAL = 1, TRIAL_MAX_STEPS = 2, TRIAL_LEFT_MAP = 3 };
+// The window of a rollout from x0 (fill_win_args in api.cu, and the plant step of stochastic trials): WW x WH cells
+// centred on the robot's cell, kept INSIDE the map (origin clamped, extents cut), the x origin floored to a multiple of
+// 16 (TMA: 16-byte aligned inner start coordinate, also for negatives).  A staged cell is then always a map cell; indices
+// outside the map take the generic kernel's wrap + clamp.  f = &RolloutWinArgs::WW: {WW, WH, wx0, wy0, ww, wh}.
+__host__ __device__ inline void win_origin(float x0x, float x0y, float pxl, float pyl, float res, int cols, int rows,
+                                           int* f) {
+#ifdef __CUDA_ARCH__
+  const int xi0 = (int)floor(__ddiv_rn(__dsub_rn((double)x0x, (double)pxl), (double)res));
+  const int yi0 = (int)floor(__ddiv_rn(__dsub_rn((double)x0y, (double)pyl), (double)res));
+#else
+  const int xi0 = (int)floor(((double)x0x - (double)pxl) / (double)res);
+  const int yi0 = (int)floor(((double)x0y - (double)pyl) / (double)res);
+#endif
+  const int WW = f[0], WH = f[1];
+  int cx = xi0 - WW / 2, cy = yi0 - WH / 2;
+  if (cx > cols - WW) cx = cols - WW;
+  if (cx < 0) cx = 0;
+  if (cy > rows - WH) cy = rows - WH;
+  if (cy < 0) cy = 0;
+  f[2] = cx & ~15;
+  f[3] = cy;
+  f[4] = WW < cols - f[2] ? WW : cols - f[2];
+  f[5] = WH < rows - f[3] ? WH : rows - f[3];
+}
 struct TrialDev {
   const double* lin; const double* ang;   // ground-truth traction (H, W), float64
   int H, W;
   double xlo, ylo, res, dt, xgoal[2], tol, pxlim[2], pylim[2];
   float* u_cur;                           // (T, 2): u_cur[0] is applied, then the sequence is shifted by one
   float* x0_out;                          // RolloutArgs::p.x0 of this planner in the batch's device descriptors
+  // stochastic trials: &RolloutWinArgs::WW of the planner in the batch's device descriptors (x0_out points into the
+  // same record), whose window is recomputed from the new x0 (win_origin) over the map of the planner's TDMs; else null
+  int* win;
+  float win_pxl, win_pyl, win_res;
+  int win_rows, win_cols;
 };
 struct TrialState {
   double x[3], cum_obj, cum_dist, dist;

@@ -410,6 +410,7 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
   xh[0] = xn; xh[1] = yn; xh[2] = thn;
   // the next rollout starts from float32(x_next), as set_params would pass it
   d.x0_out[0] = __double2float_rn(xn); d.x0_out[1] = __double2float_rn(yn); d.x0_out[2] = __double2float_rn(thn);
+  if (d.win) win_origin(d.x0_out[0], d.x0_out[1], d.win_pxl, d.win_pyl, d.win_res, d.win_cols, d.win_rows, d.win);
   const double dx = __dsub_rn(xn, d.xgoal[0]), dy = __dsub_rn(yn, d.xgoal[1]);
   const double dist = __dsub_rn(__dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy))), d.tol);
   s.cum_obj = __dadd_rn(s.cum_obj, __dadd_rn(d.dt, dist));

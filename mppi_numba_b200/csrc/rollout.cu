@@ -395,6 +395,7 @@ __global__ void __launch_bounds__(CVAR_LARGE_THREADS) cvar_large_kernel(const fl
 template <int PER>
 __global__ void __launch_bounds__(CVAR_THREADS) cvar_batch_kernel(const CvarDesc* __restrict__ descs) {
   const CvarDesc& d = descs[blockIdx.y];
+  if (d.active && !*d.active) return;
   cvar_body<PER>(d.costs_mn, d.costs, d.n_cnt, d.ld, d.M, d.numel);
 }
 // [emu:end cvar_batch]

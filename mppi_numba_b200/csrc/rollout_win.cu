@@ -182,7 +182,9 @@ __global__ void __launch_bounds__(256) noise_prepare_kernel(uint64_t* __restrict
 // iteration, as in its own solve()
 // [emu:begin noise_prepare_batch]
 __global__ void __launch_bounds__(256) noise_prepare_batch_kernel(const NoisePrepDesc* __restrict__ descs, int N, int T,
-                                                                  int npad, int iter) {
+                                                                  int npad, int iter,
+                                                                  const int* __restrict__ active = nullptr) {
+  if (active && !active[blockIdx.y]) return;
   const NoisePrepDesc& d = descs[blockIdx.y];
   noise_prepare_body(d.states, reinterpret_cast<float2*>(d.noise), d.u_cur, reinterpret_cast<double2*>(d.noiseT), d.ctrl,
                      d.reach, d.slot ^ (iter & 1), N, T, npad, d.std_v, d.std_w, d.lambda, d.sv2, d.sw2, d.v_lo, d.v_hi,
@@ -198,8 +200,9 @@ void launch_noise_prepare(uint64_t* states, float* noise, const float* u_cur, fl
                                                  wrange[0], wrange[1]);
 }
 void launch_noise_prepare_batch(const NoisePrepDesc* descs, int count, int N, int T, int npad, int iter,
-                                cudaStream_t st) {
-  noise_prepare_batch_kernel<<<dim3((unsigned)(npad / NP_NB), (unsigned)count), 256, 0, st>>>(descs, N, T, npad, iter);
+                                const int* active, cudaStream_t st) {
+  noise_prepare_batch_kernel<<<dim3((unsigned)(npad / NP_NB), (unsigned)count), 256, 0, st>>>(descs, N, T, npad, iter,
+                                                                                               active);
 }
 void launch_prepare_rollout(const float* noise, const float* u_cur, float* noiseT, float* ctrl, float* reach, int N,
                             int T, int npad, float lambda, float std_v, float std_w, const float vrange[2],
@@ -399,7 +402,7 @@ template <int THREADS, int WH, bool MASK01, bool BATCH>
 __device__ __forceinline__ void rollout_win_body(const RolloutWinArgs& g, const CUtensorMap* tm_lin,
                                                  const CUtensorMap* tm_ang, const CUtensorMap* tm_obs,
                                                  const CUtensorMap* tm_unk, const RolloutWinArgs* descs,
-                                                 const CUtensorMap* tmaps, int count) {
+                                                 const CUtensorMap* tmaps, int count, const int* active) {
   extern __shared__ __align__(128) unsigned char smem[];
   constexpr int WW = WIN_WW;
   constexpr int PLANE = WW * WH;
@@ -486,6 +489,9 @@ __device__ __forceinline__ void rollout_win_body(const RolloutWinArgs& g, const 
     const int c_lo = (int)(w - (long long)u * cpm);
     const int c_hi = (int)min((long long)cpm, w_hi - (long long)u * cpm);       // this map's part of the share
     w += c_hi - c_lo;
+    if constexpr (BATCH) {
+      if (active && !active[u / g.p.M]) continue;           // a stopped planner (closed-loop trials): CTA-uniform
+    }
     __syncthreads();                                        // every warp has left the previous window (and the tables are written)
     if constexpr (BATCH) {
       const int k = u / g.p.M;                              // CTA-uniform
@@ -667,7 +673,7 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
                                                                  const __grid_constant__ CUtensorMap tm_ang,
                                                                  const __grid_constant__ CUtensorMap tm_obs,
                                                                  const __grid_constant__ CUtensorMap tm_unk) {
-  rollout_win_body<THREADS, WH, MASK01, false>(a, &tm_lin, &tm_ang, &tm_obs, &tm_unk, nullptr, nullptr, 1);
+  rollout_win_body<THREADS, WH, MASK01, false>(a, &tm_lin, &tm_ang, &tm_obs, &tm_unk, nullptr, nullptr, 1, nullptr);
 }
 
 // [emu:end win_kernel]
@@ -675,8 +681,9 @@ __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWi
 template <int THREADS, int WH, bool MASK01>
 __global__ void __launch_bounds__(THREADS, 1) rollout_win_batch_kernel(const RolloutWinArgs g,
                                                                        const RolloutWinArgs* __restrict__ descs,
-                                                                       const CUtensorMap* __restrict__ tmaps, int count) {
-  rollout_win_body<THREADS, WH, MASK01, true>(g, nullptr, nullptr, nullptr, nullptr, descs, tmaps, count);
+                                                                       const CUtensorMap* __restrict__ tmaps, int count,
+                                                                       const int* __restrict__ active = nullptr) {
+  rollout_win_body<THREADS, WH, MASK01, true>(g, nullptr, nullptr, nullptr, nullptr, descs, tmaps, count, active);
 }
 // [emu:end win_batch]
 // ---------------------------------------------------------------------------------------------
@@ -828,8 +835,8 @@ int rollout_win_batch_height(int T) { return win_batch_smem(232, T) <= (size_t)W
 // The launch-wide choices of launch_rollout_win (persistent CTAs, share unit) over units = count * M; its tuning hooks
 // (B200MPPI_WIN_*) and the debug hook are not applied to batched launches.
 cudaError_t launch_rollout_win_batch(const RolloutWinArgs& g, const RolloutWinArgs* descs, const void* tmaps, int count,
-                                     bool masks01, cudaStream_t st) {
-  typedef void (*WinBatchKernel)(const RolloutWinArgs, const RolloutWinArgs*, const CUtensorMap*, int);
+                                     bool masks01, const int* active, cudaStream_t st) {
+  typedef void (*WinBatchKernel)(const RolloutWinArgs, const RolloutWinArgs*, const CUtensorMap*, int, const int*);
   static const WinBatchKernel kernels[2][2] = {
       {rollout_win_batch_kernel<WIN_THREADS, 232, false>, rollout_win_batch_kernel<WIN_THREADS, 232, true>},
       {rollout_win_batch_kernel<WIN_THREADS, 224, false>, rollout_win_batch_kernel<WIN_THREADS, 224, true>}};
@@ -856,7 +863,7 @@ cudaError_t launch_rollout_win_batch(const RolloutWinArgs& g, const RolloutWinAr
   b.sync_passes = (total + 32LL * grid.x - 1) / (32LL * grid.x) <= WIN_SYNC_MAX_PASSES;
   b.stagger = WIN_STAGGER_DEFAULT; b.rotate = 0; b.dbg = nullptr; b.sig = CostSignal{};
   kernels[g.WH == 232 ? 0 : 1][masks01 ? 1 : 0]<<<grid, WIN_THREADS, smem, st>>>(
-      b, descs, reinterpret_cast<const CUtensorMap*>(tmaps), count);
+      b, descs, reinterpret_cast<const CUtensorMap*>(tmaps), count, active);
   return cudaGetLastError();
 }
 

@@ -429,9 +429,9 @@ __global__ void __launch_bounds__(256, 4) sample_grids_v2_kernel(const SampleGri
 
 // whole-tile advance of every generator (box mode: the sampler walks only part of each tile, so the states a
 // whole-map walk would leave behind are produced by ONE GF(2) jump per generator).  Tile classes as sample_tile_draws.
-__global__ void __launch_bounds__(128) advance_states_kernel(const ulonglong2* __restrict__ in, ulonglong2* __restrict__ out0,
-                                                             ulonglong2* __restrict__ out1, const ulonglong2* __restrict__ mats,
-                                                             int rows, int cols, int tx, int ty, int num_maps) {
+__device__ __forceinline__ void advance_states_body(const ulonglong2* __restrict__ in, ulonglong2* __restrict__ out0,
+                                                    ulonglong2* __restrict__ out1, const ulonglong2* __restrict__ mats,
+                                                    int rows, int cols, int tx, int ty, int num_maps) {
   extern __shared__ __align__(16) unsigned char smem[];
   ulonglong2* s_M = reinterpret_cast<ulonglong2*>(smem);      // the four tile-class matrices, 8 KB
   for (int i = threadIdx.x; i < 4 * 128; i += blockDim.x) s_M[i] = __ldg(mats + i);
@@ -448,6 +448,11 @@ __global__ void __launch_bounds__(128) advance_states_kernel(const ulonglong2* _
   out0[gen] = make_ulonglong2(s.s0, s.s1);
   if (out1) out1[gen] = make_ulonglong2(s.s0, s.s1);
 }
+__global__ void __launch_bounds__(128) advance_states_kernel(const ulonglong2* __restrict__ in, ulonglong2* __restrict__ out0,
+                                                             ulonglong2* __restrict__ out1, const ulonglong2* __restrict__ mats,
+                                                             int rows, int cols, int tx, int ty, int num_maps) {
+  advance_states_body(in, out0, out1, mats, rows, cols, tx, ty, num_maps);
+}
 
 // [emu:end sampler_v2]
 // [emu:begin sampler_batch]
@@ -462,6 +467,66 @@ __global__ void __launch_bounds__(256) sample_grids_v2_batch_kernel(const Sample
   sample_grids_v2_body<NT, NW>(descs[blockIdx.z]);
 }
 // [emu:end sampler_batch]
+// [emu:begin sampler_box_batch]
+// closed-loop trials of a stochastic batch: the fused pair blockIdx.z samples the reach box its planner's solve() would
+// sample (reach_box_decide from the x0 the plant step wrote and this step's reach statistic), or whole maps.  The launch
+// is sized for the largest box the static bound allows: `mrows` tile rows times the pair's box row segments, `ncact`
+// tile columns and the boxed launch's maps per CTA (a.gm).  A boxed step is one pass whose tile rows start at the box's
+// first one; a CTA narrows to the box rows, columns and disc as the single boxed launch does, so it writes the same
+// cells with the same draws.  A whole-map step (and any box larger than the launch) loops over groups of mrows tile rows
+// and ncact tile columns.
+template <int NW>
+__global__ void __launch_bounds__(256) sample_grids_v2_box_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
+                                                                        const SampleBoxDesc* __restrict__ boxes,
+                                                                        const int* __restrict__ active, int iter,
+                                                                        int mrows, int ncact) {
+  if (active && !active[blockIdx.z]) return;
+  SampleGridsV2Args a = descs[blockIdx.z];
+  const SampleBoxDesc& bd = boxes[blockIdx.z];
+  const float reach = bd.reach[bd.slot ^ (iter & 1)];
+  ReachBox b;
+  const int how = reach_box_decide(bd.c, bd.x0[0], bd.x0[1], bd.c.mode == 2 ? &reach : nullptr, &b);
+  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
+    bd.record[0] = how;
+    bd.record[1] = how ? b.row_lo : 0; bd.record[2] = how ? b.row_hi : a.rows;
+    bd.record[3] = how ? b.col_lo : 0; bd.record[4] = how ? b.col_hi : a.cols;
+  }
+  const int nrow = (a.rows + a.tx - 1) / a.tx;
+  int tix_lo = 0, tix_hi = a.tx, tiy_lo = 0, tiy_hi = a.ty;          // tile rows / columns to cover, [lo, hi)
+  if (how) {
+    a.row_lo = b.row_lo; a.row_hi = b.row_hi;
+    a.disc_cx = b.cx; a.disc_cy = b.cy; a.disc_r = b.r;
+    tix_lo = b.row_lo / nrow; tix_hi = min(a.tx, (b.row_hi - 1) / nrow + 1);
+    tiy_lo = b.tiy_lo; tiy_hi = b.tiy_lo + b.nact;
+  }
+  a.write_states = 0;
+  const int tsub = (int)blockIdx.x / a.segs, seg = (int)blockIdx.x % a.segs;
+  for (int tg = tix_lo; tg < tix_hi; tg += mrows) {
+    const int tix = tg + tsub;
+    if (tix >= tix_hi) continue;                                   // CTA-uniform
+    const int t0 = min(tix * nrow, a.rows), t1 = min(t0 + nrow, a.rows);
+    const int r0 = min(t0 + seg * a.seg_rows, t1), r1 = min(r0 + a.seg_rows, t1);
+    if (max(r0, a.row_lo) >= min(r1, a.row_hi)) continue;          // no box rows in this segment
+    for (int cg = tiy_lo; cg < tiy_hi; cg += ncact) {
+      a.tix_lo = tg; a.tiy_lo = cg; a.nact = min(ncact, tiy_hi - cg);
+      sample_grids_v2_body<2, NW>(a);
+      __syncthreads();                                             // the next pass restages the shared memory
+    }
+  }
+}
+
+// the state advance of those boxed samplings for every pair (pair blockIdx.y): lin's states into both TDMs' other buffers
+__global__ void __launch_bounds__(128) advance_states_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
+                                                                   const SampleBoxDesc* __restrict__ boxes,
+                                                                   const int* __restrict__ active, int rows, int cols,
+                                                                   int tx, int ty, int num_maps) {
+  if (active && !active[blockIdx.y]) return;
+  const SampleGridsV2Args& a = descs[blockIdx.y];
+  advance_states_body(reinterpret_cast<const ulonglong2*>(a.t[0].states), reinterpret_cast<ulonglong2*>(a.t[0].states_out),
+                      reinterpret_cast<ulonglong2*>(a.t[1].states_out),
+                      reinterpret_cast<const ulonglong2*>(boxes[blockIdx.y].jump_tile), rows, cols, tx, ty, num_maps);
+}
+// [emu:end sampler_box_batch]
 
 void launch_advance_states(const uint64_t* states, uint64_t* out0, uint64_t* out1, const uint64_t* mats, int rows,
                            int cols, int tx, int ty, int num_maps, cudaStream_t st) {
@@ -481,19 +546,8 @@ void sample_tile_draws(int rows, int cols, int tx, int ty, int64_t ks[4]) {
   ks[2] = (int64_t)last_h * ncol; ks[3] = (int64_t)last_h * last_w;
 }
 
-static int v2_window_cols(const SampleGridsV2Args& a) {
-  const int ncol = (a.cols + a.ty - 1) / a.ty;
-  const int cfirst = std::min(a.tiy_lo * ncol, a.cols);
-  const int cs1 = std::min((a.tiy_lo + a.nact) * ncol, a.cols);
-  return cs1 - (cfirst & ~15);
-}
-
 size_t sample_grids_v2_smem(const SampleGridsV2Args& a, int nt) {
-  const int wcols = v2_window_cols(a);
-  const int row_bytes_al = (wcols * a.t[0].bpad + 15) & ~15;
-  const int stage_pitch = (wcols + 15) & ~15;
-  const size_t stage = std::max((size_t)nt * a.gm * stage_pitch, (size_t)2 * 128 * 16);     // the jump matrices overlay it
-  return (size_t)nt * row_bytes_al + stage + SAMPLE_TABLE_WORDS * 8 + (size_t)nt * 128;
+  return sample_v2_smem_hd(a.tiy_lo, a.nact, a.ty, a.cols, a.t[0].bpad, a.gm, nt);
 }
 
 static int v2_threads(const SampleGridsV2Args& a) { return ((a.nact * a.gm + 31) / 32) * 32; }
@@ -517,9 +571,7 @@ static void launch_v2_nt(const SampleGridsV2Args& a, cudaStream_t st) {
 }
 
 bool sample_grids_v2_fits(const SampleGridsV2Args& a, int nt) {
-  return a.gm >= 1 && a.gm <= SG_GM_MAX && a.nact >= 1 && a.tiy_lo >= 0 && a.tiy_lo + a.nact <= a.ty &&
-         v2_threads(a) <= 256 && a.t[0].bpad <= 32 && sample_grids_v2_smem(a, nt) <= 200 * 1024 &&
-         (nt == 1 || a.t[0].bpad == a.t[1].bpad);
+  return sample_v2_fits_hd(a.tiy_lo, a.nact, a.ty, a.cols, a.t[0].bpad, a.t[1].bpad, a.gm, nt);
 }
 
 void launch_sample_grids_v2(const SampleGridsV2Args& a, int nt, cudaStream_t st) {
@@ -549,6 +601,44 @@ void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGri
   else if (nw == 8) go(sample_grids_v2_batch_kernel<2, 8>);
   else if (nw == 1) go(sample_grids_v2_batch_kernel<2, 1>);
   else go(sample_grids_v2_batch_kernel<2, 0>);
+}
+
+// shared memory of the box batch launch: the widest window of ncact tile columns anywhere in the map
+static size_t box_batch_smem(const SampleGridsV2Args& geom, int ncact) {
+  size_t smem = 0;
+  for (int lo = 0; lo + ncact <= geom.ty; ++lo)
+    smem = std::max(smem, sample_v2_smem_hd(lo, ncact, geom.ty, geom.cols, geom.t[0].bpad, geom.gm, 2));
+  return smem;
+}
+
+bool sample_box_batch_fits(const SampleGridsV2Args& geom, int ncact) {
+  return ncact >= 1 && ncact <= geom.ty && sample_v2_fits_hd(0, ncact, geom.ty, geom.cols, geom.t[0].bpad,
+                                                             geom.t[1].bpad, geom.gm, 2) &&
+         box_batch_smem(geom, ncact) <= 200 * 1024;
+}
+
+void launch_sample_grids_v2_box_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
+                                      const SampleBoxDesc* boxes, int count, const int* active, int iter, int mrows,
+                                      int ncact, cudaStream_t st) {
+  const dim3 grid(mrows * geom.segs, (geom.num_maps + geom.gm - 1) / geom.gm, count);
+  const int threads = ((ncact * geom.gm + 31) / 32) * 32;
+  const size_t smem = box_batch_smem(geom, ncact);
+  const int nw = geom.t[0].bpad / 4;
+  auto go = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    kern<<<grid, threads, smem, st>>>(descs, boxes, active, iter, mrows, ncact);
+  };
+  if (nw == 3) go(sample_grids_v2_box_batch_kernel<3>);
+  else if (nw == 8) go(sample_grids_v2_box_batch_kernel<8>);
+  else if (nw == 1) go(sample_grids_v2_box_batch_kernel<1>);
+  else go(sample_grids_v2_box_batch_kernel<0>);
+}
+
+void launch_advance_states_batch(const SampleGridsV2Args* descs, const SampleBoxDesc* boxes, int count, int rows,
+                                 int cols, int tx, int ty, int num_maps, const int* active, cudaStream_t st) {
+  const int64_t total = (int64_t)tx * ty * num_maps;
+  advance_states_batch_kernel<<<dim3((unsigned)((total + 127) / 128), (unsigned)count), 128, 4 * 128 * 16, st>>>(
+      descs, boxes, active, rows, cols, tx, ty, num_maps);
 }
 
 static inline void next_h(uint64_t& s0, uint64_t& s1);
