@@ -2436,7 +2436,8 @@ extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b20
   }
   // the one sampler launch is sized for the largest box the static bound allows (reach_box_decide: at most 2 R / res + 5
   // cells a side) over all planners that sample a box: mrows tile rows x ncact tile columns with the boxed launch's maps
-  // per CTA.  Whole-map steps loop over such groups.
+  // per CTA.  Whole-map steps loop over such groups.  x0 moves during a trial, so R's rounding terms take their bounds
+  // from the padded map's limits (a box exists only for an x0 inside them).
   const SampleGridsV2Args& sg = plans[0].a[0];
   const int nrow = (sg.rows + sg.tx - 1) / sg.tx, ncol = (sg.cols + sg.ty - 1) / sg.ty;
   double span = 0.0;                                  // cells a side, + margin
@@ -2445,9 +2446,13 @@ extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b20
     ReachBoxConst c;
     fill_reach_const(b->pl[i], plans[i], &c);
     if (c.mode == 0) continue;
+    const double w = (double)c.cols * (double)c.res, h = (double)c.rows * (double)c.res;
+    const double A = std::fmax(std::fabs((double)c.pxl), std::fabs((double)c.pxl + w)) +
+                     std::fmax(std::fabs((double)c.pyl), std::fabs((double)c.pyl + h));
+    const double R = reach_radius(c, (double)c.T * std::fmax(std::fabs((double)c.vr0), std::fabs((double)c.vr1)), A,
+                                  w + h);
+    if (!(R >= 0.0)) continue;                        // that planner never gets a box
     any_box = true;
-    const double R = (double)c.dt * (double)c.tr_abs_max * ((double)c.T * std::fmax(std::fabs((double)c.vr0),
-                                                                                       std::fabs((double)c.vr1))) * 1.0002;
     span = std::fmax(span, 2.0 * R / (double)c.res + 8.0);
   }
   int mrows = sg.tx, ncact = sg.ty;

@@ -76,6 +76,9 @@ __host__ __device__ inline bool sample_v2_fits_hd(int tiy_lo, int nact, int ty, 
 // over the N control sequences actually drawn.  Whole maps (0) whenever the bound is not airtight: the box would leave
 // the map (out-of-map indices wrap), non-finite inputs, a reach beyond the speed limit.  Float64 operations are
 // explicitly rounded on the device, so host and device decide alike.
+// Float32 rounding moves a rollout further than that: every step stores x = f32(x + dv cos th), up to half an ulp of |x|
+// away, so far from the origin (georeferenced maps) a displacement just above half an ulp rounds up to a whole one at
+// every step.  reach_radius adds that drift and the rounding of f32(x - xlo) in the cell index.
 #ifdef __CUDA_ARCH__
 #define RB_MUL(a, b) __dmul_rn(a, b)
 #define RB_ADD(a, b) __dadd_rn(a, b)
@@ -104,6 +107,23 @@ struct ReachBox {
   float cx, cy, r;              // reach disc in cells (r = 0: none)
   int tiy_lo, nact, gm;         // the boxed launch's tile columns and maps per CTA (how != 0)
 };
+// R in metres for a path length S (sum_t |v_t|) from a start x0 with |x0| + |y0| <= A and |x0 - pxl| + |y0 - pyl| <= B:
+// every cell a rollout reads at steps 0 .. T-1 lies within R of x0, per axis and in Euclidean distance.
+//   R0 = dt * max|traction| * S * 1.0002: the exact path (1.0002: cos/sin.approx may exceed 1 by ~1e-6).
+//   Each of the T state roundings is off by at most u |x|, |x| <= A + D (D: the distance travelled so far), so
+//   D <= R0 + T u (A + D), i.e. D <= (R0 + T u A) / (1 - T u).  u = 2^-24 rounded up also covers the float64 rounding of
+//   the FMA before the narrowing to float32.
+//   The cell index rounds x - xlo once more: u (|x0 - pxl| + |y0 - pyl| + 2 D).
+// Negative (no usable bound) when T u is not small.
+__host__ __device__ inline double reach_radius(const ReachBoxConst& c, double S, double A, double B) {
+  const double u = 5.9605e-8;                            // 2^-24 = 5.96046e-8
+  const double Tu = RB_MUL((double)c.T, u);
+  if (!(Tu < 0.5)) return -1.0;
+  const double R0 = RB_MUL(RB_MUL(RB_MUL((double)c.dt, (double)c.tr_abs_max), S), 1.0002);
+  if (!(R0 >= 0.0)) return -1.0;                         // negative or NaN
+  const double D = RB_DIV(RB_ADD(R0, RB_MUL(Tu, A)), RB_SUB(1.0, Tu));
+  return RB_ADD(D, RB_MUL(u, RB_ADD(B, RB_MUL(2.0, D))));
+}
 __host__ __device__ inline int reach_box_decide(const ReachBoxConst& c, float x0x, float x0y, const float* reach,
                                                 ReachBox* b) {
   b->geo = 0; b->how = 0;
@@ -118,10 +138,11 @@ __host__ __device__ inline int reach_box_decide(const ReachBoxConst& c, float x0
     S = (double)*reach;
     how = 2;
   }
-  // 1.0002: cos/sin.approx may exceed 1 by ~1e-6, float32 rounding of the state adds ~1e-7 per step; + one cell below
-  const double R = RB_MUL(RB_MUL(RB_MUL((double)c.dt, (double)c.tr_abs_max), S), 1.0002);
-  if (!(R >= 0.0 && R <= 1.7976931348623157e308)) return 0;      // negative, NaN or infinite
+  // R from the start's own coordinates; the box adds a cell of margin on each side below
   const double res = (double)c.res, x = (double)x0x, y = (double)x0y;
+  const double R = reach_radius(c, S, RB_ADD(fabs(x), fabs(y)),
+                                RB_ADD(fabs(RB_SUB(x, (double)c.pxl)), fabs(RB_SUB(y, (double)c.pyl))));
+  if (!(R >= 0.0 && R <= 1.7976931348623157e308)) return 0;      // negative, NaN or infinite
   const double fx0 = RB_DIV(RB_SUB(RB_SUB(x, R), (double)c.pxl), res);
   const double fx1 = RB_DIV(RB_SUB(RB_ADD(x, R), (double)c.pxl), res);
   const double fy0 = RB_DIV(RB_SUB(RB_SUB(y, R), (double)c.pyl), res);

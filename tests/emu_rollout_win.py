@@ -195,6 +195,18 @@ extern "C" int emu_noise_prepare(const uint64_t* states_in, const float* u_cur, 
   return 0;
 }
 
+// the prepare kernel alone on given noise (N, T, 2): its reach statistic max_n sum_t |clip(u_v + e_v)| (round-up adds)
+extern "C" float emu_prepare_reach(const float* noise, const float* u_cur, int N, int T, const float* vr, const float* wr) {
+  using namespace b200;
+  const int npad = (N + 31) / 32 * 32;
+  std::vector<double2> noiseT((size_t)T * npad, double2{0, 0});
+  std::vector<float> ctrl(npad, 0.0f);
+  float reach = 0.0f;
+  run([&] { prepare_rollout_kernel(reinterpret_cast<const float2*>(noise), u_cur, noiseT.data(), ctrl.data(), &reach, N, T,
+                                   npad, 1.0f, 1.0f, 1.0f, vr[0], vr[1], wr[0], wr[1]); }, 256, (unsigned)(npad / 32), 1);
+  return reach;
+}
+
 // cell_from_interval (the division-free decision of the rare path) against the reference's exact sequence:
 // out_new[i] = the kernel's result for a[i] (magic-number floors of the interval's ends, then cell_from_interval),
 // out_ref[i] = cell_index_exact(a[i], res); differ[i] = 1 when the floors differed (the decision ran)
@@ -316,6 +328,8 @@ def build(out_dir):
     lib.emu_noise_prepare.restype = I
     lib.emu_noise_prepare.argtypes = [P, P, I, I, C.c_float, C.c_float, C.c_float, P, P, P, P, P, P, P]
     lib.emu_rollout_win.restype = I
+    lib.emu_prepare_reach.restype = C.c_float
+    lib.emu_prepare_reach.argtypes = [P, P, I, I, P, P]
     lib.emu_cell_between.argtypes = [P, I, C.c_float, P, P, P]
     lib.emu_cell_between.restype = None
     lib.emu_rollout_win.argtypes = [P, P, P, P, P, P, P, P, P, P, I, I, P, P, I, I, I, I, I]

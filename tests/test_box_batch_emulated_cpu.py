@@ -173,7 +173,10 @@ def test_box_batch_equals_per_pair_boxed_launches(libs, case):
     reach = np.array([3.9, 2.1, 1.0, 100.0, 0.0, 4.0], dtype=np.float32)
     active = np.array([1, 1, 1, 1, 1, 0], dtype=np.int32)
     K = len(x0)
-    span = 2 * dt * trm * T_ * vmax * 1.0002 / res + 8
+    # b200mppi_batch_run_stochastic_trials: R of the speed limit with the rounding terms bounded by the map's limits
+    u, w, h = 5.9605e-8, cols * res, rows * res
+    D = (dt * trm * T_ * vmax * 1.0002 + T_ * u * (w + h)) / (1 - T_ * u)
+    span = 2 * (D + u * (w + h + 2 * D)) / res + 8
     nrow, ncol = -(-rows // tx), -(-cols // ty)
     mrows, ncact = min(tx, int(span) // nrow + 2), min(ty, int(span) // ncol + 2)
     if case == "wide_box":                     # a launch narrower than the box: the group loop covers it

@@ -1024,10 +1024,13 @@ def test_boxed_solve_identical_to_whole_map_solve(eng, monkeypatch, N, M, T, H, 
     ref = runs["off"]
     assert all(m[0] == 0 for m in ref["modes"])
     # a box that would leave the map is not used (whole maps); the box from the controls is the tighter one.
-    # speed-limit box of the FIRST solve (planner_reach_box, api.cu): R = dt * max|traction| * T * vmax * 1.0002
+    # speed-limit box of the FIRST solve (reach_radius, kernels.h): R = dt * max|traction| * T * vmax * 1.0002 plus the
+    # float32 rounding of the state and of the cell index
     pad = int(np.ceil(5.0 * 0.1 / res))
-    R = 0.1 * 1.0 * T * 3.0 * 1.0002
-    c0 = sc["params"]["x0"][:2]
+    c0 = sc["params"]["x0"][:2].astype(np.float32).astype(np.float64)
+    u, pxl = 5.9605e-8, float(np.float32(-pad * res))
+    D = (0.1 * 1.0 * T * 3.0 * 1.0002 + T * u * np.abs(c0).sum()) / (1 - T * u)
+    R = D + u * (np.abs(c0 - pxl).sum() + 2 * D)
     static_fits = all((c - R + pad * res) / res > 2.0 and (c + R + pad * res) / res < H + 2 * pad - 3.0 for c in c0)
     assert runs["static"]["modes"][0][0] == (1 if static_fits else 0), runs["static"]["modes"]
     assert all(m[0] in (0, 1) for m in runs["static"]["modes"])

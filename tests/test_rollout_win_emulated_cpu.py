@@ -226,6 +226,48 @@ def test_fused_noise_and_controls_kernel_equals_the_two_kernels(emu, N, T):
     assert (noiseT[:, :N, 1] == np.clip(u_cur[:, None, 1] + noise[:, :, 1].T, F32(-np.pi), F32(np.pi)).astype(np.float64)).all()
 
 
+@pytest.mark.parametrize("case", ["big_then_tiny", "tiny_then_big", "reverse", "reverse_tiny", "random"])
+def test_reach_statistic_bounds_the_exact_path_length(emu, case):
+    """The reach box rests on the prepare kernel's statistic: it must never fall below the exact float64 sum of the
+    float32 |v| each rollout uses, even where a round-to-nearest float32 sum loses terms (T = 1024: one large |v| and
+    1023 tiny ones below half its ulp), nor with a negative vrange (reverse driving).  Round-up adds overshoot by at
+    most one ulp of the sum per step."""
+    win, _ = emu
+    N, T = 70, 1024
+    rng = np.random.default_rng(len(case))
+    vr = _c({"reverse": [-3, -0.5], "reverse_tiny": [-3, 0]}.get(case, [0, 3]), F32)
+    wr = _c([-np.pi, np.pi], F32)
+    u_cur = np.zeros((T, 2), F32)
+    noise = np.zeros((N, T, 2), F32)
+    if case == "big_then_tiny":
+        u_cur[0, 0] = 2.5
+        noise[:, 1:, 0] = rng.uniform(1e-8, 1e-7, (N, T - 1))          # each below half an ulp of 2.5 (1.2e-7)
+    elif case == "tiny_then_big":
+        noise[:, :-1, 0] = rng.uniform(1e-9, 3e-8, (N, T - 1))
+        u_cur[-1, 0] = 2.9
+    elif case == "reverse":
+        u_cur[:, 0] = -1.7
+        noise[..., 0] = rng.standard_normal((N, T)) * 0.8
+    elif case == "reverse_tiny":
+        u_cur[0, 0] = -2.75
+        noise[:, 1:, 0] = -rng.uniform(1e-8, 1e-7, (N, T - 1))
+    else:
+        u_cur[:, 0] = rng.uniform(0, 2, T)
+        noise[..., 0] = rng.standard_normal((N, T)) * 2
+    noise[..., 1] = rng.standard_normal((N, T))
+    noise = np.ascontiguousarray(noise)
+    reach = float(win.emu_prepare_reach(_p(noise), _p(u_cur), N, T, _p(vr), _p(wr)))
+    v = np.clip((u_cur[None, :, 0] + noise[..., 0]).astype(F32), vr[0], vr[1]).astype(F32)     # fminf / fmaxf clip
+    exact = np.abs(v.astype(np.float64)).sum(1)
+    assert reach >= exact.max(), (case, reach, exact.max())
+    assert reach <= exact.max() + T * float(np.spacing(F32(reach))), (case, reach, exact.max())
+    rn = np.zeros(N, F32)                                    # what a round-to-nearest float32 sum would have given
+    for t in range(T):
+        rn = (rn + np.abs(v[:, t])).astype(F32)
+    if case in ("big_then_tiny", "reverse_tiny"):
+        assert float(rn.max()) < exact.max()                 # the case is adversarial: round-to-nearest loses the tail
+
+
 def test_veltkamp_split_equals_float32_rounding_including_ties():
     """round_to_f32_precision (csrc/rollout_win.cu, WIN_ROUND_FP64): g = RN(a * (2^29 + 1)), hi = RN(g + RN(a - g)) must be
     the float64 value of float32(a) -- round to nearest, ties to EVEN -- for every magnitude the state can take.  numpy

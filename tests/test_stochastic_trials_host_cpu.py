@@ -1,8 +1,9 @@
 """Closed-loop trials of stochastic batches without a GPU: the C-ABI entry point (export, prototype as the header declares
 it, argument errors before any device work), MPPI_StochasticBatch.run_stochastic_trials on a fake backend (marshalling,
 logs and NaN conventions, refusals issuing nothing, run_trials still refused), and the shared host / device helpers
-compiled from the header's text for the host: the reach-box decision against a restatement of the decision solve()
-made before it was shared, and the window origin against fill_win_args' former code."""
+compiled from the header's text for the host: the reach-box decision against a host restatement of it (the decision
+solve() made before it was shared, with the float32 rounding terms of reach_radius), and the window origin against
+fill_win_args' former code."""
 import ctypes as C
 import os
 import re
@@ -187,9 +188,10 @@ def helpers(tmp_path_factory):
     return lib
 
 
-def former_decision(ci, cf, x, y, reach):
+def host_decision(ci, cf, x, y, reach):
     """planner_reach_box, apply_box and sample_grids_v2_fits as sample_finish combined them before the decision was
-    shared with the device: (last_box 5-tuple, disc) -- Python floats are IEEE doubles, float32 via numpy."""
+    shared with the device, R widened by the float32 rounding of the state and of the cell index (reach_radius):
+    (last_box 5-tuple, disc) -- Python floats are IEEE doubles, float32 via numpy."""
     mode, disc, T, rows, cols, nt, tx, ty, M, bp0, bp1 = ci
     vr0, vr1, dt, trm, res, pxl, pyl = [float(np.float32(v)) for v in cf]
     whole = ((0, 0, rows, 0, cols), None)
@@ -201,7 +203,14 @@ def former_decision(ci, cf, x, y, reach):
         if not float(np.float32(reach)) <= S:
             return whole
         S, how = float(np.float32(reach)), 2
-    R = dt * trm * S * 1.0002
+    # plus the float32 rounding of the state (T steps, at most 2^-24 |x| each) and of the cell index (reach_radius)
+    u = 5.9605e-8
+    Tu = T * u
+    R0 = dt * trm * S * 1.0002
+    if not Tu < 0.5 or not R0 >= 0.0:
+        return whole
+    D = (R0 + Tu * (abs(x) + abs(y))) / (1.0 - Tu)
+    R = D + u * ((abs(x - pxl) + abs(y - pyl)) + 2.0 * D)
     if not (R >= 0.0) or not np.isfinite(R):
         return whole
     fx0, fx1 = (x - R - pxl) / res, (x + R - pxl) / res
@@ -223,15 +232,17 @@ def former_decision(ci, cf, x, y, reach):
     return ((how,) + box, dsc) if fits else whole
 
 
-def test_box_decision_matches_former_host_decision(helpers):
+def test_box_decision_matches_host_restatement(helpers):
     rng = np.random.default_rng(7)
-    cases = 0
+    cases, far_boxed = 0, 0
     for mode in (0, 1, 2):
         for disc in (0, 1):
             for (rows, cols, res, pxl, pyl, ty, M, nt, bp) in [(512, 512, 0.1, -0.8, -0.8, 16, 64, 2, 12),
                                                                (100, 130, 0.25, -1.0, 0.5, 8, 24, 1, 32),
                                                                (13, 13, 1.0, -2.0, -2.0, 4, 1024, 2, 12),
-                                                               (300, 40, 0.2, 0.0, 0.0, 2, 8, 0, 12)]:
+                                                               (300, 40, 0.2, 0.0, 0.0, 2, 8, 0, 12),
+                                                               # georeferenced: the rounding terms are metres here
+                                                               (2000, 2000, 0.1, 4.0e5, -4.0e5, 64, 64, 1, 12)]:
                 T, vr, dt, trm = 64, (-1.0, 2.5), 0.1, 1.27
                 ci = [mode, disc, T, rows, cols, nt, 8, ty, M, bp, bp]
                 cf = [vr[0], vr[1], dt, trm, res, pxl, pyl]
@@ -248,13 +259,14 @@ def test_box_decision_matches_former_host_decision(helpers):
                             r = None if reach is None else C.c_float(reach)
                             helpers.emu_decide((C.c_int * 11)(*ci), (C.c_float * 7)(*cf), float(x), float(y),
                                                None if r is None else C.byref(r), out, outf)
-                            last, dsc = former_decision(ci, cf, float(x), float(y), reach)
+                            last, dsc = host_decision(ci, cf, float(x), float(y), reach)
                             got = (out[0],) + tuple(out[3:7]) if out[0] else (0, 0, rows, 0, cols)
                             assert got == last, (ci, cf, x, y, reach, got, last)
                             if out[0]:
                                 assert (np.float32(outf[0]), np.float32(outf[1]), np.float32(outf[2])) == dsc
+                                far_boxed += abs(pxl) > 1000
                             cases += 1
-    assert cases > 10000
+    assert cases > 10000 and far_boxed > 100, (cases, far_boxed)
 
 
 def test_window_origin_matches_fill_win_args(helpers):
