@@ -272,6 +272,17 @@ int b200mppi_planner_synchronize(b200mppi_planner* pl);
 int b200mppi_debug_sample_threshold(double alpha_dyn, int32_t q_cap, const uint64_t* draws, int64_t n,
                                     uint8_t* q_out);
 
+/* Test hook (needs a GPU): out[i] = op(a[i]) or op(a[i], b[i]) for n host floats, evaluated on the device by the
+ * approximate operations the kernels use -- sin.approx / cos.approx / sqrt.approx / div.approx / div.full (.ftz) of
+ * csrc/common.cuh and the libdevice logf / cosf of the Box-Muller noise -- so that a host oracle can reproduce every
+ * rollout cost and noise value exactly.  b is read only by the two divisions.  B200MPPI_EINVAL for an unknown op,
+ * n < 0 or a missing array. */
+enum {
+  B200MPPI_MATH_SIN_APPROX = 0, B200MPPI_MATH_COS_APPROX = 1, B200MPPI_MATH_SQRT_APPROX = 2,
+  B200MPPI_MATH_DIV_APPROX = 3, B200MPPI_MATH_DIV_FULL = 4, B200MPPI_MATH_LOGF = 5, B200MPPI_MATH_COSF = 6
+};
+int b200mppi_debug_device_math(int32_t op, const float* a, const float* b, float* out, int64_t n);
+
 /* Debug hook: per-CTA start / end times (ns) and chunk shares of the windowed rollout kernel's launches that follow
  * (enable != 0), read back into out[6 * ctas]: start, end, share lo / hi (SM id in bits 40+ of lo), lane-steps on the slow
  * path, of which outside the staged window (bits 40+: warp-steps run) (tools/rollout_cta_times.py). */

@@ -98,6 +98,7 @@ def _load():
         "b200mppi_planner_solve_reduce": (C.c_int, [P, P]),
         "b200mppi_planner_solve_finish": (C.c_int, [P, P, P]),
         "b200mppi_debug_sample_threshold": (C.c_int, [C.c_double, C.c_int32, P, C.c_int64, P]),
+        "b200mppi_debug_device_math": (C.c_int, [C.c_int32, P, P, P, C.c_int64]),
         "b200mppi_planner_p2p_export": (C.c_int, [P, P, C.c_size_t]),
         "b200mppi_planner_p2p_import": (C.c_int, [P, P, C.c_size_t]),
         "b200mppi_planner_p2p_connect_local": (C.c_int, [P, P, C.c_int32]),

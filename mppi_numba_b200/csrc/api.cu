@@ -1,6 +1,7 @@
 // api.cu -- the C-ABI of include/b200mppi.h: handles, device buffers, and the per-solve launch
 // sequence that replaces the bodies of MPPI_Numba.solve_* (mppi_numba/mppi.py:237-451) and
 // TDM_Numba.sample_grids (terrain.py:610-622).
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -604,6 +605,54 @@ extern "C" int b200mppi_debug_sample_threshold(double alpha_dyn, int32_t q_cap, 
     return fail(B200MPPI_ESTATE, "debug_sample_threshold: alpha_dyn / q_cap not representable by the bucket table "
                                  "(the sampler falls back to its generic kernel)");
   for (int64_t i = 0; i < n; ++i) q_out[i] = (uint8_t)sample_threshold_q(draws[i], T);
+  return B200MPPI_OK;
+}
+
+// The approximate float32 operations of the kernels, evaluated on the device by the very inline helpers the kernels
+// use (common.cuh; logf / cosf are the libdevice routines of xoro_normal), compiled with the library's flags: their
+// results are deterministic functions of the inputs, so the test oracle can take them from here and predict every
+// rollout cost bit for bit.
+__global__ void debug_device_math_kernel(int op, const float* __restrict__ a, const float* __restrict__ b,
+                                         float* __restrict__ out, int64_t n) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float x = a[i];
+    float r;
+    switch (op) {
+      case B200MPPI_MATH_SIN_APPROX: r = sin_approx(x); break;
+      case B200MPPI_MATH_COS_APPROX: r = cos_approx(x); break;
+      case B200MPPI_MATH_SQRT_APPROX: r = sqrt_approx(x); break;
+      case B200MPPI_MATH_DIV_APPROX: r = div_approx(x, b[i]); break;
+      case B200MPPI_MATH_DIV_FULL: r = div_full(x, b[i]); break;
+      case B200MPPI_MATH_LOGF: r = logf(x); break;
+      default: r = cosf(x); break;                         // B200MPPI_MATH_COSF (op checked on the host)
+    }
+    out[i] = r;
+  }
+}
+
+extern "C" int b200mppi_debug_device_math(int32_t op, const float* a, const float* b, float* out, int64_t n) {
+  if (op < B200MPPI_MATH_SIN_APPROX || op > B200MPPI_MATH_COSF) return fail(B200MPPI_EINVAL, "debug_device_math: unknown op");
+  const bool binary = op == B200MPPI_MATH_DIV_APPROX || op == B200MPPI_MATH_DIV_FULL;
+  if (n < 0 || (n > 0 && (!a || !out || (binary && !b)))) return fail(B200MPPI_EINVAL, "debug_device_math: bad argument");
+  if (n == 0) return B200MPPI_OK;
+  const size_t bytes = (size_t)n * sizeof(float);
+  float *da = nullptr, *db = nullptr, *dout = nullptr;
+  cudaError_t e = cudaMalloc(&da, bytes);
+  if (e == cudaSuccess && binary) e = cudaMalloc(&db, bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&dout, bytes);
+  if (e == cudaSuccess) e = cudaMemcpy(da, a, bytes, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && binary) e = cudaMemcpy(db, b, bytes, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) {
+    const int threads = 256;
+    const int64_t blocks = std::min<int64_t>((n + threads - 1) / threads, 65535);
+    debug_device_math_kernel<<<(unsigned)blocks, threads>>>(op, da, db, dout, n);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpy(out, dout, bytes, cudaMemcpyDeviceToHost);
+  cudaFree(da);
+  cudaFree(db);
+  cudaFree(dout);
+  if (e != cudaSuccess) return fail(B200MPPI_ECUDA, std::string("debug_device_math: ") + cudaGetErrorString(e));
   return B200MPPI_OK;
 }
 

@@ -8,13 +8,27 @@ SURVEY.md 2.3; re-derived from ``numba.cuda.compile_ptx`` of the reference kerne
   * rollout_det_dyn_w_speed_map   mppi.py:1013-1111 (nominal dynamics + worst-case speed map)
   * update_useq_numba             mppi.py:1113-1191
   * shift_optimal_control_sequence mppi.py:539-542
-Exact-math stand-ins: numpy float32 sin/cos/sqrt and IEEE division replace sin.approx/cos.approx/
-sqrt.approx/div.approx/div.full of the GPU build (~1e-7 relative per op).  Everything else --
-float64 intermediates, FMA contractions, add order -- mirrors the compiled code.
+Every floating-point operation of the rollouts and of the noise goes through an arithmetic object
+(oracle/arith.py, argument ``arith``):
+
+* default (``arith=None``, ``oracle.arith.NUMPY``) -- exact-math stand-ins: numpy float32 sin/cos/sqrt and IEEE
+  division replace sin.approx/cos.approx/sqrt.approx/div.approx/div.full of the GPU build (~1e-7 relative per op), and
+  a float32 FMA is a float64 multiply-add rounded twice, a float64 FMA a product and a sum.  What the reference's
+  golden vectors are checked against (<= 2e-6), and what bench.py's cpu_baseline leg times.
+* ``oracle.arith.Exact(provider, ftz)`` -- the exact oracle: each operation placed and rounded where the kernels
+  (csrc/rollout.cu, csrc/rollout_win.cu) place it -- the FMA contractions the compiled code has, each rounded once,
+  float32 add / sub / mul rounded once, optionally the .ftz flushes -- and the approximate operations from a provider:
+  ``LibmProvider`` (what the host emulation of the kernels uses) or ``DeviceProvider`` (the GPU's own results).  With
+  the provider of the machine that runs the kernel, costs, states and noise are predicted bit for bit.
+
+``ctrl_order`` chooses the control-cost summation of the stochastic mode: "sequential" (each term added to the running
+cost, as the reference and the generic kernel do) or "presummed" (the windowed kernel: the terms summed from 0 by
+an FMA chain, the total added after the stage costs).
 """
 import math
 import numpy as np
 
+from . import arith as AR
 from . import xoroshiro as X
 
 F32 = np.float32
@@ -37,25 +51,31 @@ def _fma32(a, b, c):
 
 
 # ----------------------------------------------------------------------------- noise
-def sample_noise(states, u_std, N, T):
+def sample_noise(states, u_std, N, T, arith=None):
     """mppi.py:1365-1370: generator n*T+t produces BOTH components (two Box-Muller calls = 4 draws)."""
+    A = arith or AR.NUMPY
     us = np.asarray(u_std, dtype=F32)
-    z0 = X.normal_float32(states)            # all N*T generators advance together
-    z1 = X.normal_float32(states)
+    z0 = X.normal_float32(states, arith=arith)            # all N*T generators advance together
+    z1 = X.normal_float32(states, arith=arith)
     noise = np.empty((N, T, 2), dtype=F32)
-    noise[..., 0] = (us[0] * z0).reshape(N, T)
-    noise[..., 1] = (us[1] * z1).reshape(N, T)
+    noise[..., 0] = A.mul32(us[0], z0).reshape(N, T)
+    noise[..., 1] = A.mul32(us[1], z1).reshape(N, T)
     return noise
 
 
 # ----------------------------------------------------------------------------- cell index
-def floor_div_f32(a, r):
+def floor_div_f32(a, r, arith=None):
     """Python ``//`` on float32 as Numba lowers it (numba/cpython/numbers.py real_divmod; PTX of
     rollout_det_dyn_numba): remainder via abs/div.rn/floor/mul/sub, quotient (a-mod)/r, sign fix,
     floor, snap-to-nearest.  ptxas contracts the remainder's mul+sub into ONE FMA (SASS of the
     reference kernel: FFMA.FTZ m = -floor(t)*|r| + |a|), i.e. the remainder is exact -- the same
     result CPython's fmod-based float_divmod gives in the simulator.
-    ``a`` float32 array, ``r`` float32 scalar != 0."""
+    ``a`` float32 array, ``r`` float32 scalar != 0.
+
+    With an exact ``arith`` the sequence is csrc/common.cuh::cell_index_exact operation by operation (div.rn,
+    cvt.rmi, the contracted FMA, div.full from the provider, the q == 0 / NaN branch, cvt.rzi)."""
+    if arith is not None and arith.exact:
+        return _floor_div_exact(a, r, arith)
     a = a.astype(F32)
     r = F32(r)
     aa = np.abs(a)
@@ -72,17 +92,41 @@ def floor_div_f32(a, r):
     return res.astype(np.int32)                      # cvt.rzi
 
 
+def _floor_div_exact(a, r, A):
+    a = np.asarray(a, dtype=F32)
+    r = F32(r)
+    aa, rr = np.abs(A.f2d(a).astype(F32)), np.abs(r)              # fabsf of the (flushed) operand
+    t = A.div_rn32(aa, rr)
+    m = A.fma32(-A.floor32(t), rr, aa)
+    m = np.where(a < 0, -m, m).astype(F32)
+    q = A.div_full32(A.sub32(a, m), r)
+    fix = (m != 0) & ((r < 0) != (m < 0))
+    q = np.where(fix, A.add32(q, F32(-1)), q).astype(F32)
+    fl = A.floor32(q)
+    res = np.where(A.sub32(q, fl) > F32(0.5), A.add32(fl, F32(1)), fl).astype(F32)
+    odd = (q == 0) | np.isnan(q)
+    if odd.any():
+        res = np.where(odd, A.div_full32(A.mul32(a, A.mul32(q, q)), r), res).astype(F32)
+    res = np.where(np.isnan(res), F32(0), res)        # cvt.rzi of NaN is 0
+    return np.trunc(res).astype(np.int32)
+
+
 # ----------------------------------------------------------------------------- rollouts
 def rollout_costs(mode, lin_grid, ang_grid, lin_bounds, ang_bounds, obstacle_map, unknown_map,
                   res, xlimits, ylimits, vrange, wrange, xgoal, v_post_rollout, obs_cost, unknown_cost,
                   goal_tolerance, lambda_weight, u_std, x0, dt, dist_weight, noise, u_cur,
-                  risk_map=None, return_states=False):
+                  risk_map=None, return_states=False, arith=None, ctrl_order="sequential", wrap_clamp=False):
     """Per-(n, m) rollout cost, float32 (N, Mg).  Mg = lin_grid.shape[0] maps are used in
     MODE_STOCHASTIC, map 0 only otherwise (tid == 0 in the one-thread blocks, mppi.py:334,978).
 
     Loop body mppi.py:677-706 / 969-1001 / 1069-1103; epilogue order: stochastic adds the control
     cost then the terminal cost (:708-713), the deterministic kernels add terminal then control
-    (:1004-1009, :1106-1111)."""
+    (:1004-1009, :1106-1111).  ``arith`` / ``ctrl_order``: see the module docstring.  ``wrap_clamp``: the engine's rule
+    for cells outside the map (negative indices wrapped like Numba's indexing, then clamped into the array; the
+    reference reads outside its allocation there -- DESIGN.md 2); otherwise such a lookup is an IndexError."""
+    A = arith or AR.NUMPY
+    if ctrl_order not in ("sequential", "presummed"):
+        raise ValueError("ctrl_order: 'sequential' or 'presummed'")
     noise = np.asarray(noise, dtype=F32)
     u_cur = np.asarray(u_cur, dtype=F32)
     N, T, _ = noise.shape
@@ -104,7 +148,8 @@ def rollout_costs(mode, lin_grid, ang_grid, lin_bounds, ang_bounds, obstacle_map
 
     lin_ratio = 0.01 * F64(F32(lb[1] - lb[0]))       # float64 (mppi.py:674)
     ang_ratio = 0.01 * F64(F32(ab[1] - ab[0]))
-    dt64 = F64(dt)
+    dt64 = A.f2d(dt)
+    lin_lo, ang_lo = A.f2d(lb[0]), A.f2d(ab[0])
 
     x = np.full((N, Mg), x0[0], dtype=F32)
     y = np.full((N, Mg), x0[1], dtype=F32)
@@ -121,35 +166,39 @@ def rollout_costs(mode, lin_grid, ang_grid, lin_bounds, ang_bounds, obstacle_map
     for t in range(T):
         if not active.any():
             break
-        xi = floor_div_f32((x - xl[0]).astype(F32), res)
-        yi = floor_div_f32((y - yl[0]).astype(F32), res)
-        ql = lin_grid[m_idx, yi, xi].astype(F64)
-        qa = ang_grid[m_idx, yi, xi].astype(F64)
-        vtr = lin_ratio * ql + F64(lb[0])
-        wtr = ang_ratio * qa + F64(ab[0])
-        v_nom = (u_cur[t, 0] + noise[:, t, 0]).astype(F32)
-        w_nom = (u_cur[t, 1] + noise[:, t, 1]).astype(F32)
+        xi = floor_div_f32(A.sub32(x, xl[0]), res, A)
+        yi = floor_div_f32(A.sub32(y, yl[0]), res, A)
+        gy, gx, my, mx = yi, xi, yi, xi
+        if wrap_clamp:
+            gy, gx = _wrap_clamp(yi, lin_grid.shape[1]), _wrap_clamp(xi, lin_grid.shape[2])
+            my, mx = _wrap_clamp(yi, obstacle_map.shape[0]), _wrap_clamp(xi, obstacle_map.shape[1])
+        ql = lin_grid[m_idx, gy, gx].astype(F64)
+        qa = ang_grid[m_idx, gy, gx].astype(F64)
+        vtr = A.fma64(lin_ratio, ql, lin_lo)          # fma(ratio, q, lo): the traction value, one rounding
+        wtr = A.fma64(ang_ratio, qa, ang_lo)
+        v_nom = A.add32(u_cur[t, 0], noise[:, t, 0])
+        w_nom = A.add32(u_cur[t, 1], noise[:, t, 1])
         v = np.maximum(vr[0], np.minimum(vr[1], v_nom)).astype(F32)[:, None]
         w = np.maximum(wr[0], np.minimum(wr[1], w_nom)).astype(F32)[:, None]
-        dv = (vtr * dt64) * v.astype(F64)
-        c32 = np.cos(th).astype(F32)
-        s32 = np.sin(th).astype(F32)
-        xn = (dv * c32.astype(F64) + x.astype(F64)).astype(F32)
-        yn = (dv * s32.astype(F64) + y.astype(F64)).astype(F32)
-        thn = ((wtr * dt64) * w.astype(F64) + th.astype(F64)).astype(F32)
-        dx = (xg[0] - xn).astype(F32)
-        dy = (xg[1] - yn).astype(F32)
-        d2n = _fma32(dx, dx, (dy * dy).astype(F32))
-        sq = np.sqrt(d2n).astype(F32)
+        dv = (vtr * dt64) * A.f2d(v)
+        c32 = A.cos32(th)
+        s32 = A.sin32(th)
+        xn = A.d2f(A.fma64(dv, A.f2d(c32), A.f2d(x)))  # float64 FMA rounded once to float32
+        yn = A.d2f(A.fma64(dv, A.f2d(s32), A.f2d(y)))
+        thn = A.d2f(A.fma64(wtr * dt64, A.f2d(w), A.f2d(th)))
+        dx = A.sub32(xg[0], xn)
+        dy = A.sub32(xg[1], yn)
+        d2n = A.fma32(dx, dx, A.mul32(dy, dy))
+        sq = A.sqrt32(d2n)
         if mode == MODE_SPEED_MAP:
-            eff = F64(lb[0]) + lin_ratio * risk_map[0, yi, xi].astype(F64)
-            dt_eff = (dt64 / (eff + 1e-6)).astype(F32)
-            stage = _fma32(sq, w_dist, dt_eff)
+            eff = A.fma64(lin_ratio, risk_map[0, my, mx].astype(F64), lin_lo)
+            dt_eff = A.d2f(dt64 / (eff + 1e-6))
+            stage = A.fma32(sq, w_dist, dt_eff)
         else:
-            stage = _fma32(sq, w_dist, np.full_like(sq, dt))
-        cn = (cost + stage).astype(F32)
-        cn = _fma32(obstacle_map[yi, xi].astype(F32), obs_c, cn)
-        cn = _fma32(unknown_map[yi, xi].astype(F32), unk_c, cn)
+            stage = A.fma32(sq, w_dist, np.full_like(sq, dt))
+        cn = A.add32(cost, stage)
+        cn = A.fma32(obstacle_map[my, mx].astype(F32), obs_c, cn)
+        cn = A.fma32(unknown_map[my, mx].astype(F32), unk_c, cn)
         x = np.where(active, xn, x)
         y = np.where(active, yn, y)
         th = np.where(active, thn, th)
@@ -164,18 +213,18 @@ def rollout_costs(mode, lin_grid, ang_grid, lin_bounds, ang_bounds, obstacle_map
             states[:, :, t + 1, 2] = th
 
     def add_terminal(c):
-        term = ((1.0 - reached.astype(F64)) * np.sqrt(d2).astype(F32).astype(F64)) / (F64(v_post) + 1e-6)
-        return (c + term.astype(F32)).astype(F32)
+        term = ((1.0 - reached.astype(F64)) * A.f2d(A.sqrt32(d2))) / (A.f2d(v_post) + 1e-6)
+        return A.add32(c, A.d2f(term))
 
     def add_control(c):
-        sv2 = F32(us[0] * us[0])
-        sw2 = F32(us[1] * us[1])
-        for t in range(T):
-            a = F32(u_cur[t, 0] / sv2)
-            b = F32(u_cur[t, 1] / sw2)
-            p = (b * noise[:, t, 1]).astype(F32)
-            s = _fma32(np.full(N, a, dtype=F32), noise[:, t, 0], p)
-            c = _fma32(np.broadcast_to(s[:, None], c.shape).astype(F32), lam, c)
+        terms = _control_terms(A, us, u_cur, noise)
+        if ctrl_order == "presummed":                 # rollout_win.cu: FMA chain from 0, total added once
+            acc = np.zeros(N, dtype=F32)
+            for s in terms:
+                acc = A.fma32(s, lam, acc)
+            return A.add32(c, acc[:, None])
+        for s in terms:
+            c = A.fma32(np.broadcast_to(s[:, None], c.shape).astype(F32), lam, c)
         return c
 
     if mode == MODE_STOCHASTIC:
@@ -187,8 +236,26 @@ def rollout_costs(mode, lin_grid, ang_grid, lin_bounds, ang_bounds, obstacle_map
     return cost
 
 
+def _wrap_clamp(i, n):
+    """csrc/rollout.cu wrap_clamp: i < 0 -> i + n, then clamped to [0, n - 1]."""
+    return np.clip(np.where(i < 0, i + n, i), 0, n - 1)
+
+
+def _control_terms(A, us, u_cur, noise):
+    """The per-step control-cost terms u_v/s_v^2 * e_v + u_w/s_w^2 * e_w (mppi.py:708-710; rollout.cu ctrl_term),
+    float32 (N,) each."""
+    N, T, _ = noise.shape
+    sv2 = A.mul32(us[0], us[0])
+    sw2 = A.mul32(us[1], us[1])
+    for t in range(T):
+        a = A.div_approx32(u_cur[t, 0], sv2)
+        b = A.div_approx32(u_cur[t, 1], sw2)
+        p = A.mul32(b, noise[:, t, 1])
+        yield A.fma32(np.full(N, a, dtype=F32), noise[:, t, 0], p)
+
+
 def state_rollouts(mode, V, lin_grid, ang_grid, lin_bounds, ang_bounds, res, xlimits, ylimits, x0, dt,
-                   u_cur, u_prev=None, noise=None, vrange=None, wrange=None):
+                   u_cur, u_prev=None, noise=None, vrange=None, wrange=None, arith=None, wrap_clamp=False):
     """get_state_rollout's kernels (mppi.py:1194-1351): float32 (V, T+1, 3), no goal test, no costs.
 
     MODE_STOCHASTIC -- get_state_rollout_across_envs_numba (:1303-1351): u_cur, unclipped and without
@@ -205,7 +272,7 @@ def state_rollouts(mode, V, lin_grid, ang_grid, lin_bounds, ang_bounds, res, xli
     def run(grid_mode, lg, ag, noise_, u_, vr, wr):
         _, st = rollout_costs(grid_mode, lg, ag, lin_bounds, ang_bounds, zeros, zeros, res, xlimits, ylimits,
                               vr, wr, far, 1.0, 0.0, 0.0, 0.0, 1.0, [1.0, 1.0], x0, dt, 1.0, noise_, u_,
-                              return_states=True)
+                              return_states=True, arith=arith, wrap_clamp=wrap_clamp)
         return st
     if mode == MODE_STOCHASTIC:
         st = run(MODE_STOCHASTIC, lin_grid[:V], ang_grid[:V], np.zeros((1, T, 2), dtype=F32), u_cur, wide, wide)
@@ -220,11 +287,13 @@ def state_rollouts(mode, V, lin_grid, ang_grid, lin_bounds, ang_bounds, res, xli
 
 
 def rollout_costs_barebone(obs_pos, obs_r, vrange, wrange, xgoal, obs_cost, goal_tolerance, lambda_weight, u_std,
-                           x0, dt, dist_weight, noise, u_cur, return_states=False):
+                           x0, dt, dist_weight, noise, u_cur, return_states=False, arith=None):
     """The map-free variant of the reference's barebone_mppi_numba.ipynb (cell 3, rollout_numba): nominal
     unicycle in float32 (dv = dt*v; x = fma(dv, cos, x); theta = fma(w, dt, theta)), stage cost w*d^2,
     circular obstacles (indicator of d^2 - r^2 <= 0, float64 FMA into the float32 cost), terminal cost
-    (1-reached)*d^2, then the control cost.  Contractions as in the SASS of the compiled kernel."""
+    (1-reached)*d^2, then the control cost.  Contractions as in the SASS of the compiled kernel.  ``arith``: see the
+    module docstring."""
+    A = arith or AR.NUMPY
     noise = np.asarray(noise, dtype=F32)
     u_cur = np.asarray(u_cur, dtype=F32)
     N, T, _ = noise.shape
@@ -248,21 +317,21 @@ def rollout_costs_barebone(obs_pos, obs_r, vrange, wrange, xgoal, obs_cost, goal
     for t in range(T):
         if not active.any():
             break
-        v = np.maximum(vr[0], np.minimum(vr[1], (u_cur[t, 0] + noise[:, t, 0]).astype(F32))).astype(F32)
-        w = np.maximum(wr[0], np.minimum(wr[1], (u_cur[t, 1] + noise[:, t, 1]).astype(F32))).astype(F32)
-        dv = (v * dt).astype(F32)
-        xn = _fma32(dv, np.cos(th).astype(F32), x)
-        yn = _fma32(dv, np.sin(th).astype(F32), y)
-        thn = _fma32(w, dt, th)
-        dx, dy = (xg[0] - xn).astype(F32), (xg[1] - yn).astype(F32)
-        d2n = _fma32(dx, dx, (dy * dy).astype(F32))
-        cn = _fma32(d2n, w_dist, cost)
+        v = np.maximum(vr[0], np.minimum(vr[1], A.add32(u_cur[t, 0], noise[:, t, 0]))).astype(F32)
+        w = np.maximum(wr[0], np.minimum(wr[1], A.add32(u_cur[t, 1], noise[:, t, 1]))).astype(F32)
+        dv = A.mul32(v, dt)
+        xn = A.fma32(dv, A.cos32(th), x)
+        yn = A.fma32(dv, A.sin32(th), y)
+        thn = A.fma32(w, dt, th)
+        dx, dy = A.sub32(xg[0], xn), A.sub32(xg[1], yn)
+        d2n = A.fma32(dx, dx, A.mul32(dy, dy))
+        cn = A.fma32(d2n, w_dist, cost)
         for k in range(len(orad)):
-            ddx, ddy = (xn - op[k, 0]).astype(F32), (yn - op[k, 1]).astype(F32)
-            q = _fma32(ddx, ddx, (ddy * ddy).astype(F32))
-            diff = (q.astype(F64) - F64(orad[k]) * F64(orad[k])).astype(F32)          # FFMA(-r, r, q)
+            ddx, ddy = A.sub32(xn, op[k, 0]), A.sub32(yn, op[k, 1])
+            q = A.fma32(ddx, ddx, A.mul32(ddy, ddy))
+            diff = A.fma32(-orad[k], orad[k], q)                                          # FFMA(-r, r, q)
             ind = (diff > 0).astype(F64)
-            cn = ((1.0 - ind) * F64(obs_c) + cn.astype(F64)).astype(F32)
+            cn = A.d2f(A.fma64(1.0 - ind, A.f2d(obs_c), A.f2d(cn)))
         x, y, th = np.where(active, xn, x), np.where(active, yn, y), np.where(active, thn, th)
         cost, d2 = np.where(active, cn, cost), np.where(active, d2n, d2)
         hit = active & (d2n <= tol2)
@@ -270,12 +339,9 @@ def rollout_costs_barebone(obs_pos, obs_r, vrange, wrange, xgoal, obs_cost, goal
         active &= ~hit
         if return_states:
             states[:, t + 1, 0], states[:, t + 1, 1], states[:, t + 1, 2] = x, y, th
-    cost = (cost + np.where(reached, F32(0), d2).astype(F32)).astype(F32)
-    sv2, sw2 = F32(us[0] * us[0]), F32(us[1] * us[1])
-    for t in range(T):
-        a, b = F32(u_cur[t, 0] / sv2), F32(u_cur[t, 1] / sw2)
-        sterm = _fma32(np.full(N, a, dtype=F32), noise[:, t, 0], (b * noise[:, t, 1]).astype(F32))
-        cost = _fma32(sterm, lam, cost)
+    cost = A.add32(cost, A.d2f(np.where(reached, 0.0, 1.0) * A.f2d(d2)))
+    for sterm in _control_terms(A, us, u_cur, noise):
+        cost = A.fma32(sterm, lam, cost)
     if return_states:
         return cost, states
     return cost

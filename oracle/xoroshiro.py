@@ -130,12 +130,18 @@ def uniform_float32(x: np.ndarray) -> np.ndarray:
 TWO_PI_F32 = np.float32(2 * np.pi)                 # random.py:172
 
 
-def normal_float32(states: np.ndarray, idx=None) -> np.ndarray:
+def normal_float32(states: np.ndarray, idx=None, arith=None) -> np.ndarray:
     """random.py:176-197: Box-Muller in float32, two draws per call, the sine branch is
     discarded.  (Compiled for CUDA this uses libdevice's precise logf/cosf and sqrt.approx;
-    numpy's float32 log/cos/sqrt are the exact-math stand-in -- SURVEY.md 2.3.)"""
+    by default numpy's float32 log/cos/sqrt are the exact-math stand-in -- SURVEY.md 2.3; an exact
+    ``arith`` (oracle/arith.py) takes them from its provider and rounds each product once, as
+    csrc/common.cuh::xoro_normal does.)"""
     u1 = uniform_float32(next_u64(states, idx))
     u2 = uniform_float32(next_u64(states, idx))
+    if arith is not None and arith.exact:
+        with np.errstate(divide="ignore", invalid="ignore"):
+            r = arith.sqrt32(arith.mul32(np.float32(-2.0), arith.logf32(u1)))
+            return arith.mul32(r, arith.cosf32(arith.mul32(TWO_PI_F32, u2)))
     with np.errstate(divide="ignore", invalid="ignore"):
         r = np.sqrt(np.float32(-2.0) * np.log(u1))
         return (r * np.cos(TWO_PI_F32 * u2)).astype(np.float32)

@@ -53,8 +53,9 @@ def make_scenario(mode, N, M, T, H, W, res, B, seed=1, near_goal=False, warm_sta
     return sc
 
 
-def oracle_rollout_costs(sc, lin, ang, noise, u_cur, grids=None):
-    """Oracle per-(n,m) costs for a scenario given the engine's TDM objects (for geometry / padded masks)."""
+def oracle_rollout_costs(sc, lin, ang, noise, u_cur, grids=None, **kw):
+    """Oracle per-(n,m) costs for a scenario given the engine's TDM objects (for geometry / padded masks); ``kw`` goes
+    to MR.rollout_costs (arith, ctrl_order, wrap_clamp)."""
     from oracle import mppi_ref as MR
     p = sc["params"]
     mode = dict(tdm=MR.MODE_STOCHASTIC, det=MR.MODE_DET_DYN, spd=MR.MODE_SPEED_MAP)[sc["mode"]]
@@ -66,4 +67,4 @@ def oracle_rollout_costs(sc, lin, ang, noise, u_cur, grids=None):
         lin.unknown_map_d.copy_to_host(), np.float32(lin.res), lin.padded_xlimits.astype(np.float32),
         lin.padded_ylimits.astype(np.float32), p["vrange"], p["wrange"], p["xgoal"], p["v_post_rollout"],
         p.get("obs_penalty", 1e5), p.get("unknown_penalty", 1e2), p["goal_tolerance"], p["lambda_weight"],
-        p["u_std"], p["x0"], p["dt"], p.get("dist_weight", 1.0), noise, u_cur, risk_map=risk)
+        p["u_std"], p["x0"], p["dt"], p.get("dist_weight", 1.0), noise, u_cur, risk_map=risk, **kw)

@@ -81,9 +81,11 @@ def snapshot(p):
 
 
 def assert_same(a, b, what):
+    """Bit for bit: an untouched buffer may hold NaN patterns (what its allocation held), which == never equates."""
     assert a.keys() == b.keys()
     for key in a:
-        assert np.array_equal(a[key], b[key]), "%s: %s differs" % (what, key)
+        x, y = np.asarray(a[key]), np.asarray(b[key])
+        assert x.dtype == y.dtype and x.shape == y.shape and x.tobytes() == y.tobytes(), "%s: %s differs" % (what, key)
 
 
 def batch_vs_sequential(E, make, K, rounds=3, check_every=True):

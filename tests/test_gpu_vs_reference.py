@@ -4,7 +4,8 @@ The reference cannot be committed to this repository; build() compiles it to git
 oracle/_ref/ where its sources are readable (oracle/ref_build.py).  When that was not built the tests skip.
 What is asserted (same inputs on both sides: seed, PMFs, masks, params):
   * control noise: bit-identical;  sampled traction maps: bit-identical
-  * deterministic-mode rollout costs: bit-identical
+  * deterministic-mode rollout costs: bit-identical, also with a nonzero lower traction bound on inputs where fusing
+    lo + ratio*q (and the state's dv*cos + x) into one FMA decides the goal flag -- what pins the exact oracle's FMAs
   * stochastic CVaR costs: within 1e-4 relative (only the summation order of the CVaR mean differs),
     including M > 1024 against the reference's oversized kernel at cvar_alpha = 1
   * updated control sequence given the reference's costs: within 1e-4
@@ -124,3 +125,38 @@ def test_kernels_vs_reference_numba_cuda(ref, mode, N, M, T, H, res, B, det_alph
     L.check(L.lib.b200mppi_planner_update(ep._handle, L.ptr(c)))
     eu = ep.u_cur_d.copy_to_host()
     np.testing.assert_allclose(eu, ref_u, rtol=1e-4, atol=1e-5)
+
+
+@pytest.mark.parametrize("kind", ["state", "traction"])
+def test_reference_fuses_traction_and_state_updates(ref, kind):
+    """rollout_det_dyn_numba itself on a directed case (tests/directed_cases.py, traction bounds [0.2, 1.3]): rounding
+    lo + ratio*q, or dt*vtr*v*cos + x, before the add would move the first step's x by one float32 ulp and flip the goal
+    flag.  The reference's costs equal the engine's and the exact oracle's (device provider) bit for bit, so the
+    reference fuses both as the oracle does."""
+    RConfig, RTDM, RMPPI, cuda = ref
+    import __graft_entry__
+    __graft_entry__.build_engine()
+    import mppi_numba_b200 as E
+    from oracle import arith as AR
+    from tests.directed_cases import directed_scenario, fma_boundary_case
+    from tests.test_gpu_exact_oracle import assert_all_equal, directed_oracle, run_directed
+    f32 = np.float32
+    dev = AR.Exact(AR.DeviceProvider(E._lib), ftz=True)
+    case = fma_boundary_case(dev, kind)
+    assert case["x1_exact"] != case["x1_other"]
+    s = directed_scenario(case, N=40, M=1)
+    N = s["N"]
+    lim = np.array([s["xlo"], s["xlo"] + s["Cc"] * s["res"]], f32)
+    costs_d = cuda.device_array(N, dtype=f32)
+    RMPPI.rollout_det_dyn_numba[N, 1](
+        cuda.to_device(s["lin"]), cuda.to_device(s["ang"]), cuda.to_device(np.array(s["lb"], f32)),
+        cuda.to_device(np.array(s["ab"], f32)), cuda.to_device(s["obs"]), cuda.to_device(s["unk"]), f32(s["res"]),
+        cuda.to_device(lim), cuda.to_device(lim), cuda.to_device(np.array([0, 3], f32)),
+        cuda.to_device(np.array([-np.pi, np.pi], f32)), cuda.to_device(np.array(s["goal"], f32)), f32(0.01), f32(1e5),
+        f32(1e2), f32(s["tol"]), f32(1.0), cuda.to_device(np.array([2, 3], f32)), cuda.to_device(np.array(s["x0"], f32)),
+        f32(0.1), 1.0, cuda.to_device(s["noise"]), cuda.to_device(s["u_cur"]), costs_d)
+    cuda.synchronize()
+    ref_costs = costs_d.copy_to_host()[:, None]
+    want = directed_oracle(s, 1, dev)
+    assert_all_equal(ref_costs, want, "reference, %s boundary" % kind)
+    assert_all_equal(run_directed(E, s, 1), want, "engine, %s boundary" % kind)

@@ -65,6 +65,15 @@ def test_rollout_kernels_match_reference(emu, gname):
     np.testing.assert_allclose(det, g["det_" + gname], rtol=3e-6)
     _, spd = launch(2, 1)
     np.testing.assert_allclose(spd, g["spd_" + gname], rtol=3e-6)
+    # and every cost equals the exact oracle (libm provider: what the emulation substitutes for the MUFU operations)
+    from oracle import mppi_ref as MR
+    from tests.test_exact_oracle_cpu import EXACT, assert_equal
+    for mode, got in ((MR.MODE_STOCHASTIC, cnm), (MR.MODE_DET_DYN, det[:, None]), (MR.MODE_SPEED_MAP, spd[:, None])):
+        want = MR.rollout_costs(mode, lin, ang, g["lin_bounds"], g["ang_bounds"], obs, unk, F32(g["res"]), g["xlim"],
+                                g["ylim"], g["vrange"], g["wrange"], goal, g["v_post"], g["obs_cost"], g["unk_cost"],
+                                g["goal_tol"], g["lam"], g["u_std"], g["x0"], g["dt"], g["dist_weight"], noise, u_cur,
+                                risk_map=risk[None], arith=EXACT)
+        assert_equal(got, want, "mode %d" % mode)
     if gname == "near":
         assert (cnm < 50).any() and (cnm > 50).any()        # the early-exit branch is exercised
 
@@ -82,6 +91,12 @@ def test_barebone_kernel_matches_reference_notebook(emu, gname):
     emu.emu_rollout(3, _p(f), _p(geo), _p(_c([0.01, 0.01], np.float64)), None, None, None, None, None, _p(noise), _p(u_cur),
                     None, _p(costs), _p(ob), ob.shape[0])
     np.testing.assert_allclose(costs, g["costs_" + gname], rtol=3e-6)
+    from oracle import mppi_ref as MR
+    from tests.test_exact_oracle_cpu import EXACT
+    want = MR.rollout_costs_barebone(g["obs_pos"], g["obs_r"], g["vrange"], g["wrange"], g["goal_" + gname], g["obs_cost"],
+                                     g["goal_tol"], g["lam"], g["u_std"], g["x0"], g["dt"], g["dist_weight"], noise, u_cur,
+                                     arith=EXACT)
+    assert (costs.view(np.uint32) == want.view(np.uint32)).all(), int((costs != want).sum())
 
 
 @pytest.mark.parametrize("mode", ["tdm", "det", "spd"])
@@ -100,3 +115,9 @@ def test_state_rollout_kernel_matches_reference(emu, mode):
     emu.emu_state_rollout(0 if mode == "tdm" else 1, V, _p(f), _p(geo), _p(_ratios(b, b)), _p(lin), _p(ang), _p(noise),
                           _p(u_cur), _p(u_prev), _p(out))
     np.testing.assert_allclose(out, g[mode + "_states"], rtol=3e-6, atol=3e-6)
+    from oracle import mppi_ref as MR
+    from tests.test_exact_oracle_cpu import EXACT
+    want = MR.state_rollouts(dict(tdm=MR.MODE_STOCHASTIC, det=MR.MODE_DET_DYN, spd=MR.MODE_SPEED_MAP)[mode], V, lin, ang, b, b,
+                             g["res"], [F32(g[mode + "_pxl"][0]), 0], [F32(g[mode + "_pyl"][0]), 0], g["x0"], g["dt"], u_cur,
+                             u_prev, noise, g["vrange"], g["wrange"], arith=EXACT)
+    assert (out.view(np.uint32) == want.view(np.uint32)).all(), int((out != want).sum())

@@ -11,6 +11,7 @@ import pytest
 from tests.emu_rollout import build as build_generic
 from tests.emu_rollout_win import build
 from tests.test_rollout_emulated_cpu import _c, _fparams, _p, _ratios
+from tests.test_exact_oracle_cpu import EXACT, assert_equal
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 F32 = np.float32
@@ -57,8 +58,14 @@ def test_windowed_kernel_matches_reference_and_generic_kernel(emu, gname):
     cnm, costs = np.zeros((N, M), F32), np.zeros(N, F32)
     gen.emu_rollout(0, _p(f), _p(geo), _p(ratios), _p(lin), _p(ang), _p(obs), _p(unk), None, _p(noise), _p(u_cur), _p(cnm),
                     _p(costs), None, 0)
-    # the generic kernel adds the control-cost terms one by one, the windowed one adds their pre-summed total: ~1 ulp
-    assert (np.abs(inside - cnm) / np.maximum(np.abs(cnm), 1e-6)).max() < 2e-6
+    # the generic kernel adds the control-cost terms one by one, the windowed one adds their pre-summed total: each
+    # equals the exact oracle (libm provider) in its own order
+    from oracle import mppi_ref as MR
+    args = (MR.MODE_STOCHASTIC, lin, ang, g["lin_bounds"], g["ang_bounds"], obs, unk, F32(g["res"]), g["xlim"], g["ylim"],
+            g["vrange"], g["wrange"], g["xgoal_" + gname], g["v_post"], g["obs_cost"], g["unk_cost"], g["goal_tol"], g["lam"],
+            g["u_std"], g["x0"], g["dt"], g["dist_weight"], noise, u_cur)
+    assert_equal(inside, MR.rollout_costs(*args, arith=EXACT, ctrl_order="presummed"), "windowed kernel")
+    assert_equal(cnm, MR.rollout_costs(*args, arith=EXACT), "generic kernel")
 
 
 def test_two_sided_floor_criterion_never_disagrees_with_the_reference_floor_division():
@@ -144,7 +151,7 @@ def test_windowed_kernel_multi_tile_random_scenario_matches_generic_kernel_and_o
     `ctas` CTAs (0: the launcher's own rule): shares of 132 chunks that start and end inside a map, CTAs that
     stage two windows one after the other, warps pulling chunks from the shared counter; 200 x 200 cells of random
     traction, obstacles and unknown cells, T = 40: windowed kernel == generic kernel (~1 ulp: pre-summed control
-    cost) whatever the grid, and both follow the oracle.  blocks > 1: the sharded destination layout -- every cost
+    cost) whatever the grid, and both equal the exact oracle (libm provider), each in its control-cost order.  blocks > 1: the sharded destination layout -- every cost
     stored into the "receive buffer" of the rank that reduces its control sequence, flags raised once by the last
     CTA (checked inside the harness).  N = 2100 = 3 x 700 = 7 x 300.  unit > 0: share boundaries at multiples of
     `unit` chunks (0 = the launcher's rule; -1 = shares that never cross a map: map m gets ctas/M or one more of the
@@ -181,12 +188,10 @@ def test_windowed_kernel_multi_tile_random_scenario_matches_generic_kernel_and_o
     cnm, costs = np.zeros((N, M), F32), np.zeros(N, F32)
     gen.emu_rollout(0, _p(f), _p(geo), _p(ratios), _p(lin), _p(ang), _p(obs), _p(unk), None, _p(noise), _p(u_cur), _p(cnm),
                     _p(costs), None, 0)
-    rel = np.abs(out - cnm) / np.maximum(np.abs(cnm), 1e-6)
-    assert rel.max() < 2e-6, rel.max()
-    want = MR.rollout_costs(MR.MODE_STOCHASTIC, lin, ang, [0, 1], [0, 1], obs, unk, res, [0.0, Cc * 0.1], [0.0, R * 0.1],
-                            [0, 3], [-np.pi, np.pi], goal, 0.01, 1e5, 1e2, 0.5, 1.0, [2, 3], x0, 0.1, 1.0, noise, u_cur)
-    r2 = np.abs(out - want) / np.maximum(np.abs(want), 1e-6)
-    assert (r2 < 1e-4).mean() > 0.995 and np.median(r2) < 2e-6          # libm vs numpy sin/cos: a few cell flips at most
+    args = (MR.MODE_STOCHASTIC, lin, ang, [0, 1], [0, 1], obs, unk, res, [0.0, Cc * 0.1], [0.0, R * 0.1],
+            [0, 3], [-np.pi, np.pi], goal, 0.01, 1e5, 1e2, 0.5, 1.0, [2, 3], x0, 0.1, 1.0, noise, u_cur)
+    assert_equal(out, MR.rollout_costs(*args, arith=EXACT, ctrl_order="presummed"), "windowed kernel")
+    assert_equal(cnm, MR.rollout_costs(*args, arith=EXACT), "generic kernel")
     assert (out < 0.5 * np.median(out)).any()                          # early exits happened
     if ctas == 3:
         # window pushed 110 cells right / 100 up: the robot sits near its edge, many lookups take the global-memory
@@ -319,8 +324,11 @@ def test_share_arithmetic_covers_every_chunk_once(emu, ctas, M, N, unit):
     gen.emu_rollout(0, _p(f), _p(geo), _p(ratios), _p(lin), _p(ang), _p(obs), _p(unk), None, _p(noise), _p(u_cur), _p(cnm),
                     _p(costs), None, 0)
     assert (out > 0).all()
-    rel = np.abs(out - cnm) / np.maximum(np.abs(cnm), 1e-6)
-    assert rel.max() < 2e-6, rel.max()
+    from oracle import mppi_ref as MR
+    args = (MR.MODE_STOCHASTIC, lin, ang, [0, 1], [0, 1], obs, unk, res, [0.0, Cc * 0.1], [0.0, R * 0.1],
+            [0, 3], [-np.pi, np.pi], goal, 0.01, 1e5, 1e2, 0.5, 1.0, [2, 3], x0, 0.1, 1.0, noise, u_cur)
+    assert_equal(out, MR.rollout_costs(*args, arith=EXACT, ctrl_order="presummed"), "windowed kernel")
+    assert_equal(cnm, MR.rollout_costs(*args, arith=EXACT), "generic kernel")
 
 
 @pytest.mark.parametrize("res", [0.1, 0.05, 0.3, 1.0, 0.0625, 0.7])
