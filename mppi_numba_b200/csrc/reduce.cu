@@ -187,38 +187,45 @@ __device__ __forceinline__ void update_partial_body(const UpdateArgs& a, const U
   float S = 0.0f;
   // accumulators for up to 4 column-chunks (T <= 4*UPD_THREADS = 1024, the reference's own cap)
   float2 acc[4] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};
-  for (int rb = r0; rb < r1; rb += 64) {
-    const int nr = min(64, r1 - rb);
-    __syncthreads();
-    if (tid < nr) {
-      const float w = softmax_weight(a.costs[rb + tid], beta, a.lambda);
-      s_w[tid] = w;
-      a.w_raw[rb + tid] = w;
-    }
-    __syncthreads();
-    // rows in batches of eight: the loads of a batch are issued before its FMAs (issue is in order -- an FMA waiting
-    // for its row would hold back the next row's load); accumulation order is the row order, as before
-    for (int i0 = 0; i0 < nr; i0 += 8) {
+  // a slab whose every cost is +inf: c - beta would be inf - inf = NaN.  Its rollouts get the reference's weight
+  // exp(-inf) = 0 (its beta is the global minimum) and the slab's partial is S = 0, V = 0 with beta = +inf, which
+  // merge_partials gives scale 0.  The branch is uniform over the CTA.
+  if (beta == INFINITY) {
+    for (int r = r0 + tid; r < r1; r += blockDim.x) a.w_raw[r] = 0.0f;
+  } else {
+    for (int rb = r0; rb < r1; rb += 64) {
+      const int nr = min(64, r1 - rb);
+      __syncthreads();
+      if (tid < nr) {
+        const float w = softmax_weight(a.costs[rb + tid], beta, a.lambda);
+        s_w[tid] = w;
+        a.w_raw[rb + tid] = w;
+      }
+      __syncthreads();
+      // rows in batches of eight: the loads of a batch are issued before its FMAs (issue is in order -- an FMA waiting
+      // for its row would hold back the next row's load); accumulation order is the row order, as before
+      for (int i0 = 0; i0 < nr; i0 += 8) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int j = tid + k * UPD_THREADS;
-        if (j < a.T) {
-          float2 e[8];
+        for (int k = 0; k < 4; ++k) {
+          const int j = tid + k * UPD_THREADS;
+          if (j < a.T) {
+            float2 e[8];
 #pragma unroll
-          for (int q = 0; q < 8; ++q)
-            e[q] = (i0 + q < nr) ? __ldg(eps + (size_t)(rb + i0 + q) * a.T + j) : make_float2(0.f, 0.f);
+            for (int q = 0; q < 8; ++q)
+              e[q] = (i0 + q < nr) ? __ldg(eps + (size_t)(rb + i0 + q) * a.T + j) : make_float2(0.f, 0.f);
 #pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            if (i0 + q < nr) {
-              const float w = s_w[i0 + q];
-              acc[k].x = fmaf(w, e[q].x, acc[k].x);
-              acc[k].y = fmaf(w, e[q].y, acc[k].y);
+            for (int q = 0; q < 8; ++q) {
+              if (i0 + q < nr) {
+                const float w = s_w[i0 + q];
+                acc[k].x = fmaf(w, e[q].x, acc[k].x);
+                acc[k].y = fmaf(w, e[q].y, acc[k].y);
+              }
             }
           }
         }
+        if (tid == 0)
+          for (int q = 0; q < 8 && i0 + q < nr; ++q) S += s_w[i0 + q];
       }
-      if (tid == 0)
-        for (int q = 0; q < 8 && i0 + q < nr; ++q) S += s_w[i0 + q];
     }
   }
   if (tid == 0) { part[0] = (r1 > r0) ? beta : INFINITY; part[1] = S; }

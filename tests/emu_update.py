@@ -1,7 +1,8 @@
 """Host emulation of the control-update kernels (TEST INFRASTRUCTURE; technique of tests/emu_sampler.py): the text of
 update_partial_kernel / merge_partials / update_rank_kernel / update_apply_kernel (csrc/reduce.cu between the
 ``[emu:... update]`` markers) compiled with g++, one std::thread per CUDA thread.  Float arithmetic follows the
-kernel's own order; ``exp`` is libm's instead of CUDA's (both within an ulp), so comparisons use a tolerance."""
+kernel's own order; ``exp`` is libm's instead of CUDA's (both within an ulp), so results are compared within the
+bounds of tests/reduce_bounds.py."""
 import ctypes as C
 import os
 import re

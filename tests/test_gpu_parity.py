@@ -19,6 +19,7 @@ pytestmark = pytest.mark.gpu
 from oracle import mppi_ref as MR          # noqa: E402
 from oracle import terrain_ref as TR       # noqa: E402
 from oracle import xoroshiro as X          # noqa: E402
+from tests import reduce_bounds as RB      # noqa: E402
 from tests.scenarios import make_scenario, oracle_rollout_costs   # noqa: E402
 from tests.test_gpu_exact_oracle import assert_all_equal           # noqa: E402
 
@@ -376,8 +377,8 @@ def test_rollout_costs_vs_oracle(eng, dev, mode, N, M, T, H, res, B, near, warm)
     assert_all_equal(got, want, "%s N%d M%d T%d" % (mode, N, M, T))
     if mode == "tdm":
         cv = pl.costs_d.copy_to_host()
-        # CVaR of the engine's own per-(n,m) costs: pure selection/mean (summation order differs by design) -> tight
-        np.testing.assert_allclose(cv, MR.cvar_reduce(got, sc["params"]["cvar_alpha"]), rtol=2e-6)
+        # CVaR of the engine's own per-(n,m) costs: the exact mean of the numel largest, within the kernel's bound
+        RB.check_cvar(cv, got, sc["params"]["cvar_alpha"], label="%s N%d M%d" % (mode, N, M))
     if near:
         assert (got < 0.5 * np.median(got)).any(), "near-goal case should contain early exits"
 
@@ -417,13 +418,30 @@ def test_window_kernel_equals_generic_kernel(eng, monkeypatch, maskmax):
     assert r.max() < 2e-6, r.max()
 
 
+CVAR_SHAPES = [1, 31, 32, 33, 63, 64, 65, 255, 256, 257, 511, 512, 513, 1023, 1024, 1025, 4097, 16384]
+
+
+def _cvar_alpha(M, numel):
+    if numel >= M:
+        return 1.0
+    a = (numel - 0.5) / M
+    assert RB.cvar_numel(M, a) == numel
+    return a
+
+
 def test_cvar_selection_properties(eng):
-    """CVaR kernel alone on adversarial inputs: ties, negatives, M not a multiple of 32, alpha edge
-    cases; against the oracle's sort-based restatement (mppi.py:718-755)."""
+    """CVaR kernel alone on adversarial inputs: ties (also at the threshold), signed zeros, +inf, negatives, magnitudes
+    1e-30 .. 1e30, M around every PER step and the CTA kernel, numel in {1, 2, M-1, M} and the alpha edge cases; the
+    exact mean of the numel largest values within the kernel's bound (tests/reduce_bounds.py)."""
     L = eng._lib
     rng = np.random.default_rng(0)
-    for M, alpha in ((6, 0.5), (33, 0.1), (100, 0.999), (256, 0.5), (1000, 0.25), (1024, 1.0), (7, 0.01), (1, 0.5),
-                     (1025, 0.5), (3000, 0.1), (2048, 1.0), (15000, 0.999), (4097, 0.0001)):   # CTA kernel (M > 1024)
+    cases = [(6, 0.5), (33, 0.1), (100, 0.999), (256, 0.5), (1000, 0.25), (1024, 1.0), (7, 0.01), (1, 0.5),
+             (1025, 0.5), (3000, 0.1), (2048, 1.0), (15000, 0.999), (4097, 0.0001),     # CTA kernel (M > 1024)
+             (1000, 0.1)]                 # float32(0.1) * 1000: ceil 101 in float64, 100 in float32
+    cases = list(dict.fromkeys(cases + sorted({(M, _cvar_alpha(M, k)) for M in CVAR_SHAPES for k in (1, 2, M - 1, M)
+                                               if 1 <= k <= M})))
+    worst = 0.0
+    for M, alpha in cases:
         N = 130
         rp = RawPlanner(eng, 0, N, M, 4, 8, 8)
         try:
@@ -431,14 +449,16 @@ def test_cvar_selection_properties(eng):
             c[:, ::3] = np.round(c[:, ::3])            # many exact ties
             c[5] = 7.0                                  # all equal
             c[6] = -np.abs(c[6])                        # all negative
+            extra = RB.cvar_rows(M, RB.cvar_numel(M, alpha), M)
+            c[10:10 + len(extra)] = extra
             rp.copy_in(L.BUF_COSTS_NM, c)
             rp.set_params(cvar_alpha=alpha)
             rp.call("cvar")
             got = rp.copy_out(L.BUF_COSTS, (N,))
-            want = MR.cvar_reduce(c, alpha)
-            np.testing.assert_allclose(got, want, rtol=2e-5, atol=2e-4, err_msg="M=%d alpha=%g" % (M, alpha))
+            worst = max(worst, RB.check_cvar(got, c, alpha, label="M=%d alpha=%r" % (M, alpha)))
         finally:
             rp.close()
+    print("\n[cvar] largest |error| / bound %.3g" % worst)
 
 
 # ----------------------------------------------------------------------------- 4. update
@@ -457,39 +477,86 @@ def test_update_vs_reference_golden(eng, golden_dir, lam):
         w = rp.copy_out(eng._lib.BUF_WEIGHTS, (N,))
         np.testing.assert_allclose(w, g["w_lam%02d" % int(lam * 10)], rtol=1e-4, atol=1e-9)
         np.testing.assert_allclose(u, g["u_lam%02d" % int(lam * 10)], rtol=1e-4, atol=1e-5)
+        RB.check_update(u, w, g["costs"], g["noise"], g["u0"], lam, g["vrange"], g["wrange"], label="golden")
         assert (rp.copy_out(eng._lib.BUF_COSTS, (N,)) == g["costs"]).all()     # costs_d is not clobbered
     finally:
         rp.close()
 
 
-@pytest.mark.parametrize("N,T", [(8192, 128), (1000, 50), (100, 1024), (37, 3)])
-def test_update_vs_oracle_large(eng, N, T):
-    rng = np.random.default_rng(N)
-    costs = rng.uniform(4000, 4020, N).astype(np.float32)
-    noise = (rng.standard_normal((N, T, 2)) * [2, 3]).astype(np.float32)
-    u0 = np.stack([rng.uniform(0, 2, T), rng.uniform(-1, 1, T)], 1).astype(np.float32)
+VR32, WR32 = np.array([0, 3], np.float32), np.array([-np.pi, np.pi], np.float32)
+UPD_SHAPES = [(8192, 128), (1000, 50), (100, 1024), (37, 3),
+              (1, 1024), (2, 513), (31, 512), (32, 511), (33, 257), (9472, 256), (9473, 255), (16384, 1), (15000, 64),
+              (16384, 1024)]
+UPD_VALUES = [(k, lam) for k in ("mild", "underflow", "far", "signed", "inf", "clip", "cancel")
+              for lam in (1e-3, 0.3, 1.0, 1e3)]
+
+
+def _gpu_update(eng, costs, noise, u0, lam):
+    N, T = noise.shape[:2]
     rp = RawPlanner(eng, 1, N, 1, T, 8, 8)
     try:
-        rp.set_params(lambda_weight=1.0)
+        rp.set_params(lambda_weight=lam)
         rp.copy_in(eng._lib.BUF_NOISE, noise)
         rp.copy_in(eng._lib.BUF_U_CUR, u0)
-        rp.call("update", eng._lib.ptr(costs))
-        u = rp.copy_out(eng._lib.BUF_U_CUR, (T, 2))
-        w = rp.copy_out(eng._lib.BUF_WEIGHTS, (N,))
-        uw, ww = MR.update_useq(1.0, costs, noise, [0, 3], [-np.pi, np.pi], u0)
-        np.testing.assert_allclose(w, ww, rtol=1e-4, atol=1e-12)
-        np.testing.assert_allclose(u, uw, rtol=1e-4, atol=1e-5)
-        assert abs(float(w.sum(dtype=np.float64)) - 1.0) < 1e-5
+        c = np.ascontiguousarray(costs)
+        rp.call("update", eng._lib.ptr(c))
+        return rp.copy_out(eng._lib.BUF_U_CUR, (T, 2)), rp.copy_out(eng._lib.BUF_WEIGHTS, (N,))
     finally:
         rp.close()
 
 
+@pytest.mark.parametrize("N,T,kind,lam", [pytest.param(N, T, "base", 1.0, id="%d-%d" % (N, T)) for N, T in UPD_SHAPES] +
+                         [(N, T, k, lam) for N, T in ((1000, 50), (9473, 33)) for k, lam in UPD_VALUES])
+def test_update_vs_oracle_large(eng, N, T, kind, lam):
+    """The one-launch update against the float64 reference within the bound of tests/reduce_bounds.py, across the
+    row batches, the four column chunks and the value cases (underflowing CTAs, costs near 1e6, signed costs,
+    scattered +inf, u0 on the clip bounds, cancelling noise, lambda 1e-3 .. 1e3)."""
+    if kind == "base":
+        rng = np.random.default_rng(N)
+        costs = rng.uniform(4000, 4020, N).astype(np.float32)
+        noise = (rng.standard_normal((N, T, 2)) * [2, 3]).astype(np.float32)
+        u0 = np.stack([rng.uniform(0, 2, T), rng.uniform(-1, 1, T)], 1).astype(np.float32)
+    else:
+        costs, noise, u0 = RB.update_inputs(kind, N, T, seed=N + T, lam=lam)
+    u, w = _gpu_update(eng, costs, noise, u0, lam)
+    ru, rw = RB.check_update(u, w, costs, noise, u0, lam, VR32, WR32, label="N%d T%d %s lam %g" % (N, T, kind, lam))
+    print("\n[update N%d T%d %s lam %g] |error| / bound: u %.3g, weights %.3g" % (N, T, kind, lam, ru, rw))
+    assert abs(float(w.sum(dtype=np.float64)) - 1.0) < 1e-5
+
+
+@pytest.mark.parametrize("N", [1000, 9473])
+def test_update_with_an_all_inf_cta_slab(eng, N):
+    """One CTA slab of +inf costs (its baseline is +inf, c - beta = inf - inf): the slab's rollouts get weight exactly
+    0, no weight is NaN and u equals the float64 reference (whose beta is the global minimum) within the bound --
+    before, the slab's NaN partial made u the clip bounds' upper ends."""
+    T = 4 if N == 1000 else 64
+    costs = RB.inf_slab_costs(N)
+    rng = np.random.default_rng(N)
+    noise = (rng.standard_normal((N, T, 2)) * [2, 3]).astype(np.float32)
+    u0 = np.stack([rng.uniform(0, 2.9, T), rng.uniform(-3, 3, T)], 1).astype(np.float32)
+    u, w = _gpu_update(eng, costs, noise, u0, 1.0)
+    RB.check_update(u, w, costs, noise, u0, 1.0, VR32, WR32, label="all-inf slab, N %d" % N)
+
+
 def test_update_sharded_equals_single(eng):
-    """N sharded over 4 'ranks' (4 planners on one GPU), partials gathered by hand -> same u as 1 rank."""
+    """N sharded over 4 'ranks' (4 planners on one GPU), partials gathered by hand -> same u as 1 rank, each within the
+    bound of the float64 reference (host combine and device combine)."""
+    _sharded_update(eng, "mild")
+
+
+def test_update_sharded_with_an_all_inf_rank(eng):
+    """One rank's rollouts all cost +inf: that rank's partial (beta +inf, S 0, V 0) must not poison the others' u, in
+    the host combine and in every rank's device combine; its rollouts get weight exactly 0."""
+    _sharded_update(eng, "inf_rank")
+
+
+def _sharded_update(eng, kind):
     L = eng._lib
     N, T, ws = 2048, 64, 4
     rng = np.random.default_rng(3)
     costs = rng.uniform(900, 930, N).astype(np.float32)
+    if kind == "inf_rank":
+        costs[N // ws: 2 * N // ws] = np.inf
     noise = (rng.standard_normal((N, T, 2)) * [2, 3]).astype(np.float32)
     u0 = rng.uniform(0, 1, (T, 2)).astype(np.float32)
     single = RawPlanner(eng, 1, N, 1, T, 8, 8)
@@ -501,6 +568,7 @@ def test_update_sharded_equals_single(eng):
         single.call("update", L.ptr(costs))
         u1 = single.copy_out(L.BUF_U_CUR, (T, 2))
         w1 = single.copy_out(L.BUF_WEIGHTS, (N,))
+        RB.check_update(u1, w1, costs, noise, u0, 1.0, VR32, WR32, label="one rank " + kind)
         parts = []
         for r, rp in enumerate(ranks):
             sl = slice(N * r // ws, N * (r + 1) // ws)
@@ -513,20 +581,21 @@ def test_update_sharded_equals_single(eng):
         gathered = np.ascontiguousarray(np.stack(parts))
         # host combine (the library's reference implementation of the exchange math)
         out = np.empty((T, 2), np.float32)
-        vr, wr = np.array([0, 3], np.float32), np.array([-np.pi, np.pi], np.float32)
-        L.check(L.lib.b200mppi_combine_partials_host(L.ptr(gathered), ws, T, np.float32(1.0), L.ptr(u0), L.ptr(vr),
-                                                     L.ptr(wr), L.ptr(out)))
-        np.testing.assert_allclose(out, u1, rtol=1e-5, atol=2e-6)
+        L.check(L.lib.b200mppi_combine_partials_host(L.ptr(gathered), ws, T, np.float32(1.0), L.ptr(u0), L.ptr(VR32),
+                                                     L.ptr(WR32), L.ptr(out)))
+        RB.check_update(out, None, costs, noise, u0, 1.0, VR32, WR32, N=N // ws, merges=ws, label="host combine " + kind)
         # device combine on every rank from a device copy of the gathered partials
         import torch
         gd = torch.from_numpy(gathered).cuda()
-        ws_w = []
+        ws_w, us = [], []
         for r, rp in enumerate(ranks):
             rp.call("solve_finish", C.c_void_p(gd.data_ptr()), None)
             rp.call("synchronize")
-            np.testing.assert_allclose(rp.copy_out(L.BUF_U_CUR, (T, 2)), u1, rtol=1e-5, atol=2e-6)
+            us.append(rp.copy_out(L.BUF_U_CUR, (T, 2)))
             ws_w.append(rp.copy_out(L.BUF_WEIGHTS, (rp.n_local,)))
-        np.testing.assert_allclose(np.concatenate(ws_w), w1, rtol=1e-4, atol=1e-12)
+        assert all((x == us[0]).all() for x in us)
+        RB.check_update(us[0], np.concatenate(ws_w), costs, noise, u0, 1.0, VR32, WR32, N=N // ws, merges=ws,
+                        label="device combine " + kind)
     finally:
         single.close()
         for rp in ranks:
@@ -935,7 +1004,7 @@ def test_oversized_map_count_solve(eng, capsys):
         L.check(getattr(L.lib, "b200mppi_planner_" + stage)(b._handle))
     nm = b.costs_nm_d.copy_to_host()
     cv = b.costs_d.copy_to_host()
-    np.testing.assert_allclose(cv, MR.cvar_reduce(nm, 0.3), rtol=2e-6)
+    RB.check_cvar(cv, nm, 0.3, label="oversized")
     c = np.ascontiguousarray(cv)
     L.check(L.lib.b200mppi_planner_update(b._handle, L.ptr(c)))
     assert (b.u_cur_d.copy_to_host() == u).all()
