@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench_batch.py -- K planners: K sequential solve() calls against one batched MPPI_Batch / MPPI_StochasticBatch solve().
 
-    python bench_batch.py --workload c2|c3|c4 --batch K [--steps S] [--warmup W] [--profile]
+    python bench_batch.py --workload c2|c3|c4|c3m --batch K [--steps S] [--warmup W] [--profile]
 
 K planners of the workload (bench.py's WORKLOADS, seeds 1..K: different maps, start poses and goals; num_opt = 1).
 First one MPPI_Batch.solve() is checked against K solve() calls on identical twins, bit for bit (u, u_prev, costs,
@@ -11,8 +11,9 @@ events on the one stream all planners and the batch use, and the wall clock (eac
 synchronisation); solves/s, state-steps/s and kernel launches per round.  Prints one JSON line; writes nothing to the
 tree (the library is built by build() beforehand).
 c3 (stochastic, use_tdm) runs MPPI_StochasticBatch; its parity check also compares the per-(m, n) costs and the reach
-box of every planner.  --profile adds a torch.profiler split of one batched round's kernel time into map sampler,
-rollout and the rest (a separate run after the timings).
+box of every planner.  c3m is c3 with 2048 sampled maps (defined here): its CVaR runs the CTA kernel, one CTA per
+control sequence, instead of the warp kernel.  --profile adds a torch.profiler split of one batched round's kernel time
+into map sampler, rollout and the rest (a separate run after the timings).
 """
 import argparse
 import json
@@ -29,6 +30,15 @@ if ROOT not in sys.path:
 
 from bench import WORKLOADS, make_planner, workload_name_of   # noqa: E402
 
+# config 3 with M 2048: above the warp CVaR kernel's 1024 maps
+LOCAL_WORKLOADS = {"c3m": WORKLOADS["c3"][:2] + (2048,) + WORKLOADS["c3"][3:]}
+
+
+def local_name_of(name):
+    mode, N, M, T, H, res, B, da = LOCAL_WORKLOADS[name]
+    return "%s: CVaR-cost MPPI N=%d M=%d T=%d, %dx%d PMF grid (%d bins, res %.1f m), num_opt=1 (config 3 with M %d)" % (
+        name, N, M, T, H, H, B, res, M)
+
 
 def run(args, emit):
     import ctypes as C
@@ -39,7 +49,7 @@ def run(args, emit):
     from mppi_numba_b200._lib import lib, check
     from tests.scenarios import make_scenario
     K = args.batch
-    mode, N, M, T, H, res, B, da = WORKLOADS[args.workload]
+    mode, N, M, T, H, res, B, da = LOCAL_WORKLOADS.get(args.workload) or WORKLOADS[args.workload]
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     scs = [make_scenario(mode, N=N, M=M, T=T, H=H, W=H, res=res, B=B, seed=k + 1, det_alpha=da) for k in range(K)]
@@ -124,7 +134,8 @@ def run(args, emit):
         gpu["power_limit_and_max_sm_clock"] = "unavailable (%r)" % e
     out = {"metric": "batched one-map solves: K sequential solve() calls vs one MPPI_Batch.solve()",
                      "unit": "solves/s", "value": bat["solves_per_s"], "higher_is_better": True,
-                     "config": {"workload": workload_name_of(args.workload), "batch": K,
+                     "config": {"workload": (local_name_of(args.workload) if args.workload in LOCAL_WORKLOADS else
+                                             workload_name_of(args.workload)), "batch": K,
                                 "planners": "seeds 1..K (different maps, start poses and goals), num_opt=1"},
                      "steps": args.steps, "warmup": args.warmup, "gpu": gpu, "parity_check": parity,
                      "sequential": seq, "batched": bat,
@@ -173,7 +184,7 @@ def main():
     def emit(line):
         os.write(real_stdout, (line + "\n").encode())
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[1])
-    ap.add_argument("--workload", default="c2", choices=["c2", "c3", "c4"])
+    ap.add_argument("--workload", default="c2", choices=["c2", "c3", "c4", "c3m"])
     ap.add_argument("--batch", type=int, default=64, metavar="K", help="planners in the batch")
     ap.add_argument("--steps", type=int, default=20, help="timed rounds per measurement")
     ap.add_argument("--warmup", type=int, default=5)

@@ -1,11 +1,12 @@
 #!/usr/bin/env python
 """bench_trials.py -- closed-loop episodes of K planners: the host-driven loop against the batch's device episodes.
 
-    python bench_trials.py --workload c2|c4|c3|ref --batch K --closed-loop S [--rounds R] [--profile]
+    python bench_trials.py --workload c2|c4|c3|ref|refm --batch K --closed-loop S [--rounds R] [--profile]
 
 c2 and c4 are one-map workloads (MPPI_Batch.run_trials); c3 and ref are stochastic (use_tdm, CVaR cost:
 MPPI_StochasticBatch.run_stochastic_trials).  ref is the reference benchmark's noisy_dyn trial shape (N 1024, M 1024,
 T 100, a 9 x 9-cell map at 1 m), defined here: every reach box leaves that map, so every step samples whole maps.
+refm is ref with 2048 sampled maps: a less noisy tail estimate, whose CVaR runs the CTA kernel.
 
 K planners of the workload (bench.py's WORKLOADS, seeds 1..K: different maps, start poses and warm starts), each with
 a seeded ground-truth TractionGrid over its map; every other planner has its goal 1.5 m away (reached within S steps),
@@ -15,7 +16,7 @@ final planner state (u, u_prev, noise, costs, weights, RNG states, sampled maps,
 exits non-zero.  Then R rounds of each, alternating, every round from the same start (params, warm start):
   host: the best host loop available -- the batch's solve() of all K, then per running planner a numpy plant step and
         shift_and_update, until every planner has stopped;
-  device: one run_trials(grids, S) (run_stochastic_trials for c3 and ref).
+  device: one run_trials(grids, S) (run_stochastic_trials for c3, ref and refm).
 Wall clock per round (each ends in a host synchronisation); control steps/s (planner-steps run), episodes/s, kernel
 launches per round.  Prints one JSON line with the card's name and power limit; writes nothing to the tree.
 """
@@ -35,7 +36,8 @@ if ROOT not in sys.path:
 from bench import WORKLOADS, make_planner, workload_name_of   # noqa: E402
 
 # the reference benchmark's noisy_dyn trial: N 1024, M 1024, T 100 on a 9 x 9-cell map at 1 m (c3's bins)
-LOCAL_WORKLOADS = {"ref": ("tdm", 1024, 1024, 100, 9, 1.0) + tuple(WORKLOADS["c3"][6:])}
+LOCAL_WORKLOADS = {"ref": ("tdm", 1024, 1024, 100, 9, 1.0) + tuple(WORKLOADS["c3"][6:]),
+                   "refm": ("tdm", 1024, 2048, 100, 9, 1.0) + tuple(WORKLOADS["c3"][6:])}
 
 
 def run(args, emit):
@@ -179,7 +181,7 @@ def main():
     def emit(line):
         os.write(real_stdout, (line + "\n").encode())
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[1])
-    ap.add_argument("--workload", default="c2", choices=["c2", "c4", "c3", "ref"])
+    ap.add_argument("--workload", default="c2", choices=["c2", "c4", "c3", "ref", "refm"])
     ap.add_argument("--batch", type=int, default=64, metavar="K", help="planners in the batch")
     ap.add_argument("--closed-loop", type=int, default=150, metavar="S", help="max control steps per episode")
     ap.add_argument("--rounds", type=int, default=3, help="timed rounds of each loop")

@@ -343,7 +343,8 @@ int b200mppi_batch_launch_count(b200mppi_batch* b, int64_t* out);
  * destroy work on it as above; b200mppi_batch_run_trials refuses it (b200mppi_batch_run_stochastic_trials below runs
  * its closed-loop trials).
  *   create: planners on one device, MODE_TDM, world_size 1, equal num_steps, num_control_rollouts and
- *           num_grid_samples (at most 1024), no planner listed twice.  Anything else: B200MPPI_EINVAL naming the planner.
+ *           num_grid_samples (any M a MODE_TDM planner takes, up to 16384), no planner listed twice.  Anything else:
+ *           B200MPPI_EINVAL naming the planner.
  *   solve : == b200mppi_planner_solve on planners[0], planners[1], ... in that order, bit for bit: u, noise, per-(m, n)
  *           costs, costs, weights, the planners' and their TDMs' RNG states, the sampled maps (boxed or whole), the
  *           reach-box decisions (b200mppi_planner_sample_box) and the host-side solve state.  Refused before any work is

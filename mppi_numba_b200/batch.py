@@ -12,8 +12,8 @@ Each planner keeps its own params, TDMs, warm start and RNG streams; ``solve()``
 solves).  The planners must share N, T, the device and the mode; their TDMs must not be shared between planners.
 
 ``MPPI_StochasticBatch(planners)`` does the same for use_tdm (CVaR-cost) planners of equal N, T and
-num_grid_samples (at most 1024): one launch per stage for noise, rollout, CVaR and update, the map sampling per planner
-(include/b200mppi.h, batched stochastic solves).
+num_grid_samples (any M a use_tdm planner takes, up to 15000 through Config): one launch per stage for noise, rollout,
+CVaR and update, the map sampling per planner (include/b200mppi.h, batched stochastic solves).
 
 ``run_trials(traction_grids, max_steps)`` runs the benchmark's closed-loop episode (solve, plant step on a ground-truth
 ``TractionGrid``, shift_and_update, stop at the goal) for every det-dynamics or speed-map planner at once on the GPU,
@@ -203,8 +203,10 @@ class MPPI_Batch(object):
 
 class MPPI_StochasticBatch(MPPI_Batch):
     """Borrows use_tdm ``planners`` (keeps them alive) and solves them with one launch per stage: noise, windowed
-    rollout, CVaR and update; each planner's map sampling keeps its own launches.  ``solve()``, ``set_stream`` and
-    ``launch_count`` as in MPPI_Batch; closed-loop trials through ``run_stochastic_trials``."""
+    rollout, CVaR and update; each planner's map sampling keeps its own launches.  The planners share N, T and
+    num_grid_samples, which may be any M a use_tdm planner takes: above 1024 maps the one CVaR launch runs one CTA
+    per control sequence instead of one warp.  ``solve()``, ``set_stream`` and ``launch_count`` as in MPPI_Batch;
+    closed-loop trials through ``run_stochastic_trials``."""
 
     def __init__(self, planners):
         planners = list(planners)

@@ -1913,10 +1913,11 @@ extern "C" int b200mppi_batch_create_stochastic(b200mppi_planner* const* planner
     if (p->M != q->M)
       return fail(B200MPPI_EINVAL, who + " has num_grid_samples " + std::to_string(p->M) + ", planner 0 " +
                                        std::to_string(q->M) + " (M must be equal)");
-    if (p->M > cvar_warp_max_maps())
-      return fail(B200MPPI_EINVAL, who + " has num_grid_samples " + std::to_string(p->M) + " (a stochastic batch takes " +
-                                       "at most " + std::to_string(cvar_warp_max_maps()) + " maps)");
   }
+  // any M a planner can have (planner_create: at most cvar_max_maps()).  Index ranges at the largest batch, 65535
+  // planners of 16384 maps: the windowed rollout's count * M (planner, map) units stay below 2^30 (an int), its chunk
+  // totals are 64-bit; the CVaR and sampler grids put the planner on y or z (<= 65535) and the map groups on y
+  // (<= 16384); the state advance's grid x and every descriptor offset are computed in 64 bits.
   CU(cudaSetDevice(planners[0]->cfg.device));
   b200mppi_batch* b = new b200mppi_batch();
   b->pl.assign(planners, planners + count);

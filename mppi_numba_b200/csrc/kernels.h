@@ -350,8 +350,9 @@ int cvar_max_maps();   // largest M the CVaR kernels accept
 // fw: flags to wait for before the costs are read (sharded solve, peer-memory exchange); FlagWait{} = none
 void launch_cvar(const float* costs_mn, float* costs, int n_cnt, int ld, int M, float cvar_alpha, const FlagWait& fw,
                  cudaStream_t st);
-int cvar_warp_max_maps();   // largest M of the warp kernel (the one the batched launch runs)
-// batched stochastic solves: one warp-kernel launch for `count` planners of equal n_cnt and M (planner = blockIdx.y)
+int cvar_warp_max_maps();   // largest M of the warp kernel (above it: the CTA kernel)
+// batched stochastic solves: one launch for `count` planners of equal n_cnt and M (planner = blockIdx.y) -- the warp
+// kernel up to cvar_warp_max_maps() maps, the CTA kernel (one CTA per control sequence) above
 // [emu:begin cvar_desc]
 struct CvarDesc {
   const float* costs_mn;    // map-major (M, ld)

@@ -344,14 +344,15 @@ __global__ void __launch_bounds__(CVAR_THREADS) cvar_kernel(const float* __restr
 // sequence, the M keys in shared memory, the same bitwise radix select with a CTA-wide count per bit.
 constexpr int CVAR_LARGE_THREADS = 256;
 
-__global__ void __launch_bounds__(CVAR_LARGE_THREADS) cvar_large_kernel(const float* __restrict__ costs_mn,
-                                                                        float* __restrict__ costs, int n_cnt, int ld,
-                                                                        int M, int numel, const FlagWait fw) {
+// control sequence n (blockIdx.x) by thread tid (threadIdx.x); M * 4 bytes of dynamic shared memory.  The kernels read
+// n and tid themselves: read here, the thread index of cvar_large_kernel would be hoisted above its flag_wait, and that
+// kernel's code would change with the split.
+__device__ __forceinline__ void cvar_large_body(const float* __restrict__ costs_mn, float* __restrict__ costs, int n_cnt,
+                                                int ld, int M, int numel, int n, int tid) {
   extern __shared__ uint32_t s_keys[];
-  flag_wait(fw);
   __shared__ int s_cnt[2][CVAR_LARGE_THREADS / 32];
   __shared__ float s_sum[CVAR_LARGE_THREADS / 32];
-  const int n = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int lane = tid & 31, warp = tid >> 5;
   for (int j = tid; j < M; j += CVAR_LARGE_THREADS) s_keys[j] = float_key(__ldcg(costs_mn + (size_t)j * ld + n));
   __syncthreads();
   uint32_t prefix = 0;
@@ -389,6 +390,13 @@ __global__ void __launch_bounds__(CVAR_LARGE_THREADS) cvar_large_kernel(const fl
   }
 }
 
+__global__ void __launch_bounds__(CVAR_LARGE_THREADS) cvar_large_kernel(const float* __restrict__ costs_mn,
+                                                                        float* __restrict__ costs, int n_cnt, int ld,
+                                                                        int M, int numel, const FlagWait fw) {
+  flag_wait(fw);
+  cvar_large_body(costs_mn, costs, n_cnt, ld, M, numel, blockIdx.x, threadIdx.x);
+}
+
 // [emu:end cvar]
 // batched stochastic solves: planner blockIdx.y; every planner has the batch's n_cnt and M (hence PER and the grid)
 // [emu:begin cvar_batch]
@@ -399,6 +407,14 @@ __global__ void __launch_bounds__(CVAR_THREADS) cvar_batch_kernel(const CvarDesc
   cvar_body<PER>(d.costs_mn, d.costs, d.n_cnt, d.ld, d.M, d.numel);
 }
 // [emu:end cvar_batch]
+// M > 1024: the CTA kernel, grid (n_cnt, count), control sequence blockIdx.x of planner blockIdx.y
+// [emu:begin cvar_large_batch]
+__global__ void __launch_bounds__(CVAR_LARGE_THREADS) cvar_large_batch_kernel(const CvarDesc* __restrict__ descs) {
+  const CvarDesc& d = descs[blockIdx.y];
+  if (d.active && !*d.active) return;
+  cvar_large_body(d.costs_mn, d.costs, d.n_cnt, d.ld, d.M, d.numel, blockIdx.x, threadIdx.x);
+}
+// [emu:end cvar_large_batch]
 int cvar_max_maps() { return CVAR_LARGE_MAX_MAPS; }
 int cvar_warp_max_maps() { return 32 * CVAR_MAX_PER_LANE; }
 
@@ -410,6 +426,13 @@ int cvar_numel(int M, float cvar_alpha) {
 }
 
 void launch_cvar_batch(const CvarDesc* descs, int count, int n_cnt, int M, cudaStream_t st) {
+  if (M > 32 * CVAR_MAX_PER_LANE) {
+    cudaFuncSetAttribute(cvar_large_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,   // per device
+                         CVAR_LARGE_MAX_MAPS * (int)sizeof(uint32_t));
+    const dim3 grid((unsigned)n_cnt, (unsigned)count);
+    cvar_large_batch_kernel<<<grid, CVAR_LARGE_THREADS, (size_t)M * sizeof(uint32_t), st>>>(descs);
+    return;
+  }
   const int nb = cvar_block_n(M);
   const dim3 grid((unsigned)((n_cnt + nb - 1) / nb), (unsigned)count);
   const int per = (M + 31) / 32;
