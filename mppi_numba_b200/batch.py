@@ -62,13 +62,17 @@ class MPPI_Batch(object):
             if kind != kinds[0][0]:
                 raise ValueError("MPPI_Batch: planner %d is a %s planner, planner 0 a %s planner (kinds cannot be mixed)"
                                  % (i, kind, kinds[0][0]))
+        self._create(planners, kinds[0][0], lib.b200mppi_batch_create)
+
+    def _create(self, planners, kind, create):
+        """Borrow ``planners`` and create the batch's handle with the C constructor ``create``."""
         self.planners = planners
-        self.kind = kinds[0][0]
+        self.kind = kind
         self.num_steps = planners[0].num_steps
         self._handle = None
         handles = (C.c_void_p * len(planners))(*[p._handle.value for p in planners])
         h = C.c_void_p()
-        check(lib.b200mppi_batch_create(handles, len(planners), C.byref(h)))
+        check(create(handles, len(planners), C.byref(h)))
         self._handle = h
 
     def __del__(self):
@@ -220,14 +224,7 @@ class MPPI_StochasticBatch(MPPI_Batch):
             if ws != 1:
                 raise ValueError("MPPI_StochasticBatch: planner %d has world_size %d (a batch holds single-rank planners)"
                                  % (i, ws))
-        self.planners = planners
-        self.kind = "tdm"
-        self.num_steps = planners[0].num_steps
-        self._handle = None
-        handles = (C.c_void_p * len(planners))(*[p._handle.value for p in planners])
-        h = C.c_void_p()
-        check(lib.b200mppi_batch_create_stochastic(handles, len(planners), C.byref(h)))
-        self._handle = h
+        self._create(planners, "tdm", lib.b200mppi_batch_create_stochastic)
 
     def solve(self):
         """One solve() of every planner.  Returns np.float32 (K, T, 2), or None (with the planner's index and the

@@ -1837,27 +1837,33 @@ static int batch_init(b200mppi_batch* b) {
   return B200MPPI_OK;
 }
 
-extern "C" int b200mppi_batch_create(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out) {
-  if (!planners || !out) return fail(B200MPPI_EINVAL, "batch_create: null argument");
-  if (count < 1) return fail(B200MPPI_EINVAL, "batch_create: count < 1");
-  if (count > 65535) return fail(B200MPPI_EINVAL, "batch_create: more than 65535 planners");
+// One-map batches hold MODE_DET_DYN, MODE_SPEED_MAP or MODE_BAREBONE planners of one mode; stochastic batches hold
+// MODE_TDM planners of equal M.  Both hold single-rank planners of one device, T and N.
+static int batch_create(b200mppi_planner* const* planners, int32_t count, bool stochastic, b200mppi_batch** out) {
+  const std::string fn = stochastic ? "batch_create_stochastic" : "batch_create";
+  if (!planners || !out) return fail(B200MPPI_EINVAL, fn + ": null argument");
+  if (count < 1) return fail(B200MPPI_EINVAL, fn + ": count < 1");
+  if (count > 65535) return fail(B200MPPI_EINVAL, fn + ": more than 65535 planners");
   for (int i = 0; i < count; ++i) {
     const b200mppi_planner* p = planners[i];
-    const std::string who = "batch_create: planner " + std::to_string(i);
+    const std::string who = fn + ": planner " + std::to_string(i);
     if (!p) return fail(B200MPPI_EINVAL, who + " is null");
     for (int j = 0; j < i; ++j)
       if (planners[j] == p) return fail(B200MPPI_EINVAL, who + " is planner " + std::to_string(j) + " again");
+    if (stochastic && p->cfg.mode != B200MPPI_MODE_TDM)
+      return fail(B200MPPI_EINVAL, who + " has mode " + std::to_string(p->cfg.mode) +
+                                       " (a stochastic batch holds MODE_TDM planners)");
+    if (!stochastic && p->cfg.mode == B200MPPI_MODE_TDM)
+      return fail(B200MPPI_EINVAL, who + " is MODE_TDM: the stochastic mode is not batched (batches hold "
+                                         "MODE_DET_DYN, MODE_SPEED_MAP or MODE_BAREBONE planners)");
     if (p->cfg.world_size != 1)
       return fail(B200MPPI_EINVAL, who + " has world_size " + std::to_string(p->cfg.world_size) +
                                        " (a batch holds single-rank planners)");
-    if (p->cfg.mode == B200MPPI_MODE_TDM)
-      return fail(B200MPPI_EINVAL, who + " is MODE_TDM: the stochastic mode is not batched (batches hold "
-                                         "MODE_DET_DYN, MODE_SPEED_MAP or MODE_BAREBONE planners)");
     const b200mppi_planner* q = planners[0];
     if (p->cfg.device != q->cfg.device)
       return fail(B200MPPI_EINVAL, who + " is on device " + std::to_string(p->cfg.device) + ", planner 0 on device " +
                                        std::to_string(q->cfg.device));
-    if (p->cfg.mode != q->cfg.mode)
+    if (!stochastic && p->cfg.mode != q->cfg.mode)
       return fail(B200MPPI_EINVAL, who + " has mode " + std::to_string(p->cfg.mode) + ", planner 0 mode " +
                                        std::to_string(q->cfg.mode) + " (modes cannot be mixed)");
     if (p->T != q->T) return fail(B200MPPI_EINVAL, who + " has num_steps " + std::to_string(p->T) + ", planner 0 " +
@@ -1865,12 +1871,21 @@ extern "C" int b200mppi_batch_create(b200mppi_planner* const* planners, int32_t 
     if (p->n_local != q->n_local)
       return fail(B200MPPI_EINVAL, who + " has num_control_rollouts " + std::to_string(p->n_local) + ", planner 0 " +
                                        std::to_string(q->n_local) + " (N must be equal)");
+    if (stochastic && p->M != q->M)
+      return fail(B200MPPI_EINVAL, who + " has num_grid_samples " + std::to_string(p->M) + ", planner 0 " +
+                                       std::to_string(q->M) + " (M must be equal)");
   }
+  // any M a planner can have (planner_create: at most cvar_max_maps()).  Index ranges at the largest batch, 65535
+  // planners of 16384 maps: the windowed rollout's count * M (planner, map) units stay below 2^30 (an int), its chunk
+  // totals are 64-bit; the CVaR and sampler grids put the planner on y or z (<= 65535) and the map groups on y
+  // (<= 16384); the state advance's grid x and every descriptor offset are computed in 64 bits.
   CU(cudaSetDevice(planners[0]->cfg.device));
   b200mppi_batch* b = new b200mppi_batch();
   b->pl.assign(planners, planners + count);
   b->device = planners[0]->cfg.device; b->mode = planners[0]->cfg.mode;
   b->T = planners[0]->T; b->N = planners[0]->n_local;
+  b->stochastic = stochastic;
+  if (stochastic) b->M = planners[0]->M;
   const int rc = batch_init(b);
   if (rc) {
     const std::string keep = g_err;
@@ -1882,57 +1897,15 @@ extern "C" int b200mppi_batch_create(b200mppi_planner* const* planners, int32_t 
   return B200MPPI_OK;
 }
 
+extern "C" int b200mppi_batch_create(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out) {
+  return batch_create(planners, count, false, out);
+}
+
 // K independent MODE_TDM planners of equal N, T and M solved with one launch per stage (noise + controls, windowed
 // rollout, CVaR, update); the map sampling stays per planner (each planner's reach box is its own).  The results are
 // those of K solve() calls in planner order, bit for bit (include/b200mppi.h).
 extern "C" int b200mppi_batch_create_stochastic(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out) {
-  if (!planners || !out) return fail(B200MPPI_EINVAL, "batch_create_stochastic: null argument");
-  if (count < 1) return fail(B200MPPI_EINVAL, "batch_create_stochastic: count < 1");
-  if (count > 65535) return fail(B200MPPI_EINVAL, "batch_create_stochastic: more than 65535 planners");
-  for (int i = 0; i < count; ++i) {
-    const b200mppi_planner* p = planners[i];
-    const std::string who = "batch_create_stochastic: planner " + std::to_string(i);
-    if (!p) return fail(B200MPPI_EINVAL, who + " is null");
-    for (int j = 0; j < i; ++j)
-      if (planners[j] == p) return fail(B200MPPI_EINVAL, who + " is planner " + std::to_string(j) + " again");
-    if (p->cfg.mode != B200MPPI_MODE_TDM)
-      return fail(B200MPPI_EINVAL, who + " has mode " + std::to_string(p->cfg.mode) +
-                                       " (a stochastic batch holds MODE_TDM planners)");
-    if (p->cfg.world_size != 1)
-      return fail(B200MPPI_EINVAL, who + " has world_size " + std::to_string(p->cfg.world_size) +
-                                       " (a batch holds single-rank planners)");
-    const b200mppi_planner* q = planners[0];
-    if (p->cfg.device != q->cfg.device)
-      return fail(B200MPPI_EINVAL, who + " is on device " + std::to_string(p->cfg.device) + ", planner 0 on device " +
-                                       std::to_string(q->cfg.device));
-    if (p->T != q->T) return fail(B200MPPI_EINVAL, who + " has num_steps " + std::to_string(p->T) + ", planner 0 " +
-                                                      std::to_string(q->T) + " (T must be equal)");
-    if (p->n_local != q->n_local)
-      return fail(B200MPPI_EINVAL, who + " has num_control_rollouts " + std::to_string(p->n_local) + ", planner 0 " +
-                                       std::to_string(q->n_local) + " (N must be equal)");
-    if (p->M != q->M)
-      return fail(B200MPPI_EINVAL, who + " has num_grid_samples " + std::to_string(p->M) + ", planner 0 " +
-                                       std::to_string(q->M) + " (M must be equal)");
-  }
-  // any M a planner can have (planner_create: at most cvar_max_maps()).  Index ranges at the largest batch, 65535
-  // planners of 16384 maps: the windowed rollout's count * M (planner, map) units stay below 2^30 (an int), its chunk
-  // totals are 64-bit; the CVaR and sampler grids put the planner on y or z (<= 65535) and the map groups on y
-  // (<= 16384); the state advance's grid x and every descriptor offset are computed in 64 bits.
-  CU(cudaSetDevice(planners[0]->cfg.device));
-  b200mppi_batch* b = new b200mppi_batch();
-  b->pl.assign(planners, planners + count);
-  b->device = planners[0]->cfg.device; b->mode = B200MPPI_MODE_TDM;
-  b->T = planners[0]->T; b->N = planners[0]->n_local; b->M = planners[0]->M;
-  b->stochastic = true;
-  const int rc = batch_init(b);
-  if (rc) {
-    const std::string keep = g_err;
-    b200mppi_batch_destroy(b);
-    g_err = keep;
-    return rc;
-  }
-  *out = b;
-  return B200MPPI_OK;
+  return batch_create(planners, count, true, out);
 }
 
 extern "C" int b200mppi_batch_set_stream(b200mppi_batch* b, void* s) {
@@ -1976,6 +1949,11 @@ static int batch_validate(b200mppi_batch* b) {
   return B200MPPI_OK;
 }
 
+// sample_box() after a whole-map sampling
+static void last_box_whole_map(b200mppi_planner* p) {
+  p->last_box[0] = 0; p->last_box[1] = 0; p->last_box[2] = p->lin->rows; p->last_box[3] = 0; p->last_box[4] = p->lin->cols;
+}
+
 // The maps of every planner, as its solve() samples them: the pairs whose plan is fused and whose launch equals the
 // first such pair's go into ONE launch; every other pair runs its own plan, in planner order.  One-map modes never
 // sample a reach box.
@@ -2007,7 +1985,6 @@ static int batch_run_sample(b200mppi_batch* b, const SampleGridsV2Args* h_sg, co
     CHECK_LAUNCH();
   }
   for (size_t i = 0; i < plans.size(); ++i) {
-    b200mppi_planner* p = b->pl[i];
     if (joined[i]) {
       plan_commit(plans[i], 0);
       plan_commit(plans[i], 1);
@@ -2015,7 +1992,7 @@ static int batch_run_sample(b200mppi_batch* b, const SampleGridsV2Args* h_sg, co
       const int rc = plan_launch(plans[i], false, b->stream, &b->launches);
       if (rc) return rc;
     }
-    p->last_box[0] = 0; p->last_box[1] = 0; p->last_box[2] = p->lin->rows; p->last_box[3] = 0; p->last_box[4] = p->lin->cols;
+    last_box_whole_map(b->pl[i]);
   }
   return B200MPPI_OK;
 }
@@ -2033,34 +2010,40 @@ static int batch_wait_members(b200mppi_batch* b) {
   return B200MPPI_OK;
 }
 
-static int batch_solve_stochastic(b200mppi_batch* b, float* u_out);
+// planner p's batched update: UPD_TAIL_APPLY also stores the new u at u_out (the batch's (K, T, 2)) and u_prev if set
+static void fill_update_apply(b200mppi_planner* p, UpdateBatchDesc& u, float* u_out, float* u_prev) {
+  fill_update_args(p, u.a, nullptr);
+  u.tl = UpdateTail{};
+  u.tl.counter = p->upd_counter_d;
+  u.tl.mode = UPD_TAIL_APPLY;
+  u.tl.u_prev = u_prev;
+  u.tl.u_out = u_out;
+}
 
-extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
-  if (!b) return fail(B200MPPI_EINVAL, "null batch");
-  if (b->stochastic) return batch_solve_stochastic(b, u_out);
-  int rc = batch_validate(b);
-  if (rc) return rc;
-  CU(cudaSetDevice(b->device));
-  const int K = (int)b->pl.size(), T = b->T;
-  cudaStream_t st = b->stream;
-  if ((rc = batch_wait_members(b))) return rc;
-  // descriptors, built on the host for this solve and uploaded with ONE copy before the first launch (the sampler's
-  // are decided here too: its host-side preparation may synchronise the stream)
-  NoiseDesc* hn = reinterpret_cast<NoiseDesc*>(b->h_desc);
-  SampleGridsV2Args* hs = reinterpret_cast<SampleGridsV2Args*>(b->h_desc + b->off_sample);
-  RolloutArgs* hr = reinterpret_cast<RolloutArgs*>(b->h_desc + b->off_roll);
-  UpdateBatchDesc* hu = reinterpret_cast<UpdateBatchDesc*>(b->h_desc + b->off_upd);
-  for (int i = 0; i < K; ++i) {
+// A one-map batch's noise, rollout and update descriptors at byte offset 0 of `h` (b->h_desc's layout)
+static void onemap_descs(b200mppi_batch* b, unsigned char* h) {
+  NoiseDesc* hn = reinterpret_cast<NoiseDesc*>(h);
+  RolloutArgs* hr = reinterpret_cast<RolloutArgs*>(h + b->off_roll);
+  UpdateBatchDesc* hu = reinterpret_cast<UpdateBatchDesc*>(h + b->off_upd);
+  for (int i = 0; i < (int)b->pl.size(); ++i) {
     b200mppi_planner* p = b->pl[i];
     hn[i] = NoiseDesc{p->states, p->noise, p->prm.u_std[0], p->prm.u_std[1]};
     fill_rollout_args(p, hr[i]);
-    fill_update_args(p, hu[i].a, nullptr);
-    hu[i].tl = UpdateTail{};
-    hu[i].tl.counter = p->upd_counter_d;
-    hu[i].tl.mode = UPD_TAIL_APPLY;
-    hu[i].tl.u_prev = p->u_prev;                       // self.u_prev_d = self.u_cur_d (alias, mppi.py:292,362)
-    hu[i].tl.u_out = b->u_d + (size_t)i * T * 2;
+    // self.u_prev_d = self.u_cur_d (alias, mppi.py:292,362)
+    fill_update_apply(p, hu[i], b->u_d + (size_t)i * b->T * 2, p->u_prev);
   }
+}
+
+static int batch_solve_onemap(b200mppi_batch* b) {
+  CU(cudaSetDevice(b->device));
+  const int K = (int)b->pl.size(), T = b->T;
+  cudaStream_t st = b->stream;
+  int rc = batch_wait_members(b);
+  if (rc) return rc;
+  // descriptors, built on the host for this solve and uploaded with ONE copy before the first launch (the sampler's
+  // are decided here too: its host-side preparation may synchronise the stream)
+  onemap_descs(b, b->h_desc);
+  SampleGridsV2Args* hs = reinterpret_cast<SampleGridsV2Args*>(b->h_desc + b->off_sample);
   const NoiseDesc* dn = reinterpret_cast<const NoiseDesc*>(b->d_desc);
   const SampleGridsV2Args* ds = reinterpret_cast<const SampleGridsV2Args*>(b->d_desc + b->off_sample);
   const RolloutArgs* dr = reinterpret_cast<const RolloutArgs*>(b->d_desc + b->off_roll);
@@ -2072,12 +2055,8 @@ extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
   if (maps && (rc = batch_plan_sample(b, hs, plans, joined, &nj))) return rc;
   CU(cudaMemcpyAsync(b->d_desc, b->h_desc, b->desc_bytes, cudaMemcpyHostToDevice, st));
   const int num_opt = b->pl[0]->prm.num_opt;
-  if (num_opt <= 0) {                                  // the reference samples before its (empty) loop; u unchanged
-    if (maps && (rc = batch_run_sample(b, hs, ds, plans, joined, nj))) return rc;
-    for (int i = 0; i < K; ++i)
-      CU(cudaMemcpyAsync(b->u_d + (size_t)i * T * 2, b->pl[i]->u_cur, (size_t)T * 2 * sizeof(float),
-                         cudaMemcpyDeviceToDevice, st));
-  }
+  // the reference samples before its (empty) loop
+  if (num_opt <= 0 && maps && (rc = batch_run_sample(b, hs, ds, plans, joined, nj))) return rc;
   // solve(): num_opt x (noise, [first iteration: maps], rollout, update)
   for (int k = 0; k < num_opt; ++k) {
     launch_sample_noise_batch(dn, K, b->N, T, nullptr, st);
@@ -2093,10 +2072,6 @@ extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
     b->launches++;
     CHECK_LAUNCH();
   }
-  CU(cudaMemcpyAsync(b->h_u, b->u_d, (size_t)K * T * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
-  // the host waits for the whole batch: work issued afterwards on any member's stream sees its results
-  CU(cudaStreamSynchronize(st));
-  if (u_out) std::memcpy(u_out, b->h_u, (size_t)K * T * 2 * sizeof(float));
   return B200MPPI_OK;
 }
 
@@ -2147,20 +2122,16 @@ static void stochastic_descs(b200mppi_batch* b, unsigned char* h, int WW, int WH
     *masks01 = *masks01 && hw[i].masks01;
     std::memcpy(ht + (size_t)i * sizeof(b200mppi_planner::tmaps), p->tmaps, sizeof(b200mppi_planner::tmaps));
     hc[i] = CvarDesc{p->costs_nm, p->costs, p->n_local, p->n_local, p->M, cvar_numel(p->M, q.cvar_alpha), nullptr};
-    fill_update_args(p, hu[i].a, nullptr);
-    hu[i].tl = UpdateTail{};
-    hu[i].tl.counter = p->upd_counter_d;
-    hu[i].tl.mode = UPD_TAIL_APPLY;
-    hu[i].tl.u_out = b->u_d + (size_t)i * T * 2;        // u_prev stays null: a stochastic solve does not alias it
+    // u_prev stays null: a stochastic solve does not alias it
+    fill_update_apply(p, hu[i], b->u_d + (size_t)i * T * 2, nullptr);
   }
 }
 
-static int batch_solve_stochastic(b200mppi_batch* b, float* u_out) {
-  int rc = batch_validate(b);
-  if (rc) return rc;
+static int batch_solve_stochastic(b200mppi_batch* b) {
   const int K = (int)b->pl.size(), T = b->T, N = b->N;
   int WW, WH;
-  if ((rc = stochastic_validate(b, "batch_solve", &WW, &WH))) return rc;
+  int rc = stochastic_validate(b, "batch_solve", &WW, &WH);
+  if (rc) return rc;
   cudaStream_t st = b->stream;
   if ((rc = batch_wait_members(b))) return rc;
   const RolloutWinArgs* hw = reinterpret_cast<const RolloutWinArgs*>(b->h_desc + b->off_win);
@@ -2177,13 +2148,9 @@ static int batch_solve_stochastic(b200mppi_batch* b, float* u_out) {
   const CvarDesc* dc = reinterpret_cast<const CvarDesc*>(b->d_desc + b->off_cvar);
   const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(b->d_desc + b->off_upd);
   const int num_opt = b->pl[0]->prm.num_opt;
-  if (num_opt <= 0) {                                  // the reference samples before its (empty) loop; u unchanged
-    for (int i = 0; i < K; ++i) {
+  if (num_opt <= 0)                                    // the reference samples before its (empty) loop
+    for (int i = 0; i < K; ++i)
       if ((rc = sample_finish(b->pl[i], plans[i], nullptr, false, st, &b->launches))) return rc;
-      CU(cudaMemcpyAsync(b->u_d + (size_t)i * T * 2, b->pl[i]->u_cur, (size_t)T * 2 * sizeof(float),
-                         cudaMemcpyDeviceToDevice, st));
-    }
-  }
   for (int k = 0; k < num_opt; ++k) {
     launch_noise_prepare_batch(dn, K, N, T, b->pl[0]->npad, k, nullptr, st);
     b->launches++;
@@ -2228,9 +2195,22 @@ static int batch_solve_stochastic(b200mppi_batch* b, float* u_out) {
     b->launches++;
     CHECK_LAUNCH();
   }
-  CU(cudaMemcpyAsync(b->h_u, b->u_d, (size_t)K * T * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  if (u_out) std::memcpy(u_out, b->h_u, (size_t)K * T * 2 * sizeof(float));
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  int rc = batch_validate(b);
+  if (rc) return rc;
+  if ((rc = b->stochastic ? batch_solve_stochastic(b) : batch_solve_onemap(b))) return rc;
+  const size_t n = (size_t)b->T * 2, ubytes = b->pl.size() * n * sizeof(float);
+  if (b->pl[0]->prm.num_opt <= 0)                      // u unchanged
+    for (size_t i = 0; i < b->pl.size(); ++i)
+      CU(cudaMemcpyAsync(b->u_d + i * n, b->pl[i]->u_cur, n * sizeof(float), cudaMemcpyDeviceToDevice, b->stream));
+  CU(cudaMemcpyAsync(b->h_u, b->u_d, ubytes, cudaMemcpyDeviceToHost, b->stream));
+  // the host waits for the whole batch: work issued afterwards on any member's stream sees its results
+  CU(cudaStreamSynchronize(b->stream));
+  if (u_out) std::memcpy(u_out, b->h_u, ubytes);
   return B200MPPI_OK;
 }
 
@@ -2268,219 +2248,21 @@ static int trial_validate(b200mppi_batch* b, const b200mppi_trial_desc* tr, int3
   return B200MPPI_OK;
 }
 
-extern "C" int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps,
-                                         double* xhist, float* uhist, b200mppi_trial_result* results,
-                                         int32_t* steps_issued) {
-  if (!b) return fail(B200MPPI_EINVAL, "null batch");
-  if (b->stochastic)
-    return fail(B200MPPI_EINVAL, "run_trials: planner 0 is MODE_TDM (trials run det-dynamics or speed-map batches: a "
-                                 "stochastic solve sizes each planner's map-sampling box on the host)");
-  int rc = trial_validate(b, trials, max_steps);
-  if (rc) return rc;
-  if (!xhist || !uhist || !results) return fail(B200MPPI_EINVAL, "run_trials: null output buffer");
-  CU(cudaSetDevice(b->device));
-  const int K = (int)b->pl.size(), T = b->T, S = max_steps;
-  cudaStream_t st = b->stream;
-  // the sampler plans first (their host preparation may synchronise the stream): every pair must join the one launch
-  std::vector<unsigned char> hd(b->desc_bytes + align256((size_t)K * sizeof(SampleGridsV2Args)));
-  SampleGridsV2Args* hs0 = reinterpret_cast<SampleGridsV2Args*>(hd.data() + b->off_sample);
-  std::vector<SamplePlan> plans;
-  std::vector<char> joined;
-  int nj = 0;
-  if ((rc = batch_plan_sample(b, hs0, plans, joined, &nj))) return rc;
-  for (int i = 0; i < K; ++i)
-    if (!joined[i])
-      return fail(B200MPPI_EINVAL, "run_trials: planner " + std::to_string(i) + ": its TDM pair cannot join the batch's "
-                                   "one sampler launch (map geometry, PMF or generator streams differ from planner 0's)");
-  for (b200mppi_planner* p : b->pl) {
-    if (p->stream == st) continue;
-    const cudaError_t q = cudaStreamQuery(p->stream);
-    if (q == cudaSuccess) continue;
-    if (q != cudaErrorNotReady) CU(q);
-    CU(cudaEventRecord(b->ev, p->stream));
-    CU(cudaStreamWaitEvent(st, b->ev, 0));
-  }
-  // device buffers of this call: [descriptors + the parity-1 sampler set | trials | states | active K + count | grids
-  // | xhist | uhist]
-  const size_t off_s1 = b->desc_bytes;
-  const size_t off_tr = off_s1 + align256((size_t)K * sizeof(SampleGridsV2Args));
-  const size_t off_state = off_tr + align256((size_t)K * sizeof(TrialDev));
-  const size_t off_act = off_state + align256((size_t)K * sizeof(TrialState));
-  size_t off = off_act + align256((size_t)(K + 1) * sizeof(int));
-  std::vector<size_t> off_grid(K);
-  for (int i = 0; i < K; ++i) {
-    off_grid[i] = off;
-    off += align256((size_t)2 * trials[i].height * trials[i].width * sizeof(double));
-  }
-  const size_t off_xh = off, off_uh = off_xh + align256((size_t)K * (S + 1) * 3 * sizeof(double));
-  const size_t total = off_uh + align256((size_t)K * S * 2 * sizeof(float));
-  const size_t head = off_xh;                         // uploaded part
-  unsigned char* d = nullptr;
-  unsigned char* h = nullptr;
-  CU(cudaMalloc(&d, total));
-  if (cudaMallocHost(&h, total) != cudaSuccess) { cudaFree(d); return fail(B200MPPI_ECUDA, "run_trials: cudaMallocHost"); }
-  struct Free {
-    unsigned char *d, *h;
-    ~Free() { cudaFree(d); cudaFreeHost(h); }
-  } guard{d, h};
-  std::memcpy(h, hd.data(), b->desc_bytes);
-  NoiseDesc* hn = reinterpret_cast<NoiseDesc*>(h);
-  SampleGridsV2Args* hs[2] = {reinterpret_cast<SampleGridsV2Args*>(h + b->off_sample),
-                              reinterpret_cast<SampleGridsV2Args*>(h + off_s1)};
-  RolloutArgs* hr = reinterpret_cast<RolloutArgs*>(h + b->off_roll);
-  UpdateBatchDesc* hu = reinterpret_cast<UpdateBatchDesc*>(h + b->off_upd);
-  TrialDev* ht = reinterpret_cast<TrialDev*>(h + off_tr);
-  TrialState* hst = reinterpret_cast<TrialState*>(h + off_state);
-  int* hact = reinterpret_cast<int*>(h + off_act);
-  RolloutArgs* dr = reinterpret_cast<RolloutArgs*>(d + b->off_roll);
+// A stochastic batch's trial sampler sets (set0: parity 0) and launch size.  Every pair must join the one boxed sampler
+// launch: a fused plan (identical generator streams, well-formed PMF at its alpha, lin != ang) whose launch and box
+// segments equal planner 0's.
+static int stochastic_trial_plans(b200mppi_batch* b, const std::string& fn, std::vector<SamplePlan>& plans,
+                                  std::vector<SampleGridsV2Args>& set0, int* mrows, int* ncact) {
+  const int K = (int)b->pl.size();
+  plans.resize(K);
   for (int i = 0; i < K; ++i) {
     b200mppi_planner* p = b->pl[i];
-    hn[i] = NoiseDesc{p->states, p->noise, p->prm.u_std[0], p->prm.u_std[1]};
-    fill_rollout_args(p, hr[i]);
-    fill_update_args(p, hu[i].a, nullptr);
-    hu[i].tl = UpdateTail{};
-    hu[i].tl.counter = p->upd_counter_d;
-    hu[i].tl.mode = UPD_TAIL_APPLY;
-    hu[i].tl.u_prev = p->u_prev;                       // self.u_prev_d = self.u_cur_d (alias, mppi.py:292,362)
-    hu[i].tl.u_out = b->u_d + (size_t)i * T * 2;
-    // parity 1: the pair samples from the buffers parity 0 wrote into
-    hs[1][i] = hs[0][i];
-    for (SampleTdm& td : hs[1][i].t) {
-      uint64_t* in = td.states_out;
-      td.states_out = const_cast<uint64_t*>(td.states);
-      td.states = in;
-    }
-    const b200mppi_trial_desc& q = trials[i];
-    const size_t cells = (size_t)q.height * q.width;
-    double* g = reinterpret_cast<double*>(h + off_grid[i]);
-    std::memcpy(g, q.lin, cells * sizeof(double));
-    std::memcpy(g + cells, q.ang, cells * sizeof(double));
-    const double* dg = reinterpret_cast<const double*>(d + off_grid[i]);
-    TrialDev& t = ht[i];
-    t = TrialDev{};                                   // win stays null: one-map rollouts have no window
-    t.lin = dg; t.ang = dg + cells; t.H = q.height; t.W = q.width;
-    t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res; t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1];
-    t.tol = q.goal_tolerance;
-    t.pxlim[0] = q.pxlim[0]; t.pxlim[1] = q.pxlim[1]; t.pylim[0] = q.pylim[0]; t.pylim[1] = q.pylim[1];
-    t.u_cur = p->u_cur;
-    t.x0_out = dr[i].p.x0;
-    hst[i] = TrialState{};
-    for (int c = 0; c < 3; ++c) hst[i].x[c] = q.x0[c];
-    hact[i] = 1;
-  }
-  hact[K] = K;
-  CU(cudaMemcpyAsync(d, h, head, cudaMemcpyHostToDevice, st));
-  const NoiseDesc* dn = reinterpret_cast<const NoiseDesc*>(d);
-  const SampleGridsV2Args* ds[2] = {reinterpret_cast<const SampleGridsV2Args*>(d + b->off_sample),
-                                    reinterpret_cast<const SampleGridsV2Args*>(d + off_s1)};
-  const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(d + b->off_upd);
-  int* dact = reinterpret_cast<int*>(d + off_act);
-  PlantArgs pa{};
-  pa.trials = reinterpret_cast<const TrialDev*>(d + off_tr);
-  pa.state = reinterpret_cast<TrialState*>(d + off_state);
-  pa.active = dact; pa.active_count = dact + K;
-  pa.xhist = reinterpret_cast<double*>(d + off_xh);
-  pa.uhist = reinterpret_cast<float*>(d + off_uh);
-  pa.K = K; pa.T = T; pa.max_steps = S;
-  // the polled counts live in the (no longer needed) head of the pinned staging, one slot per step in flight
-  CU(cudaStreamSynchronize(st));                      // the staging is read by the upload above
-  int* hcount = reinterpret_cast<int*>(h);
-  cudaEvent_t ev[TRIAL_POLL] = {};
-  struct Events {
-    cudaEvent_t* e;
-    ~Events() { for (int i = 0; i < TRIAL_POLL; ++i) if (e[i]) cudaEventDestroy(e[i]); }
-  } evguard{ev};
-  for (auto& e : ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  const int num_opt = b->pl[0]->prm.num_opt;
-  int issued = 0;
-  for (int s = 0; s < S; ++s) {
-    if (s >= TRIAL_POLL) {                            // the count after step s - POLL
-      CU(cudaEventSynchronize(ev[s % TRIAL_POLL]));
-      if (hcount[s % TRIAL_POLL] == 0) break;
-    }
-    for (int k = 0; k < num_opt; ++k) {
-      launch_sample_noise_batch(dn, K, b->N, T, dact, st);
-      CHECK_LAUNCH();
-      if (k == 0) {
-        launch_sample_grids_v2_batch(hs[0][0], ds[s & 1], K, dact, st);
-        CHECK_LAUNCH();
-      }
-      launch_rollout_batch(dr, K, b->mode, b->N, T, dact, st);
-      CHECK_LAUNCH();
-      launch_update_partial_batch(du, K, b->pl[0]->num_ctas, dact, st);
-      CHECK_LAUNCH();
-    }
-    pa.step = s;
-    launch_plant_step(pa, st);
-    CHECK_LAUNCH();
-    b->launches += 3 * num_opt + 2;
-    ++issued;
-    CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, dact + K, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(ev[s % TRIAL_POLL], st));
-  }
-  CU(cudaMemcpyAsync(h + off_state, d + off_state, off_act - off_state, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(h + off_xh, d + off_xh, total - off_xh, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  const double* hx = reinterpret_cast<const double*>(h + off_xh);
-  const float* hu_h = reinterpret_cast<const float*>(h + off_uh);
-  const double dnan = std::nan("");
-  const float fnan = std::nanf("");
-  for (int i = 0; i < K; ++i) {
-    const TrialState& r = hst[i];
-    const int n = r.steps;
-    double* xo = xhist + (size_t)i * (S + 1) * 3;
-    float* uo = uhist + (size_t)i * S * 2;
-    for (int c = 0; c < 3; ++c) xo[c] = trials[i].x0[c];
-    std::memcpy(xo + 3, hx + ((size_t)i * (S + 1) + 1) * 3, (size_t)n * 3 * sizeof(double));
-    for (size_t j = (size_t)(n + 1) * 3; j < (size_t)(S + 1) * 3; ++j) xo[j] = dnan;
-    std::memcpy(uo, hu_h + (size_t)i * S * 2, (size_t)n * 2 * sizeof(float));
-    for (size_t j = (size_t)n * 2; j < (size_t)S * 2; ++j) uo[j] = fnan;
-    results[i] = b200mppi_trial_result{r.cum_obj, r.cum_dist, r.dist, n, r.status};
-    // host state as after n rounds of the host loop: n samplings of the pair, the last solve's x0 in the params
-    b200mppi_planner* p = b->pl[i];
-    for (int s = 0; s < n; ++s) { plan_commit(plans[i], 0); plan_commit(plans[i], 1); }
-    p->prepared = false;
-    p->pushed_direct = false;
-    p->last_box[0] = 0; p->last_box[1] = 0; p->last_box[2] = p->lin->rows; p->last_box[3] = 0; p->last_box[4] = p->lin->cols;
-    for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)xo[(size_t)(n - 1) * 3 + c];
-  }
-  if (steps_issued) *steps_issued = issued;
-  return B200MPPI_OK;
-}
-
-// Closed-loop trials of a stochastic batch.  As for one-map batches, only x0 and the parity of the generator-state
-// double buffers change from step to step -- plus each planner's reach box, which moves with the robot and, with
-// box_mode 2 and num_opt 1, depends on the controls drawn: the batched boxed sampler decides it on the device
-// (reach_box_decide, the function sample_finish calls), so a step needs no host round trip.  Per step: num_opt x (noise +
-// controls, [first iteration: boxed sampler, state advance], windowed rollout, CVaR, update) and the plant step, which
-// also moves each planner's rollout window.
-extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials,
-                                                    int32_t max_steps, double* xhist, float* uhist,
-                                                    b200mppi_trial_result* results, int32_t* steps_issued) {
-  static const char* FN = "run_stochastic_trials";
-  if (!b) return fail(B200MPPI_EINVAL, "null batch");
-  if (!b->stochastic)
-    return fail(B200MPPI_EINVAL, std::string(FN) + ": planner 0 is " +
-                                     (b->mode == B200MPPI_MODE_DET_DYN ? "MODE_DET_DYN" :
-                                      b->mode == B200MPPI_MODE_SPEED_MAP ? "MODE_SPEED_MAP" : "MODE_BAREBONE") +
-                                     " (stochastic trials run MODE_TDM batches; b200mppi_batch_run_trials runs the others)");
-  int rc = trial_validate(b, trials, max_steps, FN);
-  if (rc) return rc;
-  if (!xhist || !uhist || !results) return fail(B200MPPI_EINVAL, std::string(FN) + ": null output buffer");
-  int WW, WH;
-  if ((rc = stochastic_validate(b, FN, &WW, &WH))) return rc;
-  const int K = (int)b->pl.size(), T = b->T, N = b->N, S = max_steps;
-  cudaStream_t st = b->stream;
-  // every pair must join the one boxed sampler launch: a fused plan (identical generator streams, well-formed PMF at
-  // its alpha, lin != ang) whose launch and box segments equal planner 0's
-  std::vector<SamplePlan> plans(K);
-  for (int i = 0; i < K; ++i) {
-    b200mppi_planner* p = b->pl[i];
-    if ((rc = plan_sampling(p->lin, p->ang, sample_alpha(p), st, &plans[i]))) return rc;
+    const int rc = plan_sampling(p->lin, p->ang, sample_alpha(p), b->stream, &plans[i]);
+    if (rc) return rc;
     const b200mppi_tdm* l = p->lin; const b200mppi_tdm* l0 = b->pl[0]->lin;
     if (!plans[i].fused || !sample_grids_v2_same_launch(plans[0].a[0], plans[i].a[0]) || l->box_segs != l0->box_segs ||
         l->box_seg_rows != l0->box_seg_rows)
-      return fail(B200MPPI_EINVAL, std::string(FN) + ": planner " + std::to_string(i) + ": its TDM pair cannot join the "
+      return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(i) + ": its TDM pair cannot join the "
                                    "batch's one sampler launch (lin == ang, or map geometry, PMF or generator streams "
                                    "differ from planner 0's)");
   }
@@ -2505,31 +2287,85 @@ extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b20
     any_box = true;
     span = std::fmax(span, 2.0 * R / (double)c.res + 8.0);
   }
-  int mrows = sg.tx, ncact = sg.ty;
+  *mrows = sg.tx;
+  *ncact = sg.ty;
   if (any_box && span < (double)(sg.rows + sg.cols)) {
-    mrows = std::min(sg.tx, (int)span / nrow + 2);
-    ncact = std::min(sg.ty, (int)span / ncol + 2);
+    *mrows = std::min(sg.tx, (int)span / nrow + 2);
+    *ncact = std::min(sg.ty, (int)span / ncol + 2);
   }
-  int gm_b = 128 / ncact;                             // apply_box's maps per CTA for that many tile columns
+  int gm_b = 128 / *ncact;                            // apply_box's maps per CTA for that many tile columns
   gm_b = std::max(1, std::min(std::min(gm_b, SG_GM_MAX), sg.num_maps));
-  {
-    SampleGridsV2Args geom = sg;
-    geom.gm = gm_b;
-    if (!sample_box_batch_fits(geom, ncact))
-      return fail(B200MPPI_EINVAL, std::string(FN) + ": planner 0: the batched sampler launch (" + std::to_string(ncact) +
-                                   " tile columns x " + std::to_string(gm_b) + " maps per CTA) does not fit a CTA");
+  // the boxed launch's row segments over the whole-map plan
+  for (int i = 0; i < K; ++i) {
+    const b200mppi_tdm* l = b->pl[i]->lin;
+    set0[i] = plans[i].a[0];
+    set0[i].segs = l->box_segs; set0[i].seg_rows = l->box_seg_rows; set0[i].jump = l->jump_box_d;
+    set0[i].write_states = 0;
+    set0[i].gm = gm_b;
+  }
+  if (!sample_box_batch_fits(set0[0], *ncact))
+    return fail(B200MPPI_EINVAL, fn + ": planner 0: the batched sampler launch (" + std::to_string(*ncact) +
+                                 " tile columns x " + std::to_string(gm_b) + " maps per CTA) does not fit a CTA");
+  return B200MPPI_OK;
+}
+
+// The closed-loop trials of both kinds of batch.  Stochastic trials also move each planner's reach box with the robot;
+// with box_mode 2 and num_opt 1 it depends on the controls drawn, so the batched boxed sampler decides it on the device
+// (reach_box_decide, the function sample_finish calls) and a step needs no host round trip.  Per step: num_opt x
+// (noise [+ controls], [first iteration: sampler (stochastic: boxed, then the state advance)], rollout [windowed, then
+// CVaR], update) and the plant step, which for stochastic trials also moves each planner's rollout window.
+// Device buffer of a call: [descriptors (b->h_desc's layout; a one-map batch's parity-0 sampler set is its own section
+// there) | stochastic: the parity-0 sampler set | the parity-1 set | stochastic: box descriptors, box records | states |
+// trials | active K + count | grids | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds xhist
+// and uhist: the float64 ground-truth grids (tens of MB for a batch of large maps) are copied straight from the
+// caller's arrays.
+static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_trial_desc* trials, int32_t max_steps,
+                            double* xhist, float* uhist, b200mppi_trial_result* results, int32_t* steps_issued) {
+  const std::string fn = stochastic ? "run_stochastic_trials" : "run_trials";
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  if (b->stochastic && !stochastic)
+    return fail(B200MPPI_EINVAL, "run_trials: planner 0 is MODE_TDM (trials run det-dynamics or speed-map batches: a "
+                                 "stochastic solve sizes each planner's map-sampling box on the host)");
+  if (!b->stochastic && stochastic)
+    return fail(B200MPPI_EINVAL, fn + ": planner 0 is " +
+                                     (b->mode == B200MPPI_MODE_DET_DYN ? "MODE_DET_DYN" :
+                                      b->mode == B200MPPI_MODE_SPEED_MAP ? "MODE_SPEED_MAP" : "MODE_BAREBONE") +
+                                     " (stochastic trials run MODE_TDM batches; b200mppi_batch_run_trials runs the others)");
+  int rc = trial_validate(b, trials, max_steps, fn.c_str());
+  if (rc) return rc;
+  if (!xhist || !uhist || !results) return fail(B200MPPI_EINVAL, fn + ": null output buffer");
+  int WW = 0, WH = 0;
+  if (stochastic && (rc = stochastic_validate(b, fn.c_str(), &WW, &WH))) return rc;
+  CU(cudaSetDevice(b->device));
+  const int K = (int)b->pl.size(), T = b->T, N = b->N, S = max_steps;
+  cudaStream_t st = b->stream;
+  // the sampler plans first (their host preparation may synchronise the stream): every pair must join the one launch
+  std::vector<SamplePlan> plans;
+  std::vector<SampleGridsV2Args> set0(K);
+  int mrows = 0, ncact = 0;
+  if (stochastic) {
+    if ((rc = stochastic_trial_plans(b, fn, plans, set0, &mrows, &ncact))) return rc;
+  } else {
+    std::vector<char> joined;
+    int nj = 0;
+    if ((rc = batch_plan_sample(b, set0.data(), plans, joined, &nj))) return rc;
+    for (int i = 0; i < K; ++i)
+      if (!joined[i])
+        return fail(B200MPPI_EINVAL, "run_trials: planner " + std::to_string(i) + ": its TDM pair cannot join the "
+                                     "batch's one sampler launch (map geometry, PMF or generator streams differ from "
+                                     "planner 0's)");
   }
   if ((rc = batch_wait_members(b))) return rc;
-  // device buffers of this call: [descriptors | sampler sets of parity 0, 1 | box descriptors | box records | trials |
-  // states | active K + count | grids | xhist | uhist]
-  const size_t off_s0 = b->desc_bytes;
-  const size_t off_s1 = off_s0 + align256((size_t)K * sizeof(SampleGridsV2Args));
+  const size_t nbox = stochastic ? (size_t)K : 0;      // stochastic-only sections
+  const size_t off_s0 = stochastic ? b->desc_bytes : b->off_sample;
+  const size_t off_s1 = b->desc_bytes + align256(nbox * sizeof(SampleGridsV2Args));
   const size_t off_box = off_s1 + align256((size_t)K * sizeof(SampleGridsV2Args));
-  const size_t off_rec = off_box + align256((size_t)K * sizeof(SampleBoxDesc));
-  const size_t off_tr = off_rec + align256((size_t)K * 5 * sizeof(int));
-  const size_t off_state = off_tr + align256((size_t)K * sizeof(TrialDev));
-  const size_t off_act = off_state + align256((size_t)K * sizeof(TrialState));
+  const size_t off_rec = off_box + align256(nbox * sizeof(SampleBoxDesc));
+  const size_t off_state = off_rec + align256(nbox * 5 * sizeof(int));
+  const size_t off_tr = off_state + align256((size_t)K * sizeof(TrialState));
+  const size_t off_act = off_tr + align256((size_t)K * sizeof(TrialDev));
   size_t off = off_act + align256((size_t)(K + 1) * sizeof(int));
+  const size_t head = off;
   std::vector<size_t> off_grid(K);
   for (int i = 0; i < K; ++i) {
     off_grid[i] = off;
@@ -2537,142 +2373,137 @@ extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b20
   }
   const size_t off_xh = off, off_uh = off_xh + align256((size_t)K * (S + 1) * 3 * sizeof(double));
   const size_t total = off_uh + align256((size_t)K * S * 2 * sizeof(float));
-  // pinned staging holds the head and the histories only: the ground-truth grids (float64, tens of MB for a batch of
-  // large maps) go to the device straight from the caller's arrays
-  const size_t head = off_grid.empty() ? off : off_grid[0];
-  const size_t h_xh = head, h_uh = head + (off_uh - off_xh);
-  unsigned char* d = nullptr;
-  unsigned char* h = nullptr;
-  CU(cudaMalloc(&d, total));
-  if (cudaMallocHost(&h, head + (total - off_xh)) != cudaSuccess) {
-    cudaFree(d);
-    return fail(B200MPPI_ECUDA, std::string(FN) + ": cudaMallocHost");
+  struct Buffers {                                     // freed on every return
+    unsigned char* d = nullptr;
+    unsigned char* h = nullptr;
+    cudaEvent_t ev[TRIAL_POLL] = {};
+    ~Buffers() {
+      cudaFree(d);
+      if (h) cudaFreeHost(h);
+      for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    }
+  } buf;
+  CU(cudaMalloc(&buf.d, total));
+  if (cudaMallocHost(&buf.h, head + (total - off_xh)) != cudaSuccess) {
+    buf.h = nullptr;
+    return fail(B200MPPI_ECUDA, fn + ": cudaMallocHost");
   }
-  struct Free {
-    unsigned char *d, *h;
-    ~Free() { cudaFree(d); cudaFreeHost(h); }
-  } guard{d, h};
+  unsigned char* d = buf.d;
+  unsigned char* h = buf.h;
   bool masks01 = true;
-  stochastic_descs(b, h, WW, WH, &masks01);
-  const RolloutWinArgs* hw = reinterpret_cast<const RolloutWinArgs*>(h + b->off_win);
-  CvarDesc* hc = reinterpret_cast<CvarDesc*>(h + b->off_cvar);
+  if (stochastic) stochastic_descs(b, h, WW, WH, &masks01);
+  else onemap_descs(b, h);
   SampleGridsV2Args* hs[2] = {reinterpret_cast<SampleGridsV2Args*>(h + off_s0),
                               reinterpret_cast<SampleGridsV2Args*>(h + off_s1)};
   SampleBoxDesc* hb = reinterpret_cast<SampleBoxDesc*>(h + off_box);
-  TrialDev* ht = reinterpret_cast<TrialDev*>(h + off_tr);
   TrialState* hst = reinterpret_cast<TrialState*>(h + off_state);
+  TrialDev* ht = reinterpret_cast<TrialDev*>(h + off_tr);
   int* hact = reinterpret_cast<int*>(h + off_act);
-  RolloutWinArgs* dw = reinterpret_cast<RolloutWinArgs*>(d + b->off_win);
   int* dact = reinterpret_cast<int*>(d + off_act);
-  int* drec = reinterpret_cast<int*>(d + off_rec);
+  // the rollout descriptors whose x0 the plant step writes: RolloutArgs (one-map), RolloutWinArgs (stochastic)
+  RolloutArgs* dr = reinterpret_cast<RolloutArgs*>(d + b->off_roll);
+  RolloutWinArgs* dw = reinterpret_cast<RolloutWinArgs*>(d + b->off_win);
   for (int i = 0; i < K; ++i) {
     b200mppi_planner* p = b->pl[i];
-    const b200mppi_tdm* l = p->lin;
-    hc[i].active = dact + i;
-    // the boxed launch's row segments over the whole-map plan; parity 1 samples from the buffers parity 0 wrote into
-    hs[0][i] = plans[i].a[0];
-    hs[0][i].segs = l->box_segs; hs[0][i].seg_rows = l->box_seg_rows; hs[0][i].jump = l->jump_box_d;
-    hs[0][i].write_states = 0;
-    hs[0][i].gm = gm_b;
-    hs[1][i] = hs[0][i];
+    // parity 1: the pair samples from the buffers parity 0 wrote into
+    hs[0][i] = hs[1][i] = set0[i];
     for (SampleTdm& td : hs[1][i].t) {
       uint64_t* in = td.states_out;
       td.states_out = const_cast<uint64_t*>(td.states);
       td.states = in;
     }
-    hb[i] = SampleBoxDesc{};
-    fill_reach_const(p, plans[i], &hb[i].c);
-    hb[i].x0 = dw[i].p.x0;
-    hb[i].reach = p->reach_d;
-    hb[i].slot = p->reach_slot ^ 1;
-    hb[i].record = drec + 5 * i;
-    hb[i].jump_tile = l->jump_tile_d;
     const b200mppi_trial_desc& q = trials[i];
-    const size_t cells = (size_t)q.height * q.width;
     const double* dg = reinterpret_cast<const double*>(d + off_grid[i]);
     TrialDev& t = ht[i];
     t = TrialDev{};
-    t.lin = dg; t.ang = dg + cells; t.H = q.height; t.W = q.width;
+    t.lin = dg; t.ang = dg + (size_t)q.height * q.width; t.H = q.height; t.W = q.width;
     t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res; t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1];
     t.tol = q.goal_tolerance;
     t.pxlim[0] = q.pxlim[0]; t.pxlim[1] = q.pxlim[1]; t.pylim[0] = q.pylim[0]; t.pylim[1] = q.pylim[1];
     t.u_cur = p->u_cur;
-    t.x0_out = dw[i].p.x0;
-    t.win = &dw[i].WW;
-    t.win_pxl = l->pxl[0]; t.win_pyl = l->pyl[0]; t.win_res = l->res; t.win_rows = l->rows; t.win_cols = l->cols;
     hst[i] = TrialState{};
     for (int c = 0; c < 3; ++c) hst[i].x[c] = q.x0[c];
     hact[i] = 1;
+    if (!stochastic) {
+      t.x0_out = dr[i].p.x0;                           // win stays null: one-map rollouts have no window
+      continue;
+    }
+    const b200mppi_tdm* l = p->lin;
+    t.x0_out = dw[i].p.x0;
+    t.win = &dw[i].WW;
+    t.win_pxl = l->pxl[0]; t.win_pyl = l->pyl[0]; t.win_res = l->res; t.win_rows = l->rows; t.win_cols = l->cols;
+    reinterpret_cast<CvarDesc*>(h + b->off_cvar)[i].active = dact + i;
+    hb[i] = SampleBoxDesc{{}, dw[i].p.x0, p->reach_d, p->reach_slot ^ 1, reinterpret_cast<int*>(d + off_rec) + 5 * i,
+                          l->jump_tile_d};
+    fill_reach_const(p, plans[i], &hb[i].c);
   }
   hact[K] = K;
+  const RolloutWinArgs g0 = stochastic ? *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win) : RolloutWinArgs{};
   CU(cudaMemcpyAsync(d, h, head, cudaMemcpyHostToDevice, st));
   for (int i = 0; i < K; ++i) {                       // pageable sources: staged by the driver before the call returns
     const size_t bytes = (size_t)trials[i].height * trials[i].width * sizeof(double);
     CU(cudaMemcpyAsync(d + off_grid[i], trials[i].lin, bytes, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(d + off_grid[i] + bytes, trials[i].ang, bytes, cudaMemcpyHostToDevice, st));
   }
-  const NoisePrepDesc* dn = reinterpret_cast<const NoisePrepDesc*>(d);
-  const void* dtm = d + b->off_tm;
-  const CvarDesc* dc = reinterpret_cast<const CvarDesc*>(d + b->off_cvar);
-  const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(d + b->off_upd);
   const SampleGridsV2Args* ds[2] = {reinterpret_cast<const SampleGridsV2Args*>(d + off_s0),
                                     reinterpret_cast<const SampleGridsV2Args*>(d + off_s1)};
   const SampleBoxDesc* db = reinterpret_cast<const SampleBoxDesc*>(d + off_box);
-  PlantArgs pa{};
-  pa.trials = reinterpret_cast<const TrialDev*>(d + off_tr);
-  pa.state = reinterpret_cast<TrialState*>(d + off_state);
-  pa.active = dact; pa.active_count = dact + K;
-  pa.xhist = reinterpret_cast<double*>(d + off_xh);
-  pa.uhist = reinterpret_cast<float*>(d + off_uh);
-  pa.K = K; pa.T = T; pa.max_steps = S;
-  const SampleGridsV2Args geom = hs[0][0];
-  const RolloutWinArgs g0 = hw[0];
+  const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(d + b->off_upd);
+  PlantArgs pa{reinterpret_cast<const TrialDev*>(d + off_tr), reinterpret_cast<TrialState*>(d + off_state), dact,
+               dact + K, reinterpret_cast<double*>(d + off_xh), reinterpret_cast<float*>(d + off_uh), K, T, S, 0};
   CU(cudaStreamSynchronize(st));                      // the staging is read by the upload above
   int* hcount = reinterpret_cast<int*>(h);             // the polled counts, in the no longer needed head of the staging
-  cudaEvent_t ev[TRIAL_POLL] = {};
-  struct Events {
-    cudaEvent_t* e;
-    ~Events() { for (int i = 0; i < TRIAL_POLL; ++i) if (e[i]) cudaEventDestroy(e[i]); }
-  } evguard{ev};
-  for (auto& e : ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  for (cudaEvent_t& e : buf.ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   const int num_opt = b->pl[0]->prm.num_opt, npad = b->pl[0]->npad;
+  const SampleGridsV2Args& geom = set0[0];
   int issued = 0;
   for (int s = 0; s < S; ++s) {
     if (s >= TRIAL_POLL) {                            // the count after step s - POLL
-      CU(cudaEventSynchronize(ev[s % TRIAL_POLL]));
+      CU(cudaEventSynchronize(buf.ev[s % TRIAL_POLL]));
       if (hcount[s % TRIAL_POLL] == 0) break;
     }
     for (int k = 0; k < num_opt; ++k) {
-      const int iter = s * num_opt + k;               // every planner's reach slot toggles once per iteration
-      launch_noise_prepare_batch(dn, K, N, T, npad, iter, dact, st);
-      CHECK_LAUNCH();
-      if (k == 0) {
-        launch_sample_grids_v2_box_batch(geom, ds[s & 1], db, K, dact, iter, mrows, ncact, st);
+      if (stochastic) {
+        const int iter = s * num_opt + k;             // every planner's reach slot toggles once per iteration
+        launch_noise_prepare_batch(reinterpret_cast<const NoisePrepDesc*>(d), K, N, T, npad, iter, dact, st);
         CHECK_LAUNCH();
-        launch_advance_states_batch(ds[s & 1], db, K, geom.rows, geom.cols, geom.tx, geom.ty, geom.num_maps, dact, st);
+        if (k == 0) {
+          launch_sample_grids_v2_box_batch(geom, ds[s & 1], db, K, dact, iter, mrows, ncact, st);
+          CHECK_LAUNCH();
+          launch_advance_states_batch(ds[s & 1], db, K, geom.rows, geom.cols, geom.tx, geom.ty, geom.num_maps, dact, st);
+          CHECK_LAUNCH();
+        }
+        CU(launch_rollout_win_batch(g0, dw, d + b->off_tm, K, masks01, dact, st));
+        launch_cvar_batch(reinterpret_cast<const CvarDesc*>(d + b->off_cvar), K, N, b->M, st);
+        CHECK_LAUNCH();
+      } else {
+        launch_sample_noise_batch(reinterpret_cast<const NoiseDesc*>(d), K, N, T, dact, st);
+        CHECK_LAUNCH();
+        if (k == 0) {
+          launch_sample_grids_v2_batch(geom, ds[s & 1], K, dact, st);
+          CHECK_LAUNCH();
+        }
+        launch_rollout_batch(dr, K, b->mode, N, T, dact, st);
         CHECK_LAUNCH();
       }
-      CU(launch_rollout_win_batch(g0, dw, dtm, K, masks01, dact, st));
-      launch_cvar_batch(dc, K, N, b->M, st);
-      CHECK_LAUNCH();
       launch_update_partial_batch(du, K, b->pl[0]->num_ctas, dact, st);
       CHECK_LAUNCH();
     }
     pa.step = s;
     launch_plant_step(pa, st);
     CHECK_LAUNCH();
-    b->launches += 4 * num_opt + 3;
+    b->launches += stochastic ? 4 * num_opt + 3 : 3 * num_opt + 2;
     ++issued;
     CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, dact + K, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(ev[s % TRIAL_POLL], st));
+    CU(cudaEventRecord(buf.ev[s % TRIAL_POLL], st));
   }
+  // the box records (stochastic) and the states, then the histories
   CU(cudaMemcpyAsync(h + off_rec, d + off_rec, off_tr - off_rec, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(h + off_state, d + off_state, off_act - off_state, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(h + h_xh, d + off_xh, total - off_xh, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(h + head, d + off_xh, total - off_xh, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   const int* hrec = reinterpret_cast<const int*>(h + off_rec);
-  const double* hx = reinterpret_cast<const double*>(h + h_xh);
-  const float* hu_h = reinterpret_cast<const float*>(h + h_uh);
+  const double* hx = reinterpret_cast<const double*>(h + head);
+  const float* hu = reinterpret_cast<const float*>(h + head + (off_uh - off_xh));
   const double dnan = std::nan("");
   const float fnan = std::nanf("");
   for (int i = 0; i < K; ++i) {
@@ -2683,22 +2514,38 @@ extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b20
     for (int c = 0; c < 3; ++c) xo[c] = trials[i].x0[c];
     std::memcpy(xo + 3, hx + ((size_t)i * (S + 1) + 1) * 3, (size_t)n * 3 * sizeof(double));
     for (size_t j = (size_t)(n + 1) * 3; j < (size_t)(S + 1) * 3; ++j) xo[j] = dnan;
-    std::memcpy(uo, hu_h + (size_t)i * S * 2, (size_t)n * 2 * sizeof(float));
+    std::memcpy(uo, hu + (size_t)i * S * 2, (size_t)n * 2 * sizeof(float));
     for (size_t j = (size_t)n * 2; j < (size_t)S * 2; ++j) uo[j] = fnan;
     results[i] = b200mppi_trial_result{r.cum_obj, r.cum_dist, r.dist, n, r.status};
-    // host state as after n rounds of the host loop: n boxed or whole-map samplings of the pair (the last one's kind
-    // in grid_partial), the reach slot toggled once per iteration, the last solve's box and x0
+    // host state as after n rounds of the host loop: n samplings of the pair (stochastic: boxed or whole-map, the last
+    // one's kind in grid_partial), the reach slot toggled once per iteration, the last solve's box and x0
     b200mppi_planner* p = b->pl[i];
     const int* rec = hrec + 5 * i;
-    plans[i].boxed[0] = plans[i].boxed[1] = rec[0] != 0;
+    if (stochastic) plans[i].boxed[0] = plans[i].boxed[1] = rec[0] != 0;
     for (int s = 0; s < n; ++s) { plan_commit(plans[i], 0); plan_commit(plans[i], 1); }
-    p->reach_slot ^= (n * num_opt) & 1;
-    p->reach_valid = true;
+    if (stochastic) {
+      p->reach_slot ^= (n * num_opt) & 1;
+      p->reach_valid = true;
+      for (int c = 0; c < 5; ++c) p->last_box[c] = rec[c];
+    } else {
+      last_box_whole_map(p);
+    }
     p->prepared = false;
     p->pushed_direct = false;
-    for (int c = 0; c < 5; ++c) p->last_box[c] = rec[c];
     for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)xo[(size_t)(n - 1) * 3 + c];
   }
   if (steps_issued) *steps_issued = issued;
   return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps,
+                                         double* xhist, float* uhist, b200mppi_trial_result* results,
+                                         int32_t* steps_issued) {
+  return batch_run_trials(b, false, trials, max_steps, xhist, uhist, results, steps_issued);
+}
+
+extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials,
+                                                    int32_t max_steps, double* xhist, float* uhist,
+                                                    b200mppi_trial_result* results, int32_t* steps_issued) {
+  return batch_run_trials(b, true, trials, max_steps, xhist, uhist, results, steps_issued);
 }
