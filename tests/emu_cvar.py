@@ -1,88 +1,15 @@
-"""Host emulation of the CVaR kernels (TEST INFRASTRUCTURE), same technique as tests/emu_sampler.py: the kernels'
-text (csrc/rollout.cu between the ``[emu:... cvar]`` markers, ``warp_sum`` from csrc/common.cuh) is compiled with
-g++; one std::thread per CUDA thread, ``__syncthreads()`` = a barrier over the block, the warp collectives
-(``__reduce_add_sync``, ``__shfl_xor_sync``) = exchanges through a per-warp buffer between two warp barriers."""
-import ctypes as C
-import os
-import re
-import subprocess
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "mppi_numba_b200", "csrc")
-
-PRELUDE = r'''
-#include <algorithm>
-#include <barrier>
-#include <cmath>
-#include <cstdint>
-#include <cstring>
-#include <memory>
-#include <thread>
-#include <vector>
-struct EmuDim3 { unsigned x, y, z; };
-static thread_local EmuDim3 threadIdx, blockIdx, blockDim, gridDim;
-static std::barrier<>* g_bar = nullptr;
-struct EmuWarp { std::barrier<> bar{32}; int ibuf[32]; float fbuf[32]; };
-static thread_local EmuWarp* g_warp = nullptr;
-#define __global__
-#define __device__
-#define __host__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(...)
-#define __shared__
-static inline void __syncthreads() { g_bar->arrive_and_wait(); }
-static inline int __reduce_add_sync(unsigned, int v) {
-  const int lane = threadIdx.x & 31;
-  g_warp->ibuf[lane] = v;
-  g_warp->bar.arrive_and_wait();
-  int s = 0;
-  for (int i = 0; i < 32; ++i) s += g_warp->ibuf[i];
-  g_warp->bar.arrive_and_wait();
-  return s;
-}
-static inline float __shfl_xor_sync(unsigned, float v, int o) {
-  const int lane = threadIdx.x & 31;
-  g_warp->fbuf[lane] = v;
-  g_warp->bar.arrive_and_wait();
-  const float r = g_warp->fbuf[lane ^ o];
-  g_warp->bar.arrive_and_wait();
-  return r;
-}
-static inline uint32_t __float_as_uint(float f) { uint32_t u; std::memcpy(&u, &f, 4); return u; }
-static inline float __uint_as_float(uint32_t u) { float f; std::memcpy(&f, &u, 4); return f; }
-namespace b200 {
-uint32_t s_keys[1 << 15];
-template <class T> static inline T __ldcg(const T* p) { return *p; }
-static inline int __clz(int v) { return v ? __builtin_clz((unsigned)v) : 32; }
-struct FlagWait { const uint32_t* flags; int ws; uint32_t epoch; unsigned long long timeout_ns; int* status; };
-static inline void flag_wait(const FlagWait&) {}
-'''
+"""Host emulation of the CVaR kernels (TEST INFRASTRUCTURE; tests/emu_core.py): the kernels' text (csrc/rollout.cu
+between the ``[emu:... cvar]`` markers, ``warp_sum`` from csrc/common.cuh) is compiled with g++; one std::thread per
+CUDA thread, ``__syncthreads()`` = a barrier over the block, the warp collectives (``__reduce_add_sync``,
+``__shfl_xor_sync``) = exchanges through a per-warp buffer between two warp barriers."""
+from tests.emu_core import build as _build
+from tests.emu_core import extern_shared, region, shared_static
 
 HARNESS = r'''
-template <class K>
-static void run(K kernel, int threads, unsigned blocks) {
-  for (unsigned bx = 0; bx < blocks; ++bx) {
-    std::barrier<> bar(threads);
-    g_bar = &bar;
-    std::vector<std::unique_ptr<EmuWarp>> warps;
-    for (int w = 0; w < threads / 32; ++w) warps.emplace_back(new EmuWarp());
-    std::vector<std::thread> th;
-    for (int t = 0; t < threads; ++t)
-      th.emplace_back([&, t] {
-        threadIdx = {(unsigned)t, 0, 0}; blockIdx = {bx, 0, 0}; blockDim = {(unsigned)threads, 1, 1}; gridDim = {blocks, 1, 1};
-        g_warp = warps[t / 32].get();
-        kernel();
-      });
-    for (auto& x : th) x.join();
-  }
-}
-}  // namespace b200
-
+using namespace b200;
 // as launch_cvar (csrc/rollout.cu): which kernel, which PER, which grid.  costs_nm: the logical (N, M) array; the
 // kernels get the map-major (M, ld) device layout, ld >= N (a row stride larger than the row exercises `ld`).
 extern "C" int emu_cvar(const float* costs_nm, float* costs, int N, int M, int ld, float cvar_alpha) {
-  using namespace b200;
   if (ld < N) return 2;
   std::vector<float> mn((size_t)M * ld, 12345.0f);
   for (int n = 0; n < N; ++n)
@@ -92,42 +19,25 @@ extern "C" int emu_cvar(const float* costs_nm, float* costs, int N, int M, int l
   if (numel > M) numel = M;
   if (M > 32 * CVAR_MAX_PER_LANE) {
     if (M > (1 << 15)) return 1;
-    run([&] { cvar_large_kernel(mn.data(), costs, N, ld, M, numel, FlagWait{}); }, CVAR_LARGE_THREADS, (unsigned)N);
+    emu::launch({(unsigned)N, 1, 1}, CVAR_LARGE_THREADS, [&] { cvar_large_kernel(mn.data(), costs, N, ld, M, numel, FlagWait{}); });
     return 0;
   }
   const int nb = cvar_block_n(M);
   const unsigned blocks = (unsigned)((N + nb - 1) / nb);
-  const int per = (M + 31) / 32;
-  if (per <= 1) run([&] { cvar_kernel<1>(mn.data(), costs, N, ld, M, numel, FlagWait{}); }, CVAR_THREADS, blocks);
-  else if (per <= 2) run([&] { cvar_kernel<2>(mn.data(), costs, N, ld, M, numel, FlagWait{}); }, CVAR_THREADS, blocks);
-  else if (per <= 4) run([&] { cvar_kernel<4>(mn.data(), costs, N, ld, M, numel, FlagWait{}); }, CVAR_THREADS, blocks);
-  else if (per <= 8) run([&] { cvar_kernel<8>(mn.data(), costs, N, ld, M, numel, FlagWait{}); }, CVAR_THREADS, blocks);
-  else if (per <= 16) run([&] { cvar_kernel<16>(mn.data(), costs, N, ld, M, numel, FlagWait{}); }, CVAR_THREADS, blocks);
-  else run([&] { cvar_kernel<32>(mn.data(), costs, N, ld, M, numel, FlagWait{}); }, CVAR_THREADS, blocks);
+  emu::cvar_per(M, [&](auto P) {
+    emu::launch({blocks, 1, 1}, CVAR_THREADS, [&] { cvar_kernel<decltype(P)::value>(mn.data(), costs, N, ld, M, numel, FlagWait{}); });
+  });
   return 0;
 }
 '''
 
 
-def _region(path, name):
-    text = open(path).read()
-    m = re.search(r"// \[emu:begin %s\][^\n]*\n(.*?)// \[emu:end %s\]" % (name, name), text, re.S)
-    assert m, "marker %s not found in %s" % (name, path)
-    return m.group(1)
+def kernels(*more):
+    """The CVaR kernels' text (``cvar`` region, then the named regions of csrc/rollout.cu) with warp_sum and the
+    descriptor of the batched kernels."""
+    return [region("kernels.h", "cvar_desc"), region("common.cuh", "warp_sum"),
+            extern_shared(shared_static("".join(region("rollout.cu", r) for r in ("cvar",) + more), 3), 1)]
 
 
-def build(out_dir):
-    kernels = _region(os.path.join(CSRC, "rollout.cu"), "cvar")
-    # block-shared arrays declared inside a kernel: one instance for all threads of the (only running) block
-    kernels = re.sub(r"(?m)^(\s*)__shared__ ", r"\1static ", kernels)
-    src = PRELUDE + _region(os.path.join(CSRC, "common.cuh"), "warp_sum") + kernels + HARNESS
-    cpp = os.path.join(out_dir, "cvar_emu.cpp")
-    so = os.path.join(out_dir, "libcvar_emu.so")
-    open(cpp, "w").write(src)
-    r = subprocess.run(["g++", "-O1", "-std=c++20", "-pthread", "-shared", "-fPIC", "-Wno-unknown-pragmas", cpp, "-o", so],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    lib = C.CDLL(so)
-    lib.emu_cvar.restype = C.c_int
-    lib.emu_cvar.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float]
-    return lib
+def build(out_dir, extra=""):
+    return _build(out_dir, "cvar_emu", kernels(), HARNESS + extra)

@@ -1,54 +1,19 @@
-"""Host emulation of sample_noise_kernel (TEST INFRASTRUCTURE; technique of tests/emu_sampler.py): the kernel's text
-(csrc/reduce.cu, ``[emu:... noise]``) and the xoroshiro128+ step (csrc/common.cuh) compiled with g++.  logf / cosf
-are libm's (the GPU uses libdevice's, both within an ulp or two), sqrt.approx becomes sqrtf."""
-import ctypes as C
-import os
-import subprocess
-
-from tests.emu_rollout import _region
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "mppi_numba_b200", "csrc")
-
-PRELUDE = r'''
-#include <cmath>
-#include <cstdint>
-struct EmuDim3 { unsigned x, y, z; };
-static EmuDim3 threadIdx, blockIdx, blockDim;          // the kernel has no barriers: threads run one after the other
-#define __global__
-#define __device__
-#define __forceinline__ inline
-#define __restrict__
-#define __launch_bounds__(...)
-struct float2 { float x, y; };
-struct ulonglong2 { unsigned long long x, y; };
-static inline ulonglong2 make_ulonglong2(unsigned long long x, unsigned long long y) { return ulonglong2{x, y}; }
-namespace b200 {
-static inline float fmul(float a, float b) { return a * b; }
-static inline float sqrt_approx(float x) { return sqrtf(x); }
-static inline float xoro_unit_f32(uint64_t x) { return (float)((double)(x >> 11) * (1.0 / 9007199254740992.0)); }
-'''
+"""Host emulation of sample_noise_kernel (TEST INFRASTRUCTURE; tests/emu_core.py): the kernel's text (csrc/reduce.cu,
+``[emu:... noise]``) and the xoroshiro128+ step (csrc/common.cuh) compiled with g++.  logf / cosf are libm's (the GPU
+uses libdevice's, both within an ulp or two), sqrt.approx becomes sqrtf.  The kernel has no barriers: its threads run
+one after the other."""
+from tests.emu_core import build as _build
+from tests.emu_core import region
 
 HARNESS = r'''
-}  // namespace b200
 extern "C" void emu_sample_noise(uint64_t* states, float* noise, long long count, float std_v, float std_w, float* reach) {
-  blockDim = {256, 1, 1};
-  for (long long g = 0; g < (count + 255) / 256 * 256; ++g) {
-    blockIdx = {(unsigned)(g / 256), 0, 0}; threadIdx = {(unsigned)(g % 256), 0, 0};
+  emu::launch_serial({(unsigned)((count + 255) / 256), 1, 1}, 256, [&] {
     b200::sample_noise_kernel(states, reinterpret_cast<float2*>(noise), count, std_v, std_w, reach);
-  }
+  });
 }
 '''
 
 
-def build(out_dir):
-    src = PRELUDE + _region(os.path.join(CSRC, "common.cuh"), "xoro") + _region(os.path.join(CSRC, "common.cuh"), "normal") + _region(os.path.join(CSRC, "reduce.cu"), "noise") + HARNESS
-    cpp, so = os.path.join(out_dir, "noise_emu.cpp"), os.path.join(out_dir, "libnoise_emu.so")
-    open(cpp, "w").write(src)
-    r = subprocess.run(["g++", "-O1", "-std=c++17", "-shared", "-fPIC", "-ffp-contract=off", cpp, "-o", so],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    lib = C.CDLL(so)
-    lib.emu_sample_noise.restype = None
-    lib.emu_sample_noise.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_float, C.c_float, C.c_void_p]
-    return lib
+def build(out_dir, extra=""):
+    parts = [region("common.cuh", "xoro"), region("common.cuh", "normal"), region("reduce.cu", "noise")]
+    return _build(out_dir, "noise_emu", parts, HARNESS + extra)

@@ -1,99 +1,21 @@
-"""Host emulation of the generic rollout kernels and the visualisation kernel (TEST INFRASTRUCTURE; technique of
-tests/emu_sampler.py).  The kernels' text (csrc/rollout.cu between the ``[emu:... rollout]`` / ``[emu:... vis]``
-markers, cell_index* and the parameter structs from csrc/common.cuh / kernels.h) is compiled with g++.  The
-inline-PTX arithmetic helpers of common.cuh are replaced by their IEEE meaning (add / sub / mul / fma rounded to
-nearest, floor, float<->double conversions); the three MUFU approximations (sin, cos, sqrt) and the approximate
-divisions by libm's correctly rounded ones -- which is what the oracle and the reference's simulator goldens use,
-so the comparison tolerance is a few ulp, tighter than on the GPU."""
-import ctypes as C
-import os
-import re
-import subprocess
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "mppi_numba_b200", "csrc")
-
-PRELUDE = r'''
-#include <algorithm>
-#include <barrier>
-#include <cmath>
-#include <cstdint>
-#include <cstring>
-#include <thread>
-#include <vector>
-struct EmuDim3 { unsigned x, y, z; };
-static thread_local EmuDim3 threadIdx, blockIdx, blockDim, gridDim;
-static std::barrier<>* g_bar = nullptr;
-#define __global__
-#define __device__
-#define __host__
-#define __forceinline__ inline
-#define __noinline__
-#define __restrict__
-#define __launch_bounds__(...)
-#define __shared__
-static inline void __syncthreads() { g_bar->arrive_and_wait(); }
-template <class T> static inline T __ldg(const T* p) { return *p; }
-struct float2 { float x, y; };
-using std::min;
-using std::max;
-namespace b200 {
-float s_u[4096];
-static inline float sin_approx(float x) { return sinf(x); }
-static inline float cos_approx(float x) { return cosf(x); }
-static inline float sqrt_approx(float x) { return sqrtf(x); }
-static inline float div_approx(float a, float b) { return a / b; }
-static inline float div_full(float a, float b) { return a / b; }
-static inline float div_rn(float a, float b) { return a / b; }
-static inline float fadd(float a, float b) { return a + b; }
-static inline float fsub(float a, float b) { return a - b; }
-static inline float fmul(float a, float b) { return a * b; }
-static inline float ffma(float a, float b, float c) { return fmaf(a, b, c); }
-static inline float ffloor(float a) { return floorf(a); }
-static inline double f2d(float a) { return (double)a; }
-static inline float d2f(double a) { return (float)a; }
-'''
+"""Host emulation of the generic rollout kernels and the visualisation kernel (TEST INFRASTRUCTURE; tests/emu_core.py).
+The kernels' text (csrc/rollout.cu between the ``[emu:... rollout]`` / ``[emu:... vis]`` markers, cell_index* and the
+parameter structs from csrc/common.cuh / kernels.h) is compiled with g++.  The arithmetic helpers of common.cuh have
+their IEEE meaning and the MUFU approximations and approximate divisions are libm's correctly rounded ones
+(tests/emu_cuda.h) -- which is what the oracle and the reference's simulator goldens use, so the comparison tolerance
+is a few ulp, tighter than on the GPU."""
+from tests.emu_core import build as _build
+from tests.emu_core import cell_index_rzi, extern_shared, region
 
 HARNESS = r'''
-template <class K>
-static void run(K kernel, int threads, unsigned gx, unsigned gy) {
-  for (unsigned by = 0; by < gy; ++by)
-    for (unsigned bx = 0; bx < gx; ++bx) {
-      std::barrier<> bar(threads);
-      g_bar = &bar;
-      std::vector<std::thread> th;
-      for (int t = 0; t < threads; ++t)
-        th.emplace_back([&, t] {
-          threadIdx = {(unsigned)t, 0, 0}; blockIdx = {bx, by, 0}; blockDim = {(unsigned)threads, 1, 1}; gridDim = {gx, gy, 1};
-          kernel();
-        });
-      for (auto& x : th) x.join();
-    }
-}
-static RolloutParams params(const float* f, const int* g, const double* ratios) {
-  // f: res, xlo, ylo, dt, x0[3], xgoal[2], goal_tol, v_post, lambda, u_std[2], vrange[2], wrange[2], obs, unk, dist_w,
-  //    lin_lo, ang_lo (23 floats);  g: rows, cols, grid_rows, grid_cols, grid_pitch, mask_pitch, T, N, M
-  RolloutParams p{};
-  p.g.res = f[0]; p.g.inv_res = 1.0f / f[0]; p.g.xlo = f[1]; p.g.ylo = f[2];
-  p.g.rows = g[0]; p.g.cols = g[1]; p.g.grid_rows = g[2]; p.g.grid_cols = g[3]; p.g.grid_pitch = g[4]; p.g.mask_pitch = g[5];
-  p.dt = f[3]; p.x0[0] = f[4]; p.x0[1] = f[5]; p.x0[2] = f[6]; p.xgoal[0] = f[7]; p.xgoal[1] = f[8];
-  p.tol2 = f[9] * f[9]; p.v_post = f[10]; p.lambda = f[11]; p.u_std[0] = f[12]; p.u_std[1] = f[13];
-  p.vrange[0] = f[14]; p.vrange[1] = f[15]; p.wrange[0] = f[16]; p.wrange[1] = f[17];
-  p.obs_cost = f[18]; p.unk_cost = f[19]; p.dist_weight = f[20]; p.lin_lo = f[21]; p.ang_lo = f[22];
-  p.lin_ratio = ratios[0]; p.ang_ratio = ratios[1];
-  p.T = g[6]; p.N = g[7]; p.M = g[8];
-  return p;
-}
-}  // namespace b200
-
+using namespace b200;
 // as launch_rollout (csrc/rollout.cu): mode 0 / 1 / 2 generic kernels, mode 3 the barebone kernel
 extern "C" void emu_rollout(int mode, const float* f, const int* g, const double* ratios, const int8_t* lin,
                             const int8_t* ang, const int8_t* obs, const int8_t* unk, const int8_t* risk,
                             const float* noise, const float* u_cur, float* costs_nm, float* costs,
                             const float* obstacles, int num_obstacles) {
-  using namespace b200;
   RolloutArgs a{};
-  a.p = params(f, g, ratios);
+  emu::params(a.p, f, g, ratios, g[8]);
   a.mode = mode; a.lin_grid = lin; a.ang_grid = ang; a.obstacle = obs; a.unknown = unk; a.risk = risk;
   a.noise = noise; a.u_cur = u_cur; a.costs = costs; a.obstacles = obstacles;
   a.num_obstacles = num_obstacles;
@@ -101,10 +23,10 @@ extern "C" void emu_rollout(int mode, const float* f, const int* g, const double
   a.dst.base[0] = mn.data(); a.dst.n_per = std::max(a.p.N, 1); a.dst.ld = a.p.N; a.dst.row0 = 0;
   const int threads = 128;
   const unsigned gx = (unsigned)((a.p.N + threads - 1) / threads);
-  if (mode == 3) run([&] { rollout_barebone_kernel(a); }, threads, gx, 1);
-  else if (mode == 0) run([&] { rollout_kernel<0>(a); }, threads, gx, (unsigned)a.p.M);
-  else if (mode == 1) run([&] { rollout_kernel<1>(a); }, threads, gx, 1);
-  else run([&] { rollout_kernel<2>(a); }, threads, gx, 1);
+  if (mode == 3) emu::launch({gx, 1, 1}, threads, [&] { rollout_barebone_kernel(a); });
+  else if (mode == 0) emu::launch({gx, (unsigned)a.p.M, 1}, threads, [&] { rollout_kernel<0>(a); });
+  else if (mode == 1) emu::launch({gx, 1, 1}, threads, [&] { rollout_kernel<1>(a); });
+  else emu::launch({gx, 1, 1}, threads, [&] { rollout_kernel<2>(a); });
   if (mode == 0 && costs_nm)                                      // hand back the logical (N, M) array
     for (int n = 0; n < a.p.N; ++n)
       for (int m = 0; m < a.p.M; ++m) costs_nm[(size_t)n * a.p.M + m] = mn[(size_t)m * a.p.N + n];
@@ -113,42 +35,17 @@ extern "C" void emu_rollout(int mode, const float* f, const int* g, const double
 extern "C" void emu_state_rollout(int mode, int V, const float* f, const int* g, const double* ratios, const int8_t* lin,
                                   const int8_t* ang, const float* noise, const float* u_cur, const float* u_prev,
                                   float* out) {
-  using namespace b200;
   VisArgs a{};
-  a.p = params(f, g, ratios);
+  emu::params(a.p, f, g, ratios, g[8]);
   a.mode = mode; a.V = V; a.lin_grid = lin; a.ang_grid = ang; a.noise = noise; a.u_cur = u_cur; a.u_prev = u_prev;
   a.out = out;
-  run([&] { state_rollout_kernel(a); }, 32, (unsigned)((V + 31) / 32), 1);
+  emu::launch({(unsigned)((V + 31) / 32), 1, 1}, 32, [&] { state_rollout_kernel(a); });
 }
 '''
 
 
-def _region(path, name):
-    text = open(path).read()
-    m = re.search(r"// \[emu:begin %s\][^\n]*\n(.*?)// \[emu:end %s\]" % (name, name), text, re.S)
-    assert m, "marker %s not found in %s" % (name, path)
-    return m.group(1)
-
-
-def build(out_dir):
-    cell = _region(os.path.join(CSRC, "common.cuh"), "cell_index")
-    cell, n = re.subn(r'int k; asm\("cvt\.rzi\.ftz\.s32\.f32[^;]*;[^;]*;', "int k = (int)res;   /* cvt.rzi */", cell)
-    assert n == 1, "cvt.rzi line of cell_index_exact not found"
-    kernels = _region(os.path.join(CSRC, "rollout.cu"), "rollout") + _region(os.path.join(CSRC, "rollout.cu"), "vis")
-    kernels = kernels.replace("extern __shared__ float s_u[];", "")          # the namespace-level s_u of the prelude
-    src = (PRELUDE + _region(os.path.join(CSRC, "common.cuh"), "params") + cell +
-           _region(os.path.join(CSRC, "kernels.h"), "cost_dst") + _region(os.path.join(CSRC, "kernels.h"), "rollout_args") + _region(os.path.join(CSRC, "kernels.h"), "vis_args") +
-           kernels + HARNESS)
-    cpp = os.path.join(out_dir, "rollout_emu.cpp")
-    so = os.path.join(out_dir, "librollout_emu.so")
-    open(cpp, "w").write(src)
-    r = subprocess.run(["g++", "-O1", "-std=c++20", "-pthread", "-shared", "-fPIC", "-Wno-unknown-pragmas",
-                        "-ffp-contract=off", cpp, "-o", so], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    lib = C.CDLL(so)
-    P, I = C.c_void_p, C.c_int
-    lib.emu_rollout.restype = None
-    lib.emu_rollout.argtypes = [I, P, P, P, P, P, P, P, P, P, P, P, P, P, I]
-    lib.emu_state_rollout.restype = None
-    lib.emu_state_rollout.argtypes = [I, I, P, P, P, P, P, P, P, P, P]
-    return lib
+def build(out_dir, extra=""):
+    parts = [region("common.cuh", "params"), cell_index_rzi(region("common.cuh", "cell_index")),
+             region("kernels.h", "cost_dst"), region("kernels.h", "rollout_args"), region("kernels.h", "vis_args"),
+             extern_shared(region("rollout.cu", "rollout"), 2), region("rollout.cu", "vis")]
+    return _build(out_dir, "rollout_emu", parts, HARNESS + extra)

@@ -1,65 +1,25 @@
-"""Host emulation of the setter kernels (TEST INFRASTRUCTURE; technique of tests/emu_sampler.py): build_cum_kernel
-(the cumulative table the sampler reads) and collapse_pad_kernel (CVaR / mean collapse + crop + padding of the
-one-map modes), text lifted from csrc/sample.cu.  No barriers in these kernels: threads run one after the other;
-the explicitly rounded float64 intrinsics (__dmul_rn ...) are plain IEEE operations."""
-import ctypes as C
-import os
-import subprocess
-
-from tests.emu_rollout import _region
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "mppi_numba_b200", "csrc")
-
-PRELUDE = r'''
-#include <algorithm>
-#include <cstddef>
-#include <cstdint>
-struct EmuDim3 { unsigned x, y, z; };
-static EmuDim3 threadIdx, blockIdx, blockDim;
-#define __global__
-#define __restrict__
-static inline double __dmul_rn(double a, double b) { return a * b; }
-static inline double __dadd_rn(double a, double b) { return a + b; }
-static inline double __ddiv_rn(double a, double b) { return a / b; }
-static inline int atomicAdd(int* p, int v) { const int o = *p; *p += v; return o; }
-using std::min;
-using std::max;
-namespace b200 {
-'''
+"""Host emulation of the setter kernels (TEST INFRASTRUCTURE; tests/emu_core.py): build_cum_kernel (the cumulative
+table the sampler reads) and collapse_pad_kernel (CVaR / mean collapse + crop + padding of the one-map modes), text
+lifted from csrc/sample.cu.  No barriers in these kernels: threads run one after the other."""
+from tests.emu_core import build as _build
+from tests.emu_core import region
 
 HARNESS = r'''
-template <class K> static void run(K k, long long threads_total) {
-  blockDim = {256, 1, 1};
-  for (long long g = 0; g < (threads_total + 255) / 256 * 256; ++g) {
-    blockIdx = {(unsigned)(g / 256), 0, 0}; threadIdx = {(unsigned)(g % 256), 0, 0};
-    k();
-  }
-}
-}  // namespace b200
+static EmuDim3 blocks_for(long long threads_total) { return {(unsigned)((threads_total + 255) / 256), 1, 1}; }
 extern "C" void emu_build_cum(const int8_t* pmf, int8_t* cum, int B, int bpad, int rows, int cols) {
-  b200::run([&] { b200::build_cum_kernel(pmf, cum, B, bpad, rows, cols); }, (long long)rows * cols);
+  emu::launch_serial(blocks_for((long long)rows * cols), 256, [&] { b200::build_cum_kernel(pmf, cum, B, bpad, rows, cols); });
 }
 extern "C" void emu_collapse_pad(const int8_t* raw, int8_t* out, int8_t* risk, int* bad, const float* bin_values, int B,
                                  int H, int W, int keep_r, int keep_c, int pad, int risk_pitch, double alpha, float lo,
                                  float range, int mode) {
-  b200::run([&] { b200::collapse_pad_kernel(raw, out, risk, bad, bin_values, B, H, W, keep_r, keep_c, pad, risk_pitch, alpha,
-                                            lo, range, mode); }, (long long)(keep_r + 2 * pad) * (keep_c + 2 * pad));
+  emu::launch_serial(blocks_for((long long)(keep_r + 2 * pad) * (keep_c + 2 * pad)), 256, [&] {
+    b200::collapse_pad_kernel(raw, out, risk, bad, bin_values, B, H, W, keep_r, keep_c, pad, risk_pitch, alpha, lo, range,
+                              mode);
+  });
 }
 '''
 
 
-def build(out_dir):
-    src = PRELUDE + _region(os.path.join(CSRC, "sample.cu"), "build_cum") + _region(os.path.join(CSRC, "sample.cu"), "collapse_pad") + HARNESS
-    cpp, so = os.path.join(out_dir, "setter_emu.cpp"), os.path.join(out_dir, "libsetter_emu.so")
-    open(cpp, "w").write(src)
-    r = subprocess.run(["g++", "-O1", "-std=c++17", "-shared", "-fPIC", "-ffp-contract=off", cpp, "-o", so],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    lib = C.CDLL(so)
-    P, I = C.c_void_p, C.c_int
-    lib.emu_build_cum.restype = None
-    lib.emu_build_cum.argtypes = [P, P, I, I, I, I]
-    lib.emu_collapse_pad.restype = None
-    lib.emu_collapse_pad.argtypes = [P, P, P, P, P, I, I, I, I, I, I, I, C.c_double, C.c_float, C.c_float, I]
-    return lib
+def build(out_dir, extra=""):
+    return _build(out_dir, "setter_emu", [region("sample.cu", "build_cum"), region("sample.cu", "collapse_pad")],
+                  HARNESS + extra)

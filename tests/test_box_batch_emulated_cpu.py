@@ -5,22 +5,17 @@ every generator state bit for bit, the decision record, boxes at different posit
 fallbacks (map edge, reach beyond the speed limit, box off), ragged last tile rows and columns, the group loop of a box
 larger than the launch, and a gated pair left untouched byte for byte."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from oracle import terrain_ref as TR
 from oracle import xoroshiro as X
-from tests.emu_sampler import CSRC, PRELUDE, ROOT, _region, build, cumulative_table
+from tests import emu_core, emu_sampler
+from tests.emu_sampler import cumulative_table, kernels
 from tests.scenarios import random_pmf
 
 HARNESS = r'''
-bool build_sample_thresholds(double alpha, int q_cap, uint64_t* table);
-void sample_tile_draws(int rows, int cols, int tx, int ty, int64_t ks[4]);
-}  // namespace b200
-
 // K fused pairs of one geometry (shared cum / qvals / thresholds; own maps, states, x0 and reach): ONE batched boxed
 // launch (iteration 0: reach slot `slot`) and ONE batched advance, as run_stochastic_trials issues them.
 // grid0 / grid1: K x (M, grid_rows, pitch); states: K x (ngen, 2) in; out0 / out1: K x (ngen, 2) out; rec: K x 5.
@@ -29,22 +24,11 @@ extern "C" int emu_box_batch(int K, int8_t* grid0, int8_t* grid1, const int8_t* 
                              int bpad, int rows, int cols, int grid_rows, int pitch, int tx, int ty, int M, int segs,
                              double alpha, int q_cap, const int* ci, const float* cf, const float* x0, const float* reach,
                              const int* active, int mrows, int ncact, int gm, int* rec) {
-  using namespace b200;
   std::vector<uint64_t> T(SAMPLE_TABLE_WORDS);
   if (!build_sample_thresholds(alpha, q_cap, T.data())) return 1;
-  const int nrow = (rows + tx - 1) / tx, ncol = (cols + ty - 1) / ty;
-  if (segs > nrow) segs = nrow;
-  const int seg_rows = (nrow + segs - 1) / segs;
-  std::vector<uint64_t> J;                          // tdm_prepare_jump's segment jumps
-  if (segs > 1) {
-    int last_w = cols - (ty - 1) * ncol;
-    for (int iy = ty - 1; iy >= 0 && last_w <= 0; --iy) last_w = cols - iy * ncol;
-    if (last_w > ncol) last_w = ncol;
-    std::vector<int64_t> ks;
-    for (int s = 1; s < segs; ++s) { ks.push_back((int64_t)s * seg_rows * ncol); ks.push_back((int64_t)s * seg_rows * last_w); }
-    J.resize(ks.size() * 256);
-    build_jump_matrices(ks.data(), (int)ks.size(), J.data());
-  }
+  int seg_rows;
+  std::vector<uint64_t> J;
+  emu::segment_jumps(rows, cols, tx, ty, segs, seg_rows, J);
   int64_t kt[4];
   sample_tile_draws(rows, cols, tx, ty, kt);
   std::vector<uint64_t> mats(4 * 256);
@@ -72,38 +56,14 @@ extern "C" int emu_box_batch(int K, int8_t* grid0, int8_t* grid1, const int8_t* 
     bx[k].jump_tile = mats.data();
   }
   const int threads = ((ncact * gm + 31) / 32) * 32;
-  const unsigned gx = (unsigned)(mrows * segs), gy = (unsigned)((M + gm - 1) / gm);
-  for (unsigned z = 0; z < (unsigned)K; ++z)
-    for (unsigned by = 0; by < gy; ++by)
-      for (unsigned bxi = 0; bxi < gx; ++bxi) {
-        std::barrier<> bar(threads);
-        g_bar = &bar;
-        std::vector<std::thread> th;
-        for (int t = 0; t < threads; ++t)
-          th.emplace_back([&, t] {
-            threadIdx = {(unsigned)t, 0, 0}; blockIdx = {bxi, by, z}; blockDim = {(unsigned)threads, 1, 1};
-            gridDim = {gx, gy, (unsigned)K};
-            const int nw = bpad / 4;
-            if (nw == 3) sample_grids_v2_box_batch_kernel<3>(d.data(), bx.data(), active, 0, mrows, ncact);
-            else if (nw == 1) sample_grids_v2_box_batch_kernel<1>(d.data(), bx.data(), active, 0, mrows, ncact);
-            else if (nw == 8) sample_grids_v2_box_batch_kernel<8>(d.data(), bx.data(), active, 0, mrows, ncact);
-            else sample_grids_v2_box_batch_kernel<0>(d.data(), bx.data(), active, 0, mrows, ncact);
-          });
-        for (auto& x : th) x.join();
-      }
-  const unsigned nblk = (unsigned)((ngen + 127) / 128);
-  for (unsigned y = 0; y < (unsigned)K; ++y)
-    for (unsigned bxi = 0; bxi < nblk; ++bxi) {
-      std::barrier<> bar(128);
-      g_bar = &bar;
-      std::vector<std::thread> th;
-      for (int t = 0; t < 128; ++t)
-        th.emplace_back([&, t] {
-          threadIdx = {(unsigned)t, 0, 0}; blockIdx = {bxi, y, 0}; blockDim = {128, 1, 1}; gridDim = {nblk, (unsigned)K, 1};
-          advance_states_batch_kernel(d.data(), bx.data(), active, rows, cols, tx, ty, M);
-        });
-      for (auto& x : th) x.join();
-    }
+  emu::sampler_nw(bpad, [&](auto NW) {
+    emu::launch({(unsigned)(mrows * segs), (unsigned)((M + gm - 1) / gm), (unsigned)K}, threads, [&] {
+      sample_grids_v2_box_batch_kernel<decltype(NW)::value>(d.data(), bx.data(), active, 0, mrows, ncact);
+    });
+  });
+  emu::launch({(unsigned)((ngen + 127) / 128), (unsigned)K, 1}, 128, [&] {
+    advance_states_batch_kernel(d.data(), bx.data(), active, rows, cols, tx, ty, M);
+  });
   return 0;
 }
 
@@ -111,7 +71,6 @@ extern "C" int emu_box_batch(int K, int8_t* grid0, int8_t* grid1, const int8_t* 
 // disc = cx, cy, r
 extern "C" int emu_decide(const int* ci, const float* cf, int rows, int cols, int tx, int ty, int M, int bpad, float x,
                           float y, float reach, int* out, float* disc) {
-  using namespace b200;
   ReachBoxConst c{};
   c.mode = ci[0]; c.disc = ci[1]; c.T = ci[2]; c.rows = rows; c.cols = cols; c.nt = 2; c.tx = tx; c.ty = ty;
   c.num_maps = M; c.bpad0 = c.bpad1 = bpad;
@@ -130,23 +89,10 @@ extern "C" int emu_decide(const int* ci, const float* cf, int rows, int cols, in
 def libs(tmp_path_factory):
     import __graft_entry__
     __graft_entry__.build_engine()
-    d = tmp_path_factory.mktemp("boxbatch")
-    kh, sc = os.path.join(CSRC, "kernels.h"), os.path.join(CSRC, "sample.cu")
-    src = (PRELUDE + _region(kh, "sampler_args") + _region(kh, "box_desc") + _region(os.path.join(CSRC, "common.cuh"), "xoro") +
-           _region(os.path.join(CSRC, "common.cuh"), "threshold") + _region(sc, "sampler_v2") +
-           _region(sc, "sampler_box_batch") + HARNESS)
-    cpp, so = d / "boxbatch.cpp", d / "libboxbatch.so"
-    cpp.write_text(src)
-    libdir = os.path.join(ROOT, "mppi_numba_b200")
-    r = subprocess.run(["g++", "-O1", "-std=c++20", "-pthread", "-shared", "-fPIC", "-Wno-unknown-pragmas",
-                        "-ffp-contract=off", str(cpp), "-o", str(so), "-L" + libdir, "-l:libb200mppi.so",
-                        "-Wl,-rpath," + libdir], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    lib = C.CDLL(str(so))
-    lib.emu_box_batch.restype = C.c_int
-    lib.emu_decide.restype = C.c_int
-    lib.emu_decide.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int] * 6 + [C.c_float] * 3 + [C.c_void_p, C.c_void_p]
-    return lib, build(str(d))
+    # emu_sample_v2 (tests/emu_sampler.py) is the per-pair reference, compiled into the same library
+    lib = emu_core.build(str(tmp_path_factory.mktemp("boxbatch")), "boxbatch", kernels(None, "sampler_box_batch"),
+                         emu_sampler.HARNESS + HARNESS, link_engine=True)
+    return lib, lib
 
 
 def _p(a):

@@ -1,5 +1,5 @@
 """The batched CTA-wide CVaR kernel (cvar_large_batch_kernel, csrc/rollout.cu: stochastic batches of more than 1024
-maps) from its real source on the host, with the technique and hardware stand-ins of tests/emu_cvar.py.  For K planners
+maps) from its real source on the host, with the kernels and harness of tests/emu_cvar.py.  For K planners
 of equal N and M, each with its own alpha, one batched launch (grid (N, K)) must equal cvar_large_kernel run once per
 planner bit for bit, and each result must lie within the CTA kernel's derived bound around the exact CVaR
 (tests/reduce_bounds.py): M from just above the warp kernel's limit to the largest the kernel takes; numel 1, M - 1, M
@@ -7,16 +7,13 @@ and the benchmark's alpha 0.2; ties, signed zeros, +-inf and 1e+-30 magnitudes a
 reduce_bounds.cvar_rows), scattered +inf; a row stride larger than N.  With CvarDesc::active, stopped planners' outputs
 stay byte for byte as they were and running planners equal the ungated launch."""
 import ctypes as C
-import os
-import re
-import subprocess
 
 import numpy as np
 import pytest
 
 from tests import emu_cvar
 from tests import reduce_bounds as RB
-from tests.emu_rollout import _region
+from tests.emu_core import build
 
 F32 = np.float32
 
@@ -26,7 +23,6 @@ HARNESS = r'''
 // out_single: cvar_large_kernel once per planner
 extern "C" int emu_cvar_large_batch(int K, const float* costs_mn, int N, int M, int ld, const int* numel,
                                     const int* active, float* out_batch, float* out_single) {
-  using namespace b200;
   if (M <= 32 * CVAR_MAX_PER_LANE || M > (1 << 15) || ld < N) return 1;
   std::vector<CvarDesc> d(K);
   for (int k = 0; k < K; ++k)
@@ -34,10 +30,10 @@ extern "C" int emu_cvar_large_batch(int K, const float* costs_mn, int N, int M, 
                     active ? active + k : nullptr};
   if (out_single)
     for (int k = 0; k < K; ++k)
-      run([&] { cvar_large_kernel(costs_mn + (size_t)k * M * ld, out_single + (size_t)k * N, N, ld, M, numel[k],
-                                  FlagWait{}); }, CVAR_LARGE_THREADS, (unsigned)N);
-  for (int k = 0; k < K; ++k)
-    run([&] { blockIdx.y = (unsigned)k; cvar_large_batch_kernel(d.data()); }, CVAR_LARGE_THREADS, (unsigned)N);
+      emu::launch({(unsigned)N, 1, 1}, CVAR_LARGE_THREADS, [&] {
+        cvar_large_kernel(costs_mn + (size_t)k * M * ld, out_single + (size_t)k * N, N, ld, M, numel[k], FlagWait{});
+      });
+  emu::launch({(unsigned)N, (unsigned)K, 1}, CVAR_LARGE_THREADS, [&] { cvar_large_batch_kernel(d.data()); });
   return 0;
 }
 '''
@@ -46,22 +42,7 @@ extern "C" int emu_cvar_large_batch(int K, const float* costs_mn, int N, int M, 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
     out = str(tmp_path_factory.mktemp("emu_cvar_large_batch"))
-    csrc = emu_cvar.CSRC
-    rollout = os.path.join(csrc, "rollout.cu")
-    kern = _region(rollout, "cvar") + _region(rollout, "cvar_large_batch")
-    kern = re.sub(r"(?m)^(\s*)__shared__ ", r"\1static ", kern)
-    src = (emu_cvar.PRELUDE + _region(os.path.join(csrc, "kernels.h"), "cvar_desc") +
-           _region(os.path.join(csrc, "common.cuh"), "warp_sum") + kern + emu_cvar.HARNESS + HARNESS)
-    cpp, so = os.path.join(out, "cvar_large_batch_emu.cpp"), os.path.join(out, "libcvar_large_batch_emu.so")
-    open(cpp, "w").write(src)
-    r = subprocess.run(["g++", "-O1", "-std=c++20", "-pthread", "-shared", "-fPIC", "-Wno-unknown-pragmas", cpp, "-o", so],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    lib = C.CDLL(so)
-    P, I = C.c_void_p, C.c_int
-    lib.emu_cvar_large_batch.restype = I
-    lib.emu_cvar_large_batch.argtypes = [I, P, I, I, I, P, P, P, P]
-    return lib
+    return build(out, "cvar_large_batch_emu", emu_cvar.kernels("cvar_large_batch"), emu_cvar.HARNESS + HARNESS)
 
 
 def _p(a):

@@ -9,17 +9,13 @@ from 0 (georeferenced maps), reverse driving, negative traction, cos / sin off b
 Their float32 states follow the oracle's arithmetic (oracle/mppi_ref.py rollout_costs: dv = (traction * dt) * v in
 float64, x = f32(dv * cos + x), cell = floor_div_f32(f32(x - xlo), res)).  Boxed decisions must also stay tight."""
 import ctypes as C
-import os
-import re
-import subprocess
 
 import numpy as np
 import pytest
 
 from oracle import mppi_ref as MR
+from tests.emu_core import build, region
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-KH = os.path.join(ROOT, "mppi_numba_b200", "csrc", "kernels.h")
 F32, F64 = np.float32, np.float64
 U = 2.0 ** -24
 
@@ -41,19 +37,7 @@ extern "C" int emu_decide(const int* ci, const float* cf, float x, float y, cons
 
 @pytest.fixture(scope="module")
 def decide(tmp_path_factory):
-    out = tmp_path_factory.mktemp("reachbox")
-    m = re.search(r"// \[emu:begin sampler_args\][^\n]*\n(.*?)// \[emu:end sampler_args\]", open(KH).read(), re.S)
-    assert m
-    src = ("#include <cmath>\n#include <cstddef>\n#include <cstdint>\n#define __host__\n#define __device__\n"
-           "namespace b200 {\n" + m.group(1) + "}\n" + HARNESS)
-    cpp, so = out / "reachbox.cpp", out / "libreachbox.so"
-    cpp.write_text(src)
-    r = subprocess.run(["g++", "-O1", "-std=c++17", "-shared", "-fPIC", "-ffp-contract=off", str(cpp), "-o", str(so)],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    lib = C.CDLL(str(so))
-    lib.emu_decide.restype = C.c_int
-    lib.emu_decide.argtypes = [C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib = build(str(tmp_path_factory.mktemp("reachbox")), "reachbox", [region("kernels.h", "sampler_args")], HARNESS)
 
     def run(mode, T, rows, cols, vr, dt, trm, res, pxl, pyl, x, y, reach=None):
         # one TDM, 16 x 256 generator tiles, 64 maps: a staged launch that fits any box of these maps

@@ -6,17 +6,16 @@ solve() made before it was shared, with the float32 rounding terms of reach_radi
 fill_win_args' former code."""
 import ctypes as C
 import os
-import re
 import subprocess
 
 import numpy as np
 import pytest
 
+from tests import emu_core, emu_trial
 from tests.fake_backend import disarm
 from tests.test_stochastic_batch_host_cpu import StochasticFake, planner
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "mppi_numba_b200", "csrc")
 NAME = "b200mppi_batch_run_stochastic_trials"
 
 
@@ -163,29 +162,11 @@ extern "C" void emu_win(float x, float y, float pxl, float pyl, float res, int c
 '''
 
 
-def _region(path, name):
-    m = re.search(r"// \[emu:begin %s\][^\n]*\n(.*?)// \[emu:end %s\]" % (name, name), open(path).read(), re.S)
-    assert m, name
-    return m.group(1)
-
-
 @pytest.fixture(scope="module")
 def helpers(tmp_path_factory):
-    out = tmp_path_factory.mktemp("helpers")
-    kh = os.path.join(CSRC, "kernels.h")
-    src = ("#include <cmath>\n#include <cstddef>\n#include <cstdint>\n#define __host__\n#define __device__\n"
-           "namespace b200 {\n" + _region(kh, "sampler_args") + _region(kh, "trial_args").split("struct TrialDev")[0] +
-           "}\n" + HARNESS)
-    cpp, so = out / "helpers.cpp", out / "libhelpers.so"
-    cpp.write_text(src)
-    r = subprocess.run(["g++", "-O1", "-std=c++17", "-shared", "-fPIC", "-ffp-contract=off", str(cpp), "-o", str(so)],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    lib = C.CDLL(str(so))
-    lib.emu_decide.restype = C.c_int
-    lib.emu_decide.argtypes = [C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.emu_win.argtypes = [C.c_float] * 5 + [C.c_int, C.c_int, C.c_void_p]
-    return lib
+    return emu_core.build(str(tmp_path_factory.mktemp("helpers")), "helpers",
+                          [emu_core.region("kernels.h", "sampler_args"), emu_core.region("kernels.h", "trial_args")],
+                          HARNESS)
 
 
 def host_decision(ci, cf, x, y, reach):
@@ -286,7 +267,6 @@ def test_window_origin_matches_fill_win_args(helpers):
 
 
 PLANT_HARNESS = r'''
-}  // namespace b200
 // one plant step of one planner on a uniform grid (traction lt, at) from pose x; win = {WW, WH, wx0, wy0, ww, wh} of its
 // RolloutWinArgs, recomputed by the kernel over a map of rows x cols cells at res from (pxl, pyl)
 extern "C" void emu_plant_win(const double* x, float v, float w, double lt, double at, double dt, float pxl, float pyl,
@@ -305,11 +285,7 @@ extern "C" void emu_plant_win(const double* x, float v, float w, double lt, doub
   double xh[6];
   float uh[2];
   PlantArgs a{&d, &st, &active, &count, xh, uh, 1, 2, 1, 0};
-  std::barrier<> bar(32);
-  g_bar = &bar;
-  std::vector<std::thread> th;
-  for (int lane = 0; lane < 32; ++lane) th.emplace_back([&, lane] { plant_step_body(a, 0, lane); });
-  for (auto& t : th) t.join();
+  emu::launch({1, 1, 1}, 32, [&] { plant_step_body(a, 0, (int)threadIdx.x); });
 }
 '''
 
@@ -317,13 +293,7 @@ extern "C" void emu_plant_win(const double* x, float v, float w, double lt, doub
 def test_plant_step_window_matches_fill_win_args(tmp_path):
     """The window fields the plant step writes into a stochastic planner's RolloutWinArgs (TrialDev::win) against
     fill_win_args' former computation from the float32 x0 it wrote, including maps smaller than one window."""
-    from tests.emu_batch import _compile, _src
-    from tests.emu_trial import PRELUDE
-    lib = _compile(str(tmp_path), "plant_win_emu", PRELUDE + _src("kernels.h", "trial_args") + _src("reduce.cu", "trial") +
-                   PLANT_HARNESS)
-    lib.emu_plant_win.restype = None
-    lib.emu_plant_win.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_double, C.c_double, C.c_double, C.c_float,
-                                  C.c_float, C.c_float, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    lib = emu_trial.build(str(tmp_path), extra=PLANT_HARNESS)
     rng = np.random.default_rng(5)
     for (rows, cols, res, pxl, pyl) in [(512, 512, 0.1, -0.8, -0.8), (9, 9, 1.0, -2.0, -2.0), (200, 90, 0.25, 1.5, 0.0),
                                          (300, 700, 0.2, 0.0, -3.0)]:

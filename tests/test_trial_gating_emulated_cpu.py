@@ -7,36 +7,23 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests import emu_noise, emu_update
-from tests.emu_batch import _compile, _src
+from tests import emu_batch
 
 NOISE = r'''
-}  // namespace b200
 extern "C" void emu_noise_gated(int K, const int* active, uint64_t** states, float** noise, const float* std, long long count) {
-  using namespace b200;
   std::vector<NoiseDesc> d(K);
   for (int i = 0; i < K; ++i) d[i] = NoiseDesc{states[i], noise[i], std[2 * i], std[2 * i + 1]};
-  blockDim = {256, 1, 1};
-  const long long padded = (count + 255) / 256 * 256;
-  for (int i = 0; i < K; ++i)
-    for (long long g = 0; g < padded; ++g) {
-      blockIdx = {(unsigned)(g / 256), (unsigned)i, 0}; threadIdx = {(unsigned)(g % 256), 0, 0};
-      sample_noise_batch_kernel(d.data(), count, active);
-    }
+  emu::launch_serial({(unsigned)((count + 255) / 256), (unsigned)K, 1}, 256, [&] { sample_noise_batch_kernel(d.data(), count, active); });
 }
 '''
 
 UPDATE = r'''
-}  // namespace b200
 extern "C" void emu_update_gated(int K, const int* active, const float** costs, const float** noise, float** w_raw,
                                  float** parts, float** rank_partial, float** u_cur, float** weights, float** u_prev,
                                  float** u_out, unsigned* counters, int N, int T) {
-  using namespace b200;
   std::vector<UpdateBatchDesc> d(K);
-  int ctas = (N + 31) / 32;
-  if (ctas > 296) ctas = 296;
-  const int rows_per_cta = (N + ctas - 1) / ctas;
-  ctas = (N + rows_per_cta - 1) / rows_per_cta;
+  int ctas, rows_per_cta;
+  emu::update_geometry(N, ctas, rows_per_cta);
   for (int i = 0; i < K; ++i) {
     UpdateArgs a{};
     a.costs = costs[i]; a.noise = noise[i]; a.w_raw = w_raw[i]; a.cta_partials = parts[i]; a.rank_partial = rank_partial[i];
@@ -46,40 +33,19 @@ extern "C" void emu_update_gated(int K, const int* active, const float** costs, 
     tl.counter = &counters[i]; tl.mode = UPD_TAIL_APPLY; tl.u_prev = u_prev[i]; tl.u_out = u_out[i];
     d[i] = UpdateBatchDesc{a, tl};
   }
-  for (unsigned by = 0; by < (unsigned)K; ++by)
-    for (unsigned bx = 0; bx < (unsigned)ctas; ++bx) {
-      std::barrier<> bar(UPD_THREADS);
-      g_bar = &bar;
-      std::vector<std::unique_ptr<EmuWarp>> warps;
-      for (int w = 0; w < UPD_THREADS / 32; ++w) warps.emplace_back(new EmuWarp());
-      std::vector<std::thread> th;
-      for (int t = 0; t < UPD_THREADS; ++t)
-        th.emplace_back([&, t] {
-          threadIdx = {(unsigned)t, 0, 0}; blockIdx = {bx, by, 0}; blockDim = {(unsigned)UPD_THREADS, 1, 1};
-          gridDim = {(unsigned)ctas, (unsigned)K, 1};
-          g_warp = warps[t / 32].get();
-          update_partial_batch_kernel(d.data(), active);
-        });
-      for (auto& x : th) x.join();
-    }
+  emu::launch({(unsigned)ctas, (unsigned)K, 1}, UPD_THREADS, [&] { update_partial_batch_kernel(d.data(), active); });
 }
 '''
 
 
 @pytest.fixture(scope="module")
 def libs(tmp_path_factory):
-    import re
     out = str(tmp_path_factory.mktemp("gating"))
-    noise = _compile(out, "noise_gated", "#include <vector>\n" + emu_noise.PRELUDE + _src("common.cuh", "xoro") +
-                     _src("common.cuh", "normal") + _src("reduce.cu", "noise") + _src("kernels.h", "noise_desc") +
-                     _src("reduce.cu", "noise_batch") + NOISE, std="c++17")
-    kernels = _src("reduce.cu", "update") + _src("reduce.cu", "update_batch")
-    kernels = re.sub(r"(?m)^(\s*)__shared__ ", r"\1static ", kernels)
-    kernels = kernels.replace("int update_num_ctas(int N) {", "static int update_num_ctas_unused(int N) {")
-    update = _compile(out, "update_gated", emu_update.PRELUDE + "constexpr int P2P_MAX_PEERS = 16;\n" +
-                      _src("kernels.h", "update_args") + _src("kernels.h", "update_tail") + _src("kernels.h", "update_desc") +
-                      _src("common.cuh", "warp_min") + _src("common.cuh", "warp_sum") + kernels + UPDATE)
-    return noise, update
+    return emu_batch.build_noise(out, extra=NOISE), emu_batch.build_update(out, extra=UPDATE)
+
+
+def _p(a):
+    return C.c_void_p(a.ctypes.data)
 
 
 def ptrs(arrs):
@@ -97,7 +63,7 @@ def test_noise_gating(libs):
         st = [s.copy() for s in states0]
         nz = [np.full((N, T, 2), 9.0, np.float32) for _ in range(K)]
         act = np.array(active, np.int32)
-        noise_lib.emu_noise_gated(K, act.ctypes.data, ptrs(st), ptrs(nz), std.ctypes.data, C.c_longlong(N * T))
+        noise_lib.emu_noise_gated(K, _p(act), ptrs(st), ptrs(nz), _p(std), N * T)
         runs.append((st, nz))
     (s_all, n_all), (s_g, n_g) = runs
     assert np.array_equal(s_g[1], states0[1]) and (n_g[1] == 9.0).all()
@@ -124,9 +90,9 @@ def test_update_gating_leaves_the_ticket_counter(libs):
                     out=[np.full((T, 2), 5.0, np.float32) for _ in range(K)])
         counters = np.array([7, 0, 0], np.uint32) if active[0] == 0 else np.zeros(K, np.uint32)
         act = np.array(active, np.int32)
-        update_lib.emu_update_gated(K, act.ctypes.data, ptrs(costs), ptrs(noise), ptrs(bufs["w"]), ptrs(bufs["parts"]),
+        update_lib.emu_update_gated(K, _p(act), ptrs(costs), ptrs(noise), ptrs(bufs["w"]), ptrs(bufs["parts"]),
                                     ptrs(bufs["rank"]), ptrs(bufs["u"]), ptrs(bufs["weights"]), ptrs(bufs["prev"]),
-                                    ptrs(bufs["out"]), counters.ctypes.data, N, T)
+                                    ptrs(bufs["out"]), _p(counters), N, T)
         runs.append((bufs, counters))
     (b_all, c_all), (b_g, c_g) = runs
     assert c_g.tolist() == [7, 0, 0] and c_all.tolist() == [0, 0, 0]

@@ -14,7 +14,6 @@ NOISE = r'''
 // 0 when the running planners agree and the stopped ones are untouched
 extern "C" int emu_noise_gated(int K, const uint64_t* states_in, const float* u_cur, int N, int T, const float* fp,
                                int iter, const int* active) {
-  using namespace b200;
   const int npad = (N + 31) / 32 * 32;
   const size_t ns = (size_t)N * T * 2, nT = (size_t)(T + 1) * npad;
   struct Bufs {
@@ -33,8 +32,9 @@ extern "C" int emu_noise_gated(int K, const uint64_t* states_in, const float* u_
       x.reach[2 * k + ((k & 1) ^ (iter & 1))] = 0.0f;
     }
   }
-  run([&] { noise_prepare_batch_kernel(b[0].d.data(), N, T, npad, iter, active); }, 256, (unsigned)(npad / NP_NB), (unsigned)K);
-  run([&] { noise_prepare_batch_kernel(b[1].d.data(), N, T, npad, iter); }, 256, (unsigned)(npad / NP_NB), (unsigned)K);
+  const EmuDim3 grid{(unsigned)(npad / NP_NB), (unsigned)K, 1};
+  emu::launch(grid, 256, [&] { noise_prepare_batch_kernel(b[0].d.data(), N, T, npad, iter, active); });
+  emu::launch(grid, 256, [&] { noise_prepare_batch_kernel(b[1].d.data(), N, T, npad, iter); });
   for (int k = 0; k < K; ++k) {
     const Bufs& want = active[k] ? b[1] : b[2];        // b[2]: never launched
     if (std::memcmp(b[0].st.data() + k * ns, want.st.data() + k * ns, ns * 8)) return 1;
@@ -49,22 +49,18 @@ extern "C" int emu_noise_gated(int K, const uint64_t* states_in, const float* u_
 
 CVAR = r'''
 extern "C" int emu_cvar_gated(int K, const float* costs_mn, int N, int M, const int* numel, const int* active) {
-  using namespace b200;
   std::vector<float> gated(K * N, -3.0f), full(K * N, -3.0f);
   std::vector<CvarDesc> dg(K), df(K);
   for (int k = 0; k < K; ++k) {
     dg[k] = CvarDesc{costs_mn + (size_t)k * M * N, gated.data() + (size_t)k * N, N, N, M, numel[k], active + k};
     df[k] = CvarDesc{costs_mn + (size_t)k * M * N, full.data() + (size_t)k * N, N, N, M, numel[k]};
   }
-  const int nb = cvar_block_n(M), per = (M + 31) / 32;
-  const unsigned blocks = (unsigned)((N + nb - 1) / nb);
-  auto batched = [&](auto kern, std::vector<CvarDesc>& d) {
-    for (int k = 0; k < K; ++k) run([&] { blockIdx.y = (unsigned)k; kern(d.data()); }, CVAR_THREADS, blocks);
-  };
-  auto both = [&](auto kern) { batched(kern, dg); batched(kern, df); };
-  if (per <= 1) both(cvar_batch_kernel<1>); else if (per <= 2) both(cvar_batch_kernel<2>);
-  else if (per <= 4) both(cvar_batch_kernel<4>); else if (per <= 8) both(cvar_batch_kernel<8>);
-  else if (per <= 16) both(cvar_batch_kernel<16>); else both(cvar_batch_kernel<32>);
+  const int nb = cvar_block_n(M);
+  const EmuDim3 grid{(unsigned)((N + nb - 1) / nb), (unsigned)K, 1};
+  emu::cvar_per(M, [&](auto P) {
+    emu::launch(grid, CVAR_THREADS, [&] { cvar_batch_kernel<decltype(P)::value>(dg.data()); });
+    emu::launch(grid, CVAR_THREADS, [&] { cvar_batch_kernel<decltype(P)::value>(df.data()); });
+  });
   for (int k = 0; k < K; ++k)
     for (int n = 0; n < N; ++n) {
       const float want = active[k] ? full[(size_t)k * N + n] : -3.0f;
@@ -76,20 +72,8 @@ extern "C" int emu_cvar_gated(int K, const float* costs_mn, int N, int M, const 
 
 
 @pytest.fixture(scope="module")
-def libs(tmp_path_factory, monkeypatch_module=None):
-    mp = pytest.MonkeyPatch()
-    mp.setattr(ESB, "HARNESS", ESB.HARNESS + NOISE)
-    mp.setattr(ESB, "CVAR_HARNESS", ESB.CVAR_HARNESS + CVAR)
-    try:
-        lib, cvl = ESB.build(str(tmp_path_factory.mktemp("gating")))
-    finally:
-        mp.undo()
-    P, I = C.c_void_p, C.c_int
-    lib.emu_noise_gated.restype = I
-    lib.emu_noise_gated.argtypes = [I, P, P, I, I, P, I, P]
-    cvl.emu_cvar_gated.restype = I
-    cvl.emu_cvar_gated.argtypes = [I, P, I, I, P, P]
-    return lib, cvl
+def libs(tmp_path_factory):
+    return ESB.build(str(tmp_path_factory.mktemp("gating")), extra=NOISE, cvar_extra=CVAR)
 
 
 def _p(a):
