@@ -1,49 +1,19 @@
 """Batched one-map solves on the GPU (run with ``-m gpu``): one MPPI_Batch.solve() of K planners against K solve()
 calls on identical twins, bit for bit -- the returned u, every planner buffer solve() writes, the planners' and their
 TDMs' RNG states and the sampled maps -- over several closed-loop rounds; launch counts; every rejection path."""
-import contextlib
 import ctypes as C
-import io
 
 import numpy as np
 import pytest
 
+from tests.gpu_harness import (assert_same, batch_vs_sequential, eng, planner_launches, quiet,  # noqa: F401
+                               snapshot, tdm_planner, vary)
 from tests.scenarios import make_scenario
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__
-    __graft_entry__.build_engine()
-    import mppi_numba_b200 as E
-    assert E.device_count() >= 1, "GPU tests need a CUDA device"
-    return E
-
-
-def _quiet():
-    return contextlib.redirect_stdout(io.StringIO())
-
-
-# ----------------------------------------------------------------------------- planners and their state
-def map_planner(E, sc, k):
-    """One det / speed-map planner of scenario `sc`, varied by its index k (lambda, u_std, warm start)."""
-    with _quiet():
-        cfg = E.Config(**sc["cfg"])
-        lin, ang = E.TDM_Numba(cfg), E.TDM_Numba(cfg)
-        lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        pl = E.MPPI_Numba(cfg)
-    params = dict(sc["params"])
-    params["lambda_weight"] = [1.0, 0.5, 2.0, 0.8, 1.3][k % 5]
-    params["u_std"] = np.array([2.0, 3.0]) * (1.0 + 0.1 * (k % 7))
-    pl.setup(params, lin, ang)
-    if "u0" in sc:
-        pl.u_cur_d.copy_to_device(sc["u0"])
-    return pl
-
-
+# ----------------------------------------------------------------------------- planners
 def map_scenario(mode, k, N=256, T=24, H=48, res=0.2, B=6, det_alpha=1.0, num_opt=1):
     sc = make_scenario(mode, N=N, M=1, T=T, H=H, W=H, res=res, B=B, seed=11 + 7 * k, det_alpha=det_alpha,
                        warm_start=(k % 2 == 1))
@@ -53,7 +23,7 @@ def map_scenario(mode, k, N=256, T=24, H=48, res=0.2, B=6, det_alpha=1.0, num_op
 
 def barebone_planner(E, k, N=300, T=20, num_opt=1):
     from mppi_numba_b200 import barebone as BB
-    with _quiet():
+    with quiet():
         pl = BB.MPPI_Numba(BB.Config(T=T * 0.1 + 0.05, dt=0.1, num_control_rollouts=N, num_vis_state_rollouts=4,
                                      seed=3 + k))
     rng = np.random.default_rng(40 + k)
@@ -69,48 +39,6 @@ def barebone_planner(E, k, N=300, T=20, num_opt=1):
     return pl
 
 
-def planner_launches(E, p):
-    n = C.c_int64()
-    E._lib.check(E._lib.lib.b200mppi_planner_launch_count(p._handle, C.byref(n)))
-    return int(n.value)
-
-
-def snapshot(p):
-    d = dict(u_cur=p.u_cur_d.copy_to_host(), u_prev=p.u_prev_d.copy_to_host(), noise=p.noise_samples_d.copy_to_host(),
-             costs=p.costs_d.copy_to_host(), weights=p.weights_d.copy_to_host(), rng=p.rng_states_d.copy_to_host())
-    if getattr(p, "lin_tdm", None) is not None:
-        for name, t in (("lin", p.lin_tdm), ("ang", p.ang_tdm)):
-            d[name + "_rng"] = t.rng_states_d.copy_to_host()
-            d[name + "_map"] = t.sample_grid_batch_d.copy_to_host()
-    return d
-
-
-def assert_same(a, b, what):
-    assert a.keys() == b.keys()
-    for key in a:
-        assert np.array_equal(a[key], b[key]), "%s: %s differs" % (what, key)
-
-
-def batch_vs_sequential(E, make, K, rounds=3):
-    """Twins built by make(k); batch solve on one set, K solve() calls on the other, `rounds` closed-loop rounds."""
-    with _quiet():
-        A = [make(k) for k in range(K)]
-        B = [make(k) for k in range(K)]
-        batch = E.MPPI_Batch(A)
-        for r in range(rounds):
-            ub = batch.solve()
-            us = np.stack([p.solve() for p in B])
-            assert ub.shape == us.shape and ub.dtype == np.float32
-            assert np.array_equal(ub, us), "round %d: u differs" % r
-            for k in range(K):
-                assert_same(snapshot(A[k]), snapshot(B[k]), "round %d planner %d" % (r, k))
-            for k in range(K):
-                x0 = np.asarray(A[k].params["x0"], dtype=np.float64) + np.array([0.03 * (k + 1), -0.02 * r, 0.05])
-                A[k].shift_and_update(x0.copy(), ub[k], 1)
-                B[k].shift_and_update(x0.copy(), us[k], 1)
-    return A, B, batch
-
-
 # ----------------------------------------------------------------------------- equality with sequential solves
 @pytest.mark.parametrize("mode", ["det", "spd", "barebone"])
 def test_batch_equals_sequential_closed_loop(eng, mode):
@@ -118,23 +46,23 @@ def test_batch_equals_sequential_closed_loop(eng, mode):
         make = lambda k: barebone_planner(eng, k)                       # noqa: E731
     else:
         scs = [map_scenario(mode, k, det_alpha=0.5 if mode == "det" else 1.0) for k in range(5)]
-        make = lambda k: map_planner(eng, scs[k], k)                    # noqa: E731
-    A, B, batch = batch_vs_sequential(eng, make, 5)
+        make = lambda k: tdm_planner(eng, vary(scs[k], k))              # noqa: E731
+    A, B, batch = batch_vs_sequential(eng.MPPI_Batch, make, 5)
     # the batch keeps its own launch counter: one launch per stage per round, whatever K
     assert batch.launch_count() == 3 * (3 if mode == "barebone" else 4)
-    assert planner_launches(eng, A[0]) == 0 and planner_launches(eng, B[0]) == batch.launch_count()
+    assert planner_launches(A[0]) == 0 and planner_launches(B[0]) == batch.launch_count()
 
 
 def test_batch_of_one_and_num_opt_two(eng):
     sc = map_scenario("det", 0)
-    batch_vs_sequential(eng, lambda k: map_planner(eng, sc, k), 1, rounds=2)
+    batch_vs_sequential(eng.MPPI_Batch, lambda k: tdm_planner(eng, vary(sc, k)), 1, rounds=2)
     scs = [map_scenario("det", k, num_opt=2) for k in range(3)]
-    A, B, batch = batch_vs_sequential(eng, lambda k: map_planner(eng, scs[k], k), 3, rounds=2)
+    A, B, batch = batch_vs_sequential(eng.MPPI_Batch, lambda k: tdm_planner(eng, vary(scs[k], k)), 3, rounds=2)
     assert batch.launch_count() == 2 * (4 + 3)                          # sampler in the first iteration only
-    bb = batch_vs_sequential(eng, lambda k: barebone_planner(eng, k, num_opt=2), 3, rounds=1)[2]
+    bb = batch_vs_sequential(eng.MPPI_Batch, lambda k: barebone_planner(eng, k, num_opt=2), 3, rounds=1)[2]
     assert bb.launch_count() == 6
     scs = [map_scenario("det", k, num_opt=0) for k in range(2)]         # maps sampled, u returned unchanged
-    A, B, batch = batch_vs_sequential(eng, lambda k: map_planner(eng, scs[k], k), 2, rounds=1)
+    A, B, batch = batch_vs_sequential(eng.MPPI_Batch, lambda k: tdm_planner(eng, vary(scs[k], k)), 2, rounds=1)
     assert batch.launch_count() == 1
 
 
@@ -142,22 +70,22 @@ def test_batch_heterogeneous_map_sizes_take_the_sampler_fallback(eng):
     """Pairs whose map geometry differs from the first pair's are sampled by their own launches: same results,
     one sampler launch more per such pair."""
     scs = [map_scenario("det", k, H=[40, 56, 40, 56][k]) for k in range(4)]
-    A, B, batch = batch_vs_sequential(eng, lambda k: map_planner(eng, scs[k], k), 4, rounds=2)
+    A, B, batch = batch_vs_sequential(eng.MPPI_Batch, lambda k: tdm_planner(eng, vary(scs[k], k)), 4, rounds=2)
     assert batch.launch_count() == 2 * (1 + (1 + 2) + 1 + 1)
     scs = [map_scenario("det", k, H=48) for k in range(4)]
-    A, B, batch = batch_vs_sequential(eng, lambda k: map_planner(eng, scs[k], k), 4, rounds=2)
+    A, B, batch = batch_vs_sequential(eng.MPPI_Batch, lambda k: tdm_planner(eng, vary(scs[k], k)), 4, rounds=2)
     assert batch.launch_count() == 2 * 4
 
 
 def test_batch_launch_count_does_not_grow_with_k(eng):
     """Config-2 shape (N 1024, T 64, 256 x 256, nominal 2-bin maps): K = 16 issues the launches of K = 1."""
     scs = [map_scenario("det", k, N=1024, T=64, H=256, B=2) for k in range(16)]
-    with _quiet():
-        one = map_planner(eng, scs[0], 0)
+    with quiet():
+        one = tdm_planner(eng, vary(scs[0], 0))
         l0 = one.launch_count()
         one.solve()
         single = one.launch_count() - l0
-        planners = [map_planner(eng, scs[k], k) for k in range(16)]
+        planners = [tdm_planner(eng, vary(scs[k], k)) for k in range(16)]
         batch = eng.MPPI_Batch(planners)
         assert batch.solve() is not None
     assert single == 4 and batch.launch_count() == single
@@ -167,7 +95,7 @@ def test_batch_config4_shape_k32_equals_sequential(eng):
     """Config-4 shape: N 4096, T 128, 512 x 512 PMF, 32 bins, det alpha 0.3; K = 32 planners."""
     scs = [make_scenario("det", N=4096, M=1, T=128, H=512, W=512, res=0.2, B=32, seed=100 + k, det_alpha=0.3,
                          warm_start=(k % 3 == 0)) for k in range(32)]
-    batch_vs_sequential(eng, lambda k: map_planner(eng, scs[k], k), 32, rounds=1)
+    batch_vs_sequential(eng.MPPI_Batch, lambda k: tdm_planner(eng, vary(scs[k], k)), 32, rounds=1)
 
 
 # ----------------------------------------------------------------------------- rejections
@@ -181,13 +109,13 @@ def _raw_create(L, pls):
 def test_batch_rejections_launch_nothing_and_leave_state_untouched(eng, capsys):
     L = eng._lib
     scs = [map_scenario("det", k) for k in range(3)]
-    with _quiet():
-        dets = [map_planner(eng, scs[k], k) for k in range(3)]
-        spd = map_planner(eng, map_scenario("spd", 0), 0)
-        other_n = map_planner(eng, map_scenario("det", 5, N=128), 0)
-        other_t = map_planner(eng, map_scenario("det", 5, T=20), 0)
+    with quiet():
+        dets = [tdm_planner(eng, vary(scs[k], k)) for k in range(3)]
+        spd = tdm_planner(eng, vary(map_scenario("spd", 0), 0))
+        other_n = tdm_planner(eng, vary(map_scenario("det", 5, N=128), 0))
+        other_t = tdm_planner(eng, vary(map_scenario("det", 5, T=20), 0))
         tdm_sc = make_scenario("tdm", N=256, M=4, T=24, H=48, W=48, res=0.2, B=6, seed=2)
-        tdm = map_planner(eng, tdm_sc, 0)
+        tdm = tdm_planner(eng, vary(tdm_sc, 0))
     for p in dets:
         p.move_mppi_task_vars_to_device()
     for pls, want in (([dets[0], tdm], "planner 1 is MODE_TDM: the stochastic mode is not batched"),

@@ -12,33 +12,11 @@ pytestmark = pytest.mark.gpu
 from oracle import arith as AR              # noqa: E402
 from oracle import mppi_ref as MR           # noqa: E402
 from oracle import xoroshiro as X           # noqa: E402
+from tests.gpu_harness import (RawPlanner, assert_all_equal, dev, directed_oracle, eng,   # noqa: E402,F401
+                               run_directed, staged_rollout, tdm_planner)
 from tests.scenarios import make_scenario, oracle_rollout_costs   # noqa: E402
 
 F32 = np.float32
-
-
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__
-    __graft_entry__.build_engine()
-    import mppi_numba_b200 as E
-    assert E.device_count() >= 1, "GPU tests need a CUDA device"
-    return E
-
-
-@pytest.fixture(scope="module")
-def dev(eng):
-    return AR.Exact(AR.DeviceProvider(eng._lib), ftz=True)
-
-
-def assert_all_equal(got, want, what):
-    got, want = np.asarray(got, F32), np.asarray(want, F32)
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    bad = np.argwhere(got.view(np.uint32) != want.view(np.uint32))
-    print("\n[%s] %d mismatches of %d" % (what, len(bad), got.size))
-    assert bad.size == 0, "%s: %d of %d differ; first: %s" % (
-        what, len(bad), got.size, [(tuple(int(i) for i in ix), float(got[tuple(ix)]), float(want[tuple(ix)]))
-                                   for ix in bad[:5]])
 
 
 def test_device_math_entry_point(eng):
@@ -56,30 +34,12 @@ def test_device_math_entry_point(eng):
     assert L.lib.b200mppi_debug_device_math(0, None, None, None, 0) == 0
 
 
-def _planner_rollout(eng, sc):
-    cfg = eng.Config(**sc["cfg"])
-    lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-    lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    pl = eng.MPPI_Numba(cfg)
-    pl.setup(sc["params"], lin, ang)
-    if "u0" in sc:
-        pl.u_cur_d.copy_to_device(sc["u0"])
-    pl.move_mppi_task_vars_to_device()
-    L = eng._lib
-    lin.sample_grids(1.0)
-    ang.sample_grids(1.0)
-    L.check(L.lib.b200mppi_planner_sample_noise(pl._handle))
-    L.check(L.lib.b200mppi_planner_rollout(pl._handle))
-    return pl, lin, ang
-
-
 def test_generic_stochastic_kernel_without_window(eng, dev, monkeypatch):
     """B200MPPI_NO_WINDOW: the generic kernel on the res 0.05 row (rollouts leave the window region)."""
     monkeypatch.setenv("B200MPPI_NO_WINDOW", "1")
     sc = make_scenario("tdm", N=512, M=16, T=128, H=900, W=900, res=0.05, B=12, seed=4, warm_start=True)
-    pl, lin, ang = _planner_rollout(eng, sc)
-    want = oracle_rollout_costs(sc, lin, ang, pl.noise_samples_d.copy_to_host(), pl.u_cur_d.copy_to_host(), arith=dev,
+    pl = staged_rollout(eng, sc)
+    want = oracle_rollout_costs(sc, pl.lin_tdm, pl.ang_tdm, pl.noise_samples_d.copy_to_host(), pl.u_cur_d.copy_to_host(), arith=dev,
                                 wrap_clamp=True)
     assert_all_equal(pl.costs_nm_d.copy_to_host(), want, "generic kernel, no window")
 
@@ -90,15 +50,14 @@ def test_windowed_kernel_both_mask_variants(eng, dev, maskmax):
     if maskmax > 1:
         rng = np.random.default_rng(3)
         sc["obstacle"] = (sc["obstacle"].astype(np.int64) * rng.integers(1, maskmax + 1, sc["obstacle"].shape)).astype(np.int8)
-    pl, lin, ang = _planner_rollout(eng, sc)
-    want = oracle_rollout_costs(sc, lin, ang, pl.noise_samples_d.copy_to_host(), pl.u_cur_d.copy_to_host(), arith=dev,
+    pl = staged_rollout(eng, sc)
+    want = oracle_rollout_costs(sc, pl.lin_tdm, pl.ang_tdm, pl.noise_samples_d.copy_to_host(), pl.u_cur_d.copy_to_host(), arith=dev,
                                 ctrl_order="presummed", wrap_clamp=True)
     assert_all_equal(pl.costs_nm_d.copy_to_host(), want, "windowed kernel, mask max %d" % maskmax)
 
 
 # ----------------------------------------------------------------------------- raw C-ABI cases: any bounds, any origin
 def _raw_case(eng, dev, mode, N, M, T, cells, res, origin, lb, ab, x0, goal, seed, tol=0.5, vr=(0, 3)):
-    from tests.test_gpu_parity import RawPlanner
     rng = np.random.default_rng(seed)
     rp = RawPlanner(eng, mode, N, M, T, cells, cells)
     try:
@@ -152,13 +111,8 @@ def test_far_origins(eng, dev, mode, origin, res, cells, T, vr):
 def test_state_rollout_all_modes(eng, dev, mode):
     sc = make_scenario(mode, N=256, M=8, T=40, H=200, W=200, res=0.1, B=12, seed=6, warm_start=True)
     sc["cfg"]["num_vis_state_rollouts"] = 8
-    cfg = eng.Config(**sc["cfg"])
-    lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-    lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    pl = eng.MPPI_Numba(cfg)
-    pl.setup(sc["params"], lin, ang)
-    pl.u_cur_d.copy_to_device(sc["u0"])
+    pl = tdm_planner(eng, sc)
+    lin, ang = pl.lin_tdm, pl.ang_tdm
     pl.solve()
     got = pl.get_state_rollout()
     m = dict(tdm=MR.MODE_STOCHASTIC, det=MR.MODE_DET_DYN, spd=MR.MODE_SPEED_MAP)[mode]
@@ -175,12 +129,8 @@ def test_state_rollout_flushes_a_subnormal_heading(eng, dev):
     step, which the ftz oracle predicts and the non-ftz one does not."""
     sc = make_scenario("det", N=128, M=1, T=16, H=100, W=100, res=0.1, B=12, seed=7)
     sc["params"]["x0"] = np.array([5.03, 4.97, 1e-40])
-    cfg = eng.Config(**sc["cfg"])
-    lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-    lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    pl = eng.MPPI_Numba(cfg)
-    pl.setup(sc["params"], lin, ang)
+    pl = tdm_planner(eng, sc)
+    lin, ang = pl.lin_tdm, pl.ang_tdm
     pl.solve()
     u = np.zeros((16, 2), F32)
     u[:, 0] = 1.0
@@ -220,7 +170,8 @@ def test_config5_full_launch_on_a_subset_of_maps(eng, dev):
     """Config 5 (N 8192, M 256, T 128, 1024 x 1024 cells at 0.1 m): the kernel runs whole, the oracle checks 8 maps x all
     8192 control sequences."""
     sc = make_scenario("tdm", N=8192, M=256, T=128, H=1024, W=1024, res=0.1, B=12, seed=1, warm_start=True)
-    pl, lin, ang = _planner_rollout(eng, sc)
+    pl = staged_rollout(eng, sc)
+    lin, ang = pl.lin_tdm, pl.ang_tdm
     got = pl.costs_nm_d.copy_to_host()
     maps = np.array([0, 1, 37, 100, 128, 199, 254, 255])
     gl, ga = lin.sample_grid_batch_d.copy_to_host()[maps], ang.sample_grid_batch_d.copy_to_host()[maps]
@@ -232,7 +183,6 @@ def test_config5_full_launch_on_a_subset_of_maps(eng, dev):
 def test_config5_noise_draw_equals_oracle(eng, dev):
     """A whole config-5 noise draw (8192 x 128 x 2): every element equals the oracle's Box-Muller with the device's
     logf / cosf / sqrt.approx."""
-    from tests.test_gpu_parity import RawPlanner
     N, T = 8192, 128
     rp = RawPlanner(eng, 1, N, 1, T, 8, 8, seed=5)
     try:
@@ -243,37 +193,6 @@ def test_config5_noise_draw_equals_oracle(eng, dev):
         rp.close()
     want = MR.sample_noise(X.create_states(N * T, 5), [2.0, 3.0], N, T, arith=dev)
     assert_all_equal(got, want, "config 5 noise")
-
-
-def run_directed(eng, s, mode):
-    """A directed case (tests/directed_cases.py) through the C-ABI planner: uniform grids set directly, its bounds."""
-    from tests.test_gpu_parity import RawPlanner
-    N, T, R, Cc = s["N"], s["T"], s["R"], s["Cc"]
-    rp = RawPlanner(eng, mode, N, s["M"], T, R, Cc)
-    try:
-        lim = np.array([s["xlo"], s["xlo"] + Cc * s["res"]], F32)
-        dummy = np.zeros((2, R, Cc), np.int8)
-        dummy[1] = 100
-        rp.set_map("lin", dummy, [0.0, 1.0], s["lb"], s["res"], lim, lim, s["obs"], s["unk"], s["risk"] if mode == 2 else None)
-        rp.set_map("ang", dummy, [0.0, 1.0], s["ab"], s["res"], lim, lim, s["obs"], s["unk"], None)
-        rp.set_grids("lin", s["lin"][:rp.M])
-        rp.set_grids("ang", s["ang"][:rp.M])
-        rp.copy_in(eng._lib.BUF_NOISE, s["noise"])
-        rp.copy_in(eng._lib.BUF_U_CUR, s["u_cur"])
-        rp.set_params(x0=list(s["x0"]), xgoal=list(s["goal"]), goal_tolerance=s["tol"])
-        rp.call("rollout")
-        return rp.copy_out(eng._lib.BUF_COSTS_NM, (N, rp.M)) if mode == 0 else rp.copy_out(eng._lib.BUF_COSTS, (N,))[:, None]
-    finally:
-        rp.close()
-
-
-def directed_oracle(s, mode, arith):
-    lim = [s["xlo"], s["xlo"] + s["Cc"] * s["res"]]
-    return MR.rollout_costs(mode, s["lin"] if mode == 0 else s["lin"][:1], s["ang"] if mode == 0 else s["ang"][:1],
-                            s["lb"], s["ab"], s["obs"], s["unk"], s["res"], lim, lim, [0, 3], [-np.pi, np.pi], s["goal"],
-                            0.01, 1e5, 1e2, s["tol"], 1.0, [2, 3], s["x0"], 0.1, 1.0, s["noise"], s["u_cur"],
-                            risk_map=s["risk"][None], arith=arith, ctrl_order="presummed" if mode == 0 else "sequential",
-                            wrap_clamp=True)
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2])

@@ -20,24 +20,9 @@ from oracle import mppi_ref as MR          # noqa: E402
 from oracle import terrain_ref as TR       # noqa: E402
 from oracle import xoroshiro as X          # noqa: E402
 from tests import reduce_bounds as RB      # noqa: E402
+from tests.gpu_harness import (RawPlanner, assert_all_equal, assert_same, dev, eng,  # noqa: E402,F401
+                               staged_rollout, tdm_pair, tdm_planner)
 from tests.scenarios import make_scenario, oracle_rollout_costs   # noqa: E402
-from tests.test_gpu_exact_oracle import assert_all_equal           # noqa: E402
-
-
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__
-    __graft_entry__.build_engine()
-    import mppi_numba_b200 as E
-    assert E.device_count() >= 1, "GPU tests need a CUDA device"
-    return E
-
-
-@pytest.fixture(scope="module")
-def dev(eng):
-    """The exact oracle's arithmetic with this GPU's approximate operations and .ftz flushes."""
-    from oracle import arith as AR
-    return AR.Exact(AR.DeviceProvider(eng._lib), ftz=True)
 
 
 def load(golden_dir, name):
@@ -46,85 +31,6 @@ def load(golden_dir, name):
 
 def rel_err(a, b):
     return np.abs(a - b) / np.maximum(np.abs(b), 1e-6)
-
-
-# ----------------------------------------------------------------------------- raw C-ABI helpers
-class RawPlanner:
-    """Drives libb200mppi.so directly (no Python API objects): what a foreign-language binding would do."""
-
-    def __init__(self, E, mode, N, M, T, Rmax, Cmax, seed=1, thread_dim=(4, 4), V=1, rank=0, world=1):
-        L = E._lib
-        self.L, self.lib = L, L.lib
-        self.pod = L.ConfigPOD(num_steps=T, num_control_rollouts=N, num_grid_samples=M, max_map_rows=Rmax,
-                               max_map_cols=Cmax, tdm_thread_x=thread_dim[0], tdm_thread_y=thread_dim[1],
-                               num_vis_state_rollouts=V, mode=mode, device=0, rank=rank, world_size=world, seed=seed)
-        self.lin, self.ang, self.pl = C.c_void_p(), C.c_void_p(), C.c_void_p()
-        L.check(self.lib.b200mppi_tdm_create(C.byref(self.pod), C.byref(self.lin)))
-        L.check(self.lib.b200mppi_tdm_create(C.byref(self.pod), C.byref(self.ang)))
-        L.check(self.lib.b200mppi_planner_create(C.byref(self.pod), C.byref(self.pl)))
-        self.N, self.M, self.T, self.Rmax, self.Cmax = N, (M if mode == 0 else 1), T, Rmax, Cmax
-        self.n_local = N * (rank + 1) // world - N * rank // world
-
-    def close(self):
-        self.lib.b200mppi_planner_destroy(self.pl)
-        self.lib.b200mppi_tdm_destroy(self.lin)
-        self.lib.b200mppi_tdm_destroy(self.ang)
-
-    def set_map(self, which, pmf_padded, bin_values, bounds, res, pxl, pyl, obs=None, unk=None, risk=None):
-        L, t = self.L, (self.lin if which == "lin" else self.ang)
-        pmf = np.ascontiguousarray(pmf_padded, dtype=np.int8)
-        bv = np.ascontiguousarray(bin_values, dtype=np.float32)
-        bb = np.ascontiguousarray(bounds, dtype=np.float32)
-        xl = np.ascontiguousarray(pxl, dtype=np.float32)
-        yl = np.ascontiguousarray(pyl, dtype=np.float32)
-        L.check(self.lib.b200mppi_tdm_set_pmf(t, L.ptr(pmf), pmf.shape[0], pmf.shape[1], pmf.shape[2], L.ptr(bv),
-                                              L.ptr(bb), np.float32(res), L.ptr(xl), L.ptr(yl)))
-        if obs is not None:
-            o = np.ascontiguousarray(obs, dtype=np.int8)
-            u = np.ascontiguousarray(unk, dtype=np.int8)
-            L.check(self.lib.b200mppi_tdm_set_masks(t, L.ptr(o), L.ptr(u), o.shape[0], o.shape[1]))
-        if risk is not None:
-            r = np.ascontiguousarray(risk, dtype=np.int8)
-            L.check(self.lib.b200mppi_tdm_set_risk_map(t, L.ptr(r), r.shape[0], r.shape[1]))
-
-    def set_grids(self, which, g):
-        g = np.ascontiguousarray(g, dtype=np.int8)
-        self.L.check(self.lib.b200mppi_tdm_set_sample_grids(self.lin if which == "lin" else self.ang,
-                                                            self.L.ptr(g), g.nbytes))
-
-    def get_grids(self, which):
-        maps = self.M
-        out = np.empty((maps, self.Rmax, self.Cmax), dtype=np.int8)
-        self.L.check(self.lib.b200mppi_tdm_get_sample_grids(self.lin if which == "lin" else self.ang,
-                                                            self.L.ptr(out), out.nbytes))
-        return out
-
-    def set_params(self, **kw):
-        L = self.L
-        p = L.ParamsPOD()
-        d = dict(dt=0.1, x0=[0, 0, 0], xgoal=[0, 0], goal_tolerance=0.5, v_post_rollout=0.01, cvar_alpha=1.0,
-                 lambda_weight=1.0, u_std=[2, 3], vrange=[0, 3], wrange=[-np.pi, np.pi], obs_penalty=1e5,
-                 unknown_penalty=1e2, dist_weight=1.0, num_opt=1, alpha_dyn=1.0)
-        d.update(kw)
-        for k, v in d.items():
-            if k in ("x0", "xgoal", "u_std", "vrange", "wrange"):
-                setattr(p, k, L.c_floats(np.asarray(v, dtype=np.float32), len(v)))
-            else:
-                setattr(p, k, v)
-        L.check(self.lib.b200mppi_planner_set_tdms(self.pl, self.lin, self.ang))
-        L.check(self.lib.b200mppi_planner_set_params(self.pl, C.byref(p)))
-
-    def copy_in(self, buf, arr):
-        arr = np.ascontiguousarray(arr)
-        self.L.check(self.lib.b200mppi_planner_copy_in(self.pl, buf, self.L.ptr(arr), arr.nbytes))
-
-    def copy_out(self, buf, shape, dtype=np.float32):
-        out = np.empty(shape, dtype=dtype)
-        self.L.check(self.lib.b200mppi_planner_copy_out(self.pl, buf, self.L.ptr(out), out.nbytes))
-        return out
-
-    def call(self, name, *args):
-        self.L.check(getattr(self.lib, "b200mppi_planner_" + name)(self.pl, *args))
 
 
 # ----------------------------------------------------------------------------- 1. noise
@@ -251,21 +157,9 @@ def test_sampling_generic_path_ill_formed_pmf_and_large_alpha(eng):
 def test_long_horizon_uses_smaller_window(eng, dev):
     """T = 800 steps (> 700): the windowed kernel switches to its 224-row variant; every cost equals the exact oracle."""
     sc = make_scenario("tdm", N=128, M=4, T=800, H=200, W=200, res=0.2, B=5, seed=14, warm_start=True)
-    cfg = eng.Config(**sc["cfg"])
-    assert cfg.num_steps == 800
-    lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-    lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    pl = eng.MPPI_Numba(cfg)
-    pl.setup(sc["params"], lin, ang)
-    pl.u_cur_d.copy_to_device(sc["u0"])
-    pl.move_mppi_task_vars_to_device()
-    L = eng._lib
-    lin.sample_grids(1.0)
-    ang.sample_grids(1.0)
-    L.check(L.lib.b200mppi_planner_sample_noise(pl._handle))
-    L.check(L.lib.b200mppi_planner_rollout(pl._handle))
-    want = oracle_rollout_costs(sc, lin, ang, pl.noise_samples_d.copy_to_host(), pl.u_cur_d.copy_to_host(), arith=dev,
+    pl = staged_rollout(eng, sc)
+    assert pl.cfg.num_steps == 800
+    want = oracle_rollout_costs(sc, pl.lin_tdm, pl.ang_tdm, pl.noise_samples_d.copy_to_host(), pl.u_cur_d.copy_to_host(), arith=dev,
                                 ctrl_order="presummed", wrap_clamp=True)
     assert_all_equal(pl.costs_nm_d.copy_to_host(), want, "T 800")
     assert pl.solve().shape == (800, 2)
@@ -349,26 +243,13 @@ def test_rollouts_vs_reference_golden(eng, golden_dir, gname):
 def test_rollout_costs_vs_oracle(eng, dev, mode, N, M, T, H, res, B, near, warm):
     sc = make_scenario(mode, N=N, M=M, T=T, H=H, W=H, res=res, B=B, seed=4, near_goal=near, warm_start=warm,
                        det_alpha=0.3 if B == 32 else 1.0)
-    cfg = eng.Config(**sc["cfg"])
-    assert cfg.num_steps == T
-    lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-    lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    pl = eng.MPPI_Numba(cfg)
-    pl.setup(sc["params"], lin, ang)
-    if warm:
-        pl.u_cur_d.copy_to_device(sc["u0"])
-    pl.move_mppi_task_vars_to_device()
-    L = eng._lib
-    lin.sample_grids(1.0)
-    ang.sample_grids(1.0)
-    L.check(L.lib.b200mppi_planner_sample_noise(pl._handle))
-    L.check(L.lib.b200mppi_planner_rollout(pl._handle))
+    pl = staged_rollout(eng, sc)                          # warm-started from sc["u0"] exactly when `warm`
+    assert pl.cfg.num_steps == T
     noise = pl.noise_samples_d.copy_to_host()
     u_cur = pl.u_cur_d.copy_to_host()
     # the windowed kernel (stochastic mode) adds the pre-summed control cost, the deterministic kernels add the terms
     # one by one: the exact oracle in each kernel's order, every (n, m) equal
-    want = oracle_rollout_costs(sc, lin, ang, noise, u_cur, arith=dev, wrap_clamp=True,
+    want = oracle_rollout_costs(sc, pl.lin_tdm, pl.ang_tdm, noise, u_cur, arith=dev, wrap_clamp=True,
                                 ctrl_order="presummed" if mode == "tdm" else "sequential")
     if mode == "tdm":
         got = pl.costs_nm_d.copy_to_host()
@@ -394,24 +275,11 @@ def test_window_kernel_equals_generic_kernel(eng, monkeypatch, maskmax):
         rng = np.random.default_rng(3)
         sc["obstacle"] = (sc["obstacle"].astype(np.int64) * rng.integers(1, maskmax + 1, sc["obstacle"].shape)).astype(sc["obstacle"].dtype)
         assert sc["obstacle"].max() > 1
-    L = eng._lib
     outs = []
-    noise = grids = None
     for no_win in (False, True):
         if no_win:
             monkeypatch.setenv("B200MPPI_NO_WINDOW", "1")
-        cfg = eng.Config(**sc["cfg"])
-        lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-        lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        pl = eng.MPPI_Numba(cfg)
-        pl.setup(sc["params"], lin, ang)
-        pl.u_cur_d.copy_to_device(sc["u0"])
-        pl.move_mppi_task_vars_to_device()
-        lin.sample_grids(1.0)
-        ang.sample_grids(1.0)
-        L.check(L.lib.b200mppi_planner_sample_noise(pl._handle))
-        L.check(L.lib.b200mppi_planner_rollout(pl._handle))
+        pl = staged_rollout(eng, sc)
         outs.append(pl.costs_nm_d.copy_to_host())
     monkeypatch.delenv("B200MPPI_NO_WINDOW")
     r = rel_err(outs[0], outs[1])
@@ -602,6 +470,13 @@ def _sharded_update(eng, kind):
             rp.close()
 
 
+def _rank_planner(eng, sc, rank, world):
+    """(planner, lin, ang) of scenario sc as rank `rank` of `world`, its params on the device."""
+    pl = tdm_planner(eng, sc, rank=rank, world_size=world)
+    pl.move_mppi_task_vars_to_device()
+    return pl, pl.lin_tdm, pl.ang_tdm
+
+
 def test_map_sharded_solve_equals_single_rank(eng):
     """MODE_TDM on 2 'ranks' (both on this GPU, the all-to-all / all-gather done by hand): each rank's
     sampled maps are bit-identical to its slice of the single-rank maps, its CVaR costs are bit-identical
@@ -610,23 +485,11 @@ def test_map_sharded_solve_equals_single_rank(eng):
     L = eng._lib
     ws = 2
     sc = make_scenario("tdm", N=256, M=16, T=32, H=120, W=120, res=0.2, B=8, seed=10, warm_start=True)
-
-    def build(rank, world):
-        cfg = eng.Config(**sc["cfg"])
-        lin = eng.TDM_Numba(cfg, rank=rank, world_size=world)
-        ang = eng.TDM_Numba(cfg, rank=rank, world_size=world)
-        lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        pl = eng.MPPI_Numba(cfg, rank=rank, world_size=world)
-        pl.setup(sc["params"], lin, ang)
-        pl.u_cur_d.copy_to_device(sc["u0"])
-        pl.move_mppi_task_vars_to_device()
-        return pl, lin, ang
-    single, slin, sang = build(0, 1)
+    single, slin, sang = _rank_planner(eng, sc, 0, 1)
     u_single = single.solve()
     maps_single = slin.sample_grid_batch_d.copy_to_host()
     costs_single = single.costs_d.copy_to_host()
-    ranks = [build(r, ws) for r in range(ws)]
+    ranks = [_rank_planner(eng, sc, r, ws) for r in range(ws)]
     N, M = sc["N"], sc["M"]
     sends = []
     for r, (pl, lin, ang) in enumerate(ranks):
@@ -669,20 +532,8 @@ def test_p2p_exchange_equals_single_rank(eng, mode, ws):
     L = eng._lib
     sc = make_scenario(mode, N=512, M=16 if mode == "tdm" else 1, T=32, H=120, W=120, res=0.2, B=8, seed=14,
                        warm_start=True)
-
-    def build(rank, world):
-        cfg = eng.Config(**sc["cfg"])
-        lin = eng.TDM_Numba(cfg, rank=rank, world_size=world)
-        ang = eng.TDM_Numba(cfg, rank=rank, world_size=world)
-        lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        pl = eng.MPPI_Numba(cfg, rank=rank, world_size=world)
-        pl.setup(sc["params"], lin, ang)
-        pl.u_cur_d.copy_to_device(sc["u0"])
-        pl.move_mppi_task_vars_to_device()
-        return pl, lin, ang
-    single = build(0, 1)
-    ranks = [build(r, ws) for r in range(ws)]
+    single = _rank_planner(eng, sc, 0, 1)
+    ranks = [_rank_planner(eng, sc, r, ws) for r in range(ws)]
     pls = [r[0] for r in ranks]
     _connect_local(L, pls)
     N = sc["N"]
@@ -715,16 +566,7 @@ def test_p2p_wait_times_out_instead_of_hanging(eng, monkeypatch):
     L = eng._lib
     monkeypatch.setenv("B200MPPI_P2P_TIMEOUT_MS", "50")
     sc = make_scenario("det", N=256, M=1, T=16, H=60, W=60, res=0.2, B=4, seed=15)
-    pls = []
-    for r in range(2):
-        cfg = eng.Config(**sc["cfg"])
-        lin, ang = eng.TDM_Numba(cfg, rank=r, world_size=2), eng.TDM_Numba(cfg, rank=r, world_size=2)
-        lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        pl = eng.MPPI_Numba(cfg, rank=r, world_size=2)
-        pl.setup(sc["params"], lin, ang)
-        pl.move_mppi_task_vars_to_device()
-        pls.append((pl, lin, ang))
+    pls = [_rank_planner(eng, sc, r, 2) for r in range(2)]
     _connect_local(L, [p[0] for p in pls])
     pl = pls[0][0]
     L.check(L.lib.b200mppi_planner_solve_local(pl._handle, 1))
@@ -736,31 +578,35 @@ def test_p2p_wait_times_out_instead_of_hanging(eng, monkeypatch):
 
 
 # ----------------------------------------------------------------------------- 5. whole solve through the public API
-@pytest.mark.parametrize("mode", ["tdm", "det", "spd"])
-def test_solve_vs_reference_golden(eng, golden_dir, mode):
-    """Config -> TDM setters -> setup -> solve -> shift_and_update -> solve, the reference's public call
-    sequence, against what the reference itself returned for the same seed (ref_solve.npz)."""
-    g = load(golden_dir, "ref_solve.npz")
+def _golden_solve_planner(eng, g, mode, **cfg_kw):
+    """(planner, lin, ang) of the ref_solve.npz scenario in `mode`, set up as the reference's public calls set it up."""
     flags = dict(tdm=dict(use_tdm=True), det=dict(use_det_dynamics=True),
                  spd=dict(use_nom_dynamics_with_speed_map=True))[mode]
     cfg = eng.Config(T=float(g["T_s"]), dt=float(g["dt"]), num_grid_samples=int(g["M"]),
                      num_control_rollouts=int(g["N"]), seed=int(g["seed"]),
                      max_map_dim=tuple(int(v) for v in g["max_map_dim"]),
                      tdm_sample_thread_dim=tuple(int(v) for v in g["thread_dim"]),
-                     max_speed_padding=float(g["max_speed_padding"]), **flags)
+                     max_speed_padding=float(g["max_speed_padding"]), **cfg_kw, **flags)
     H, W = g["obstacle"].shape
     res = float(g["res"])
     d = dict(res=res, xlimits=np.array([0.0, W * res]), ylimits=np.array([0.0, H * res]),
              bin_values=g["bin_values"], bin_values_bounds=np.array([0.0, 1.0]), det_dynamics_cvar_alpha=0.4)
-    lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-    lin.set_TDM_from_PMF_grid(g["pmf_lin"], d, g["obstacle"], g["unknown"])
-    ang.set_TDM_from_PMF_grid(g["pmf_ang"], d, g["obstacle"], g["unknown"])
+    lin, ang = tdm_pair(eng, cfg, g["pmf_lin"], g["pmf_ang"], d, g["obstacle"], g["unknown"])
     pl = eng.MPPI_Numba(cfg)
     p = dict(dt=0.1, x0=np.array([2.3, 3.1, 0.3]), xgoal=np.array([5.0, 4.5]), goal_tolerance=0.5,
              v_post_rollout=0.01, cvar_alpha=0.5, alpha_dyn=1.0, dist_weight=1.0, lambda_weight=1.0, num_opt=1,
              u_std=np.array([2.0, 3.0]), vrange=np.array([0.0, 3.0]), wrange=np.array([-np.pi, np.pi]),
              obs_penalty=1e5, unknown_penalty=1e2)
     pl.setup(p, lin, ang)
+    return pl, lin, ang
+
+
+@pytest.mark.parametrize("mode", ["tdm", "det", "spd"])
+def test_solve_vs_reference_golden(eng, golden_dir, mode):
+    """Config -> TDM setters -> setup -> solve -> shift_and_update -> solve, the reference's public call
+    sequence, against what the reference itself returned for the same seed (ref_solve.npz)."""
+    g = load(golden_dir, "ref_solve.npz")
+    pl, lin, ang = _golden_solve_planner(eng, g, mode)
     u1 = pl.solve()
     assert (lin.sample_grid_batch_d.copy_to_host() == g[mode + "_lin_grid1"]).all()
     assert (ang.sample_grid_batch_d.copy_to_host() == g[mode + "_ang_grid1"]).all()
@@ -780,26 +626,8 @@ def test_state_rollout_vs_reference_golden(eng, dev, golden_dir, mode):
     own buffers."""
     g = load(golden_dir, "ref_solve.npz")
     s = load(golden_dir, "ref_state_rollout.npz")
-    flags = dict(tdm=dict(use_tdm=True), det=dict(use_det_dynamics=True),
-                 spd=dict(use_nom_dynamics_with_speed_map=True))[mode]
-    cfg = eng.Config(T=float(g["T_s"]), dt=float(g["dt"]), num_grid_samples=int(g["M"]),
-                     num_control_rollouts=int(g["N"]), seed=int(g["seed"]),
-                     max_map_dim=tuple(int(v) for v in g["max_map_dim"]),
-                     tdm_sample_thread_dim=tuple(int(v) for v in g["thread_dim"]),
-                     max_speed_padding=float(g["max_speed_padding"]), num_vis_state_rollouts=5, **flags)
-    H, W = g["obstacle"].shape
-    res = float(g["res"])
-    d = dict(res=res, xlimits=np.array([0.0, W * res]), ylimits=np.array([0.0, H * res]),
-             bin_values=g["bin_values"], bin_values_bounds=np.array([0.0, 1.0]), det_dynamics_cvar_alpha=0.4)
-    lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-    lin.set_TDM_from_PMF_grid(g["pmf_lin"], d, g["obstacle"], g["unknown"])
-    ang.set_TDM_from_PMF_grid(g["pmf_ang"], d, g["obstacle"], g["unknown"])
-    pl = eng.MPPI_Numba(cfg)
-    p = dict(dt=0.1, x0=np.array([2.3, 3.1, 0.3]), xgoal=np.array([5.0, 4.5]), goal_tolerance=0.5,
-             v_post_rollout=0.01, cvar_alpha=0.5, alpha_dyn=1.0, dist_weight=1.0, lambda_weight=1.0, num_opt=1,
-             u_std=np.array([2.0, 3.0]), vrange=np.array([0.0, 3.0]), wrange=np.array([-np.pi, np.pi]),
-             obs_penalty=1e5, unknown_penalty=1e2)
-    pl.setup(p, lin, ang)
+    pl, lin, ang = _golden_solve_planner(eng, g, mode, num_vis_state_rollouts=5)
+    res, p = float(g["res"]), pl.params
     pl.solve()
     got = pl.get_state_rollout()
     assert got.shape == s[mode + "_states"].shape
@@ -911,16 +739,8 @@ def test_full_size_config5_properties(eng, dev):
     from bench import build_scenario
     sc = build_scenario("c5")
     L = eng._lib
-
-    def build():
-        cfg = eng.Config(**sc["cfg"])
-        lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-        lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        pl = eng.MPPI_Numba(cfg)
-        pl.setup(sc["params"], lin, ang)
-        return pl, lin, ang
-    a, alin, aang = build()
+    a = tdm_planner(eng, sc)
+    alin = a.lin_tdm
     u1 = a.solve()
     u2 = a.solve()
     cnm = a.costs_nm_d.copy_to_host()
@@ -944,7 +764,8 @@ def test_full_size_config5_properties(eng, dev):
     got_top = float((g[:8, pad:-pad, pad:-pad] == q[-1]).mean())
     assert abs(got_top - exp_top) < 2e-3
     # determinism: a second engine with the same seed reproduces both solves bit for bit
-    b, blin, bang = build()
+    b = tdm_planner(eng, sc)
+    blin, bang = b.lin_tdm, b.ang_tdm
     assert (b.solve() == u1).all() and (b.solve() == u2).all()
     # oracle parity on a slice of the second solve's inputs
     noise = b.noise_samples_d.copy_to_host()[:256]
@@ -956,22 +777,13 @@ def test_full_size_config5_properties(eng, dev):
 
 def test_determinism_and_checkpoint_resume(eng):
     sc = make_scenario("tdm", N=256, M=16, T=32, H=100, W=100, res=0.2, B=8, seed=6)
-
-    def build():
-        cfg = eng.Config(**sc["cfg"])
-        lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-        lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        pl = eng.MPPI_Numba(cfg)
-        pl.setup(sc["params"], lin, ang)
-        return pl, lin, ang
-    a, *_ka = build()
-    b, *_kb = build()
+    a = tdm_planner(eng, sc)
+    b = tdm_planner(eng, sc)
     ua = [a.solve() for _ in range(3)]
     ub = [b.solve() for _ in range(2)]
     assert (ua[0] == ub[0]).all() and (ua[1] == ub[1]).all()     # same seed -> bit-identical, run to run
     st = b.get_state()
-    c, *_kc = build()
+    c = tdm_planner(eng, sc)
     c.set_state(st)
     assert (c.solve() == ua[2]).all()                            # resume from checkpoint == uninterrupted
     assert not (ua[0] == ua[1]).all()                            # streams advance between solves
@@ -981,27 +793,13 @@ def test_oversized_map_count_solve(eng, capsys):
     """num_grid_samples > 1024: solve() dispatches to solve_stochastic_oversized (mppi.py:199-203) and equals
     the stage-by-stage replay through the C-ABI, whose CVaR stage is checked against the oracle's sort."""
     sc = make_scenario("tdm", N=128, M=1030, T=16, H=40, W=40, res=0.25, B=6, seed=21, cvar_alpha=0.3)
-
-    def build():
-        cfg = eng.Config(**sc["cfg"])
-        lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-        lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-        pl = eng.MPPI_Numba(cfg)
-        pl.setup(sc["params"], lin, ang)
-        return pl, lin, ang
-    a, *_ka = build()
+    a = tdm_planner(eng, sc)
     assert "oversized kernel" in capsys.readouterr().out          # Config's warning, like the reference's
     assert a.cfg.num_grid_samples == 1030
     u = a.solve()
     assert u.shape == (16, 2) and np.isfinite(u).all()
-    b, lin, ang = build()
+    b = staged_rollout(eng, sc)
     L = eng._lib
-    b.move_mppi_task_vars_to_device()
-    lin.sample_grids(1.0)
-    ang.sample_grids(1.0)
-    for stage in ("sample_noise", "rollout"):
-        L.check(getattr(L.lib, "b200mppi_planner_" + stage)(b._handle))
     nm = b.costs_nm_d.copy_to_host()
     cv = b.costs_d.copy_to_host()
     RB.check_cvar(cv, nm, 0.3, label="oversized")
@@ -1014,17 +812,12 @@ def test_closed_loop_reaches_goal(eng):
     """The reference's test.ipynb scenario in miniature: receding-horizon loop on the mean-traction map
     until the goal tolerance is met (SURVEY.md section 4-iv)."""
     sc = make_scenario("det", N=512, M=1, T=40, H=60, W=60, res=0.25, B=6, seed=12, mask_p=0.0)
-    cfg = eng.Config(**sc["cfg"])
-    lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-    lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"])
-    ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"])
     p = dict(sc["params"])
     p["x0"] = np.array([3.0, 3.0, 0.0])
     p["xgoal"] = np.array([10.0, 10.0])
     p["num_opt"] = 2
-    pl = eng.MPPI_Numba(cfg)
-    pl.setup(p, lin, ang)
-    bv = lin.bin_values
+    pl = tdm_planner(eng, dict(sc, obstacle=None, unknown=None), params=p)     # no masks
+    bv = pl.lin_tdm.bin_values
     mean_l = (sc["pmf_lin"].astype(float) * bv[:, None, None]).sum(0) / 100
     mean_a = (sc["pmf_ang"].astype(float) * bv[:, None, None]).sum(0) / 100
     world = eng.TractionGrid(mean_l, mean_a, res=0.25)
@@ -1042,19 +835,6 @@ def test_closed_loop_reaches_goal(eng):
 
 
 # ----------------------------------------------------------------------------- reach-box map sampling
-def _tdm_planner(eng, sc, monkeypatch, box):
-    monkeypatch.setenv("B200MPPI_SAMPLE_BOX", box)           # read when the planner handle is created
-    cfg = eng.Config(**sc["cfg"])
-    lin, ang = eng.TDM_Numba(cfg), eng.TDM_Numba(cfg)
-    lin.set_TDM_from_PMF_grid(sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    ang.set_TDM_from_PMF_grid(sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    pl = eng.MPPI_Numba(cfg)
-    pl.setup(sc["params"], lin, ang)
-    if "u0" in sc:
-        pl.u_cur_d.copy_to_device(sc["u0"])
-    return cfg, lin, ang, pl
-
-
 @pytest.mark.parametrize("N,M,T,H,res,warm,tdim,diverge", [
     # BASELINE config 3
     pytest.param(1024, 64, 64, 512, 0.1, False, (16, 16), False, id="1024-64-64-512-0.1-False-tdim0"),
@@ -1075,7 +855,8 @@ def test_boxed_solve_identical_to_whole_map_solve(eng, monkeypatch, N, M, T, H, 
     sc = make_scenario("tdm", N=N, M=M, T=T, H=H, W=H, res=res, B=12, seed=11, warm_start=warm, thread_dim=tdim)
     runs = {}
     for box in ("off", "static", "dynamic"):
-        cfg, lin, ang, pl = _tdm_planner(eng, sc, monkeypatch, box)
+        pl = tdm_planner(eng, sc, box=box, monkeypatch=monkeypatch)
+        lin, ang = pl.lin_tdm, pl.ang_tdm
         if diverge:
             lin.sample_grids(sc["params"]["alpha_dyn"])
         x0 = sc["params"]["x0"].copy()
@@ -1085,13 +866,14 @@ def test_boxed_solve_identical_to_whole_map_solve(eng, monkeypatch, N, M, T, H, 
             u = pl.solve()
             launches.append(pl.launch_count() - l0)
             modes.append(pl.sample_box())
-            hist.append((u.copy(), pl.costs_d.copy_to_host(), pl.costs_nm_d.copy_to_host()))
+            hist.append(dict(u=u.copy(), costs=pl.costs_d.copy_to_host(), costs_nm=pl.costs_nm_d.copy_to_host()))
             x0 = x0 + np.array([0.37, -0.21, 0.05])
             pl.shift_and_update(x0, u, 1)
-        runs[box] = dict(hist=hist, modes=modes, launches=launches, lin_rng=lin.rng_states_d.copy_to_host(),
-                         ang_rng=ang.rng_states_d.copy_to_host(), rng=pl.rng_states_d.copy_to_host(),
-                         noise=pl.noise_samples_d.copy_to_host(), lin_grid=lin.sample_grid_batch_d.copy_to_host(),
-                         ang_grid=ang.sample_grid_batch_d.copy_to_host())
+        runs[box] = dict(hist=hist, modes=modes, launches=launches,
+                         state=dict(lin_rng=lin.rng_states_d.copy_to_host(), ang_rng=ang.rng_states_d.copy_to_host(),
+                                    rng=pl.rng_states_d.copy_to_host(), noise=pl.noise_samples_d.copy_to_host(),
+                                    lin_grid=lin.sample_grid_batch_d.copy_to_host(),
+                                    ang_grid=ang.sample_grid_batch_d.copy_to_host()))
     ref = runs["off"]
     assert all(m[0] == 0 for m in ref["modes"])
     # a box that would leave the map is not used (whole maps); the box from the controls is the tighter one.
@@ -1117,12 +899,9 @@ def test_boxed_solve_identical_to_whole_map_solve(eng, monkeypatch, N, M, T, H, 
     Hp = H + 2 * int(np.ceil(5.0 * 0.1 / res))
     for box in ("static", "dynamic"):
         r = runs[box]
-        for k, ((u, c, cnm), (u0, c0, cnm0)) in enumerate(zip(r["hist"], ref["hist"])):
-            assert (cnm == cnm0).all(), (box, k)
-            assert (c == c0).all(), (box, k)
-            assert (u == u0).all(), (box, k)
-        for key in ("lin_rng", "ang_rng", "rng", "noise", "lin_grid", "ang_grid"):
-            assert (r[key] == ref[key]).all(), (box, key)
+        for k, (h, h0) in enumerate(zip(r["hist"], ref["hist"])):
+            assert_same(h, h0, "box %s, solve %d" % (box, k))
+        assert_same(r["state"], ref["state"], "box %s" % box)
     # the dynamic box is the smaller one, and a real restriction
     ms, md = runs["static"]["modes"][-1], runs["dynamic"]["modes"][-1]
     area = lambda m: (m[2] - m[1]) * (m[4] - m[3])
@@ -1136,19 +915,21 @@ def test_boxed_solve_falls_back_near_the_map_edge_and_for_several_iterations(eng
     solve's controls (the maps are sampled once for several noise draws) and takes the static bound."""
     sc = make_scenario("tdm", N=256, M=16, T=32, H=200, W=200, res=0.1, B=12, seed=5, thread_dim=(4, 4))
     sc["params"]["x0"] = np.array([1.0, 10.0, 0.3])                 # 10 cells from the left edge: reach > 10 cells
-    cfg, lin, ang, pl = _tdm_planner(eng, sc, monkeypatch, "dynamic")
+    pl = tdm_planner(eng, sc, box="dynamic", monkeypatch=monkeypatch)
     assert pl.solve() is not None
     assert pl.sample_box()[0] == 0
     sc["params"]["x0"] = np.array([10.0, 10.0, 0.3])
     sc["params"]["num_opt"] = 2
     sc["params"]["vrange"] = np.array([0.0, 1.0])                   # static reach 3.2 m = 32 cells: inside the 20 m map
-    cfg, lin, ang, pl = _tdm_planner(eng, sc, monkeypatch, "dynamic")
+    pl = tdm_planner(eng, sc, box="dynamic", monkeypatch=monkeypatch)
     u = pl.solve()
     assert pl.sample_box()[0] == 1
-    cfg, lin2, ang2, pl2 = _tdm_planner(eng, sc, monkeypatch, "off")
-    assert (pl2.solve() == u).all()
-    assert (lin.sample_grid_batch_d.copy_to_host() == lin2.sample_grid_batch_d.copy_to_host()).all()
-    assert (lin.rng_states_d.copy_to_host() == lin2.rng_states_d.copy_to_host()).all()
+    pl2 = tdm_planner(eng, sc, box="off", monkeypatch=monkeypatch)
+    u2 = pl2.solve()
+    lin, lin2 = pl.lin_tdm, pl2.lin_tdm
+    assert_same(dict(u=u2, lin_map=lin2.sample_grid_batch_d.copy_to_host(), lin_rng=lin2.rng_states_d.copy_to_host()),
+                dict(u=u, lin_map=lin.sample_grid_batch_d.copy_to_host(), lin_rng=lin.rng_states_d.copy_to_host()),
+                "whole maps against the static box")
 
 
 def test_state_rollout_and_public_sampling_after_boxed_solve(eng, monkeypatch):
@@ -1157,7 +938,8 @@ def test_state_rollout_and_public_sampling_after_boxed_solve(eng, monkeypatch):
     sc = make_scenario("tdm", N=256, M=16, T=48, H=240, W=240, res=0.1, B=12, seed=9, thread_dim=(5, 6))
     out = {}
     for box in ("off", "dynamic"):
-        cfg, lin, ang, pl = _tdm_planner(eng, sc, monkeypatch, box)
+        pl = tdm_planner(eng, sc, box=box, monkeypatch=monkeypatch)
+        lin, ang = pl.lin_tdm, pl.ang_tdm
         pl.solve()
         if box == "dynamic":
             assert pl.sample_box()[0] == 2
@@ -1167,9 +949,9 @@ def test_state_rollout_and_public_sampling_after_boxed_solve(eng, monkeypatch):
         cnm = pl.costs_nm_d.copy_to_host()
         pl.solve()                                                      # boxed again
         g2 = lin.sample_grids(1.0).copy_to_host()                       # public call: whole fresh maps
-        out[box] = (st, cnm, g2, ang.rng_states_d.copy_to_host(), lin.rng_states_d.copy_to_host())
-    for a, b in zip(out["off"], out["dynamic"]):
-        assert (a == b).all()
+        out[box] = dict(state_rollout=st, costs_nm=cnm, lin_map=g2, ang_rng=ang.rng_states_d.copy_to_host(),
+                        lin_rng=lin.rng_states_d.copy_to_host())
+    assert_same(out["off"], out["dynamic"], "after a boxed solve")
 
 
 def test_sampler_wide_thread_tiles(eng):

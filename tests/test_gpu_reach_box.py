@@ -6,26 +6,12 @@ robot move up to twice as far as its exact path -- and at the reach disc's edge 
 Before every sampling both TDMs' sampled maps are filled with byte 0 (traction 0) while every sampled cell decodes to
 traction 1 inside the map: a rollout that reads a cell the boxed launch did not write stops there, which changes its
 cost."""
-import contextlib
-import io
-
 import numpy as np
 import pytest
 
+from tests.gpu_harness import assert_same, eng, quiet, tdm_planner  # noqa: F401
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__
-    __graft_entry__.build_engine()
-    import mppi_numba_b200 as E
-    assert E.device_count() >= 1, "GPU tests need a CUDA device"
-    return E
-
-
-def _quiet():
-    return contextlib.redirect_stdout(io.StringIO())
 
 
 # origin (both axes), res, map cells a side, T, start inside the map (m), heading, vrange, u_cur[v], u_std[v]
@@ -45,7 +31,7 @@ def scenario(case, seed=3, heading=None):
                num_vis_state_rollouts=4, use_tdm=True)
     pmf = np.zeros((2, cells, cells), dtype=np.int8)
     pmf[1] = 100                                             # every map cell: traction 1 (padding: bin 0, traction 0)
-    zero = np.zeros((cells, cells), dtype=np.int8)
+    zero = np.zeros((cells, cells), dtype=np.int8)           # no obstacle, nothing unknown
     lim = np.array([origin, origin + cells * res])
     tdm_dict = dict(res=res, xlimits=lim, ylimits=lim, bin_values=np.array([0.0, 1.0]),
                     bin_values_bounds=np.array([0.0, 1.0]), det_dynamics_cvar_alpha=1.0)
@@ -55,21 +41,13 @@ def scenario(case, seed=3, heading=None):
                   vrange=np.array(vr), wrange=np.array([0.0, 0.0]))
     u0 = np.zeros((T, 2), dtype=np.float32)
     u0[:, 0] = u
-    return dict(cfg=cfg, pmf=pmf, zero=zero, tdm_dict=tdm_dict, params=params, u0=u0, T=T, res=res, cells=cells,
-                lim=lim)
+    return dict(cfg=cfg, pmf_lin=pmf, pmf_ang=pmf, obstacle=zero, unknown=zero, tdm_dict=tdm_dict, params=params, u0=u0,
+                T=T, res=res, cells=cells, lim=lim)
 
 
 def planner(E, sc, box, monkeypatch):
-    monkeypatch.setenv("B200MPPI_SAMPLE_BOX", box)           # read when the planner handle is created
-    with _quiet():
-        cfg = E.Config(**sc["cfg"])
-        lin, ang = E.TDM_Numba(cfg), E.TDM_Numba(cfg)
-        lin.set_TDM_from_PMF_grid(sc["pmf"], sc["tdm_dict"], sc["zero"], sc["zero"])
-        ang.set_TDM_from_PMF_grid(sc["pmf"], sc["tdm_dict"], sc["zero"], sc["zero"])
-        pl = E.MPPI_Numba(cfg)
-        pl.setup(dict(sc["params"]), lin, ang)
-    pl.u_cur_d.copy_to_device(sc["u0"])
-    return pl
+    with quiet():
+        return tdm_planner(E, sc, box=box, monkeypatch=monkeypatch)
 
 
 def zero_maps(pl):
@@ -81,7 +59,7 @@ def closed_loop(E, sc, box, monkeypatch, solves=3):
     pl = planner(E, sc, box, monkeypatch)
     hist, boxes = [], []
     x = np.asarray(sc["params"]["x0"], dtype=np.float64)
-    with _quiet():
+    with quiet():
         for _ in range(solves):
             zero_maps(pl)
             u = pl.solve()
@@ -105,9 +83,7 @@ def assert_boxed_equals_off(E, sc, monkeypatch):
         side = sc["cells"] + 2 * int(np.ceil(0.5 / sc["res"]))
         assert all(b[2] - b[1] < side and b[4] - b[3] < side for b in boxes), (box, boxes)
         for k, (h, h0) in enumerate(zip(hist, ref)):
-            for key in h0:
-                assert np.array_equal(h[key], h0[key]), "%s solve %d: %s differs from whole-map sampling (box %s)" \
-                    % (box, k, key, boxes[k])
+            assert_same(h, h0, "%s solve %d, against whole-map sampling (box %s)" % (box, k, boxes[k]))
 
 
 @pytest.mark.parametrize("case", ["far", "utm"])
@@ -142,7 +118,7 @@ def test_device_decided_box_far_origin(eng, monkeypatch):
                                 xlimits=tuple(sc["lim"]), ylimits=tuple(sc["lim"])) for sc in scs]
         for p in pls:
             zero_maps(p)
-        with _quiet():
+        with quiet():
             out = E.MPPI_StochasticBatch(pls).run_stochastic_trials(grids, 4)
         assert list(out["steps"]) == [4, 4], out["status"]
         runs[box] = dict(xhist=out["xhist"], uhist=out["uhist"], boxes=[p.sample_box() for p in pls],
@@ -152,18 +128,17 @@ def test_device_decided_box_far_origin(eng, monkeypatch):
                                      ang_map=p.ang_tdm.sample_grid_batch_d.copy_to_host()) for p in pls])
     assert all(b[0] == 0 for b in runs["off"]["boxes"])
     assert all(b[0] == 2 for b in runs["dynamic"]["boxes"]), runs["dynamic"]["boxes"]
-    for key in ("xhist", "uhist"):
-        assert np.array_equal(runs["dynamic"][key], runs["off"][key]), key
+    assert_same({key: runs["dynamic"][key] for key in ("xhist", "uhist")},
+                {key: runs["off"][key] for key in ("xhist", "uhist")}, "trials")
     for k in range(2):
-        for key, v in runs["off"]["state"][k].items():
-            assert np.array_equal(runs["dynamic"]["state"][k][key], v), "trials, planner %d: %s" % (k, key)
+        assert_same(runs["dynamic"]["state"][k], runs["off"]["state"][k], "trials, planner %d" % k)
 
     solved = {}
     for box in ("off", "dynamic"):
         pls, _ = _batch_twins(E, box, monkeypatch)
         batch = E.MPPI_StochasticBatch(pls)
         hist = []
-        with _quiet():
+        with quiet():
             for r in range(3):
                 for p in pls:
                     zero_maps(p)
@@ -180,7 +155,8 @@ def test_device_decided_box_far_origin(eng, monkeypatch):
         solved[box] = hist
     for r, (h, h0) in enumerate(zip(solved["dynamic"], solved["off"])):
         assert h["boxes"] == [2, 2] and h0["boxes"] == [0, 0], (h["boxes"], h0["boxes"])
-        assert np.array_equal(h["u"], h0["u"]), "batch solve round %d: u differs" % r
-        for key in ("costs_nm", "costs", "rng", "lin_rng"):
-            for k in range(2):
-                assert np.array_equal(h[key][k], h0[key][k]), "batch solve round %d planner %d: %s" % (r, k, key)
+        assert_same(dict(u=h["u"]), dict(u=h0["u"]), "batch solve round %d" % r)
+        for k in range(2):
+            keys = ("costs_nm", "costs", "rng", "lin_rng")
+            assert_same({key: h[key][k] for key in keys}, {key: h0[key][k] for key in keys},
+                        "batch solve round %d planner %d" % (r, k))

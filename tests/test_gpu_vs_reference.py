@@ -20,6 +20,8 @@ import sys
 import numpy as np
 import pytest
 
+from tests.gpu_harness import assert_all_equal, directed_oracle, quiet, run_directed, tdm_planner
+
 pytestmark = pytest.mark.gpu
 
 
@@ -74,13 +76,9 @@ def test_kernels_vs_reference_numba_cuda(ref, mode, N, M, T, H, res, B, det_alph
     rp = _quiet(RMPPI, rcfg)
     rp.setup(p, rl, ra)
     rp.u_cur_d = cuda.to_device(sc["u0"])
-    cfg = _quiet(E.Config, **sc["cfg"])
-    el, ea = _quiet(E.TDM_Numba, cfg), _quiet(E.TDM_Numba, cfg)
-    _quiet(el.set_TDM_from_PMF_grid, sc["pmf_lin"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    _quiet(ea.set_TDM_from_PMF_grid, sc["pmf_ang"], sc["tdm_dict"], sc["obstacle"], sc["unknown"])
-    ep = _quiet(E.MPPI_Numba, cfg)
-    ep.setup(p, el, ea)
-    ep.u_cur_d.copy_to_device(sc["u0"])
+    with quiet():
+        ep = tdm_planner(E, sc)
+    el, ea = ep.lin_tdm, ep.ang_tdm
     ep.move_mppi_task_vars_to_device()
     L = E._lib
     Hp, Wp = el.pmf_grid_d.shape[1:]
@@ -164,7 +162,6 @@ def test_reference_fuses_traction_and_state_updates(ref, kind):
     import mppi_numba_b200 as E
     from oracle import arith as AR
     from tests.directed_cases import directed_scenario, fma_boundary_case
-    from tests.test_gpu_exact_oracle import assert_all_equal, directed_oracle, run_directed
     f32 = np.float32
     dev = AR.Exact(AR.DeviceProvider(E._lib), ftz=True)
     case = fma_boundary_case(dev, kind)
