@@ -1,12 +1,14 @@
 #!/usr/bin/env python
 """bench_trials.py -- closed-loop episodes of K planners: the host-driven loop against the batch's device episodes.
 
-    python bench_trials.py --workload c2|c4|c3|ref|refm --batch K --closed-loop S [--rounds R] [--profile]
+    python bench_trials.py --workload c2|c4|c3|ref|refm|bb --batch K --closed-loop S [--rounds R] [--profile]
 
 c2 and c4 are one-map workloads (MPPI_Batch.run_trials); c3 and ref are stochastic (use_tdm, CVaR cost:
 MPPI_StochasticBatch.run_stochastic_trials).  ref is the reference benchmark's noisy_dyn trial shape (N 1024, M 1024,
 T 100, a 9 x 9-cell map at 1 m), defined here: every reach box leaves that map, so every step samples whole maps.
-refm is ref with 2048 sampled maps: a less noisy tail estimate, whose CVaR runs the CTA kernel.
+refm is ref with 2048 sampled maps: a less noisy tail estimate, whose CVaR runs the CTA kernel.  bb is the barebone
+notebook's map-free loop (MPPI_Batch.run_barebone_trials, run_bb below), whose parity check also holds the obstacle
+contact counts against numpy's rule on the device's trajectory.
 
 K planners of the workload (bench.py's WORKLOADS, seeds 1..K: different maps, start poses and warm starts), each with
 a seeded ground-truth TractionGrid over its map; every other planner has its goal 1.5 m away (reached within S steps),
@@ -125,6 +127,19 @@ def run(args, emit):
         torch.cuda.synchronize(dev)
         return int(o["steps"].sum())
 
+    measure(args, emit, host_round, device_round, ba, bb, parity, dev,
+            "closed-loop trials: host-driven loop vs " +
+            ("MPPI_StochasticBatch.run_stochastic_trials" if stochastic else "MPPI_Batch.run_trials"),
+            {"workload": (args.workload if args.workload in LOCAL_WORKLOADS else workload_name_of(args.workload)),
+             "batch": K, "max_steps": S,
+             "planners": "seeds 1..K, warm started; even k: goal 1.5 m away, odd k: distant goal"})
+
+
+def measure(args, emit, host_round, device_round, ba, bb, parity, dev, metric, config):
+    """R alternating timed rounds of the host loop (on batch bb) and the device episodes (on batch ba), then the JSON
+    line."""
+    import torch
+    K = len(ba)
     host_round(), device_round()                          # warm-up of both paths
     res = {"host": [], "device": []}
     launches = {}
@@ -161,15 +176,115 @@ def run(args, emit):
         gpu["power_limit_and_max_sm_clock"] = q
     except Exception as e:                               # noqa: BLE001
         gpu["power_limit_and_max_sm_clock"] = "unavailable (%r)" % e
-    emit(json.dumps({"metric": "closed-loop trials: host-driven loop vs " +
-                     ("MPPI_StochasticBatch.run_stochastic_trials" if stochastic else "MPPI_Batch.run_trials"),
-                     "unit": "episodes/s", "value": devr["episodes_per_s"], "higher_is_better": True,
-                     "config": {"workload": (args.workload if args.workload in LOCAL_WORKLOADS else
-                                             workload_name_of(args.workload)), "batch": K, "max_steps": S,
-                                "planners": "seeds 1..K, warm started; even k: goal 1.5 m away, odd k: distant goal"},
-                     "rounds": args.rounds, "gpu": gpu, "parity_check": parity, "host": host, "device": devr,
-                     "speedup_wall": host["s_per_round_wall"] / devr["s_per_round_wall"],
+    emit(json.dumps({"metric": metric, "unit": "episodes/s", "value": devr["episodes_per_s"], "higher_is_better": True,
+                     "config": config, "rounds": args.rounds, "gpu": gpu, "parity_check": parity, "host": host,
+                     "device": devr, "speedup_wall": host["s_per_round_wall"] / devr["s_per_round_wall"],
                      "device_kernel_split_one_round": split}))
+
+
+def run_bb(args, emit):
+    """The bb workload: barebone planners of the notebook's shape (N 1000, T 50, dt 0.1, its two obstacles, vrange
+    [0, 2], u_std [1, 1], dist_weight 10, obs_penalty 1e6, goal_tolerance 0.5), planner k with its own seed and seeded
+    perturbations of the start, the goal and the obstacles; even k: a goal about 1.2 m away, odd k: the notebook's
+    goal, 8.6 m away.  Host loop: the batch's solve() of all K, then per running planner the numpy plant step and
+    shift_and_update; device: one run_barebone_trials(S)."""
+    import torch
+    import __graft_entry__
+    __graft_entry__.build_engine()
+    import mppi_numba_b200 as E
+    from mppi_numba_b200 import barebone as BB
+    from tests.barebone_trial_loop import goal_distance, in_contact, obstacles, plant_step
+    K, S = args.batch, args.closed_loop
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    params = []
+    for k in range(K):
+        rng = np.random.default_rng(1000 + k)
+        x0 = np.array([0.0, 0.0, np.pi / 4]) + rng.uniform(-0.3, 0.3, 3)
+        xgoal = x0[:2] + np.array([0.3, 1.2]) if k % 2 == 0 else np.array([7.0, 5.0]) + rng.uniform(-0.3, 0.3, 2)
+        params.append(dict(dt=0.1, x0=x0, xgoal=xgoal, goal_tolerance=0.5, dist_weight=10, lambda_weight=1.0, num_opt=1,
+                           u_std=np.array([1.0, 1.0]), vrange=np.array([0.0, 2.0]), wrange=np.array([-np.pi, np.pi]),
+                           obstacle_positions=np.array([[5.0, 4.5], [2.0, 1.0]]) + rng.uniform(-0.2, 0.2, (2, 2)),
+                           obstacle_radius=np.array([1.5, 1.0]), obs_penalty=1e6))
+
+    def planners():
+        pls = []
+        for k, q in enumerate(params):
+            p = BB.MPPI_Numba(BB.Config(T=5.0, dt=0.1, num_control_rollouts=1000, seed=k + 1))
+            p.setup(q)
+            pls.append(p)
+        return pls
+    A, Bs = planners(), planners()
+    T = A[0].num_steps
+
+    def reset(pls):
+        for p, q in zip(pls, params):
+            p.params["x0"] = q["x0"].copy()
+            p.u_cur_d.copy_to_device(np.zeros((T, 2), np.float32))
+
+    reset(A), reset(Bs)
+    ba, bb = E.MPPI_Batch(A), E.MPPI_Batch(Bs)
+
+    # ---- parity: the device episodes == the host loop replayed with the device's trajectory; the contact counts ==
+    # numpy's rule on the device's trajectory
+    out = ba.run_barebone_trials(S)
+    ok_u = ok_contacts = True
+    for k, p in enumerate(Bs):
+        one = E.MPPI_Batch([p])
+        n = int(out["steps"][k])
+        for t in range(n):
+            useq = one.solve()[0]
+            ok_u &= useq[0].tobytes() == out["uhist"][k, t].tobytes()
+            p.shift_and_update(out["xhist"][k, t + 1], useq, 1)
+        obs = obstacles(p)
+        ok_contacts &= int(out["contact_steps"][k]) == sum(in_contact(out["xhist"][k, t], obs) for t in range(1, n + 1))
+
+    def state(p):
+        d = [p.u_cur_d, p.u_prev_d, p.costs_d, p.weights_d, p.noise_samples_d, p.rng_states_d]
+        return [a.copy_to_host() for a in d] + [np.asarray(p.params["x0"])]
+    ok_state = all(all(x.dtype == y.dtype and x.tobytes() == y.tobytes() for x, y in zip(state(a), state(b)))
+                   for a, b in zip(A, Bs))
+    parity = {"passed": bool(ok_u and ok_state and ok_contacts), "u_bitwise": bool(ok_u),
+              "state_bitwise": bool(ok_state), "contacts_exact": bool(ok_contacts), "planners": K,
+              "steps": out["steps"].tolist(), "status": out["status"], "contact_steps": out["contact_steps"].tolist(),
+              "against": "the host loop replayed with the device's trajectory on identical twins"}
+    if not parity["passed"]:
+        sys.stderr.write("bench_trials.py: PARITY CHECK FAILED: %s\n" % json.dumps(parity))
+        emit(json.dumps({"metric": "closed-loop trials", "error": "parity_check failed", "parity_check": parity}))
+        raise SystemExit(3)
+
+    def host_round():
+        reset(Bs)
+        x = [np.asarray(p.params["x0"], dtype=np.float64) for p in Bs]
+        running, steps = list(range(K)), 0
+        for t in range(S):
+            u = bb.solve()
+            still = []
+            for k in running:
+                p = Bs[k]
+                xn = plant_step(x[k], u[k, 0], float(p.params["dt"]))
+                p.shift_and_update(xn, u[k], 1)
+                x[k] = xn
+                steps += 1
+                if goal_distance(p, xn) > 0:
+                    still.append(k)
+            running = still
+            if not running:
+                break
+        torch.cuda.synchronize(dev)
+        return steps
+
+    def device_round():
+        reset(A)
+        o = ba.run_barebone_trials(S)
+        torch.cuda.synchronize(dev)
+        return int(o["steps"].sum())
+
+    measure(args, emit, host_round, device_round, ba, bb, parity, dev,
+            "closed-loop trials: host-driven loop vs MPPI_Batch.run_barebone_trials",
+            {"workload": "bb: barebone notebook (N 1000, T 50, dt 0.1, two obstacles)", "batch": K, "max_steps": S,
+             "planners": "seeds 1..K, seeded start / goal / obstacle perturbations; even k: goal 1.2 m away, odd k: "
+                         "the notebook's goal"})
 
 
 def main():
@@ -181,7 +296,7 @@ def main():
     def emit(line):
         os.write(real_stdout, (line + "\n").encode())
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[1])
-    ap.add_argument("--workload", default="c2", choices=["c2", "c4", "c3", "ref", "refm"])
+    ap.add_argument("--workload", default="c2", choices=["c2", "c4", "c3", "ref", "refm", "bb"])
     ap.add_argument("--batch", type=int, default=64, metavar="K", help="planners in the batch")
     ap.add_argument("--closed-loop", type=int, default=150, metavar="S", help="max control steps per episode")
     ap.add_argument("--rounds", type=int, default=3, help="timed rounds of each loop")
@@ -189,7 +304,7 @@ def main():
     args = ap.parse_args()
     if args.batch < 1 or args.closed_loop < 1 or args.rounds < 1:
         ap.error("--batch, --closed-loop and --rounds must be at least 1")
-    run(args, emit)
+    (run_bb if args.workload == "bb" else run)(args, emit)
 
 
 if __name__ == "__main__":

@@ -411,6 +411,29 @@ int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b200mppi_trial
                                          double* xhist, float* uhist, b200mppi_trial_result* results,
                                          int32_t* steps_issued);
 
+/* ------------------------------------------------------------------ closed-loop trials of a barebone batch
+ * The episodes of the barebone notebook's closed loop for a MODE_BAREBONE batch made by b200mppi_batch_create, entirely
+ * on the device: per step 3*num_opt + 1 launches for the whole batch, num_opt x (noise, rollout, update), then the
+ * plant step.  The plant step is the notebook's nominal unicycle in float64: u = u_cur[0]; x += dt*cos(theta)*v,
+ * y += dt*sin(theta)*v, theta += dt*w; u_cur shifted by one (the last row kept); d = |(x, y) - xgoal| - goal_tolerance,
+ * cum_obj += dt + d, cum_dist_to_goal += d.  A planner stops once d <= 0 (GOAL) or after max_steps steps (MAX_STEPS);
+ * there is no map to leave.  Every new pose is checked against the planner's obstacles (b200mppi_planner_set_obstacles):
+ * it touches obstacle (ox, oy, r) when (x - ox)^2 + (y - oy)^2 <= r^2 in float64 (each operation rounded on its own),
+ * the rollout's rule, and contact_steps[k] counts the steps whose new pose touches at least one.  An episode does not
+ * stop on contact.  Polling, stop gating and the state left behind are those of b200mppi_batch_run_trials: every
+ * planner is exactly as `steps` rounds of batch_solve -> plant step -> set_u(shifted u) -> set_params(x0 = float32(new
+ * pose)) would leave it, and the C-side params keep the x0 of the last solve.
+ *   trials       : count descriptors; the call reads x0, xgoal, goal_tolerance and dt.  lin and ang must be NULL; the
+ *                  grid fields, the padded limits and v_post_rollout are ignored.
+ *   contact_steps: int32 (count).  xhist, uhist, results and steps_issued as in b200mppi_batch_run_trials.
+ * Refused (B200MPPI_EINVAL naming the planner) before any work is issued: what batch_solve refuses, a batch that is not
+ * MODE_BAREBONE (naming planner 0's mode), max_steps < 1, num_opt < 1, non-NULL grids, a non-finite x0, xgoal or
+ * goal_tolerance, and a dt that is not finite and positive.  b200mppi_batch_run_trials and
+ * b200mppi_batch_run_stochastic_trials refuse MODE_BAREBONE batches. */
+int b200mppi_batch_run_barebone_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps,
+                                       double* xhist, float* uhist, b200mppi_trial_result* results,
+                                       int32_t* contact_steps, int32_t* steps_issued);
+
 #ifdef __cplusplus
 }
 #endif

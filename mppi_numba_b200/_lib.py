@@ -132,6 +132,8 @@ def _load():
                                                            C.POINTER(I32)]),
         "b200mppi_batch_run_trials": (C.c_int, [P, C.POINTER(TrialDesc), I32, P, P, C.POINTER(TrialResult),
                                                 C.POINTER(I32)]),
+        "b200mppi_batch_run_barebone_trials": (C.c_int, [P, C.POINTER(TrialDesc), I32, P, P, C.POINTER(TrialResult), P,
+                                                         C.POINTER(I32)]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)          # AttributeError here == ABI drift, fail loudly

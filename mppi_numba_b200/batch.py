@@ -18,7 +18,8 @@ CVaR and update, the map sampling per planner (include/b200mppi.h, batched stoch
 ``run_trials(traction_grids, max_steps)`` runs the benchmark's closed-loop episode (solve, plant step on a ground-truth
 ``TractionGrid``, shift_and_update, stop at the goal) for every det-dynamics or speed-map planner at once on the GPU,
 without a host round trip per step (include/b200mppi.h, closed-loop trials); ``MPPI_StochasticBatch.
-run_stochastic_trials`` does the same for use_tdm planners.
+run_stochastic_trials`` does the same for use_tdm planners.  ``run_barebone_trials(max_steps)`` runs the barebone
+notebook's closed loop (nominal unicycle, no map) for barebone planners and counts the steps that end in an obstacle.
 """
 import ctypes as C
 
@@ -140,11 +141,38 @@ class MPPI_Batch(object):
                              "planners)" % self.kind)
         return self._trials("MPPI_Batch.run_trials", lib.b200mppi_batch_run_trials, traction_grids, max_steps, dt)
 
+    def run_barebone_trials(self, max_steps, dt=None):
+        """The barebone notebook's closed loop for every planner at once, on the GPU: up to ``max_steps`` rounds of
+        ``u = solve()``, a nominal unicycle step with ``u[0]`` in float64 (``dt`` as a float64, default: each planner's
+        ``params['dt']``) and ``shift_and_update``, stopping once the planner is within ``goal_tolerance`` of its goal.
+        Each step's new pose is checked against the planner's obstacles: it touches one when
+        ``(x - ox)**2 + (y - oy)**2 <= r**2`` in float64, the rollout's rule.  Contacts are counted; they do not stop
+        the episode.
+
+        Afterwards every planner (controls, u_prev_d alias, noise, costs, weights, RNG streams and ``params['x0']``) is
+        exactly as after that host loop.  Returns a dict:
+          ``logs``: per planner, time_to_goal, success, dist_to_goal, cum_dist_to_goal and avg_dist_to_goal with
+                    run_trials' NaN conventions, and contact_steps (barebone params have no v_post_rollout, so there
+                    is no cum_obj);
+          ``xhist`` float64 (K, max_steps+1, 3) and ``uhist`` float32 (K, max_steps, 2), NaN after a planner's last
+          step; ``steps`` (K,) int; ``status`` (K,) of "goal" | "max_steps"; ``contact_steps`` (K,) int, the steps
+          whose new pose touched an obstacle.
+        Raises ValueError (naming the planner) for other batches, max_steps < 1, num_opt < 1, a planner that cannot
+        solve, a non-finite x0, xgoal or goal_tolerance, or a dt that is not finite and positive.  Nothing is issued
+        when the call is refused."""
+        if self.kind != "barebone":
+            raise ValueError("MPPI_Batch.run_barebone_trials: planner 0 is a %s planner (barebone trials run barebone "
+                             "planners; run_trials runs det-dynamics and speed-map planners)" % self.kind)
+        return self._trials("MPPI_Batch.run_barebone_trials", lib.b200mppi_batch_run_barebone_trials, None, max_steps,
+                            dt)
+
     def _trials(self, name, entry, traction_grids, max_steps, dt):
         """The marshalling of a closed-loop trial call through the C entry point ``entry`` and the logs built from its
-        results (run_trials, MPPI_StochasticBatch.run_stochastic_trials); ``name`` prefixes the refusals."""
+        results (run_trials, run_barebone_trials with traction_grids None, MPPI_StochasticBatch.run_stochastic_trials);
+        ``name`` prefixes the refusals."""
         K = len(self.planners)
-        grids = list(traction_grids)
+        barebone = traction_grids is None
+        grids = [None] * K if barebone else list(traction_grids)
         if len(grids) != K:
             raise ValueError("%s: %d traction grids for %d planners" % (name, len(grids), K))
         max_steps = int(max_steps)
@@ -157,6 +185,17 @@ class MPPI_Batch(object):
                 raise ValueError("%s: planner %d cannot solve (reason printed above)" % (name, i))
             if int(p.params["num_opt"]) < 1:
                 raise ValueError("%s: planner %d has num_opt %d < 1" % (name, i, int(p.params["num_opt"])))
+            d, q = descs[i], p.params
+            if barebone:
+                d.x0[:] = [float(v) for v in np.asarray(q["x0"], dtype=np.float64)[:3]]
+                d.xgoal[:] = [float(v) for v in np.asarray(q["xgoal"], dtype=np.float64)[:2]]
+                d.goal_tolerance = float(q["goal_tolerance"])
+                d.dt = float(q["dt"] if dt is None else dt)
+                if not np.isfinite(list(d.x0) + list(d.xgoal) + [d.goal_tolerance]).all():
+                    raise ValueError("%s: planner %d: start pose, goal or goal_tolerance not finite" % (name, i))
+                if not (np.isfinite(d.dt) and d.dt > 0):
+                    raise ValueError("%s: planner %d: dt %r not finite and positive" % (name, i, d.dt))
+                continue
             lin, ang = np.asarray(g.lin_traction), np.asarray(g.ang_traction)
             for a in (lin, ang):
                 if a.dtype != np.float64 and not np.issubdtype(a.dtype, np.integer):
@@ -168,7 +207,6 @@ class MPPI_Batch(object):
             lin = np.ascontiguousarray(lin, dtype=np.float64)
             ang = np.ascontiguousarray(ang, dtype=np.float64)
             keep += [lin, ang]
-            d, q = descs[i], p.params
             d.lin, d.ang = lin.ctypes.data, ang.ctypes.data
             d.height, d.width = lin.shape
             d.xlo, d.ylo, d.res = float(g.xlimits[0]), float(g.ylimits[0]), float(g.res)
@@ -184,7 +222,9 @@ class MPPI_Batch(object):
         uhist = np.empty((K, max_steps, 2), dtype=np.float32)
         res = (_lib.TrialResult * K)()
         issued = C.c_int32()
-        check(entry(self._handle, descs, max_steps, ptr(xhist), ptr(uhist), res, C.byref(issued)))
+        contacts = np.zeros(K, dtype=np.int32)
+        outs = (ptr(xhist), ptr(uhist), res) + ((ptr(contacts),) if barebone else ())
+        check(entry(self._handle, descs, max_steps, *outs, C.byref(issued)))
         self.steps_issued = int(issued.value)
         steps = np.array([r.steps for r in res], dtype=np.int64)
         status = [TRIAL_STATUS[r.status] for r in res]
@@ -197,12 +237,19 @@ class MPPI_Batch(object):
             cum_obj, dist = r.cum_obj, r.dist_to_goal
             if reached:
                 dist = np.nan
-            else:
+            elif not barebone:
                 cum_obj += dist / descs[i].v_post_rollout
-            logs.append(dict(time_to_goal=n * descs[i].dt if reached else np.nan, success=reached, dist_to_goal=dist,
-                             cum_dist_to_goal=r.cum_dist_to_goal, avg_dist_to_goal=r.cum_dist_to_goal / n,
-                             cum_obj=cum_obj))
-        return dict(logs=logs, xhist=xhist, uhist=uhist, steps=steps, status=status)
+            log = dict(time_to_goal=n * descs[i].dt if reached else np.nan, success=reached, dist_to_goal=dist,
+                       cum_dist_to_goal=r.cum_dist_to_goal, avg_dist_to_goal=r.cum_dist_to_goal / n)
+            if barebone:
+                log["contact_steps"] = int(contacts[i])
+            else:
+                log["cum_obj"] = cum_obj
+            logs.append(log)
+        out = dict(logs=logs, xhist=xhist, uhist=uhist, steps=steps, status=status)
+        if barebone:
+            out["contact_steps"] = contacts.astype(np.int64)
+        return out
 
 
 class MPPI_StochasticBatch(MPPI_Batch):
@@ -235,6 +282,10 @@ class MPPI_StochasticBatch(MPPI_Batch):
     def run_trials(self, traction_grids, max_steps, dt=None):
         raise ValueError("MPPI_StochasticBatch.run_trials: closed-loop trials run det-dynamics or speed-map batches "
                          "(a stochastic batch runs them with run_stochastic_trials)")
+
+    def run_barebone_trials(self, max_steps, dt=None):
+        raise ValueError("MPPI_StochasticBatch.run_barebone_trials: barebone trials run barebone batches (a stochastic "
+                         "batch runs its trials with run_stochastic_trials)")
 
     def run_stochastic_trials(self, traction_grids, max_steps, dt=None):
         """MPPI_Batch.run_trials for use_tdm planners: the same arguments, episode, stop rules, returned dict and NaN

@@ -2222,12 +2222,15 @@ extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
 // planners through pinned memory POLL steps behind the GPU and stops issuing once it reads zero.
 constexpr int TRIAL_POLL = 4;
 
-static int trial_validate(b200mppi_batch* b, const b200mppi_trial_desc* tr, int32_t max_steps,
-                          const char* fn = "run_trials") {
+// one-map (MODE_DET_DYN, MODE_SPEED_MAP), stochastic (MODE_TDM) and barebone (MODE_BAREBONE, no map) trials
+enum class TrialKind { onemap, stochastic, barebone };
+
+static int trial_validate(b200mppi_batch* b, TrialKind kind, const b200mppi_trial_desc* tr, int32_t max_steps,
+                          const char* fn) {
   const int K = (int)b->pl.size();
   if (!tr) return fail(B200MPPI_EINVAL, std::string(fn) + ": null trial descriptors");
   if (max_steps < 1) return fail(B200MPPI_EINVAL, std::string(fn) + ": max_steps < 1");
-  if (b->mode == B200MPPI_MODE_BAREBONE)
+  if (kind != TrialKind::barebone && b->mode == B200MPPI_MODE_BAREBONE)
     return fail(B200MPPI_EINVAL, "run_trials: planner 0 is MODE_BAREBONE (trials need traction maps: MODE_DET_DYN or "
                                  "MODE_SPEED_MAP batches)");
   int rc = batch_validate(b);
@@ -2236,6 +2239,17 @@ static int trial_validate(b200mppi_batch* b, const b200mppi_trial_desc* tr, int3
     const std::string who = std::string(fn) + ": planner " + std::to_string(i);
     const b200mppi_trial_desc& d = tr[i];
     if (b->pl[i]->prm.num_opt < 1) return fail(B200MPPI_EINVAL, who + " has num_opt < 1");
+    if (kind == TrialKind::barebone) {
+      if (d.lin || d.ang)
+        return fail(B200MPPI_EINVAL, who + ": traction grids given (barebone trials step the nominal unicycle: lin and "
+                                           "ang must be NULL)");
+      bool finite = std::isfinite(d.goal_tolerance);
+      for (int c = 0; c < 3; ++c) finite = finite && std::isfinite(d.x0[c]);
+      for (int c = 0; c < 2; ++c) finite = finite && std::isfinite(d.xgoal[c]);
+      if (!finite) return fail(B200MPPI_EINVAL, who + ": start pose, goal or goal_tolerance not finite");
+      if (!(d.dt > 0.0) || !std::isfinite(d.dt)) return fail(B200MPPI_EINVAL, who + ": dt not finite and positive");
+      continue;
+    }
     if (!d.lin || !d.ang || d.height < 1 || d.width < 1)
       return fail(B200MPPI_EINVAL, who + ": empty or missing traction grid");
     if (!(d.res > 0.0) || !std::isfinite(d.res) || !std::isfinite(d.xlo) || !std::isfinite(d.ylo) || !(d.dt > 0.0) ||
@@ -2309,31 +2323,42 @@ static int stochastic_trial_plans(b200mppi_batch* b, const std::string& fn, std:
   return B200MPPI_OK;
 }
 
-// The closed-loop trials of both kinds of batch.  Stochastic trials also move each planner's reach box with the robot;
+static const char* mode_name(int mode) {
+  return mode == B200MPPI_MODE_DET_DYN ? "MODE_DET_DYN" : mode == B200MPPI_MODE_SPEED_MAP ? "MODE_SPEED_MAP" :
+         mode == B200MPPI_MODE_BAREBONE ? "MODE_BAREBONE" : "MODE_TDM";
+}
+
+// The closed-loop trials of every kind of batch.  Stochastic trials also move each planner's reach box with the robot;
 // with box_mode 2 and num_opt 1 it depends on the controls drawn, so the batched boxed sampler decides it on the device
 // (reach_box_decide, the function sample_finish calls) and a step needs no host round trip.  Per step: num_opt x
-// (noise [+ controls], [first iteration: sampler (stochastic: boxed, then the state advance)], rollout [windowed, then
-// CVaR], update) and the plant step, which for stochastic trials also moves each planner's rollout window.
+// (noise [+ controls], [first iteration, not barebone: sampler (stochastic: boxed, then the state advance)], rollout
+// [windowed, then CVaR], update) and the plant step, which for stochastic trials also moves each planner's rollout
+// window and for barebone trials counts obstacle contacts.
 // Device buffer of a call: [descriptors (b->h_desc's layout; a one-map batch's parity-0 sampler set is its own section
-// there) | stochastic: the parity-0 sampler set | the parity-1 set | stochastic: box descriptors, box records | states |
-// trials | active K + count | grids | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds xhist
-// and uhist: the float64 ground-truth grids (tens of MB for a batch of large maps) are copied straight from the
-// caller's arrays.
-static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_trial_desc* trials, int32_t max_steps,
-                            double* xhist, float* uhist, b200mppi_trial_result* results, int32_t* steps_issued) {
-  const std::string fn = stochastic ? "run_stochastic_trials" : "run_trials";
+// there) | stochastic: the parity-0 sampler set | not barebone: the parity-1 set | stochastic: box descriptors, box
+// records | states | barebone: contacts | trials | active K + count | not barebone: grids | xhist | uhist].  The pinned
+// staging mirrors it up to the grids, then holds xhist and uhist: the float64 ground-truth grids (tens of MB for a batch
+// of large maps) are copied straight from the caller's arrays.
+static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_trial_desc* trials, int32_t max_steps,
+                            double* xhist, float* uhist, b200mppi_trial_result* results, int32_t* contact_steps,
+                            int32_t* steps_issued) {
+  const bool stochastic = kind == TrialKind::stochastic, barebone = kind == TrialKind::barebone;
+  const std::string fn = stochastic ? "run_stochastic_trials" : barebone ? "run_barebone_trials" : "run_trials";
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
-  if (b->stochastic && !stochastic)
+  if (barebone && b->mode != B200MPPI_MODE_BAREBONE)
+    return fail(B200MPPI_EINVAL, fn + ": planner 0 is " + mode_name(b->mode) + " (barebone trials run MODE_BAREBONE "
+                                 "batches; b200mppi_batch_run_trials and b200mppi_batch_run_stochastic_trials run the "
+                                 "others)");
+  if (b->stochastic && kind == TrialKind::onemap)
     return fail(B200MPPI_EINVAL, "run_trials: planner 0 is MODE_TDM (trials run det-dynamics or speed-map batches: a "
                                  "stochastic solve sizes each planner's map-sampling box on the host)");
   if (!b->stochastic && stochastic)
-    return fail(B200MPPI_EINVAL, fn + ": planner 0 is " +
-                                     (b->mode == B200MPPI_MODE_DET_DYN ? "MODE_DET_DYN" :
-                                      b->mode == B200MPPI_MODE_SPEED_MAP ? "MODE_SPEED_MAP" : "MODE_BAREBONE") +
+    return fail(B200MPPI_EINVAL, fn + ": planner 0 is " + mode_name(b->mode) +
                                      " (stochastic trials run MODE_TDM batches; b200mppi_batch_run_trials runs the others)");
-  int rc = trial_validate(b, trials, max_steps, fn.c_str());
+  int rc = trial_validate(b, kind, trials, max_steps, fn.c_str());
   if (rc) return rc;
-  if (!xhist || !uhist || !results) return fail(B200MPPI_EINVAL, fn + ": null output buffer");
+  if (!xhist || !uhist || !results || (barebone && !contact_steps))
+    return fail(B200MPPI_EINVAL, fn + ": null output buffer");
   int WW = 0, WH = 0;
   if (stochastic && (rc = stochastic_validate(b, fn.c_str(), &WW, &WH))) return rc;
   CU(cudaSetDevice(b->device));
@@ -2345,7 +2370,7 @@ static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_t
   int mrows = 0, ncact = 0;
   if (stochastic) {
     if ((rc = stochastic_trial_plans(b, fn, plans, set0, &mrows, &ncact))) return rc;
-  } else {
+  } else if (!barebone) {
     std::vector<char> joined;
     int nj = 0;
     if ((rc = batch_plan_sample(b, set0.data(), plans, joined, &nj))) return rc;
@@ -2357,19 +2382,22 @@ static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_t
   }
   if ((rc = batch_wait_members(b))) return rc;
   const size_t nbox = stochastic ? (size_t)K : 0;      // stochastic-only sections
+  const size_t nset = barebone ? 0 : (size_t)K;        // sections of planners with maps
+  const size_t ncon = barebone ? (size_t)K : 0;        // barebone-only section
   const size_t off_s0 = stochastic ? b->desc_bytes : b->off_sample;
   const size_t off_s1 = b->desc_bytes + align256(nbox * sizeof(SampleGridsV2Args));
-  const size_t off_box = off_s1 + align256((size_t)K * sizeof(SampleGridsV2Args));
+  const size_t off_box = off_s1 + align256(nset * sizeof(SampleGridsV2Args));
   const size_t off_rec = off_box + align256(nbox * sizeof(SampleBoxDesc));
   const size_t off_state = off_rec + align256(nbox * 5 * sizeof(int));
-  const size_t off_tr = off_state + align256((size_t)K * sizeof(TrialState));
+  const size_t off_con = off_state + align256((size_t)K * sizeof(TrialState));
+  const size_t off_tr = off_con + align256(ncon * sizeof(int));
   const size_t off_act = off_tr + align256((size_t)K * sizeof(TrialDev));
   size_t off = off_act + align256((size_t)(K + 1) * sizeof(int));
   const size_t head = off;
   std::vector<size_t> off_grid(K);
   for (int i = 0; i < K; ++i) {
     off_grid[i] = off;
-    off += align256((size_t)2 * trials[i].height * trials[i].width * sizeof(double));
+    if (!barebone) off += align256((size_t)2 * trials[i].height * trials[i].width * sizeof(double));
   }
   const size_t off_xh = off, off_uh = off_xh + align256((size_t)K * (S + 1) * 3 * sizeof(double));
   const size_t total = off_uh + align256((size_t)K * S * 2 * sizeof(float));
@@ -2403,8 +2431,23 @@ static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_t
   // the rollout descriptors whose x0 the plant step writes: RolloutArgs (one-map), RolloutWinArgs (stochastic)
   RolloutArgs* dr = reinterpret_cast<RolloutArgs*>(d + b->off_roll);
   RolloutWinArgs* dw = reinterpret_cast<RolloutWinArgs*>(d + b->off_win);
+  int* hcon = reinterpret_cast<int*>(h + off_con);
   for (int i = 0; i < K; ++i) {
     b200mppi_planner* p = b->pl[i];
+    const b200mppi_trial_desc& q = trials[i];
+    TrialDev& t = ht[i];
+    t = TrialDev{};
+    t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1]; t.tol = q.goal_tolerance;
+    t.u_cur = p->u_cur;
+    hst[i] = TrialState{};
+    for (int c = 0; c < 3; ++c) hst[i].x[c] = q.x0[c];
+    hact[i] = 1;
+    if (barebone) {                                    // lin null: nominal unicycle, no map; contacts counted
+      t.x0_out = dr[i].p.x0;
+      t.obstacles = p->obstacles; t.num_obstacles = p->num_obstacles;
+      hcon[i] = 0;
+      continue;
+    }
     // parity 1: the pair samples from the buffers parity 0 wrote into
     hs[0][i] = hs[1][i] = set0[i];
     for (SampleTdm& td : hs[1][i].t) {
@@ -2412,18 +2455,10 @@ static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_t
       td.states_out = const_cast<uint64_t*>(td.states);
       td.states = in;
     }
-    const b200mppi_trial_desc& q = trials[i];
     const double* dg = reinterpret_cast<const double*>(d + off_grid[i]);
-    TrialDev& t = ht[i];
-    t = TrialDev{};
     t.lin = dg; t.ang = dg + (size_t)q.height * q.width; t.H = q.height; t.W = q.width;
-    t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res; t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1];
-    t.tol = q.goal_tolerance;
+    t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res;
     t.pxlim[0] = q.pxlim[0]; t.pxlim[1] = q.pxlim[1]; t.pylim[0] = q.pylim[0]; t.pylim[1] = q.pylim[1];
-    t.u_cur = p->u_cur;
-    hst[i] = TrialState{};
-    for (int c = 0; c < 3; ++c) hst[i].x[c] = q.x0[c];
-    hact[i] = 1;
     if (!stochastic) {
       t.x0_out = dr[i].p.x0;                           // win stays null: one-map rollouts have no window
       continue;
@@ -2440,7 +2475,7 @@ static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_t
   hact[K] = K;
   const RolloutWinArgs g0 = stochastic ? *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win) : RolloutWinArgs{};
   CU(cudaMemcpyAsync(d, h, head, cudaMemcpyHostToDevice, st));
-  for (int i = 0; i < K; ++i) {                       // pageable sources: staged by the driver before the call returns
+  for (int i = 0; i < K && !barebone; ++i) {          // pageable sources: staged by the driver before the call returns
     const size_t bytes = (size_t)trials[i].height * trials[i].width * sizeof(double);
     CU(cudaMemcpyAsync(d + off_grid[i], trials[i].lin, bytes, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(d + off_grid[i] + bytes, trials[i].ang, bytes, cudaMemcpyHostToDevice, st));
@@ -2450,7 +2485,8 @@ static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_t
   const SampleBoxDesc* db = reinterpret_cast<const SampleBoxDesc*>(d + off_box);
   const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(d + b->off_upd);
   PlantArgs pa{reinterpret_cast<const TrialDev*>(d + off_tr), reinterpret_cast<TrialState*>(d + off_state), dact,
-               dact + K, reinterpret_cast<double*>(d + off_xh), reinterpret_cast<float*>(d + off_uh), K, T, S, 0};
+               dact + K, reinterpret_cast<double*>(d + off_xh), reinterpret_cast<float*>(d + off_uh), K, T, S, 0,
+               barebone ? reinterpret_cast<int*>(d + off_con) : nullptr};
   CU(cudaStreamSynchronize(st));                      // the staging is read by the upload above
   int* hcount = reinterpret_cast<int*>(h);             // the polled counts, in the no longer needed head of the staging
   for (cudaEvent_t& e : buf.ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -2479,7 +2515,7 @@ static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_t
       } else {
         launch_sample_noise_batch(reinterpret_cast<const NoiseDesc*>(d), K, N, T, dact, st);
         CHECK_LAUNCH();
-        if (k == 0) {
+        if (k == 0 && !barebone) {
           launch_sample_grids_v2_batch(geom, ds[s & 1], K, dact, st);
           CHECK_LAUNCH();
         }
@@ -2492,12 +2528,12 @@ static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_t
     pa.step = s;
     launch_plant_step(pa, st);
     CHECK_LAUNCH();
-    b->launches += stochastic ? 4 * num_opt + 3 : 3 * num_opt + 2;
+    b->launches += stochastic ? 4 * num_opt + 3 : barebone ? 3 * num_opt + 1 : 3 * num_opt + 2;
     ++issued;
     CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, dact + K, sizeof(int), cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(buf.ev[s % TRIAL_POLL], st));
   }
-  // the box records (stochastic) and the states, then the histories
+  // the box records (stochastic), the states and the contacts (barebone), then the histories
   CU(cudaMemcpyAsync(h + off_rec, d + off_rec, off_tr - off_rec, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(h + head, d + off_xh, total - off_xh, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
@@ -2517,17 +2553,19 @@ static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_t
     std::memcpy(uo, hu + (size_t)i * S * 2, (size_t)n * 2 * sizeof(float));
     for (size_t j = (size_t)n * 2; j < (size_t)S * 2; ++j) uo[j] = fnan;
     results[i] = b200mppi_trial_result{r.cum_obj, r.cum_dist, r.dist, n, r.status};
+    if (barebone) contact_steps[i] = hcon[i];
     // host state as after n rounds of the host loop: n samplings of the pair (stochastic: boxed or whole-map, the last
     // one's kind in grid_partial), the reach slot toggled once per iteration, the last solve's box and x0
     b200mppi_planner* p = b->pl[i];
     const int* rec = hrec + 5 * i;
     if (stochastic) plans[i].boxed[0] = plans[i].boxed[1] = rec[0] != 0;
-    for (int s = 0; s < n; ++s) { plan_commit(plans[i], 0); plan_commit(plans[i], 1); }
+    if (!barebone)
+      for (int s = 0; s < n; ++s) { plan_commit(plans[i], 0); plan_commit(plans[i], 1); }
     if (stochastic) {
       p->reach_slot ^= (n * num_opt) & 1;
       p->reach_valid = true;
       for (int c = 0; c < 5; ++c) p->last_box[c] = rec[c];
-    } else {
+    } else if (!barebone) {
       last_box_whole_map(p);
     }
     p->prepared = false;
@@ -2541,11 +2579,19 @@ static int batch_run_trials(b200mppi_batch* b, bool stochastic, const b200mppi_t
 extern "C" int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps,
                                          double* xhist, float* uhist, b200mppi_trial_result* results,
                                          int32_t* steps_issued) {
-  return batch_run_trials(b, false, trials, max_steps, xhist, uhist, results, steps_issued);
+  return batch_run_trials(b, TrialKind::onemap, trials, max_steps, xhist, uhist, results, nullptr, steps_issued);
 }
 
 extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials,
                                                     int32_t max_steps, double* xhist, float* uhist,
                                                     b200mppi_trial_result* results, int32_t* steps_issued) {
-  return batch_run_trials(b, true, trials, max_steps, xhist, uhist, results, steps_issued);
+  return batch_run_trials(b, TrialKind::stochastic, trials, max_steps, xhist, uhist, results, nullptr, steps_issued);
+}
+
+extern "C" int b200mppi_batch_run_barebone_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials,
+                                                  int32_t max_steps, double* xhist, float* uhist,
+                                                  b200mppi_trial_result* results, int32_t* contact_steps,
+                                                  int32_t* steps_issued) {
+  return batch_run_trials(b, TrialKind::barebone, trials, max_steps, xhist, uhist, results, contact_steps,
+                          steps_issued);
 }

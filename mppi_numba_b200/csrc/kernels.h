@@ -436,7 +436,7 @@ __host__ __device__ inline void win_origin(float x0x, float x0y, float pxl, floa
   f[5] = WH < rows - f[3] ? WH : rows - f[3];
 }
 struct TrialDev {
-  const double* lin; const double* ang;   // ground-truth traction (H, W), float64
+  const double* lin; const double* ang;   // ground-truth traction (H, W), float64; null: nominal unicycle, no map
   int H, W;
   double xlo, ylo, res, dt, xgoal[2], tol, pxlim[2], pylim[2];
   float* u_cur;                           // (T, 2): u_cur[0] is applied, then the sequence is shifted by one
@@ -446,6 +446,9 @@ struct TrialDev {
   int* win;
   float win_pxl, win_pyl, win_res;
   int win_rows, win_cols;
+  // barebone trials: the planner's obstacles (RolloutArgs::obstacles, (num_obstacles, 3) = x, y, radius)
+  const float* obstacles;
+  int num_obstacles;
 };
 struct TrialState {
   double x[3], cum_obj, cum_dist, dist;
@@ -457,6 +460,7 @@ struct PlantArgs {
   double* xhist;                          // (K, max_steps+1, 3)
   float* uhist;                           // (K, max_steps, 2)
   int K, T, max_steps, step;
+  int* contacts;                          // barebone trials: (K) steps whose new pose touches an obstacle; else null
 };
 // [emu:end trial_args]
 void launch_plant_step(const PlantArgs& a, cudaStream_t st);

@@ -380,6 +380,8 @@ __device__ __forceinline__ double py_floordiv(double vx, double wx) {
 
 // One warp per planner (warp k of the grid = planner k): apply u_cur[0], shift u_cur by one row (the last row kept),
 // record the step, and stop the planner on the goal, on leaving the padded map or after max_steps steps.
+// Barebone trials (TrialDev::lin null) step the notebook's nominal unicycle (traction 1: dt * 1.0 == dt), have no map
+// to leave, and count in contacts[k] the steps whose new pose lies in one of the planner's obstacles.
 __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int lane) {
   if (k >= a.K || !a.active[k]) return;
   const TrialDev& d = a.trials[k];
@@ -401,12 +403,15 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
   float* uh = a.uhist + ((size_t)k * a.max_steps + t) * 2;
   uh[0] = v; uh[1] = w;
   const double x = s.x[0], y = s.x[1], th = s.x[2];
-  // TractionGrid.get: int((x - xlo) // res), (0, 0) outside [0, W) x [0, H)
-  const double fx = py_floordiv(__dsub_rn(x, d.xlo), d.res), fy = py_floordiv(__dsub_rn(y, d.ylo), d.res);
-  double lt = 0.0, at = 0.0;
-  if (fx >= 0.0 && fx < (double)d.W && fy >= 0.0 && fy < (double)d.H) {
-    const size_t cell = (size_t)fy * (size_t)d.W + (size_t)fx;
-    lt = d.lin[cell]; at = d.ang[cell];
+  double lt = 1.0, at = 1.0;
+  if (d.lin) {
+    // TractionGrid.get: int((x - xlo) // res), (0, 0) outside [0, W) x [0, H)
+    const double fx = py_floordiv(__dsub_rn(x, d.xlo), d.res), fy = py_floordiv(__dsub_rn(y, d.ylo), d.res);
+    lt = 0.0; at = 0.0;
+    if (fx >= 0.0 && fx < (double)d.W && fy >= 0.0 && fy < (double)d.H) {
+      const size_t cell = (size_t)fy * (size_t)d.W + (size_t)fx;
+      lt = d.lin[cell]; at = d.ang[cell];
+    }
   }
   const double dtl = __dmul_rn(d.dt, lt);
   const double xn = __dadd_rn(x, __dmul_rn(__dmul_rn(dtl, cos(th)), (double)v));
@@ -424,9 +429,21 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
   s.cum_dist = __dadd_rn(s.cum_dist, dist);
   s.dist = dist;
   s.steps = t + 1;
+  if (a.contacts) {
+    // (x - ox)^2 + (y - oy)^2 <= r^2 in float64 from the float32 obstacle: the rollout's rule (only diff > 0 is outside);
+    // one contact per step however many obstacles overlap there
+    bool hit = false;
+    for (int j = 0; j < d.num_obstacles && !hit; ++j) {
+      const double ex = __dsub_rn(xn, (double)d.obstacles[3 * j]), ey = __dsub_rn(yn, (double)d.obstacles[3 * j + 1]);
+      const double r = (double)d.obstacles[3 * j + 2];
+      hit = __dadd_rn(__dmul_rn(ex, ex), __dmul_rn(ey, ey)) <= __dmul_rn(r, r);
+    }
+    if (hit) a.contacts[k] += 1;
+  }
   int status = TRIAL_RUNNING;
   if (dist <= 0.0) status = TRIAL_GOAL;
-  else if (!(xn >= d.pxlim[0] && xn <= d.pxlim[1] && yn >= d.pylim[0] && yn <= d.pylim[1])) status = TRIAL_LEFT_MAP;
+  else if (d.lin && !(xn >= d.pxlim[0] && xn <= d.pxlim[1] && yn >= d.pylim[0] && yn <= d.pylim[1]))
+    status = TRIAL_LEFT_MAP;
   else if (t + 1 >= a.max_steps) status = TRIAL_MAX_STEPS;
   if (status != TRIAL_RUNNING) {
     s.status = status;
