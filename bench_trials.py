@@ -1,14 +1,16 @@
 #!/usr/bin/env python
 """bench_trials.py -- closed-loop episodes of K planners: the host-driven loop against the batch's device episodes.
 
-    python bench_trials.py --workload c2|c4|c3|ref|refm|bb --batch K --closed-loop S [--rounds R] [--profile]
+    python bench_trials.py --workload c2|c4|c3|ref|refm|gif|bb --batch K --closed-loop S [--rounds R] [--profile]
+                           [--record-every n]
 
 c2 and c4 are one-map workloads (MPPI_Batch.run_trials); c3 and ref are stochastic (use_tdm, CVaR cost:
 MPPI_StochasticBatch.run_stochastic_trials).  ref is the reference benchmark's noisy_dyn trial shape (N 1024, M 1024,
 T 100, a 9 x 9-cell map at 1 m), defined here: every reach box leaves that map, so every step samples whole maps.
 refm is ref with 2048 sampled maps: a less noisy tail estimate, whose CVaR runs the CTA kernel.  bb is the barebone
 notebook's map-free loop (MPPI_Batch.run_barebone_trials, run_bb below), whose parity check also holds the obstacle
-contact counts against numpy's rule on the device's trajectory.
+contact counts against numpy's rule on the device's trajectory.  gif is the shape of the reference's GIF notebook
+(use_tdm, N 1024, M 1024, T 100, 100 visualisation rollouts, a 12 x 6-cell map at 1 m), whose loop draws every step.
 
 K planners of the workload (bench.py's WORKLOADS, seeds 1..K: different maps, start poses and warm starts), each with
 a seeded ground-truth TractionGrid over its map; every other planner has its goal 1.5 m away (reached within S steps),
@@ -21,8 +23,14 @@ exits non-zero.  Then R rounds of each, alternating, every round from the same s
   device: one run_trials(grids, S) (run_stochastic_trials for c3, ref and refm).
 Wall clock per round (each ends in a host synchronisation); control steps/s (planner-steps run), episodes/s, kernel
 launches per round.  Prints one JSON line with the card's name and power limit; writes nothing to the tree.
+--record-every n (not bb): the notebooks' drawing loop, get_state_rollout() at every n-th step after solve() and before
+shift_and_update.  The parity check also holds the device's records (run_trials(..., record_every=n)) against the
+replayed host loop's get_state_rollout(), bit for bit; the host rounds call it; and device rounds with recording are
+timed alternately with those without.  --profile then profiles a recording round and reports the share of the
+visualisation and map-completion kernels.
 """
 import argparse
+import functools
 import json
 import os
 import subprocess
@@ -39,7 +47,11 @@ from bench import WORKLOADS, make_planner, workload_name_of   # noqa: E402
 
 # the reference benchmark's noisy_dyn trial: N 1024, M 1024, T 100 on a 9 x 9-cell map at 1 m (c3's bins)
 LOCAL_WORKLOADS = {"ref": ("tdm", 1024, 1024, 100, 9, 1.0) + tuple(WORKLOADS["c3"][6:]),
-                   "refm": ("tdm", 1024, 2048, 100, 9, 1.0) + tuple(WORKLOADS["c3"][6:])}
+                   "refm": ("tdm", 1024, 2048, 100, 9, 1.0) + tuple(WORKLOADS["c3"][6:]),
+                   "gif": ("tdm", 1024, 1024, 100, 6, 1.0) + tuple(WORKLOADS["c3"][6:])}
+# the GIF notebook's map is 12 cells wide and 6 high, and it draws 100 rollouts; elsewhere square maps, the scenario's V
+MAP_WIDTH = {"gif": 12}
+VIS_ROLLOUTS = {"gif": 100}
 
 
 def run(args, emit):
@@ -53,17 +65,21 @@ def run(args, emit):
     mode, N, M, T, H, res, B, da = LOCAL_WORKLOADS.get(args.workload) or WORKLOADS[args.workload]
     stochastic = mode == "tdm"
     Batch = E.MPPI_StochasticBatch if stochastic else E.MPPI_Batch
-    trials = (lambda b, g, s: b.run_stochastic_trials(g, s)) if stochastic else (lambda b, g, s: b.run_trials(g, s))
+    trials = ((lambda b, g, s, **kw: b.run_stochastic_trials(g, s, **kw)) if stochastic else
+              (lambda b, g, s, **kw: b.run_trials(g, s, **kw)))
+    W, every = MAP_WIDTH.get(args.workload, H), args.record_every
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     scs = []
     for k in range(K):
-        sc = make_scenario(mode, N=N, M=M, T=T, H=H, W=H, res=res, B=B, seed=k + 1, det_alpha=da, warm_start=True)
+        sc = make_scenario(mode, N=N, M=M, T=T, H=H, W=W, res=res, B=B, seed=k + 1, det_alpha=da, warm_start=True)
+        if args.workload in VIS_ROLLOUTS:
+            sc["cfg"]["num_vis_state_rollouts"] = VIS_ROLLOUTS[args.workload]
         if k % 2 == 0:
             sc["params"]["xgoal"] = sc["params"]["x0"][:2] + np.array([1.2, -0.9])
         scs.append(sc)
     rng = np.random.default_rng(7)
-    grids = [E.TractionGrid(rng.uniform(0.3, 1.0, (H, H)), rng.uniform(0.3, 1.0, (H, H)), res=res) for _ in range(K)]
+    grids = [E.TractionGrid(rng.uniform(0.3, 1.0, (H, W)), rng.uniform(0.3, 1.0, (H, W)), res=res) for _ in range(K)]
     A, Bs = [[make_planner(E, sc, 0)[3] for sc in scs] for _ in range(2)]
 
     def reset(pls):
@@ -75,14 +91,19 @@ def run(args, emit):
     ba, bb = Batch(A), Batch(Bs)
 
     # ---- parity: the device episodes == the host loop replayed with the device's trajectory
-    out = trials(ba, grids, S)
-    ok_u = True
+    out = trials(ba, grids, S, **({} if every is None else dict(record_every=every)))
+    ok_u = ok_rec = True
     for k, p in enumerate(Bs):
         one = Batch([p])
-        for t in range(int(out["steps"][k])):
+        n = int(out["steps"][k])
+        for t in range(n):
             useq = one.solve()[0]
             ok_u &= bool(np.array_equal(useq[0], out["uhist"][k, t]))
+            if every is not None and t % every == 0:
+                ok_rec &= p.get_state_rollout().tobytes() == out["state_rollouts"][k, t // every].tobytes()
             p.shift_and_update(out["xhist"][k, t + 1], useq, 1)
+        if every is not None:
+            ok_rec &= bool(np.isnan(out["state_rollouts"][k, -(-n // every):]).all())
 
     def state(p):
         d = [p.u_cur_d, p.u_prev_d, p.costs_d, p.weights_d, p.noise_samples_d, p.rng_states_d, p.lin_tdm.rng_states_d,
@@ -91,9 +112,11 @@ def run(args, emit):
             d.append(p.costs_nm_d)
         return [a.copy_to_host() for a in d] + [p.params["x0"], np.asarray(p.sample_box())]
     ok_state = all(all(np.array_equal(x, y) for x, y in zip(state(a), state(b))) for a, b in zip(A, Bs))
-    parity = {"passed": ok_u and ok_state, "u_bitwise": ok_u, "state_bitwise": ok_state, "planners": K,
+    parity = {"passed": bool(ok_u and ok_state and ok_rec), "u_bitwise": ok_u, "state_bitwise": ok_state, "planners": K,
               "steps": out["steps"].tolist(), "status": out["status"],
               "against": "the host loop replayed with the device's trajectory on identical twins"}
+    if every is not None:
+        parity["records_bitwise"] = bool(ok_rec)
     if not parity["passed"]:
         sys.stderr.write("bench_trials.py: PARITY CHECK FAILED: %s\n" % json.dumps(parity))
         emit(json.dumps({"metric": "closed-loop trials", "error": "parity_check failed", "parity_check": parity}))
@@ -109,6 +132,8 @@ def run(args, emit):
             for k in running:
                 p = Bs[k]
                 xn = plant_step(grids[k], x[k], u[k, 0], float(p.params["dt"]))
+                if every is not None and t % every == 0:
+                    p.get_state_rollout()
                 p.shift_and_update(xn, u[k], 1)
                 x[k] = xn
                 steps += 1
@@ -121,30 +146,38 @@ def run(args, emit):
         torch.cuda.synchronize(dev)
         return steps
 
-    def device_round():
+    def device_round(**kw):
         reset(A)
-        o = trials(ba, grids, S)
+        o = trials(ba, grids, S, **kw)
         torch.cuda.synchronize(dev)
         return int(o["steps"].sum())
 
+    config = {"workload": (args.workload if args.workload in LOCAL_WORKLOADS else workload_name_of(args.workload)),
+              "batch": K, "max_steps": S, "vis_rollouts": A[0].num_vis_state_rollouts,
+              "planners": "seeds 1..K, warm started; even k: goal 1.5 m away, odd k: distant goal"}
+    if every is not None:
+        config["record_every"] = every
+        config["host"] = "the host loop calls get_state_rollout() at every recorded step of every running planner"
     measure(args, emit, host_round, device_round, ba, bb, parity, dev,
             "closed-loop trials: host-driven loop vs " +
-            ("MPPI_StochasticBatch.run_stochastic_trials" if stochastic else "MPPI_Batch.run_trials"),
-            {"workload": (args.workload if args.workload in LOCAL_WORKLOADS else workload_name_of(args.workload)),
-             "batch": K, "max_steps": S,
-             "planners": "seeds 1..K, warm started; even k: goal 1.5 m away, odd k: distant goal"})
+            ("MPPI_StochasticBatch.run_stochastic_trials" if stochastic else "MPPI_Batch.run_trials"), config,
+            None if every is None else functools.partial(device_round, record_every=every))
 
 
-def measure(args, emit, host_round, device_round, ba, bb, parity, dev, metric, config):
-    """R alternating timed rounds of the host loop (on batch bb) and the device episodes (on batch ba), then the JSON
-    line."""
+def measure(args, emit, host_round, device_round, ba, bb, parity, dev, metric, config, recorded_round=None):
+    """R alternating timed rounds of the host loop (on batch bb), the device episodes (on batch ba) and, when given, the
+    device episodes with recording, then the JSON line."""
     import torch
     K = len(ba)
-    host_round(), device_round()                          # warm-up of both paths
-    res = {"host": [], "device": []}
+    legs = [("host", host_round, bb), ("device", device_round, ba)]
+    if recorded_round is not None:
+        legs.append(("device_recorded", recorded_round, ba))
+    for _, fn, _ in legs:                                 # warm-up of every path
+        fn()
+    res = {name: [] for name, _, _ in legs}
     launches = {}
     for _ in range(args.rounds):
-        for name, fn, b in (("host", host_round, bb), ("device", device_round, ba)):
+        for name, fn, b in legs:
             l0 = b.launch_count()
             t0 = time.perf_counter()
             steps = fn()
@@ -158,17 +191,21 @@ def measure(args, emit, host_round, device_round, ba, bb, parity, dev, metric, c
                 "control_steps_per_s": res[name][0][1] / med, "episodes_per_s": K / med,
                 "kernel_launches_per_round": launches[name]}
     host, devr = summary("host"), summary("device")
-    split = None
+    split = record_share = None
     if args.profile:                                     # a separate run: tracing slows the host
         from torch.profiler import ProfilerActivity, profile
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            device_round()
+            (recorded_round or device_round)()
         split = {}
         for ev in prof.key_averages():
             if ev.device_type.name == "CUDA" and ev.count:
                 t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0.0)
                 split[ev.key] = {"ms": t / 1e3, "launches": ev.count}
         split = dict(sorted(split.items(), key=lambda kv: -kv[1]["ms"]))
+        if recorded_round is not None:                   # the recording's own kernels in the profiled recording round
+            total = sum(v["ms"] for v in split.values())
+            record_share = {name: sum(v["ms"] for key, v in split.items() if name in key) / total
+                            for name in ("state_rollout_batch_kernel", "sample_grids_v2_complete_batch_kernel")}
     gpu = {"name": torch.cuda.get_device_name(dev)}
     try:
         q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -176,10 +213,15 @@ def measure(args, emit, host_round, device_round, ba, bb, parity, dev, metric, c
         gpu["power_limit_and_max_sm_clock"] = q
     except Exception as e:                               # noqa: BLE001
         gpu["power_limit_and_max_sm_clock"] = "unavailable (%r)" % e
-    emit(json.dumps({"metric": metric, "unit": "episodes/s", "value": devr["episodes_per_s"], "higher_is_better": True,
-                     "config": config, "rounds": args.rounds, "gpu": gpu, "parity_check": parity, "host": host,
-                     "device": devr, "speedup_wall": host["s_per_round_wall"] / devr["s_per_round_wall"],
-                     "device_kernel_split_one_round": split}))
+    line = {"metric": metric, "unit": "episodes/s", "value": devr["episodes_per_s"], "higher_is_better": True,
+            "config": config, "rounds": args.rounds, "gpu": gpu, "parity_check": parity, "host": host, "device": devr,
+            "speedup_wall": host["s_per_round_wall"] / devr["s_per_round_wall"], "device_kernel_split_one_round": split}
+    if recorded_round is not None:
+        rec = summary("device_recorded")
+        line.update(device_recorded=rec, speedup_wall_recorded=host["s_per_round_wall"] / rec["s_per_round_wall"],
+                    recording_cost_wall=rec["s_per_round_wall"] / devr["s_per_round_wall"] - 1.0,
+                    record_kernels_share_of_device_time=record_share)
+    emit(json.dumps(line))
 
 
 def run_bb(args, emit):
@@ -296,14 +338,18 @@ def main():
     def emit(line):
         os.write(real_stdout, (line + "\n").encode())
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[1])
-    ap.add_argument("--workload", default="c2", choices=["c2", "c4", "c3", "ref", "refm", "bb"])
+    ap.add_argument("--workload", default="c2", choices=["c2", "c4", "c3", "ref", "refm", "gif", "bb"])
     ap.add_argument("--batch", type=int, default=64, metavar="K", help="planners in the batch")
     ap.add_argument("--closed-loop", type=int, default=150, metavar="S", help="max control steps per episode")
     ap.add_argument("--rounds", type=int, default=3, help="timed rounds of each loop")
     ap.add_argument("--profile", action="store_true", help="then one device round under torch.profiler: kernel split")
+    ap.add_argument("--record-every", type=int, default=None, metavar="n",
+                    help="record the visualisation rollouts of every n-th step (not bb)")
     args = ap.parse_args()
     if args.batch < 1 or args.closed_loop < 1 or args.rounds < 1:
         ap.error("--batch, --closed-loop and --rounds must be at least 1")
+    if args.record_every is not None and (args.record_every < 1 or args.workload == "bb"):
+        ap.error("--record-every must be at least 1, and the bb workload does not take it")
     (run_bb if args.workload == "bb" else run)(args, emit)
 
 

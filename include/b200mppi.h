@@ -353,6 +353,18 @@ int b200mppi_batch_launch_count(b200mppi_batch* b, int64_t* out);
  *           tensor maps that cannot be encoded).  u_prev is not touched (a stochastic solve does not alias it). */
 int b200mppi_batch_create_stochastic(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out);
 
+/* ------------------------------------------------------------------ visualisation rollouts of a batch
+ * b200mppi_planner_get_state_rollout of every planner of a batch (either kind) with ONE launch: for MODE_TDM planners
+ * u_cur over the first V sampled maps, for the others u_cur and V-1 clipped u_prev + noise rollouts (MODE_BAREBONE
+ * without a map).  MODE_TDM planners whose last sampling was boxed first get their maps completed, as the single call
+ * does.  Each planner's own state-rollout buffer (B200MPPI_BUF_STATE_ROLLOUT) is written, then copied into out with one
+ * synchronisation: afterwards every planner is exactly as after get_state_rollout on planners[0], planners[1], ... in
+ * that order, bit for bit (per-planner launch counts are not touched; the batch's count grows by one).
+ *   out: float32 (count, V, T+1, 3), bytes its size.
+ * Refused (B200MPPI_EINVAL or the planner's own error, naming the planner) before any work is issued: a planner that is
+ * not ready (params not set, ...), unequal num_vis_state_rollouts, and V larger than a planner's M (MODE_TDM) or N. */
+int b200mppi_batch_get_state_rollout(b200mppi_batch* b, float* out, size_t bytes);
+
 /* ------------------------------------------------------------------ closed-loop trials of a batch
  * Every planner of a MODE_DET_DYN or MODE_SPEED_MAP batch drives a unicycle through one receding-horizon episode on
  * its own ground-truth traction grid, entirely on the device: per step ONE launch each of noise, map sampling, rollout
@@ -433,6 +445,31 @@ int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b200mppi_trial
 int b200mppi_batch_run_barebone_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps,
                                        double* xhist, float* uhist, b200mppi_trial_result* results,
                                        int32_t* contact_steps, int32_t* steps_issued);
+
+/* ------------------------------------------------------------------ closed-loop trials with visualisation records
+ * One of the three trial calls above (kind: B200MPPI_TRIALS_MAP = b200mppi_batch_run_trials, _STOCHASTIC =
+ * b200mppi_batch_run_stochastic_trials, _BAREBONE = b200mppi_batch_run_barebone_trials; contact_steps as that call
+ * takes it, NULL for the first two) that also records the visualisation rollouts of every step s with
+ * s % record_every == 0, as a host loop calling b200mppi_planner_get_state_rollout after solve() and the plant step and
+ * before shift_and_update records them: u_cur and x0 of that step's solve.  Everything else -- episodes, results,
+ * histories and the state every planner is left in -- is that call's, bit for bit; in addition each planner's
+ * state-rollout buffer holds its last record.
+ *   rollouts: float32 (count, R, V, T+1, 3), R = ceil(max_steps / record_every), rollout_bytes its size.  Record r
+ *             belongs to step r * record_every; it is NaN when that step is >= the planner's steps.  The records stay
+ *             in device memory during the call; at the end each written record is copied into rollouts once, and the
+ *             rest are set to NaN on the host.
+ * Launches: one more per recorded step (the batched visualisation rollouts, before the plant step), and for a
+ * stochastic batch one more again: a whole-map sampling of maps [0, V) for every pair whose step sampled a reach box,
+ * from that step's pre-call generator states (the maps the rollouts read; no generator state changes, maps >= V keep
+ * their box and are completed by any later reader, as after the host loop).
+ * Refused (B200MPPI_EINVAL naming the planner) before any work is issued: what the chosen call refuses, an unknown kind,
+ * record_every < 1, a NULL rollouts or a wrong rollout_bytes, unequal num_vis_state_rollouts and V larger than a
+ * planner's M (MODE_TDM) or N. */
+enum { B200MPPI_TRIALS_MAP = 0, B200MPPI_TRIALS_STOCHASTIC = 1, B200MPPI_TRIALS_BAREBONE = 2 };
+int b200mppi_batch_run_trials_recorded(b200mppi_batch* b, int32_t kind, const b200mppi_trial_desc* trials,
+                                       int32_t max_steps, double* xhist, float* uhist, b200mppi_trial_result* results,
+                                       int32_t* contact_steps, int32_t record_every, float* rollouts,
+                                       size_t rollout_bytes, int32_t* steps_issued);
 
 #ifdef __cplusplus
 }

@@ -56,6 +56,7 @@ class TrialResult(C.Structure):
 
 
 TRIAL_GOAL, TRIAL_MAX_STEPS, TRIAL_LEFT_MAP = 1, 2, 3
+TRIALS_MAP, TRIALS_STOCHASTIC, TRIALS_BAREBONE = 0, 1, 2
 
 
 def _load():
@@ -134,6 +135,9 @@ def _load():
                                                 C.POINTER(I32)]),
         "b200mppi_batch_run_barebone_trials": (C.c_int, [P, C.POINTER(TrialDesc), I32, P, P, C.POINTER(TrialResult), P,
                                                          C.POINTER(I32)]),
+        "b200mppi_batch_get_state_rollout": (C.c_int, [P, P, SZ]),
+        "b200mppi_batch_run_trials_recorded": (C.c_int, [P, I32, C.POINTER(TrialDesc), I32, P, P,
+                                                         C.POINTER(TrialResult), P, I32, P, SZ, C.POINTER(I32)]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)          # AttributeError here == ABI drift, fail loudly

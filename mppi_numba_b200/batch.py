@@ -20,6 +20,9 @@ CVaR and update, the map sampling per planner (include/b200mppi.h, batched stoch
 without a host round trip per step (include/b200mppi.h, closed-loop trials); ``MPPI_StochasticBatch.
 run_stochastic_trials`` does the same for use_tdm planners.  ``run_barebone_trials(max_steps)`` runs the barebone
 notebook's closed loop (nominal unicycle, no map) for barebone planners and counts the steps that end in an obstacle.
+
+``get_state_rollout()`` is every planner's get_state_rollout() with one launch, and ``record_every=n`` on any trial call
+records those rollouts at every n-th step inside the episodes, as the notebooks' drawing loop calls it.
 """
 import ctypes as C
 
@@ -117,8 +120,34 @@ class MPPI_Batch(object):
         check(lib.b200mppi_batch_launch_count(self._handle, C.byref(n)))
         return int(n.value)
 
+    def get_state_rollout(self):
+        """Every planner's get_state_rollout() with one launch: np.float32 (K, V, T+1, 3), the state sequences of each
+        planner's current optimal controls (over its first V sampled maps for use_tdm planners; for the others the
+        optimal sequence plus V-1 noisy samples).  Afterwards every planner, its state_rollout_batch_d included, is as
+        after planners[0].get_state_rollout(), planners[1].get_state_rollout(), ...  Raises ValueError (naming the
+        planner) when a planner's params are not set or the planners' num_vis_state_rollouts differ; nothing is issued
+        then."""
+        V = self._vis_count("MPPI_Batch.get_state_rollout")
+        for i, p in enumerate(self.planners):
+            if not p.params_set:
+                raise ValueError("MPPI_Batch.get_state_rollout: planner %d: MPPI parameters are not set" % i)
+        for p in self.planners:
+            p.move_mppi_task_vars_to_device()
+        out = np.empty((len(self.planners), V, self.num_steps + 1, 3), dtype=np.float32)
+        check(lib.b200mppi_batch_get_state_rollout(self._handle, ptr(out), out.nbytes))
+        return out
 
-    def run_trials(self, traction_grids, max_steps, dt=None):
+    def _vis_count(self, name):
+        """V of the batch's visualisation rollouts: every planner's num_vis_state_rollouts, which must be equal."""
+        V = int(self.planners[0].num_vis_state_rollouts)
+        for i, p in enumerate(self.planners):
+            if int(p.num_vis_state_rollouts) != V:
+                raise ValueError("%s: planner %d has num_vis_state_rollouts %d, planner 0 %d (V must be equal)"
+                                 % (name, i, int(p.num_vis_state_rollouts), V))
+        return V
+
+
+    def run_trials(self, traction_grids, max_steps, dt=None, record_every=None):
         """One closed-loop episode per planner, on the GPU: up to ``max_steps`` rounds of ``u = solve()``, a plant step
         on ``traction_grids[k]`` (a ``TractionGrid``, float or ``use_int8``) with ``u[0]`` and ``shift_and_update``,
         stopping once the planner is within ``goal_tolerance`` of its goal -- the loop of the benchmark's ``trial()``,
@@ -132,16 +161,24 @@ class MPPI_Batch(object):
                     that did not reach its goal;
           ``xhist`` float64 (K, max_steps+1, 3) and ``uhist`` float32 (K, max_steps, 2), NaN after a planner's last
           step; ``steps`` (K,) int; ``status`` (K,) of "goal" | "max_steps" | "left_map".
+        ``record_every=n`` also records the visualisation rollouts of every step ``s`` with ``s % n == 0``, what
+        ``get_state_rollout()`` called after the plant step and before ``shift_and_update`` returns (the notebooks'
+        ``t % plot_every_n == 0``), and the dict gains ``state_rollouts`` float32 (K, R, V, T+1, 3), R =
+        ceil(max_steps / n), whose record r belongs to step ``rollout_steps[r]`` = r n and is NaN from the planner's
+        ``steps`` on, and ``rollout_steps`` (R,).  Everything else is as without recording, and each planner's
+        state_rollout_batch_d holds its last record.
         Raises ValueError (naming the planner) for barebone batches, a grid count other than K, max_steps < 1,
-        num_opt < 1, a grid of another dtype than float64 or integer, or a planner that cannot solve (e.g. its start
-        pose is outside the padded map limits); B200MPPIError when the planners' maps cannot all be sampled by the
-        batch's one sampler launch.  Nothing is issued when the call is refused."""
+        num_opt < 1, a grid of another dtype than float64 or integer, a planner that cannot solve (e.g. its start
+        pose is outside the padded map limits), record_every < 1 and unequal num_vis_state_rollouts; B200MPPIError
+        when the planners' maps cannot all be sampled by the batch's one sampler launch.  Nothing is issued when the
+        call is refused."""
         if self.kind not in ("det", "spd"):
             raise ValueError("MPPI_Batch.run_trials: planner 0 is a %s planner (trials need det-dynamics or speed-map "
                              "planners)" % self.kind)
-        return self._trials("MPPI_Batch.run_trials", lib.b200mppi_batch_run_trials, traction_grids, max_steps, dt)
+        return self._trials("MPPI_Batch.run_trials", lib.b200mppi_batch_run_trials, traction_grids, max_steps, dt,
+                            record_every, _lib.TRIALS_MAP)
 
-    def run_barebone_trials(self, max_steps, dt=None):
+    def run_barebone_trials(self, max_steps, dt=None, record_every=None):
         """The barebone notebook's closed loop for every planner at once, on the GPU: up to ``max_steps`` rounds of
         ``u = solve()``, a nominal unicycle step with ``u[0]`` in float64 (``dt`` as a float64, default: each planner's
         ``params['dt']``) and ``shift_and_update``, stopping once the planner is within ``goal_tolerance`` of its goal.
@@ -156,20 +193,21 @@ class MPPI_Batch(object):
                     is no cum_obj);
           ``xhist`` float64 (K, max_steps+1, 3) and ``uhist`` float32 (K, max_steps, 2), NaN after a planner's last
           step; ``steps`` (K,) int; ``status`` (K,) of "goal" | "max_steps"; ``contact_steps`` (K,) int, the steps
-          whose new pose touched an obstacle.
+          whose new pose touched an obstacle.  ``record_every`` as in run_trials.
         Raises ValueError (naming the planner) for other batches, max_steps < 1, num_opt < 1, a planner that cannot
-        solve, a non-finite x0, xgoal or goal_tolerance, or a dt that is not finite and positive.  Nothing is issued
-        when the call is refused."""
+        solve, a non-finite x0, xgoal or goal_tolerance, a dt that is not finite and positive, record_every < 1 and
+        unequal num_vis_state_rollouts.  Nothing is issued when the call is refused."""
         if self.kind != "barebone":
             raise ValueError("MPPI_Batch.run_barebone_trials: planner 0 is a %s planner (barebone trials run barebone "
                              "planners; run_trials runs det-dynamics and speed-map planners)" % self.kind)
         return self._trials("MPPI_Batch.run_barebone_trials", lib.b200mppi_batch_run_barebone_trials, None, max_steps,
-                            dt)
+                            dt, record_every, _lib.TRIALS_BAREBONE)
 
-    def _trials(self, name, entry, traction_grids, max_steps, dt):
-        """The marshalling of a closed-loop trial call through the C entry point ``entry`` and the logs built from its
-        results (run_trials, run_barebone_trials with traction_grids None, MPPI_StochasticBatch.run_stochastic_trials);
-        ``name`` prefixes the refusals."""
+    def _trials(self, name, entry, traction_grids, max_steps, dt, record_every, kind):
+        """The marshalling of a closed-loop trial call through the C entry point ``entry`` (with record_every set:
+        b200mppi_batch_run_trials_recorded with trial kind ``kind``) and the logs built from its results (run_trials,
+        run_barebone_trials with traction_grids None, MPPI_StochasticBatch.run_stochastic_trials); ``name`` prefixes
+        the refusals."""
         K = len(self.planners)
         barebone = traction_grids is None
         grids = [None] * K if barebone else list(traction_grids)
@@ -178,6 +216,11 @@ class MPPI_Batch(object):
         max_steps = int(max_steps)
         if max_steps < 1:
             raise ValueError("%s: max_steps %d < 1" % (name, max_steps))
+        if record_every is not None:
+            record_every = int(record_every)
+            if record_every < 1:
+                raise ValueError("%s: record_every %d < 1" % (name, record_every))
+            V = self._vis_count(name)
         descs = (_lib.TrialDesc * K)()
         keep = []
         for i, (p, g) in enumerate(zip(self.planners, grids)):
@@ -223,8 +266,15 @@ class MPPI_Batch(object):
         res = (_lib.TrialResult * K)()
         issued = C.c_int32()
         contacts = np.zeros(K, dtype=np.int32)
-        outs = (ptr(xhist), ptr(uhist), res) + ((ptr(contacts),) if barebone else ())
-        check(entry(self._handle, descs, max_steps, *outs, C.byref(issued)))
+        if record_every is None:
+            outs = (ptr(xhist), ptr(uhist), res) + ((ptr(contacts),) if barebone else ())
+            check(entry(self._handle, descs, max_steps, *outs, C.byref(issued)))
+        else:
+            R = -(-max_steps // record_every)
+            rollouts = np.empty((K, R, V, self.num_steps + 1, 3), dtype=np.float32)
+            check(lib.b200mppi_batch_run_trials_recorded(self._handle, kind, descs, max_steps, ptr(xhist), ptr(uhist),
+                                                         res, ptr(contacts) if barebone else None, record_every,
+                                                         ptr(rollouts), rollouts.nbytes, C.byref(issued)))
         self.steps_issued = int(issued.value)
         steps = np.array([r.steps for r in res], dtype=np.int64)
         status = [TRIAL_STATUS[r.status] for r in res]
@@ -249,6 +299,9 @@ class MPPI_Batch(object):
         out = dict(logs=logs, xhist=xhist, uhist=uhist, steps=steps, status=status)
         if barebone:
             out["contact_steps"] = contacts.astype(np.int64)
+        if record_every is not None:
+            out["state_rollouts"] = rollouts
+            out["rollout_steps"] = np.arange(R, dtype=np.int64) * record_every
         return out
 
 
@@ -279,23 +332,25 @@ class MPPI_StochasticBatch(MPPI_Batch):
         stochastic planner's own solve() leaves it."""
         return self._solve("MPPI_StochasticBatch")
 
-    def run_trials(self, traction_grids, max_steps, dt=None):
+    def run_trials(self, traction_grids, max_steps, dt=None, record_every=None):
         raise ValueError("MPPI_StochasticBatch.run_trials: closed-loop trials run det-dynamics or speed-map batches "
                          "(a stochastic batch runs them with run_stochastic_trials)")
 
-    def run_barebone_trials(self, max_steps, dt=None):
+    def run_barebone_trials(self, max_steps, dt=None, record_every=None):
         raise ValueError("MPPI_StochasticBatch.run_barebone_trials: barebone trials run barebone batches (a stochastic "
                          "batch runs its trials with run_stochastic_trials)")
 
-    def run_stochastic_trials(self, traction_grids, max_steps, dt=None):
+    def run_stochastic_trials(self, traction_grids, max_steps, dt=None, record_every=None):
         """MPPI_Batch.run_trials for use_tdm planners: the same arguments, episode, stop rules, returned dict and NaN
         conventions, one episode per planner on the GPU without a host round trip per step (each planner's
         map-sampling reach box is decided on the device).  Afterwards every planner is exactly as after ``steps[k]``
         rounds of ``u = batch.solve()``, the plant step on ``traction_grids[k]`` and ``shift_and_update(x_next, u[k])``:
         controls, noise, per-(m, n) and CVaR costs, weights, RNG streams, its TDMs' streams and sampled maps,
         ``sample_box()`` and ``params['x0']``.  u_prev_d is left alone, as a stochastic solve leaves it.
+        ``record_every`` as in run_trials: the records equal ``get_state_rollout()`` of that host loop, which completes
+        the maps of a boxed sampling first.
         Raises ValueError (naming the planner) as run_trials does; B200MPPIError when a planner cannot take the windowed
         rollout or its TDM pair cannot join the batch's one sampler launch.  Nothing is issued when the call is
         refused."""
         return self._trials("MPPI_StochasticBatch.run_stochastic_trials", lib.b200mppi_batch_run_stochastic_trials,
-                            traction_grids, max_steps, dt)
+                            traction_grids, max_steps, dt, record_every, _lib.TRIALS_STOCHASTIC)

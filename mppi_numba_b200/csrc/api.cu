@@ -1796,6 +1796,9 @@ struct b200mppi_batch {
   bool stochastic = false;
   int M = 0;
   size_t off_win = 0, off_tm = 0, off_cvar = 0;
+  // b200mppi_batch_get_state_rollout's section, after the solve's (a solve does not upload it):
+  // [RolloutParams K | VisBatchDesc K] from off_vis, vis_bytes long
+  size_t off_vis = 0, off_visd = 0, vis_bytes = 0;
 };
 
 static size_t align256(size_t v) { return (v + 255) / 256 * 256; }
@@ -1826,11 +1829,14 @@ static int batch_init(b200mppi_batch* b) {
     b->off_upd = b->off_roll + align256(K * sizeof(RolloutArgs));
   }
   b->desc_bytes = b->off_upd + align256(K * sizeof(UpdateBatchDesc));
+  b->off_vis = b->desc_bytes;
+  b->off_visd = b->off_vis + align256(K * sizeof(RolloutParams));
+  b->vis_bytes = b->off_visd + align256(K * sizeof(VisBatchDesc)) - b->off_vis;
   CU(cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
   b->own_stream = true;
   CU(cudaEventCreateWithFlags(&b->ev, cudaEventDisableTiming));
-  CU(cudaMallocHost(&b->h_desc, b->desc_bytes));
-  CU(cudaMalloc(&b->d_desc, b->desc_bytes));
+  CU(cudaMallocHost(&b->h_desc, b->desc_bytes + b->vis_bytes));
+  CU(cudaMalloc(&b->d_desc, b->desc_bytes + b->vis_bytes));
   const size_t ubytes = K * (size_t)b->T * 2 * sizeof(float);
   CU(cudaMallocHost(&b->h_u, ubytes));
   CU(cudaMalloc(&b->u_d, ubytes));
@@ -2214,6 +2220,81 @@ extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
   return B200MPPI_OK;
 }
 
+// --------------------------------------------------------------------------------------------- visualisation rollouts
+static int vis_count(const b200mppi_planner* p) {
+  return p->cfg.num_vis_state_rollouts < 1 ? 1 : p->cfg.num_vis_state_rollouts;
+}
+
+// The batch's V, checked before any work is issued: every planner ready (what get_state_rollout checks), equal V, and V
+// within each planner's sampled maps (MODE_TDM) or control rollouts.  `fn` prefixes the messages.
+static int batch_vis_validate(b200mppi_batch* b, const std::string& fn, int* V) {
+  const int V0 = vis_count(b->pl[0]);
+  for (int i = 0; i < (int)b->pl.size(); ++i) {
+    b200mppi_planner* p = b->pl[i];
+    const std::string who = fn + ": planner " + std::to_string(i);
+    const int rc = planner_check_ready(p);
+    if (rc) return fail(rc, who + ": " + g_err);
+    const int v = vis_count(p);
+    if (v != V0)
+      return fail(B200MPPI_EINVAL, who + " has num_vis_state_rollouts " + std::to_string(v) + ", planner 0 " +
+                                       std::to_string(V0) + " (V must be equal)");
+    const bool tdm = p->cfg.mode == B200MPPI_MODE_TDM;
+    if (tdm ? v > p->lin->num_maps : v > p->n_local)
+      return fail(B200MPPI_EINVAL, who + " has num_vis_state_rollouts " + std::to_string(v) + ", more than its " +
+                                       std::to_string(tdm ? p->lin->num_maps : p->n_local) +
+                                       (tdm ? " sampled maps" : " control rollouts"));
+  }
+  *V = V0;
+  return B200MPPI_OK;
+}
+
+// planner p's visualisation rollouts with its RolloutParams at dp (device) into out (device, (V, T+1, 3))
+static VisBatchDesc vis_desc(const b200mppi_planner* p, const RolloutParams* dp, float* out) {
+  VisBatchDesc v{};
+  v.p = dp;
+  v.mode = p->cfg.mode; v.V = vis_count(p);
+  if (p->cfg.mode != B200MPPI_MODE_BAREBONE) { v.lin_grid = p->lin->grid; v.ang_grid = p->ang->grid; }
+  v.noise = p->noise; v.u_cur = p->u_cur; v.u_prev = p->u_prev; v.out = out;
+  return v;
+}
+
+extern "C" int b200mppi_batch_get_state_rollout(b200mppi_batch* b, float* out, size_t bytes) {
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  if (!out) return fail(B200MPPI_EINVAL, "batch_get_state_rollout: null output");
+  int V = 0;
+  int rc = batch_vis_validate(b, "batch_get_state_rollout", &V);
+  if (rc) return rc;
+  const int K = (int)b->pl.size();
+  const size_t per = (size_t)V * (b->T + 1) * 3;
+  if (bytes != (size_t)K * per * sizeof(float))
+    return fail(B200MPPI_EINVAL, "batch_get_state_rollout: size mismatch (" + std::to_string(bytes) + " bytes, (K, V, "
+                                 "T+1, 3) float32 is " + std::to_string((size_t)K * per * sizeof(float)) + ")");
+  CU(cudaSetDevice(b->device));
+  cudaStream_t st = b->stream;
+  if ((rc = batch_wait_members(b))) return rc;
+  RolloutParams* hp = reinterpret_cast<RolloutParams*>(b->h_desc + b->off_vis);
+  VisBatchDesc* hv = reinterpret_cast<VisBatchDesc*>(b->h_desc + b->off_visd);
+  const RolloutParams* dp = reinterpret_cast<const RolloutParams*>(b->d_desc + b->off_vis);
+  for (int i = 0; i < K; ++i) {
+    b200mppi_planner* p = b->pl[i];
+    if (p->cfg.mode != B200MPPI_MODE_BAREBONE) {   // as get_state_rollout: the maps of a boxed solve are completed
+      if ((rc = tdm_complete_grid(p->lin, st))) return rc;
+      if ((rc = tdm_complete_grid(p->ang, st))) return rc;
+    }
+    hp[i] = RolloutParams{};
+    fill_rollout_params(p, hp[i]);
+    hv[i] = vis_desc(p, dp + i, p->state_rollout);
+  }
+  CU(cudaMemcpyAsync(b->d_desc + b->off_vis, b->h_desc + b->off_vis, b->vis_bytes, cudaMemcpyHostToDevice, st));
+  launch_state_rollout_batch(reinterpret_cast<const VisBatchDesc*>(b->d_desc + b->off_visd), K, V, nullptr, 0, st);
+  b->launches++;
+  CHECK_LAUNCH();
+  for (int i = 0; i < K; ++i)
+    CU(cudaMemcpyAsync(out + (size_t)i * per, b->pl[i]->state_rollout, per * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return B200MPPI_OK;
+}
+
 // --------------------------------------------------------------------------------------------- closed-loop trials
 // A batch's planners run whole receding-horizon episodes on the device.  Only x0 (written by the plant kernel into the
 // rollout descriptors) and the parity of the TDMs' generator-state double buffers change from step to step: every
@@ -2334,14 +2415,19 @@ static const char* mode_name(int mode) {
 // (noise [+ controls], [first iteration, not barebone: sampler (stochastic: boxed, then the state advance)], rollout
 // [windowed, then CVaR], update) and the plant step, which for stochastic trials also moves each planner's rollout
 // window and for barebone trials counts obstacle contacts.
+// record_every = n > 0 records the visualisation rollouts of every step s with s % n == 0, after the step's last update
+// and before the plant step (which shifts u_cur and overwrites x0): one batched launch, and for a stochastic batch first
+// one launch that completes maps [0, V) of every pair whose step sampled a box (the maps the rollouts read).
 // Device buffer of a call: [descriptors (b->h_desc's layout; a one-map batch's parity-0 sampler set is its own section
 // there) | stochastic: the parity-0 sampler set | not barebone: the parity-1 set | stochastic: box descriptors, box
-// records | states | barebone: contacts | trials | active K + count | not barebone: grids | xhist | uhist].  The pinned
-// staging mirrors it up to the grids, then holds xhist and uhist: the float64 ground-truth grids (tens of MB for a batch
-// of large maps) are copied straight from the caller's arrays.
+// records | states | barebone: contacts | trials | active K + count | recording: vis descriptors | not barebone: grids |
+// recording: the records (K, R, V, T+1, 3) | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds
+// xhist and uhist: the float64 ground-truth grids (tens of MB for a batch of large maps) are copied straight from the
+// caller's arrays, and the written records (of K * R * V * (T+1) * 12 bytes, 145 MB for K 8, 150 steps, V 100, T 100)
+// straight into the caller's array.
 static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_trial_desc* trials, int32_t max_steps,
                             double* xhist, float* uhist, b200mppi_trial_result* results, int32_t* contact_steps,
-                            int32_t* steps_issued) {
+                            int32_t record_every, float* rollouts, size_t rollout_bytes, int32_t* steps_issued) {
   const bool stochastic = kind == TrialKind::stochastic, barebone = kind == TrialKind::barebone;
   const std::string fn = stochastic ? "run_stochastic_trials" : barebone ? "run_barebone_trials" : "run_trials";
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
@@ -2359,10 +2445,22 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   if (rc) return rc;
   if (!xhist || !uhist || !results || (barebone && !contact_steps))
     return fail(B200MPPI_EINVAL, fn + ": null output buffer");
+  const int K = (int)b->pl.size(), T = b->T, N = b->N, S = max_steps;
+  const bool record = record_every > 0;
+  int V = 0, R = 0;
+  size_t per = 0, rec_bytes = 0;                       // floats of one planner's record, bytes of all records
+  if (record) {
+    if ((rc = batch_vis_validate(b, fn, &V))) return rc;
+    R = (S + record_every - 1) / record_every;
+    per = (size_t)V * (T + 1) * 3;
+    rec_bytes = (size_t)K * R * per * sizeof(float);
+    if (!rollouts || rollout_bytes != rec_bytes)
+      return fail(B200MPPI_EINVAL, fn + ": rollouts buffer of " + std::to_string(rollout_bytes) + " bytes, the records "
+                                   "(K, R, V, T+1, 3) float32 need " + std::to_string(rec_bytes));
+  }
   int WW = 0, WH = 0;
   if (stochastic && (rc = stochastic_validate(b, fn.c_str(), &WW, &WH))) return rc;
   CU(cudaSetDevice(b->device));
-  const int K = (int)b->pl.size(), T = b->T, N = b->N, S = max_steps;
   cudaStream_t st = b->stream;
   // the sampler plans first (their host preparation may synchronise the stream): every pair must join the one launch
   std::vector<SamplePlan> plans;
@@ -2392,13 +2490,16 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   const size_t off_con = off_state + align256((size_t)K * sizeof(TrialState));
   const size_t off_tr = off_con + align256(ncon * sizeof(int));
   const size_t off_act = off_tr + align256((size_t)K * sizeof(TrialDev));
-  size_t off = off_act + align256((size_t)(K + 1) * sizeof(int));
+  const size_t off_vis = off_act + align256((size_t)(K + 1) * sizeof(int));
+  size_t off = off_vis + align256((record ? (size_t)K : 0) * sizeof(VisBatchDesc));
   const size_t head = off;
   std::vector<size_t> off_grid(K);
   for (int i = 0; i < K; ++i) {
     off_grid[i] = off;
     if (!barebone) off += align256((size_t)2 * trials[i].height * trials[i].width * sizeof(double));
   }
+  const size_t off_vrec = off;
+  off += align256(rec_bytes);
   const size_t off_xh = off, off_uh = off_xh + align256((size_t)K * (S + 1) * 3 * sizeof(double));
   const size_t total = off_uh + align256((size_t)K * S * 2 * sizeof(float));
   struct Buffers {                                     // freed on every return
@@ -2432,9 +2533,13 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   RolloutArgs* dr = reinterpret_cast<RolloutArgs*>(d + b->off_roll);
   RolloutWinArgs* dw = reinterpret_cast<RolloutWinArgs*>(d + b->off_win);
   int* hcon = reinterpret_cast<int*>(h + off_con);
+  VisBatchDesc* hv = reinterpret_cast<VisBatchDesc*>(h + off_vis);
+  float* drec = reinterpret_cast<float*>(d + off_vrec);
   for (int i = 0; i < K; ++i) {
     b200mppi_planner* p = b->pl[i];
     const b200mppi_trial_desc& q = trials[i];
+    if (record)                                        // x0 from the record the plant step writes
+      hv[i] = vis_desc(p, stochastic ? &dw[i].p : &dr[i].p, drec + (size_t)i * R * per);
     TrialDev& t = ht[i];
     t = TrialDev{};
     t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1]; t.tol = q.goal_tolerance;
@@ -2525,10 +2630,21 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       launch_update_partial_batch(du, K, b->pl[0]->num_ctas, dact, st);
       CHECK_LAUNCH();
     }
+    const bool rec_step = record && s % record_every == 0;
+    if (rec_step) {
+      if (stochastic) {                               // from the pre-call states this step's sampling read
+        launch_sample_grids_v2_complete_batch(geom, ds[s & 1], db, K, dact, V, mrows, ncact, st);
+        CHECK_LAUNCH();
+      }
+      launch_state_rollout_batch(reinterpret_cast<const VisBatchDesc*>(d + off_vis), K, V, dact,
+                                 (size_t)(s / record_every) * per, st);
+      CHECK_LAUNCH();
+    }
     pa.step = s;
     launch_plant_step(pa, st);
     CHECK_LAUNCH();
     b->launches += stochastic ? 4 * num_opt + 3 : barebone ? 3 * num_opt + 1 : 3 * num_opt + 2;
+    if (rec_step) b->launches += stochastic ? 2 : 1;
     ++issued;
     CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, dact + K, sizeof(int), cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(buf.ev[s % TRIAL_POLL], st));
@@ -2572,6 +2688,21 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     p->pushed_direct = false;
     for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)xo[(size_t)(n - 1) * 3 + c];
   }
+  if (record) {
+    // record r belongs to step r * record_every.  Only the written ones are copied (records past a planner's last step
+    // are never written, and an early stop leaves most of them so): the rest is NaN.  The last one is what the
+    // planner's state_rollout buffer holds after the host loop's last get_state_rollout.
+    for (int i = 0; i < K; ++i) {
+      const int done = (hst[i].steps + record_every - 1) / record_every;
+      float* slab = rollouts + (size_t)i * R * per;
+      CU(cudaMemcpyAsync(slab, drec + (size_t)i * R * per, (size_t)done * per * sizeof(float), cudaMemcpyDeviceToHost,
+                         st));
+      CU(cudaMemcpyAsync(b->pl[i]->state_rollout, drec + ((size_t)i * R + done - 1) * per, per * sizeof(float),
+                         cudaMemcpyDeviceToDevice, st));
+      std::fill(slab + (size_t)done * per, slab + (size_t)R * per, fnan);
+    }
+    CU(cudaStreamSynchronize(st));
+  }
   if (steps_issued) *steps_issued = issued;
   return B200MPPI_OK;
 }
@@ -2579,19 +2710,37 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
 extern "C" int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps,
                                          double* xhist, float* uhist, b200mppi_trial_result* results,
                                          int32_t* steps_issued) {
-  return batch_run_trials(b, TrialKind::onemap, trials, max_steps, xhist, uhist, results, nullptr, steps_issued);
+  return batch_run_trials(b, TrialKind::onemap, trials, max_steps, xhist, uhist, results, nullptr, 0, nullptr, 0,
+                          steps_issued);
 }
 
 extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials,
                                                     int32_t max_steps, double* xhist, float* uhist,
                                                     b200mppi_trial_result* results, int32_t* steps_issued) {
-  return batch_run_trials(b, TrialKind::stochastic, trials, max_steps, xhist, uhist, results, nullptr, steps_issued);
+  return batch_run_trials(b, TrialKind::stochastic, trials, max_steps, xhist, uhist, results, nullptr, 0, nullptr, 0,
+                          steps_issued);
 }
 
 extern "C" int b200mppi_batch_run_barebone_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials,
                                                   int32_t max_steps, double* xhist, float* uhist,
                                                   b200mppi_trial_result* results, int32_t* contact_steps,
                                                   int32_t* steps_issued) {
-  return batch_run_trials(b, TrialKind::barebone, trials, max_steps, xhist, uhist, results, contact_steps,
-                          steps_issued);
+  return batch_run_trials(b, TrialKind::barebone, trials, max_steps, xhist, uhist, results, contact_steps, 0, nullptr,
+                          0, steps_issued);
+}
+
+extern "C" int b200mppi_batch_run_trials_recorded(b200mppi_batch* b, int32_t kind, const b200mppi_trial_desc* trials,
+                                                  int32_t max_steps, double* xhist, float* uhist,
+                                                  b200mppi_trial_result* results, int32_t* contact_steps,
+                                                  int32_t record_every, float* rollouts, size_t rollout_bytes,
+                                                  int32_t* steps_issued) {
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  if (kind != B200MPPI_TRIALS_MAP && kind != B200MPPI_TRIALS_STOCHASTIC && kind != B200MPPI_TRIALS_BAREBONE)
+    return fail(B200MPPI_EINVAL, "run_trials_recorded: unknown trial kind " + std::to_string(kind));
+  if (record_every < 1)
+    return fail(B200MPPI_EINVAL, "run_trials_recorded: record_every " + std::to_string(record_every) + " < 1");
+  const TrialKind k = kind == B200MPPI_TRIALS_STOCHASTIC ? TrialKind::stochastic
+                      : kind == B200MPPI_TRIALS_BAREBONE ? TrialKind::barebone : TrialKind::onemap;
+  return batch_run_trials(b, k, trials, max_steps, xhist, uhist, results, contact_steps, record_every, rollouts,
+                          rollout_bytes, steps_issued);
 }

@@ -201,6 +201,11 @@ void launch_sample_grids_v2_box_batch(const SampleGridsV2Args& geom, const Sampl
                                       int ncact, cudaStream_t st);
 // the launch above holds ncact tile columns with geom.gm maps per CTA (threads, shared memory)
 bool sample_box_batch_fits(const SampleGridsV2Args& geom, int ncact);
+// recording stochastic trials: whole maps [0, map_end) of every pair whose step sampled a box (record[0] != 0), from the
+// pre-call states of descs[pair].t[0], with the launch geometry of the box launch; no state stores
+void launch_sample_grids_v2_complete_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
+                                           const SampleBoxDesc* boxes, int count, const int* active, int map_end,
+                                           int mrows, int ncact, cudaStream_t st);
 // launch_advance_states for `count` pairs (pair blockIdx.y): descs[y].t[0].states -> both TDMs' states_out
 void launch_advance_states_batch(const SampleGridsV2Args* descs, const SampleBoxDesc* boxes, int count, int rows,
                                  int cols, int tx, int ty, int num_maps, const int* active, cudaStream_t st);
@@ -474,8 +479,20 @@ struct VisArgs {
   const float* noise; const float* u_cur; const float* u_prev;
   float* out;   // (V, T+1, 3)
 };
+// batched visualisation rollouts (b200mppi_batch_get_state_rollout, recording closed-loop trials): one per planner
+struct VisBatchDesc {
+  const RolloutParams* p;   // RolloutArgs::p (one-map, barebone) or RolloutWinArgs::p (stochastic) in device memory
+  int mode, V;
+  const int8_t* lin_grid; const int8_t* ang_grid;
+  const float* noise; const float* u_cur; const float* u_prev;
+  float* out;               // (V, T+1, 3), plus the launch's out_off
+};
 // [emu:end vis_args]
 void launch_state_rollout(const VisArgs& a, cudaStream_t st);
+// ONE launch for `count` planners of equal V and T (planner = blockIdx.y); active (device, may be null): active[y] == 0
+// -> that planner is left untouched
+void launch_state_rollout_batch(const VisBatchDesc* descs, int count, int V, const int* active, size_t out_off,
+                                cudaStream_t st);
 
 // peer-memory exchange of the sharded solve (p2p.cu)
 struct P2PPushArgs {

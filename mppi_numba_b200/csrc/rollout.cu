@@ -469,7 +469,7 @@ void launch_cvar(const float* costs_mn, float* costs, int n_cnt, int ld, int M, 
 // Visualisation rollouts (mppi.py:1194-1351).  mode != 0: block 0 rolls out u_cur without noise,
 // block b > 0 rolls out clip(u_prev + eps[b]) ; mode 0: u_cur over the first V sampled maps.
 // [emu:begin vis]
-__global__ void state_rollout_kernel(const VisArgs a) {
+__device__ __forceinline__ void state_rollout_body(const VisArgs& a) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= a.V) return;
   const RolloutParams& p = a.p;
@@ -519,9 +519,36 @@ __global__ void state_rollout_kernel(const VisArgs a) {
   }
 }
 
+__global__ void state_rollout_kernel(const VisArgs a) {
+  state_rollout_body(a);
+}
+
 // [emu:end vis]
+// [emu:begin vis_batch]
+// the visualisation rollouts of `count` planners of equal V and T, planner blockIdx.y: its VisArgs from the descriptor,
+// the RolloutParams (x0 included) read where the batch's rollout descriptors hold them, the output at d.out + out_off
+// (closed-loop trials: the record of this step).  A planner with active[y] == 0 is left untouched (active null: every
+// planner runs).
+__global__ void state_rollout_batch_kernel(const VisBatchDesc* __restrict__ descs, const int* __restrict__ active,
+                                           size_t out_off) {
+  if (active && !active[blockIdx.y]) return;
+  const VisBatchDesc& d = descs[blockIdx.y];
+  VisArgs a;
+  a.p = *d.p;
+  a.mode = d.mode; a.V = d.V;
+  a.lin_grid = d.lin_grid; a.ang_grid = d.ang_grid;
+  a.noise = d.noise; a.u_cur = d.u_cur; a.u_prev = d.u_prev;
+  a.out = d.out + out_off;
+  state_rollout_body(a);
+}
+// [emu:end vis_batch]
 void launch_state_rollout(const VisArgs& a, cudaStream_t st) {
   state_rollout_kernel<<<(a.V + 31) / 32, 32, 0, st>>>(a);
+}
+
+void launch_state_rollout_batch(const VisBatchDesc* descs, int count, int V, const int* active, size_t out_off,
+                                cudaStream_t st) {
+  state_rollout_batch_kernel<<<dim3((unsigned)((V + 31) / 32), (unsigned)count), 32, 0, st>>>(descs, active, out_off);
 }
 
 }  // namespace b200

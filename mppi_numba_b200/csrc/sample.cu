@@ -207,8 +207,9 @@ constexpr bool SG_VALUES_IN_REGISTERS = false;
 #endif
 constexpr bool SG_POPC_PER_WORD = SG_POPC_VARIANT;
 
-template <int NT, int NW>
-__device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a) {
+// BOUNDED: only maps [0, map_end) are sampled (else all a.num_maps); the generator of map m is the same either way
+template <int NT, int NW, bool BOUNDED = false>
+__device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a, int map_end = 0) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int nw = (NW > 0) ? NW : a.t[0].bpad / 4;
   const int bpad = nw * 4;
@@ -261,7 +262,7 @@ __device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a)
   const int tid = threadIdx.x, nthreads = blockDim.x;
   const int tiy = tiy_lo + tid % nact, mloc = tid / nact;
   const int m = blockIdx.y * gm + mloc;
-  const bool active = (mloc < gm) && (m < a.num_maps);
+  const bool active = (mloc < gm) && (m < (BOUNDED ? map_end : a.num_maps));
 
   for (int i = tid; i < SAMPLE_TABLE_WORDS; i += nthreads) s_T[i] = a.thresholds[i];
   // value table indexed by ge = number of cumulative bytes >= q (the SIMD compare yields that count directly):
@@ -396,7 +397,7 @@ __device__ __forceinline__ void sample_grids_v2_body(const SampleGridsV2Args& a)
     if (ri + 1 < rs1) stage_cum_row(ri + 1);
     // coalesced write-back of the gm x NT staged rows: 16-byte chunks, bytes at the ragged ends of the window
     const int chunks = (wcols + 15) / 16;
-    const int maps_here = min(gm, a.num_maps - (int)blockIdx.y * gm);
+    const int maps_here = min(gm, (BOUNDED ? map_end : a.num_maps) - (int)blockIdx.y * gm);
     for (int idx = tid; idx < NT * maps_here * chunks; idx += nthreads) {
       const int ch = idx % chunks;
       const int km = idx / chunks;
@@ -475,6 +476,26 @@ __global__ void __launch_bounds__(256) sample_grids_v2_batch_kernel(const Sample
 // first one; a CTA narrows to the box rows, columns and disc as the single boxed launch does, so it writes the same
 // cells with the same draws.  A whole-map step (and any box larger than the launch) loops over groups of mrows tile rows
 // and ncact tile columns.
+// The passes of one CTA over tile rows [tix_lo, tix_hi) and tile columns [tiy_lo, tiy_hi) of maps [0, map_end).
+template <int NW>
+__device__ __forceinline__ void box_batch_passes(SampleGridsV2Args& a, int tix_lo, int tix_hi, int tiy_lo, int tiy_hi,
+                                                 int mrows, int ncact, int map_end) {
+  const int nrow = (a.rows + a.tx - 1) / a.tx;
+  const int tsub = (int)blockIdx.x / a.segs, seg = (int)blockIdx.x % a.segs;
+  for (int tg = tix_lo; tg < tix_hi; tg += mrows) {
+    const int tix = tg + tsub;
+    if (tix >= tix_hi) continue;                                   // CTA-uniform
+    const int t0 = min(tix * nrow, a.rows), t1 = min(t0 + nrow, a.rows);
+    const int r0 = min(t0 + seg * a.seg_rows, t1), r1 = min(r0 + a.seg_rows, t1);
+    if (max(r0, a.row_lo) >= min(r1, a.row_hi)) continue;          // no box rows in this segment
+    for (int cg = tiy_lo; cg < tiy_hi; cg += ncact) {
+      a.tix_lo = tg; a.tiy_lo = cg; a.nact = min(ncact, tiy_hi - cg);
+      sample_grids_v2_body<2, NW, true>(a, map_end);
+      __syncthreads();                                             // the next pass restages the shared memory
+    }
+  }
+}
+
 template <int NW>
 __global__ void __launch_bounds__(256) sample_grids_v2_box_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
                                                                         const SampleBoxDesc* __restrict__ boxes,
@@ -500,19 +521,22 @@ __global__ void __launch_bounds__(256) sample_grids_v2_box_batch_kernel(const Sa
     tiy_lo = b.tiy_lo; tiy_hi = b.tiy_lo + b.nact;
   }
   a.write_states = 0;
-  const int tsub = (int)blockIdx.x / a.segs, seg = (int)blockIdx.x % a.segs;
-  for (int tg = tix_lo; tg < tix_hi; tg += mrows) {
-    const int tix = tg + tsub;
-    if (tix >= tix_hi) continue;                                   // CTA-uniform
-    const int t0 = min(tix * nrow, a.rows), t1 = min(t0 + nrow, a.rows);
-    const int r0 = min(t0 + seg * a.seg_rows, t1), r1 = min(r0 + a.seg_rows, t1);
-    if (max(r0, a.row_lo) >= min(r1, a.row_hi)) continue;          // no box rows in this segment
-    for (int cg = tiy_lo; cg < tiy_hi; cg += ncact) {
-      a.tix_lo = tg; a.tiy_lo = cg; a.nact = min(ncact, tiy_hi - cg);
-      sample_grids_v2_body<2, NW>(a);
-      __syncthreads();                                             // the next pass restages the shared memory
-    }
-  }
+  box_batch_passes<NW>(a, tix_lo, tix_hi, tiy_lo, tiy_hi, mrows, ncact, a.num_maps);
+}
+
+// recording stochastic trials: the whole maps [0, map_end) of every pair whose step sampled a box (its record says so),
+// re-walked from the step's pre-call states (descs[z].t[0].states) with the launch geometry of the box launch above and
+// no state stores.  Inside the box that rewrites the values the boxed launch wrote; maps >= map_end keep their box.
+template <int NW>
+__global__ void __launch_bounds__(256) sample_grids_v2_complete_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
+                                                                             const SampleBoxDesc* __restrict__ boxes,
+                                                                             const int* __restrict__ active, int map_end,
+                                                                             int mrows, int ncact) {
+  if (active && !active[blockIdx.z]) return;
+  if (boxes[blockIdx.z].record[0] == 0) return;                    // this step sampled whole maps already
+  SampleGridsV2Args a = descs[blockIdx.z];
+  a.write_states = 0;
+  box_batch_passes<NW>(a, 0, a.tx, 0, a.ty, mrows, ncact, map_end);
 }
 
 // the state advance of those boxed samplings for every pair (pair blockIdx.y): lin's states into both TDMs' other buffers
@@ -632,6 +656,23 @@ void launch_sample_grids_v2_box_batch(const SampleGridsV2Args& geom, const Sampl
   else if (nw == 8) go(sample_grids_v2_box_batch_kernel<8>);
   else if (nw == 1) go(sample_grids_v2_box_batch_kernel<1>);
   else go(sample_grids_v2_box_batch_kernel<0>);
+}
+
+void launch_sample_grids_v2_complete_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
+                                           const SampleBoxDesc* boxes, int count, const int* active, int map_end,
+                                           int mrows, int ncact, cudaStream_t st) {
+  const dim3 grid(mrows * geom.segs, (map_end + geom.gm - 1) / geom.gm, count);
+  const int threads = ((ncact * geom.gm + 31) / 32) * 32;
+  const size_t smem = box_batch_smem(geom, ncact);
+  const int nw = geom.t[0].bpad / 4;
+  auto go = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    kern<<<grid, threads, smem, st>>>(descs, boxes, active, map_end, mrows, ncact);
+  };
+  if (nw == 3) go(sample_grids_v2_complete_batch_kernel<3>);
+  else if (nw == 8) go(sample_grids_v2_complete_batch_kernel<8>);
+  else if (nw == 1) go(sample_grids_v2_complete_batch_kernel<1>);
+  else go(sample_grids_v2_complete_batch_kernel<0>);
 }
 
 void launch_advance_states_batch(const SampleGridsV2Args* descs, const SampleBoxDesc* boxes, int count, int rows,
