@@ -2,7 +2,7 @@
 """bench_trials.py -- closed-loop episodes of K planners: the host-driven loop against the batch's device episodes.
 
     python bench_trials.py --workload c2|c4|c3|ref|refm|gif|bb --batch K --closed-loop S [--rounds R] [--profile]
-                           [--record-every n]
+                           [--record-every n] [--share-tdms]
 
 c2 and c4 are one-map workloads (MPPI_Batch.run_trials); c3 and ref are stochastic (use_tdm, CVaR cost:
 MPPI_StochasticBatch.run_stochastic_trials).  ref is the reference benchmark's noisy_dyn trial shape (N 1024, M 1024,
@@ -28,6 +28,13 @@ shift_and_update.  The parity check also holds the device's records (run_trials(
 replayed host loop's get_state_rollout(), bit for bit; the host rounds call it; and device rounds with recording are
 timed alternately with those without.  --profile then profiles a recording round and reports the share of the
 visualisation and map-completion kernels.
+--share-tdms (not bb): many planners on one terrain belief.  The workload becomes seed 1's map with K planners whose
+start poses, warm starts and goals come from seeds 1..K (for ref and refm the planners also cycle cvar_alpha through the
+reference benchmark's [1.0, 0.8, 0.6, 0.4, 0.2]: its noisy_dyn sweep on one environment), and two legs of device
+episodes on the same inputs: K private TDM pairs of that map and ONE pair shared by all K (share_tdms=True: sampled once
+per step while any planner runs).  The parity check holds the histories, steps, statuses (and records), every
+planner's state and the shared pair against the longest-running planner's private pair, byte for byte; then rounds of
+the two legs alternate.  The JSON line adds the device bytes of each leg's TDM allocations, computed from the shapes.
 """
 import argparse
 import functools
@@ -162,6 +169,109 @@ def run(args, emit):
             "closed-loop trials: host-driven loop vs " +
             ("MPPI_StochasticBatch.run_stochastic_trials" if stochastic else "MPPI_Batch.run_trials"), config,
             None if every is None else functools.partial(device_round, record_every=every))
+
+
+BENCH_ALPHAS = [1.0, 0.8, 0.6, 0.4, 0.2]               # the reference benchmark's cvar_alpha sweep
+
+
+def run_shared(args, emit):
+    """--share-tdms: device episodes of K planners on one map, K private TDM pairs against one shared pair."""
+    import torch
+    import __graft_entry__
+    __graft_entry__.build_engine()
+    import mppi_numba_b200 as E
+    from bench_batch import gpu_info, pair_state, planner_state, same, shared_map_planners, tdm_bytes
+    from tests.scenarios import make_scenario
+    K, S, every = args.batch, args.closed_loop, args.record_every
+    mode, N, M, T, H, res, B, da = LOCAL_WORKLOADS.get(args.workload) or WORKLOADS[args.workload]
+    stochastic = mode == "tdm"
+    Batch = E.MPPI_StochasticBatch if stochastic else E.MPPI_Batch
+    trials = ((lambda b, g, s, **kw: b.run_stochastic_trials(g, s, **kw)) if stochastic else
+              (lambda b, g, s, **kw: b.run_trials(g, s, **kw)))
+    W = MAP_WIDTH.get(args.workload, H)
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    scs = []
+    for k in range(K):
+        sc = make_scenario(mode, N=N, M=M, T=T, H=H, W=W, res=res, B=B, seed=k + 1, det_alpha=da, warm_start=True)
+        if args.workload in VIS_ROLLOUTS:
+            sc["cfg"]["num_vis_state_rollouts"] = VIS_ROLLOUTS[args.workload]
+        if k % 2 == 0:
+            sc["params"]["xgoal"] = sc["params"]["x0"][:2] + np.array([1.2, -0.9])
+        scs.append(sc)
+    alphas = BENCH_ALPHAS if args.workload in ("ref", "refm") else None
+    grid = E.TractionGrid(*np.random.default_rng(7).uniform(0.3, 1.0, (2, H, W)), res=res)   # one ground truth
+    grids = [grid] * K
+    with _quiet():
+        P = shared_map_planners(E, scs, False, alphas)    # private pairs
+        Q = shared_map_planners(E, scs, True, alphas)     # one shared pair
+    bp, bq = Batch(P), Batch(Q, share_tdms=True)
+
+    def reset(pls):
+        for p, sc in zip(pls, scs):
+            p.params["x0"] = sc["params"]["x0"].copy()
+            p.u_cur_d.copy_to_device(sc["u0"])
+
+    def leg(b, pls, **kw):
+        reset(pls)
+        o = trials(b, grids, S, **kw)
+        torch.cuda.synchronize(dev)
+        return o
+
+    start = all(same(pair_state(p), pair_state(q)) for p, q in zip(P, Q))
+    kw = {} if every is None else dict(record_every=every)
+    with _quiet():
+        op, oq = leg(bp, P, **kw), leg(bq, Q, **kw)
+    keys = ["xhist", "uhist", "steps"] + ([] if every is None else ["state_rollouts"])
+    ok_hist = all(op[k].tobytes() == oq[k].tobytes() for k in keys) and op["status"] == oq["status"]
+    ok_state = all(same(planner_state(p, stochastic) + [p.params["x0"]], planner_state(q, stochastic) + [q.params["x0"]])
+                   for p, q in zip(P, Q))
+    longest = int(np.argmax(op["steps"]))
+    ok_pair = same(pair_state(Q[0]), pair_state(P[longest]))
+    parity = {"passed": bool(start and ok_hist and ok_state and ok_pair), "same_start": bool(start),
+              "histories_bitwise": bool(ok_hist), "state_bitwise": bool(ok_state),
+              "shared_pair_equals_longest_private": bool(ok_pair), "planners": K, "steps": op["steps"].tolist(),
+              "against": "the same planners' device episodes on K private TDM pairs of the map"}
+    if not parity["passed"]:
+        sys.stderr.write("bench_trials.py: PARITY CHECK FAILED: %s\n" % json.dumps(parity))
+        emit(json.dumps({"metric": "closed-loop trials on one map", "error": "parity_check failed",
+                         "parity_check": parity}))
+        raise SystemExit(3)
+
+    legs = (("private", bp, P), ("shared", bq, Q))
+    res_ = {name: [] for name, _, _ in legs}
+    launches = {}
+    for _ in range(args.rounds):                         # alternate: private, shared, ...
+        for name, b, pls in legs:
+            l0 = b.launch_count()
+            t0 = time.perf_counter()
+            with _quiet():
+                o = leg(b, pls, **kw)
+            res_[name].append((time.perf_counter() - t0, int(o["steps"].sum())))
+            launches[name] = b.launch_count() - l0
+
+    def summary(name, pls):
+        wall = [r[0] for r in res_[name]]
+        med = float(np.median(wall))
+        return {"s_per_round_wall": med, "s_per_round_wall_runs": wall, "control_steps_per_round": res_[name][0][1],
+                "episodes_per_s": K / med, "kernel_launches_per_round": launches[name], "tdm_device_bytes": tdm_bytes(pls)}
+    pri, sha = summary("private", P), summary("shared", Q)
+    config = {"workload": (args.workload if args.workload in LOCAL_WORKLOADS else workload_name_of(args.workload)),
+              "batch": K, "max_steps": S,
+              "planners": "seed 1's map and ground truth; start poses, warm starts of seeds 1..K; even k: goal 1.5 m "
+                          "away, odd k: distant goal" + ("; cvar_alpha cycling %s" % alphas if alphas else "")}
+    if every is not None:
+        config["record_every"] = every
+    emit(json.dumps({"metric": "closed-loop trials of K planners on one map: K private TDM pairs vs one shared pair",
+                     "unit": "episodes/s", "value": sha["episodes_per_s"], "higher_is_better": True, "config": config,
+                     "rounds": args.rounds, "gpu": gpu_info(dev), "parity_check": parity, "private": pri,
+                     "shared": sha, "speedup_wall": pri["s_per_round_wall"] / sha["s_per_round_wall"]}))
+
+
+def _quiet():
+    import contextlib
+    import io
+    return contextlib.redirect_stdout(io.StringIO())
 
 
 def measure(args, emit, host_round, device_round, ba, bb, parity, dev, metric, config, recorded_round=None):
@@ -345,12 +455,16 @@ def main():
     ap.add_argument("--profile", action="store_true", help="then one device round under torch.profiler: kernel split")
     ap.add_argument("--record-every", type=int, default=None, metavar="n",
                     help="record the visualisation rollouts of every n-th step (not bb)")
+    ap.add_argument("--share-tdms", action="store_true",
+                    help="K planners on one map: K private TDM pairs against one pair shared by all (not bb)")
     args = ap.parse_args()
     if args.batch < 1 or args.closed_loop < 1 or args.rounds < 1:
         ap.error("--batch, --closed-loop and --rounds must be at least 1")
     if args.record_every is not None and (args.record_every < 1 or args.workload == "bb"):
         ap.error("--record-every must be at least 1, and the bb workload does not take it")
-    (run_bb if args.workload == "bb" else run)(args, emit)
+    if args.share_tdms and args.workload == "bb":
+        ap.error("--share-tdms: barebone planners have no TDMs")
+    (run_bb if args.workload == "bb" else run_shared if args.share_tdms else run)(args, emit)
 
 
 if __name__ == "__main__":

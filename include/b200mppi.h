@@ -353,6 +353,32 @@ int b200mppi_batch_launch_count(b200mppi_batch* b, int64_t* out);
  *           tensor maps that cannot be encoded).  u_prev is not touched (a stochastic solve does not alias it). */
 int b200mppi_batch_create_stochastic(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out);
 
+/* ------------------------------------------------------------------ planners sharing TDM pairs
+ * b200mppi_batch_share_tdms(b, 1) lets planners of a one-map or stochastic batch share a lin/ang TDM pair (many robots
+ * on one map, or one environment solved at several cvar_alpha): each shared pair is sampled ONCE per call instead of
+ * once per planner.  Off (the default, enable = 0) the batch behaves exactly as described above.  Barebone batches
+ * have no TDMs and accept the call as a no-op.  It applies to batch_solve and to every trial call.
+ *   groups: planners with the same (lin, ang) objects form one group.  Refused before any work (B200MPPI_EINVAL, naming
+ *           both planners): a TDM that is lin of one planner and ang of another, two planners sharing lin but not ang,
+ *           and, in a stochastic batch, members of one group with unequal params.alpha_dyn.
+ *   solve : each group's pair is sampled once, in the first iteration after the noise launch.  Afterwards every planner
+ *           is byte for byte as after its own b200mppi_planner_solve on a PRIVATE copy of its pair taken before the call
+ *           (same PMF, masks, risk map and generator states): u (and the u_prev alias of one-map planners), noise,
+ *           per-(m, n) and CVaR costs, weights and its RNG streams.  The shared TDMs end with the generator states of
+ *           every copy, and their completed maps equal every copy's.  This is not "K solves in order": sequential
+ *           solves would sample a shared pair K times.
+ *   box   : a stochastic group samples one box.  One member: exactly its own reach-box decision, disc included.  Two or
+ *           more: the rectangle hull of the members' boxes without a disc, or whole maps if any member decides whole
+ *           maps or the hull's sampler launch does not fit; the mode is the largest of the members'.
+ *           b200mppi_planner_sample_box of every member reports the box its group sampled -- the one piece of planner
+ *           state that may differ from the private copy's.
+ *   trials: a group's pair is sampled once per step while any member runs and not at all once every member has
+ *           stopped.  Every planner ends as after its own episode on a private copy (planner state as above, histories,
+ *           steps, status, logs and records); the shared TDMs end as the copy of the group's longest-running member.
+ *           sample_box is the box of the planner's own last step.
+ *   A planner alone in its group behaves exactly as without sharing, sample_box included. */
+int b200mppi_batch_share_tdms(b200mppi_batch* b, int32_t enable);
+
 /* ------------------------------------------------------------------ visualisation rollouts of a batch
  * b200mppi_planner_get_state_rollout of every planner of a batch (either kind) with ONE launch: for MODE_TDM planners
  * u_cur over the first V sampled maps, for the others u_cur and V-1 clipped u_prev + noise rollouts (MODE_BAREBONE

@@ -129,6 +129,7 @@ def _load():
         "b200mppi_batch_set_stream": (C.c_int, [P, P]),
         "b200mppi_batch_solve": (C.c_int, [P, P]),
         "b200mppi_batch_launch_count": (C.c_int, [P, C.POINTER(I64)]),
+        "b200mppi_batch_share_tdms": (C.c_int, [P, I32]),
         "b200mppi_batch_run_stochastic_trials": (C.c_int, [P, C.POINTER(TrialDesc), I32, P, P, C.POINTER(TrialResult),
                                                            C.POINTER(I32)]),
         "b200mppi_batch_run_trials": (C.c_int, [P, C.POINTER(TrialDesc), I32, P, P, C.POINTER(TrialResult),

@@ -23,6 +23,10 @@ notebook's closed loop (nominal unicycle, no map) for barebone planners and coun
 
 ``get_state_rollout()`` is every planner's get_state_rollout() with one launch, and ``record_every=n`` on any trial call
 records those rollouts at every n-th step inside the episodes, as the notebooks' drawing loop calls it.
+
+``share_tdms=True`` lets planners share a lin/ang TDM pair (many robots on one map, or one environment solved at several
+cvar_alpha): each shared pair is sampled once per call, and each planner ends as its own call on a private copy of the
+pair would leave it (include/b200mppi.h, planners sharing TDM pairs).
 """
 import ctypes as C
 
@@ -49,9 +53,10 @@ def _kind(p):
 
 
 class MPPI_Batch(object):
-    """Borrows ``planners`` (keeps them alive) and solves them with one launch per stage."""
+    """Borrows ``planners`` (keeps them alive) and solves them with one launch per stage.  ``share_tdms=True``: planners
+    with the same (lin_tdm, ang_tdm) objects form a group whose pair is sampled once per call (see ``solve``)."""
 
-    def __init__(self, planners):
+    def __init__(self, planners, share_tdms=False):
         planners = list(planners)
         if not planners:
             raise ValueError("MPPI_Batch: no planners")
@@ -66,18 +71,44 @@ class MPPI_Batch(object):
             if kind != kinds[0][0]:
                 raise ValueError("MPPI_Batch: planner %d is a %s planner, planner 0 a %s planner (kinds cannot be mixed)"
                                  % (i, kind, kinds[0][0]))
-        self._create(planners, kinds[0][0], lib.b200mppi_batch_create)
+        self._create(planners, kinds[0][0], lib.b200mppi_batch_create, share_tdms)
 
-    def _create(self, planners, kind, create):
-        """Borrow ``planners`` and create the batch's handle with the C constructor ``create``."""
+    def _create(self, planners, kind, create, share_tdms):
+        """Borrow ``planners`` and create the batch's handle with the C constructor ``create``; ``share_tdms``: turn
+        TDM sharing on."""
         self.planners = planners
         self.kind = kind
         self.num_steps = planners[0].num_steps
+        self.share_tdms = bool(share_tdms)
         self._handle = None
         handles = (C.c_void_p * len(planners))(*[p._handle.value for p in planners])
         h = C.c_void_p()
         check(create(handles, len(planners), C.byref(h)))
         self._handle = h
+        if self.share_tdms:
+            check(lib.b200mppi_batch_share_tdms(self._handle, 1))
+
+    def _check_groups(self, name):
+        """With share_tdms: the overlaps between planners' TDMs that sharing refuses (a TDM that is lin_tdm of one
+        planner and ang_tdm of another, lin shared but not ang or the reverse, unequal alpha_dyn on one stochastic
+        pair), as ValueError naming both planners, before any work is issued.  The library refuses the same."""
+        if not self.share_tdms or self.kind == "barebone":
+            return
+        for i, p in enumerate(self.planners):
+            for j, q in enumerate(self.planners[:i]):
+                both = "%s: planners %d and %d" % (name, j, i)
+                if p.lin_tdm is q.ang_tdm or p.ang_tdm is q.lin_tdm:
+                    raise ValueError(both + ": a TDM is lin_tdm of one and ang_tdm of the other (a shared TDM pair "
+                                     "must be the same (lin_tdm, ang_tdm) of every planner on it)")
+                if (p.lin_tdm is q.lin_tdm) != (p.ang_tdm is q.ang_tdm):
+                    raise ValueError(both + " share %s (a shared TDM pair must be the same (lin_tdm, ang_tdm) of every "
+                                     "planner on it)" % ("lin_tdm but not ang_tdm" if p.lin_tdm is q.lin_tdm
+                                                         else "ang_tdm but not lin_tdm"))
+                if self.kind == "tdm" and p.lin_tdm is q.lin_tdm:
+                    a, b = float(q.params.get("alpha_dyn", 1.0)), float(p.params.get("alpha_dyn", 1.0))
+                    if a != b:
+                        raise ValueError(both + " share a TDM pair but have alpha_dyn %r and %r (a shared pair is "
+                                         "sampled once, at one alpha_dyn)" % (a, b))
 
     def __del__(self):
         h, self._handle = getattr(self, "_handle", None), None
@@ -92,7 +123,11 @@ class MPPI_Batch(object):
 
     def solve(self):
         """One solve() of every planner.  Returns np.float32 (K, T, 2), or None (with the planner's index and the
-        reason printed) when a planner's preconditions fail -- then nothing is solved."""
+        reason printed) when a planner's preconditions fail -- then nothing is solved.
+        With share_tdms, each shared TDM pair is sampled once, and every planner (u, u_prev_d alias, noise, costs,
+        weights, RNG streams) ends exactly as after its own solve() on a private copy of its pair taken before the
+        call; the shared TDMs end as every copy.  Raises ValueError (naming both planners) before any work for the
+        overlaps sharing refuses."""
         u = self._solve("MPPI_Batch")
         if u is not None:
             for p in self.planners:                    # as each planner's own solve() does (mppi.py:292,362)
@@ -104,6 +139,7 @@ class MPPI_Batch(object):
             if not p.check_solve_conditions():
                 print("{}: planner {}: MPPI solve condition not met. Cannot solve. Return".format(name, i))
                 return None
+        self._check_groups(name)
         for p in self.planners:
             p.move_mppi_task_vars_to_device()          # each planner's params POD (and TDMs / obstacles)
         u = np.empty((len(self.planners), self.num_steps, 2), dtype=np.float32)
@@ -155,7 +191,10 @@ class MPPI_Batch(object):
         its pose leaves the padded map limits, where its next ``solve()`` would be refused.
 
         Afterwards every planner (controls, noise, costs, weights, RNG streams, its TDMs' streams and sampled maps, and
-        ``params['x0']``) is exactly as after that host loop.  Returns a dict:
+        ``params['x0']``) is exactly as after that host loop.  With share_tdms, a shared pair is sampled once per step
+        while any of its planners runs: every planner ends as after its own episode on a private copy of its pair
+        (histories, logs and records included), and the shared TDMs as the copy of the longest-running planner.
+        Returns a dict:
           ``logs``: per planner, the trial log of ``trial()`` (time_to_goal, success, dist_to_goal, cum_dist_to_goal,
                     avg_dist_to_goal, cum_obj) with its NaN conventions; a planner that left the map is logged as one
                     that did not reach its goal;
@@ -170,8 +209,8 @@ class MPPI_Batch(object):
         Raises ValueError (naming the planner) for barebone batches, a grid count other than K, max_steps < 1,
         num_opt < 1, a grid of another dtype than float64 or integer, a planner that cannot solve (e.g. its start
         pose is outside the padded map limits), record_every < 1 and unequal num_vis_state_rollouts; B200MPPIError
-        when the planners' maps cannot all be sampled by the batch's one sampler launch.  Nothing is issued when the
-        call is refused."""
+        when the planners' maps cannot all be sampled by the batch's one sampler launch; with share_tdms, ValueError for
+        the overlaps sharing refuses.  Nothing is issued when the call is refused."""
         if self.kind not in ("det", "spd"):
             raise ValueError("MPPI_Batch.run_trials: planner 0 is a %s planner (trials need det-dynamics or speed-map "
                              "planners)" % self.kind)
@@ -221,6 +260,7 @@ class MPPI_Batch(object):
             if record_every < 1:
                 raise ValueError("%s: record_every %d < 1" % (name, record_every))
             V = self._vis_count(name)
+        self._check_groups(name)
         descs = (_lib.TrialDesc * K)()
         keep = []
         for i, (p, g) in enumerate(zip(self.planners, grids)):
@@ -310,9 +350,10 @@ class MPPI_StochasticBatch(MPPI_Batch):
     rollout, CVaR and update; each planner's map sampling keeps its own launches.  The planners share N, T and
     num_grid_samples, which may be any M a use_tdm planner takes: above 1024 maps the one CVaR launch runs one CTA
     per control sequence instead of one warp.  ``solve()``, ``set_stream`` and ``launch_count`` as in MPPI_Batch;
-    closed-loop trials through ``run_stochastic_trials``."""
+    closed-loop trials through ``run_stochastic_trials``.  ``share_tdms`` as in MPPI_Batch; the planners of a shared
+    pair must have equal ``alpha_dyn``."""
 
-    def __init__(self, planners):
+    def __init__(self, planners, share_tdms=False):
         planners = list(planners)
         if not planners:
             raise ValueError("MPPI_StochasticBatch: no planners")
@@ -324,12 +365,16 @@ class MPPI_StochasticBatch(MPPI_Batch):
             if ws != 1:
                 raise ValueError("MPPI_StochasticBatch: planner %d has world_size %d (a batch holds single-rank planners)"
                                  % (i, ws))
-        self._create(planners, "tdm", lib.b200mppi_batch_create_stochastic)
+        self._create(planners, "tdm", lib.b200mppi_batch_create_stochastic, share_tdms)
 
     def solve(self):
         """One solve() of every planner.  Returns np.float32 (K, T, 2), or None (with the planner's index and the
         reason printed) when a planner's preconditions fail -- then nothing is solved.  u_prev_d is left alone, as a
-        stochastic planner's own solve() leaves it."""
+        stochastic planner's own solve() leaves it.
+        With share_tdms, each shared pair is sampled once, over the hull of its planners' reach boxes (one planner: its
+        own box; whole maps if any planner's box is whole maps).  Every planner (u, noise, per-(m, n) and CVaR costs,
+        weights, RNG streams) ends exactly as after its own solve() on a private copy of its pair taken before the
+        call; ``sample_box()`` reports the box the pair was sampled over."""
         return self._solve("MPPI_StochasticBatch")
 
     def run_trials(self, traction_grids, max_steps, dt=None, record_every=None):
@@ -346,7 +391,10 @@ class MPPI_StochasticBatch(MPPI_Batch):
         map-sampling reach box is decided on the device).  Afterwards every planner is exactly as after ``steps[k]``
         rounds of ``u = batch.solve()``, the plant step on ``traction_grids[k]`` and ``shift_and_update(x_next, u[k])``:
         controls, noise, per-(m, n) and CVaR costs, weights, RNG streams, its TDMs' streams and sampled maps,
-        ``sample_box()`` and ``params['x0']``.  u_prev_d is left alone, as a stochastic solve leaves it.
+        ``sample_box()`` and ``params['x0']``.  u_prev_d is left alone, as a stochastic solve leaves it.  With
+        share_tdms, a shared pair is sampled once per step over the hull of its running planners' boxes, and every
+        planner ends as after its own episode on a private copy of its pair, except that ``sample_box()`` is the box
+        its pair was sampled over at its last step.
         ``record_every`` as in run_trials: the records equal ``get_state_rollout()`` of that host loop, which completes
         the maps of a boxed sampling first.
         Raises ValueError (naming the planner) as run_trials does; B200MPPIError when a planner cannot take the windowed

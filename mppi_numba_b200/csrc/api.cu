@@ -1236,20 +1236,36 @@ static bool sample_reads_reach(const b200mppi_planner* p) {
 
 static float* sample_reach_host(b200mppi_planner* p) { return p->h_u + (size_t)p->T * 2 + 2; }
 
-// reach: the read-back statistic or null (static box); advanced: a fused pair's state advance is already queued
-static int sample_finish(b200mppi_planner* p, SamplePlan& plan, const float* reach, bool advanced, cudaStream_t st,
-                         int64_t* launches) {
+// The sampling of the pair of the n planners ps (a TDM group of a batch; n = 1: one planner's solve), each deciding its
+// box from reach[j] (the read-back statistic or null: static box), the pair sampling their hull (reach_box_hull); every
+// member's sample_box() reports the box actually sampled.  advanced: a fused pair's state advance is already queued.
+static int sample_finish_group(b200mppi_planner* const* ps, const float* const* reach, int n, SamplePlan& plan,
+                               bool advanced, cudaStream_t st, int64_t* launches) {
   ReachBoxConst c;
-  fill_reach_const(p, plan, &c);
   ReachBox box;
-  const int how = reach_box_decide(c, p->prm.x0[0], p->prm.x0[1], reach, &box);
+  for (int j = 0; j < n; ++j) {
+    const b200mppi_planner* p = ps[j];
+    fill_reach_const(p, plan, &c);
+    ReachBox m;
+    reach_box_decide(c, p->prm.x0[0], p->prm.x0[1], reach[j], &m);
+    reach_box_hull_add(&box, j, m);
+  }
+  const int how = reach_box_hull_close(c, n, &box);
   if (box.geo) plan_box(&plan, box);                      // an unfused pair's TDM 1 may take the box on its own
   const int rc = plan_launch(plan, advanced, st, launches);
   const bool used = plan.boxed[0];                        // the box may not fit the sampler's launch: whole maps
-  p->last_box[0] = used ? how : 0;
-  p->last_box[1] = used ? box.row_lo : 0; p->last_box[2] = used ? box.row_hi : p->lin->rows;
-  p->last_box[3] = used ? box.col_lo : 0; p->last_box[4] = used ? box.col_hi : p->lin->cols;
+  for (int j = 0; j < n; ++j) {
+    b200mppi_planner* p = ps[j];
+    p->last_box[0] = used ? how : 0;
+    p->last_box[1] = used ? box.row_lo : 0; p->last_box[2] = used ? box.row_hi : p->lin->rows;
+    p->last_box[3] = used ? box.col_lo : 0; p->last_box[4] = used ? box.col_hi : p->lin->cols;
+  }
   return rc;
+}
+
+static int sample_finish(b200mppi_planner* p, SamplePlan& plan, const float* reach, bool advanced, cudaStream_t st,
+                         int64_t* launches) {
+  return sample_finish_group(&p, &reach, 1, plan, advanced, st, launches);
 }
 
 static int stage_sample_tdms(b200mppi_planner* p) {
@@ -1799,6 +1815,7 @@ struct b200mppi_batch {
   // b200mppi_batch_get_state_rollout's section, after the solve's (a solve does not upload it):
   // [RolloutParams K | VisBatchDesc K] from off_vis, vis_bytes long
   size_t off_vis = 0, off_visd = 0, vis_bytes = 0;
+  bool share = false;                  // b200mppi_batch_share_tdms: planners on one TDM pair sample it once per call
 };
 
 static size_t align256(size_t v) { return (v + 255) / 256 * 256; }
@@ -1928,6 +1945,46 @@ extern "C" int b200mppi_batch_launch_count(b200mppi_batch* b, int64_t* out) {
   return B200MPPI_OK;
 }
 
+extern "C" int b200mppi_batch_share_tdms(b200mppi_batch* b, int32_t enable) {
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  b->share = enable != 0;
+  return B200MPPI_OK;
+}
+
+// The batch's TDM groups for one call: with sharing on, planners with the same (lin, ang) objects form one group (in the
+// order of their first members); otherwise, and in barebone batches, every planner is a group of its own.  Group g's
+// planners are members[first[g] .. first[g + 1]), in planner order; per group, plans, launches and commits run once.
+struct TdmGroups {
+  std::vector<int> of;                 // planner -> group
+  std::vector<int> first;              // G + 1 offsets into members
+  std::vector<int> members;
+  int size() const { return (int)first.size() - 1; }
+  int count(int g) const { return first[g + 1] - first[g]; }
+  int lead(int g) const { return members[first[g]]; }
+  bool shared() const { return (int)members.size() > size(); }
+};
+
+static TdmGroups batch_groups(const b200mppi_batch* b) {
+  const int K = (int)b->pl.size();
+  TdmGroups gr;
+  gr.of.assign(K, -1);
+  std::vector<std::vector<int>> g;
+  for (int i = 0; i < K; ++i) {
+    const b200mppi_planner* p = b->pl[i];
+    if (b->share && b->mode != B200MPPI_MODE_BAREBONE)
+      for (int j = 0; j < i && gr.of[i] < 0; ++j)
+        if (b->pl[j]->lin == p->lin && b->pl[j]->ang == p->ang) gr.of[i] = gr.of[j];
+    if (gr.of[i] < 0) { gr.of[i] = (int)g.size(); g.emplace_back(); }
+    g[gr.of[i]].push_back(i);
+  }
+  gr.first.push_back(0);
+  for (const std::vector<int>& m : g) {
+    gr.members.insert(gr.members.end(), m.begin(), m.end());
+    gr.first.push_back((int)gr.members.size());
+  }
+  return gr;
+}
+
 // Everything a batch solve checks before it issues any work.
 static int batch_validate(b200mppi_batch* b) {
   const int K = (int)b->pl.size();
@@ -1944,13 +2001,27 @@ static int batch_validate(b200mppi_batch* b) {
   }
   if (b->mode == B200MPPI_MODE_BAREBONE) return B200MPPI_OK;
   // sequential solves would sample a TDM shared by two planners twice, one after the other: those planners are not
-  // independent, so the batch refuses them (one planner's lin == ang is fine: its own solve samples it twice too)
+  // independent, so the batch refuses them (one planner's lin == ang is fine: its own solve samples it twice too).  With
+  // sharing on, planners on the same (lin, ang) pair form a group sampled once; any other overlap is still refused.
   for (int i = 0; i < K; ++i)
     for (int j = 0; j < i; ++j) {
       const b200mppi_planner* p = b->pl[i]; const b200mppi_planner* q = b->pl[j];
-      if (p->lin == q->lin || p->lin == q->ang || p->ang == q->lin || p->ang == q->ang)
-        return fail(B200MPPI_EINVAL, "batch_solve: planners " + std::to_string(j) + " and " + std::to_string(i) +
-                                         " share a TDM (batched planners must be independent)");
+      const std::string both = "batch_solve: planners " + std::to_string(j) + " and " + std::to_string(i);
+      if (!b->share) {
+        if (p->lin == q->lin || p->lin == q->ang || p->ang == q->lin || p->ang == q->ang)
+          return fail(B200MPPI_EINVAL, both + " share a TDM (batched planners must be independent)");
+        continue;
+      }
+      if (p->lin == q->ang || p->ang == q->lin)
+        return fail(B200MPPI_EINVAL, both + ": a TDM is lin of one and ang of the other (a shared TDM pair must be "
+                                            "the same (lin, ang) of every planner on it)");
+      if ((p->lin == q->lin) != (p->ang == q->ang))
+        return fail(B200MPPI_EINVAL, both + " share " + (p->lin == q->lin ? "lin but not ang" : "ang but not lin") +
+                                         " (a shared TDM pair must be the same (lin, ang) of every planner on it)");
+      if (p->lin == q->lin && sample_alpha(p) != sample_alpha(q))
+        return fail(B200MPPI_EINVAL, both + " share a TDM pair but have alpha_dyn " + std::to_string(sample_alpha(q)) +
+                                         " and " + std::to_string(sample_alpha(p)) +
+                                         " (a shared pair is sampled once, at one alpha_dyn)");
     }
   return B200MPPI_OK;
 }
@@ -1966,39 +2037,42 @@ static void last_box_whole_map(b200mppi_planner* p) {
 // Planning (host tables, the batched pairs' descriptors) comes before the solve's one upload, the launches after the noise.
 constexpr double BATCH_ALPHA = 1.0;   // det / speed-map solves sample with the default alpha_dyn (stage_sample_tdms)
 
-static int batch_plan_sample(b200mppi_batch* b, SampleGridsV2Args* h_sg, std::vector<SamplePlan>& plans,
-                             std::vector<char>& joined, int* njoined) {
-  const int K = (int)b->pl.size();
-  plans.resize(K);
-  joined.assign(K, 0);
+// One plan per TDM group (a shared pair is sampled once: one entry of the batched launch or one plan of its own).
+static int batch_plan_sample(b200mppi_batch* b, const TdmGroups& gr, SampleGridsV2Args* h_sg,
+                             std::vector<SamplePlan>& plans, std::vector<char>& joined, int* njoined) {
+  const int G = gr.size();
+  plans.resize(G);
+  joined.assign(G, 0);
   int nj = 0;
-  for (int i = 0; i < K; ++i) {
-    const int rc = plan_sampling(b->pl[i]->lin, b->pl[i]->ang, BATCH_ALPHA, b->stream, &plans[i]);
+  for (int g = 0; g < G; ++g) {
+    const b200mppi_planner* p = b->pl[gr.lead(g)];
+    const int rc = plan_sampling(p->lin, p->ang, BATCH_ALPHA, b->stream, &plans[g]);
     if (rc) return rc;
-    if (!plans[i].fused || (nj > 0 && !sample_grids_v2_same_launch(h_sg[0], plans[i].a[0]))) continue;
-    h_sg[nj++] = plans[i].a[0];
-    joined[i] = 1;
+    if (!plans[g].fused || (nj > 0 && !sample_grids_v2_same_launch(h_sg[0], plans[g].a[0]))) continue;
+    h_sg[nj++] = plans[g].a[0];
+    joined[g] = 1;
   }
   *njoined = nj;
   return B200MPPI_OK;
 }
 
-static int batch_run_sample(b200mppi_batch* b, const SampleGridsV2Args* h_sg, const SampleGridsV2Args* d_sg,
-                            std::vector<SamplePlan>& plans, const std::vector<char>& joined, int nj) {
+static int batch_run_sample(b200mppi_batch* b, const TdmGroups& gr, const SampleGridsV2Args* h_sg,
+                            const SampleGridsV2Args* d_sg, std::vector<SamplePlan>& plans,
+                            const std::vector<char>& joined, int nj) {
   if (nj > 0) {
     launch_sample_grids_v2_batch(h_sg[0], d_sg, nj, nullptr, b->stream);
     b->launches++;
     CHECK_LAUNCH();
   }
-  for (size_t i = 0; i < plans.size(); ++i) {
-    if (joined[i]) {
-      plan_commit(plans[i], 0);
-      plan_commit(plans[i], 1);
+  for (int g = 0; g < gr.size(); ++g) {
+    if (joined[g]) {
+      plan_commit(plans[g], 0);
+      plan_commit(plans[g], 1);
     } else {
-      const int rc = plan_launch(plans[i], false, b->stream, &b->launches);
+      const int rc = plan_launch(plans[g], false, b->stream, &b->launches);
       if (rc) return rc;
     }
-    last_box_whole_map(b->pl[i]);
+    for (int j = gr.first[g]; j < gr.first[g + 1]; ++j) last_box_whole_map(b->pl[gr.members[j]]);
   }
   return B200MPPI_OK;
 }
@@ -2055,21 +2129,22 @@ static int batch_solve_onemap(b200mppi_batch* b) {
   const RolloutArgs* dr = reinterpret_cast<const RolloutArgs*>(b->d_desc + b->off_roll);
   const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(b->d_desc + b->off_upd);
   const bool maps = b->mode != B200MPPI_MODE_BAREBONE;
+  const TdmGroups gr = batch_groups(b);
   std::vector<SamplePlan> plans;
   std::vector<char> joined;
   int nj = 0;
-  if (maps && (rc = batch_plan_sample(b, hs, plans, joined, &nj))) return rc;
+  if (maps && (rc = batch_plan_sample(b, gr, hs, plans, joined, &nj))) return rc;
   CU(cudaMemcpyAsync(b->d_desc, b->h_desc, b->desc_bytes, cudaMemcpyHostToDevice, st));
   const int num_opt = b->pl[0]->prm.num_opt;
   // the reference samples before its (empty) loop
-  if (num_opt <= 0 && maps && (rc = batch_run_sample(b, hs, ds, plans, joined, nj))) return rc;
+  if (num_opt <= 0 && maps && (rc = batch_run_sample(b, gr, hs, ds, plans, joined, nj))) return rc;
   // solve(): num_opt x (noise, [first iteration: maps], rollout, update)
   for (int k = 0; k < num_opt; ++k) {
     launch_sample_noise_batch(dn, K, b->N, T, nullptr, st);
     b->launches++;
     CHECK_LAUNCH();
     for (b200mppi_planner* p : b->pl) p->prepared = false;
-    if (k == 0 && maps && (rc = batch_run_sample(b, hs, ds, plans, joined, nj))) return rc;
+    if (k == 0 && maps && (rc = batch_run_sample(b, gr, hs, ds, plans, joined, nj))) return rc;
     launch_rollout_batch(dr, K, b->mode, b->N, T, nullptr, st);
     b->launches++;
     CHECK_LAUNCH();
@@ -2143,10 +2218,16 @@ static int batch_solve_stochastic(b200mppi_batch* b) {
   const RolloutWinArgs* hw = reinterpret_cast<const RolloutWinArgs*>(b->h_desc + b->off_win);
   bool masks01 = true;
   stochastic_descs(b, b->h_desc, WW, WH, &masks01);
-  // the sampler plans (their host preparation may synchronise the stream) before the one upload
-  std::vector<SamplePlan> plans(K);
-  for (int i = 0; i < K; ++i)
-    if ((rc = plan_sampling(b->pl[i]->lin, b->pl[i]->ang, sample_alpha(b->pl[i]), st, &plans[i]))) return rc;
+  // the sampler plans, one per TDM group (their host preparation may synchronise the stream) before the one upload
+  const TdmGroups gr = batch_groups(b);
+  const int G = gr.size();
+  std::vector<SamplePlan> plans(G);
+  std::vector<b200mppi_planner*> ps(K);                // planners by group
+  for (int j = 0; j < K; ++j) ps[j] = b->pl[gr.members[j]];
+  for (int g = 0; g < G; ++g) {
+    const b200mppi_planner* p = b->pl[gr.lead(g)];
+    if ((rc = plan_sampling(p->lin, p->ang, sample_alpha(p), st, &plans[g]))) return rc;
+  }
   CU(cudaMemcpyAsync(b->d_desc, b->h_desc, b->desc_bytes, cudaMemcpyHostToDevice, st));
   const NoisePrepDesc* dn = reinterpret_cast<const NoisePrepDesc*>(b->d_desc);
   const RolloutWinArgs* dw = reinterpret_cast<const RolloutWinArgs*>(b->d_desc + b->off_win);
@@ -2154,9 +2235,12 @@ static int batch_solve_stochastic(b200mppi_batch* b) {
   const CvarDesc* dc = reinterpret_cast<const CvarDesc*>(b->d_desc + b->off_cvar);
   const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(b->d_desc + b->off_upd);
   const int num_opt = b->pl[0]->prm.num_opt;
+  std::vector<const float*> reach(K, nullptr);         // by group, as ps
   if (num_opt <= 0)                                    // the reference samples before its (empty) loop
-    for (int i = 0; i < K; ++i)
-      if ((rc = sample_finish(b->pl[i], plans[i], nullptr, false, st, &b->launches))) return rc;
+    for (int g = 0; g < G; ++g)
+      if ((rc = sample_finish_group(&ps[gr.first[g]], &reach[gr.first[g]], gr.count(g), plans[g], false, st,
+                                    &b->launches)))
+        return rc;
   for (int k = 0; k < num_opt; ++k) {
     launch_noise_prepare_batch(dn, K, N, T, b->pl[0]->npad, k, nullptr, st);
     b->launches++;
@@ -2166,8 +2250,8 @@ static int batch_solve_stochastic(b200mppi_batch* b) {
       p->prepared = true;
       p->reach_valid = true;
     }
-    if (k == 0) {                                      // stage_sample_tdms of every planner, one host wait
-      std::vector<char> reads(K), advanced(K);
+    if (k == 0) {                                      // stage_sample_tdms of every TDM group, one host wait
+      std::vector<char> reads(K), advanced(G);
       bool any = false;
       for (int i = 0; i < K; ++i) {
         b200mppi_planner* p = b->pl[i];
@@ -2176,20 +2260,21 @@ static int batch_solve_stochastic(b200mppi_batch* b) {
         any = true;
       }
       if (any) CU(cudaEventRecord(b->ev, st));
-      for (int i = 0; i < K; ++i) {
-        if (!reads[i] || !plans[i].fused) continue;
-        launch_plan_advance(plans[i], 0, st);
+      for (int g = 0; g < G; ++g) {                    // a fused group's advance, if any member waits for its reach
+        bool wait = false;
+        for (int j = gr.first[g]; j < gr.first[g + 1]; ++j) wait = wait || reads[gr.members[j]];
+        if (!wait || !plans[g].fused) continue;
+        launch_plan_advance(plans[g], 0, st);
         CHECK_LAUNCH();
         b->launches++;
-        advanced[i] = 1;
+        advanced[g] = 1;
       }
       if (any) CU(cudaEventSynchronize(b->ev));
-      for (int i = 0; i < K; ++i) {
-        b200mppi_planner* p = b->pl[i];
-        if ((rc = sample_finish(p, plans[i], reads[i] ? sample_reach_host(p) : nullptr, advanced[i] != 0, st,
-                                &b->launches)))
+      for (int j = 0; j < K; ++j) reach[j] = reads[gr.members[j]] ? sample_reach_host(ps[j]) : nullptr;
+      for (int g = 0; g < G; ++g)
+        if ((rc = sample_finish_group(&ps[gr.first[g]], &reach[gr.first[g]], gr.count(g), plans[g], advanced[g] != 0,
+                                      st, &b->launches)))
           return rc;
-      }
     }
     CU(launch_rollout_win_batch(hw[0], dw, dt, K, masks01, nullptr, st));
     b->launches++;
@@ -2346,18 +2431,19 @@ static int trial_validate(b200mppi_batch* b, TrialKind kind, const b200mppi_tria
 // A stochastic batch's trial sampler sets (set0: parity 0) and launch size.  Every pair must join the one boxed sampler
 // launch: a fused plan (identical generator streams, well-formed PMF at its alpha, lin != ang) whose launch and box
 // segments equal planner 0's.
-static int stochastic_trial_plans(b200mppi_batch* b, const std::string& fn, std::vector<SamplePlan>& plans,
-                                  std::vector<SampleGridsV2Args>& set0, int* mrows, int* ncact) {
-  const int K = (int)b->pl.size();
-  plans.resize(K);
-  for (int i = 0; i < K; ++i) {
-    b200mppi_planner* p = b->pl[i];
-    const int rc = plan_sampling(p->lin, p->ang, sample_alpha(p), b->stream, &plans[i]);
+static int stochastic_trial_plans(b200mppi_batch* b, const TdmGroups& gr, const std::string& fn,
+                                  std::vector<SamplePlan>& plans, std::vector<SampleGridsV2Args>& set0, int* mrows,
+                                  int* ncact) {
+  const int K = (int)b->pl.size(), G = gr.size();
+  plans.resize(G);
+  for (int g = 0; g < G; ++g) {                       // one plan per TDM group
+    b200mppi_planner* p = b->pl[gr.lead(g)];
+    const int rc = plan_sampling(p->lin, p->ang, sample_alpha(p), b->stream, &plans[g]);
     if (rc) return rc;
     const b200mppi_tdm* l = p->lin; const b200mppi_tdm* l0 = b->pl[0]->lin;
-    if (!plans[i].fused || !sample_grids_v2_same_launch(plans[0].a[0], plans[i].a[0]) || l->box_segs != l0->box_segs ||
+    if (!plans[g].fused || !sample_grids_v2_same_launch(plans[0].a[0], plans[g].a[0]) || l->box_segs != l0->box_segs ||
         l->box_seg_rows != l0->box_seg_rows)
-      return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(i) + ": its TDM pair cannot join the "
+      return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(gr.lead(g)) + ": its TDM pair cannot join the "
                                    "batch's one sampler launch (lin == ang, or map geometry, PMF or generator streams "
                                    "differ from planner 0's)");
   }
@@ -2371,7 +2457,7 @@ static int stochastic_trial_plans(b200mppi_batch* b, const std::string& fn, std:
   bool any_box = false;
   for (int i = 0; i < K; ++i) {
     ReachBoxConst c;
-    fill_reach_const(b->pl[i], plans[i], &c);
+    fill_reach_const(b->pl[i], plans[gr.of[i]], &c);
     if (c.mode == 0) continue;
     const double w = (double)c.cols * (double)c.res, h = (double)c.rows * (double)c.res;
     const double A = std::fmax(std::fabs((double)c.pxl), std::fabs((double)c.pxl + w)) +
@@ -2391,12 +2477,12 @@ static int stochastic_trial_plans(b200mppi_batch* b, const std::string& fn, std:
   int gm_b = 128 / *ncact;                            // apply_box's maps per CTA for that many tile columns
   gm_b = std::max(1, std::min(std::min(gm_b, SG_GM_MAX), sg.num_maps));
   // the boxed launch's row segments over the whole-map plan
-  for (int i = 0; i < K; ++i) {
-    const b200mppi_tdm* l = b->pl[i]->lin;
-    set0[i] = plans[i].a[0];
-    set0[i].segs = l->box_segs; set0[i].seg_rows = l->box_seg_rows; set0[i].jump = l->jump_box_d;
-    set0[i].write_states = 0;
-    set0[i].gm = gm_b;
+  for (int g = 0; g < G; ++g) {
+    const b200mppi_tdm* l = b->pl[gr.lead(g)]->lin;
+    set0[g] = plans[g].a[0];
+    set0[g].segs = l->box_segs; set0[g].seg_rows = l->box_seg_rows; set0[g].jump = l->jump_box_d;
+    set0[g].write_states = 0;
+    set0[g].gm = gm_b;
   }
   if (!sample_box_batch_fits(set0[0], *ncact))
     return fail(B200MPPI_EINVAL, fn + ": planner 0: the batched sampler launch (" + std::to_string(*ncact) +
@@ -2420,8 +2506,9 @@ static const char* mode_name(int mode) {
 // one launch that completes maps [0, V) of every pair whose step sampled a box (the maps the rollouts read).
 // Device buffer of a call: [descriptors (b->h_desc's layout; a one-map batch's parity-0 sampler set is its own section
 // there) | stochastic: the parity-0 sampler set | not barebone: the parity-1 set | stochastic: box descriptors, box
-// records | states | barebone: contacts | trials | active K + count | recording: vis descriptors | not barebone: grids |
-// recording: the records (K, R, V, T+1, 3) | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds
+// records | shared TDM pairs: group records (stochastic), group descriptors, members | states | barebone: contacts |
+// trials | active K + count | recording: vis descriptors | not barebone: grids | recording: the records (K, R, V, T+1,
+// 3) | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds
 // xhist and uhist: the float64 ground-truth grids (tens of MB for a batch of large maps) are copied straight from the
 // caller's arrays, and the written records (of K * R * V * (T+1) * 12 bytes, 145 MB for K 8, 150 steps, V 100, T 100)
 // straight into the caller's array.
@@ -2462,31 +2549,39 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   if (stochastic && (rc = stochastic_validate(b, fn.c_str(), &WW, &WH))) return rc;
   CU(cudaSetDevice(b->device));
   cudaStream_t st = b->stream;
-  // the sampler plans first (their host preparation may synchronise the stream): every pair must join the one launch
+  // the sampler plans first (their host preparation may synchronise the stream): every TDM group's pair must join the
+  // one launch.  Groups of more than one planner (shared pairs) take the group-aware sampler launches.
+  const TdmGroups gr = batch_groups(b);
+  const int G = gr.size();
+  const bool grouped = !barebone && gr.shared();
   std::vector<SamplePlan> plans;
   std::vector<SampleGridsV2Args> set0(K);
   int mrows = 0, ncact = 0;
   if (stochastic) {
-    if ((rc = stochastic_trial_plans(b, fn, plans, set0, &mrows, &ncact))) return rc;
+    if ((rc = stochastic_trial_plans(b, gr, fn, plans, set0, &mrows, &ncact))) return rc;
   } else if (!barebone) {
     std::vector<char> joined;
     int nj = 0;
-    if ((rc = batch_plan_sample(b, set0.data(), plans, joined, &nj))) return rc;
-    for (int i = 0; i < K; ++i)
-      if (!joined[i])
-        return fail(B200MPPI_EINVAL, "run_trials: planner " + std::to_string(i) + ": its TDM pair cannot join the "
-                                     "batch's one sampler launch (map geometry, PMF or generator streams differ from "
+    if ((rc = batch_plan_sample(b, gr, set0.data(), plans, joined, &nj))) return rc;
+    for (int g = 0; g < G; ++g)
+      if (!joined[g])
+        return fail(B200MPPI_EINVAL, "run_trials: planner " + std::to_string(gr.lead(g)) + ": its TDM pair cannot join "
+                                     "the batch's one sampler launch (map geometry, PMF or generator streams differ from "
                                      "planner 0's)");
   }
   if ((rc = batch_wait_members(b))) return rc;
   const size_t nbox = stochastic ? (size_t)K : 0;      // stochastic-only sections
-  const size_t nset = barebone ? 0 : (size_t)K;        // sections of planners with maps
+  const size_t nset = barebone ? 0 : (size_t)G;        // sections of TDM groups
   const size_t ncon = barebone ? (size_t)K : 0;        // barebone-only section
+  const size_t ngrp = grouped ? (size_t)G : 0;         // shared pairs: group descriptors, group records, members
   const size_t off_s0 = stochastic ? b->desc_bytes : b->off_sample;
-  const size_t off_s1 = b->desc_bytes + align256(nbox * sizeof(SampleGridsV2Args));
+  const size_t off_s1 = b->desc_bytes + align256((stochastic ? nset : 0) * sizeof(SampleGridsV2Args));
   const size_t off_box = off_s1 + align256(nset * sizeof(SampleGridsV2Args));
   const size_t off_rec = off_box + align256(nbox * sizeof(SampleBoxDesc));
-  const size_t off_state = off_rec + align256(nbox * 5 * sizeof(int));
+  const size_t off_grec = off_rec + align256(nbox * 5 * sizeof(int));
+  const size_t off_grp = off_grec + align256(ngrp * 5 * sizeof(int));
+  const size_t off_mem = off_grp + align256(ngrp * sizeof(SampleGroupDesc));
+  const size_t off_state = off_mem + align256((grouped ? (size_t)K : 0) * sizeof(int));
   const size_t off_con = off_state + align256((size_t)K * sizeof(TrialState));
   const size_t off_tr = off_con + align256(ncon * sizeof(int));
   const size_t off_act = off_tr + align256((size_t)K * sizeof(TrialDev));
@@ -2553,13 +2648,6 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       hcon[i] = 0;
       continue;
     }
-    // parity 1: the pair samples from the buffers parity 0 wrote into
-    hs[0][i] = hs[1][i] = set0[i];
-    for (SampleTdm& td : hs[1][i].t) {
-      uint64_t* in = td.states_out;
-      td.states_out = const_cast<uint64_t*>(td.states);
-      td.states = in;
-    }
     const double* dg = reinterpret_cast<const double*>(d + off_grid[i]);
     t.lin = dg; t.ang = dg + (size_t)q.height * q.width; t.H = q.height; t.W = q.width;
     t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res;
@@ -2575,8 +2663,24 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     reinterpret_cast<CvarDesc*>(h + b->off_cvar)[i].active = dact + i;
     hb[i] = SampleBoxDesc{{}, dw[i].p.x0, p->reach_d, p->reach_slot ^ 1, reinterpret_cast<int*>(d + off_rec) + 5 * i,
                           l->jump_tile_d};
-    fill_reach_const(p, plans[i], &hb[i].c);
+    fill_reach_const(p, plans[gr.of[i]], &hb[i].c);
   }
+  for (int g = 0; g < (int)nset; ++g) {
+    // parity 1: the pair samples from the buffers parity 0 wrote into
+    hs[0][g] = hs[1][g] = set0[g];
+    for (SampleTdm& td : hs[1][g].t) {
+      uint64_t* in = td.states_out;
+      td.states_out = const_cast<uint64_t*>(td.states);
+      td.states = in;
+    }
+  }
+  SampleGroupDesc* hg = reinterpret_cast<SampleGroupDesc*>(h + off_grp);
+  int* hmem = reinterpret_cast<int*>(h + off_mem);
+  for (int g = 0; g < (int)ngrp; ++g)
+    hg[g] = SampleGroupDesc{gr.first[g], gr.count(g), stochastic ? reinterpret_cast<int*>(d + off_grec) + 5 * g : nullptr};
+  if (grouped) std::copy(gr.members.begin(), gr.members.end(), hmem);
+  const SampleGroupDesc* dgrp = grouped ? reinterpret_cast<const SampleGroupDesc*>(d + off_grp) : nullptr;
+  const int* dmem = grouped ? reinterpret_cast<const int*>(d + off_mem) : nullptr;
   hact[K] = K;
   const RolloutWinArgs g0 = stochastic ? *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win) : RolloutWinArgs{};
   CU(cudaMemcpyAsync(d, h, head, cudaMemcpyHostToDevice, st));
@@ -2609,9 +2713,10 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
         launch_noise_prepare_batch(reinterpret_cast<const NoisePrepDesc*>(d), K, N, T, npad, iter, dact, st);
         CHECK_LAUNCH();
         if (k == 0) {
-          launch_sample_grids_v2_box_batch(geom, ds[s & 1], db, K, dact, iter, mrows, ncact, st);
+          launch_sample_grids_v2_box_batch(geom, ds[s & 1], db, G, dact, iter, mrows, ncact, st, dgrp, dmem);
           CHECK_LAUNCH();
-          launch_advance_states_batch(ds[s & 1], db, K, geom.rows, geom.cols, geom.tx, geom.ty, geom.num_maps, dact, st);
+          launch_advance_states_batch(ds[s & 1], db, G, geom.rows, geom.cols, geom.tx, geom.ty, geom.num_maps, dact, st,
+                                      dgrp, dmem);
           CHECK_LAUNCH();
         }
         CU(launch_rollout_win_batch(g0, dw, d + b->off_tm, K, masks01, dact, st));
@@ -2621,7 +2726,7 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
         launch_sample_noise_batch(reinterpret_cast<const NoiseDesc*>(d), K, N, T, dact, st);
         CHECK_LAUNCH();
         if (k == 0 && !barebone) {
-          launch_sample_grids_v2_batch(geom, ds[s & 1], K, dact, st);
+          launch_sample_grids_v2_batch(geom, ds[s & 1], G, dact, st, dgrp, dmem);
           CHECK_LAUNCH();
         }
         launch_rollout_batch(dr, K, b->mode, N, T, dact, st);
@@ -2633,7 +2738,7 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     const bool rec_step = record && s % record_every == 0;
     if (rec_step) {
       if (stochastic) {                               // from the pre-call states this step's sampling read
-        launch_sample_grids_v2_complete_batch(geom, ds[s & 1], db, K, dact, V, mrows, ncact, st);
+        launch_sample_grids_v2_complete_batch(geom, ds[s & 1], db, G, dact, V, mrows, ncact, st, dgrp, dmem);
         CHECK_LAUNCH();
       }
       launch_state_rollout_batch(reinterpret_cast<const VisBatchDesc*>(d + off_vis), K, V, dact,
@@ -2670,13 +2775,10 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     for (size_t j = (size_t)n * 2; j < (size_t)S * 2; ++j) uo[j] = fnan;
     results[i] = b200mppi_trial_result{r.cum_obj, r.cum_dist, r.dist, n, r.status};
     if (barebone) contact_steps[i] = hcon[i];
-    // host state as after n rounds of the host loop: n samplings of the pair (stochastic: boxed or whole-map, the last
-    // one's kind in grid_partial), the reach slot toggled once per iteration, the last solve's box and x0
+    // host state as after n rounds of the host loop: the reach slot toggled once per iteration, the last solve's box and
+    // x0 (the samplings of the pair below)
     b200mppi_planner* p = b->pl[i];
     const int* rec = hrec + 5 * i;
-    if (stochastic) plans[i].boxed[0] = plans[i].boxed[1] = rec[0] != 0;
-    if (!barebone)
-      for (int s = 0; s < n; ++s) { plan_commit(plans[i], 0); plan_commit(plans[i], 1); }
     if (stochastic) {
       p->reach_slot ^= (n * num_opt) & 1;
       p->reach_valid = true;
@@ -2687,6 +2789,15 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     p->prepared = false;
     p->pushed_direct = false;
     for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)xo[(size_t)(n - 1) * 3 + c];
+  }
+  // each TDM group's pair as after the samplings of its longest-running member (a group samples at every step while any
+  // member runs), the last one's kind from the group's record (a group of one: its planner's)
+  for (int g = 0; g < G && !barebone; ++g) {
+    int n = 0;
+    for (int j = gr.first[g]; j < gr.first[g + 1]; ++j) n = std::max(n, hst[gr.members[j]].steps);
+    const int* rec = grouped && stochastic ? reinterpret_cast<const int*>(h + off_grec) + 5 * g : hrec + 5 * gr.lead(g);
+    if (stochastic) plans[g].boxed[0] = plans[g].boxed[1] = rec[0] != 0;
+    for (int s = 0; s < n; ++s) { plan_commit(plans[g], 0); plan_commit(plans[g], 1); }
   }
   if (record) {
     // record r belongs to step r * record_every.  Only the written ones are copied (records past a planner's last step

@@ -169,6 +169,46 @@ __host__ __device__ inline int reach_box_decide(const ReachBoxConst& c, float x0
   b->how = how;
   return how;
 }
+// The box of a TDM pair shared by several planners of a batch (b200mppi_batch_share_tdms): one sampling serves every
+// member, so it covers every member's box.  Members are added one by one (n: members added so far), then closed:
+//   one member: exactly its reach_box_decide result, disc included;
+//   two or more: the rectangle hull of their boxes without a disc; whole maps (how 0, geo 0) if any member decided whole
+//   maps or the hull's launch does not fit.  how is the largest of the members' decisions.
+// c: the constants of any member (the pair's geometry and launch are the same for all).  sample_finish (api.cu) and the
+// group-aware trial sampler (sample.cu) both decide with these two functions.
+__host__ __device__ inline void reach_box_hull_add(ReachBox* h, int n, const ReachBox& m) {
+  if (n == 0) { *h = m; return; }
+  h->how = (h->how == 0 || m.how == 0) ? 0 : (m.how > h->how ? m.how : h->how);
+  h->geo = h->geo && m.geo;
+  h->row_lo = m.row_lo < h->row_lo ? m.row_lo : h->row_lo; h->row_hi = m.row_hi > h->row_hi ? m.row_hi : h->row_hi;
+  h->col_lo = m.col_lo < h->col_lo ? m.col_lo : h->col_lo; h->col_hi = m.col_hi > h->col_hi ? m.col_hi : h->col_hi;
+}
+__host__ __device__ inline int reach_box_hull_close(const ReachBoxConst& c, int n, ReachBox* h) {
+  if (n < 2) return h->how;
+  h->cx = h->cy = h->r = 0.0f;
+  int gm = 0;
+  if (h->how) {
+    const int ncol = (c.cols + c.ty - 1) / c.ty;
+    h->tiy_lo = h->col_lo / ncol;
+    h->nact = (h->col_hi - 1) / ncol - h->tiy_lo + 1;
+    gm = 128 / h->nact;
+    if (gm > SG_GM_MAX) gm = SG_GM_MAX;
+    if (gm > c.num_maps) gm = c.num_maps;
+    if (gm < 1) gm = 1;
+    if (c.nt == 0 || !sample_v2_fits_hd(h->tiy_lo, h->nact, c.ty, c.cols, c.bpad0, c.bpad1, gm, c.nt)) h->how = 0;
+  }
+  if (!h->how) {
+    h->geo = 0;
+    h->row_lo = 0; h->row_hi = c.rows; h->col_lo = 0; h->col_hi = c.cols;
+    h->tiy_lo = 0; h->nact = c.ty; gm = 0;
+  }
+  h->gm = gm;
+  return h->how;
+}
+__host__ __device__ inline int reach_box_hull(const ReachBoxConst& c, const ReachBox* m, int count, ReachBox* h) {
+  for (int i = 0; i < count; ++i) reach_box_hull_add(h, i, m[i]);
+  return reach_box_hull_close(c, count, h);
+}
 // [emu:end sampler_args]
 bool build_sample_thresholds(double alpha, int q_cap, uint64_t* table /*[SAMPLE_TABLE_WORDS]*/);
 bool sample_grids_v2_fits(const SampleGridsV2Args& a, int nt);
@@ -177,8 +217,12 @@ void launch_sample_grids_v2(const SampleGridsV2Args& a, int nt, cudaStream_t st)
 bool sample_grids_v2_same_launch(const SampleGridsV2Args& a, const SampleGridsV2Args& b);
 // ONE fused (nt = 2) launch for `count` pairs: descs = device array of their args, geom = any of them (host)
 // active (device, may be null): active[pair] == 0 -> that pair's CTAs return at once (closed-loop trials)
+// groups (device, may be null): `count` groups of planners members[] (shared pairs, one descriptor per group), a group
+// running while any member is active (closed-loop trials with shared TDM pairs)
+struct SampleGroupDesc;
 void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs, int count,
-                                  const int* active, cudaStream_t st);
+                                  const int* active, cudaStream_t st, const SampleGroupDesc* groups = nullptr,
+                                  const int* members = nullptr);
 // closed-loop trials of a stochastic batch: each pair's reach box decided on the device, from the x0 the plant step
 // wrote and the reach statistic of the step's first iteration (slot ^ (iter & 1)).  The decision goes to `record`:
 // [how, row_lo, row_hi, col_lo, col_hi] as b200mppi_planner_sample_box reports it.
@@ -191,24 +235,42 @@ struct SampleBoxDesc {
   int* record;                  // [5]
   const uint64_t* jump_tile;    // [4][128][2] whole-tile advance matrices (advance_states_batch_kernel)
 };
+// A TDM pair shared by several planners of a trial batch (b200mppi_batch_share_tdms): the group-aware launches below take
+// one entry per group, their descriptors one per group, and run a group while any of its planners is active.
+struct SampleGroupDesc {
+  int first, count;             // its planners: members[first .. first + count), in planner order
+  int* record;                  // [5]: the group's decision at its last sampled step (stochastic trials), or null
+};
+__host__ __device__ inline bool group_running(const SampleGroupDesc& g, const int* members, const int* active) {
+  for (int j = g.first; j < g.first + g.count; ++j)
+    if (active[members[j]]) return true;
+  return false;
+}
 // [emu:end box_desc]
 // ONE launch for `count` fused pairs of equal geometry (geom: a whole-map plan with the boxed launch's segs / seg_rows /
 // jump and maps per CTA gm): mrows tile rows x the row segments x ncact tile columns, sized for the largest box of the
 // static bound; every CTA narrows to its pair's box and disc, whole maps loop over row and column groups.  No state
 // stores: launch_advance_states_batch advances the states.
+// groups (may be null): `count` groups as in launch_sample_grids_v2_batch, boxes one per planner; every CTA of a group
+// decides its running members' boxes and samples their hull (reach_box_hull), recorded in the group's record and in
+// every running member's
 void launch_sample_grids_v2_box_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
                                       const SampleBoxDesc* boxes, int count, const int* active, int iter, int mrows,
-                                      int ncact, cudaStream_t st);
+                                      int ncact, cudaStream_t st, const SampleGroupDesc* groups = nullptr,
+                                      const int* members = nullptr);
 // the launch above holds ncact tile columns with geom.gm maps per CTA (threads, shared memory)
 bool sample_box_batch_fits(const SampleGridsV2Args& geom, int ncact);
 // recording stochastic trials: whole maps [0, map_end) of every pair whose step sampled a box (record[0] != 0), from the
 // pre-call states of descs[pair].t[0], with the launch geometry of the box launch; no state stores
+// (groups: the group's record decides)
 void launch_sample_grids_v2_complete_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
                                            const SampleBoxDesc* boxes, int count, const int* active, int map_end,
-                                           int mrows, int ncact, cudaStream_t st);
+                                           int mrows, int ncact, cudaStream_t st, const SampleGroupDesc* groups = nullptr,
+                                           const int* members = nullptr);
 // launch_advance_states for `count` pairs (pair blockIdx.y): descs[y].t[0].states -> both TDMs' states_out
 void launch_advance_states_batch(const SampleGridsV2Args* descs, const SampleBoxDesc* boxes, int count, int rows,
-                                 int cols, int tx, int ty, int num_maps, const int* active, cudaStream_t st);
+                                 int cols, int tx, int ty, int num_maps, const int* active, cudaStream_t st,
+                                 const SampleGroupDesc* groups = nullptr, const int* members = nullptr);
 // tile classes of a generator: (full | last) tile height x (full | last) tile width -> draws per whole-map walk
 void sample_tile_draws(int rows, int cols, int tx, int ty, int64_t ks[4]);
 // states_out[g] = states[g] advanced by the draws of a whole-map walk of generator g's tile (GF(2) jump with

@@ -467,6 +467,16 @@ __global__ void __launch_bounds__(256) sample_grids_v2_batch_kernel(const Sample
   if (active && !active[blockIdx.z]) return;
   sample_grids_v2_body<NT, NW>(descs[blockIdx.z]);
 }
+// Trials of planners sharing TDM pairs: blockIdx.z is a group (its pair's descriptor), which samples at every step while
+// any of its members runs (group_running, kernels.h).
+template <int NT, int NW>
+__global__ void __launch_bounds__(256) sample_grids_v2_group_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
+                                                                          const SampleGroupDesc* __restrict__ groups,
+                                                                          const int* __restrict__ members,
+                                                                          const int* __restrict__ active) {
+  if (!group_running(groups[blockIdx.z], members, active)) return;
+  sample_grids_v2_body<NT, NW>(descs[blockIdx.z]);
+}
 // [emu:end sampler_batch]
 // [emu:begin sampler_box_batch]
 // closed-loop trials of a stochastic batch: the fused pair blockIdx.z samples the reach box its planner's solve() would
@@ -550,6 +560,76 @@ __global__ void __launch_bounds__(128) advance_states_batch_kernel(const SampleG
                       reinterpret_cast<ulonglong2*>(a.t[1].states_out),
                       reinterpret_cast<const ulonglong2*>(boxes[blockIdx.y].jump_tile), rows, cols, tx, ty, num_maps);
 }
+
+// The same three launches for groups of planners on one shared pair (group blockIdx.z / blockIdx.y, descs one per group,
+// boxes one per planner).  A group's CTAs return while none of its members runs.  The box kernel decides every running
+// member's box and samples their hull (reach_box_hull: one running member's box is exactly its own, disc included);
+// CTA (0, 0) records the decision in the group's record and in every running member's.
+template <int NW>
+__global__ void __launch_bounds__(256) sample_grids_v2_group_box_batch_kernel(
+    const SampleGridsV2Args* __restrict__ descs, const SampleBoxDesc* __restrict__ boxes,
+    const SampleGroupDesc* __restrict__ groups, const int* __restrict__ members, const int* __restrict__ active, int iter,
+    int mrows, int ncact) {
+  const SampleGroupDesc& gd = groups[blockIdx.z];
+  ReachBox b;
+  int n = 0;
+  for (int j = gd.first; j < gd.first + gd.count; ++j) {
+    const int k = members[j];
+    if (!active[k]) continue;
+    const SampleBoxDesc& bd = boxes[k];
+    const float reach = bd.reach[bd.slot ^ (iter & 1)];
+    ReachBox m;
+    reach_box_decide(bd.c, bd.x0[0], bd.x0[1], bd.c.mode == 2 ? &reach : nullptr, &m);
+    reach_box_hull_add(&b, n++, m);
+  }
+  if (n == 0) return;
+  const int how = reach_box_hull_close(boxes[members[gd.first]].c, n, &b);
+  SampleGridsV2Args a = descs[blockIdx.z];
+  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
+    const int r[5] = {how, how ? b.row_lo : 0, how ? b.row_hi : a.rows, how ? b.col_lo : 0, how ? b.col_hi : a.cols};
+    for (int c = 0; c < 5; ++c) gd.record[c] = r[c];
+    for (int j = gd.first; j < gd.first + gd.count; ++j)
+      if (active[members[j]])
+        for (int c = 0; c < 5; ++c) boxes[members[j]].record[c] = r[c];
+  }
+  const int nrow = (a.rows + a.tx - 1) / a.tx;
+  int tix_lo = 0, tix_hi = a.tx, tiy_lo = 0, tiy_hi = a.ty;          // tile rows / columns to cover, [lo, hi)
+  if (how) {
+    a.row_lo = b.row_lo; a.row_hi = b.row_hi;
+    a.disc_cx = b.cx; a.disc_cy = b.cy; a.disc_r = b.r;
+    tix_lo = b.row_lo / nrow; tix_hi = min(a.tx, (b.row_hi - 1) / nrow + 1);
+    tiy_lo = b.tiy_lo; tiy_hi = b.tiy_lo + b.nact;
+  }
+  a.write_states = 0;
+  box_batch_passes<NW>(a, tix_lo, tix_hi, tiy_lo, tiy_hi, mrows, ncact, a.num_maps);
+}
+
+template <int NW>
+__global__ void __launch_bounds__(256) sample_grids_v2_group_complete_batch_kernel(
+    const SampleGridsV2Args* __restrict__ descs, const SampleGroupDesc* __restrict__ groups,
+    const int* __restrict__ members, const int* __restrict__ active, int map_end, int mrows, int ncact) {
+  const SampleGroupDesc& gd = groups[blockIdx.z];
+  if (!group_running(gd, members, active)) return;
+  if (gd.record[0] == 0) return;                                   // this step sampled whole maps already
+  SampleGridsV2Args a = descs[blockIdx.z];
+  a.write_states = 0;
+  box_batch_passes<NW>(a, 0, a.tx, 0, a.ty, mrows, ncact, map_end);
+}
+
+__global__ void __launch_bounds__(128) advance_states_group_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
+                                                                         const SampleBoxDesc* __restrict__ boxes,
+                                                                         const SampleGroupDesc* __restrict__ groups,
+                                                                         const int* __restrict__ members,
+                                                                         const int* __restrict__ active, int rows,
+                                                                         int cols, int tx, int ty, int num_maps) {
+  const SampleGroupDesc& gd = groups[blockIdx.y];
+  if (!group_running(gd, members, active)) return;
+  const SampleGridsV2Args& a = descs[blockIdx.y];
+  advance_states_body(reinterpret_cast<const ulonglong2*>(a.t[0].states), reinterpret_cast<ulonglong2*>(a.t[0].states_out),
+                      reinterpret_cast<ulonglong2*>(a.t[1].states_out),
+                      reinterpret_cast<const ulonglong2*>(boxes[members[gd.first]].jump_tile), rows, cols, tx, ty,
+                      num_maps);
+}
 // [emu:end sampler_box_batch]
 
 void launch_advance_states(const uint64_t* states, uint64_t* out0, uint64_t* out1, const uint64_t* mats, int rows,
@@ -610,7 +690,8 @@ bool sample_grids_v2_same_launch(const SampleGridsV2Args& a, const SampleGridsV2
 }
 
 void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs, int count,
-                                  const int* active, cudaStream_t st) {
+                                  const int* active, cudaStream_t st, const SampleGroupDesc* groups,
+                                  const int* members) {
   const int nrow = (geom.rows + geom.tx - 1) / geom.tx;
   const int tix_hi = std::min(geom.tx - 1, (std::max(geom.row_hi, geom.row_lo + 1) - 1) / nrow);
   const dim3 grid((tix_hi - geom.tix_lo + 1) * geom.segs, (geom.num_maps + geom.gm - 1) / geom.gm, count);
@@ -621,6 +702,17 @@ void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGri
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     kern<<<grid, threads, smem, st>>>(descs, active);
   };
+  auto go_groups = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    kern<<<grid, threads, smem, st>>>(descs, groups, members, active);
+  };
+  if (groups) {
+    if (nw == 3) go_groups(sample_grids_v2_group_batch_kernel<2, 3>);
+    else if (nw == 8) go_groups(sample_grids_v2_group_batch_kernel<2, 8>);
+    else if (nw == 1) go_groups(sample_grids_v2_group_batch_kernel<2, 1>);
+    else go_groups(sample_grids_v2_group_batch_kernel<2, 0>);
+    return;
+  }
   if (nw == 3) go(sample_grids_v2_batch_kernel<2, 3>);
   else if (nw == 8) go(sample_grids_v2_batch_kernel<2, 8>);
   else if (nw == 1) go(sample_grids_v2_batch_kernel<2, 1>);
@@ -643,7 +735,7 @@ bool sample_box_batch_fits(const SampleGridsV2Args& geom, int ncact) {
 
 void launch_sample_grids_v2_box_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
                                       const SampleBoxDesc* boxes, int count, const int* active, int iter, int mrows,
-                                      int ncact, cudaStream_t st) {
+                                      int ncact, cudaStream_t st, const SampleGroupDesc* groups, const int* members) {
   const dim3 grid(mrows * geom.segs, (geom.num_maps + geom.gm - 1) / geom.gm, count);
   const int threads = ((ncact * geom.gm + 31) / 32) * 32;
   const size_t smem = box_batch_smem(geom, ncact);
@@ -652,6 +744,17 @@ void launch_sample_grids_v2_box_batch(const SampleGridsV2Args& geom, const Sampl
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     kern<<<grid, threads, smem, st>>>(descs, boxes, active, iter, mrows, ncact);
   };
+  auto go_groups = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    kern<<<grid, threads, smem, st>>>(descs, boxes, groups, members, active, iter, mrows, ncact);
+  };
+  if (groups) {
+    if (nw == 3) go_groups(sample_grids_v2_group_box_batch_kernel<3>);
+    else if (nw == 8) go_groups(sample_grids_v2_group_box_batch_kernel<8>);
+    else if (nw == 1) go_groups(sample_grids_v2_group_box_batch_kernel<1>);
+    else go_groups(sample_grids_v2_group_box_batch_kernel<0>);
+    return;
+  }
   if (nw == 3) go(sample_grids_v2_box_batch_kernel<3>);
   else if (nw == 8) go(sample_grids_v2_box_batch_kernel<8>);
   else if (nw == 1) go(sample_grids_v2_box_batch_kernel<1>);
@@ -660,7 +763,8 @@ void launch_sample_grids_v2_box_batch(const SampleGridsV2Args& geom, const Sampl
 
 void launch_sample_grids_v2_complete_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
                                            const SampleBoxDesc* boxes, int count, const int* active, int map_end,
-                                           int mrows, int ncact, cudaStream_t st) {
+                                           int mrows, int ncact, cudaStream_t st, const SampleGroupDesc* groups,
+                                           const int* members) {
   const dim3 grid(mrows * geom.segs, (map_end + geom.gm - 1) / geom.gm, count);
   const int threads = ((ncact * geom.gm + 31) / 32) * 32;
   const size_t smem = box_batch_smem(geom, ncact);
@@ -669,6 +773,17 @@ void launch_sample_grids_v2_complete_batch(const SampleGridsV2Args& geom, const 
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     kern<<<grid, threads, smem, st>>>(descs, boxes, active, map_end, mrows, ncact);
   };
+  auto go_groups = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    kern<<<grid, threads, smem, st>>>(descs, groups, members, active, map_end, mrows, ncact);
+  };
+  if (groups) {
+    if (nw == 3) go_groups(sample_grids_v2_group_complete_batch_kernel<3>);
+    else if (nw == 8) go_groups(sample_grids_v2_group_complete_batch_kernel<8>);
+    else if (nw == 1) go_groups(sample_grids_v2_group_complete_batch_kernel<1>);
+    else go_groups(sample_grids_v2_group_complete_batch_kernel<0>);
+    return;
+  }
   if (nw == 3) go(sample_grids_v2_complete_batch_kernel<3>);
   else if (nw == 8) go(sample_grids_v2_complete_batch_kernel<8>);
   else if (nw == 1) go(sample_grids_v2_complete_batch_kernel<1>);
@@ -676,10 +791,15 @@ void launch_sample_grids_v2_complete_batch(const SampleGridsV2Args& geom, const 
 }
 
 void launch_advance_states_batch(const SampleGridsV2Args* descs, const SampleBoxDesc* boxes, int count, int rows,
-                                 int cols, int tx, int ty, int num_maps, const int* active, cudaStream_t st) {
+                                 int cols, int tx, int ty, int num_maps, const int* active, cudaStream_t st,
+                                 const SampleGroupDesc* groups, const int* members) {
   const int64_t total = (int64_t)tx * ty * num_maps;
-  advance_states_batch_kernel<<<dim3((unsigned)((total + 127) / 128), (unsigned)count), 128, 4 * 128 * 16, st>>>(
-      descs, boxes, active, rows, cols, tx, ty, num_maps);
+  const dim3 grid((unsigned)((total + 127) / 128), (unsigned)count);
+  if (groups)
+    advance_states_group_batch_kernel<<<grid, 128, 4 * 128 * 16, st>>>(descs, boxes, groups, members, active, rows, cols,
+                                                                        tx, ty, num_maps);
+  else
+    advance_states_batch_kernel<<<grid, 128, 4 * 128 * 16, st>>>(descs, boxes, active, rows, cols, tx, ty, num_maps);
 }
 
 static inline void next_h(uint64_t& s0, uint64_t& s1);
