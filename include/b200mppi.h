@@ -306,9 +306,19 @@ int b200mppi_planner_launch_count(b200mppi_planner* pl, int64_t* out);
  * those of whole-map sampling.  Readers of the sampled maps outside solve() (get_sample_grids, sample_grid_view,
  * get_state_rollout, planner_rollout) first complete the maps from the pre-solve states.  Whole maps are sampled
  * whenever the bound is not airtight (box not strictly inside the map, ill-formed PMF, generic rollout kernel).
- * Environment: B200MPPI_SAMPLE_BOX = off | static | dynamic (default).
+ * Window-first (the default): a single-rank solve() of one iteration with the windowed rollout samples only the
+ * window the rollout kernel stages around the robot plus a ring of 8 cells, with no host wait; the rollout flags the
+ * maps whose rollouts read outside that rectangle, and two launches gated on the flags complete those maps from the
+ * pre-solve states and rerun their rollouts, so results are again those of whole-map sampling.  sample_box() then
+ * reports the reach box the solve would have sampled (decided on the device, copied back with u).  Sharded solves,
+ * num_opt != 1, batches and trials sample their reach box.
+ * Environment: B200MPPI_SAMPLE_BOX = off | static | dynamic | window (unset: window; any other value: dynamic).
  * out[5] = { mode used by the last solve (0 whole maps, 1 static, 2 dynamic), row_lo, row_hi, col_lo, col_hi }. */
 int b200mppi_planner_sample_box(b200mppi_planner* pl, int32_t out[5]);
+/* Window-first sampling of the last solve(): out[6] = { 1 if it sampled window-first (else 0 and zeros), row_lo,
+ * row_hi, col_lo, col_hi of the rectangle sampled up front, number of maps whose rollouts read outside it (completed
+ * and rerun) }. */
+int b200mppi_planner_sample_window(b200mppi_planner* pl, int32_t out[6]);
 
 /* ------------------------------------------------------------------ batched one-map solves
  * K independent planners of the same shape solved with ONE launch per stage for the whole batch (noise, map sampling,

@@ -122,6 +122,7 @@ def _load():
         "b200mppi_planner_last_timings": (C.c_int, [P, P]),
         "b200mppi_planner_launch_count": (C.c_int, [P, C.POINTER(I64)]),
         "b200mppi_planner_sample_box": (C.c_int, [P, C.POINTER(I32 * 5)]),
+        "b200mppi_planner_sample_window": (C.c_int, [P, C.POINTER(I32 * 6)]),
         "b200mppi_debug_rollout_cta_times": (C.c_int, [I32, P, I32]),
         "b200mppi_batch_create": (C.c_int, [C.POINTER(P), I32, C.POINTER(P)]),
         "b200mppi_batch_create_stochastic": (C.c_int, [C.POINTER(P), I32, C.POINTER(P)]),

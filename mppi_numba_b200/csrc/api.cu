@@ -741,7 +741,7 @@ struct b200mppi_planner {
   bool use_win = true;
   // reach-box sampling: 0 = whole maps every solve, 1 = box from the speed limit, 2 = box from this solve's
   // own clipped controls (max_n sum_t |v|, reduced by the prepare kernel into reach_d and read back mid-solve)
-  int box_mode = 2;
+  int box_mode = 3;              // 3: window-first (planner_window_first), else as 2
   bool disc = true;              // sample the reach disc inside the box (B200MPPI_SAMPLE_DISC=0: the whole box)
   float* reach_d = nullptr;            // two slots, used alternately (noise_prepare_kernel)
   int reach_slot = 0;
@@ -751,7 +751,18 @@ struct b200mppi_planner {
   bool prepared = false;         // noiseT / ctrl hold this iteration's controls
   bool pushed_direct = false;    // the last rollout kernel stored its costs straight into the peers (and signalled)
   int32_t last_box[5] = {};      // b200mppi_planner_sample_box
-  float* h_u = nullptr;        // pinned staging for the T x 2 result (+ one int: exchange status)
+  // window-first sampling (stage_sample_tdms): this solve sampled only the window + ring up front (win_used), the
+  // rectangle win_rect = [row_lo, row_hi, col_lo, col_hi) of its cells; escape flags of the two solve parities (M each)
+  bool win_used = false;
+  bool win_pending = false;            // the maps are sampled window-first for the next stage_rollout
+  int32_t win_rect[4] = {};
+  int32_t win_flagged = 0;             // maps flagged by the last window-first solve
+  unsigned char* esc_d = nullptr;
+  int esc_par = 0;
+  SampleGridsV2Args win_whole{};       // the pair's whole-map plan (completion of the flagged maps)
+  ReachBoxConst win_c{};               // the reach-box decision the completion records
+  float* h_u = nullptr;        // pinned staging for the T x 2 result (+ one int: exchange status, + the reach statistic at
+                               // 2T + 2; a window-first solve's record overwrites [2T, 2T + 8): sample_reach_host)
   // peer-memory exchange (p2p.cu): ONE allocation per planner so that one IPC handle describes it:
   // [ receive buffer (ws, N/ws, M/ws) | gather buffers 2 x (ws, 2T+2) | cost flags | partial flags | counter | status ]
   unsigned char* xbuf = nullptr;
@@ -846,7 +857,8 @@ static int planner_init(b200mppi_planner* p, const b200mppi_config* cfg) {
   p->own_stream = true;
   const size_t nT = (size_t)p->n_local * p->T;
   CU(cudaMalloc(&p->noise, nT * 2 * sizeof(float)));
-  CU(cudaMalloc(&p->u_cur, (size_t)p->T * 2 * sizeof(float)));
+  // + 8 ints: the window-first record (sample_window_complete_kernel), copied back with u at the end of solve()
+  CU(cudaMalloc(&p->u_cur, ((size_t)p->T * 2 + 8) * sizeof(float)));
   CU(cudaMalloc(&p->u_prev, (size_t)p->T * 2 * sizeof(float)));
   CU(cudaMalloc(&p->costs, (size_t)p->n_red * sizeof(float)));
   CU(cudaMalloc(&p->weights, (size_t)p->n_red * sizeof(float)));
@@ -865,7 +877,8 @@ static int planner_init(b200mppi_planner* p, const b200mppi_config* cfg) {
   if (const char* e = getenv("B200MPPI_SAMPLE_BOX")) {
     if (!strcmp(e, "off") || !strcmp(e, "0")) p->box_mode = 0;
     else if (!strcmp(e, "static")) p->box_mode = 1;
-    else p->box_mode = 2;
+    else if (!strcmp(e, "window")) p->box_mode = 3;
+    else p->box_mode = 2;                                  // "dynamic" (and, as before window-first, any other value)
   }
   if (const char* e = getenv("B200MPPI_SAMPLE_DISC")) p->disc = atoi(e) != 0;
   p->num_ctas = update_num_ctas(p->n_red);
@@ -881,7 +894,7 @@ static int planner_init(b200mppi_planner* p, const b200mppi_config* cfg) {
   CU(cudaMemsetAsync(p->costs, 0, (size_t)p->n_red * sizeof(float), p->stream));
   CU(cudaMemsetAsync(p->weights, 0, (size_t)p->n_red * sizeof(float), p->stream));
   CU(cudaMemsetAsync(p->state_rollout, 0, (size_t)V * (p->T + 1) * 3 * sizeof(float), p->stream));
-  CU(cudaMallocHost(&p->h_u, ((size_t)p->T * 2 + 4) * sizeof(float)));
+  CU(cudaMallocHost(&p->h_u, ((size_t)p->T * 2 + 4 + 8) * sizeof(float)));
   // generators n_global*T + t of this shard (mppi.py:118,1367)
   std::vector<uint64_t> h(nT * 2);
   create_xoroshiro_states(h.data(), p->shard_maps ? 0 : (int64_t)p->n_begin * p->T, (int64_t)nT, cfg->seed);
@@ -921,7 +934,7 @@ extern "C" int b200mppi_planner_destroy(b200mppi_planner* p) {
   cudaFree(p->noise); cudaFree(p->u_cur); cudaFree(p->u_prev); cudaFree(p->costs); cudaFree(p->weights);
   cudaFree(p->w_raw); cudaFree(p->costs_nm); cudaFree(p->cta_partials); cudaFree(p->rank_partial);
   cudaFree(p->state_rollout); cudaFree(p->states); cudaFree(p->noiseT); cudaFree(p->ctrl); cudaFree(p->costs_x);
-  cudaFree(p->obstacles); cudaFree(p->reach_d); cudaFree(p->upd_counter_d);
+  cudaFree(p->obstacles); cudaFree(p->reach_d); cudaFree(p->upd_counter_d); cudaFree(p->esc_d);
   for (int s = 0; s < P2P_MAX_PEERS; ++s)
     if (p->peer_ipc[s] && p->peer_x[s]) cudaIpcCloseMemHandle(p->peer_x[s]);
   cudaFree(p->xbuf);
@@ -1089,6 +1102,8 @@ static void fill_win_args(const b200mppi_planner* p, int WW, int WH, RolloutWinA
   w.noiseT = p->noiseT; w.ctrl = p->ctrl; w.u_cur = p->u_cur;
 }
 
+static void last_box_whole_map(b200mppi_planner* p);
+
 static int stage_rollout(b200mppi_planner* p) {
   RolloutArgs a;
   fill_rollout_args(p, a);
@@ -1119,11 +1134,32 @@ static int stage_rollout(b200mppi_planner* p) {
         w.sig.epoch = ++p->epoch_cost;
         for (int r = 0; r < ws; ++r) w.sig.peer_flags[r] = (uint32_t*)(p->peer_x[r] + p->x_flags_cost);
       }
+      if (p->win_pending) w.esc = p->esc_d + (size_t)p->esc_par * p->M;
       CU(launch_rollout_win(w, p->tmaps[0], p->tmaps[1], p->tmaps[2], p->tmaps[3], p->stream));
       p->launches++;
       p->pushed_direct = direct;
       done = true;
+      if (p->win_pending) {
+        p->win_pending = false;
+        // the flagged maps: completed from the pre-call states (the commit swapped them into states_alt), then rerun
+        SampleGridsV2Args c = p->win_whole;
+        c.t[0].states = p->lin->states_alt;
+        launch_sample_window_complete(c, p->win_c, p->prm.x0[0], p->prm.x0[1], p->reach_d + p->reach_slot,
+                                      (int*)(p->u_cur + (size_t)p->T * 2), w.esc,
+                                      p->esc_d + (size_t)(p->esc_par ^ 1) * p->M, p->stream);
+        CHECK_LAUNCH();
+        w.redo = 1;
+        CU(launch_rollout_win(w, p->tmaps[0], p->tmaps[1], p->tmaps[2], p->tmaps[3], p->stream));
+        p->launches += 2;
+        p->esc_par ^= 1;
+      }
     }
+  }
+  if (!done && p->win_pending) {                 // no windowed launch after all: the generic kernel needs whole maps
+    p->win_pending = p->win_used = false;          // no window-first record: sample_box() reports the whole maps
+    last_box_whole_map(p);
+    int rc;
+    if ((rc = tdm_complete_grid(p->lin, p->stream)) || (rc = tdm_complete_grid(p->ang, p->stream))) return rc;
   }
   if (!done) {
     launch_rollout(a, p->stream);
@@ -1209,7 +1245,7 @@ static void fill_reach_const(const b200mppi_planner* p, const SamplePlan& pl, Re
   const b200mppi_tdm* l = p->lin;
   const b200mppi_params& q = p->prm;
   *c = ReachBoxConst{};
-  c->mode = (p->box_mode == 0 || !planner_uses_window(p)) ? 0 : (p->box_mode == 2 && q.num_opt == 1) ? 2 : 1;
+  c->mode = (p->box_mode == 0 || !planner_uses_window(p)) ? 0 : (p->box_mode >= 2 && q.num_opt == 1) ? 2 : 1;
   c->disc = p->disc ? 1 : 0;
   c->T = p->T;
   c->vr0 = q.vrange[0]; c->vr1 = q.vrange[1]; c->dt = q.dt; c->tr_abs_max = l->tr_abs_max;
@@ -1231,9 +1267,11 @@ static double sample_alpha(const b200mppi_planner* p) {
 
 // a box from this solve's own controls: the host waits for their reach statistic only (an event, not the stream)
 static bool sample_reads_reach(const b200mppi_planner* p) {
-  return p->box_mode == 2 && p->prm.num_opt == 1 && p->prepared && p->reach_valid && planner_uses_window(p);
+  return p->box_mode >= 2 && p->prm.num_opt == 1 && p->prepared && p->reach_valid && planner_uses_window(p);
 }
 
+// h_u[2T + 2]: the reach statistic read back by a reach-box solve.  A window-first solve never reads it back; its record
+// (8 ints behind u in u_cur, copied with u) occupies h_u[2T .. 2T + 8), this slot and the exchange status included.
 static float* sample_reach_host(b200mppi_planner* p) { return p->h_u + (size_t)p->T * 2 + 2; }
 
 // The sampling of the pair of the n planners ps (a TDM group of a batch; n = 1: one planner's solve), each deciding its
@@ -1268,11 +1306,61 @@ static int sample_finish(b200mppi_planner* p, SamplePlan& plan, const float* rea
   return sample_finish_group(&p, &reach, 1, plan, advanced, st, launches);
 }
 
+// Window-first sampling: a single-rank solve() of one iteration with the windowed rollout samples only the cells
+// around the window the rollout kernel stages (win_origin) -- known from x0 alone, so no host wait -- plus a ring of
+// WIN_SAMPLE_RING cells.  The rollout flags the maps whose lanes read outside that rectangle (an escape); a completion
+// launch then re-walks those maps whole and records the reach box the solve would have sampled, and a redo launch
+// reruns their rollouts (stage_rollout).  Costs, u and every state are those of whole-map sampling.  Applies to a
+// fused pair whose maps are larger than the window and whose whole-map and windowed launches fit the staged sampler;
+// otherwise the solve samples its reach box.
+static bool planner_window_first(const b200mppi_planner* p, const SamplePlan& plan) {
+  if (p->box_mode != 3 || p->cfg.world_size != 1 || p->shard_maps || p->prm.num_opt != 1 || !p->prepared ||
+      !planner_uses_window(p) || !plan.fused || !plan.v2[0])
+    return false;
+  int WW, WH; size_t smem;
+  rollout_win_geometry(p->T, &WW, &WH, &smem);
+  return p->lin->cols > WW || p->lin->rows > WH;
+}
+
+static int stage_sample_window(b200mppi_planner* p, SamplePlan& plan, bool* used) {
+  *used = false;
+  const b200mppi_tdm* l = p->lin;
+  RolloutWinArgs w{};
+  int WW, WH; size_t smem;
+  rollout_win_geometry(p->T, &WW, &WH, &smem);
+  w.WW = WW; w.WH = WH;
+  win_origin(p->prm.x0[0], p->prm.x0[1], l->pxl[0], l->pyl[0], l->res, l->cols, l->rows, &w.WW);
+  const int R = WIN_SAMPLE_RING;
+  ReachBox b{};
+  b.geo = 1; b.how = 2;
+  b.row_lo = std::max(w.wy0 - R, 0); b.row_hi = std::min(w.wy0 + w.wh + R, l->rows);
+  b.col_lo = std::max(w.wx0 - R, 0); b.col_hi = std::min(w.wx0 + w.ww + R, l->cols);
+  const SampleGridsV2Args whole = plan.a[0];
+  plan_box(&plan, b);
+  if (!plan.boxed[0]) return B200MPPI_OK;                 // the windowed launch does not fit: sample the reach box
+  if (!p->esc_d) {
+    CU(cudaMalloc(&p->esc_d, (size_t)2 * p->M));
+    CU(cudaMemsetAsync(p->esc_d, 0, (size_t)2 * p->M, p->stream));
+  }
+  p->win_whole = whole;
+  p->win_whole.write_states = 0;
+  fill_reach_const(p, plan, &p->win_c);
+  p->win_rect[0] = b.row_lo; p->win_rect[1] = b.row_hi; p->win_rect[2] = b.col_lo; p->win_rect[3] = b.col_hi;
+  p->win_used = p->win_pending = *used = true;
+  return plan_launch(plan, false, p->stream, &p->launches);
+}
+
 static int stage_sample_tdms(b200mppi_planner* p) {
   if (p->cfg.mode == B200MPPI_MODE_BAREBONE) return B200MPPI_OK;      // no maps
   SamplePlan plan;
   int rc = plan_sampling(p->lin, p->ang, sample_alpha(p), p->stream, &plan);
   if (rc) return rc;
+  p->win_used = p->win_pending = false;
+  if (planner_window_first(p, plan)) {
+    bool used;
+    if ((rc = stage_sample_window(p, plan, &used)) || used) return rc;
+    if ((rc = plan_sampling(p->lin, p->ang, sample_alpha(p), p->stream, &plan))) return rc;
+  }
   const float* reach = nullptr;
   bool advanced = false;
   if (sample_reads_reach(p)) {
@@ -1336,9 +1424,17 @@ extern "C" int b200mppi_planner_solve(b200mppi_planner* p, float* u_out) {
     if ((rc = stage_update_partial(p, UPD_TAIL_APPLY))) return rc;
     if (p->profiling) cudaEventRecord(p->ev[5], p->stream);
   }
-  CU(cudaMemcpyAsync(p->h_u, p->u_cur, (size_t)p->T * 2 * sizeof(float), cudaMemcpyDeviceToHost, p->stream));
+  // a window-first solve: its record (sample_window_complete_kernel) sits behind u and comes back in the same copy
+  const bool win = p->win_used && p->prm.num_opt > 0;
+  CU(cudaMemcpyAsync(p->h_u, p->u_cur, ((size_t)p->T * 2 + (win ? 8 : 0)) * sizeof(float), cudaMemcpyDeviceToHost,
+                     p->stream));
   CU(cudaStreamSynchronize(p->stream));
   if (u_out) std::memcpy(u_out, p->h_u, (size_t)p->T * 2 * sizeof(float));
+  if (win) {
+    const int32_t* rec = reinterpret_cast<const int32_t*>(p->h_u + (size_t)p->T * 2);
+    for (int i = 0; i < 5; ++i) p->last_box[i] = rec[i];
+    p->win_flagged = rec[5];
+  }
   if (p->prm.num_opt > 0) collect_timings(p);
   return B200MPPI_OK;
 }
@@ -1773,6 +1869,14 @@ extern "C" int b200mppi_debug_rollout_cta_times(int32_t enable, int64_t* out, in
     CU(cudaMemcpy(out, dev, (size_t)ctas * 6 * sizeof(long long), cudaMemcpyDeviceToHost));
   }
   if (!enable) rollout_win_set_debug(nullptr);
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_planner_sample_window(b200mppi_planner* p, int32_t out[6]) {
+  if (!p || !out) return fail(B200MPPI_EINVAL, "sample_window: null argument");
+  out[0] = p->win_used ? 1 : 0;
+  for (int i = 0; i < 4; ++i) out[1 + i] = p->win_used ? p->win_rect[i] : 0;
+  out[5] = p->win_used ? p->win_flagged : 0;
   return B200MPPI_OK;
 }
 

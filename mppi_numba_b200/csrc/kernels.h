@@ -247,6 +247,12 @@ __host__ __device__ inline bool group_running(const SampleGroupDesc& g, const in
   return false;
 }
 // [emu:end box_desc]
+// window-first sampling's completion (solve()): the reach-box record[6] of this solve (decided on the device, + the
+// number of maps flagged in esc), `clear` zeroed, and the whole maps of every CTA with a flagged map re-walked (a: the
+// fused pair's whole-map plan on its pre-call states, write_states = 0)
+void launch_sample_window_complete(const SampleGridsV2Args& a, const ReachBoxConst& c, float x0x, float x0y,
+                                   const float* reach, int* record, const unsigned char* esc, unsigned char* clear,
+                                   cudaStream_t st);
 // ONE launch for `count` fused pairs of equal geometry (geom: a whole-map plan with the boxed launch's segs / seg_rows /
 // jump and maps per CTA gm): mrows tile rows x the row segments x ncact tile columns, sized for the largest box of the
 // static bound; every CTA narrows to its pair's box and disc, whole maps loop over row and column groups.  No state
@@ -350,6 +356,8 @@ void launch_rollout_batch(const RolloutArgs* descs, int count, int mode, int N, 
                           cudaStream_t st);
 // windowed (TMA-staged) stochastic rollout kernel -- rollout_win.cu
 // [emu:begin win_args]
+// window-first sampling (solve(), api.cu): cells sampled up front around the staged window, on every side
+constexpr int WIN_SAMPLE_RING = 8;
 struct RolloutWinArgs {
   RolloutParams p;
   int WW, WH, wx0, wy0;     // window size / origin in cells (origin inside the map, wx0 a multiple of 16)
@@ -367,6 +375,11 @@ struct RolloutWinArgs {
   const float* u_cur;
   CostDst dst;              // per-(m, n) costs
   CostSignal sig;           // sharded solve with the peer-memory exchange: flags to raise when the kernel is done
+  // window-first sampling (solve(), api.cu): only the window plus a ring of WIN_SAMPLE_RING cells (clipped to the map)
+  // was sampled up front.  esc[m] = 1 when a lane of map m reads the sampled maps at a map cell outside that rectangle (null: the
+  // maps are whole, no test).  redo = 1: run only the maps flagged in esc (completed meanwhile), spread over the grid.
+  unsigned char* esc;
+  int redo;
 };
 // [emu:end win_args]
 // reach (may be null): *reach = max(*reach, max_n sum_t |clipped v[n,t]|) -- bounds how far a rollout can travel

@@ -322,13 +322,16 @@ static __device__ __forceinline__ int cell_from_interval(float a, float r, float
   return cell_index_exact(a, r);
 }
 
+constexpr int WIN_ESCAPE = (int)0x80808080u;   // lookup_slow's report of an escape: four codes -128 (see stage_planner)
+enum { WIN_WHOLE = 0, WIN_DETECT = 1, WIN_REDO = 2 };
+
 // everything that is not "cell proven by the magic-number floors and staged in the window" (~0.1 % of the steps near
 // cell edges, plus the steps of rollouts that left the window): exact reference cell index, then the staged window
 // if the cell is in it, else global memory with the generic kernel's wrap + clamp.  Out of line: one call site, one
 // reconvergence region in the hot loop.
+template <int WW, int PLANE, bool DETECT>
 static __device__ __noinline__ int lookup_slow(float ax, float ay, float res, float inv_lo, float inv_hi, uint32_t sb_win,
-                                               unsigned uww, unsigned uwh,
-                                               int WW, int PLANE, int wx0, int wy0, int rows, int cols, int grid_rows,
+                                               unsigned uww, unsigned uwh, int wx0, int wy0, int rows, int cols, int grid_rows,
                                                int grid_cols, int grid_pitch, int mask_pitch,
                                                const int8_t* __restrict__ g_lin, const int8_t* __restrict__ g_ang,
                                                const int8_t* __restrict__ obstacle, const int8_t* __restrict__ unknown) {
@@ -352,6 +355,13 @@ static __device__ __noinline__ int lookup_slow(float ax, float ay, float res, fl
     qa = __ldg(g_ang + (size_t)gy2 * grid_pitch + gx2);
     ob = __ldg(obstacle + (size_t)my * mask_pitch + mx);
     un = __ldg(unknown + (size_t)my * mask_pitch + mx);
+    // window-first sampling: a map cell outside the sampled rectangle holds a stale byte -- an escape, reported as
+    // WIN_ESCAPE (cells of the allocation beyond the map are never sampled in any mode)
+    constexpr int R = WIN_SAMPLE_RING;
+    if (DETECT && gy2 < rows && gx2 < cols &&
+        (gx2 < max(wx0 - R, 0) || gx2 >= min(wx0 + (int)uww + R, cols) || gy2 < max(wy0 - R, 0) ||
+         gy2 >= min(wy0 + (int)uwh + R, rows)))
+      return WIN_ESCAPE;
   }
   return (ql & 0xff) | ((qa & 0xff) << 8) | ((ob & 0xff) << 16) | (un << 24);     // four int8 in one register
 }
@@ -398,7 +408,7 @@ constexpr int WIN_WW = 240;       // window width in cells (inner TMA box extent
 // copies that planner's RolloutWinArgs from `descs` into shared memory behind the window (per-step scalars are then
 // shared-memory loads, never global ones) and rebuilds the traction tables, s_u and the derived registers from it.
 // Single launch: `g` is the planner's own RolloutWinArgs and the tensor maps are kernel parameters.
-template <int THREADS, int WH, bool MASK01, bool BATCH>
+template <int THREADS, int WH, bool MASK01, bool BATCH, int MODE = WIN_WHOLE>
 __device__ __forceinline__ void rollout_win_body(const RolloutWinArgs& g, const CUtensorMap* tm_lin,
                                                  const CUtensorMap* tm_ang, const CUtensorMap* tm_obs,
                                                  const CUtensorMap* tm_unk, const RolloutWinArgs* descs,
@@ -418,7 +428,20 @@ __device__ __forceinline__ void rollout_win_body(const RolloutWinArgs& g, const 
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int cpm = g.npad >> 5;                               // chunks per map
-  const int units_n = BATCH ? count * g.p.M : g.p.M;         // maps, or (planner, map) units
+  int units_n = BATCH ? count * g.p.M : g.p.M;               // maps, or (planner, map) units
+  if (MODE == WIN_REDO) {
+    // redo: the units are the flagged maps only, in map order (g.unit = 1: dealt chunk by chunk); no flag: every CTA
+    // leaves here
+    int mine = 0;
+    for (int i = tid; i < g.p.M; i += THREADS) mine += g.esc[i] != 0;
+    if (tid == 0) *s_next = 0;
+    __syncthreads();
+    if (mine) atomicAdd(s_next, mine);
+    __syncthreads();
+    units_n = *s_next;
+    __syncthreads();                                        // (s_next is the chunk counter from here on)
+    if (units_n == 0) return;
+  }
   const long long total = (long long)units_n * cpm;
   // share boundaries are multiples of a.unit chunks (32 = one chunk per warp of the CTA when the shares are long
   // enough: every map segment is then a whole number of passes and all warps reach the end-of-segment barrier
@@ -458,6 +481,11 @@ __device__ __forceinline__ void rollout_win_body(const RolloutWinArgs& g, const 
       s_lutL[i] = fma(p.lin_ratio, q, f2d(p.lin_lo)) * dt64;
       s_lutA[i] = fma(p.ang_ratio, q, f2d(p.ang_lo)) * dt64;
     }
+    // window-first sampling: an escape reads the codes of WIN_ESCAPE, whose linear traction is NaN here -- the state, and
+    // with it the cost, turn NaN (NaN stays NaN through every later operation), the map is flagged after the loop and
+    // its costs are recomputed by the REDO launch on complete maps.  A genuine code -128, or a NaN cost without an
+    // escape, only costs a redo that yields the same costs.
+    if (MODE == WIN_DETECT && tid == 0) s_lutL[0] = __hiloint2double(0x7ff80000, 0);
     for (int i = tid; i < 2 * g.p.T; i += THREADS) s_u[i] = a.u_cur[i];
 
     sb_win = smem_u32(smem);
@@ -485,7 +513,11 @@ __device__ __forceinline__ void rollout_win_body(const RolloutWinArgs& g, const 
   uint32_t phase = 0;
   for (long long w = w_lo; w < w_hi;) {
     const int u = (int)(w / cpm);
-    const int m = BATCH ? u % g.p.M : u;
+    int m = BATCH ? u % g.p.M : u;
+    if (MODE == WIN_REDO) {                                 // the u-th flagged map (CTA-uniform: every thread scans)
+      for (int i = 0, seen = 0; i < g.p.M; ++i)
+        if (g.esc[i] && seen++ == u) { m = i; break; }
+    }
     const int c_lo = (int)(w - (long long)u * cpm);
     const int c_hi = (int)min((long long)cpm, w_hi - (long long)u * cpm);       // this map's part of the share
     w += c_hi - c_lo;
@@ -591,8 +623,10 @@ __device__ __forceinline__ void rollout_win_body(const RolloutWinArgs& g, const 
           if (!(((unsigned)wx < uww) & ((unsigned)wy < uwh)))
             atomicAdd(reinterpret_cast<unsigned long long*>(g.dbg) + 6 * blockIdx.x + 5, 1ull);
         }
-        const int pk = lookup_slow(ax, ay, res, inv_lo, inv_hi, sb_win, uww, uwh, WW, PLANE, a.wx0, a.wy0, p.g.rows, p.g.cols, p.g.grid_rows,
-                                   p.g.grid_cols, p.g.grid_pitch, p.g.mask_pitch, g_lin, g_ang, a.obstacle, a.unknown);
+        const int pk = lookup_slow<WW, PLANE, MODE == WIN_DETECT>(ax, ay, res, inv_lo, inv_hi, sb_win, uww, uwh, a.wx0, a.wy0,
+                                                                  p.g.rows, p.g.cols, p.g.grid_rows, p.g.grid_cols,
+                                                                  p.g.grid_pitch, p.g.mask_pitch, g_lin, g_ang, a.obstacle,
+                                                                  a.unknown);
         ql = (int)(int8_t)pk; qa = (int)(int8_t)(pk >> 8); ob = (int)(int8_t)(pk >> 16); un = pk >> 24;
       }
       // ---- noisy clipped control (mppi.py:686-689): `c2`, precomputed per (n, t) by the prepare kernel
@@ -637,6 +671,7 @@ __device__ __forceinline__ void rollout_win_body(const RolloutWinArgs& g, const 
     cost = fadd(cost, a.ctrl[n]);                                           // control cost (mppi.py:708-710)
     const double num = f2d(not_reached) * f2d(sqrt_approx(d2));              // terminal cost (mppi.py:26-28)
     cost = fadd(cost, d2f(num / (f2d(p.v_post) + 1e-6)));
+    if (MODE == WIN_DETECT && cost != cost) a.esc[m] = 1;      // plain byte store, no ordering needed
     if (live) *cost_ptr(a.dst, m, n) = cost;                // map-major: the warp's 32 lanes store one 128-byte line
     }
   }
@@ -667,13 +702,15 @@ __device__ __forceinline__ void rollout_win_body(const RolloutWinArgs& g, const 
   }
 }
 
-template <int THREADS, int WH, bool MASK01>
+// MODE: WIN_WHOLE (complete maps), WIN_DETECT (window-first sampling: flag the maps whose lanes escape, a.esc) or
+// WIN_REDO (rerun the flagged maps once completed: same body, same lane arithmetic)
+template <int THREADS, int WH, bool MASK01, int MODE = WIN_WHOLE>
 __global__ void __launch_bounds__(THREADS, 1) rollout_win_kernel(const RolloutWinArgs a,
                                                                  const __grid_constant__ CUtensorMap tm_lin,
                                                                  const __grid_constant__ CUtensorMap tm_ang,
                                                                  const __grid_constant__ CUtensorMap tm_obs,
                                                                  const __grid_constant__ CUtensorMap tm_unk) {
-  rollout_win_body<THREADS, WH, MASK01, false>(a, &tm_lin, &tm_ang, &tm_obs, &tm_unk, nullptr, nullptr, 1, nullptr);
+  rollout_win_body<THREADS, WH, MASK01, false, MODE>(a, &tm_lin, &tm_ang, &tm_obs, &tm_unk, nullptr, nullptr, 1, nullptr);
 }
 
 // [emu:end win_kernel]
@@ -757,20 +794,25 @@ cudaError_t launch_rollout_win(const RolloutWinArgs& a, const void* tm_lin, cons
                                const void* tm_unk, cudaStream_t st) {
   const WinSmem L = win_smem_layout(a.WW, a.WH, a.p.T);
   typedef void (*WinKernel)(const RolloutWinArgs, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap);
-  static const WinKernel kernels[2][2] = {
-      {rollout_win_kernel<WIN_THREADS, 232, false>, rollout_win_kernel<WIN_THREADS, 232, true>},
-      {rollout_win_kernel<WIN_THREADS, 224, false>, rollout_win_kernel<WIN_THREADS, 224, true>}};
+  static const WinKernel kernels[3][2][2] = {
+      {{rollout_win_kernel<WIN_THREADS, 232, false, WIN_WHOLE>, rollout_win_kernel<WIN_THREADS, 232, true, WIN_WHOLE>},
+       {rollout_win_kernel<WIN_THREADS, 224, false, WIN_WHOLE>, rollout_win_kernel<WIN_THREADS, 224, true, WIN_WHOLE>}},
+      {{rollout_win_kernel<WIN_THREADS, 232, false, WIN_DETECT>, rollout_win_kernel<WIN_THREADS, 232, true, WIN_DETECT>},
+       {rollout_win_kernel<WIN_THREADS, 224, false, WIN_DETECT>, rollout_win_kernel<WIN_THREADS, 224, true, WIN_DETECT>}},
+      {{rollout_win_kernel<WIN_THREADS, 232, false, WIN_REDO>, rollout_win_kernel<WIN_THREADS, 232, true, WIN_REDO>},
+       {rollout_win_kernel<WIN_THREADS, 224, false, WIN_REDO>, rollout_win_kernel<WIN_THREADS, 224, true, WIN_REDO>}}};
   {
     // the opt-in is per device (per-context function): a process may run planners on several GPUs
     static bool attr_set[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-      for (int i = 0; i < 2; ++i)
-        for (int j = 0; j < 2; ++j) {
-          const cudaError_t e = cudaFuncSetAttribute(kernels[i][j], cudaFuncAttributeMaxDynamicSharedMemorySize, WIN_MAX_SMEM);
-          if (e != cudaSuccess) return e;
-        }
+      for (int r = 0; r < 3; ++r)
+        for (int i = 0; i < 2; ++i)
+          for (int j = 0; j < 2; ++j) {
+            const cudaError_t e = cudaFuncSetAttribute(kernels[r][i][j], cudaFuncAttributeMaxDynamicSharedMemorySize, WIN_MAX_SMEM);
+            if (e != cudaSuccess) return e;
+          }
       if (dev >= 0 && dev < 64) attr_set[dev] = true;
     }
   }
@@ -815,13 +857,14 @@ cudaError_t launch_rollout_win(const RolloutWinArgs& a, const void* tm_lin, cons
     unit_read = true;
   }
   if (unit_override == 1 || unit_override == 32 || (unit_override == 0 && (int)grid.x >= a.p.M)) b.unit = unit_override;
+  if (a.redo) b.unit = 1;                                   // a few flagged maps over every CTA, chunk by chunk
   const long long passes = (total + 32LL * grid.x - 1) / (32LL * grid.x);
   b.sync_passes = sync_mode >= 0 ? (sync_mode != 0) : (passes <= WIN_SYNC_MAX_PASSES);
   const CUtensorMap& t0 = *reinterpret_cast<const CUtensorMap*>(tm_lin);
   const CUtensorMap& t1 = *reinterpret_cast<const CUtensorMap*>(tm_ang);
   const CUtensorMap& t2 = *reinterpret_cast<const CUtensorMap*>(tm_obs);
   const CUtensorMap& t3 = *reinterpret_cast<const CUtensorMap*>(tm_unk);
-  kernels[a.WH == 232 ? 0 : 1][a.masks01 ? 1 : 0]<<<grid, WIN_THREADS, L.total, st>>>(b, t0, t1, t2, t3);
+  kernels[!a.esc ? WIN_WHOLE : a.redo ? WIN_REDO : WIN_DETECT][a.WH == 232 ? 0 : 1][a.masks01 ? 1 : 0]<<<grid, WIN_THREADS, L.total, st>>>(b, t0, t1, t2, t3);
   return cudaGetLastError();
 }
 

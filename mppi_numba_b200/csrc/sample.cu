@@ -720,6 +720,58 @@ void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGri
 }
 
 // shared memory of the box batch launch: the widest window of ncact tile columns anywhere in the map
+// window-first sampling (solve(), api.cu), after the detecting rollout: CTA (0, 0) decides this solve's reach box from
+// its reach statistic, as a reach-box solve would (record[0..4], as b200mppi_planner_sample_box reports it), counts the
+// maps flagged in esc (record[5]) and clears `clear` (the other solve parity's flags); then every CTA whose maps include
+// a flagged one re-walks its whole maps from the pre-call states (a: a whole-map plan on states_alt, no state stores)
+// -- inside the sampled rectangle that rewrites the bytes already there.  No flag: every CTA returns after its check.
+template <int NW>
+__global__ void __launch_bounds__(256) sample_window_complete_kernel(const SampleGridsV2Args a, const ReachBoxConst c,
+                                                                     float x0x, float x0y, const float* __restrict__ reach,
+                                                                     int* __restrict__ record,
+                                                                     const unsigned char* __restrict__ esc,
+                                                                     unsigned char* __restrict__ clear) {
+  if (blockIdx.x == 0 && blockIdx.y == 0) {
+    int flagged = 0;
+    for (int i0 = 0; i0 < a.num_maps; i0 += blockDim.x)
+      flagged += __syncthreads_count(i0 + (int)threadIdx.x < a.num_maps && esc[i0 + threadIdx.x]);
+    for (int i = threadIdx.x; i < a.num_maps; i += blockDim.x) clear[i] = 0;
+    if (threadIdx.x == 0) {
+      const float r = *reach;
+      ReachBox b;
+      const int how = reach_box_decide(c, x0x, x0y, c.mode == 2 ? &r : nullptr, &b);
+      record[0] = how;
+      record[1] = how ? b.row_lo : 0; record[2] = how ? b.row_hi : a.rows;
+      record[3] = how ? b.col_lo : 0; record[4] = how ? b.col_hi : a.cols;
+      record[5] = flagged;
+    }
+  }
+  bool any = false;
+  for (int j = 0; j < a.gm; ++j) {
+    const int m = (int)blockIdx.y * a.gm + j;
+    any |= m < a.num_maps && esc[m] != 0;
+  }
+  if (!any) return;                                                  // CTA-uniform
+  sample_grids_v2_body<2, NW>(a);
+}
+
+void launch_sample_window_complete(const SampleGridsV2Args& a, const ReachBoxConst& c, float x0x, float x0y,
+                                   const float* reach, int* record, const unsigned char* esc, unsigned char* clear,
+                                   cudaStream_t st) {
+  const dim3 grid(a.tx * a.segs, (a.num_maps + a.gm - 1) / a.gm);
+  const int threads = v2_threads(a);
+  const size_t smem = sample_grids_v2_smem(a, 2);
+  const int nw = a.t[0].bpad / 4;
+  auto go = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    kern<<<grid, threads, smem, st>>>(a, c, x0x, x0y, reach, record, esc, clear);
+  };
+  if (nw == 3) go(sample_window_complete_kernel<3>);
+  else if (nw == 8) go(sample_window_complete_kernel<8>);
+  else if (nw == 1) go(sample_window_complete_kernel<1>);
+  else go(sample_window_complete_kernel<0>);
+}
+
 static size_t box_batch_smem(const SampleGridsV2Args& geom, int ncact) {
   size_t smem = 0;
   for (int lo = 0; lo + ncact <= geom.ty; ++lo)

@@ -372,6 +372,14 @@ class MPPI_Numba(object):
         check(lib.b200mppi_planner_sample_box(self._handle, C.byref(out)))
         return tuple(int(v) for v in out)
 
+    def sample_window(self):
+        """Window-first sampling of the last solve(): ``(used, row_lo, row_hi, col_lo, col_hi, flagged)`` -- whether it
+        sampled only the rectangle around the rollout window up front, that rectangle, and how many maps had rollouts
+        reading outside it (completed and rerun; include/b200mppi.h, b200mppi_planner_sample_window)."""
+        out = (C.c_int32 * 6)()
+        check(lib.b200mppi_planner_sample_window(self._handle, C.byref(out)))
+        return tuple(int(v) for v in out)
+
     def launch_count(self):
         n = C.c_int64()
         check(lib.b200mppi_planner_launch_count(self._handle, C.byref(n)))
