@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench_trials.py -- closed-loop episodes of K planners: the host-driven loop against the batch's device episodes.
 
-    python bench_trials.py --workload c2|c4|c3|ref|refm|gif|bb --batch K --closed-loop S [--rounds R] [--profile]
+    python bench_trials.py --workload c2|c4|c3|ref|refm|gif|mix|bb --batch K --closed-loop S [--rounds R] [--profile]
                            [--record-every n] [--share-tdms]
 
 c2 and c4 are one-map workloads (MPPI_Batch.run_trials); c3 and ref are stochastic (use_tdm, CVaR cost:
@@ -11,6 +11,10 @@ refm is ref with 2048 sampled maps: a less noisy tail estimate, whose CVaR runs 
 notebook's map-free loop (MPPI_Batch.run_barebone_trials, run_bb below), whose parity check also holds the obstacle
 contact counts against numpy's rule on the device's trajectory.  gif is the shape of the reference's GIF notebook
 (use_tdm, N 1024, M 1024, T 100, 100 visualisation rollouts, a 12 x 6-cell map at 1 m), whose loop draws every step.
+mix is c3's N, M and T with planner k on a map of MIX_SIZES[k % 3] cells a side at c3's resolution and MIX_BINS[k % 2]
+bins: six map geometries in two launch classes (the bins pad to 12 and 8), one run_stochastic_trials call for all.  Its
+rounds add a third leg, "device_per_geometry": one run_stochastic_trials call per map geometry, one after the other,
+the only way to run such planners before trials took several launch classes.
 
 K planners of the workload (bench.py's WORKLOADS, seeds 1..K: different maps, start poses and warm starts), each with
 a seeded ground-truth TractionGrid over its map; every other planner has its goal 1.5 m away (reached within S steps),
@@ -55,7 +59,11 @@ from bench import WORKLOADS, make_planner, workload_name_of   # noqa: E402
 # the reference benchmark's noisy_dyn trial: N 1024, M 1024, T 100 on a 9 x 9-cell map at 1 m (c3's bins)
 LOCAL_WORKLOADS = {"ref": ("tdm", 1024, 1024, 100, 9, 1.0) + tuple(WORKLOADS["c3"][6:]),
                    "refm": ("tdm", 1024, 2048, 100, 9, 1.0) + tuple(WORKLOADS["c3"][6:]),
-                   "gif": ("tdm", 1024, 1024, 100, 6, 1.0) + tuple(WORKLOADS["c3"][6:])}
+                   "gif": ("tdm", 1024, 1024, 100, 6, 1.0) + tuple(WORKLOADS["c3"][6:]),
+                   "mix": WORKLOADS["c3"]}
+# mix: planner k's map size (cells a side) and bin count
+MIX_SIZES = [512, 384, 256]
+MIX_BINS = [12, 8]
 # the GIF notebook's map is 12 cells wide and 6 high, and it draws 100 rollouts; elsewhere square maps, the scenario's V
 MAP_WIDTH = {"gif": 12}
 VIS_ROLLOUTS = {"gif": 100}
@@ -75,18 +83,22 @@ def run(args, emit):
     trials = ((lambda b, g, s, **kw: b.run_stochastic_trials(g, s, **kw)) if stochastic else
               (lambda b, g, s, **kw: b.run_trials(g, s, **kw)))
     W, every = MAP_WIDTH.get(args.workload, H), args.record_every
+    mix = args.workload == "mix"
+    shape = [(MIX_SIZES[k % 3], MIX_SIZES[k % 3], MIX_BINS[k % 2]) if mix else (H, W, B) for k in range(K)]
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     scs = []
     for k in range(K):
-        sc = make_scenario(mode, N=N, M=M, T=T, H=H, W=W, res=res, B=B, seed=k + 1, det_alpha=da, warm_start=True)
+        Hk, Wk, Bk = shape[k]
+        sc = make_scenario(mode, N=N, M=M, T=T, H=Hk, W=Wk, res=res, B=Bk, seed=k + 1, det_alpha=da, warm_start=True)
         if args.workload in VIS_ROLLOUTS:
             sc["cfg"]["num_vis_state_rollouts"] = VIS_ROLLOUTS[args.workload]
         if k % 2 == 0:
             sc["params"]["xgoal"] = sc["params"]["x0"][:2] + np.array([1.2, -0.9])
         scs.append(sc)
     rng = np.random.default_rng(7)
-    grids = [E.TractionGrid(rng.uniform(0.3, 1.0, (H, W)), rng.uniform(0.3, 1.0, (H, W)), res=res) for _ in range(K)]
+    grids = [E.TractionGrid(rng.uniform(0.3, 1.0, shape[k][:2]), rng.uniform(0.3, 1.0, shape[k][:2]), res=res)
+             for k in range(K)]
     A, Bs = [[make_planner(E, sc, 0)[3] for sc in scs] for _ in range(2)]
 
     def reset(pls):
@@ -165,10 +177,29 @@ def run(args, emit):
     if every is not None:
         config["record_every"] = every
         config["host"] = "the host loop calls get_state_rollout() at every recorded step of every running planner"
+    extra = []
+    if mix:
+        geos = sorted(set(shape), reverse=True)
+        parts = [[k for k in range(K) if shape[k] == g] for g in geos]
+        split = [(Batch([A[k] for k in ks]), [grids[k] for k in ks]) for ks in parts]
+
+        def per_geometry_round():
+            reset(A)
+            steps = sum(int(trials(b, g, S)["steps"].sum()) for b, g in split)
+            torch.cuda.synchronize(dev)
+            return steps
+
+        class Launches:                                  # the launches of every per-geometry batch
+            def launch_count(self):
+                return sum(b.launch_count() for b, _ in split)
+        extra.append(("device_per_geometry", per_geometry_round, Launches()))
+        config.update(workload="mix: c3's N, M, T on maps of %s cells a side (res %.1f m), %s bins; planner k: size k %% 3, "
+                               "bins k %% 2" % (MIX_SIZES, res, MIX_BINS),
+                      geometries=[{"cells": g[0], "bins": g[2], "planners": len(ks)} for g, ks in zip(geos, parts)])
     measure(args, emit, host_round, device_round, ba, bb, parity, dev,
             "closed-loop trials: host-driven loop vs " +
             ("MPPI_StochasticBatch.run_stochastic_trials" if stochastic else "MPPI_Batch.run_trials"), config,
-            None if every is None else functools.partial(device_round, record_every=every))
+            None if every is None else functools.partial(device_round, record_every=every), extra)
 
 
 BENCH_ALPHAS = [1.0, 0.8, 0.6, 0.4, 0.2]               # the reference benchmark's cvar_alpha sweep
@@ -274,14 +305,16 @@ def _quiet():
     return contextlib.redirect_stdout(io.StringIO())
 
 
-def measure(args, emit, host_round, device_round, ba, bb, parity, dev, metric, config, recorded_round=None):
-    """R alternating timed rounds of the host loop (on batch bb), the device episodes (on batch ba) and, when given, the
-    device episodes with recording, then the JSON line."""
+def measure(args, emit, host_round, device_round, ba, bb, parity, dev, metric, config, recorded_round=None, extra=()):
+    """R alternating timed rounds of the host loop (on batch bb), the device episodes (on batch ba), when given the
+    device episodes with recording, and the `extra` legs (name, round, object whose launch_count() counts its launches),
+    then the JSON line."""
     import torch
     K = len(ba)
     legs = [("host", host_round, bb), ("device", device_round, ba)]
     if recorded_round is not None:
         legs.append(("device_recorded", recorded_round, ba))
+    legs += list(extra)
     for _, fn, _ in legs:                                 # warm-up of every path
         fn()
     res = {name: [] for name, _, _ in legs}
@@ -331,6 +364,10 @@ def measure(args, emit, host_round, device_round, ba, bb, parity, dev, metric, c
         line.update(device_recorded=rec, speedup_wall_recorded=host["s_per_round_wall"] / rec["s_per_round_wall"],
                     recording_cost_wall=rec["s_per_round_wall"] / devr["s_per_round_wall"] - 1.0,
                     record_kernels_share_of_device_time=record_share)
+    for name, _, _ in extra:
+        ex = summary(name)
+        line[name] = ex
+        line["speedup_wall_over_" + name] = ex["s_per_round_wall"] / devr["s_per_round_wall"]
     emit(json.dumps(line))
 
 
@@ -448,7 +485,7 @@ def main():
     def emit(line):
         os.write(real_stdout, (line + "\n").encode())
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[1])
-    ap.add_argument("--workload", default="c2", choices=["c2", "c4", "c3", "ref", "refm", "gif", "bb"])
+    ap.add_argument("--workload", default="c2", choices=["c2", "c4", "c3", "ref", "refm", "gif", "mix", "bb"])
     ap.add_argument("--batch", type=int, default=64, metavar="K", help="planners in the batch")
     ap.add_argument("--closed-loop", type=int, default=150, metavar="S", help="max control steps per episode")
     ap.add_argument("--rounds", type=int, default=3, help="timed rounds of each loop")
@@ -462,8 +499,8 @@ def main():
         ap.error("--batch, --closed-loop and --rounds must be at least 1")
     if args.record_every is not None and (args.record_every < 1 or args.workload == "bb"):
         ap.error("--record-every must be at least 1, and the bb workload does not take it")
-    if args.share_tdms and args.workload == "bb":
-        ap.error("--share-tdms: barebone planners have no TDMs")
+    if args.share_tdms and args.workload in ("bb", "mix"):
+        ap.error("--share-tdms: barebone planners have no TDMs, and mix planners no common map")
     (run_bb if args.workload == "bb" else run_shared if args.share_tdms else run)(args, emit)
 
 

@@ -403,8 +403,11 @@ int b200mppi_batch_get_state_rollout(b200mppi_batch* b, float* out, size_t bytes
 
 /* ------------------------------------------------------------------ closed-loop trials of a batch
  * Every planner of a MODE_DET_DYN or MODE_SPEED_MAP batch drives a unicycle through one receding-horizon episode on
- * its own ground-truth traction grid, entirely on the device: per step ONE launch each of noise, map sampling, rollout
- * and update for the whole batch (num_opt = 1; num_opt > 1 repeats noise, rollout and update), then the plant step.
+ * its own ground-truth traction grid, entirely on the device: per step ONE launch each of noise, rollout and update for
+ * the whole batch (num_opt > 1 repeats them) and one map-sampling launch per launch class, then the plant step:
+ * 3*num_opt + 1 + C launches for C classes.  The planners' maps may differ in size, resolution and bin count; a launch
+ * class holds the TDM pairs that share the padded bin count of both TDMs, the thread tile and the number of maps, so a
+ * batch on one map geometry is one class (5 launches at num_opt = 1).
  * The plant step is the benchmark loop's: u = u_cur[0]; (lt, at) = grid value of the cell holding (x, y), (0, 0)
  * outside the grid; x += dt*lt*cos(theta)*v, y += dt*lt*sin(theta)*v, theta += dt*at*w in float64; u_cur shifted by
  * one (the last row kept); d = |(x, y) - xgoal| - goal_tolerance, cum_obj += dt + d, cum_dist_to_goal += d.  A planner
@@ -415,8 +418,8 @@ int b200mppi_batch_get_state_rollout(b200mppi_batch* b, float* out, size_t bytes
  * solve() -> plant step -> set_u(shifted u) -> set_params(x0 = float32(new pose)) would leave them, except that the
  * C-side params keep the x0 of the last solve (as in that loop, where the new pose is uploaded by the next solve).
  * Refused (B200MPPI_EINVAL naming the planner) before any work is issued: what batch_solve refuses, MODE_BAREBONE,
- * max_steps < 1, num_opt < 1, a grid or limit that is not usable, a start pose outside the padded limits, and a batch
- * whose TDM pairs cannot all be sampled by the one batched sampler launch.
+ * max_steps < 1, num_opt < 1, a grid or limit that is not usable, a start pose outside the padded limits, and a TDM
+ * pair that the batched sampler cannot take (diverged lin / ang streams, a PMF the staged sampler cannot take).
  *   trials  : count descriptors, in planner order; the grids are uploaded and freed by the call.
  *   xhist   : float64 (count, max_steps+1, 3), NaN after a planner's last step;  uhist: float32 (count, max_steps, 2),
  *             NaN after it;  results: count records;  steps_issued (may be NULL): steps the batch issued. */
@@ -444,16 +447,18 @@ int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial_desc* tria
  * The same episodes, plant step, stop rules, descriptors and results as b200mppi_batch_run_trials, for a batch made by
  * b200mppi_batch_create_stochastic (MODE_TDM, CVaR cost).  Each planner's map-sampling reach box is decided on the device
  * by the function the host-side solve uses, from the pose the plant step wrote and the reach of the controls just drawn,
- * so no step waits for the host.  Per step 4*num_opt + 3 launches for the whole batch: num_opt x (noise + controls,
- * windowed rollout, CVaR, update), one boxed map sampling of every pair, one state advance of every pair and the plant
- * step, which also moves each planner's rollout window.
+ * so no step waits for the host.  Per step 4*num_opt + 1 + 2*C launches for the whole batch and C launch classes (as in
+ * b200mppi_batch_run_trials; 7 at num_opt = 1 on one map geometry): num_opt x (noise + controls, windowed rollout, CVaR,
+ * update), per class one boxed map sampling of its pairs and one state advance of its pairs, and the plant step, which
+ * also moves each planner's rollout window.
  * Afterwards every planner is exactly as `steps` rounds of batch_solve (b200mppi_batch_solve on this batch) -> plant step
  * -> set_u(shifted u) -> set_params(x0 = float32(new pose)) would leave it, bit for bit: u, noise, per-(m, n) costs,
  * costs, weights, the planners' and their TDMs' RNG states, the sampled maps, b200mppi_planner_sample_box and the host-side
  * solve state; the C-side params keep the x0 of the last solve.
  * Refused (B200MPPI_EINVAL naming the planner) before any work is issued: what b200mppi_batch_run_trials and the
- * stochastic batch_solve refuse, and a TDM pair that cannot join the one batched sampler launch (lin == ang, diverged
- * lin / ang streams, a PMF the staged sampler cannot take, a geometry that differs from planner 0's).  A batch made by
+ * stochastic batch_solve refuse, and a TDM pair that the batched sampler cannot take (lin == ang, diverged lin / ang
+ * streams, a PMF the staged sampler cannot take at the planner's alpha_dyn), or a launch class whose boxed sampler
+ * launch does not fit a CTA (naming its first planner).  A batch made by
  * b200mppi_batch_create is refused, naming planner 0's mode. */
 int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps,
                                          double* xhist, float* uhist, b200mppi_trial_result* results,
@@ -495,7 +500,8 @@ int b200mppi_batch_run_barebone_trials(b200mppi_batch* b, const b200mppi_trial_d
  *             in device memory during the call; at the end each written record is copied into rollouts once, and the
  *             rest are set to NaN on the host.
  * Launches: one more per recorded step (the batched visualisation rollouts, before the plant step), and for a
- * stochastic batch one more again: a whole-map sampling of maps [0, V) for every pair whose step sampled a reach box,
+ * stochastic batch one more per launch class: a whole-map sampling of maps [0, V) for every pair whose step sampled a
+ * reach box,
  * from that step's pre-call generator states (the maps the rollouts read; no generator state changes, maps >= V keep
  * their box and are completed by any later reader, as after the host loop).
  * Refused (B200MPPI_EINVAL naming the planner) before any work is issued: what the chosen call refuses, an unknown kind,

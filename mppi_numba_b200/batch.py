@@ -209,8 +209,12 @@ class MPPI_Batch(object):
         Raises ValueError (naming the planner) for barebone batches, a grid count other than K, max_steps < 1,
         num_opt < 1, a grid of another dtype than float64 or integer, a planner that cannot solve (e.g. its start
         pose is outside the padded map limits), record_every < 1 and unequal num_vis_state_rollouts; B200MPPIError
-        when the planners' maps cannot all be sampled by the batch's one sampler launch; with share_tdms, ValueError for
-        the overlaps sharing refuses.  Nothing is issued when the call is refused."""
+        when a planner's TDM pair cannot be sampled by the batched sampler (its lin and ang streams diverged, or its
+        PMF is not one the staged sampler takes); with share_tdms, ValueError for the overlaps sharing refuses.  Nothing
+        is issued when the call is refused.
+        The planners' maps may differ in size, resolution and bin count: each step samples the maps with one launch
+        per class of pairs sharing the padded bin count and thread tile, so a batch on one map geometry issues the
+        launches it always did."""
         if self.kind not in ("det", "spd"):
             raise ValueError("MPPI_Batch.run_trials: planner 0 is a %s planner (trials need det-dynamics or speed-map "
                              "planners)" % self.kind)
@@ -397,8 +401,11 @@ class MPPI_StochasticBatch(MPPI_Batch):
         its pair was sampled over at its last step.
         ``record_every`` as in run_trials: the records equal ``get_state_rollout()`` of that host loop, which completes
         the maps of a boxed sampling first.
+        The planners' maps may differ in size, resolution and bin count, as in run_trials: each step issues one boxed
+        sampler launch and one state advance per class of pairs sharing the padded bin count and thread tile.
         Raises ValueError (naming the planner) as run_trials does; B200MPPIError when a planner cannot take the windowed
-        rollout or its TDM pair cannot join the batch's one sampler launch.  Nothing is issued when the call is
+        rollout, its TDM pair cannot be sampled by the batched sampler (lin == ang, diverged streams, a PMF the staged
+        sampler cannot take) or a class's boxed sampler launch does not fit a CTA.  Nothing is issued when the call is
         refused."""
         return self._trials("MPPI_StochasticBatch.run_stochastic_trials", lib.b200mppi_batch_run_stochastic_trials,
                             traction_grids, max_steps, dt, record_every, _lib.TRIALS_STOCHASTIC)

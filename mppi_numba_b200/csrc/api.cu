@@ -2164,7 +2164,8 @@ static int batch_run_sample(b200mppi_batch* b, const TdmGroups& gr, const Sample
                             const SampleGridsV2Args* d_sg, std::vector<SamplePlan>& plans,
                             const std::vector<char>& joined, int nj) {
   if (nj > 0) {
-    launch_sample_grids_v2_batch(h_sg[0], d_sg, nj, nullptr, b->stream);
+    const SampleGridsV2Args* g0 = h_sg;
+    launch_sample_grids_v2_batch(sample_class_launch(&g0, 1), d_sg, nj, nullptr, nullptr, b->stream);
     b->launches++;
     CHECK_LAUNCH();
   }
@@ -2532,33 +2533,69 @@ static int trial_validate(b200mppi_batch* b, TrialKind kind, const b200mppi_tria
   return B200MPPI_OK;
 }
 
-// A stochastic batch's trial sampler sets (set0: parity 0) and launch size.  Every pair must join the one boxed sampler
-// launch: a fused plan (identical generator streams, well-formed PMF at its alpha, lin != ang) whose launch and box
-// segments equal planner 0's.
+// The launch classes of a trial batch's TDM groups: groups whose fused pairs share what one batched sampler launch fixes
+// in its kernel variant and block shape -- the padded bins of both TDMs (the NW instantiation), the thread tile tx x ty
+// and num_maps -- form one class, in the order of their first group.  Everything else (rows, cols, pitch, row segments,
+// jump tables, boxes) each pair's CTAs read from its own descriptor, so a batch on one map geometry is one class.  A step
+// issues one sampler launch per class (stochastic: and one state advance).
+struct LaunchClasses {
+  std::vector<int> groups;              // class c: groups[first[c] .. first[c + 1]), ascending
+  std::vector<int> first;
+  int size() const { return (int)first.size() - 1; }
+  int count(int c) const { return first[c + 1] - first[c]; }
+};
+
+static LaunchClasses launch_classes(const std::vector<SamplePlan>& plans) {
+  const int G = (int)plans.size();
+  auto same = [](const SampleGridsV2Args& a, const SampleGridsV2Args& b) {
+    return a.t[0].bpad == b.t[0].bpad && a.t[1].bpad == b.t[1].bpad && a.tx == b.tx && a.ty == b.ty &&
+           a.num_maps == b.num_maps;
+  };
+  std::vector<int> of(G, -1), lead;
+  for (int g = 0; g < G; ++g) {
+    for (int c = 0; c < (int)lead.size() && of[g] < 0; ++c)
+      if (same(plans[lead[c]].a[0], plans[g].a[0])) of[g] = c;
+    if (of[g] < 0) { of[g] = (int)lead.size(); lead.push_back(g); }
+  }
+  LaunchClasses lc;
+  lc.first.push_back(0);
+  for (int c = 0; c < (int)lead.size(); ++c) {
+    for (int g = 0; g < G; ++g)
+      if (of[g] == c) lc.groups.push_back(g);
+    lc.first.push_back((int)lc.groups.size());
+  }
+  return lc;
+}
+
+// One class's sampler launches in a trial: its shape, and (stochastic) the launch's tile rows and columns
+struct TrialClass {
+  SampleClassLaunch L{};
+  int mrows = 0, ncact = 0;
+};
+
+// A stochastic batch's trial sampler sets (set0: parity 0), launch classes and per-class launch sizes.  Every pair must
+// be fused (identical generator streams, well-formed PMF at its alpha, lin != ang).
 static int stochastic_trial_plans(b200mppi_batch* b, const TdmGroups& gr, const std::string& fn,
-                                  std::vector<SamplePlan>& plans, std::vector<SampleGridsV2Args>& set0, int* mrows,
-                                  int* ncact) {
+                                  std::vector<SamplePlan>& plans, std::vector<SampleGridsV2Args>& set0,
+                                  LaunchClasses& lc, std::vector<TrialClass>& cls) {
   const int K = (int)b->pl.size(), G = gr.size();
   plans.resize(G);
   for (int g = 0; g < G; ++g) {                       // one plan per TDM group
     b200mppi_planner* p = b->pl[gr.lead(g)];
     const int rc = plan_sampling(p->lin, p->ang, sample_alpha(p), b->stream, &plans[g]);
     if (rc) return rc;
-    const b200mppi_tdm* l = p->lin; const b200mppi_tdm* l0 = b->pl[0]->lin;
-    if (!plans[g].fused || !sample_grids_v2_same_launch(plans[0].a[0], plans[g].a[0]) || l->box_segs != l0->box_segs ||
-        l->box_seg_rows != l0->box_seg_rows)
+    if (!plans[g].fused)
       return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(gr.lead(g)) + ": its TDM pair cannot join the "
                                    "batch's one sampler launch (lin == ang, or map geometry, PMF or generator streams "
                                    "differ from planner 0's)");
   }
-  // the one sampler launch is sized for the largest box the static bound allows (reach_box_decide: at most 2 R / res + 5
-  // cells a side) over all planners that sample a box: mrows tile rows x ncact tile columns with the boxed launch's maps
-  // per CTA.  Whole-map steps loop over such groups.  x0 moves during a trial, so R's rounding terms take their bounds
-  // from the padded map's limits (a box exists only for an x0 inside them).
-  const SampleGridsV2Args& sg = plans[0].a[0];
-  const int nrow = (sg.rows + sg.tx - 1) / sg.tx, ncol = (sg.cols + sg.ty - 1) / sg.ty;
-  double span = 0.0;                                  // cells a side, + margin
-  bool any_box = false;
+  lc = launch_classes(plans);
+  // a class's sampler launch is sized for the largest box the static bound allows (reach_box_decide: at most 2 R / res + 5
+  // cells a side) over its planners that sample a box: mrows tile rows x ncact tile columns with the boxed launch's maps
+  // per CTA, each the largest over the class's pairs of what the pair's own tile size needs.  Whole-map steps loop over
+  // such groups.  x0 moves during a trial, so R's rounding terms take their bounds from the padded map's limits (a box
+  // exists only for an x0 inside them).
+  std::vector<double> span(G, -1.0);                  // per pair: cells a side + margin (-1: no planner gets a box)
   for (int i = 0; i < K; ++i) {
     ReachBoxConst c;
     fill_reach_const(b->pl[i], plans[gr.of[i]], &c);
@@ -2569,28 +2606,67 @@ static int stochastic_trial_plans(b200mppi_batch* b, const TdmGroups& gr, const 
     const double R = reach_radius(c, (double)c.T * std::fmax(std::fabs((double)c.vr0), std::fabs((double)c.vr1)), A,
                                   w + h);
     if (!(R >= 0.0)) continue;                        // that planner never gets a box
-    any_box = true;
-    span = std::fmax(span, 2.0 * R / (double)c.res + 8.0);
+    span[gr.of[i]] = std::fmax(span[gr.of[i]], 2.0 * R / (double)c.res + 8.0);
   }
-  *mrows = sg.tx;
-  *ncact = sg.ty;
-  if (any_box && span < (double)(sg.rows + sg.cols)) {
-    *mrows = std::min(sg.tx, (int)span / nrow + 2);
-    *ncact = std::min(sg.ty, (int)span / ncol + 2);
+  cls.assign(lc.size(), TrialClass{});
+  for (int c = 0; c < lc.size(); ++c) {
+    TrialClass& tc = cls[c];
+    const SampleGridsV2Args& sg0 = plans[lc.groups[lc.first[c]]].a[0];
+    for (int j = lc.first[c]; j < lc.first[c + 1]; ++j) {
+      const int g = lc.groups[j];
+      if (span[g] < 0.0) continue;
+      const SampleGridsV2Args& sg = plans[g].a[0];
+      const int nrow = (sg.rows + sg.tx - 1) / sg.tx, ncol = (sg.cols + sg.ty - 1) / sg.ty;
+      const bool small = span[g] < (double)(sg.rows + sg.cols);
+      tc.mrows = std::max(tc.mrows, small ? std::min(sg.tx, (int)span[g] / nrow + 2) : sg.tx);
+      tc.ncact = std::max(tc.ncact, small ? std::min(sg.ty, (int)span[g] / ncol + 2) : sg.ty);
+    }
+    if (tc.mrows == 0) { tc.mrows = sg0.tx; tc.ncact = sg0.ty; }
+    int gm_b = 128 / tc.ncact;                        // apply_box's maps per CTA for that many tile columns
+    gm_b = std::max(1, std::min(std::min(gm_b, SG_GM_MAX), sg0.num_maps));
+    // the boxed launch's row segments over the whole-map plan
+    std::vector<const SampleGridsV2Args*> mem;
+    for (int j = lc.first[c]; j < lc.first[c + 1]; ++j) {
+      const int g = lc.groups[j];
+      const b200mppi_tdm* l = b->pl[gr.lead(g)]->lin;
+      set0[g] = plans[g].a[0];
+      set0[g].segs = l->box_segs; set0[g].seg_rows = l->box_seg_rows; set0[g].jump = l->jump_box_d;
+      set0[g].write_states = 0;
+      set0[g].gm = gm_b;
+      if (!sample_box_batch_fits(set0[g], tc.ncact))
+        return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(gr.lead(lc.groups[lc.first[c]])) +
+                                     ": the batched sampler launch (" + std::to_string(tc.ncact) + " tile columns x " +
+                                     std::to_string(gm_b) + " maps per CTA) does not fit a CTA");
+      mem.push_back(&set0[g]);
+    }
+    tc.L = sample_box_class_launch(mem.data(), (int)mem.size(), tc.mrows, tc.ncact);
   }
-  int gm_b = 128 / *ncact;                            // apply_box's maps per CTA for that many tile columns
-  gm_b = std::max(1, std::min(std::min(gm_b, SG_GM_MAX), sg.num_maps));
-  // the boxed launch's row segments over the whole-map plan
+  return B200MPPI_OK;
+}
+
+// A one-map batch's trial sampler sets (set0: parity 0, each pair's whole-map plan), launch classes and their shapes.
+// Every pair must be fused.
+static int onemap_trial_plans(b200mppi_batch* b, const TdmGroups& gr, std::vector<SamplePlan>& plans,
+                              std::vector<SampleGridsV2Args>& set0, LaunchClasses& lc, std::vector<TrialClass>& cls) {
+  const int G = gr.size();
+  plans.resize(G);
   for (int g = 0; g < G; ++g) {
-    const b200mppi_tdm* l = b->pl[gr.lead(g)]->lin;
+    const b200mppi_planner* p = b->pl[gr.lead(g)];
+    const int rc = plan_sampling(p->lin, p->ang, BATCH_ALPHA, b->stream, &plans[g]);
+    if (rc) return rc;
+    if (!plans[g].fused)
+      return fail(B200MPPI_EINVAL, "run_trials: planner " + std::to_string(gr.lead(g)) + ": its TDM pair cannot join "
+                                   "the batch's one sampler launch (map geometry, PMF or generator streams differ from "
+                                   "planner 0's)");
     set0[g] = plans[g].a[0];
-    set0[g].segs = l->box_segs; set0[g].seg_rows = l->box_seg_rows; set0[g].jump = l->jump_box_d;
-    set0[g].write_states = 0;
-    set0[g].gm = gm_b;
   }
-  if (!sample_box_batch_fits(set0[0], *ncact))
-    return fail(B200MPPI_EINVAL, fn + ": planner 0: the batched sampler launch (" + std::to_string(*ncact) +
-                                 " tile columns x " + std::to_string(gm_b) + " maps per CTA) does not fit a CTA");
+  lc = launch_classes(plans);
+  cls.assign(lc.size(), TrialClass{});
+  for (int c = 0; c < lc.size(); ++c) {
+    std::vector<const SampleGridsV2Args*> mem;
+    for (int j = lc.first[c]; j < lc.first[c + 1]; ++j) mem.push_back(&set0[lc.groups[j]]);
+    cls[c].L = sample_class_launch(mem.data(), (int)mem.size());
+  }
   return B200MPPI_OK;
 }
 
@@ -2602,15 +2678,19 @@ static const char* mode_name(int mode) {
 // The closed-loop trials of every kind of batch.  Stochastic trials also move each planner's reach box with the robot;
 // with box_mode 2 and num_opt 1 it depends on the controls drawn, so the batched boxed sampler decides it on the device
 // (reach_box_decide, the function sample_finish calls) and a step needs no host round trip.  Per step: num_opt x
-// (noise [+ controls], [first iteration, not barebone: sampler (stochastic: boxed, then the state advance)], rollout
-// [windowed, then CVaR], update) and the plant step, which for stochastic trials also moves each planner's rollout
-// window and for barebone trials counts obstacle contacts.
+// (noise [+ controls], [first iteration, not barebone: per launch class the sampler (stochastic: boxed, then the state
+// advance)], rollout [windowed, then CVaR], update) and the plant step, which for stochastic trials also moves each
+// planner's rollout window and for barebone trials counts obstacle contacts.  With C launch classes (launch_classes; 1
+// for a batch on one map geometry) that is 3 num_opt + 1 + C launches per one-map step, 4 num_opt + 1 + 2 C per
+// stochastic step and 3 num_opt + 1 per barebone step.
 // record_every = n > 0 records the visualisation rollouts of every step s with s % n == 0, after the step's last update
 // and before the plant step (which shifts u_cur and overwrites x0): one batched launch, and for a stochastic batch first
-// one launch that completes maps [0, V) of every pair whose step sampled a box (the maps the rollouts read).
+// one launch per launch class that completes maps [0, V) of every pair whose step sampled a box (the maps the rollouts
+// read).
 // Device buffer of a call: [descriptors (b->h_desc's layout; a one-map batch's parity-0 sampler set is its own section
 // there) | stochastic: the parity-0 sampler set | not barebone: the parity-1 set | stochastic: box descriptors, box
-// records | shared TDM pairs: group records (stochastic), group descriptors, members | states | barebone: contacts |
+// records | shared TDM pairs: group records (stochastic), group descriptors, members | not barebone: the launch classes'
+// pairs | states | barebone: contacts |
 // trials | active K + count | recording: vis descriptors | not barebone: grids | recording: the records (K, R, V, T+1,
 // 3) | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds
 // xhist and uhist: the float64 ground-truth grids (tens of MB for a batch of large maps) are copied straight from the
@@ -2660,19 +2740,14 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   const bool grouped = !barebone && gr.shared();
   std::vector<SamplePlan> plans;
   std::vector<SampleGridsV2Args> set0(K);
-  int mrows = 0, ncact = 0;
+  LaunchClasses lc;
+  std::vector<TrialClass> cls;
   if (stochastic) {
-    if ((rc = stochastic_trial_plans(b, gr, fn, plans, set0, &mrows, &ncact))) return rc;
+    if ((rc = stochastic_trial_plans(b, gr, fn, plans, set0, lc, cls))) return rc;
   } else if (!barebone) {
-    std::vector<char> joined;
-    int nj = 0;
-    if ((rc = batch_plan_sample(b, gr, set0.data(), plans, joined, &nj))) return rc;
-    for (int g = 0; g < G; ++g)
-      if (!joined[g])
-        return fail(B200MPPI_EINVAL, "run_trials: planner " + std::to_string(gr.lead(g)) + ": its TDM pair cannot join "
-                                     "the batch's one sampler launch (map geometry, PMF or generator streams differ from "
-                                     "planner 0's)");
+    if ((rc = onemap_trial_plans(b, gr, plans, set0, lc, cls))) return rc;
   }
+  const int C = barebone ? 0 : lc.size();             // sampler launch classes
   if ((rc = batch_wait_members(b))) return rc;
   const size_t nbox = stochastic ? (size_t)K : 0;      // stochastic-only sections
   const size_t nset = barebone ? 0 : (size_t)G;        // sections of TDM groups
@@ -2685,7 +2760,8 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   const size_t off_grec = off_rec + align256(nbox * 5 * sizeof(int));
   const size_t off_grp = off_grec + align256(ngrp * 5 * sizeof(int));
   const size_t off_mem = off_grp + align256(ngrp * sizeof(SampleGroupDesc));
-  const size_t off_state = off_mem + align256((grouped ? (size_t)K : 0) * sizeof(int));
+  const size_t off_cls = off_mem + align256((grouped ? (size_t)K : 0) * sizeof(int));
+  const size_t off_state = off_cls + align256(nset * sizeof(int));
   const size_t off_con = off_state + align256((size_t)K * sizeof(TrialState));
   const size_t off_tr = off_con + align256(ncon * sizeof(int));
   const size_t off_act = off_tr + align256((size_t)K * sizeof(TrialDev));
@@ -2783,6 +2859,8 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   for (int g = 0; g < (int)ngrp; ++g)
     hg[g] = SampleGroupDesc{gr.first[g], gr.count(g), stochastic ? reinterpret_cast<int*>(d + off_grec) + 5 * g : nullptr};
   if (grouped) std::copy(gr.members.begin(), gr.members.end(), hmem);
+  std::copy(lc.groups.begin(), lc.groups.end(), reinterpret_cast<int*>(h + off_cls));
+  const int* dcls = reinterpret_cast<const int*>(d + off_cls);     // class c's pairs: dcls + lc.first[c]
   const SampleGroupDesc* dgrp = grouped ? reinterpret_cast<const SampleGroupDesc*>(d + off_grp) : nullptr;
   const int* dmem = grouped ? reinterpret_cast<const int*>(d + off_mem) : nullptr;
   hact[K] = K;
@@ -2804,7 +2882,6 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   int* hcount = reinterpret_cast<int*>(h);             // the polled counts, in the no longer needed head of the staging
   for (cudaEvent_t& e : buf.ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   const int num_opt = b->pl[0]->prm.num_opt, npad = b->pl[0]->npad;
-  const SampleGridsV2Args& geom = set0[0];
   int issued = 0;
   for (int s = 0; s < S; ++s) {
     if (s >= TRIAL_POLL) {                            // the count after step s - POLL
@@ -2816,11 +2893,14 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
         const int iter = s * num_opt + k;             // every planner's reach slot toggles once per iteration
         launch_noise_prepare_batch(reinterpret_cast<const NoisePrepDesc*>(d), K, N, T, npad, iter, dact, st);
         CHECK_LAUNCH();
-        if (k == 0) {
-          launch_sample_grids_v2_box_batch(geom, ds[s & 1], db, G, dact, iter, mrows, ncact, st, dgrp, dmem);
+        for (int c = 0; c < C && k == 0; ++c) {
+          const TrialClass& tc = cls[c];
+          const SampleGridsV2Args& g0 = set0[lc.groups[lc.first[c]]];
+          launch_sample_grids_v2_box_batch(tc.L, ds[s & 1], db, lc.count(c), dcls + lc.first[c], dact, iter, tc.mrows,
+                                           tc.ncact, st, dgrp, dmem);
           CHECK_LAUNCH();
-          launch_advance_states_batch(ds[s & 1], db, G, geom.rows, geom.cols, geom.tx, geom.ty, geom.num_maps, dact, st,
-                                      dgrp, dmem);
+          launch_advance_states_batch(ds[s & 1], db, lc.count(c), dcls + lc.first[c], g0.tx, g0.ty, g0.num_maps, dact,
+                                      st, dgrp, dmem);
           CHECK_LAUNCH();
         }
         CU(launch_rollout_win_batch(g0, dw, d + b->off_tm, K, masks01, dact, st));
@@ -2829,8 +2909,8 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       } else {
         launch_sample_noise_batch(reinterpret_cast<const NoiseDesc*>(d), K, N, T, dact, st);
         CHECK_LAUNCH();
-        if (k == 0 && !barebone) {
-          launch_sample_grids_v2_batch(geom, ds[s & 1], G, dact, st, dgrp, dmem);
+        for (int c = 0; c < C && k == 0; ++c) {
+          launch_sample_grids_v2_batch(cls[c].L, ds[s & 1], lc.count(c), dcls + lc.first[c], dact, st, dgrp, dmem);
           CHECK_LAUNCH();
         }
         launch_rollout_batch(dr, K, b->mode, N, T, dact, st);
@@ -2841,8 +2921,10 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     }
     const bool rec_step = record && s % record_every == 0;
     if (rec_step) {
-      if (stochastic) {                               // from the pre-call states this step's sampling read
-        launch_sample_grids_v2_complete_batch(geom, ds[s & 1], db, G, dact, V, mrows, ncact, st, dgrp, dmem);
+      for (int c = 0; c < C && stochastic; ++c) {    // from the pre-call states this step's sampling read
+        const TrialClass& tc = cls[c];
+        launch_sample_grids_v2_complete_batch(tc.L, ds[s & 1], db, lc.count(c), dcls + lc.first[c], dact, V, tc.mrows,
+                                              tc.ncact, st, dgrp, dmem);
         CHECK_LAUNCH();
       }
       launch_state_rollout_batch(reinterpret_cast<const VisBatchDesc*>(d + off_vis), K, V, dact,
@@ -2852,8 +2934,8 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     pa.step = s;
     launch_plant_step(pa, st);
     CHECK_LAUNCH();
-    b->launches += stochastic ? 4 * num_opt + 3 : barebone ? 3 * num_opt + 1 : 3 * num_opt + 2;
-    if (rec_step) b->launches += stochastic ? 2 : 1;
+    b->launches += stochastic ? 4 * num_opt + 1 + 2 * C : 3 * num_opt + 1 + C;
+    if (rec_step) b->launches += stochastic ? 1 + C : 1;
     ++issued;
     CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, dact + K, sizeof(int), cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(buf.ev[s % TRIAL_POLL], st));

@@ -69,6 +69,26 @@ __host__ __device__ inline bool sample_v2_fits_hd(int tiy_lo, int nact, int ty, 
          ((nact * gm + 31) / 32) * 32 <= 256 && bpad0 <= 32 &&
          sample_v2_smem_hd(tiy_lo, nact, ty, cols, bpad0, gm, nt) <= 200 * 1024 && (nt == 1 || bpad0 == bpad1);
 }
+// CTAs along x of a staged launch of `a` on its own: its tile rows [tix_lo, last tile row with box rows] x row segments
+__host__ __device__ inline int sample_v2_grid_x(const SampleGridsV2Args& a) {
+  const int nrow = (a.rows + a.tx - 1) / a.tx;
+  const int last = ((a.row_hi > a.row_lo + 1 ? a.row_hi : a.row_lo + 1) - 1) / nrow;
+  return ((last < a.tx - 1 ? last : a.tx - 1) - a.tix_lo + 1) * a.segs;
+}
+// The shape of one batched launch (launch_sample_grids_v2_batch and the box / completion launches of stochastic trials)
+// over a class of fused pairs that share the bin words of both TDMs (the kernel variant), the thread tile and num_maps:
+// the largest member's CTAs along x and y, threads and shared memory.  Each pair's CTAs beyond its own launch return,
+// so every pair gets exactly the work of its own launch.
+struct SampleClassLaunch {
+  int gx, gy, gm, threads, nw;
+  size_t smem;
+};
+// of the members' whole-map launches (host descriptors)
+SampleClassLaunch sample_class_launch(const SampleGridsV2Args* const* members, int count);
+// of the members' boxed trial launches: mrows tile rows x each member's row segments, ncact tile columns, gm maps per CTA
+SampleClassLaunch sample_box_class_launch(const SampleGridsV2Args* const* members, int count, int mrows, int ncact);
+// the boxed trial launch holds ncact tile columns of pair geom with geom.gm maps per CTA (threads, shared memory)
+bool sample_box_batch_fits(const SampleGridsV2Args& geom, int ncact);
 
 // The reach box of a solve's map sampling (planner_reach_box + plan_box in api.cu; the batched trial sampler decides it
 // on the device with the same function).  A rollout moves at most |traction| * |v| * dt per step, so it stays within
@@ -215,14 +235,16 @@ bool sample_grids_v2_fits(const SampleGridsV2Args& a, int nt);
 void launch_sample_grids_v2(const SampleGridsV2Args& a, int nt, cudaStream_t st);
 // batched one-map solves: equal launch configuration (grid, threads, shared memory, kernel variant)
 bool sample_grids_v2_same_launch(const SampleGridsV2Args& a, const SampleGridsV2Args& b);
-// ONE fused (nt = 2) launch for `count` pairs: descs = device array of their args, geom = any of them (host)
+// ONE fused (nt = 2) launch for `count` pairs: descs = device array of their args, L = their class's shape;
+// pairs (device, may be null): launch entry z is pair pairs[z] (null: pair z) -- the index into descs, active, boxes
+// and groups
 // active (device, may be null): active[pair] == 0 -> that pair's CTAs return at once (closed-loop trials)
-// groups (device, may be null): `count` groups of planners members[] (shared pairs, one descriptor per group), a group
+// groups (device, may be null): groups of planners members[] (shared pairs, one descriptor per group), a group
 // running while any member is active (closed-loop trials with shared TDM pairs)
 struct SampleGroupDesc;
-void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs, int count,
-                                  const int* active, cudaStream_t st, const SampleGroupDesc* groups = nullptr,
-                                  const int* members = nullptr);
+void launch_sample_grids_v2_batch(const SampleClassLaunch& L, const SampleGridsV2Args* descs, int count,
+                                  const int* pairs, const int* active, cudaStream_t st,
+                                  const SampleGroupDesc* groups = nullptr, const int* members = nullptr);
 // closed-loop trials of a stochastic batch: each pair's reach box decided on the device, from the x0 the plant step
 // wrote and the reach statistic of the step's first iteration (slot ^ (iter & 1)).  The decision goes to `record`:
 // [how, row_lo, row_hi, col_lo, col_hi] as b200mppi_planner_sample_box reports it.
@@ -253,29 +275,29 @@ __host__ __device__ inline bool group_running(const SampleGroupDesc& g, const in
 void launch_sample_window_complete(const SampleGridsV2Args& a, const ReachBoxConst& c, float x0x, float x0y,
                                    const float* reach, int* record, const unsigned char* esc, unsigned char* clear,
                                    cudaStream_t st);
-// ONE launch for `count` fused pairs of equal geometry (geom: a whole-map plan with the boxed launch's segs / seg_rows /
-// jump and maps per CTA gm): mrows tile rows x the row segments x ncact tile columns, sized for the largest box of the
-// static bound; every CTA narrows to its pair's box and disc, whole maps loop over row and column groups.  No state
-// stores: launch_advance_states_batch advances the states.
-// groups (may be null): `count` groups as in launch_sample_grids_v2_batch, boxes one per planner; every CTA of a group
-// decides its running members' boxes and samples their hull (reach_box_hull), recorded in the group's record and in
-// every running member's
-void launch_sample_grids_v2_box_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
-                                      const SampleBoxDesc* boxes, int count, const int* active, int iter, int mrows,
-                                      int ncact, cudaStream_t st, const SampleGroupDesc* groups = nullptr,
-                                      const int* members = nullptr);
-// the launch above holds ncact tile columns with geom.gm maps per CTA (threads, shared memory)
-bool sample_box_batch_fits(const SampleGridsV2Args& geom, int ncact);
+// ONE launch for `count` fused pairs of one class (each descriptor: a whole-map plan with its boxed launch's segs /
+// seg_rows / jump, and the class's maps per CTA gm): mrows tile rows x the row segments x ncact tile columns, sized for
+// the largest box of the static bound over the class; every CTA narrows to its pair's box and disc, whole maps loop over
+// row and column groups.  No state stores: launch_advance_states_batch advances the states.
+// L: sample_box_class_launch of the members; pairs as in launch_sample_grids_v2_batch
+// groups (may be null): groups as in launch_sample_grids_v2_batch, boxes one per planner; every CTA of a group decides
+// its running members' boxes and samples their hull (reach_box_hull), recorded in the group's record and in every
+// running member's
+void launch_sample_grids_v2_box_batch(const SampleClassLaunch& L, const SampleGridsV2Args* descs,
+                                      const SampleBoxDesc* boxes, int count, const int* pairs, const int* active,
+                                      int iter, int mrows, int ncact, cudaStream_t st,
+                                      const SampleGroupDesc* groups = nullptr, const int* members = nullptr);
 // recording stochastic trials: whole maps [0, map_end) of every pair whose step sampled a box (record[0] != 0), from the
-// pre-call states of descs[pair].t[0], with the launch geometry of the box launch; no state stores
+// pre-call states of descs[pair].t[0], with the launch shape of the box launch; no state stores
 // (groups: the group's record decides)
-void launch_sample_grids_v2_complete_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
-                                           const SampleBoxDesc* boxes, int count, const int* active, int map_end,
-                                           int mrows, int ncact, cudaStream_t st, const SampleGroupDesc* groups = nullptr,
-                                           const int* members = nullptr);
-// launch_advance_states for `count` pairs (pair blockIdx.y): descs[y].t[0].states -> both TDMs' states_out
-void launch_advance_states_batch(const SampleGridsV2Args* descs, const SampleBoxDesc* boxes, int count, int rows,
-                                 int cols, int tx, int ty, int num_maps, const int* active, cudaStream_t st,
+void launch_sample_grids_v2_complete_batch(const SampleClassLaunch& L, const SampleGridsV2Args* descs,
+                                           const SampleBoxDesc* boxes, int count, const int* pairs, const int* active,
+                                           int map_end, int mrows, int ncact, cudaStream_t st,
+                                           const SampleGroupDesc* groups = nullptr, const int* members = nullptr);
+// launch_advance_states for `count` pairs of one class (pair blockIdx.y, or pairs[blockIdx.y]): descs[pair].t[0].states
+// -> both TDMs' states_out; tx, ty, num_maps: the class's
+void launch_advance_states_batch(const SampleGridsV2Args* descs, const SampleBoxDesc* boxes, int count, const int* pairs,
+                                 int tx, int ty, int num_maps, const int* active, cudaStream_t st,
                                  const SampleGroupDesc* groups = nullptr, const int* members = nullptr);
 // tile classes of a generator: (full | last) tile height x (full | last) tile width -> draws per whole-map walk
 void sample_tile_draws(int rows, int cols, int tx, int ty, int64_t ks[4]);

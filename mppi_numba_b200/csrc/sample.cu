@@ -457,32 +457,46 @@ __global__ void __launch_bounds__(128) advance_states_kernel(const ulonglong2* _
 
 // [emu:end sampler_v2]
 // [emu:begin sampler_batch]
-// batched one-map solves: one fused lin + ang whole-map launch for every pair of the batch, pair blockIdx.z.  The
-// launch geometry (rows, cols, bins, pitch, thread tiles, segments) is the batch's; each descriptor brings its own
-// TDM buffers, threshold table and jump matrices.  A pair with active[z] == 0 is left untouched (active null: every
-// pair runs).
+// batched one-map solves: one fused lin + ang whole-map launch for every pair of the batch, pair blockIdx.z (or
+// pairs[blockIdx.z]: the pairs of one launch class of a trial batch).  The pairs share the kernel variant (bins) and the
+// thread tile; the launch is sized for the largest pair, and each pair's CTAs do what its own launch does, from its
+// descriptor (rows, cols, pitch, segments, TDM buffers, threshold table, jump matrices): the CTAs beyond its own
+// launch return.  A pair with active[z] == 0 is left untouched (active null: every pair runs).
+// The CTA lies inside its own pair's launch (CTA-uniform)
+__device__ __forceinline__ bool v2_cta_in_launch(const SampleGridsV2Args& a) {
+  return (int)blockIdx.x < sample_v2_grid_x(a) && (int)blockIdx.y * a.gm < a.num_maps;
+}
 template <int NT, int NW>
 __global__ void __launch_bounds__(256) sample_grids_v2_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
-                                                                    const int* __restrict__ active = nullptr) {
-  if (active && !active[blockIdx.z]) return;
-  sample_grids_v2_body<NT, NW>(descs[blockIdx.z]);
+                                                                    const int* __restrict__ active = nullptr,
+                                                                    const int* __restrict__ pairs = nullptr) {
+  const int z = pairs ? pairs[blockIdx.z] : (int)blockIdx.z;
+  if (active && !active[z]) return;
+  const SampleGridsV2Args& a = descs[z];
+  if (!v2_cta_in_launch(a)) return;
+  sample_grids_v2_body<NT, NW>(a);
 }
-// Trials of planners sharing TDM pairs: blockIdx.z is a group (its pair's descriptor), which samples at every step while
-// any of its members runs (group_running, kernels.h).
+// Trials of planners sharing TDM pairs: blockIdx.z (or pairs[blockIdx.z]) is a group (its pair's descriptor), which
+// samples at every step while any of its members runs (group_running, kernels.h).
 template <int NT, int NW>
 __global__ void __launch_bounds__(256) sample_grids_v2_group_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
                                                                           const SampleGroupDesc* __restrict__ groups,
                                                                           const int* __restrict__ members,
-                                                                          const int* __restrict__ active) {
-  if (!group_running(groups[blockIdx.z], members, active)) return;
-  sample_grids_v2_body<NT, NW>(descs[blockIdx.z]);
+                                                                          const int* __restrict__ active,
+                                                                          const int* __restrict__ pairs = nullptr) {
+  const int z = pairs ? pairs[blockIdx.z] : (int)blockIdx.z;
+  if (!group_running(groups[z], members, active)) return;
+  const SampleGridsV2Args& a = descs[z];
+  if (!v2_cta_in_launch(a)) return;
+  sample_grids_v2_body<NT, NW>(a);
 }
 // [emu:end sampler_batch]
 // [emu:begin sampler_box_batch]
-// closed-loop trials of a stochastic batch: the fused pair blockIdx.z samples the reach box its planner's solve() would
-// sample (reach_box_decide from the x0 the plant step wrote and this step's reach statistic), or whole maps.  The launch
-// is sized for the largest box the static bound allows: `mrows` tile rows times the pair's box row segments, `ncact`
-// tile columns and the boxed launch's maps per CTA (a.gm).  A boxed step is one pass whose tile rows start at the box's
+// closed-loop trials of a stochastic batch: the fused pair blockIdx.z (or pairs[blockIdx.z]: the pairs of one launch
+// class) samples the reach box its planner's solve() would sample (reach_box_decide from the x0 the plant step wrote and
+// this step's reach statistic), or whole maps.  The launch is sized for the largest box the static bound allows over
+// the class: `mrows` tile rows times the largest pair's box row segments, `ncact` tile columns and the boxed launch's
+// maps per CTA (a.gm, the class's); a pair's CTAs beyond its own mrows x a.segs and maps return.  A boxed step is one pass whose tile rows start at the box's
 // first one; a CTA narrows to the box rows, columns and disc as the single boxed launch does, so it writes the same
 // cells with the same draws.  A whole-map step (and any box larger than the launch) loops over groups of mrows tile rows
 // and ncact tile columns.
@@ -490,6 +504,7 @@ __global__ void __launch_bounds__(256) sample_grids_v2_group_batch_kernel(const 
 template <int NW>
 __device__ __forceinline__ void box_batch_passes(SampleGridsV2Args& a, int tix_lo, int tix_hi, int tiy_lo, int tiy_hi,
                                                  int mrows, int ncact, int map_end) {
+  if ((int)blockIdx.x >= mrows * a.segs || (int)blockIdx.y * a.gm >= map_end) return;    // beyond this pair's launch
   const int nrow = (a.rows + a.tx - 1) / a.tx;
   const int tsub = (int)blockIdx.x / a.segs, seg = (int)blockIdx.x % a.segs;
   for (int tg = tix_lo; tg < tix_hi; tg += mrows) {
@@ -510,10 +525,12 @@ template <int NW>
 __global__ void __launch_bounds__(256) sample_grids_v2_box_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
                                                                         const SampleBoxDesc* __restrict__ boxes,
                                                                         const int* __restrict__ active, int iter,
-                                                                        int mrows, int ncact) {
-  if (active && !active[blockIdx.z]) return;
-  SampleGridsV2Args a = descs[blockIdx.z];
-  const SampleBoxDesc& bd = boxes[blockIdx.z];
+                                                                        int mrows, int ncact,
+                                                                        const int* __restrict__ pairs = nullptr) {
+  const int z = pairs ? pairs[blockIdx.z] : (int)blockIdx.z;
+  if (active && !active[z]) return;
+  SampleGridsV2Args a = descs[z];
+  const SampleBoxDesc& bd = boxes[z];
   const float reach = bd.reach[bd.slot ^ (iter & 1)];
   ReachBox b;
   const int how = reach_box_decide(bd.c, bd.x0[0], bd.x0[1], bd.c.mode == 2 ? &reach : nullptr, &b);
@@ -541,36 +558,43 @@ template <int NW>
 __global__ void __launch_bounds__(256) sample_grids_v2_complete_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
                                                                              const SampleBoxDesc* __restrict__ boxes,
                                                                              const int* __restrict__ active, int map_end,
-                                                                             int mrows, int ncact) {
-  if (active && !active[blockIdx.z]) return;
-  if (boxes[blockIdx.z].record[0] == 0) return;                    // this step sampled whole maps already
-  SampleGridsV2Args a = descs[blockIdx.z];
+                                                                             int mrows, int ncact,
+                                                                             const int* __restrict__ pairs = nullptr) {
+  const int z = pairs ? pairs[blockIdx.z] : (int)blockIdx.z;
+  if (active && !active[z]) return;
+  if (boxes[z].record[0] == 0) return;                             // this step sampled whole maps already
+  SampleGridsV2Args a = descs[z];
   a.write_states = 0;
   box_batch_passes<NW>(a, 0, a.tx, 0, a.ty, mrows, ncact, map_end);
 }
 
-// the state advance of those boxed samplings for every pair (pair blockIdx.y): lin's states into both TDMs' other buffers
+// the state advance of those boxed samplings for every pair (pair blockIdx.y, or pairs[blockIdx.y]): lin's states into
+// both TDMs' other buffers.  Each pair's rows, cols and thread tile come from its descriptor; the launch covers the
+// tx x ty x num_maps generators its class shares.  The five int arguments (rows, cols, tx, ty, num_maps of a
+// one-geometry launch) are not read.
 __global__ void __launch_bounds__(128) advance_states_batch_kernel(const SampleGridsV2Args* __restrict__ descs,
                                                                    const SampleBoxDesc* __restrict__ boxes,
-                                                                   const int* __restrict__ active, int rows, int cols,
-                                                                   int tx, int ty, int num_maps) {
-  if (active && !active[blockIdx.y]) return;
-  const SampleGridsV2Args& a = descs[blockIdx.y];
+                                                                   const int* __restrict__ active, int, int, int, int, int,
+                                                                   const int* __restrict__ pairs = nullptr) {
+  const int z = pairs ? pairs[blockIdx.y] : (int)blockIdx.y;
+  if (active && !active[z]) return;
+  const SampleGridsV2Args& a = descs[z];
   advance_states_body(reinterpret_cast<const ulonglong2*>(a.t[0].states), reinterpret_cast<ulonglong2*>(a.t[0].states_out),
                       reinterpret_cast<ulonglong2*>(a.t[1].states_out),
-                      reinterpret_cast<const ulonglong2*>(boxes[blockIdx.y].jump_tile), rows, cols, tx, ty, num_maps);
+                      reinterpret_cast<const ulonglong2*>(boxes[z].jump_tile), a.rows, a.cols, a.tx, a.ty, a.num_maps);
 }
 
-// The same three launches for groups of planners on one shared pair (group blockIdx.z / blockIdx.y, descs one per group,
-// boxes one per planner).  A group's CTAs return while none of its members runs.  The box kernel decides every running
+// The same three launches for groups of planners on one shared pair (group blockIdx.z / blockIdx.y or pairs[] of it,
+// descs one per group, boxes one per planner).  A group's CTAs return while none of its members runs.  The box kernel decides every running
 // member's box and samples their hull (reach_box_hull: one running member's box is exactly its own, disc included);
 // CTA (0, 0) records the decision in the group's record and in every running member's.
 template <int NW>
 __global__ void __launch_bounds__(256) sample_grids_v2_group_box_batch_kernel(
     const SampleGridsV2Args* __restrict__ descs, const SampleBoxDesc* __restrict__ boxes,
     const SampleGroupDesc* __restrict__ groups, const int* __restrict__ members, const int* __restrict__ active, int iter,
-    int mrows, int ncact) {
-  const SampleGroupDesc& gd = groups[blockIdx.z];
+    int mrows, int ncact, const int* __restrict__ pairs = nullptr) {
+  const int z = pairs ? pairs[blockIdx.z] : (int)blockIdx.z;
+  const SampleGroupDesc& gd = groups[z];
   ReachBox b;
   int n = 0;
   for (int j = gd.first; j < gd.first + gd.count; ++j) {
@@ -584,7 +608,7 @@ __global__ void __launch_bounds__(256) sample_grids_v2_group_box_batch_kernel(
   }
   if (n == 0) return;
   const int how = reach_box_hull_close(boxes[members[gd.first]].c, n, &b);
-  SampleGridsV2Args a = descs[blockIdx.z];
+  SampleGridsV2Args a = descs[z];
   if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
     const int r[5] = {how, how ? b.row_lo : 0, how ? b.row_hi : a.rows, how ? b.col_lo : 0, how ? b.col_hi : a.cols};
     for (int c = 0; c < 5; ++c) gd.record[c] = r[c];
@@ -607,11 +631,13 @@ __global__ void __launch_bounds__(256) sample_grids_v2_group_box_batch_kernel(
 template <int NW>
 __global__ void __launch_bounds__(256) sample_grids_v2_group_complete_batch_kernel(
     const SampleGridsV2Args* __restrict__ descs, const SampleGroupDesc* __restrict__ groups,
-    const int* __restrict__ members, const int* __restrict__ active, int map_end, int mrows, int ncact) {
-  const SampleGroupDesc& gd = groups[blockIdx.z];
+    const int* __restrict__ members, const int* __restrict__ active, int map_end, int mrows, int ncact,
+    const int* __restrict__ pairs = nullptr) {
+  const int z = pairs ? pairs[blockIdx.z] : (int)blockIdx.z;
+  const SampleGroupDesc& gd = groups[z];
   if (!group_running(gd, members, active)) return;
   if (gd.record[0] == 0) return;                                   // this step sampled whole maps already
-  SampleGridsV2Args a = descs[blockIdx.z];
+  SampleGridsV2Args a = descs[z];
   a.write_states = 0;
   box_batch_passes<NW>(a, 0, a.tx, 0, a.ty, mrows, ncact, map_end);
 }
@@ -620,15 +646,17 @@ __global__ void __launch_bounds__(128) advance_states_group_batch_kernel(const S
                                                                          const SampleBoxDesc* __restrict__ boxes,
                                                                          const SampleGroupDesc* __restrict__ groups,
                                                                          const int* __restrict__ members,
-                                                                         const int* __restrict__ active, int rows,
-                                                                         int cols, int tx, int ty, int num_maps) {
-  const SampleGroupDesc& gd = groups[blockIdx.y];
+                                                                         const int* __restrict__ active, int, int,
+                                                                         int, int, int,
+                                                                         const int* __restrict__ pairs = nullptr) {
+  const int z = pairs ? pairs[blockIdx.y] : (int)blockIdx.y;
+  const SampleGroupDesc& gd = groups[z];
   if (!group_running(gd, members, active)) return;
-  const SampleGridsV2Args& a = descs[blockIdx.y];
+  const SampleGridsV2Args& a = descs[z];
   advance_states_body(reinterpret_cast<const ulonglong2*>(a.t[0].states), reinterpret_cast<ulonglong2*>(a.t[0].states_out),
                       reinterpret_cast<ulonglong2*>(a.t[1].states_out),
-                      reinterpret_cast<const ulonglong2*>(boxes[members[gd.first]].jump_tile), rows, cols, tx, ty,
-                      num_maps);
+                      reinterpret_cast<const ulonglong2*>(boxes[members[gd.first]].jump_tile), a.rows, a.cols, a.tx,
+                      a.ty, a.num_maps);
 }
 // [emu:end sampler_box_batch]
 
@@ -689,22 +717,34 @@ bool sample_grids_v2_same_launch(const SampleGridsV2Args& a, const SampleGridsV2
          a.row_hi == b.row_hi && a.t[0].bpad == b.t[0].bpad && a.t[1].bpad == b.t[1].bpad;
 }
 
-void launch_sample_grids_v2_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs, int count,
-                                  const int* active, cudaStream_t st, const SampleGroupDesc* groups,
+SampleClassLaunch sample_class_launch(const SampleGridsV2Args* const* members, int count) {
+  SampleClassLaunch L{};
+  L.nw = members[0]->t[0].bpad / 4;
+  for (int i = 0; i < count; ++i) {
+    const SampleGridsV2Args& a = *members[i];
+    L.gx = std::max(L.gx, sample_v2_grid_x(a));
+    L.gy = std::max(L.gy, (a.num_maps + a.gm - 1) / a.gm);
+    L.gm = std::max(L.gm, a.gm);
+    L.threads = std::max(L.threads, v2_threads(a));
+    L.smem = std::max(L.smem, sample_grids_v2_smem(a, 2));
+  }
+  return L;
+}
+
+void launch_sample_grids_v2_batch(const SampleClassLaunch& L, const SampleGridsV2Args* descs, int count,
+                                  const int* pairs, const int* active, cudaStream_t st, const SampleGroupDesc* groups,
                                   const int* members) {
-  const int nrow = (geom.rows + geom.tx - 1) / geom.tx;
-  const int tix_hi = std::min(geom.tx - 1, (std::max(geom.row_hi, geom.row_lo + 1) - 1) / nrow);
-  const dim3 grid((tix_hi - geom.tix_lo + 1) * geom.segs, (geom.num_maps + geom.gm - 1) / geom.gm, count);
-  const int threads = v2_threads(geom);
-  const size_t smem = sample_grids_v2_smem(geom, 2);
-  const int nw = geom.t[0].bpad / 4;
+  const dim3 grid(L.gx, L.gy, count);
+  const int threads = L.threads;
+  const size_t smem = L.smem;
+  const int nw = L.nw;
   auto go = [&](auto kern) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    kern<<<grid, threads, smem, st>>>(descs, active);
+    kern<<<grid, threads, smem, st>>>(descs, active, pairs);
   };
   auto go_groups = [&](auto kern) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    kern<<<grid, threads, smem, st>>>(descs, groups, members, active);
+    kern<<<grid, threads, smem, st>>>(descs, groups, members, active, pairs);
   };
   if (groups) {
     if (nw == 3) go_groups(sample_grids_v2_group_batch_kernel<2, 3>);
@@ -785,20 +825,35 @@ bool sample_box_batch_fits(const SampleGridsV2Args& geom, int ncact) {
          box_batch_smem(geom, ncact) <= 200 * 1024;
 }
 
-void launch_sample_grids_v2_box_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
-                                      const SampleBoxDesc* boxes, int count, const int* active, int iter, int mrows,
-                                      int ncact, cudaStream_t st, const SampleGroupDesc* groups, const int* members) {
-  const dim3 grid(mrows * geom.segs, (geom.num_maps + geom.gm - 1) / geom.gm, count);
-  const int threads = ((ncact * geom.gm + 31) / 32) * 32;
-  const size_t smem = box_batch_smem(geom, ncact);
-  const int nw = geom.t[0].bpad / 4;
+SampleClassLaunch sample_box_class_launch(const SampleGridsV2Args* const* members, int count, int mrows, int ncact) {
+  SampleClassLaunch L{};
+  L.nw = members[0]->t[0].bpad / 4;
+  for (int i = 0; i < count; ++i) {
+    const SampleGridsV2Args& a = *members[i];
+    L.gx = std::max(L.gx, mrows * a.segs);
+    L.gy = std::max(L.gy, (a.num_maps + a.gm - 1) / a.gm);
+    L.gm = std::max(L.gm, a.gm);
+    L.threads = std::max(L.threads, ((ncact * a.gm + 31) / 32) * 32);
+    L.smem = std::max(L.smem, box_batch_smem(a, ncact));
+  }
+  return L;
+}
+
+void launch_sample_grids_v2_box_batch(const SampleClassLaunch& L, const SampleGridsV2Args* descs,
+                                      const SampleBoxDesc* boxes, int count, const int* pairs, const int* active,
+                                      int iter, int mrows, int ncact, cudaStream_t st, const SampleGroupDesc* groups,
+                                      const int* members) {
+  const dim3 grid(L.gx, L.gy, count);
+  const int threads = L.threads;
+  const size_t smem = L.smem;
+  const int nw = L.nw;
   auto go = [&](auto kern) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    kern<<<grid, threads, smem, st>>>(descs, boxes, active, iter, mrows, ncact);
+    kern<<<grid, threads, smem, st>>>(descs, boxes, active, iter, mrows, ncact, pairs);
   };
   auto go_groups = [&](auto kern) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    kern<<<grid, threads, smem, st>>>(descs, boxes, groups, members, active, iter, mrows, ncact);
+    kern<<<grid, threads, smem, st>>>(descs, boxes, groups, members, active, iter, mrows, ncact, pairs);
   };
   if (groups) {
     if (nw == 3) go_groups(sample_grids_v2_group_box_batch_kernel<3>);
@@ -813,21 +868,21 @@ void launch_sample_grids_v2_box_batch(const SampleGridsV2Args& geom, const Sampl
   else go(sample_grids_v2_box_batch_kernel<0>);
 }
 
-void launch_sample_grids_v2_complete_batch(const SampleGridsV2Args& geom, const SampleGridsV2Args* descs,
-                                           const SampleBoxDesc* boxes, int count, const int* active, int map_end,
-                                           int mrows, int ncact, cudaStream_t st, const SampleGroupDesc* groups,
-                                           const int* members) {
-  const dim3 grid(mrows * geom.segs, (map_end + geom.gm - 1) / geom.gm, count);
-  const int threads = ((ncact * geom.gm + 31) / 32) * 32;
-  const size_t smem = box_batch_smem(geom, ncact);
-  const int nw = geom.t[0].bpad / 4;
+void launch_sample_grids_v2_complete_batch(const SampleClassLaunch& L, const SampleGridsV2Args* descs,
+                                           const SampleBoxDesc* boxes, int count, const int* pairs, const int* active,
+                                           int map_end, int mrows, int ncact, cudaStream_t st,
+                                           const SampleGroupDesc* groups, const int* members) {
+  const dim3 grid(L.gx, (map_end + L.gm - 1) / L.gm, count);
+  const int threads = L.threads;
+  const size_t smem = L.smem;
+  const int nw = L.nw;
   auto go = [&](auto kern) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    kern<<<grid, threads, smem, st>>>(descs, boxes, active, map_end, mrows, ncact);
+    kern<<<grid, threads, smem, st>>>(descs, boxes, active, map_end, mrows, ncact, pairs);
   };
   auto go_groups = [&](auto kern) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    kern<<<grid, threads, smem, st>>>(descs, groups, members, active, map_end, mrows, ncact);
+    kern<<<grid, threads, smem, st>>>(descs, groups, members, active, map_end, mrows, ncact, pairs);
   };
   if (groups) {
     if (nw == 3) go_groups(sample_grids_v2_group_complete_batch_kernel<3>);
@@ -842,16 +897,16 @@ void launch_sample_grids_v2_complete_batch(const SampleGridsV2Args& geom, const 
   else go(sample_grids_v2_complete_batch_kernel<0>);
 }
 
-void launch_advance_states_batch(const SampleGridsV2Args* descs, const SampleBoxDesc* boxes, int count, int rows,
-                                 int cols, int tx, int ty, int num_maps, const int* active, cudaStream_t st,
+void launch_advance_states_batch(const SampleGridsV2Args* descs, const SampleBoxDesc* boxes, int count, const int* pairs,
+                                 int tx, int ty, int num_maps, const int* active, cudaStream_t st,
                                  const SampleGroupDesc* groups, const int* members) {
   const int64_t total = (int64_t)tx * ty * num_maps;
   const dim3 grid((unsigned)((total + 127) / 128), (unsigned)count);
   if (groups)
-    advance_states_group_batch_kernel<<<grid, 128, 4 * 128 * 16, st>>>(descs, boxes, groups, members, active, rows, cols,
-                                                                        tx, ty, num_maps);
+    advance_states_group_batch_kernel<<<grid, 128, 4 * 128 * 16, st>>>(descs, boxes, groups, members, active, 0, 0, tx,
+                                                                        ty, num_maps, pairs);
   else
-    advance_states_batch_kernel<<<grid, 128, 4 * 128 * 16, st>>>(descs, boxes, active, rows, cols, tx, ty, num_maps);
+    advance_states_batch_kernel<<<grid, 128, 4 * 128 * 16, st>>>(descs, boxes, active, 0, 0, tx, ty, num_maps, pairs);
 }
 
 static inline void next_h(uint64_t& s0, uint64_t& s1);
