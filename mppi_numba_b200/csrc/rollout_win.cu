@@ -671,7 +671,9 @@ __device__ __forceinline__ void rollout_win_body(const RolloutWinArgs& g, const 
     cost = fadd(cost, a.ctrl[n]);                                           // control cost (mppi.py:708-710)
     const double num = f2d(not_reached) * f2d(sqrt_approx(d2));              // terminal cost (mppi.py:26-28)
     cost = fadd(cost, d2f(num / (f2d(p.v_post) + 1e-6)));
-    if (MODE == WIN_DETECT && cost != cost) a.esc[m] = 1;      // plain byte store, no ordering needed
+    // plain byte store, no ordering needed.  Only live lanes read cells: a padding lane's cost adds ctrl[n] beyond N,
+    // which nothing writes (whatever the allocation held, NaN included), and must not flag the map
+    if (MODE == WIN_DETECT && live && cost != cost) a.esc[m] = 1;
     if (live) *cost_ptr(a.dst, m, n) = cost;                // map-major: the warp's 32 lanes store one 128-byte line
     }
   }

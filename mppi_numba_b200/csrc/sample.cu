@@ -765,6 +765,7 @@ void launch_sample_grids_v2_batch(const SampleClassLaunch& L, const SampleGridsV
 // maps flagged in esc (record[5]) and clears `clear` (the other solve parity's flags); then every CTA whose maps include
 // a flagged one re-walks its whole maps from the pre-call states (a: a whole-map plan on states_alt, no state stores)
 // -- inside the sampled rectangle that rewrites the bytes already there.  No flag: every CTA returns after its check.
+// [emu:begin window_complete]
 template <int NW>
 __global__ void __launch_bounds__(256) sample_window_complete_kernel(const SampleGridsV2Args a, const ReachBoxConst c,
                                                                      float x0x, float x0y, const float* __restrict__ reach,
@@ -794,6 +795,7 @@ __global__ void __launch_bounds__(256) sample_window_complete_kernel(const Sampl
   if (!any) return;                                                  // CTA-uniform
   sample_grids_v2_body<2, NW>(a);
 }
+// [emu:end window_complete]
 
 void launch_sample_window_complete(const SampleGridsV2Args& a, const ReachBoxConst& c, float x0x, float x0y,
                                    const float* reach, int* record, const unsigned char* esc, unsigned char* clear,

@@ -51,6 +51,7 @@ struct Warp {
   explicit Warp(int lanes) : bar(lanes) {}
 };
 inline std::barrier<>* block_bar = nullptr;   // blocks run one after another: one block barrier at a time
+inline int block_count = 0;                     // __syncthreads_count's sum (zero between calls)
 inline thread_local Warp* warp = nullptr;
 // the block's shared memory: every `extern __shared__` array is a view of it (emu_core.extern_shared)
 alignas(128) inline unsigned char smem[1 << 20];
@@ -60,6 +61,17 @@ alignas(128) inline unsigned char smem[1 << 20];
 static thread_local EmuDim3 threadIdx, blockIdx, blockDim, gridDim;
 static inline void __syncthreads() { emu::block_bar->arrive_and_wait(); }
 static inline void __syncwarp(unsigned = 0xffffffffu) { emu::warp->bar.arrive_and_wait(); }
+// the block barrier plus the number of threads whose predicate is non-zero: counted between two barriers, cleared
+// behind a third (no thread of the next call counts before every thread has read this one's sum)
+static inline int __syncthreads_count(int pred) {
+  if (pred) __atomic_fetch_add(&emu::block_count, 1, __ATOMIC_SEQ_CST);
+  emu::block_bar->arrive_and_wait();
+  const int r = __atomic_load_n(&emu::block_count, __ATOMIC_SEQ_CST);
+  emu::block_bar->arrive_and_wait();
+  if (threadIdx.x == 0) __atomic_store_n(&emu::block_count, 0, __ATOMIC_SEQ_CST);
+  emu::block_bar->arrive_and_wait();
+  return r;
+}
 
 // ---------------------------------------------------------------------------------------- warp collectives
 static inline unsigned __activemask() { return 0xffffffffu; }

@@ -100,7 +100,7 @@ extern "C" int emu_rollout_win(const float* f, const int* g, const double* ratio
   const RolloutParams& p = w.p;
   const int npad = (p.N + 31) / 32 * 32;
   std::vector<double2> noiseT((size_t)(p.T + 1) * npad, double2{0, 0});      // + 1 row: the kernel prefetches unguarded
-  std::vector<float> ctrl(npad, 0.0f);
+  std::vector<float> ctrl(npad, std::nanf(""));               // the padding beyond N: never written (cudaMalloc)
   float reach = 0.0f;
   emu::launch({(unsigned)(npad / 32), 1, 1}, 256, [&] {
     prepare_rollout_kernel(reinterpret_cast<const float2*>(noise), u_cur, noiseT.data(), ctrl.data(), &reach, p.N, p.T, npad,
@@ -155,6 +155,54 @@ extern "C" int emu_rollout_win(const float* f, const int* g, const double* ratio
   }
   return 0;
 }
+
+// window-first sampling (stage_rollout, api.cu): the detecting launch (mode 1, WIN_DETECT) or the redo of the flagged
+// maps (mode 2, WIN_REDO) of the windowed kernel on the 232-row window, with launch_rollout_win's grid and share unit
+// for a 132-SM device (unit 1 for the redo).  costs_mn: the map-major (M, N) costs, in / out (the redo rewrites the
+// flagged maps only); esc[M]: the flags, in / out.  ctrl_pad: what ctrl holds beyond N (the planner's cudaMalloc leaves
+// it as the allocation held it).  origin_out: wx0, wy0, ww, wh.
+extern "C" int emu_rollout_win_esc(const float* f, const int* g, const double* ratios, const int8_t* lin, const int8_t* ang,
+                                   const int8_t* obs, const int8_t* unk, const float* noise, const float* u_cur,
+                                   float* costs_mn, unsigned char* esc, int mode, float ctrl_pad, int masks01,
+                                   int* origin_out) {
+  RolloutWinArgs w{};
+  emu::params(w.p, f, g, ratios, g[8]);
+  const RolloutParams& p = w.p;
+  const int npad = (p.N + 31) / 32 * 32;
+  std::vector<double2> noiseT((size_t)(p.T + 1) * npad, double2{0, 0});      // memset at create
+  std::vector<float> ctrl(npad, ctrl_pad);
+  emu::launch({(unsigned)(npad / 32), 1, 1}, 256, [&] {
+    prepare_rollout_kernel(reinterpret_cast<const float2*>(noise), u_cur, noiseT.data(), ctrl.data(), nullptr, p.N, p.T,
+                           npad, p.lambda, p.u_std[0] * p.u_std[0], p.u_std[1] * p.u_std[1], p.vrange[0], p.vrange[1],
+                           p.wrange[0], p.wrange[1]);
+  });
+  const int WW = WIN_WW, WH = 232;
+  if (win_smem_layout(WW, WH, p.T).total > 232448) return 1;
+  emu::win_place(w, WW, WH);
+  w.npad = npad;
+  w.lin_grid = lin; w.ang_grid = ang; w.obstacle = obs; w.unknown = unk;
+  w.noiseT = reinterpret_cast<const float*>(noiseT.data()); w.ctrl = ctrl.data(); w.u_cur = u_cur;
+  w.dst.n_per = p.N; w.dst.ld = p.N; w.dst.row0 = 0; w.dst.base[0] = costs_mn;
+  w.esc = esc; w.redo = mode == 2;
+  w.masks01 = masks01;
+  if (origin_out) { origin_out[0] = w.wx0; origin_out[1] = w.wy0; origin_out[2] = w.ww; origin_out[3] = w.wh; }
+  const CUtensorMap t_lin{(const unsigned char*)lin, p.g.grid_cols, p.g.grid_rows, p.M, p.g.grid_pitch, WW, WH};
+  const CUtensorMap t_ang{(const unsigned char*)ang, p.g.grid_cols, p.g.grid_rows, p.M, p.g.grid_pitch, WW, WH};
+  const CUtensorMap t_obs{(const unsigned char*)obs, p.g.cols, p.g.rows, 1, p.g.mask_pitch, WW, WH};
+  const CUtensorMap t_unk{(const unsigned char*)unk, p.g.cols, p.g.rows, 1, p.g.mask_pitch, WW, WH};
+  const long long total = (long long)p.M * (npad / 32);        // launch_rollout_win
+  const int ctas = (int)std::min<long long>(std::max<long long>(total / 8, 1), 132);
+  w.unit = (total / (32LL * ctas) >= 4) ? 32 : (ctas >= p.M ? 0 : 1);
+  if (w.redo) w.unit = 1;
+  w.sync_passes = 0;
+  auto run = [&](auto kern) { emu::launch({(unsigned)ctas, 1, 1}, 1024, [&] { kern(w, t_lin, t_ang, t_obs, t_unk); }); };
+  if (mode == 1 && masks01) run(rollout_win_kernel<1024, 232, true, WIN_DETECT>);
+  else if (mode == 1) run(rollout_win_kernel<1024, 232, false, WIN_DETECT>);
+  else if (mode == 2 && masks01) run(rollout_win_kernel<1024, 232, true, WIN_REDO>);
+  else if (mode == 2) run(rollout_win_kernel<1024, 232, false, WIN_REDO>);
+  else return 2;
+  return 0;
+}
 '''
 
 
@@ -169,5 +217,14 @@ def kernels(prep=(), win=()):
             extern_shared(drop_fences(k, 3), 1)]
 
 
-def build(out_dir, extra=""):
-    return _build(out_dir, "rollout_win_emu", kernels(), HARNESS + extra)
+# the escape flag's store as it was before padding lanes were excluded: any NaN cost of the map's chunks flags it
+FLAG_ANY_LANE = ("MODE == WIN_DETECT && live && cost != cost", "MODE == WIN_DETECT && cost != cost")
+
+
+def build(out_dir, extra="", flag_any_lane=False):
+    """``flag_any_lane``: compile the kernel with the flag store of FLAG_ANY_LANE[1] (padding lanes flag too)."""
+    parts = kernels()
+    if flag_any_lane:
+        assert parts[-1].count(FLAG_ANY_LANE[0]) == 1
+        parts[-1] = parts[-1].replace(*FLAG_ANY_LANE)
+    return _build(out_dir, "rollout_win_emu" + ("_any_lane" if flag_any_lane else ""), parts, HARNESS + extra)

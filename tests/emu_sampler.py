@@ -85,6 +85,44 @@ extern "C" int emu_sample_v2(int nt, int8_t* grid0, int8_t* grid1, const int8_t*
 }
 '''
 
+# the completion kernel's entry point (needs the window_complete region)
+WINDOW_COMPLETE = r'''// window-first sampling's completion (stage_rollout, api.cu): sample_window_complete_kernel on the fused pair's
+// whole-map plan (as emu_sample_v2 without a box) from the pre-call states, write_states = 0, with the reach-box
+// decision off (record[0..4] = whole maps).  esc[M]: this solve's flags; clear[M]: the other parity's (zeroed);
+// record[6].  Returns the plan's maps per CTA (> 0) or an error (< 0).
+extern "C" int emu_window_complete(int8_t* grid0, int8_t* grid1, const int8_t* cum0, const int8_t* cum1,
+                                   const uint64_t* states, const int8_t* qv0, const int8_t* qv1, int bpad, int rows,
+                                   int cols, int grid_rows, int pitch, int tx, int ty, int num_maps, double alpha,
+                                   int q_cap, const unsigned char* esc, unsigned char* clear, int* record) {
+  SampleGridsV2Args a{};
+  a.t[0] = SampleTdm{grid0, cum0, states, nullptr, qv0, bpad};
+  a.t[1] = SampleTdm{grid1, cum1, states, nullptr, qv1, bpad};
+  std::vector<uint64_t> T(SAMPLE_TABLE_WORDS);
+  if (!build_sample_thresholds(alpha, q_cap, T.data())) return -1;
+  a.thresholds = T.data();
+  std::vector<uint64_t> J;
+  int segs = 1;
+  emu::segment_jumps(rows, cols, tx, ty, segs, a.seg_rows, J);
+  a.jump = nullptr;
+  a.rows = rows; a.cols = cols; a.grid_rows = grid_rows; a.pitch = pitch; a.tx = tx; a.ty = ty; a.num_maps = num_maps;
+  a.segs = segs;
+  sample_box_full(a);
+  if (a.ty * a.gm > 256) a.gm = 256 / a.ty;
+  a.write_states = 0;
+  const ReachBoxConst c{};
+  const float reach = 0.0f;
+  const int threads = ((a.nact * a.gm + 31) / 32) * 32;              // v2_threads
+  if (threads > 256 || a.gm < 1) return -3;
+  const EmuDim3 grid{(unsigned)(tx * segs), (unsigned)((num_maps + a.gm - 1) / a.gm), 1};
+  emu::sampler_nw(bpad, [&](auto NW) {
+    emu::launch(grid, threads, [&] {
+      sample_window_complete_kernel<decltype(NW)::value>(a, c, 0.0f, 0.0f, &reach, record, esc, clear);
+    });
+  });
+  return a.gm;
+}
+'''
+
 
 def kernels(kernel=None, *more):
     """The sampler's text (``kernel``: the sampler_v2 region, possibly edited; then the named regions of
@@ -94,10 +132,10 @@ def kernels(kernel=None, *more):
             region("common.cuh", "threshold"), extern_shared(kernel + "".join(region("sample.cu", r) for r in more), 2)]
 
 
-def build(out_dir, values_in_registers=None, popc_per_word=None, extra=""):
+def build(out_dir, values_in_registers=None, popc_per_word=None, extra="", more=()):
     """Generate + compile the emulator; returns the loaded ctypes library.  ``values_in_registers`` / ``popc_per_word``
     override the kernel's compile-time switches SG_VALUES_IN_REGISTERS / SG_POPC_PER_WORD (the A/B variants of the
-    value lookup and of the byte count)."""
+    value lookup and of the byte count); ``more``: further regions of csrc/sample.cu (e.g. ``window_complete``)."""
     kernel = region("sample.cu", "sampler_v2")
     tag = ""
     for name, val in (("SG_VALUES_IN_REGISTERS", values_in_registers), ("SG_POPC_PER_WORD", popc_per_word)):
@@ -106,7 +144,9 @@ def build(out_dir, values_in_registers=None, popc_per_word=None, extra=""):
                                 "constexpr bool %s = %s;" % (name, "true" if val else "false"), kernel)
             assert n == 1
             tag += "_%s%d" % (name[3:8].lower(), int(bool(val)))
-    return _build(out_dir, "sampler_emu" + tag, kernels(kernel), HARNESS + extra, link_engine=True)
+    tag += "".join("_" + m for m in more)
+    harness = HARNESS + (WINDOW_COMPLETE if "window_complete" in more else "") + extra
+    return _build(out_dir, "sampler_emu" + tag, kernels(kernel, *more), harness, link_engine=True)
 
 
 def cumulative_table(pmf, bpad):
