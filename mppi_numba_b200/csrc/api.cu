@@ -737,7 +737,7 @@ struct b200mppi_planner {
   uint64_t* states = nullptr;
   float* noiseT = nullptr; float* ctrl = nullptr; int npad = 0;   // windowed rollout kernel inputs
   alignas(64) unsigned char tmaps[4][128];
-  const void* tmap_key[6] = {};  // what the cached tensor maps were encoded for (grids, masks, geometry)
+  const void* tmap_key[8] = {};  // what the cached tensor maps were encoded for (grids, masks, geometry)
   bool use_win = true;
   // reach-box sampling: 0 = whole maps every solve, 1 = box from the speed limit, 2 = box from this solve's
   // own clipped controls (max_n sum_t |v|, reduced by the prepare kernel into reach_d and read back mid-solve)
@@ -1036,12 +1036,15 @@ static int stage_noise(b200mppi_planner* p) {
   return B200MPPI_OK;
 }
 
-// tensor maps of the windowed rollout: encoded once per (buffers, geometry) -- the window origin is a launch coordinate
+// tensor maps of the windowed rollout: encoded once per (buffers, geometry) -- the window origin is a launch coordinate.
+// The allocation shapes are part of the key: a TDM pair of another shape may be handed the freed addresses of the last.
 static bool planner_tensor_maps(b200mppi_planner* p, int WW, int WH) {
   const b200mppi_tdm* l = p->lin; const b200mppi_tdm* g = p->ang;
-  const void* key[6] = {l->grid, g->grid, l->obstacle, l->unknown,
+  const void* key[8] = {l->grid, g->grid, l->obstacle, l->unknown,
                         (const void*)(((size_t)l->mask_rows << 40) ^ ((size_t)l->mask_cols << 20) ^ (size_t)l->mask_pitch),
-                        (const void*)(((size_t)WW << 40) ^ ((size_t)WH << 20) ^ (size_t)l->num_maps)};
+                        (const void*)(((size_t)WW << 40) ^ ((size_t)WH << 20) ^ (size_t)l->num_maps),
+                        (const void*)(((size_t)l->cfg.max_map_rows << 40) ^ ((size_t)l->cfg.max_map_cols << 20) ^ (size_t)l->pitch),
+                        (const void*)(((size_t)g->cfg.max_map_rows << 40) ^ ((size_t)g->cfg.max_map_cols << 20) ^ (size_t)g->pitch)};
   if (!std::memcmp(key, p->tmap_key, sizeof(key))) return true;
   const bool ok =
       make_u8_tensor_map(p->tmaps[0], l->grid, 3, l->cfg.max_map_cols, l->cfg.max_map_rows, l->num_maps, l->pitch, WW, WH) &&

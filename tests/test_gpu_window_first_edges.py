@@ -18,6 +18,7 @@ from oracle import terrain_ref as TR
 from tests import reduce_bounds as RB
 from tests import rollout_edge_cases as EC
 from tests import window_first_cases as WF
+from tests.window_first_cases import MOVING, crop as _crop, moving as _moving
 from tests.gpu_harness import assert_all_equal, dev, eng, quiet, tdm_planner  # noqa: F401
 from tests.scenarios import make_scenario, oracle_rollout_costs
 
@@ -26,20 +27,16 @@ pytestmark = pytest.mark.gpu
 F32 = np.float32
 SENTINEL = -77                       # no sampled code, and not -128 (the detecting kernel's escape code)
 MODES = ("window", "off", "dynamic")
-MOVING = np.array([0.0, 0.6, 0.7, 0.85, 1.0])    # bin values of the escape scenarios (bin 0 emptied by _moving)
 
 
-def _moving(sc):
-    """No traction-0 cell: bin 0's mass moved to bin 1, so no rollout stops before it can leave the window."""
-    for key in ("pmf_lin", "pmf_ang"):
-        sc[key][1] += sc[key][0]
-        sc[key][0] = 0
-    return sc
-
-
-def _fill(pl):
-    for t in (pl.lin_tdm, pl.ang_tdm):
-        t.sample_grid_batch_d.copy_to_device(np.full(t.sample_grid_batch_d.shape, SENTINEL, np.int8))
+def _fill(pl, fill=None):
+    """Write the pre-solve maps of both TDMs: SENTINEL everywhere, or fill(pl) = dict(lin, ang) of whole allocations.
+    Returns what was written."""
+    out = fill(pl) if fill else {w: np.full(t.sample_grid_batch_d.shape, SENTINEL, np.int8)
+                                 for w, t in (("lin", pl.lin_tdm), ("ang", pl.ang_tdm))}
+    pl.lin_tdm.sample_grid_batch_d.copy_to_device(out["lin"])
+    pl.ang_tdm.sample_grid_batch_d.copy_to_device(out["ang"])
+    return out
 
 
 def _planners(E, sc, monkeypatch):
@@ -58,11 +55,12 @@ def _state(pl):
                 lin_map=lin.sample_grid_batch_d.copy_to_host(), ang_map=ang.sample_grid_batch_d.copy_to_host())
 
 
-def _solve(pls, sc, dev, what, expect_flags=None, sentinel_read=False):
+def _solve(pls, sc, dev, what, expect_flags=None, sentinel_read=False, fill=None):
     """One solve of the three twins with sentinel maps; every check of the module docstring.  Returns None when the
     window planner did not take window-first sampling, else dict(flags (the count), reads (WF.escapes), cells
-    (WF.executed_cells), rows, cols, rect).  ``sentinel_read``: some escaping read lies outside the cells the
-    window-first sampling writes, so the byte there is the sentinel until the completion."""
+    (WF.executed_cells), rows, cols, rect, states (the oracle's)).  ``sentinel_read``: some escaping read lies outside
+    the cells the window-first sampling writes, so the byte there is the sentinel until the completion.  ``fill``: the
+    pre-solve maps (see _fill), which the oracle's sampling starts from."""
     pl = pls["window"]
     lin, ang = pl.lin_tdm, pl.ang_tdm
     u_pre = pl.u_cur_d.copy_to_host()
@@ -71,7 +69,9 @@ def _solve(pls, sc, dev, what, expect_flags=None, sentinel_read=False):
     snaps, us = {}, {}
     for mode in MODES:
         p = pls[mode]
-        _fill(p)
+        pre = _fill(p, fill)
+        if mode == "window":
+            base = pre
         n0 = p.launch_count()
         with quiet():
             us[mode] = p.solve()
@@ -89,8 +89,8 @@ def _solve(pls, sc, dev, what, expect_flags=None, sentinel_read=False):
     # the oracle: both TDMs sampled whole from lin's pre-solve stream (the fused pair), on sentinel maps
     cfg_tile, M = lin.thread_dim, lin.sample_grid_batch_d.shape[0]
     grids = []
-    for t in (lin, ang):
-        g = np.full(t.sample_grid_batch_d.shape, SENTINEL, np.int8)
+    for name, t in (("lin", lin), ("ang", ang)):
+        g = base[name].copy()
         TR.sample_grids(g, t.pmf_grid_d.copy_to_host(), st_pre.copy(), t.bin_values, t.bin_values_bounds,
                         float(pl.params.get("alpha_dyn", 1.0)), cfg_tile, M)
         grids.append(g)
@@ -117,7 +117,7 @@ def _solve(pls, sc, dev, what, expect_flags=None, sentinel_read=False):
         assert any(not (r0 <= gy < r1 and c0 <= gx < c1) for *_, gy, gx in reads), (what, rect, reads[:4])
     cells = WF.executed_cells(states, lin.padded_xlimits[0], lin.padded_ylimits[0], lin.res, pl.params["xgoal"],
                               pl.params["goal_tolerance"], dev)
-    return dict(flags=int(flags.sum()), reads=reads, cells=cells, rows=rows, cols=cols, rect=rect)
+    return dict(flags=int(flags.sum()), reads=reads, cells=cells, rows=rows, cols=cols, rect=rect, states=states)
 
 
 # ----------------------------------------------------------------------------- 1. ragged N
@@ -142,19 +142,6 @@ def test_ragged_n(eng, dev, monkeypatch, N, escape):
 # ----------------------------------------------------------------------------- 2. map edges
 EDGE_MAPS = [c for c in EC.MAP_CASES if EC.padded_grid(*c)[0] > 232 or EC.padded_grid(*c)[1] > 240] + \
     [(600, 600, 0.1), (100, 600, 0.1), (600, 100, 0.1)]
-
-
-def _crop(sc, rows, cols, res):
-    """make_scenario draws square maps: keep the rows x cols corner."""
-    pad = EC.pad_cells(res)
-    for key in ("pmf_lin", "pmf_ang"):
-        sc[key] = np.ascontiguousarray(sc[key][:, :rows, :cols])
-    for key in ("obstacle", "unknown"):
-        sc[key] = np.ascontiguousarray(sc[key][:rows, :cols])
-    sc["tdm_dict"] = dict(sc["tdm_dict"], xlimits=np.array([0.0, cols * res]), ylimits=np.array([0.0, rows * res]))
-    sc["cfg"] = dict(sc["cfg"], max_map_dim=(rows + 2 * pad, cols + 2 * pad))
-    sc["params"] = dict(sc["params"], x0=np.array([cols * res / 2, rows * res / 2, 0.0]))
-    return sc
 
 
 # heading of each robot spot: out of the map across the nearest edge (the corners), so that steps of up to 1.2 m

@@ -11,9 +11,32 @@ window_complete kernel) re-walks the maps of every map group (gm maps per CTA) t
 import numpy as np
 
 from oracle import mppi_ref as MR
+from tests import rollout_edge_cases as EC
 
 F32 = np.float32
 WIN_SAMPLE_RING = 8
+MOVING = np.array([0.0, 0.6, 0.7, 0.85, 1.0])    # bin values of the escape scenarios (bin 0 emptied by moving())
+
+
+def moving(sc):
+    """No traction-0 cell: bin 0's mass moved to bin 1, so no rollout stops before it can leave the window."""
+    for key in ("pmf_lin", "pmf_ang"):
+        sc[key][1] += sc[key][0]
+        sc[key][0] = 0
+    return sc
+
+
+def crop(sc, rows, cols, res):
+    """make_scenario draws square maps: keep the rows x cols corner."""
+    pad = EC.pad_cells(res)
+    for key in ("pmf_lin", "pmf_ang"):
+        sc[key] = np.ascontiguousarray(sc[key][:, :rows, :cols])
+    for key in ("obstacle", "unknown"):
+        sc[key] = np.ascontiguousarray(sc[key][:rows, :cols])
+    sc["tdm_dict"] = dict(sc["tdm_dict"], xlimits=np.array([0.0, cols * res]), ylimits=np.array([0.0, rows * res]))
+    sc["cfg"] = dict(sc["cfg"], max_map_dim=(rows + 2 * pad, cols + 2 * pad))
+    sc["params"] = dict(sc["params"], x0=np.array([cols * res / 2, rows * res / 2, 0.0]))
+    return sc
 
 
 def window_rect(wx0, wy0, ww, wh, rows, cols, ring=WIN_SAMPLE_RING):
