@@ -2,7 +2,7 @@
 """bench_trials.py -- closed-loop episodes of K planners: the host-driven loop against the batch's device episodes.
 
     python bench_trials.py --workload c2|c4|c3|ref|refm|gif|mix|bb --batch K --closed-loop S [--rounds R] [--profile]
-                           [--record-every n] [--share-tdms]
+                           [--record-every n] [--share-tdms] [--episodes E]
 
 c2 and c4 are one-map workloads (MPPI_Batch.run_trials); c3 and ref are stochastic (use_tdm, CVaR cost:
 MPPI_StochasticBatch.run_stochastic_trials).  ref is the reference benchmark's noisy_dyn trial shape (N 1024, M 1024,
@@ -39,6 +39,14 @@ episodes on the same inputs: K private TDM pairs of that map and ONE pair shared
 per step while any planner runs).  The parity check holds the histories, steps, statuses (and records), every
 planner's state and the shared pair against the longest-running planner's private pair, byte for byte; then rounds of
 the two legs alternate.  The JSON line adds the device bytes of each leg's TDM allocations, computed from the shapes.
+--episodes E (c2, c3, ref; with or without --share-tdms): the reference benchmark's loop over trials_per_env = E
+ground-truth realisations on the same planners (run_episodes below).  Each planner gets E seeded grids.  The parity check
+runs run_trial_sequences (no reset: the benchmark's loop) and replays the host sequence loop with the device's trajectory
+on twins, each on a private TDM pair: u[0] of every solve and every planner's final state bit for bit (with
+--share-tdms, the shared pair against the private pair of the planner that ran the most steps).  Then rounds of three
+legs, all with params['x0'] set back to the start before each episode: "sequence", one run_trial_sequences(...,
+reset_x0=True) call; "calls", E run_trials calls, each running until its slowest planner stops (without --share-tdms
+its histories must equal the sequence's, bit for bit, or the run fails); "host", the host loop over the E episodes.
 """
 import argparse
 import functools
@@ -299,6 +307,172 @@ def run_shared(args, emit):
                      "shared": sha, "speedup_wall": pri["s_per_round_wall"] / sha["s_per_round_wall"]}))
 
 
+def run_episodes(args, emit):
+    """--episodes E: E episodes per planner back to back, as the reference benchmark's run_trials loops over its
+    ground-truth realisations."""
+    import torch
+    import __graft_entry__
+    __graft_entry__.build_engine()
+    import mppi_numba_b200 as E
+    from bench_batch import gpu_info, pair_state, planner_state, same, shared_map_planners
+    from tests.scenarios import make_scenario
+    from tests.trial_loop import plant_step, within
+    K, S, n_ep = args.batch, args.closed_loop, args.episodes
+    mode, N, M, T, H, res, B, da = LOCAL_WORKLOADS.get(args.workload) or WORKLOADS[args.workload]
+    stochastic = mode == "tdm"
+    Batch = E.MPPI_StochasticBatch if stochastic else E.MPPI_Batch
+    trials = ((lambda b, g, s: b.run_stochastic_trials(g, s)) if stochastic else (lambda b, g, s: b.run_trials(g, s)))
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    scs = []
+    for k in range(K):
+        sc = make_scenario(mode, N=N, M=M, T=T, H=H, W=H, res=res, B=B, seed=k + 1, det_alpha=da, warm_start=True)
+        if k % 2 == 0:
+            sc["params"]["xgoal"] = sc["params"]["x0"][:2] + np.array([1.2, -0.9])
+        scs.append(sc)
+    rng = np.random.default_rng(7)
+    seqs = [[E.TractionGrid(rng.uniform(0.3, 1.0, (H, H)), rng.uniform(0.3, 1.0, (H, H)), res=res) for _ in range(n_ep)]
+            for _ in range(K)]
+    alphas = BENCH_ALPHAS if args.share_tdms and args.workload == "ref" else None
+    with _quiet():
+        if args.share_tdms:                              # device and host legs on one shared pair, twins on private pairs
+            A, Hs, Cs = (shared_map_planners(E, scs, True, alphas) for _ in range(3))
+            Bs = shared_map_planners(E, scs, False, alphas)
+        else:
+            A, Hs, Bs, Cs = ([make_planner(E, sc, 0)[3] for sc in scs] for _ in range(4))
+
+    def reset(pls):
+        for p, sc in zip(pls, scs):
+            p.params["x0"] = sc["params"]["x0"].copy()
+            p.u_cur_d.copy_to_device(sc["u0"])
+
+    for pls in (A, Hs, Bs, Cs):
+        reset(pls)
+    ba, bh, bc = (Batch(pls, share_tdms=args.share_tdms) for pls in (A, Hs, Cs))
+
+    # ---- parity: the benchmark's loop on the device == the host sequence loop replayed with its trajectory
+    with _quiet():
+        out = ba.run_trial_sequences(seqs, S)
+        ok_u = True
+        for k, p in enumerate(Bs):
+            one = Batch([p])
+            for e in range(int(out["episodes_run"][k])):
+                for t in range(int(out["steps"][k, e])):
+                    useq = one.solve()[0]
+                    ok_u &= bool(np.array_equal(useq[0], out["uhist"][k, e, t]))
+                    p.shift_and_update(out["xhist"][k, e, t + 1], useq, 1)
+    ok_state = all(same(planner_state(a, stochastic) + [a.params["x0"]], planner_state(b, stochastic) + [b.params["x0"]])
+                   for a, b in zip(A, Bs))
+    longest = int(np.argmax(out["steps"].sum(axis=1)))
+    ok_pair = all(same(pair_state(a), pair_state(Bs[longest] if args.share_tdms else b)) for a, b in zip(A, Bs))
+    parity = {"passed": bool(ok_u and ok_state and ok_pair), "u_bitwise": ok_u, "state_bitwise": ok_state,
+              "tdm_pairs_bitwise": ok_pair, "planners": K, "episodes_run": out["episodes_run"].tolist(),
+              "steps": out["steps"].tolist(),
+              "against": "the host sequence loop replayed with the device's trajectory on identical twins (private "
+                         "TDM pairs)"}
+    if not parity["passed"]:
+        sys.stderr.write("bench_trials.py: PARITY CHECK FAILED: %s\n" % json.dumps(parity))
+        emit(json.dumps({"metric": "trial sequences", "error": "parity_check failed", "parity_check": parity}))
+        raise SystemExit(3)
+
+    keys = ("xhist", "uhist", "steps")
+    last = {}
+
+    def sequence_round(b=ba, pls=A):
+        reset(pls)
+        o = b.run_trial_sequences(seqs, S, reset_x0=True)
+        torch.cuda.synchronize(dev)
+        last["sequence"] = o
+        return int(o["steps"].sum()), b.steps_issued
+
+    def calls_round(b=ba, pls=A):
+        reset(pls)
+        outs, issued = [], 0
+        starts = [sc["params"]["x0"] for sc in scs]
+        for e in range(n_ep):
+            for p, x in zip(pls, starts):
+                p.params["x0"] = x.copy()
+            outs.append(trials(b, [seqs[k][e] for k in range(K)], S))
+            issued += b.steps_issued
+        torch.cuda.synchronize(dev)
+        last["calls"] = {key: np.stack([o[key] for o in outs], axis=1) for key in keys}
+        return int(sum(o["steps"].sum() for o in outs)), issued
+
+    # the reset_x0 sequence against the consecutive calls, from the same planner state (the rounds below do not restore
+    # RNG streams): a shared pair is sampled at every step any member runs, so the calls (each until its slowest member
+    # stops) sample it more often than the sequence, and only private pairs give the calls' histories
+    with _quiet():
+        sequence_round(bh, Hs)
+        calls_round(bc, Cs)
+    same_hist = all(last["sequence"][key].tobytes() == last["calls"][key].tobytes() for key in keys)
+    if not same_hist and not args.share_tdms:
+        sys.stderr.write("bench_trials.py: the reset_x0 sequence differs from consecutive run_trials calls\n")
+        emit(json.dumps({"metric": "trial sequences", "error": "sequence != consecutive run_trials calls"}))
+        raise SystemExit(3)
+
+    def host_round():
+        reset(Hs)
+        steps = issued = 0
+        starts = [np.asarray(sc["params"]["x0"], dtype=np.float64) for sc in scs]
+        for e in range(n_ep):
+            x = [s.copy() for s in starts]
+            for p, s in zip(Hs, starts):
+                p.params["x0"] = s.copy()
+            running = list(range(K))
+            for t in range(S):
+                u = bh.solve()
+                issued += 1
+                still = []
+                for k in running:
+                    p = Hs[k]
+                    xn = plant_step(seqs[k][e], x[k], u[k, 0], float(p.params["dt"]))
+                    p.shift_and_update(xn, u[k], 1)
+                    x[k] = xn
+                    steps += 1
+                    d = np.linalg.norm(xn[:2] - p.params["xgoal"]) - p.params["goal_tolerance"]
+                    if d > 0 and within(p, xn):
+                        still.append(k)
+                running = still
+                if not running:
+                    break
+        torch.cuda.synchronize(dev)
+        return steps, issued
+
+    legs = [("sequence", sequence_round, ba), ("calls", calls_round, ba), ("host", host_round, bh)]
+    with _quiet():
+        for _, fn, _ in legs:                            # warm-up of every path
+            fn()
+    res_ = {name: [] for name, _, _ in legs}
+    launches = {}
+    for _ in range(args.rounds):                         # alternate: sequence, calls, host, ...
+        for name, fn, b in legs:
+            l0 = b.launch_count()
+            t0 = time.perf_counter()
+            with _quiet():
+                steps, issued = fn()
+            res_[name].append((time.perf_counter() - t0, steps, issued))
+            launches[name] = b.launch_count() - l0
+
+    def summary(name):
+        wall = [r[0] for r in res_[name]]
+        med = float(np.median(wall))
+        return {"s_per_round_wall": med, "s_per_round_wall_runs": wall, "control_steps_per_round": res_[name][0][1],
+                "steps_issued_per_round": res_[name][0][2], "episodes_per_s": K * n_ep / med,
+                "kernel_launches_per_round": launches[name]}
+    seq, calls, host = summary("sequence"), summary("calls"), summary("host")
+    config = {"workload": (args.workload if args.workload in LOCAL_WORKLOADS else workload_name_of(args.workload)),
+              "batch": K, "max_steps": S, "episodes": n_ep, "share_tdms": bool(args.share_tdms),
+              "planners": "seeds 1..K, warm started; even k: goal 1.5 m away, odd k: distant goal; E seeded grids each"
+                          + ("; one shared TDM pair, cvar_alpha cycling %s" % alphas if args.share_tdms and alphas
+                             else "; one shared TDM pair" if args.share_tdms else "")}
+    emit(json.dumps({"metric": "trial sequences: one run_trial_sequences call vs E run_trials calls vs the host loop",
+                     "unit": "episodes/s", "value": seq["episodes_per_s"], "higher_is_better": True, "config": config,
+                     "rounds": args.rounds, "gpu": gpu_info(dev), "parity_check": parity,
+                     "sequence_equals_calls_bitwise": bool(same_hist), "sequence": seq, "calls": calls, "host": host,
+                     "speedup_wall_vs_calls": calls["s_per_round_wall"] / seq["s_per_round_wall"],
+                     "speedup_wall_vs_host": host["s_per_round_wall"] / seq["s_per_round_wall"]}))
+
+
 def _quiet():
     import contextlib
     import io
@@ -494,6 +668,8 @@ def main():
                     help="record the visualisation rollouts of every n-th step (not bb)")
     ap.add_argument("--share-tdms", action="store_true",
                     help="K planners on one map: K private TDM pairs against one pair shared by all (not bb)")
+    ap.add_argument("--episodes", type=int, default=None, metavar="E",
+                    help="E ground-truth realisations per planner back to back (c2, c3, ref)")
     args = ap.parse_args()
     if args.batch < 1 or args.closed_loop < 1 or args.rounds < 1:
         ap.error("--batch, --closed-loop and --rounds must be at least 1")
@@ -501,6 +677,11 @@ def main():
         ap.error("--record-every must be at least 1, and the bb workload does not take it")
     if args.share_tdms and args.workload in ("bb", "mix"):
         ap.error("--share-tdms: barebone planners have no TDMs, and mix planners no common map")
+    if args.episodes is not None:
+        if args.episodes < 1 or args.workload not in ("c2", "c3", "ref") or args.record_every is not None:
+            ap.error("--episodes must be at least 1, with workload c2, c3 or ref and without --record-every")
+        run_episodes(args, emit)
+        return
     (run_bb if args.workload == "bb" else run_shared if args.share_tdms else run)(args, emit)
 
 

@@ -423,7 +423,8 @@ int b200mppi_batch_get_state_rollout(b200mppi_batch* b, float* out, size_t bytes
  *   trials  : count descriptors, in planner order; the grids are uploaded and freed by the call.
  *   xhist   : float64 (count, max_steps+1, 3), NaN after a planner's last step;  uhist: float32 (count, max_steps, 2),
  *             NaN after it;  results: count records;  steps_issued (may be NULL): steps the batch issued. */
-enum { B200MPPI_TRIAL_GOAL = 1, B200MPPI_TRIAL_MAX_STEPS = 2, B200MPPI_TRIAL_LEFT_MAP = 3 };
+enum { B200MPPI_TRIAL_GOAL = 1, B200MPPI_TRIAL_MAX_STEPS = 2, B200MPPI_TRIAL_LEFT_MAP = 3,
+       B200MPPI_TRIAL_NOT_RUN = 4 /* an episode of a trial sequence that never started */ };
 typedef struct {
   const double* lin;            /* ground-truth linear traction, (height, width) row-major, host */
   const double* ang;            /* ground-truth angular traction, same shape */
@@ -512,6 +513,34 @@ int b200mppi_batch_run_trials_recorded(b200mppi_batch* b, int32_t kind, const b2
                                        int32_t max_steps, double* xhist, float* uhist, b200mppi_trial_result* results,
                                        int32_t* contact_steps, int32_t record_every, float* rollouts,
                                        size_t rollout_bytes, int32_t* steps_issued);
+
+/* ------------------------------------------------------------------ trial sequences
+ * Several episodes per planner, back to back on the same planners with no reset in between, as the reference benchmark
+ * runs trials_per_env ground-truth realisations after one setup().  Planner k runs episodes[k] episodes; episode e uses
+ * descriptor trials[first[k] + e], first[k] = episodes[0] + ... + episodes[k-1] (planner-major slots).  Each episode is
+ * one episode of b200mppi_batch_run_trials (kind B200MPPI_TRIALS_MAP) or b200mppi_batch_run_stochastic_trials (kind
+ * B200MPPI_TRIALS_STOCHASTIC) on its descriptor: its plant starts at the descriptor's x0, with its grid, goal, dt, stop
+ * rules and metrics.  Between episodes the planner keeps u_cur, its RNG streams and its TDMs' streams and maps.
+ *   reset_x0 = 0: the benchmark's loop.  The first solve of an episode e > 0 plans from the final pose of episode e-1
+ *                 (the planner's params x0 is never reset there).  An episode that ends LEFT_MAP ends the sequence (the
+ *                 next solve would be refused); its later episodes are B200MPPI_TRIAL_NOT_RUN.
+ *   reset_x0 = 1: the first solve of every episode plans from float32 of the episode's x0, as after set_params with
+ *                 x0 = start before each episode; every episode runs.
+ * The step loop is that of b200mppi_batch_run_trials: the same launches per step, up to max_k episodes[k] * max_steps
+ * steps, stopped once every planner's sequence has ended.  An episode boundary costs no launch and no host round trip.
+ * Afterwards every planner, its TDMs and its params are as after that host loop of all its run episodes: the reach
+ * slots, sample box and the samplings of shared pairs follow its total steps, and the C-side params keep the x0 of the
+ * last solve.
+ *   kind        : B200MPPI_TRIALS_MAP or B200MPPI_TRIALS_STOCHASTIC, for the batches those calls take.
+ *   trials      : sum_k episodes[k] descriptors, the grids uploaded and freed by the call.  episodes: int32 (count).
+ *   xhist       : float64 (slots, max_steps+1, 3); uhist: float32 (slots, max_steps, 2); results: slots records; NaN
+ *                 after an episode's last step and in every row of an episode that never ran, whose record has steps 0
+ *                 and status B200MPPI_TRIAL_NOT_RUN.  steps_issued (may be NULL): steps the batch issued.
+ * Refused (B200MPPI_EINVAL naming the planner and episode) before any work is issued: what the call of that kind
+ * refuses (for every descriptor), another kind, a NULL episodes, an episode count < 1. */
+int b200mppi_batch_run_trial_sequences(b200mppi_batch* b, int32_t kind, const b200mppi_trial_desc* trials,
+                                       const int32_t* episodes, int32_t max_steps, int32_t reset_x0, double* xhist,
+                                       float* uhist, b200mppi_trial_result* results, int32_t* steps_issued);
 
 #ifdef __cplusplus
 }

@@ -55,7 +55,7 @@ class TrialResult(C.Structure):
                 ("steps", C.c_int32), ("status", C.c_int32)]
 
 
-TRIAL_GOAL, TRIAL_MAX_STEPS, TRIAL_LEFT_MAP = 1, 2, 3
+TRIAL_GOAL, TRIAL_MAX_STEPS, TRIAL_LEFT_MAP, TRIAL_NOT_RUN = 1, 2, 3, 4
 TRIALS_MAP, TRIALS_STOCHASTIC, TRIALS_BAREBONE = 0, 1, 2
 
 
@@ -140,6 +140,8 @@ def _load():
         "b200mppi_batch_get_state_rollout": (C.c_int, [P, P, SZ]),
         "b200mppi_batch_run_trials_recorded": (C.c_int, [P, I32, C.POINTER(TrialDesc), I32, P, P,
                                                          C.POINTER(TrialResult), P, I32, P, SZ, C.POINTER(I32)]),
+        "b200mppi_batch_run_trial_sequences": (C.c_int, [P, I32, C.POINTER(TrialDesc), P, I32, I32, P, P,
+                                                         C.POINTER(TrialResult), C.POINTER(I32)]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)          # AttributeError here == ABI drift, fail loudly

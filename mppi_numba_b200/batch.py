@@ -21,6 +21,9 @@ without a host round trip per step (include/b200mppi.h, closed-loop trials); ``M
 run_stochastic_trials`` does the same for use_tdm planners.  ``run_barebone_trials(max_steps)`` runs the barebone
 notebook's closed loop (nominal unicycle, no map) for barebone planners and counts the steps that end in an obstacle.
 
+``run_trial_sequences(traction_grids, max_steps)`` runs several such episodes per planner back to back, on the same
+planners and without a reset in between, as the reference benchmark runs its trials per environment.
+
 ``get_state_rollout()`` is every planner's get_state_rollout() with one launch, and ``record_every=n`` on any trial call
 records those rollouts at every n-th step inside the episodes, as the notebooks' drawing loop calls it.
 
@@ -35,7 +38,8 @@ import numpy as np
 from . import _lib
 from ._lib import check, lib, ptr
 
-TRIAL_STATUS = {_lib.TRIAL_GOAL: "goal", _lib.TRIAL_MAX_STEPS: "max_steps", _lib.TRIAL_LEFT_MAP: "left_map"}
+TRIAL_STATUS = {_lib.TRIAL_GOAL: "goal", _lib.TRIAL_MAX_STEPS: "max_steps", _lib.TRIAL_LEFT_MAP: "left_map",
+                _lib.TRIAL_NOT_RUN: "not_run"}
 
 
 def _kind(p):
@@ -272,37 +276,7 @@ class MPPI_Batch(object):
                 raise ValueError("%s: planner %d cannot solve (reason printed above)" % (name, i))
             if int(p.params["num_opt"]) < 1:
                 raise ValueError("%s: planner %d has num_opt %d < 1" % (name, i, int(p.params["num_opt"])))
-            d, q = descs[i], p.params
-            if barebone:
-                d.x0[:] = [float(v) for v in np.asarray(q["x0"], dtype=np.float64)[:3]]
-                d.xgoal[:] = [float(v) for v in np.asarray(q["xgoal"], dtype=np.float64)[:2]]
-                d.goal_tolerance = float(q["goal_tolerance"])
-                d.dt = float(q["dt"] if dt is None else dt)
-                if not np.isfinite(list(d.x0) + list(d.xgoal) + [d.goal_tolerance]).all():
-                    raise ValueError("%s: planner %d: start pose, goal or goal_tolerance not finite" % (name, i))
-                if not (np.isfinite(d.dt) and d.dt > 0):
-                    raise ValueError("%s: planner %d: dt %r not finite and positive" % (name, i, d.dt))
-                continue
-            lin, ang = np.asarray(g.lin_traction), np.asarray(g.ang_traction)
-            for a in (lin, ang):
-                if a.dtype != np.float64 and not np.issubdtype(a.dtype, np.integer):
-                    raise ValueError("%s: planner %d: traction grid of dtype %s (float64 or integer "
-                                     "grids only: the plant step is float64)" % (name, i, a.dtype))
-            if lin.ndim != 2 or lin.shape != ang.shape:
-                raise ValueError("%s: planner %d: lin / ang traction grids of shapes %s / %s"
-                                 % (name, i, lin.shape, ang.shape))
-            lin = np.ascontiguousarray(lin, dtype=np.float64)
-            ang = np.ascontiguousarray(ang, dtype=np.float64)
-            keep += [lin, ang]
-            d.lin, d.ang = lin.ctypes.data, ang.ctypes.data
-            d.height, d.width = lin.shape
-            d.xlo, d.ylo, d.res = float(g.xlimits[0]), float(g.ylimits[0]), float(g.res)
-            d.x0[:] = [float(v) for v in np.asarray(q["x0"], dtype=np.float64)[:3]]
-            d.xgoal[:] = [float(v) for v in np.asarray(q["xgoal"], dtype=np.float64)[:2]]
-            d.goal_tolerance, d.v_post_rollout = float(q["goal_tolerance"]), float(q["v_post_rollout"])
-            d.dt = float(q["dt"] if dt is None else dt)
-            d.pxlim[:] = [float(v) for v in p.lin_tdm.padded_xlimits]
-            d.pylim[:] = [float(v) for v in p.lin_tdm.padded_ylimits]
+            _fill_desc("%s: planner %d" % (name, i), p, g, dt, descs[i], keep)
         for p in self.planners:
             p.move_mppi_task_vars_to_device()
         xhist = np.empty((K, max_steps + 1, 3), dtype=np.float64)
@@ -327,18 +301,9 @@ class MPPI_Batch(object):
             if self.kind != "tdm":
                 p.u_prev_d = p._u_prev_buf             # as each planner's own solve() does (mppi.py:292,362)
             p.params["x0"] = xhist[i, steps[i]].copy()  # shift_and_update(x_next, ...)
-            r, n, reached = res[i], int(steps[i]), status[i] == "goal"
-            cum_obj, dist = r.cum_obj, r.dist_to_goal
-            if reached:
-                dist = np.nan
-            elif not barebone:
-                cum_obj += dist / descs[i].v_post_rollout
-            log = dict(time_to_goal=n * descs[i].dt if reached else np.nan, success=reached, dist_to_goal=dist,
-                       cum_dist_to_goal=r.cum_dist_to_goal, avg_dist_to_goal=r.cum_dist_to_goal / n)
+            log = _trial_log(res[i], descs[i], barebone)
             if barebone:
                 log["contact_steps"] = int(contacts[i])
-            else:
-                log["cum_obj"] = cum_obj
             logs.append(log)
         out = dict(logs=logs, xhist=xhist, uhist=uhist, steps=steps, status=status)
         if barebone:
@@ -347,6 +312,138 @@ class MPPI_Batch(object):
             out["state_rollouts"] = rollouts
             out["rollout_steps"] = np.arange(R, dtype=np.int64) * record_every
         return out
+
+
+    def run_trial_sequences(self, traction_grids, max_steps, dt=None, reset_x0=False):
+        """Several closed-loop episodes per planner, back to back on the GPU: planner k runs one episode of
+        ``run_trials`` (``run_stochastic_trials`` for use_tdm planners) on each ``TractionGrid`` of the non-empty list
+        ``traction_grids[k]`` in turn, each starting its plant at ``x_start = params['x0']`` of the call, with the
+        stop rules, ``dt`` and log conventions of run_trials.  Between episodes nothing is reset: the planner keeps its
+        warm start, RNG streams and its TDMs' streams and maps -- the loop the reference benchmark runs over
+        trials_per_env realisations after one setup().
+          ``reset_x0=False`` (the benchmark's loop): ``params['x0']`` is left at the previous episode's final pose, so
+              an episode's first solve plans from there.  An episode ending "left_map" ends the planner's sequence
+              (its next solve would be refused); the later episodes are "not_run".
+          ``reset_x0=True``: ``params['x0'] = x_start`` before every episode, as a user resetting it would; every
+              episode runs.
+        Afterwards every planner is exactly as after that host loop over its run episodes (buffers, RNG streams, its
+        TDMs' streams and sampled maps, ``sample_box()``), ``params['x0']`` the final pose of its last run episode.  With
+        share_tdms a shared pair ends as the copy of the member that ran the most steps in all.  Episodes cost no extra
+        launch: the batch runs until every planner's sequence has ended.
+        Returns a dict: ``logs``, K lists of E_k trial logs (None for an episode that did not run); ``xhist`` float64
+        (K, Emax, max_steps+1, 3) and ``uhist`` float32 (K, Emax, max_steps, 2), NaN wherever nothing ran; ``steps``
+        (K, Emax) int, 0 where nothing ran; ``status``, K lists of E_k of "goal" | "max_steps" | "left_map" |
+        "not_run"; ``episodes_run`` (K,) int.  ``steps_issued`` is set as run_trials sets it.
+        Raises ValueError for barebone batches, a list count other than K, an empty list, and whatever run_trials
+        refuses for any of the grids; nothing is issued then."""
+        name = "%s.run_trial_sequences" % type(self).__name__
+        if self.kind == "barebone":
+            raise ValueError("%s: planner 0 is a barebone planner (trial sequences run det-dynamics, speed-map and "
+                             "use_tdm planners)" % name)
+        K = len(self.planners)
+        seqs = [list(g) for g in traction_grids]
+        if len(seqs) != K:
+            raise ValueError("%s: %d lists of traction grids for %d planners" % (name, len(seqs), K))
+        for i, g in enumerate(seqs):
+            if not g:
+                raise ValueError("%s: planner %d: empty list of traction grids" % (name, i))
+        max_steps = int(max_steps)
+        if max_steps < 1:
+            raise ValueError("%s: max_steps %d < 1" % (name, max_steps))
+        self._check_groups(name)
+        E = np.array([len(g) for g in seqs], dtype=np.int32)
+        first = np.concatenate([[0], np.cumsum(E)])
+        descs = (_lib.TrialDesc * int(first[-1]))()
+        keep = []
+        for i, p in enumerate(self.planners):
+            if not p.check_solve_conditions():
+                raise ValueError("%s: planner %d cannot solve (reason printed above)" % (name, i))
+            if int(p.params["num_opt"]) < 1:
+                raise ValueError("%s: planner %d has num_opt %d < 1" % (name, i, int(p.params["num_opt"])))
+            for e, g in enumerate(seqs[i]):
+                _fill_desc("%s: planner %d, episode %d" % (name, i, e), p, g, dt, descs[first[i] + e], keep)
+        for p in self.planners:
+            p.move_mppi_task_vars_to_device()
+        slots = int(first[-1])
+        xs = np.empty((slots, max_steps + 1, 3), dtype=np.float64)
+        us = np.empty((slots, max_steps, 2), dtype=np.float32)
+        res = (_lib.TrialResult * slots)()
+        issued = C.c_int32()
+        kind = _lib.TRIALS_STOCHASTIC if self.kind == "tdm" else _lib.TRIALS_MAP
+        check(lib.b200mppi_batch_run_trial_sequences(self._handle, kind, descs, ptr(E), max_steps, int(bool(reset_x0)),
+                                                     ptr(xs), ptr(us), res, C.byref(issued)))
+        self.steps_issued = int(issued.value)
+        Emax = int(E.max())
+        xhist = np.full((K, Emax, max_steps + 1, 3), np.nan)
+        uhist = np.full((K, Emax, max_steps, 2), np.nan, dtype=np.float32)
+        steps = np.zeros((K, Emax), dtype=np.int64)
+        episodes_run = np.zeros(K, dtype=np.int64)
+        logs, status = [], []
+        for i, p in enumerate(self.planners):
+            n = int(E[i])
+            xhist[i, :n], uhist[i, :n] = xs[first[i]:first[i] + n], us[first[i]:first[i] + n]
+            st = [TRIAL_STATUS[res[j].status] for j in range(first[i], first[i] + n)]
+            run = sum(s != "not_run" for s in st)
+            steps[i, :run] = [res[j].steps for j in range(first[i], first[i] + run)]
+            logs.append([_trial_log(res[first[i] + e], descs[first[i] + e], False) if e < run else None
+                         for e in range(n)])
+            status.append(st)
+            episodes_run[i] = run
+            if self.kind != "tdm":
+                p.u_prev_d = p._u_prev_buf             # as each planner's own solve() does (mppi.py:292,362)
+            p.params["x0"] = xhist[i, run - 1, steps[i, run - 1]].copy()
+        return dict(logs=logs, xhist=xhist, uhist=uhist, steps=steps, status=status, episodes_run=episodes_run)
+
+
+def _fill_desc(who, p, g, dt, d, keep):
+    """Trial descriptor ``d`` of planner ``p`` on TractionGrid ``g`` (None: barebone), starting at params['x0']; the
+    float64 grids it points to are appended to ``keep``.  ``who`` prefixes the refusals."""
+    q = p.params
+    if g is None:
+        d.x0[:] = [float(v) for v in np.asarray(q["x0"], dtype=np.float64)[:3]]
+        d.xgoal[:] = [float(v) for v in np.asarray(q["xgoal"], dtype=np.float64)[:2]]
+        d.goal_tolerance = float(q["goal_tolerance"])
+        d.dt = float(q["dt"] if dt is None else dt)
+        if not np.isfinite(list(d.x0) + list(d.xgoal) + [d.goal_tolerance]).all():
+            raise ValueError("%s: start pose, goal or goal_tolerance not finite" % who)
+        if not (np.isfinite(d.dt) and d.dt > 0):
+            raise ValueError("%s: dt %r not finite and positive" % (who, d.dt))
+        return
+    lin, ang = np.asarray(g.lin_traction), np.asarray(g.ang_traction)
+    for a in (lin, ang):
+        if a.dtype != np.float64 and not np.issubdtype(a.dtype, np.integer):
+            raise ValueError("%s: traction grid of dtype %s (float64 or integer grids only: the plant step is "
+                             "float64)" % (who, a.dtype))
+    if lin.ndim != 2 or lin.shape != ang.shape:
+        raise ValueError("%s: lin / ang traction grids of shapes %s / %s" % (who, lin.shape, ang.shape))
+    lin = np.ascontiguousarray(lin, dtype=np.float64)
+    ang = np.ascontiguousarray(ang, dtype=np.float64)
+    keep += [lin, ang]
+    d.lin, d.ang = lin.ctypes.data, ang.ctypes.data
+    d.height, d.width = lin.shape
+    d.xlo, d.ylo, d.res = float(g.xlimits[0]), float(g.ylimits[0]), float(g.res)
+    d.x0[:] = [float(v) for v in np.asarray(q["x0"], dtype=np.float64)[:3]]
+    d.xgoal[:] = [float(v) for v in np.asarray(q["xgoal"], dtype=np.float64)[:2]]
+    d.goal_tolerance, d.v_post_rollout = float(q["goal_tolerance"]), float(q["v_post_rollout"])
+    d.dt = float(q["dt"] if dt is None else dt)
+    d.pxlim[:] = [float(v) for v in p.lin_tdm.padded_xlimits]
+    d.pylim[:] = [float(v) for v in p.lin_tdm.padded_ylimits]
+
+
+def _trial_log(r, d, barebone):
+    """The trial log of trial() from result record ``r`` of descriptor ``d``: a planner that did not reach its goal
+    adds the d / v_post_rollout tail to cum_obj and has no time to goal (barebone logs have no cum_obj)."""
+    n, reached = int(r.steps), r.status == _lib.TRIAL_GOAL
+    cum_obj, dist = r.cum_obj, r.dist_to_goal
+    if reached:
+        dist = np.nan
+    elif not barebone:
+        cum_obj += dist / d.v_post_rollout
+    log = dict(time_to_goal=n * d.dt if reached else np.nan, success=reached, dist_to_goal=dist,
+               cum_dist_to_goal=r.cum_dist_to_goal, avg_dist_to_goal=r.cum_dist_to_goal / n)
+    if not barebone:
+        log["cum_obj"] = cum_obj
+    return log
 
 
 class MPPI_StochasticBatch(MPPI_Batch):

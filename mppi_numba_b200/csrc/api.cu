@@ -2499,9 +2499,9 @@ constexpr int TRIAL_POLL = 4;
 // one-map (MODE_DET_DYN, MODE_SPEED_MAP), stochastic (MODE_TDM) and barebone (MODE_BAREBONE, no map) trials
 enum class TrialKind { onemap, stochastic, barebone };
 
+// first: planner i's descriptors are tr[first[i] .. first[i + 1]): one each, or (seq) its episodes in a trial sequence
 static int trial_validate(b200mppi_batch* b, TrialKind kind, const b200mppi_trial_desc* tr, int32_t max_steps,
-                          const char* fn) {
-  const int K = (int)b->pl.size();
+                          const char* fn, const std::vector<int>& first, bool seq) {
   if (!tr) return fail(B200MPPI_EINVAL, std::string(fn) + ": null trial descriptors");
   if (max_steps < 1) return fail(B200MPPI_EINVAL, std::string(fn) + ": max_steps < 1");
   if (kind != TrialKind::barebone && b->mode == B200MPPI_MODE_BAREBONE)
@@ -2509,9 +2509,11 @@ static int trial_validate(b200mppi_batch* b, TrialKind kind, const b200mppi_tria
                                  "MODE_SPEED_MAP batches)");
   int rc = batch_validate(b);
   if (rc) return rc;
-  for (int i = 0; i < K; ++i) {
-    const std::string who = std::string(fn) + ": planner " + std::to_string(i);
-    const b200mppi_trial_desc& d = tr[i];
+  for (int j = 0; j < first.back(); ++j) {
+    const int i = (int)(std::upper_bound(first.begin(), first.end(), j) - first.begin()) - 1;
+    const std::string who = std::string(fn) + ": planner " + std::to_string(i) +
+                            (seq ? ", episode " + std::to_string(j - first[i]) : std::string());
+    const b200mppi_trial_desc& d = tr[j];
     if (b->pl[i]->prm.num_opt < 1) return fail(B200MPPI_EINVAL, who + " has num_opt < 1");
     if (kind == TrialKind::barebone) {
       if (d.lin || d.ang)
@@ -2699,12 +2701,32 @@ static const char* mode_name(int mode) {
 // xhist and uhist: the float64 ground-truth grids (tens of MB for a batch of large maps) are copied straight from the
 // caller's arrays, and the written records (of K * R * V * (T+1) * 12 bytes, 145 MB for K 8, 150 steps, V 100, T 100)
 // straight into the caller's array.
+// Trial sequences (episodes non-null, b200mppi_batch_run_trial_sequences): planner i runs episodes[i] episodes back to
+// back, descriptors, histories and results per slot (planner-major: planner i's are slots first[i] .. first[i + 1]),
+// through the same step loop for up to max_i episodes[i] * max_steps steps; the plant step (plant_step_seq_kernel)
+// moves a planner to its next episode without a launch, and the commit below follows each planner's total steps.
 static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_trial_desc* trials, int32_t max_steps,
                             double* xhist, float* uhist, b200mppi_trial_result* results, int32_t* contact_steps,
-                            int32_t record_every, float* rollouts, size_t rollout_bytes, int32_t* steps_issued) {
+                            int32_t record_every, float* rollouts, size_t rollout_bytes, int32_t* steps_issued,
+                            const int32_t* episodes, int32_t reset_x0) {
   const bool stochastic = kind == TrialKind::stochastic, barebone = kind == TrialKind::barebone;
-  const std::string fn = stochastic ? "run_stochastic_trials" : barebone ? "run_barebone_trials" : "run_trials";
+  const bool seq = episodes != nullptr;
+  const std::string fn = seq ? "run_trial_sequences" : stochastic ? "run_stochastic_trials"
+                         : barebone ? "run_barebone_trials" : "run_trials";
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  std::vector<int> first(b->pl.size() + 1, 0);        // planner i's slots: first[i] .. first[i + 1]
+  int max_episodes = 1;
+  for (size_t i = 0; i < b->pl.size(); ++i) {
+    const int E = seq ? episodes[i] : 1;
+    if (E < 1)
+      return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(i) + ": episode count " + std::to_string(E) + " < 1");
+    if ((int64_t)first[i] + E > (1 << 24))
+      return fail(B200MPPI_EINVAL, fn + ": more than 2^24 episodes in all");
+    first[i + 1] = first[i] + E;
+    max_episodes = std::max(max_episodes, E);
+  }
+  if ((int64_t)max_episodes * max_steps > INT32_MAX)
+    return fail(B200MPPI_EINVAL, fn + ": max_steps x the largest episode count exceeds 2^31 - 1 steps");
   if (barebone && b->mode != B200MPPI_MODE_BAREBONE)
     return fail(B200MPPI_EINVAL, fn + ": planner 0 is " + mode_name(b->mode) + " (barebone trials run MODE_BAREBONE "
                                  "batches; b200mppi_batch_run_trials and b200mppi_batch_run_stochastic_trials run the "
@@ -2715,11 +2737,11 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   if (!b->stochastic && stochastic)
     return fail(B200MPPI_EINVAL, fn + ": planner 0 is " + mode_name(b->mode) +
                                      " (stochastic trials run MODE_TDM batches; b200mppi_batch_run_trials runs the others)");
-  int rc = trial_validate(b, kind, trials, max_steps, fn.c_str());
+  int rc = trial_validate(b, kind, trials, max_steps, fn.c_str(), first, seq);
   if (rc) return rc;
   if (!xhist || !uhist || !results || (barebone && !contact_steps))
     return fail(B200MPPI_EINVAL, fn + ": null output buffer");
-  const int K = (int)b->pl.size(), T = b->T, N = b->N, S = max_steps;
+  const int K = (int)b->pl.size(), T = b->T, N = b->N, S = max_steps, nslot = first[K];
   const bool record = record_every > 0;
   int V = 0, R = 0;
   size_t per = 0, rec_bytes = 0;                       // floats of one planner's record, bytes of all records
@@ -2766,20 +2788,24 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   const size_t off_cls = off_mem + align256((grouped ? (size_t)K : 0) * sizeof(int));
   const size_t off_state = off_cls + align256(nset * sizeof(int));
   const size_t off_con = off_state + align256((size_t)K * sizeof(TrialState));
-  const size_t off_tr = off_con + align256(ncon * sizeof(int));
-  const size_t off_act = off_tr + align256((size_t)K * sizeof(TrialDev));
-  const size_t off_vis = off_act + align256((size_t)(K + 1) * sizeof(int));
+  const size_t nres = seq ? (size_t)nslot : 0;          // sequence-only sections: per-slot results and start poses
+  const size_t off_res = off_con + align256(ncon * sizeof(int));
+  const size_t off_tr = off_res + align256(nres * sizeof(TrialState));
+  const size_t off_act = off_tr + align256((size_t)nslot * sizeof(TrialDev));
+  const size_t off_seq = off_act + align256((size_t)(K + 1) * sizeof(int));      // first (K + 1), episode (K)
+  const size_t off_start = off_seq + align256((seq ? (size_t)(2 * K + 1) : 0) * sizeof(int));
+  const size_t off_vis = off_start + align256(nres * 3 * sizeof(double));
   size_t off = off_vis + align256((record ? (size_t)K : 0) * sizeof(VisBatchDesc));
   const size_t head = off;
-  std::vector<size_t> off_grid(K);
-  for (int i = 0; i < K; ++i) {
-    off_grid[i] = off;
-    if (!barebone) off += align256((size_t)2 * trials[i].height * trials[i].width * sizeof(double));
+  std::vector<size_t> off_grid(nslot);
+  for (int j = 0; j < nslot; ++j) {
+    off_grid[j] = off;
+    if (!barebone) off += align256((size_t)2 * trials[j].height * trials[j].width * sizeof(double));
   }
   const size_t off_vrec = off;
   off += align256(rec_bytes);
-  const size_t off_xh = off, off_uh = off_xh + align256((size_t)K * (S + 1) * 3 * sizeof(double));
-  const size_t total = off_uh + align256((size_t)K * S * 2 * sizeof(float));
+  const size_t off_xh = off, off_uh = off_xh + align256((size_t)nslot * (S + 1) * 3 * sizeof(double));
+  const size_t total = off_uh + align256((size_t)nslot * S * 2 * sizeof(float));
   struct Buffers {                                     // freed on every return
     unsigned char* d = nullptr;
     unsigned char* h = nullptr;
@@ -2815,38 +2841,57 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   float* drec = reinterpret_cast<float*>(d + off_vrec);
   for (int i = 0; i < K; ++i) {
     b200mppi_planner* p = b->pl[i];
-    const b200mppi_trial_desc& q = trials[i];
     if (record)                                        // x0 from the record the plant step writes
       hv[i] = vis_desc(p, stochastic ? &dw[i].p : &dr[i].p, drec + (size_t)i * R * per);
-    TrialDev& t = ht[i];
-    t = TrialDev{};
-    t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1]; t.tol = q.goal_tolerance;
-    t.u_cur = p->u_cur;
     hst[i] = TrialState{};
-    for (int c = 0; c < 3; ++c) hst[i].x[c] = q.x0[c];
+    for (int c = 0; c < 3; ++c) hst[i].x[c] = trials[first[i]].x0[c];
     hact[i] = 1;
-    if (barebone) {                                    // lin null: nominal unicycle, no map; contacts counted
-      t.x0_out = dr[i].p.x0;
-      t.obstacles = p->obstacles; t.num_obstacles = p->num_obstacles;
-      hcon[i] = 0;
-      continue;
+    if (barebone) hcon[i] = 0;
+    for (int j = first[i]; j < first[i + 1]; ++j) {    // the planner's episodes: one, or its sequence
+      const b200mppi_trial_desc& q = trials[j];
+      TrialDev& t = ht[j];
+      t = TrialDev{};
+      t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1]; t.tol = q.goal_tolerance;
+      t.u_cur = p->u_cur;
+      if (barebone) {                                  // lin null: nominal unicycle, no map; contacts counted
+        t.x0_out = dr[i].p.x0;
+        t.obstacles = p->obstacles; t.num_obstacles = p->num_obstacles;
+        continue;
+      }
+      const double* dg = reinterpret_cast<const double*>(d + off_grid[j]);
+      t.lin = dg; t.ang = dg + (size_t)q.height * q.width; t.H = q.height; t.W = q.width;
+      t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res;
+      t.pxlim[0] = q.pxlim[0]; t.pxlim[1] = q.pxlim[1]; t.pylim[0] = q.pylim[0]; t.pylim[1] = q.pylim[1];
+      if (!stochastic) {
+        t.x0_out = dr[i].p.x0;                         // win stays null: one-map rollouts have no window
+        continue;
+      }
+      const b200mppi_tdm* l = p->lin;
+      t.x0_out = dw[i].p.x0;
+      t.win = &dw[i].WW;
+      t.win_pxl = l->pxl[0]; t.win_pyl = l->pyl[0]; t.win_res = l->res; t.win_rows = l->rows; t.win_cols = l->cols;
     }
-    const double* dg = reinterpret_cast<const double*>(d + off_grid[i]);
-    t.lin = dg; t.ang = dg + (size_t)q.height * q.width; t.H = q.height; t.W = q.width;
-    t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res;
-    t.pxlim[0] = q.pxlim[0]; t.pxlim[1] = q.pxlim[1]; t.pylim[0] = q.pylim[0]; t.pylim[1] = q.pylim[1];
-    if (!stochastic) {
-      t.x0_out = dr[i].p.x0;                           // win stays null: one-map rollouts have no window
-      continue;
-    }
-    const b200mppi_tdm* l = p->lin;
-    t.x0_out = dw[i].p.x0;
-    t.win = &dw[i].WW;
-    t.win_pxl = l->pxl[0]; t.win_pyl = l->pyl[0]; t.win_res = l->res; t.win_rows = l->rows; t.win_cols = l->cols;
+    if (!stochastic) continue;
     reinterpret_cast<CvarDesc*>(h + b->off_cvar)[i].active = dact + i;
     hb[i] = SampleBoxDesc{{}, dw[i].p.x0, p->reach_d, p->reach_slot ^ 1, reinterpret_cast<int*>(d + off_rec) + 5 * i,
-                          l->jump_tile_d};
+                          p->lin->jump_tile_d};
     fill_reach_const(p, plans[gr.of[i]], &hb[i].c);
+  }
+  TrialState* hres = reinterpret_cast<TrialState*>(h + off_res);
+  SeqArgs sa{};
+  if (seq) {                                           // slots that never run keep NOT_RUN and 0 steps
+    int* hseq = reinterpret_cast<int*>(h + off_seq);
+    double* hstart = reinterpret_cast<double*>(h + off_start);
+    std::copy(first.begin(), first.end(), hseq);
+    std::fill(hseq + K + 1, hseq + 2 * K + 1, 0);
+    for (int j = 0; j < nslot; ++j) {
+      hres[j] = TrialState{};
+      hres[j].status = B200MPPI_TRIAL_NOT_RUN;
+      for (int c = 0; c < 3; ++c) hstart[3 * j + c] = trials[j].x0[c];
+    }
+    int* dseq = reinterpret_cast<int*>(d + off_seq);
+    sa = SeqArgs{dseq, dseq + K + 1, reinterpret_cast<const double*>(d + off_start),
+                 reinterpret_cast<TrialState*>(d + off_res), reset_x0 ? 1 : 0};
   }
   for (int g = 0; g < (int)nset; ++g) {
     // parity 1: the pair samples from the buffers parity 0 wrote into
@@ -2869,10 +2914,10 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   hact[K] = K;
   const RolloutWinArgs g0 = stochastic ? *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win) : RolloutWinArgs{};
   CU(cudaMemcpyAsync(d, h, head, cudaMemcpyHostToDevice, st));
-  for (int i = 0; i < K && !barebone; ++i) {          // pageable sources: staged by the driver before the call returns
-    const size_t bytes = (size_t)trials[i].height * trials[i].width * sizeof(double);
-    CU(cudaMemcpyAsync(d + off_grid[i], trials[i].lin, bytes, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(d + off_grid[i] + bytes, trials[i].ang, bytes, cudaMemcpyHostToDevice, st));
+  for (int j = 0; j < nslot && !barebone; ++j) {      // pageable sources: staged by the driver before the call returns
+    const size_t bytes = (size_t)trials[j].height * trials[j].width * sizeof(double);
+    CU(cudaMemcpyAsync(d + off_grid[j], trials[j].lin, bytes, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d + off_grid[j] + bytes, trials[j].ang, bytes, cudaMemcpyHostToDevice, st));
   }
   const SampleGridsV2Args* ds[2] = {reinterpret_cast<const SampleGridsV2Args*>(d + off_s0),
                                     reinterpret_cast<const SampleGridsV2Args*>(d + off_s1)};
@@ -2886,7 +2931,8 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   for (cudaEvent_t& e : buf.ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   const int num_opt = b->pl[0]->prm.num_opt, npad = b->pl[0]->npad;
   int issued = 0;
-  for (int s = 0; s < S; ++s) {
+  const int last_step = S * max_episodes;
+  for (int s = 0; s < last_step; ++s) {
     if (s >= TRIAL_POLL) {                            // the count after step s - POLL
       CU(cudaEventSynchronize(buf.ev[s % TRIAL_POLL]));
       if (hcount[s % TRIAL_POLL] == 0) break;
@@ -2935,7 +2981,8 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       CHECK_LAUNCH();
     }
     pa.step = s;
-    launch_plant_step(pa, st);
+    if (seq) launch_plant_step_seq(pa, sa, st);
+    else launch_plant_step(pa, st);
     CHECK_LAUNCH();
     b->launches += stochastic ? 4 * num_opt + 1 + 2 * C : 3 * num_opt + 1 + C;
     if (rec_step) b->launches += stochastic ? 1 + C : 1;
@@ -2952,22 +2999,32 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   const float* hu = reinterpret_cast<const float*>(h + head + (off_uh - off_xh));
   const double dnan = std::nan("");
   const float fnan = std::nanf("");
+  std::vector<int> ran(K, 0);                          // steps each planner ran, over all its episodes
   for (int i = 0; i < K; ++i) {
-    const TrialState& r = hst[i];
-    const int n = r.steps;
-    double* xo = xhist + (size_t)i * (S + 1) * 3;
-    float* uo = uhist + (size_t)i * S * 2;
-    for (int c = 0; c < 3; ++c) xo[c] = trials[i].x0[c];
-    std::memcpy(xo + 3, hx + ((size_t)i * (S + 1) + 1) * 3, (size_t)n * 3 * sizeof(double));
-    for (size_t j = (size_t)(n + 1) * 3; j < (size_t)(S + 1) * 3; ++j) xo[j] = dnan;
-    std::memcpy(uo, hu + (size_t)i * S * 2, (size_t)n * 2 * sizeof(float));
-    for (size_t j = (size_t)n * 2; j < (size_t)S * 2; ++j) uo[j] = fnan;
-    results[i] = b200mppi_trial_result{r.cum_obj, r.cum_dist, r.dist, n, r.status};
+    int last = first[i];                               // the planner's last slot that ran
+    for (int j = first[i]; j < first[i + 1]; ++j) {
+      const TrialState& r = seq ? hres[j] : hst[i];
+      const int n = r.steps;                           // 0: an episode of a sequence that never ran
+      double* xo = xhist + (size_t)j * (S + 1) * 3;
+      float* uo = uhist + (size_t)j * S * 2;
+      if (n > 0) {
+        for (int c = 0; c < 3; ++c) xo[c] = trials[j].x0[c];
+        last = j;
+      }
+      std::memcpy(xo + 3, hx + ((size_t)j * (S + 1) + 1) * 3, (size_t)n * 3 * sizeof(double));
+      for (size_t q = (size_t)(n > 0 ? n + 1 : 0) * 3; q < (size_t)(S + 1) * 3; ++q) xo[q] = dnan;
+      std::memcpy(uo, hu + (size_t)j * S * 2, (size_t)n * 2 * sizeof(float));
+      for (size_t q = (size_t)n * 2; q < (size_t)S * 2; ++q) uo[q] = fnan;
+      results[j] = b200mppi_trial_result{r.cum_obj, r.cum_dist, r.dist, n, r.status};
+      ran[i] += n;
+    }
     if (barebone) contact_steps[i] = hcon[i];
-    // host state as after n rounds of the host loop: the reach slot toggled once per iteration, the last solve's box and
-    // x0 (the samplings of the pair below)
+    // host state as after ran[i] rounds of the host loop: the reach slot toggled once per iteration, the last solve's
+    // box and x0 (the samplings of the pair below).  The last solve planned from the pose before the last step -- or,
+    // when a later episode of a sequence without reset_x0 took one step, from the previous episode's final pose
     b200mppi_planner* p = b->pl[i];
     const int* rec = hrec + 5 * i;
+    const int n = ran[i];
     if (stochastic) {
       p->reach_slot ^= (n * num_opt) & 1;
       p->reach_valid = true;
@@ -2977,13 +3034,16 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     }
     p->prepared = false;
     p->pushed_direct = false;
-    for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)xo[(size_t)(n - 1) * 3 + c];
+    const double* x0 = xhist + ((size_t)last * (S + 1) + results[last].steps - 1) * 3;
+    if (results[last].steps == 1 && last > first[i] && !reset_x0)
+      x0 = xhist + ((size_t)(last - 1) * (S + 1) + results[last - 1].steps) * 3;
+    for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)x0[c];
   }
   // each TDM group's pair as after the samplings of its longest-running member (a group samples at every step while any
   // member runs), the last one's kind from the group's record (a group of one: its planner's)
   for (int g = 0; g < G && !barebone; ++g) {
     int n = 0;
-    for (int j = gr.first[g]; j < gr.first[g + 1]; ++j) n = std::max(n, hst[gr.members[j]].steps);
+    for (int j = gr.first[g]; j < gr.first[g + 1]; ++j) n = std::max(n, ran[gr.members[j]]);
     const int* rec = grouped && stochastic ? reinterpret_cast<const int*>(h + off_grec) + 5 * g : hrec + 5 * gr.lead(g);
     if (stochastic) plans[g].boxed[0] = plans[g].boxed[1] = rec[0] != 0;
     for (int s = 0; s < n; ++s) { plan_commit(plans[g], 0); plan_commit(plans[g], 1); }
@@ -3011,14 +3071,14 @@ extern "C" int b200mppi_batch_run_trials(b200mppi_batch* b, const b200mppi_trial
                                          double* xhist, float* uhist, b200mppi_trial_result* results,
                                          int32_t* steps_issued) {
   return batch_run_trials(b, TrialKind::onemap, trials, max_steps, xhist, uhist, results, nullptr, 0, nullptr, 0,
-                          steps_issued);
+                          steps_issued, nullptr, 0);
 }
 
 extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials,
                                                     int32_t max_steps, double* xhist, float* uhist,
                                                     b200mppi_trial_result* results, int32_t* steps_issued) {
   return batch_run_trials(b, TrialKind::stochastic, trials, max_steps, xhist, uhist, results, nullptr, 0, nullptr, 0,
-                          steps_issued);
+                          steps_issued, nullptr, 0);
 }
 
 extern "C" int b200mppi_batch_run_barebone_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials,
@@ -3026,7 +3086,7 @@ extern "C" int b200mppi_batch_run_barebone_trials(b200mppi_batch* b, const b200m
                                                   b200mppi_trial_result* results, int32_t* contact_steps,
                                                   int32_t* steps_issued) {
   return batch_run_trials(b, TrialKind::barebone, trials, max_steps, xhist, uhist, results, contact_steps, 0, nullptr,
-                          0, steps_issued);
+                          0, steps_issued, nullptr, 0);
 }
 
 extern "C" int b200mppi_batch_run_trials_recorded(b200mppi_batch* b, int32_t kind, const b200mppi_trial_desc* trials,
@@ -3042,5 +3102,18 @@ extern "C" int b200mppi_batch_run_trials_recorded(b200mppi_batch* b, int32_t kin
   const TrialKind k = kind == B200MPPI_TRIALS_STOCHASTIC ? TrialKind::stochastic
                       : kind == B200MPPI_TRIALS_BAREBONE ? TrialKind::barebone : TrialKind::onemap;
   return batch_run_trials(b, k, trials, max_steps, xhist, uhist, results, contact_steps, record_every, rollouts,
-                          rollout_bytes, steps_issued);
+                          rollout_bytes, steps_issued, nullptr, 0);
+}
+
+extern "C" int b200mppi_batch_run_trial_sequences(b200mppi_batch* b, int32_t kind, const b200mppi_trial_desc* trials,
+                                                  const int32_t* episodes, int32_t max_steps, int32_t reset_x0,
+                                                  double* xhist, float* uhist, b200mppi_trial_result* results,
+                                                  int32_t* steps_issued) {
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  if (kind != B200MPPI_TRIALS_MAP && kind != B200MPPI_TRIALS_STOCHASTIC)
+    return fail(B200MPPI_EINVAL, "run_trial_sequences: trial kind " + std::to_string(kind) + " (sequences run "
+                                 "B200MPPI_TRIALS_MAP or B200MPPI_TRIALS_STOCHASTIC batches)");
+  if (!episodes) return fail(B200MPPI_EINVAL, "run_trial_sequences: null episode counts");
+  return batch_run_trials(b, kind == B200MPPI_TRIALS_STOCHASTIC ? TrialKind::stochastic : TrialKind::onemap, trials,
+                          max_steps, xhist, uhist, results, nullptr, 0, nullptr, 0, steps_issued, episodes, reset_x0);
 }

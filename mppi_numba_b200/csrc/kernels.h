@@ -564,8 +564,20 @@ struct PlantArgs {
   int K, T, max_steps, step;
   int* contacts;                          // barebone trials: (K) steps whose new pose touches an obstacle; else null
 };
+// Trial sequences (b200mppi_batch_run_trial_sequences): planner k runs the episodes of slots first[k] .. first[k+1]-1
+// back to back.  PlantArgs::trials, xhist and uhist are then per slot, PlantArgs::state per planner (the running
+// episode) and PlantArgs::step unused: an episode's step is its TrialState::steps.
+struct SeqArgs {
+  const int* first;                       // (K + 1) planner k's first slot
+  int* episode;                           // (K) the running episode of planner k, from 0
+  const double* start;                    // (slots, 3) each episode's start pose
+  TrialState* results;                    // (slots) written when the episode stops
+  int reset_x0;                           // 1: an episode's first solve plans from its start pose, and LEFT_MAP does
+                                          // not end the sequence; 0: from the previous episode's final pose
+};
 // [emu:end trial_args]
 void launch_plant_step(const PlantArgs& a, cudaStream_t st);
+void launch_plant_step_seq(const PlantArgs& a, const SeqArgs& q, cudaStream_t st);
 
 // visualisation rollouts (mppi.py:1194-1351)
 // [emu:begin vis_args]

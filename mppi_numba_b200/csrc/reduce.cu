@@ -382,9 +382,16 @@ __device__ __forceinline__ double py_floordiv(double vx, double wx) {
 // record the step, and stop the planner on the goal, on leaving the padded map or after max_steps steps.
 // Barebone trials (TrialDev::lin null) step the notebook's nominal unicycle (traction 1: dt * 1.0 == dt), have no map
 // to leave, and count in contacts[k] the steps whose new pose lies in one of the planner's obstacles.
-__device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int lane) {
+// SEQ (trial sequences, SeqArgs): the planner steps its running episode e, slot first[k] + e of the descriptors and
+// histories.  When that episode stops and another follows (reset_x0, or a stop other than LEFT_MAP), its result is
+// written, the plant restarts from the next start pose with zero metrics, and the planner stays active; with reset_x0
+// the next solve also plans from that pose (x0_out and the window).  Without it x0_out keeps the final pose, as the
+// benchmark's planner keeps its params['x0'] across episodes.  active_count falls when the sequence ends.
+template <bool SEQ = false>
+__device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int lane, const SeqArgs& q = SeqArgs{}) {
   if (k >= a.K || !a.active[k]) return;
-  const TrialDev& d = a.trials[k];
+  const int slot = SEQ ? q.first[k] + q.episode[k] : k;
+  const TrialDev& d = a.trials[slot];
   float* u = d.u_cur;
   float v = 0.0f, w = 0.0f;
   if (lane == 0) { v = u[0]; w = u[1]; }
@@ -399,8 +406,8 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
   }
   if (lane != 0) return;
   TrialState& s = a.state[k];
-  const int t = a.step;
-  float* uh = a.uhist + ((size_t)k * a.max_steps + t) * 2;
+  const int t = SEQ ? s.steps : a.step;
+  float* uh = a.uhist + ((size_t)slot * a.max_steps + t) * 2;
   uh[0] = v; uh[1] = w;
   const double x = s.x[0], y = s.x[1], th = s.x[2];
   double lt = 1.0, at = 1.0;
@@ -418,7 +425,7 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
   const double yn = __dadd_rn(y, __dmul_rn(__dmul_rn(dtl, sin(th)), (double)v));
   const double thn = __dadd_rn(th, __dmul_rn(__dmul_rn(d.dt, at), (double)w));
   s.x[0] = xn; s.x[1] = yn; s.x[2] = thn;
-  double* xh = a.xhist + ((size_t)k * (a.max_steps + 1) + t + 1) * 3;
+  double* xh = a.xhist + ((size_t)slot * (a.max_steps + 1) + t + 1) * 3;
   xh[0] = xn; xh[1] = yn; xh[2] = thn;
   // the next rollout starts from float32(x_next), as set_params would pass it
   d.x0_out[0] = __double2float_rn(xn); d.x0_out[1] = __double2float_rn(yn); d.x0_out[2] = __double2float_rn(thn);
@@ -446,6 +453,24 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
     status = TRIAL_LEFT_MAP;
   else if (t + 1 >= a.max_steps) status = TRIAL_MAX_STEPS;
   if (status != TRIAL_RUNNING) {
+    if constexpr (SEQ) {
+      TrialState& r = q.results[slot];
+      r = s;
+      r.status = status;
+      if (slot + 1 < q.first[k + 1] && (q.reset_x0 || status != TRIAL_LEFT_MAP)) {
+        const double* x0 = q.start + (size_t)(slot + 1) * 3;
+        s.x[0] = x0[0]; s.x[1] = x0[1]; s.x[2] = x0[2];
+        s.cum_obj = 0.0; s.cum_dist = 0.0; s.dist = 0.0;
+        s.steps = 0;
+        q.episode[k] += 1;
+        if (q.reset_x0) {
+          d.x0_out[0] = __double2float_rn(x0[0]); d.x0_out[1] = __double2float_rn(x0[1]);
+          d.x0_out[2] = __double2float_rn(x0[2]);
+          if (d.win) win_origin(d.x0_out[0], d.x0_out[1], d.win_pxl, d.win_pyl, d.win_res, d.win_cols, d.win_rows, d.win);
+        }
+        return;
+      }
+    }
     s.status = status;
     a.active[k] = 0;
     atomicSub(a.active_count, 1);
@@ -455,10 +480,18 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
 __global__ void __launch_bounds__(128) plant_step_kernel(const PlantArgs a) {
   plant_step_body(a, (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), (int)(threadIdx.x & 31));
 }
+
+__global__ void __launch_bounds__(128) plant_step_seq_kernel(const PlantArgs a, const SeqArgs q) {
+  plant_step_body<true>(a, (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), (int)(threadIdx.x & 31), q);
+}
 // [emu:end trial]
 
 void launch_plant_step(const PlantArgs& a, cudaStream_t st) {
   plant_step_kernel<<<(unsigned)((a.K + 3) / 4), 128, 0, st>>>(a);
+}
+
+void launch_plant_step_seq(const PlantArgs& a, const SeqArgs& q, cudaStream_t st) {
+  plant_step_seq_kernel<<<(unsigned)((a.K + 3) / 4), 128, 0, st>>>(a, q);
 }
 
 }  // namespace b200
