@@ -1673,7 +1673,7 @@ extern "C" int b200mppi_combine_partials_host(const float* g, int32_t ws, int32_
   for (int j = 0; j < 2 * T; ++j) {
     float v = 0.0f;
     for (int r = 0; r < ws; ++r) v = std::fmaf(g[(size_t)r * stride + 2 + j], sc[r], v);
-    const float u = u_in[j] + v / W;
+    const float u = (W == 0.0f) ? u_in[j] : u_in[j] + v / W;      // every cost +inf: a zero step
     const float lo = (j & 1) ? wr[0] : vr[0], hi = (j & 1) ? wr[1] : vr[1];
     u_out[j] = std::fmax(lo, std::fmin(hi, u));
   }

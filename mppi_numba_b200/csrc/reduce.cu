@@ -128,6 +128,8 @@ constexpr int MAX_PARTS = 512;
 
 // u_cur (clipped) from merged partials: u[j] <- clip(u[j] + (sum_i V_i[j] * scale_i) / W), and the normalised
 // weights of this rank's rollouts, weights[n] = w_raw[n] * exp(-(beta_cta - beta)/lambda) / W   (mppi.py:1173-1174).
+// W == 0 (every cost +inf, so every partial has scale 0 and V = 0): a zero step, u[j] <- clip(u[j]), and weight 0 --
+// 0 / 0 would make u NaN, which the clip turns into the upper bounds.
 // `first` / `step`: the CTA's share of the weight slabs (the u update is done by the caller's CTA 0).
 __device__ void apply_update(const UpdateArgs& a, const float* __restrict__ parts, int count, const float* s_scale,
                              float beta, float W, bool do_u, int first, int step) {
@@ -136,7 +138,7 @@ __device__ void apply_update(const UpdateArgs& a, const float* __restrict__ part
     for (int j = threadIdx.x; j < 2 * a.T; j += blockDim.x) {
       float v = 0.0f;
       for (int i = 0; i < count; ++i) v = fmaf(__ldcg(parts + (size_t)i * stride + 2 + j), s_scale[i], v);
-      float u = a.u_cur[j] + v / W;
+      const float u = (W == 0.0f) ? a.u_cur[j] : a.u_cur[j] + v / W;
       const float lo = (j & 1) ? a.wrange[0] : a.vrange[0];
       const float hi = (j & 1) ? a.wrange[1] : a.vrange[1];
       a.u_cur[j] = fmaxf(lo, fminf(hi, u));
@@ -274,7 +276,7 @@ __device__ __forceinline__ void update_partial_body(const UpdateArgs& a, const U
     for (; i < a.num_ctas; ++i) v = fmaf(__ldcg(a.cta_partials + (size_t)i * stride + 2 + j), s_scale[i], v);
     a.rank_partial[2 + j] = v;
     if (tl.mode == UPD_TAIL_APPLY) {               // one rank: this partial is the only one -- apply straight away
-      const float u = a.u_cur[j] + v / W;
+      const float u = (W == 0.0f) ? a.u_cur[j] : a.u_cur[j] + v / W;      // W == 0: every cost +inf (apply_update)
       const float lo = (j & 1) ? a.wrange[0] : a.vrange[0];
       const float hi = (j & 1) ? a.wrange[1] : a.vrange[1];
       const float un = fmaxf(lo, fminf(hi, u));
@@ -286,7 +288,8 @@ __device__ __forceinline__ void update_partial_body(const UpdateArgs& a, const U
   if (tid == 0) { a.rank_partial[0] = s_bS[0]; a.rank_partial[1] = W; }
   if (tl.mode == UPD_TAIL_APPLY) {
     // normalised weights (mppi.py:1173-1174): the merge scale of a rollout's CTA is exp(-(beta_cta - beta)/lambda)
-    for (int r = tid; r < a.N; r += blockDim.x) a.weights[r] = __ldcg(a.w_raw + r) * (s_scale[r / a.rows_per_cta] / W);
+    for (int r = tid; r < a.N; r += blockDim.x)
+      a.weights[r] = (W == 0.0f) ? 0.0f : __ldcg(a.w_raw + r) * (s_scale[r / a.rows_per_cta] / W);
   }
   if (tl.mode == UPD_TAIL_BCAST) {
     __syncthreads();                                // rank_partial complete (this CTA wrote all of it)

@@ -37,6 +37,7 @@ F64 = np.float64
 MODE_STOCHASTIC = 0      # use_tdm
 MODE_DET_DYN = 1         # use_det_dynamics
 MODE_SPEED_MAP = 2       # use_nom_dynamics_with_speed_map
+MODE_BAREBONE = 3        # the map-free notebook planner (rollout_costs_barebone, state_rollouts_barebone)
 
 DEFAULT_UNKNOWN_COST = 1e2   # mppi.py:32
 DEFAULT_OBS_COST = 1e5       # mppi.py:33
@@ -326,12 +327,13 @@ def rollout_costs_barebone(obs_pos, obs_r, vrange, wrange, xgoal, obs_cost, goal
         dx, dy = A.sub32(xg[0], xn), A.sub32(xg[1], yn)
         d2n = A.fma32(dx, dx, A.mul32(dy, dy))
         cn = A.fma32(d2n, w_dist, cost)
-        for k in range(len(orad)):
-            ddx, ddy = A.sub32(xn, op[k, 0]), A.sub32(yn, op[k, 1])
+        if len(orad):                                   # the indicators of every obstacle at once (N, K) ...
+            ddx, ddy = A.sub32(xn[:, None], op[None, :, 0]), A.sub32(yn[:, None], op[None, :, 1])
             q = A.fma32(ddx, ddx, A.mul32(ddy, ddy))
-            diff = A.fma32(-orad[k], orad[k], q)                                          # FFMA(-r, r, q)
-            ind = (diff > 0).astype(F64)
-            cn = A.d2f(A.fma64(1.0 - ind, A.f2d(obs_c), A.f2d(cn)))
+            diff = A.fma32(-orad[None, :], orad[None, :], q)                              # FFMA(-r, r, q)
+            inside = 1.0 - (diff > 0).astype(F64)
+        for k in range(len(orad)):                      # ... and their penalties added in the kernel's order
+            cn = A.d2f(A.fma64(inside[:, k], A.f2d(obs_c), A.f2d(cn)))
         x, y, th = np.where(active, xn, x), np.where(active, yn, y), np.where(active, thn, th)
         cost, d2 = np.where(active, cn, cost), np.where(active, d2n, d2)
         hit = active & (d2n <= tol2)
@@ -345,6 +347,38 @@ def rollout_costs_barebone(obs_pos, obs_r, vrange, wrange, xgoal, obs_cost, goal
     if return_states:
         return cost, states
     return cost
+
+
+def state_rollouts_barebone(V, x0, dt, u_cur, u_prev=None, noise=None, vrange=None, wrange=None, arith=None):
+    """get_state_rollout of the barebone notebook (cell 3, get_state_rollout_across_control_noise): float32 (V, T+1, 3),
+    the nominal unicycle of rollout_costs_barebone (dv = v*dt; x = fma(dv, cos, x); theta = fma(w, dt, theta)) with no
+    goal test and no early exit.  Row 0 rolls out u_cur unclipped and without noise, row b > 0 rolls out
+    clip(u_prev + noise[b])."""
+    A = arith or AR.NUMPY
+    u_cur = np.asarray(u_cur, dtype=F32)
+    T = u_cur.shape[0]
+    x0 = np.asarray(x0, dtype=F32)
+    dt = F32(dt)
+    v = np.empty((V, T), dtype=F32)
+    w = np.empty((V, T), dtype=F32)
+    v[0], w[0] = u_cur[:, 0], u_cur[:, 1]
+    if V > 1:
+        e = np.asarray(noise, dtype=F32)[1:V]
+        u_prev = np.asarray(u_prev, dtype=F32)
+        vr, wr = np.asarray(vrange, dtype=F32), np.asarray(wrange, dtype=F32)
+        v[1:] = np.maximum(vr[0], np.minimum(vr[1], A.add32(u_prev[None, :, 0], e[..., 0])))
+        w[1:] = np.maximum(wr[0], np.minimum(wr[1], A.add32(u_prev[None, :, 1], e[..., 1])))
+    out = np.zeros((V, T + 1, 3), dtype=F32)
+    out[:, 0, :] = x0
+    x = np.full(V, x0[0], dtype=F32)
+    y = np.full(V, x0[1], dtype=F32)
+    th = np.full(V, x0[2], dtype=F32)
+    for t in range(T):
+        dv = A.mul32(v[:, t], dt)
+        cs, sn = A.cos32(th), A.sin32(th)
+        x, y, th = A.fma32(dv, cs, x), A.fma32(dv, sn, y), A.fma32(w[:, t], dt, th)
+        out[:, t + 1, 0], out[:, t + 1, 1], out[:, t + 1, 2] = x, y, th
+    return out
 
 
 def cvar_count(M, cvar_alpha):

@@ -66,6 +66,9 @@ Weights: weight_n = f32(w_raw_n * f32(scale / W_hat)) with the CTA's scale relat
 (L = 2 roundings of factors in every path), so
     weight_n in [p_lo_n / W_hi * (1 - u)^2 - 2 TINY, p_hi_n / W_lo * (1 + u)^2 + 2 TINY],
 a relative bound around w_n plus the absolute subnormal term.
+
+Every cost +inf: the reference has no weights to normalise (A = 0, its own result is NaN).  The kernels take a zero
+step: u = clip(u0) exactly and every weight exactly 0.
 """
 import math
 from fractions import Fraction
@@ -255,7 +258,20 @@ def update_bounds(ctx, N, merges=1):
 def check_update(u, weights, costs, noise, u0, lam, vrange, wrange, N=None, merges=1, label=""):
     """Assert the kernels' u (T, 2) and weights (N,) lie within the bounds of the float64 reference; a +inf cost must
     get weight exactly 0 and no weight may be NaN.  N: rollouts per rank (default: all).  Returns the largest
-    |error| / bound of u and of the weights."""
+    |error| / bound of u and of the weights.  When every cost is +inf: u == clip(u0) and every weight 0, exactly."""
+    if np.isposinf(np.asarray(costs, dtype=F32)).all():
+        want = np.asarray(u0, dtype=F32).copy()
+        want[:, 0] = np.maximum(F32(vrange[0]), np.minimum(F32(vrange[1]), want[:, 0]))
+        want[:, 1] = np.maximum(F32(wrange[0]), np.minimum(F32(wrange[1]), want[:, 1]))
+        u = np.asarray(u, dtype=F32)
+        bad = np.argwhere(u != want)
+        assert bad.size == 0, "%s: every cost +inf, u%s = %r, want clip(u0) = %r (%d elements differ)" % (
+            label, tuple(bad[0]), u[tuple(bad[0])], want[tuple(bad[0])], len(bad))
+        if weights is not None:
+            wt = np.asarray(weights, dtype=F32)
+            assert (wt == 0).all(), "%s: every cost +inf, %d weights are not 0 (first %r)" % (
+                label, int((wt != 0).sum()), wt[wt != 0][:3].tolist())
+        return 0.0, 0.0
     want_u, want_w, ctx = update_reference(costs, noise, u0, lam, vrange, wrange)
     eu, ew = update_bounds(ctx, len(want_w) if N is None else N, merges)
     u = np.asarray(u, dtype=F32).astype(F64)

@@ -186,3 +186,20 @@ def test_barebone_rollout_matches_reference_notebook(golden_dir, gname):
     np.testing.assert_allclose(c, g["costs_" + gname], rtol=3e-6)
     if gname == "near":
         assert (g["costs_near"] < 0.1 * np.median(g["costs_far"])).any()      # early exits exercised
+
+
+def test_barebone_state_rollouts_match_reference_notebook(golden_dir):
+    """The notebook's get_state_rollout after its first solve (cfg T 1.0, dt 0.1, N 100, V 5; x0 (0, 0, pi/4)).  Its
+    solve aliases u_prev_d to u_cur_d, so both are the solve's result solve_u1; the noise is that solve's draw."""
+    g = load(golden_dir, "ref_barebone.npz")
+    ref = g["solve_states1"]
+    u1 = g["solve_u1"]
+    got = MR.state_rollouts_barebone(ref.shape[0], [0.0, 0.0, np.pi / 4], 0.1, u1, u1, g["solve_noise1"], [0.0, 2.0],
+                                     [-np.pi, np.pi])
+    assert got.shape == ref.shape
+    np.testing.assert_allclose(got, ref, rtol=2e-6, atol=2e-6)
+    assert not np.allclose(ref[0], ref[1])              # row 0 = the optimal sequence, the others noisy samples
+    # the noisy rows are clipped: without the clip (or without the noise) they differ from the notebook's
+    raw = MR.state_rollouts_barebone(ref.shape[0], [0.0, 0.0, np.pi / 4], 0.1, u1, u1, g["solve_noise1"], [-1e9, 1e9],
+                                     [-1e9, 1e9])
+    assert not np.allclose(raw[1:], ref[1:], rtol=2e-6, atol=2e-6)

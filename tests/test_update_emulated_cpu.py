@@ -169,6 +169,32 @@ def test_update_with_an_all_inf_cta_slab(emu, N):
     assert (u1 == u2).all() and (w1 == w2).all()
 
 
+@pytest.mark.parametrize("N,T", [(37, 3), (1000, 4), (9473, 64)])
+def test_update_with_every_cost_inf(emu, N, T):
+    """Every cost +inf (a barebone planner whose penalties overflow float32): every partial has scale 0, so W = 0.  The
+    update is a zero step -- u = clip(u0), with u0 outside the bounds in places -- and every weight is 0, in the
+    one-launch update, the two-step path and the sharded combine of 4 ranks; 0 / 0 would make u NaN, which the clip
+    turns into the upper bounds."""
+    rng = np.random.default_rng(N + T)
+    costs = np.full(N, np.inf, np.float32)
+    noise = (rng.standard_normal((N, T, 2)) * [2, 3]).astype(np.float32)
+    u0 = np.stack([rng.uniform(-1, 4, T), rng.uniform(-4, 4, T)], 1).astype(np.float32)
+    u1, w1, _ = _one_rank(emu, costs, noise, u0, 1.0)
+    RB.check_update(u1, w1, costs, noise, u0, 1.0, VR, WR, label="one launch, N %d" % N)
+    w_raw, parts, rank = _partial(emu, costs, noise, 1.0)
+    u2, w2 = _finish(emu, rank[None, :], w_raw, parts, u0, N, T, 1.0)
+    RB.check_update(u2, w2, costs, noise, u0, 1.0, VR, WR, label="two steps, N %d" % N)
+    ws = 4
+    shards = [_partial(emu, np.ascontiguousarray(costs[N * r // ws: N * (r + 1) // ws]),
+                       np.ascontiguousarray(noise[N * r // ws: N * (r + 1) // ws]), 1.0) for r in range(ws)]
+    gathered = np.stack([s[2] for s in shards])
+    for r in range(ws):
+        n = N * (r + 1) // ws - N * r // ws
+        u, w = _finish(emu, gathered, shards[r][0], shards[r][1], u0, n, T, 1.0)
+        RB.check_update(u, None, costs, noise, u0, 1.0, VR, WR, label="sharded, rank %d" % r)
+        assert (w == 0).all()
+
+
 def test_update_tail_broadcasts_the_rank_partial_to_every_peer(emu):
     """UPD_TAIL_BCAST (peer-memory exchange): 3 'ranks', each stores its partial into slot `rank` of all three
     gather buffers and raises its own epoch flag in every peer -- the gather buffers end up identical and equal to
