@@ -2,7 +2,7 @@
 """bench_trials.py -- closed-loop episodes of K planners: the host-driven loop against the batch's device episodes.
 
     python bench_trials.py --workload c2|c4|c3|ref|refm|gif|mix|bb --batch K --closed-loop S [--rounds R] [--profile]
-                           [--record-every n] [--share-tdms] [--episodes E]
+                           [--record-every n] [--share-tdms] [--episodes E [--device-grids]]
 
 c2 and c4 are one-map workloads (MPPI_Batch.run_trials); c3 and ref are stochastic (use_tdm, CVaR cost:
 MPPI_StochasticBatch.run_stochastic_trials).  ref is the reference benchmark's noisy_dyn trial shape (N 1024, M 1024,
@@ -47,6 +47,14 @@ on twins, each on a private TDM pair: u[0] of every solve and every planner's fi
 legs, all with params['x0'] set back to the start before each episode: "sequence", one run_trial_sequences(...,
 reset_x0=True) call; "calls", E run_trials calls, each running until its slowest planner stops (without --share-tdms
 its histories must equal the sequence's, bit for bit, or the run fails); "host", the host loop over the E episodes.
+--device-grids (with --episodes E; c4, ref): the E realisations every planner runs are drawn from a ground-truth use_tdm
+pair of the workload's map geometry and M (run_device_grids below), as the reference's real-world evaluation does.  The
+parity check holds draw_traction_grids against the notebook's sample_traction_grid on a twin pair (every plane bit for
+bit), then one run_trial_sequences(..., reset_x0=True) on the device set against the same call with the helper's host
+grids on twin planners (histories, steps, statuses and every planner's state bit for bit).  Then rounds of two legs,
+alternating: "host_grids" (the helper's grids, uploaded by each call) and "device_grids" (one shared set, read in
+place); then the draw itself against the helper's sample, copy and convert.  The JSON line adds the grid bytes each call
+uploads, computed from the shapes.
 """
 import argparse
 import functools
@@ -473,6 +481,129 @@ def run_episodes(args, emit):
                      "speedup_wall_vs_host": host["s_per_round_wall"] / seq["s_per_round_wall"]}))
 
 
+def run_device_grids(args, emit):
+    """--device-grids: the benchmark's E realisations per planner, drawn on the GPU from a ground-truth TDM pair and read
+    in place, against the same realisations drawn by the reference notebook's helper and passed as host grids."""
+    import torch
+    import __graft_entry__
+    __graft_entry__.build_engine()
+    import mppi_numba_b200 as E
+    from bench_batch import gpu_info, planner_state, same
+    from tests.scenarios import make_scenario
+    K, S, n_ep = args.batch, args.closed_loop, args.episodes
+    mode, N, M, T, H, res, B, da = LOCAL_WORKLOADS.get(args.workload) or WORKLOADS[args.workload]
+    stochastic = mode == "tdm"
+    Batch = E.MPPI_StochasticBatch if stochastic else E.MPPI_Batch
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    scs = []
+    for k in range(K):
+        sc = make_scenario(mode, N=N, M=M, T=T, H=H, W=H, res=res, B=B, seed=k + 1, det_alpha=da, warm_start=True)
+        if k % 2 == 0:
+            sc["params"]["xgoal"] = sc["params"]["x0"][:2] + np.array([1.2, -0.9])
+        scs.append(sc)
+    # the ground truth: a use_tdm pair of the workload's map geometry and M, as the notebook builds it next to the planner
+    gsc = make_scenario("tdm", N=N, M=M, T=T, H=H, W=H, res=res, B=B, seed=1000)
+
+    def gt_pair():
+        with _quiet():
+            cfg = E.Config(**gsc["cfg"])
+            lin, ang = E.TDM_Numba(cfg), E.TDM_Numba(cfg)
+            lin.set_TDM_from_PMF_grid(gsc["pmf_lin"], gsc["tdm_dict"])
+            ang.set_TDM_from_PMF_grid(gsc["pmf_ang"], gsc["tdm_dict"])
+        return lin, ang
+
+    def helper(lin, ang):                                # the notebook's sample_traction_grid, widened to float64
+        lq = lin.sample_grids().copy_to_host()[0]
+        lg = lq * (lin.bin_values_bounds[1] - lin.bin_values_bounds[0]) / 100.0 + lin.bin_values_bounds[0]
+        aq = ang.sample_grids().copy_to_host()[0]
+        ag = aq * (ang.bin_values_bounds[1] - ang.bin_values_bounds[0]) / 100.0 + ang.bin_values_bounds[0]
+        return E.TractionGrid(lg.astype(np.float64), ag.astype(np.float64), lin.res, xlimits=lin.padded_xlimits,
+                              ylimits=lin.padded_ylimits)
+
+    ga, gb = gt_pair(), gt_pair()
+    with _quiet():
+        A, Bs = ([make_planner(E, sc, 0)[3] for sc in scs] for _ in range(2))
+
+    def reset(pls):
+        for p, sc in zip(pls, scs):
+            p.params["x0"] = sc["params"]["x0"].copy()
+            p.u_cur_d.copy_to_device(sc["u0"])
+
+    for pls in (A, Bs):
+        reset(pls)
+    ba, bb = Batch(A), Batch(Bs)
+    dgrids = E.draw_traction_grids(ga[0], ga[1], n_ep)
+    hgrids = [helper(*gb) for _ in range(n_ep)]
+    dseqs, hseqs = [list(dgrids)] * K, [hgrids] * K
+
+    # ---- parity: the realisations, then one sequence call on device realisations == the twins' call on host grids
+    ok_planes = all(same(list(d.get_grids()), [h.lin_traction, h.ang_traction]) for d, h in zip(dgrids, hgrids))
+    with _quiet():
+        oa = ba.run_trial_sequences(dseqs, S, reset_x0=True)
+        ob = bb.run_trial_sequences(hseqs, S, reset_x0=True)
+    ok_out = all(oa[key].tobytes() == ob[key].tobytes() for key in ("xhist", "uhist", "steps")) and \
+        oa["status"] == ob["status"]
+    ok_state = all(same(planner_state(a, stochastic) + [a.params["x0"]], planner_state(b, stochastic) + [b.params["x0"]])
+                   for a, b in zip(A, Bs))
+    parity = {"passed": bool(ok_planes and ok_out and ok_state), "planes_bitwise": ok_planes,
+              "histories_bitwise": ok_out, "state_bitwise": ok_state, "steps": oa["steps"].tolist(),
+              "against": "the notebook's sample_traction_grid on a twin ground-truth pair, as host grids, on identical "
+                         "twin planners"}
+    if not parity["passed"]:
+        sys.stderr.write("bench_trials.py: PARITY CHECK FAILED: %s\n" % json.dumps(parity))
+        emit(json.dumps({"metric": "device realisations", "error": "parity_check failed", "parity_check": parity}))
+        raise SystemExit(3)
+
+    def round_(b, pls, seqs):
+        reset(pls)
+        o = b.run_trial_sequences(seqs, S, reset_x0=True)
+        torch.cuda.synchronize(dev)
+        return int(o["steps"].sum())
+
+    legs = [("host_grids", functools.partial(round_, bb, Bs, hseqs), bb),
+            ("device_grids", functools.partial(round_, ba, A, dseqs), ba)]
+    with _quiet():
+        for _, fn, _ in legs:                            # warm-up of both paths
+            fn()
+    res_ = {name: [] for name, _, _ in legs}
+    for _ in range(args.rounds):                         # alternate: host grids, device grids, ...
+        for name, fn, _ in legs:
+            t0 = time.perf_counter()
+            with _quiet():
+                steps = fn()
+            res_[name].append((time.perf_counter() - t0, steps))
+    # the draw itself against the helper's path, alternating (each call ends in a synchronisation)
+    draw, help_ = [], []
+    for _ in range(args.rounds):
+        t0 = time.perf_counter()
+        E.draw_traction_grids(ga[0], ga[1], n_ep)
+        draw.append(time.perf_counter() - t0)
+        t0 = time.perf_counter()
+        with _quiet():
+            [helper(*gb) for _ in range(n_ep)]
+        help_.append(time.perf_counter() - t0)
+    plane = dgrids.height * dgrids.width * 8
+
+    def summary(name):
+        wall = [r[0] for r in res_[name]]
+        return {"s_per_round_wall": float(np.median(wall)), "s_per_round_wall_runs": wall,
+                "control_steps_per_round": res_[name][0][1],
+                "grid_bytes_uploaded_per_call": (2 * plane * K * n_ep if name == "host_grids" else 0)}
+    host, devr = summary("host_grids"), summary("device_grids")
+    config = {"workload": (args.workload if args.workload in LOCAL_WORKLOADS else workload_name_of(args.workload)),
+              "batch": K, "max_steps": S, "episodes": n_ep, "reset_x0": True,
+              "ground_truth": "use_tdm pair of the workload's map geometry and M %d (seed 1000); one set of E "
+                              "realisations shared by every planner" % M,
+              "plane_cells": [dgrids.height, dgrids.width]}
+    emit(json.dumps({"metric": "trial sequences: host ground-truth grids vs device realisations read in place",
+                     "unit": "s/round", "value": devr["s_per_round_wall"], "higher_is_better": False, "config": config,
+                     "rounds": args.rounds, "gpu": gpu_info(dev), "parity_check": parity, "host_grids": host,
+                     "device_grids": devr, "speedup_wall": host["s_per_round_wall"] / devr["s_per_round_wall"],
+                     "draw_s": float(np.median(draw)), "draw_s_runs": draw, "helper_s": float(np.median(help_)),
+                     "helper_s_runs": help_}))
+
+
 def _quiet():
     import contextlib
     import io
@@ -670,6 +801,8 @@ def main():
                     help="K planners on one map: K private TDM pairs against one pair shared by all (not bb)")
     ap.add_argument("--episodes", type=int, default=None, metavar="E",
                     help="E ground-truth realisations per planner back to back (c2, c3, ref)")
+    ap.add_argument("--device-grids", action="store_true",
+                    help="with --episodes: the realisations drawn and read on the GPU against host grids (c4, ref)")
     args = ap.parse_args()
     if args.batch < 1 or args.closed_loop < 1 or args.rounds < 1:
         ap.error("--batch, --closed-loop and --rounds must be at least 1")
@@ -677,6 +810,13 @@ def main():
         ap.error("--record-every must be at least 1, and the bb workload does not take it")
     if args.share_tdms and args.workload in ("bb", "mix"):
         ap.error("--share-tdms: barebone planners have no TDMs, and mix planners no common map")
+    if args.device_grids:
+        if args.episodes is None or args.episodes < 1 or args.workload not in ("c4", "ref") or args.share_tdms or \
+                args.record_every is not None:
+            ap.error("--device-grids needs --episodes E >= 1 and workload c4 or ref, without --share-tdms and "
+                     "--record-every")
+        run_device_grids(args, emit)
+        return
     if args.episodes is not None:
         if args.episodes < 1 or args.workload not in ("c2", "c3", "ref") or args.record_every is not None:
             ap.error("--episodes must be at least 1, with workload c2, c3 or ref and without --record-every")

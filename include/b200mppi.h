@@ -148,6 +148,35 @@ int b200mppi_tdm_num_generators(b200mppi_tdm* tdm, int64_t* out);
 int b200mppi_tdm_get_rng_states(b200mppi_tdm* tdm, uint64_t* out, size_t bytes);
 int b200mppi_tdm_set_rng_states(b200mppi_tdm* tdm, const uint64_t* in, size_t bytes);
 
+/* ------------------------------------------------------------------ ground-truth realisations on the device
+ * The reference's real-world evaluation (confidence_score_example_vis.ipynb) drives the plant on realisations of a
+ * ground-truth TDM pair: its sample_traction_grid(lin, ang) calls lin.sample_grids(), copies map 0 to the host and
+ * converts it with q * (hi - lo) / 100.0 + lo, then does the same for ang, and wraps both in a TractionGrid on lin's
+ * padded limits and resolution.  A realisation set holds such grids in device memory, where trial calls read them in
+ * place (b200mppi_trial_desc).
+ *   draw_realisations: realisation i is what the helper's i-th call returns: b200mppi_tdm_sample_grids(lin, 1.0), then
+ *           b200mppi_tdm_sample_grids(ang, 1.0) (the same sampling path), map 0 of each converted into the set.  lin ==
+ *           ang is allowed and follows that order (the lin plane from the first sampling, the ang plane from the
+ *           second).  Afterwards both TDMs are exactly as after those 2 * count calls: generator states and sampled
+ *           maps.  Each plane is float64 (height, width) = (max_map_rows, max_map_cols) row-major on the TDMs' device
+ *           -- the whole sample plane, as copy_to_host()[0] -- with each cell float64(((float)q * (hi - lo)) / 100 + lo)
+ *           evaluated in float32, every operation rounded to nearest on its own (no flush to zero, no contraction), hi
+ *           and lo the bounds of that plane's TDM: what NumPy 2 computes for the helper (float32 bounds keep the result
+ *           float32), widened exactly.  One conversion launch per realisation for both planes (two when lin == ang).
+ *           Refused: count < 1, a PMF not set (B200MPPI_ESTATE), TDMs on different devices or of different
+ *           max_map_dim.
+ *   info  : count, height, width, and lin's res and padded limits (as the TDM holds them, float32) and the device.
+ *   planes: the device pointers of realisation i's lin and ang planes, for b200mppi_trial_desc.
+ *   copy_out: realisation i's planes into host float64 (height, width) arrays.
+ * The library keeps a registry of live sets; destroy removes a set from it and frees its memory. */
+typedef struct b200mppi_realisations b200mppi_realisations;
+int b200mppi_tdm_draw_realisations(b200mppi_tdm* lin, b200mppi_tdm* ang, int32_t count, b200mppi_realisations** out);
+int b200mppi_realisations_destroy(b200mppi_realisations* set);
+int b200mppi_realisations_info(const b200mppi_realisations* set, int32_t* count, int32_t* height, int32_t* width,
+                               double* res, double xlimits[2], double ylimits[2], int32_t* device);
+int b200mppi_realisations_planes(const b200mppi_realisations* set, int32_t i, const double** lin, const double** ang);
+int b200mppi_realisations_copy_out(const b200mppi_realisations* set, int32_t i, double* lin, double* ang);
+
 /* ------------------------------------------------------------------ planner */
 /* MPPI_Numba.init_device_vars_before_solving (mppi.py:108-127): noise (N,T,2), u_cur/u_prev (T,2),
  * costs (N), weights (N), N*T xoroshiro128+ generators, vis buffer (V,T+1,3).  With
@@ -425,9 +454,17 @@ int b200mppi_batch_get_state_rollout(b200mppi_batch* b, float* out, size_t bytes
  *             NaN after it;  results: count records;  steps_issued (may be NULL): steps the batch issued. */
 enum { B200MPPI_TRIAL_GOAL = 1, B200MPPI_TRIAL_MAX_STEPS = 2, B200MPPI_TRIAL_LEFT_MAP = 3,
        B200MPPI_TRIAL_NOT_RUN = 4 /* an episode of a trial sequence that never started */ };
+/* Grids: lin and ang are host arrays, uploaded by the call, or both the planes of one realisation of a live
+ * b200mppi_realisations set on the batch's device (b200mppi_realisations_planes), which the call reads in place: no copy
+ * and no device grid section for that slot; height and width must be the set's.  Both kinds may be mixed in one call.
+ * The call checks every pointer with cudaPointerGetAttributes and the set registry before any work: device memory that
+ * is not the start of a plane of a live set (another allocation, a destroyed set, the middle of a plane), a set on
+ * another device, lin and ang from different sets or of different kinds are refused (B200MPPI_EINVAL naming the planner
+ * and, for sequences, the episode).  The grid's position and resolution are the descriptor's (xlo, ylo, res), as for
+ * host grids. */
 typedef struct {
-  const double* lin;            /* ground-truth linear traction, (height, width) row-major, host */
-  const double* ang;            /* ground-truth angular traction, same shape */
+  const double* lin;            /* ground-truth linear traction, (height, width) row-major: host, or a realisation plane */
+  const double* ang;            /* ground-truth angular traction, same shape and kind */
   int32_t height, width;
   double xlo, ylo, res;         /* the grid's xlimits[0], ylimits[0] and cell size: cell = floor((x - xlo) / res) */
   double x0[3];                 /* start pose */

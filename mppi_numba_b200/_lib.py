@@ -85,6 +85,12 @@ def _load():
         "b200mppi_tdm_num_generators": (C.c_int, [P, C.POINTER(I64)]),
         "b200mppi_tdm_get_rng_states": (C.c_int, [P, P, SZ]),
         "b200mppi_tdm_set_rng_states": (C.c_int, [P, P, SZ]),
+        "b200mppi_tdm_draw_realisations": (C.c_int, [P, P, I32, C.POINTER(P)]),
+        "b200mppi_realisations_destroy": (C.c_int, [P]),
+        "b200mppi_realisations_info": (C.c_int, [P, C.POINTER(I32), C.POINTER(I32), C.POINTER(I32), C.POINTER(D),
+                                                 C.POINTER(D), C.POINTER(D), C.POINTER(I32)]),
+        "b200mppi_realisations_planes": (C.c_int, [P, I32, C.POINTER(P), C.POINTER(P)]),
+        "b200mppi_realisations_copy_out": (C.c_int, [P, I32, P, P]),
         "b200mppi_planner_create": (C.c_int, [C.POINTER(ConfigPOD), C.POINTER(P)]),
         "b200mppi_planner_destroy": (C.c_int, [P]),
         "b200mppi_planner_set_stream": (C.c_int, [P, P]),

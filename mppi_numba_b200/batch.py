@@ -27,6 +27,10 @@ planners and without a reset in between, as the reference benchmark runs its tri
 ``get_state_rollout()`` is every planner's get_state_rollout() with one launch, and ``record_every=n`` on any trial call
 records those rollouts at every n-th step inside the episodes, as the notebooks' drawing loop calls it.
 
+Every trial call takes ``DeviceTractionGrid`` realisations (``draw_traction_grids``) wherever it takes a
+``TractionGrid``: the plant reads them in GPU memory, with no upload, and the results are those of the same grids on
+the host.
+
 ``share_tdms=True`` lets planners share a lin/ang TDM pair (many robots on one map, or one environment solved at several
 cvar_alpha): each shared pair is sampled once per call, and each planner ends as its own call on a private copy of the
 pair would leave it (include/b200mppi.h, planners sharing TDM pairs).
@@ -37,6 +41,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import check, lib, ptr
+from .terrain import DeviceTractionGrid
 
 TRIAL_STATUS = {_lib.TRIAL_GOAL: "goal", _lib.TRIAL_MAX_STEPS: "max_steps", _lib.TRIAL_LEFT_MAP: "left_map",
                 _lib.TRIAL_NOT_RUN: "not_run"}
@@ -189,10 +194,11 @@ class MPPI_Batch(object):
 
     def run_trials(self, traction_grids, max_steps, dt=None, record_every=None):
         """One closed-loop episode per planner, on the GPU: up to ``max_steps`` rounds of ``u = solve()``, a plant step
-        on ``traction_grids[k]`` (a ``TractionGrid``, float or ``use_int8``) with ``u[0]`` and ``shift_and_update``,
-        stopping once the planner is within ``goal_tolerance`` of its goal -- the loop of the benchmark's ``trial()``,
-        whose ``dt`` argument (default: each planner's ``params['dt']``) is used as a float64.  A planner also stops when
-        its pose leaves the padded map limits, where its next ``solve()`` would be refused.
+        on ``traction_grids[k]`` (a ``TractionGrid``, float or ``use_int8``, or a ``DeviceTractionGrid``) with
+        ``u[0]`` and ``shift_and_update``, stopping once the planner is within ``goal_tolerance`` of its goal -- the
+        loop of the benchmark's ``trial()``, whose ``dt`` argument (default: each planner's ``params['dt']``) is used as
+        a float64.  A planner also stops when its pose leaves the padded map limits, where its next ``solve()`` would
+        be refused.
 
         Afterwards every planner (controls, noise, costs, weights, RNG streams, its TDMs' streams and sampled maps, and
         ``params['x0']``) is exactly as after that host loop.  With share_tdms, a shared pair is sampled once per step
@@ -316,11 +322,11 @@ class MPPI_Batch(object):
 
     def run_trial_sequences(self, traction_grids, max_steps, dt=None, reset_x0=False):
         """Several closed-loop episodes per planner, back to back on the GPU: planner k runs one episode of
-        ``run_trials`` (``run_stochastic_trials`` for use_tdm planners) on each ``TractionGrid`` of the non-empty list
-        ``traction_grids[k]`` in turn, each starting its plant at ``x_start = params['x0']`` of the call, with the
-        stop rules, ``dt`` and log conventions of run_trials.  Between episodes nothing is reset: the planner keeps its
-        warm start, RNG streams and its TDMs' streams and maps -- the loop the reference benchmark runs over
-        trials_per_env realisations after one setup().
+        ``run_trials`` (``run_stochastic_trials`` for use_tdm planners) on each grid (``TractionGrid`` or
+        ``DeviceTractionGrid``) of the non-empty list ``traction_grids[k]`` in turn, each starting its plant at
+        ``x_start = params['x0']`` of the call, with the stop rules, ``dt`` and log conventions of run_trials.
+        Between episodes nothing is reset: the planner keeps its warm start, RNG streams and its TDMs' streams and maps
+        -- the loop the reference benchmark runs over trials_per_env realisations after one setup().
           ``reset_x0=False`` (the benchmark's loop): ``params['x0']`` is left at the previous episode's final pose, so
               an episode's first solve plans from there.  An episode ending "left_map" ends the planner's sequence
               (its next solve would be refused); the later episodes are "not_run".
@@ -396,8 +402,9 @@ class MPPI_Batch(object):
 
 
 def _fill_desc(who, p, g, dt, d, keep):
-    """Trial descriptor ``d`` of planner ``p`` on TractionGrid ``g`` (None: barebone), starting at params['x0']; the
-    float64 grids it points to are appended to ``keep``.  ``who`` prefixes the refusals."""
+    """Trial descriptor ``d`` of planner ``p`` on TractionGrid or DeviceTractionGrid ``g`` (None: barebone), starting
+    at params['x0']; the float64 grids it points to (a device grid: the grid, which keeps its set alive) are appended
+    to ``keep``.  ``who`` prefixes the refusals."""
     q = p.params
     if g is None:
         d.x0[:] = [float(v) for v in np.asarray(q["x0"], dtype=np.float64)[:3]]
@@ -409,18 +416,23 @@ def _fill_desc(who, p, g, dt, d, keep):
         if not (np.isfinite(d.dt) and d.dt > 0):
             raise ValueError("%s: dt %r not finite and positive" % (who, d.dt))
         return
-    lin, ang = np.asarray(g.lin_traction), np.asarray(g.ang_traction)
-    for a in (lin, ang):
-        if a.dtype != np.float64 and not np.issubdtype(a.dtype, np.integer):
-            raise ValueError("%s: traction grid of dtype %s (float64 or integer grids only: the plant step is "
-                             "float64)" % (who, a.dtype))
-    if lin.ndim != 2 or lin.shape != ang.shape:
-        raise ValueError("%s: lin / ang traction grids of shapes %s / %s" % (who, lin.shape, ang.shape))
-    lin = np.ascontiguousarray(lin, dtype=np.float64)
-    ang = np.ascontiguousarray(ang, dtype=np.float64)
-    keep += [lin, ang]
-    d.lin, d.ang = lin.ctypes.data, ang.ctypes.data
-    d.height, d.width = lin.shape
+    if isinstance(g, DeviceTractionGrid):                # read in place by the plant step
+        keep.append(g)
+        d.lin, d.ang = g._lin_ptr, g._ang_ptr
+        d.height, d.width = g.height, g.width
+    else:
+        lin, ang = np.asarray(g.lin_traction), np.asarray(g.ang_traction)
+        for a in (lin, ang):
+            if a.dtype != np.float64 and not np.issubdtype(a.dtype, np.integer):
+                raise ValueError("%s: traction grid of dtype %s (float64 or integer grids only: the plant step is "
+                                 "float64)" % (who, a.dtype))
+        if lin.ndim != 2 or lin.shape != ang.shape:
+            raise ValueError("%s: lin / ang traction grids of shapes %s / %s" % (who, lin.shape, ang.shape))
+        lin = np.ascontiguousarray(lin, dtype=np.float64)
+        ang = np.ascontiguousarray(ang, dtype=np.float64)
+        keep += [lin, ang]
+        d.lin, d.ang = lin.ctypes.data, ang.ctypes.data
+        d.height, d.width = lin.shape
     d.xlo, d.ylo, d.res = float(g.xlimits[0]), float(g.ylimits[0]), float(g.res)
     d.x0[:] = [float(v) for v in np.asarray(q["x0"], dtype=np.float64)[:3]]
     d.xgoal[:] = [float(v) for v in np.asarray(q["xgoal"], dtype=np.float64)[:2]]

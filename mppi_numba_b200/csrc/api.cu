@@ -6,6 +6,8 @@
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
+#include <memory>
+#include <mutex>
 #include <string>
 #include <utility>
 #include <vector>
@@ -716,6 +718,188 @@ extern "C" int b200mppi_tdm_set_rng_states(b200mppi_tdm* t, const uint64_t* in, 
   uint64_t h = 0x1234567ULL;
   for (size_t i = 0; i < bytes / 8; ++i) h = mix_sig(h, in[i]);
   t->sig = h;
+  return B200MPPI_OK;
+}
+
+// --------------------------------------------------------------------------------------------- ground-truth realisations
+// A set of `count` (lin, ang) float64 planes on one device; realisation i's lin plane is plane 2 i, its ang plane 2 i + 1.
+struct b200mppi_realisations {
+  int device = 0, count = 0, rows = 0, cols = 0;
+  float res = 1, pxl[2] = {0, 0}, pyl[2] = {0, 0};
+  double* d = nullptr;                  // (count, 2, rows, cols)
+  size_t plane() const { return (size_t)rows * cols; }
+  uintptr_t lo() const { return reinterpret_cast<uintptr_t>(d); }
+  uintptr_t hi() const { return lo() + (size_t)2 * count * plane() * sizeof(double); }
+};
+
+// The live sets, which trial calls may read in place, and the address ranges of destroyed ones: a pointer into freed
+// device memory looks like pageable host memory to cudaPointerGetAttributes, and must not be read as such.  A range is
+// forgotten once a new set covers it; the oldest are dropped beyond REALISATION_RETIRED entries.
+constexpr size_t REALISATION_RETIRED = 4096;
+static std::mutex g_sets_mu;
+static std::vector<b200mppi_realisations*> g_sets;
+struct RetiredRange { int device; uintptr_t lo, hi; };
+static std::vector<RetiredRange> g_retired;
+
+extern "C" int b200mppi_tdm_draw_realisations(b200mppi_tdm* lin, b200mppi_tdm* ang, int32_t count,
+                                              b200mppi_realisations** out) {
+  if (!lin || !ang || !out) return fail(B200MPPI_EINVAL, "draw_realisations: null argument");
+  if (count < 1) return fail(B200MPPI_EINVAL, "draw_realisations: count " + std::to_string(count) + " < 1");
+  if (!lin->pmf_set || !ang->pmf_set) return fail(B200MPPI_ESTATE, "draw_realisations: PMF grid not set");
+  if (lin->cfg.device != ang->cfg.device)
+    return fail(B200MPPI_EINVAL, "draw_realisations: lin is on device " + std::to_string(lin->cfg.device) + ", ang on " +
+                                 std::to_string(ang->cfg.device));
+  if (lin->cfg.max_map_rows != ang->cfg.max_map_rows || lin->cfg.max_map_cols != ang->cfg.max_map_cols)
+    return fail(B200MPPI_EINVAL, "draw_realisations: lin and ang sample planes differ in shape (max_map_dim)");
+  CU(cudaSetDevice(lin->cfg.device));
+  std::unique_ptr<b200mppi_realisations> s(new b200mppi_realisations());
+  s->device = lin->cfg.device; s->count = count; s->rows = lin->cfg.max_map_rows; s->cols = lin->cfg.max_map_cols;
+  s->res = lin->res;
+  s->pxl[0] = lin->pxl[0]; s->pxl[1] = lin->pxl[1]; s->pyl[0] = lin->pyl[0]; s->pyl[1] = lin->pyl[1];
+  struct Mem { double* p = nullptr; ~Mem() { cudaFree(p); } } mem;   // freed unless the set is registered
+  CU(cudaMalloc(&mem.p, (size_t)2 * count * s->plane() * sizeof(double)));
+  s->d = mem.p;
+  // everything on lin's stream, after the work already issued on ang's
+  CU(cudaStreamSynchronize(ang->stream));
+  const cudaStream_t st = lin->stream;
+  int64_t launches = 0;
+  int rc;
+  auto sample = [&](b200mppi_tdm* t) -> int {         // == b200mppi_tdm_sample_grids(t, 1.0)
+    SamplePlan pl;
+    int r = plan_sampling(t, nullptr, 1.0, st, &pl);
+    return r ? r : plan_launch(pl, false, st, &launches);
+  };
+  for (int i = 0; i < count; ++i) {
+    double* const planes = s->d + (size_t)2 * i * s->plane();
+    const RealisationPlane pl{lin->grid, lin->pitch, lin->bounds[0], lin->bounds[1], planes};
+    const RealisationPlane pa{ang->grid, ang->pitch, ang->bounds[0], ang->bounds[1], planes + s->plane()};
+    if ((rc = sample(lin))) return rc;
+    if (lin == ang) {                                 // the second sampling overwrites the first's map 0
+      launch_realisation_convert(pl, pl, 1, s->rows, s->cols, st);
+      CHECK_LAUNCH();
+      if ((rc = sample(ang))) return rc;
+      launch_realisation_convert(pa, pa, 1, s->rows, s->cols, st);
+    } else {
+      if ((rc = sample(ang))) return rc;
+      launch_realisation_convert(pl, pa, 2, s->rows, s->cols, st);
+    }
+    CHECK_LAUNCH();
+  }
+  CU(cudaStreamSynchronize(st));
+  {
+    std::lock_guard<std::mutex> g(g_sets_mu);
+    g_retired.erase(std::remove_if(g_retired.begin(), g_retired.end(), [&](const RetiredRange& r) {
+                      return r.device == s->device && r.lo < s->hi() && s->lo() < r.hi;
+                    }), g_retired.end());
+    g_sets.push_back(s.get());
+  }
+  mem.p = nullptr;
+  *out = s.release();
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_realisations_destroy(b200mppi_realisations* s) {
+  if (!s) return B200MPPI_OK;
+  {
+    std::lock_guard<std::mutex> g(g_sets_mu);
+    auto it = std::find(g_sets.begin(), g_sets.end(), s);
+    if (it == g_sets.end()) return fail(B200MPPI_EINVAL, "realisations_destroy: not a live realisation set");
+    g_sets.erase(it);
+    if (g_retired.size() >= REALISATION_RETIRED) g_retired.erase(g_retired.begin());
+    g_retired.push_back(RetiredRange{s->device, s->lo(), s->hi()});
+  }
+  cudaSetDevice(s->device);
+  cudaFree(s->d);
+  delete s;
+  return B200MPPI_OK;
+}
+
+static bool realisations_live(const b200mppi_realisations* s) {
+  std::lock_guard<std::mutex> g(g_sets_mu);
+  return s && std::find(g_sets.begin(), g_sets.end(), s) != g_sets.end();
+}
+
+extern "C" int b200mppi_realisations_info(const b200mppi_realisations* s, int32_t* count, int32_t* height,
+                                          int32_t* width, double* res, double xlimits[2], double ylimits[2],
+                                          int32_t* device) {
+  if (!realisations_live(s)) return fail(B200MPPI_EINVAL, "realisations_info: not a live realisation set");
+  if (count) *count = s->count;
+  if (height) *height = s->rows;
+  if (width) *width = s->cols;
+  if (res) *res = s->res;
+  if (xlimits) { xlimits[0] = s->pxl[0]; xlimits[1] = s->pxl[1]; }
+  if (ylimits) { ylimits[0] = s->pyl[0]; ylimits[1] = s->pyl[1]; }
+  if (device) *device = s->device;
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_realisations_planes(const b200mppi_realisations* s, int32_t i, const double** lin,
+                                            const double** ang) {
+  if (!realisations_live(s)) return fail(B200MPPI_EINVAL, "realisations_planes: not a live realisation set");
+  if (i < 0 || i >= s->count || !lin || !ang)
+    return fail(B200MPPI_EINVAL, "realisations_planes: bad index " + std::to_string(i) + " or null output");
+  *lin = s->d + (size_t)2 * i * s->plane();
+  *ang = *lin + s->plane();
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_realisations_copy_out(const b200mppi_realisations* s, int32_t i, double* lin, double* ang) {
+  const double* dl;
+  const double* da;
+  const int rc = b200mppi_realisations_planes(s, i, &dl, &da);
+  if (rc) return rc;
+  CU(cudaSetDevice(s->device));
+  CU(cudaMemcpy(lin, dl, s->plane() * sizeof(double), cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(ang, da, s->plane() * sizeof(double), cudaMemcpyDeviceToHost));
+  return B200MPPI_OK;
+}
+
+// Where descriptor `d` of a trial call on `device` reads its grids: host arrays (*in_place false), or two planes of a
+// live realisation set (*in_place true): both pointers device memory of that device, each at the start of a plane of one
+// live set whose planes have the descriptor's height and width.  Anything else is refused, naming `who`.
+static int trial_grid_source(const b200mppi_trial_desc& d, int device, const std::string& who, bool* in_place) {
+  auto memory_type = [](const void* p, int* dev) {
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return cudaMemoryTypeUnregistered; }
+    *dev = a.device;
+    return a.type;
+  };
+  const void* ptrs[2] = {d.lin, d.ang};
+  const b200mppi_realisations* sets[2] = {};
+  bool dev_mem[2] = {};
+  std::lock_guard<std::mutex> g(g_sets_mu);
+  for (int k = 0; k < 2; ++k) {
+    const char* name = k ? "ang" : "lin";
+    const uintptr_t a = reinterpret_cast<uintptr_t>(ptrs[k]);
+    int dev = -1;
+    const cudaMemoryType type = memory_type(ptrs[k], &dev);
+    dev_mem[k] = type == cudaMemoryTypeDevice || type == cudaMemoryTypeManaged;
+    for (const b200mppi_realisations* s : g_sets)
+      if (a >= s->lo() && a < s->hi()) sets[k] = s;
+    if (!sets[k]) {
+      for (const RetiredRange& r : g_retired)         // page-locked host memory is what it says it is
+        if (type != cudaMemoryTypeHost && a >= r.lo && a < r.hi)
+          return fail(B200MPPI_EINVAL, who + ": the " + name + " grid lies in a destroyed realisation set");
+      if (dev_mem[k])
+        return fail(B200MPPI_EINVAL, who + ": the " + name + " grid is device memory but not a plane of a live "
+                                     "realisation set");
+      continue;
+    }
+    if (!dev_mem[k] || dev != device || sets[k]->device != device)
+      return fail(B200MPPI_EINVAL, who + ": the " + name + " grid is a realisation on device " +
+                                   std::to_string(sets[k]->device) + ", the batch runs on device " + std::to_string(device));
+    if ((a - sets[k]->lo()) % (sets[k]->plane() * sizeof(double)) != 0)
+      return fail(B200MPPI_EINVAL, who + ": the " + name + " grid points into the middle of a realisation plane");
+  }
+  *in_place = sets[0] != nullptr;
+  if ((sets[0] != nullptr) != (sets[1] != nullptr))
+    return fail(B200MPPI_EINVAL, who + ": one grid is a device realisation, the other host memory");
+  if (*in_place && sets[0] != sets[1])
+    return fail(B200MPPI_EINVAL, who + ": lin and ang grids are planes of two different realisation sets");
+  if (*in_place && (d.height != sets[0]->rows || d.width != sets[0]->cols))
+    return fail(B200MPPI_EINVAL, who + ": grid of " + std::to_string(d.height) + " x " + std::to_string(d.width) +
+                                 " cells, its realisation planes hold " + std::to_string(sets[0]->rows) + " x " +
+                                 std::to_string(sets[0]->cols));
   return B200MPPI_OK;
 }
 
@@ -2501,7 +2685,7 @@ enum class TrialKind { onemap, stochastic, barebone };
 
 // first: planner i's descriptors are tr[first[i] .. first[i + 1]): one each, or (seq) its episodes in a trial sequence
 static int trial_validate(b200mppi_batch* b, TrialKind kind, const b200mppi_trial_desc* tr, int32_t max_steps,
-                          const char* fn, const std::vector<int>& first, bool seq) {
+                          const char* fn, const std::vector<int>& first, bool seq, std::vector<char>& in_place) {
   if (!tr) return fail(B200MPPI_EINVAL, std::string(fn) + ": null trial descriptors");
   if (max_steps < 1) return fail(B200MPPI_EINVAL, std::string(fn) + ": max_steps < 1");
   if (kind != TrialKind::barebone && b->mode == B200MPPI_MODE_BAREBONE)
@@ -2509,6 +2693,7 @@ static int trial_validate(b200mppi_batch* b, TrialKind kind, const b200mppi_tria
                                  "MODE_SPEED_MAP batches)");
   int rc = batch_validate(b);
   if (rc) return rc;
+  in_place.assign(first.back(), 0);
   for (int j = 0; j < first.back(); ++j) {
     const int i = (int)(std::upper_bound(first.begin(), first.end(), j) - first.begin()) - 1;
     const std::string who = std::string(fn) + ": planner " + std::to_string(i) +
@@ -2534,6 +2719,9 @@ static int trial_validate(b200mppi_batch* b, TrialKind kind, const b200mppi_tria
     if (!(d.x0[0] >= d.pxlim[0] && d.x0[0] <= d.pxlim[1] && d.x0[1] >= d.pylim[0] && d.x0[1] <= d.pylim[1]) ||
         !std::isfinite(d.x0[2]))
       return fail(B200MPPI_EINVAL, who + ": start pose outside the padded map limits");
+    bool dev = false;
+    if ((rc = trial_grid_source(d, b->device, who, &dev))) return rc;
+    in_place[j] = dev;
   }
   return B200MPPI_OK;
 }
@@ -2696,10 +2884,10 @@ static const char* mode_name(int mode) {
 // there) | stochastic: the parity-0 sampler set | not barebone: the parity-1 set | stochastic: box descriptors, box
 // records | shared TDM pairs: group records (stochastic), group descriptors, members | not barebone: the launch classes'
 // pairs | states | barebone: contacts |
-// trials | active K + count | recording: vis descriptors | not barebone: grids | recording: the records (K, R, V, T+1,
-// 3) | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds
+// trials | active K + count | recording: vis descriptors | not barebone: the host grids | recording: the records (K, R,
+// V, T+1, 3) | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds
 // xhist and uhist: the float64 ground-truth grids (tens of MB for a batch of large maps) are copied straight from the
-// caller's arrays, and the written records (of K * R * V * (T+1) * 12 bytes, 145 MB for K 8, 150 steps, V 100, T 100)
+// caller's arrays (a slot whose grids are planes of a realisation set has no grid section: the plant reads the planes), and the written records (of K * R * V * (T+1) * 12 bytes, 145 MB for K 8, 150 steps, V 100, T 100)
 // straight into the caller's array.
 // Trial sequences (episodes non-null, b200mppi_batch_run_trial_sequences): planner i runs episodes[i] episodes back to
 // back, descriptors, histories and results per slot (planner-major: planner i's are slots first[i] .. first[i + 1]),
@@ -2737,7 +2925,8 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   if (!b->stochastic && stochastic)
     return fail(B200MPPI_EINVAL, fn + ": planner 0 is " + mode_name(b->mode) +
                                      " (stochastic trials run MODE_TDM batches; b200mppi_batch_run_trials runs the others)");
-  int rc = trial_validate(b, kind, trials, max_steps, fn.c_str(), first, seq);
+  std::vector<char> in_place;                         // slots whose grids are realisation planes, read where they are
+  int rc = trial_validate(b, kind, trials, max_steps, fn.c_str(), first, seq, in_place);
   if (rc) return rc;
   if (!xhist || !uhist || !results || (barebone && !contact_steps))
     return fail(B200MPPI_EINVAL, fn + ": null output buffer");
@@ -2800,7 +2989,7 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   std::vector<size_t> off_grid(nslot);
   for (int j = 0; j < nslot; ++j) {
     off_grid[j] = off;
-    if (!barebone) off += align256((size_t)2 * trials[j].height * trials[j].width * sizeof(double));
+    if (!barebone && !in_place[j]) off += align256((size_t)2 * trials[j].height * trials[j].width * sizeof(double));
   }
   const size_t off_vrec = off;
   off += align256(rec_bytes);
@@ -2859,7 +3048,9 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
         continue;
       }
       const double* dg = reinterpret_cast<const double*>(d + off_grid[j]);
-      t.lin = dg; t.ang = dg + (size_t)q.height * q.width; t.H = q.height; t.W = q.width;
+      t.lin = in_place[j] ? q.lin : dg;
+      t.ang = in_place[j] ? q.ang : dg + (size_t)q.height * q.width;
+      t.H = q.height; t.W = q.width;
       t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res;
       t.pxlim[0] = q.pxlim[0]; t.pxlim[1] = q.pxlim[1]; t.pylim[0] = q.pylim[0]; t.pylim[1] = q.pylim[1];
       if (!stochastic) {
@@ -2915,6 +3106,7 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   const RolloutWinArgs g0 = stochastic ? *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win) : RolloutWinArgs{};
   CU(cudaMemcpyAsync(d, h, head, cudaMemcpyHostToDevice, st));
   for (int j = 0; j < nslot && !barebone; ++j) {      // pageable sources: staged by the driver before the call returns
+    if (in_place[j]) continue;
     const size_t bytes = (size_t)trials[j].height * trials[j].width * sizeof(double);
     CU(cudaMemcpyAsync(d + off_grid[j], trials[j].lin, bytes, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(d + off_grid[j] + bytes, trials[j].ang, bytes, cudaMemcpyHostToDevice, st));

@@ -313,6 +313,19 @@ void launch_collapse_pad(const int8_t* raw, int8_t* out, int8_t* risk, int* bad_
                          int H, int W, int keep_r, int keep_c, int pad, int risk_pitch, double alpha, float lo,
                          float range, int mode, cudaStream_t st);
 
+// ground-truth realisations (b200mppi_tdm_draw_realisations): map 0 of a TDM's sample buffer -> one float64 plane
+// [emu:begin realisation_args]
+struct RealisationPlane {
+  const int8_t* grid;   // map 0 of the sample buffer, rows of `pitch` bytes
+  int pitch;
+  float lo, hi;         // the TDM's bin_values_bounds
+  double* out;          // (rows, cols) row-major
+};
+// [emu:end realisation_args]
+// one launch converts `planes` (1 or 2: p0, then p1) planes of rows x cols cells
+void launch_realisation_convert(const RealisationPlane& p0, const RealisationPlane& p1, int planes, int rows, int cols,
+                                cudaStream_t st);
+
 // sample_noise_numba (mppi.py:1354-1370): generators (n_global*T + t); writes noise (N,T,2).
 // `reach` (may be null): a device float the kernel zeroes for the prepare kernel's max-reduction
 void launch_sample_noise(uint64_t* states, float* noise, int n_local, int T, float std_v,

@@ -814,6 +814,70 @@ void launch_sample_window_complete(const SampleGridsV2Args& a, const ReachBoxCon
   else go(sample_window_complete_kernel<0>);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Ground-truth realisations (b200mppi_tdm_draw_realisations): byte q of map 0 -> float64(((float)q * (hi - lo)) / 100
+// + lo), the expression NumPy 2 evaluates for the reference notebook's sample_traction_grid (an int8 array with float32
+// bounds stays float32), widened exactly.  Each operation is IEEE float32 rounded to nearest on its own -- no .ftz
+// (the library is built with -ftz=true), no contraction -- so subnormal bounds convert as NumPy converts them.
+// Plane blockIdx.y: p0 or p1; one thread per cell.
+// [emu:begin realisation]
+__device__ __forceinline__ float ieee_sub(float a, float b) {
+#ifdef __CUDA_ARCH__
+  float r; asm("sub.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r;
+#else
+  return a - b;
+#endif
+}
+__device__ __forceinline__ float ieee_mul(float a, float b) {
+#ifdef __CUDA_ARCH__
+  float r; asm("mul.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r;
+#else
+  return a * b;
+#endif
+}
+__device__ __forceinline__ float ieee_div(float a, float b) {
+#ifdef __CUDA_ARCH__
+  float r; asm("div.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r;
+#else
+  return a / b;
+#endif
+}
+__device__ __forceinline__ float ieee_add(float a, float b) {
+#ifdef __CUDA_ARCH__
+  float r; asm("add.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r;
+#else
+  return a + b;
+#endif
+}
+__device__ __forceinline__ double ieee_widen(float a) {
+#ifdef __CUDA_ARCH__
+  double r; asm("cvt.f64.f32 %0, %1;" : "=d"(r) : "f"(a)); return r;
+#else
+  return (double)a;
+#endif
+}
+__global__ void __launch_bounds__(256) realisation_convert_kernel(const RealisationPlane p0, const RealisationPlane p1,
+                                                                  int rows, int cols) {
+  const bool second = blockIdx.y != 0;                              // field by field: no local copy of a plane
+  const int8_t* grid = second ? p1.grid : p0.grid;
+  const int pitch = second ? p1.pitch : p0.pitch;
+  const float lo = second ? p1.lo : p0.lo, hi = second ? p1.hi : p0.hi;
+  double* out = second ? p1.out : p0.out;
+  const int64_t cell = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (cell >= (int64_t)rows * cols) return;
+  const int r = (int)(cell / cols), c = (int)(cell % cols);
+  const float q = (float)grid[(size_t)r * pitch + c];               // exact
+  out[cell] = ieee_widen(ieee_add(ieee_div(ieee_mul(q, ieee_sub(hi, lo)), 100.0f), lo));
+}
+// [emu:end realisation]
+
+void launch_realisation_convert(const RealisationPlane& p0, const RealisationPlane& p1, int planes, int rows, int cols,
+                                cudaStream_t st) {
+  const int64_t cells = (int64_t)rows * cols;
+  realisation_convert_kernel<<<dim3((unsigned)((cells + 255) / 256), (unsigned)planes), 256, 0, st>>>(p0, p1, rows,
+                                                                                                      cols);
+}
+
 static size_t box_batch_smem(const SampleGridsV2Args& geom, int ncact) {
   size_t smem = 0;
   for (int lo = 0; lo + ncact <= geom.ty; ++lo)

@@ -9,6 +9,10 @@ reference, but vectorised per terrain class / per grid instead of per cell.
 
 ``Terrain`` and ``TractionGrid`` are the small simulation-side helpers (terrain.py:24-66,750-785)
 that closed-loop drivers use next to the planner; they never touch the GPU.
+
+``draw_traction_grids(lin_tdm, ang_tdm, count)`` draws ground-truth realisations of a TDM pair on the GPU, as the
+reference notebook's ``sample_traction_grid`` helper does, and keeps them there: each ``DeviceTractionGrid`` can be
+given to the batches' trial calls wherever a ``TractionGrid`` is taken, and the plant reads it in place.
 """
 import ctypes as C
 import math
@@ -452,3 +456,80 @@ class TractionGrid(object):
 
     def get_grids(self):
         return self.lin_traction, self.ang_traction
+
+
+class DeviceTractionGrid(object):
+    """One ground-truth realisation in GPU memory, taken by the batches' trial calls wherever a ``TractionGrid`` is:
+    the plant step reads its planes in place.  ``res``, ``xlimits``, ``ylimits``, ``height`` and ``width`` as on the
+    ``TractionGrid`` the notebook's helper builds; ``get_grids()`` copies both planes to the host.  Keeps its set alive."""
+
+    def __init__(self, owner, index):
+        self._owner = owner
+        self.index = index
+        lin, ang = C.c_void_p(), C.c_void_p()
+        check(lib.b200mppi_realisations_planes(owner._handle, index, C.byref(lin), C.byref(ang)))
+        self._lin_ptr, self._ang_ptr = lin.value, ang.value
+        self.res, self.xlimits, self.ylimits = owner.res, owner.xlimits, owner.ylimits
+        self.height, self.width = owner.height, owner.width
+
+    def get_grids(self):
+        """(lin, ang): float64 (height, width) host copies of the realisation."""
+        lin = np.empty((self.height, self.width), dtype=np.float64)
+        ang = np.empty_like(lin)
+        check(lib.b200mppi_realisations_copy_out(self._owner._handle, self.index, ptr(lin), ptr(ang)))
+        return lin, ang
+
+
+class DeviceTractionGrids(object):
+    """A sequence of ``count`` DeviceTractionGrid drawn by ``draw_traction_grids``; the device memory is freed when
+    neither this object nor any of its grids is referenced."""
+
+    def __init__(self, handle, lin_tdm):
+        self._handle = handle
+        count, height, width, device = C.c_int32(), C.c_int32(), C.c_int32(), C.c_int32()
+        check(lib.b200mppi_realisations_info(handle, C.byref(count), C.byref(height), C.byref(width), None, None, None,
+                                             C.byref(device)))
+        self.height, self.width, self.device = int(height.value), int(width.value), int(device.value)
+        # the geometry of the helper's TractionGrid: the TDM's own res and padded limits (float64 on the host)
+        self.res = lin_tdm.res
+        self.xlimits = np.array(lin_tdm.padded_xlimits, dtype=np.float64)
+        self.ylimits = np.array(lin_tdm.padded_ylimits, dtype=np.float64)
+        self._grids = [DeviceTractionGrid(self, i) for i in range(int(count.value))]
+
+    def __del__(self):
+        h, self._handle = getattr(self, "_handle", None), None
+        if h:
+            try:
+                lib.b200mppi_realisations_destroy(h)
+            except Exception:
+                pass
+
+    def __len__(self):
+        return len(self._grids)
+
+    def __getitem__(self, i):
+        return self._grids[i]
+
+    def __iter__(self):
+        return iter(self._grids)
+
+
+def draw_traction_grids(lin_tdm, ang_tdm, count):
+    """``count`` ground-truth realisations of the TDM pair, drawn and kept on the GPU: realisation i equals
+    ``TractionGrid(lin.astype(np.float64), ang.astype(np.float64), lin_tdm.res, xlimits=lin_tdm.padded_xlimits,
+    ylimits=lin_tdm.padded_ylimits)`` for the (lin, ang) of the i-th call of the reference notebook's
+    ``sample_traction_grid(lin_tdm, ang_tdm)`` (``sample_grids()`` of each TDM, map 0 as ``q * (hi - lo) / 100.0 + lo``
+    in float32), and both TDMs end as after those calls.  ``lin_tdm`` may be ``ang_tdm``.  Returns a
+    DeviceTractionGrids.  Raises ValueError for count < 1, a TDM whose PMF is not set and TDMs on different devices."""
+    count = int(count)
+    if count < 1:
+        raise ValueError("draw_traction_grids: count %d < 1" % count)
+    for name, t in (("lin_tdm", lin_tdm), ("ang_tdm", ang_tdm)):
+        if not t.pmf_grid_initialized:
+            raise ValueError("draw_traction_grids: %s has no PMF grid set" % name)
+    if lin_tdm.device != ang_tdm.device:
+        raise ValueError("draw_traction_grids: lin_tdm is on device %d, ang_tdm on device %d"
+                         % (lin_tdm.device, ang_tdm.device))
+    h = C.c_void_p()
+    check(lib.b200mppi_tdm_draw_realisations(lin_tdm._handle, ang_tdm._handle, count, C.byref(h)))
+    return DeviceTractionGrids(h, lin_tdm)
