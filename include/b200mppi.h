@@ -526,9 +526,9 @@ int b200mppi_batch_run_barebone_trials(b200mppi_batch* b, const b200mppi_trial_d
                                        int32_t* contact_steps, int32_t* steps_issued);
 
 /* ------------------------------------------------------------------ closed-loop trials with visualisation records
- * One of the three trial calls above (kind: B200MPPI_TRIALS_MAP = b200mppi_batch_run_trials, _STOCHASTIC =
- * b200mppi_batch_run_stochastic_trials, _BAREBONE = b200mppi_batch_run_barebone_trials; contact_steps as that call
- * takes it, NULL for the first two) that also records the visualisation rollouts of every step s with
+ * One of the trial calls above (kind: B200MPPI_TRIALS_MAP = b200mppi_batch_run_trials, _STOCHASTIC =
+ * b200mppi_batch_run_stochastic_trials, _BAREBONE = b200mppi_batch_run_barebone_trials, _MIXED =
+ * b200mppi_batch_run_mixed_trials below; contact_steps as that call takes it, NULL for all but barebone) that also records the visualisation rollouts of every step s with
  * s % record_every == 0, as a host loop calling b200mppi_planner_get_state_rollout after solve() and the plant step and
  * before shift_and_update records them: u_cur and x0 of that step's solve.  Everything else -- episodes, results,
  * histories and the state every planner is left in -- is that call's, bit for bit; in addition each planner's
@@ -538,14 +538,14 @@ int b200mppi_batch_run_barebone_trials(b200mppi_batch* b, const b200mppi_trial_d
  *             in device memory during the call; at the end each written record is copied into rollouts once, and the
  *             rest are set to NaN on the host.
  * Launches: one more per recorded step (the batched visualisation rollouts, before the plant step), and for a
- * stochastic batch one more per launch class: a whole-map sampling of maps [0, V) for every pair whose step sampled a
+ * batch holding MODE_TDM planners one more per stochastic launch class: a whole-map sampling of maps [0, V) for every pair whose step sampled a
  * reach box,
  * from that step's pre-call generator states (the maps the rollouts read; no generator state changes, maps >= V keep
  * their box and are completed by any later reader, as after the host loop).
  * Refused (B200MPPI_EINVAL naming the planner) before any work is issued: what the chosen call refuses, an unknown kind,
  * record_every < 1, a NULL rollouts or a wrong rollout_bytes, unequal num_vis_state_rollouts and V larger than a
  * planner's M (MODE_TDM) or N. */
-enum { B200MPPI_TRIALS_MAP = 0, B200MPPI_TRIALS_STOCHASTIC = 1, B200MPPI_TRIALS_BAREBONE = 2 };
+enum { B200MPPI_TRIALS_MAP = 0, B200MPPI_TRIALS_STOCHASTIC = 1, B200MPPI_TRIALS_BAREBONE = 2, B200MPPI_TRIALS_MIXED = 3 };
 int b200mppi_batch_run_trials_recorded(b200mppi_batch* b, int32_t kind, const b200mppi_trial_desc* trials,
                                        int32_t max_steps, double* xhist, float* uhist, b200mppi_trial_result* results,
                                        int32_t* contact_steps, int32_t record_every, float* rollouts,
@@ -568,7 +568,8 @@ int b200mppi_batch_run_trials_recorded(b200mppi_batch* b, int32_t kind, const b2
  * Afterwards every planner, its TDMs and its params are as after that host loop of all its run episodes: the reach
  * slots, sample box and the samplings of shared pairs follow its total steps, and the C-side params keep the x0 of the
  * last solve.
- *   kind        : B200MPPI_TRIALS_MAP or B200MPPI_TRIALS_STOCHASTIC, for the batches those calls take.
+ *   kind        : B200MPPI_TRIALS_MAP, B200MPPI_TRIALS_STOCHASTIC or B200MPPI_TRIALS_MIXED, for the batches those
+ *                 calls take.
  *   trials      : sum_k episodes[k] descriptors, the grids uploaded and freed by the call.  episodes: int32 (count).
  *   xhist       : float64 (slots, max_steps+1, 3); uhist: float32 (slots, max_steps, 2); results: slots records; NaN
  *                 after an episode's last step and in every row of an episode that never ran, whose record has steps 0
@@ -578,6 +579,37 @@ int b200mppi_batch_run_trials_recorded(b200mppi_batch* b, int32_t kind, const b2
 int b200mppi_batch_run_trial_sequences(b200mppi_batch* b, int32_t kind, const b200mppi_trial_desc* trials,
                                        const int32_t* episodes, int32_t max_steps, int32_t reset_x0, double* xhist,
                                        float* uhist, b200mppi_trial_result* results, int32_t* steps_issued);
+
+/* ------------------------------------------------------------------ mixed batches
+ * The planners of a method comparison -- MODE_DET_DYN, MODE_SPEED_MAP and MODE_TDM planners on the same environments and
+ * realisations -- solved and run through closed-loop trials in ONE batch, with one step loop, one host poll and one
+ * grid upload per call instead of one per kind.
+ *   create: the one-map planners (MODE_DET_DYN and MODE_SPEED_MAP, in any order) first, then the MODE_TDM planners; one
+ *           device, world_size 1, equal num_steps and num_control_rollouts, equal num_grid_samples among the MODE_TDM
+ *           planners, no planner listed twice.  MODE_BAREBONE planners (b200mppi_batch_run_barebone_trials), a
+ *           one-map planner after a MODE_TDM one and anything batch_create or batch_create_stochastic refuse:
+ *           B200MPPI_EINVAL naming the planner.  Messages name planners by their index in this order.
+ *   Each planner's results and the state it is left in (u, u_prev, noise, costs, weights, RNG streams, its TDMs'
+ *   streams and maps, b200mppi_planner_sample_box, the C-side x0) are, bit for bit, those of the same call on the
+ *   batch of its kind: b200mppi_batch_create of the MODE_DET_DYN planners, of the MODE_SPEED_MAP planners, and
+ *   b200mppi_batch_create_stochastic of the MODE_TDM planners, with the same b200mppi_batch_share_tdms setting.  A TDM
+ *   pair shared by a one-map and a MODE_TDM planner is refused (B200MPPI_EINVAL naming both) before any work.
+ *   b200mppi_batch_solve, get_state_rollout, set_stream, launch_count, share_tdms and destroy take a mixed batch;
+ *   its trials run through b200mppi_batch_run_mixed_trials, b200mppi_batch_run_trials_recorded and
+ *   b200mppi_batch_run_trial_sequences with kind B200MPPI_TRIALS_MIXED.  The other trial calls refuse it, naming
+ *   b200mppi_batch_run_mixed_trials, and the mixed calls refuse every other batch.
+ *   Launches: a batch of one kind issues exactly the launches of the batch of that kind.  Holding both, a trial step at
+ *   num_opt n issues 6 n + 1 + C1 + 2 C2 launches, C1 and C2 the one-map and stochastic sampler launch classes: per
+ *   iteration the one-map noise, noise + controls, one-map rollout, windowed rollout, CVaR and ONE update over all
+ *   planners; per step the sampler classes and ONE plant step.  A recorded step adds 1 + C2.  A solve issues each
+ *   kind's launches and one update per iteration.
+ * b200mppi_batch_run_mixed_trials: b200mppi_batch_run_trials / b200mppi_batch_run_stochastic_trials of every planner
+ * of a mixed batch in one call, one descriptor per planner in the batch's order, with the same outputs and refusals
+ * (those of each planner's kind, a batch that is not mixed). */
+int b200mppi_batch_create_mixed(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out);
+int b200mppi_batch_run_mixed_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps,
+                                    double* xhist, float* uhist, b200mppi_trial_result* results,
+                                    int32_t* steps_issued);
 
 #ifdef __cplusplus
 }

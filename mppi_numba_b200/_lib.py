@@ -56,7 +56,7 @@ class TrialResult(C.Structure):
 
 
 TRIAL_GOAL, TRIAL_MAX_STEPS, TRIAL_LEFT_MAP, TRIAL_NOT_RUN = 1, 2, 3, 4
-TRIALS_MAP, TRIALS_STOCHASTIC, TRIALS_BAREBONE = 0, 1, 2
+TRIALS_MAP, TRIALS_STOCHASTIC, TRIALS_BAREBONE, TRIALS_MIXED = 0, 1, 2, 3
 
 
 def _load():
@@ -132,6 +132,7 @@ def _load():
         "b200mppi_debug_rollout_cta_times": (C.c_int, [I32, P, I32]),
         "b200mppi_batch_create": (C.c_int, [C.POINTER(P), I32, C.POINTER(P)]),
         "b200mppi_batch_create_stochastic": (C.c_int, [C.POINTER(P), I32, C.POINTER(P)]),
+        "b200mppi_batch_create_mixed": (C.c_int, [C.POINTER(P), I32, C.POINTER(P)]),
         "b200mppi_batch_destroy": (C.c_int, [P]),
         "b200mppi_batch_set_stream": (C.c_int, [P, P]),
         "b200mppi_batch_solve": (C.c_int, [P, P]),
@@ -141,6 +142,8 @@ def _load():
                                                            C.POINTER(I32)]),
         "b200mppi_batch_run_trials": (C.c_int, [P, C.POINTER(TrialDesc), I32, P, P, C.POINTER(TrialResult),
                                                 C.POINTER(I32)]),
+        "b200mppi_batch_run_mixed_trials": (C.c_int, [P, C.POINTER(TrialDesc), I32, P, P, C.POINTER(TrialResult),
+                                                      C.POINTER(I32)]),
         "b200mppi_batch_run_barebone_trials": (C.c_int, [P, C.POINTER(TrialDesc), I32, P, P, C.POINTER(TrialResult), P,
                                                          C.POINTER(I32)]),
         "b200mppi_batch_get_state_rollout": (C.c_int, [P, P, SZ]),

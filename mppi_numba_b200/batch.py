@@ -34,6 +34,10 @@ the host.
 ``share_tdms=True`` lets planners share a lin/ang TDM pair (many robots on one map, or one environment solved at several
 cvar_alpha): each shared pair is sampled once per call, and each planner ends as its own call on a private copy of the
 pair would leave it (include/b200mppi.h, planners sharing TDM pairs).
+
+``MPPI_MixedBatch(planners)`` holds det-dynamics, speed-map and use_tdm planners together -- the methods the reference
+benchmark compares -- and runs their solves, trials and trial sequences in one call each, every planner ending as the
+batch of its own kind would leave it (include/b200mppi.h, mixed batches).
 """
 import ctypes as C
 
@@ -87,6 +91,8 @@ class MPPI_Batch(object):
         TDM sharing on."""
         self.planners = planners
         self.kind = kind
+        self.order = list(range(len(planners)))        # the caller's index of each planner, named in refusals
+        self._tdm = [_kind(p)[0] == "tdm" for p in planners]
         self.num_steps = planners[0].num_steps
         self.share_tdms = bool(share_tdms)
         self._handle = None
@@ -105,7 +111,7 @@ class MPPI_Batch(object):
             return
         for i, p in enumerate(self.planners):
             for j, q in enumerate(self.planners[:i]):
-                both = "%s: planners %d and %d" % (name, j, i)
+                both = "%s: planners %d and %d" % ((name,) + tuple(sorted((self.order[j], self.order[i]))))
                 if p.lin_tdm is q.ang_tdm or p.ang_tdm is q.lin_tdm:
                     raise ValueError(both + ": a TDM is lin_tdm of one and ang_tdm of the other (a shared TDM pair "
                                      "must be the same (lin_tdm, ang_tdm) of every planner on it)")
@@ -113,7 +119,7 @@ class MPPI_Batch(object):
                     raise ValueError(both + " share %s (a shared TDM pair must be the same (lin_tdm, ang_tdm) of every "
                                      "planner on it)" % ("lin_tdm but not ang_tdm" if p.lin_tdm is q.lin_tdm
                                                          else "ang_tdm but not lin_tdm"))
-                if self.kind == "tdm" and p.lin_tdm is q.lin_tdm:
+                if self._tdm[i] and p.lin_tdm is q.lin_tdm:
                     a, b = float(q.params.get("alpha_dyn", 1.0)), float(p.params.get("alpha_dyn", 1.0))
                     if a != b:
                         raise ValueError(both + " share a TDM pair but have alpha_dyn %r and %r (a shared pair is "
@@ -146,7 +152,7 @@ class MPPI_Batch(object):
     def _solve(self, name):
         for i, p in enumerate(self.planners):
             if not p.check_solve_conditions():
-                print("{}: planner {}: MPPI solve condition not met. Cannot solve. Return".format(name, i))
+                print("{}: planner {}: MPPI solve condition not met. Cannot solve. Return".format(name, self.order[i]))
                 return None
         self._check_groups(name)
         for p in self.planners:
@@ -175,7 +181,7 @@ class MPPI_Batch(object):
         V = self._vis_count("MPPI_Batch.get_state_rollout")
         for i, p in enumerate(self.planners):
             if not p.params_set:
-                raise ValueError("MPPI_Batch.get_state_rollout: planner %d: MPPI parameters are not set" % i)
+                raise ValueError("MPPI_Batch.get_state_rollout: planner %d: MPPI parameters are not set" % self.order[i])
         for p in self.planners:
             p.move_mppi_task_vars_to_device()
         out = np.empty((len(self.planners), V, self.num_steps + 1, 3), dtype=np.float32)
@@ -187,8 +193,8 @@ class MPPI_Batch(object):
         V = int(self.planners[0].num_vis_state_rollouts)
         for i, p in enumerate(self.planners):
             if int(p.num_vis_state_rollouts) != V:
-                raise ValueError("%s: planner %d has num_vis_state_rollouts %d, planner 0 %d (V must be equal)"
-                                 % (name, i, int(p.num_vis_state_rollouts), V))
+                raise ValueError("%s: planner %d has num_vis_state_rollouts %d, planner %d %d (V must be equal)"
+                                 % (name, self.order[i], int(p.num_vis_state_rollouts), self.order[0], V))
         return V
 
 
@@ -279,10 +285,10 @@ class MPPI_Batch(object):
         keep = []
         for i, (p, g) in enumerate(zip(self.planners, grids)):
             if not p.check_solve_conditions():
-                raise ValueError("%s: planner %d cannot solve (reason printed above)" % (name, i))
+                raise ValueError("%s: planner %d cannot solve (reason printed above)" % (name, self.order[i]))
             if int(p.params["num_opt"]) < 1:
-                raise ValueError("%s: planner %d has num_opt %d < 1" % (name, i, int(p.params["num_opt"])))
-            _fill_desc("%s: planner %d" % (name, i), p, g, dt, descs[i], keep)
+                raise ValueError("%s: planner %d has num_opt %d < 1" % (name, self.order[i], int(p.params["num_opt"])))
+            _fill_desc("%s: planner %d" % (name, self.order[i]), p, g, dt, descs[i], keep)
         for p in self.planners:
             p.move_mppi_task_vars_to_device()
         xhist = np.empty((K, max_steps + 1, 3), dtype=np.float64)
@@ -304,7 +310,7 @@ class MPPI_Batch(object):
         status = [TRIAL_STATUS[r.status] for r in res]
         logs = []
         for i, p in enumerate(self.planners):
-            if self.kind != "tdm":
+            if not self._tdm[i]:
                 p.u_prev_d = p._u_prev_buf             # as each planner's own solve() does (mppi.py:292,362)
             p.params["x0"] = xhist[i, steps[i]].copy()  # shift_and_update(x_next, ...)
             log = _trial_log(res[i], descs[i], barebone)
@@ -352,7 +358,7 @@ class MPPI_Batch(object):
             raise ValueError("%s: %d lists of traction grids for %d planners" % (name, len(seqs), K))
         for i, g in enumerate(seqs):
             if not g:
-                raise ValueError("%s: planner %d: empty list of traction grids" % (name, i))
+                raise ValueError("%s: planner %d: empty list of traction grids" % (name, self.order[i]))
         max_steps = int(max_steps)
         if max_steps < 1:
             raise ValueError("%s: max_steps %d < 1" % (name, max_steps))
@@ -363,11 +369,11 @@ class MPPI_Batch(object):
         keep = []
         for i, p in enumerate(self.planners):
             if not p.check_solve_conditions():
-                raise ValueError("%s: planner %d cannot solve (reason printed above)" % (name, i))
+                raise ValueError("%s: planner %d cannot solve (reason printed above)" % (name, self.order[i]))
             if int(p.params["num_opt"]) < 1:
-                raise ValueError("%s: planner %d has num_opt %d < 1" % (name, i, int(p.params["num_opt"])))
+                raise ValueError("%s: planner %d has num_opt %d < 1" % (name, self.order[i], int(p.params["num_opt"])))
             for e, g in enumerate(seqs[i]):
-                _fill_desc("%s: planner %d, episode %d" % (name, i, e), p, g, dt, descs[first[i] + e], keep)
+                _fill_desc("%s: planner %d, episode %d" % (name, self.order[i], e), p, g, dt, descs[first[i] + e], keep)
         for p in self.planners:
             p.move_mppi_task_vars_to_device()
         slots = int(first[-1])
@@ -375,7 +381,7 @@ class MPPI_Batch(object):
         us = np.empty((slots, max_steps, 2), dtype=np.float32)
         res = (_lib.TrialResult * slots)()
         issued = C.c_int32()
-        kind = _lib.TRIALS_STOCHASTIC if self.kind == "tdm" else _lib.TRIALS_MAP
+        kind = {"tdm": _lib.TRIALS_STOCHASTIC, "mixed": _lib.TRIALS_MIXED}.get(self.kind, _lib.TRIALS_MAP)
         check(lib.b200mppi_batch_run_trial_sequences(self._handle, kind, descs, ptr(E), max_steps, int(bool(reset_x0)),
                                                      ptr(xs), ptr(us), res, C.byref(issued)))
         self.steps_issued = int(issued.value)
@@ -395,7 +401,7 @@ class MPPI_Batch(object):
                          for e in range(n)])
             status.append(st)
             episodes_run[i] = run
-            if self.kind != "tdm":
+            if not self._tdm[i]:
                 p.u_prev_d = p._u_prev_buf             # as each planner's own solve() does (mppi.py:292,362)
             p.params["x0"] = xhist[i, run - 1, steps[i, run - 1]].copy()
         return dict(logs=logs, xhist=xhist, uhist=uhist, steps=steps, status=status, episodes_run=episodes_run)
@@ -518,3 +524,130 @@ class MPPI_StochasticBatch(MPPI_Batch):
         refused."""
         return self._trials("MPPI_StochasticBatch.run_stochastic_trials", lib.b200mppi_batch_run_stochastic_trials,
                             traction_grids, max_steps, dt, record_every, _lib.TRIALS_STOCHASTIC)
+
+
+class MPPI_MixedBatch(MPPI_Batch):
+    """Borrows det-dynamics, speed-map and use_tdm ``planners`` (keeps them alive), in any mix and order, and runs them
+    together: ``solve()``, ``run_trials``, ``run_trial_sequences``, ``get_state_rollout()``, ``launch_count()`` and
+    ``set_stream`` as in MPPI_Batch, one call for all the methods of a comparison instead of one call per kind.
+
+    Every argument and result is in the caller's planner order.  Internally the one-map planners come first, in the
+    caller's order, then the use_tdm planners (``planners`` holds them so, ``order[j]`` is the caller's index of
+    ``planners[j]``).  The trial calls take a ``TractionGrid`` or ``DeviceTractionGrid`` per planner (per episode) and
+    return the dicts of MPPI_Batch.run_trials and run_trial_sequences.
+
+    The contract: each planner's outputs, and the state it is left in (u, u_prev_d alias, noise, costs, weights, RNG
+    streams, its TDMs' maps and generator states, ``sample_box()`` and ``params['x0']``), are bit for bit those of the
+    same call on the batch of its own kind: ``MPPI_Batch`` of the det-dynamics planners, ``MPPI_Batch`` of the
+    speed-map planners, ``MPPI_StochasticBatch`` of the use_tdm planners (``run_stochastic_trials`` for run_trials),
+    each with the same ``share_tdms``, which groups planners exactly as those batches do.
+
+    Raises ValueError, naming the planner(s) in the caller's order, before any work is issued: for what the batch of a
+    planner's kind refuses, barebone planners (MPPI_Batch.run_barebone_trials runs them), world_size > 1, unequal
+    N or T (at construction), unequal num_grid_samples among the use_tdm planners, unequal num_opt, a TDM used by
+    planners of two kinds, and unequal num_vis_state_rollouts when recording or in get_state_rollout().  The library's
+    own refusals raise B200MPPIError as the per-kind batches' do.  A batch of one kind issues exactly the launches of the
+    batch of that kind; with both kinds a trial step at num_opt n issues 6 n + 1 + C1 + 2 C2 launches (C1, C2: the
+    one-map and stochastic sampler launch classes)."""
+
+    def __init__(self, planners, share_tdms=False):
+        planners = list(planners)
+        if not planners:
+            raise ValueError("MPPI_MixedBatch: no planners")
+        kinds = []
+        for i, p in enumerate(planners):
+            kind, ws = _kind(p)
+            if kind == "barebone":
+                raise ValueError("MPPI_MixedBatch: planner %d is a barebone planner (a mixed batch holds det-dynamics, "
+                                 "speed-map and use_tdm planners; MPPI_Batch runs barebone planners)" % i)
+            if kind == "other":
+                raise ValueError("MPPI_MixedBatch: planner %d is neither a det-dynamics, speed-map nor use_tdm planner"
+                                 % i)
+            if ws != 1:
+                raise ValueError("MPPI_MixedBatch: planner %d has world_size %d (a batch holds single-rank planners)"
+                                 % (i, ws))
+            kinds.append(kind)
+        order = [i for i, k in enumerate(kinds) if k != "tdm"] + [i for i, k in enumerate(kinds) if k == "tdm"]
+        for i, p in enumerate(planners):
+            for what, attr in (("num_steps", "num_steps"), ("num_control_rollouts", "num_control_rollouts")):
+                if getattr(p, attr) != getattr(planners[0], attr):
+                    raise ValueError("MPPI_MixedBatch: planner %d has %s %d, planner 0 %d (N and T must be equal)"
+                                     % (i, what, getattr(p, attr), getattr(planners[0], attr)))
+        tdm = [i for i in order if kinds[i] == "tdm"]
+        for i in tdm:
+            if planners[i].num_grid_samples != planners[tdm[0]].num_grid_samples:
+                raise ValueError("MPPI_MixedBatch: planner %d has num_grid_samples %d, planner %d %d (M must be equal)"
+                                 % (i, planners[i].num_grid_samples, tdm[0], planners[tdm[0]].num_grid_samples))
+        self._create([planners[i] for i in order], "mixed", lib.b200mppi_batch_create_mixed, share_tdms)
+        self.order = order
+
+    def _check_groups(self, name):
+        """Equal num_opt and no TDM used by planners of two kinds, then MPPI_Batch's checks."""
+        K = len(self.planners)
+        for i in range(K):
+            p, o = self.planners[i], self.order
+            if int(p.params["num_opt"]) != int(self.planners[0].params["num_opt"]):
+                raise ValueError("%s: planner %d has num_opt %d, planner %d num_opt %d (must be equal)"
+                                 % (name, o[i], int(p.params["num_opt"]), o[0], int(self.planners[0].params["num_opt"])))
+            for j in range(i):
+                q = self.planners[j]
+                if self._tdm[i] != self._tdm[j] and {id(p.lin_tdm), id(p.ang_tdm)} & {id(q.lin_tdm), id(q.ang_tdm)}:
+                    a, b = sorted((o[j], o[i]))
+                    raise ValueError("%s: planners %d and %d share a TDM, but one is a use_tdm planner and the other "
+                                     "is not (a TDM belongs to planners of one kind)" % (name, a, b))
+        super()._check_groups(name)
+
+    def _to_caller(self, a):
+        """Per-planner array or list ``a`` in the batch's order -> the caller's order."""
+        if isinstance(a, np.ndarray):
+            out = np.empty_like(a)
+            out[self.order] = a
+            return out
+        out = [None] * len(a)
+        for j, i in enumerate(self.order):
+            out[i] = a[j]
+        return out
+
+    def _from_caller(self, a):
+        """Per-planner list ``a`` in the caller's order -> the batch's order (other lengths pass through, refused as
+        MPPI_Batch refuses them)."""
+        a = list(a)
+        return [a[i] for i in self.order] if len(a) == len(self.order) else a
+
+    def solve(self):
+        """One solve() of every planner: np.float32 (K, T, 2) in the caller's order, or None (the planner's index and
+        the reason printed) when a planner's preconditions fail -- then nothing is solved."""
+        u = self._solve("MPPI_MixedBatch")
+        if u is None:
+            return None
+        for i, p in enumerate(self.planners):
+            if not self._tdm[i]:
+                p.u_prev_d = p._u_prev_buf             # as each one-map planner's own solve() does (mppi.py:292,362)
+        return self._to_caller(u)
+
+    def get_state_rollout(self):
+        """MPPI_Batch.get_state_rollout in the caller's order: np.float32 (K, V, T+1, 3)."""
+        return self._to_caller(super().get_state_rollout())
+
+    def run_trials(self, traction_grids, max_steps, dt=None, record_every=None):
+        """One closed-loop episode per planner on ``traction_grids[k]``: MPPI_Batch.run_trials for det-dynamics and
+        speed-map planners, MPPI_StochasticBatch.run_stochastic_trials for use_tdm planners, with their arguments,
+        returned dict (in the caller's order), ``record_every`` and refusals."""
+        out = self._trials("MPPI_MixedBatch.run_trials", lib.b200mppi_batch_run_mixed_trials,
+                           self._from_caller(traction_grids), max_steps, dt, record_every, _lib.TRIALS_MIXED)
+        for key in ("logs", "xhist", "uhist", "steps", "status", "state_rollouts"):
+            if key in out:
+                out[key] = self._to_caller(out[key])
+        return out
+
+    def run_trial_sequences(self, traction_grids, max_steps, dt=None, reset_x0=False):
+        """MPPI_Batch.run_trial_sequences for every planner, each by its kind; lists and the returned dict in the
+        caller's order."""
+        out = super().run_trial_sequences(self._from_caller(traction_grids), max_steps, dt, reset_x0)
+        for key in ("logs", "xhist", "uhist", "steps", "status", "episodes_run"):
+            out[key] = self._to_caller(out[key])
+        return out
+
+    def run_barebone_trials(self, max_steps, dt=None, record_every=None):
+        raise ValueError("MPPI_MixedBatch.run_barebone_trials: a mixed batch holds no barebone planners (MPPI_Batch "
+                         "runs barebone trials)")

@@ -2107,6 +2107,14 @@ struct b200mppi_batch {
   // [RolloutParams K | VisBatchDesc K] from off_vis, vis_bytes long
   size_t off_vis = 0, off_visd = 0, vis_bytes = 0;
   bool share = false;                  // b200mppi_batch_share_tdms: planners on one TDM pair sample it once per call
+  // the one-map planners are pl[0 .. nmap), the MODE_TDM planners pl[nmap .. K): nmap is K in a one-map batch, 0 in a
+  // stochastic one.  A mixed batch (b200mppi_batch_create_mixed) holds both, and its descriptors both sections:
+  // [NoiseDesc nmap | SampleGridsV2Args nmap | RolloutArgs nmap | NoisePrepDesc | RolloutWinArgs | CUtensorMap 4x |
+  //  CvarDesc (K - nmap each) | UpdateBatchDesc K]; its mode is the one-map planners' mode, ROLLOUT_MODE_PER_DESC when
+  // they mix MODE_DET_DYN and MODE_SPEED_MAP
+  bool mixed = false;
+  int nmap = 0;
+  size_t off_nprep = 0;
 };
 
 static size_t align256(size_t v) { return (v + 255) / 256 * 256; }
@@ -2125,17 +2133,14 @@ extern "C" int b200mppi_batch_destroy(b200mppi_batch* b) {
 }
 
 static int batch_init(b200mppi_batch* b) {
-  const size_t K = b->pl.size();
-  if (b->stochastic) {
-    b->off_win = align256(K * sizeof(NoisePrepDesc));
-    b->off_tm = b->off_win + align256(K * sizeof(RolloutWinArgs));
-    b->off_cvar = b->off_tm + align256(K * sizeof(b200mppi_planner::tmaps));
-    b->off_upd = b->off_cvar + align256(K * sizeof(CvarDesc));
-  } else {
-    b->off_sample = align256(K * sizeof(NoiseDesc));
-    b->off_roll = b->off_sample + align256(K * sizeof(SampleGridsV2Args));
-    b->off_upd = b->off_roll + align256(K * sizeof(RolloutArgs));
-  }
+  const size_t K = b->pl.size(), K1 = b->nmap, K2 = K - K1;   // empty sections take no bytes
+  b->off_sample = align256(K1 * sizeof(NoiseDesc));
+  b->off_roll = b->off_sample + align256(K1 * sizeof(SampleGridsV2Args));
+  b->off_nprep = b->off_roll + align256(K1 * sizeof(RolloutArgs));
+  b->off_win = b->off_nprep + align256(K2 * sizeof(NoisePrepDesc));
+  b->off_tm = b->off_win + align256(K2 * sizeof(RolloutWinArgs));
+  b->off_cvar = b->off_tm + align256(K2 * sizeof(b200mppi_planner::tmaps));
+  b->off_upd = b->off_cvar + align256(K2 * sizeof(CvarDesc));
   b->desc_bytes = b->off_upd + align256(K * sizeof(UpdateBatchDesc));
   b->off_vis = b->desc_bytes;
   b->off_visd = b->off_vis + align256(K * sizeof(RolloutParams));
@@ -2152,9 +2157,13 @@ static int batch_init(b200mppi_batch* b) {
 }
 
 // One-map batches hold MODE_DET_DYN, MODE_SPEED_MAP or MODE_BAREBONE planners of one mode; stochastic batches hold
-// MODE_TDM planners of equal M.  Both hold single-rank planners of one device, T and N.
-static int batch_create(b200mppi_planner* const* planners, int32_t count, bool stochastic, b200mppi_batch** out) {
-  const std::string fn = stochastic ? "batch_create_stochastic" : "batch_create";
+// MODE_TDM planners of equal M; mixed batches hold MODE_DET_DYN and MODE_SPEED_MAP planners in any order, then MODE_TDM
+// planners of equal M.  All hold single-rank planners of one device, T and N.
+enum class BatchKind { onemap, stochastic, mixed };
+
+static int batch_create(b200mppi_planner* const* planners, int32_t count, BatchKind kind, b200mppi_batch** out) {
+  const bool stochastic = kind == BatchKind::stochastic, mixed = kind == BatchKind::mixed;
+  const std::string fn = stochastic ? "batch_create_stochastic" : mixed ? "batch_create_mixed" : "batch_create";
   if (!planners || !out) return fail(B200MPPI_EINVAL, fn + ": null argument");
   if (count < 1) return fail(B200MPPI_EINVAL, fn + ": count < 1");
   if (count > 65535) return fail(B200MPPI_EINVAL, fn + ": more than 65535 planners");
@@ -2167,7 +2176,13 @@ static int batch_create(b200mppi_planner* const* planners, int32_t count, bool s
     if (stochastic && p->cfg.mode != B200MPPI_MODE_TDM)
       return fail(B200MPPI_EINVAL, who + " has mode " + std::to_string(p->cfg.mode) +
                                        " (a stochastic batch holds MODE_TDM planners)");
-    if (!stochastic && p->cfg.mode == B200MPPI_MODE_TDM)
+    if (mixed && p->cfg.mode == B200MPPI_MODE_BAREBONE)
+      return fail(B200MPPI_EINVAL, who + " is MODE_BAREBONE (a mixed batch holds MODE_DET_DYN, MODE_SPEED_MAP and "
+                                         "MODE_TDM planners; barebone planners run in b200mppi_batch_create batches)");
+    if (mixed && i > 0 && planners[i - 1]->cfg.mode == B200MPPI_MODE_TDM && p->cfg.mode != B200MPPI_MODE_TDM)
+      return fail(B200MPPI_EINVAL, who + " has mode " + std::to_string(p->cfg.mode) + " after a MODE_TDM planner (a "
+                                         "mixed batch takes its one-map planners first, then its MODE_TDM planners)");
+    if (kind == BatchKind::onemap && p->cfg.mode == B200MPPI_MODE_TDM)
       return fail(B200MPPI_EINVAL, who + " is MODE_TDM: the stochastic mode is not batched (batches hold "
                                          "MODE_DET_DYN, MODE_SPEED_MAP or MODE_BAREBONE planners)");
     if (p->cfg.world_size != 1)
@@ -2177,7 +2192,7 @@ static int batch_create(b200mppi_planner* const* planners, int32_t count, bool s
     if (p->cfg.device != q->cfg.device)
       return fail(B200MPPI_EINVAL, who + " is on device " + std::to_string(p->cfg.device) + ", planner 0 on device " +
                                        std::to_string(q->cfg.device));
-    if (!stochastic && p->cfg.mode != q->cfg.mode)
+    if (kind == BatchKind::onemap && p->cfg.mode != q->cfg.mode)
       return fail(B200MPPI_EINVAL, who + " has mode " + std::to_string(p->cfg.mode) + ", planner 0 mode " +
                                        std::to_string(q->cfg.mode) + " (modes cannot be mixed)");
     if (p->T != q->T) return fail(B200MPPI_EINVAL, who + " has num_steps " + std::to_string(p->T) + ", planner 0 " +
@@ -2185,9 +2200,11 @@ static int batch_create(b200mppi_planner* const* planners, int32_t count, bool s
     if (p->n_local != q->n_local)
       return fail(B200MPPI_EINVAL, who + " has num_control_rollouts " + std::to_string(p->n_local) + ", planner 0 " +
                                        std::to_string(q->n_local) + " (N must be equal)");
-    if (stochastic && p->M != q->M)
-      return fail(B200MPPI_EINVAL, who + " has num_grid_samples " + std::to_string(p->M) + ", planner 0 " +
-                                       std::to_string(q->M) + " (M must be equal)");
+    int t = 0;                                         // the batch's first MODE_TDM planner
+    while (planners[t]->cfg.mode != B200MPPI_MODE_TDM && t < i) ++t;
+    if (p->cfg.mode == B200MPPI_MODE_TDM && p->M != planners[t]->M)
+      return fail(B200MPPI_EINVAL, who + " has num_grid_samples " + std::to_string(p->M) + ", planner " +
+                                       std::to_string(t) + " " + std::to_string(planners[t]->M) + " (M must be equal)");
   }
   // any M a planner can have (planner_create: at most cvar_max_maps()).  Index ranges at the largest batch, 65535
   // planners of 16384 maps: the windowed rollout's count * M (planner, map) units stay below 2^30 (an int), its chunk
@@ -2199,7 +2216,11 @@ static int batch_create(b200mppi_planner* const* planners, int32_t count, bool s
   b->device = planners[0]->cfg.device; b->mode = planners[0]->cfg.mode;
   b->T = planners[0]->T; b->N = planners[0]->n_local;
   b->stochastic = stochastic;
-  if (stochastic) b->M = planners[0]->M;
+  b->mixed = mixed;
+  while (b->nmap < count && planners[b->nmap]->cfg.mode != B200MPPI_MODE_TDM) ++b->nmap;
+  for (int i = 1; i < b->nmap; ++i)
+    if (planners[i]->cfg.mode != b->mode) b->mode = ROLLOUT_MODE_PER_DESC;
+  if (b->nmap < count) b->M = planners[b->nmap]->M;
   const int rc = batch_init(b);
   if (rc) {
     const std::string keep = g_err;
@@ -2212,14 +2233,20 @@ static int batch_create(b200mppi_planner* const* planners, int32_t count, bool s
 }
 
 extern "C" int b200mppi_batch_create(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out) {
-  return batch_create(planners, count, false, out);
+  return batch_create(planners, count, BatchKind::onemap, out);
 }
 
 // K independent MODE_TDM planners of equal N, T and M solved with one launch per stage (noise + controls, windowed
 // rollout, CVaR, update); the map sampling stays per planner (each planner's reach box is its own).  The results are
 // those of K solve() calls in planner order, bit for bit (include/b200mppi.h).
 extern "C" int b200mppi_batch_create_stochastic(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out) {
-  return batch_create(planners, count, true, out);
+  return batch_create(planners, count, BatchKind::stochastic, out);
+}
+
+// MODE_DET_DYN and MODE_SPEED_MAP planners, then MODE_TDM planners, of equal N and T: each kind's stages as in its own
+// batch, one update launch over all K planners (include/b200mppi.h)
+extern "C" int b200mppi_batch_create_mixed(b200mppi_planner* const* planners, int32_t count, b200mppi_batch** out) {
+  return batch_create(planners, count, BatchKind::mixed, out);
 }
 
 extern "C" int b200mppi_batch_set_stream(b200mppi_batch* b, void* s) {
@@ -2242,9 +2269,10 @@ extern "C" int b200mppi_batch_share_tdms(b200mppi_batch* b, int32_t enable) {
   return B200MPPI_OK;
 }
 
-// The batch's TDM groups for one call: with sharing on, planners with the same (lin, ang) objects form one group (in the
-// order of their first members); otherwise, and in barebone batches, every planner is a group of its own.  Group g's
-// planners are members[first[g] .. first[g + 1]), in planner order; per group, plans, launches and commits run once.
+// The TDM groups of the batch's planners [lo, hi) (one kind: the one-map or the MODE_TDM planners) for one call: with
+// sharing on, planners with the same (lin, ang) objects form one group (in the order of their first members); otherwise,
+// and in barebone batches, every planner is a group of its own.  Group g's planners are members[first[g] .. first[g + 1]),
+// in planner order, counted from lo (the index of the kind's launches); per group, plans, launches and commits run once.
 struct TdmGroups {
   std::vector<int> of;                 // planner -> group
   std::vector<int> first;              // G + 1 offsets into members
@@ -2255,16 +2283,17 @@ struct TdmGroups {
   bool shared() const { return (int)members.size() > size(); }
 };
 
-static TdmGroups batch_groups(const b200mppi_batch* b) {
-  const int K = (int)b->pl.size();
+static TdmGroups batch_groups(const b200mppi_batch* b, int lo, int hi) {
+  b200mppi_planner* const* pl = b->pl.data() + lo;
+  const int K = hi - lo;
   TdmGroups gr;
   gr.of.assign(K, -1);
   std::vector<std::vector<int>> g;
   for (int i = 0; i < K; ++i) {
-    const b200mppi_planner* p = b->pl[i];
+    const b200mppi_planner* p = pl[i];
     if (b->share && b->mode != B200MPPI_MODE_BAREBONE)
       for (int j = 0; j < i && gr.of[i] < 0; ++j)
-        if (b->pl[j]->lin == p->lin && b->pl[j]->ang == p->ang) gr.of[i] = gr.of[j];
+        if (pl[j]->lin == p->lin && pl[j]->ang == p->ang) gr.of[i] = gr.of[j];
     if (gr.of[i] < 0) { gr.of[i] = (int)g.size(); g.emplace_back(); }
     g[gr.of[i]].push_back(i);
   }
@@ -2274,6 +2303,11 @@ static TdmGroups batch_groups(const b200mppi_batch* b) {
     gr.first.push_back((int)gr.members.size());
   }
   return gr;
+}
+
+static const char* mode_name(int mode) {
+  return mode == B200MPPI_MODE_DET_DYN ? "MODE_DET_DYN" : mode == B200MPPI_MODE_SPEED_MAP ? "MODE_SPEED_MAP" :
+         mode == B200MPPI_MODE_BAREBONE ? "MODE_BAREBONE" : "MODE_TDM";
 }
 
 // Everything a batch solve checks before it issues any work.
@@ -2309,6 +2343,10 @@ static int batch_validate(b200mppi_batch* b) {
       if ((p->lin == q->lin) != (p->ang == q->ang))
         return fail(B200MPPI_EINVAL, both + " share " + (p->lin == q->lin ? "lin but not ang" : "ang but not lin") +
                                          " (a shared TDM pair must be the same (lin, ang) of every planner on it)");
+      if ((p->lin == q->lin || p->ang == q->ang) && (i < b->nmap) != (j < b->nmap))
+        return fail(B200MPPI_EINVAL, both + " share a TDM pair, but planner " + std::to_string(j) + " is " +
+                                         mode_name(q->cfg.mode) + " and planner " + std::to_string(i) + " " +
+                                         mode_name(p->cfg.mode) + " (a pair is shared by planners of one kind)");
       if (p->lin == q->lin && sample_alpha(p) != sample_alpha(q))
         return fail(B200MPPI_EINVAL, both + " share a TDM pair but have alpha_dyn " + std::to_string(sample_alpha(q)) +
                                          " and " + std::to_string(sample_alpha(p)) +
@@ -2392,12 +2430,12 @@ static void fill_update_apply(b200mppi_planner* p, UpdateBatchDesc& u, float* u_
   u.tl.u_out = u_out;
 }
 
-// A one-map batch's noise, rollout and update descriptors at byte offset 0 of `h` (b->h_desc's layout)
+// The one-map planners' noise, rollout and update descriptors at byte offset 0 of `h` (b->h_desc's layout)
 static void onemap_descs(b200mppi_batch* b, unsigned char* h) {
   NoiseDesc* hn = reinterpret_cast<NoiseDesc*>(h);
   RolloutArgs* hr = reinterpret_cast<RolloutArgs*>(h + b->off_roll);
   UpdateBatchDesc* hu = reinterpret_cast<UpdateBatchDesc*>(h + b->off_upd);
-  for (int i = 0; i < (int)b->pl.size(); ++i) {
+  for (int i = 0; i < b->nmap; ++i) {
     b200mppi_planner* p = b->pl[i];
     hn[i] = NoiseDesc{p->states, p->noise, p->prm.u_std[0], p->prm.u_std[1]};
     fill_rollout_args(p, hr[i]);
@@ -2406,60 +2444,55 @@ static void onemap_descs(b200mppi_batch* b, unsigned char* h) {
   }
 }
 
-static int batch_solve_onemap(b200mppi_batch* b) {
-  CU(cudaSetDevice(b->device));
-  const int K = (int)b->pl.size(), T = b->T;
-  cudaStream_t st = b->stream;
-  int rc = batch_wait_members(b);
-  if (rc) return rc;
-  // descriptors, built on the host for this solve and uploaded with ONE copy before the first launch (the sampler's
-  // are decided here too: its host-side preparation may synchronise the stream)
-  onemap_descs(b, b->h_desc);
-  SampleGridsV2Args* hs = reinterpret_cast<SampleGridsV2Args*>(b->h_desc + b->off_sample);
-  const NoiseDesc* dn = reinterpret_cast<const NoiseDesc*>(b->d_desc);
-  const SampleGridsV2Args* ds = reinterpret_cast<const SampleGridsV2Args*>(b->d_desc + b->off_sample);
-  const RolloutArgs* dr = reinterpret_cast<const RolloutArgs*>(b->d_desc + b->off_roll);
-  const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(b->d_desc + b->off_upd);
-  const bool maps = b->mode != B200MPPI_MODE_BAREBONE;
-  const TdmGroups gr = batch_groups(b);
+// A solve's one-map part (planners [0, nmap)): per iteration ONE noise launch, [first iteration: the maps,
+// batch_run_sample] and ONE rollout launch
+struct OnemapSolve {
+  TdmGroups gr;
   std::vector<SamplePlan> plans;
   std::vector<char> joined;
   int nj = 0;
-  if (maps && (rc = batch_plan_sample(b, gr, hs, plans, joined, &nj))) return rc;
-  CU(cudaMemcpyAsync(b->d_desc, b->h_desc, b->desc_bytes, cudaMemcpyHostToDevice, st));
-  const int num_opt = b->pl[0]->prm.num_opt;
-  // the reference samples before its (empty) loop
-  if (num_opt <= 0 && maps && (rc = batch_run_sample(b, gr, hs, ds, plans, joined, nj))) return rc;
-  // solve(): num_opt x (noise, [first iteration: maps], rollout, update)
-  for (int k = 0; k < num_opt; ++k) {
-    launch_sample_noise_batch(dn, K, b->N, T, nullptr, st);
-    b->launches++;
-    CHECK_LAUNCH();
-    for (b200mppi_planner* p : b->pl) p->prepared = false;
-    if (k == 0 && maps && (rc = batch_run_sample(b, gr, hs, ds, plans, joined, nj))) return rc;
-    launch_rollout_batch(dr, K, b->mode, b->N, T, nullptr, st);
-    b->launches++;
-    CHECK_LAUNCH();
-    for (b200mppi_planner* p : b->pl) p->pushed_direct = false;
-    launch_update_partial_batch(du, K, b->pl[0]->num_ctas, nullptr, st);
-    b->launches++;
-    CHECK_LAUNCH();
-  }
+};
+
+// the descriptors and sampler plans, before the solve's one upload
+static int onemap_solve_plan(b200mppi_batch* b, OnemapSolve& os) {
+  onemap_descs(b, b->h_desc);
+  if (b->mode == B200MPPI_MODE_BAREBONE) return B200MPPI_OK;
+  os.gr = batch_groups(b, 0, b->nmap);
+  return batch_plan_sample(b, os.gr, reinterpret_cast<SampleGridsV2Args*>(b->h_desc + b->off_sample), os.plans,
+                           os.joined, &os.nj);
+}
+
+static int onemap_solve_sample(b200mppi_batch* b, OnemapSolve& os) {
+  if (b->mode == B200MPPI_MODE_BAREBONE) return B200MPPI_OK;
+  return batch_run_sample(b, os.gr, reinterpret_cast<const SampleGridsV2Args*>(b->h_desc + b->off_sample),
+                          reinterpret_cast<const SampleGridsV2Args*>(b->d_desc + b->off_sample), os.plans, os.joined,
+                          os.nj);
+}
+
+static int onemap_solve_iteration(b200mppi_batch* b, OnemapSolve& os, int k) {
+  const int K1 = b->nmap;
+  launch_sample_noise_batch(reinterpret_cast<const NoiseDesc*>(b->d_desc), K1, b->N, b->T, nullptr, b->stream);
+  b->launches++;
+  CHECK_LAUNCH();
+  for (int i = 0; i < K1; ++i) b->pl[i]->prepared = false;
+  int rc;
+  if (k == 0 && (rc = onemap_solve_sample(b, os))) return rc;
+  launch_rollout_batch(reinterpret_cast<const RolloutArgs*>(b->d_desc + b->off_roll), K1, b->mode, b->N, b->T, nullptr,
+                       b->stream);
+  b->launches++;
+  CHECK_LAUNCH();
+  for (int i = 0; i < K1; ++i) b->pl[i]->pushed_direct = false;
   return B200MPPI_OK;
 }
 
-// The stochastic batch's solve: per iteration ONE noise + controls launch, [first iteration: every planner's map
-// sampling, in planner order, with the decisions of stage_sample_tdms], ONE windowed rollout launch over all (planner,
-// map) units, ONE CVaR launch and ONE update launch.  The reach statistics of all planners are read back behind one
-// event, so the host waits once.
-// The windowed rollout of every planner of a stochastic batch (its kernel and its encoded tensor maps at the batch's
+// The windowed rollout of every MODE_TDM planner of a batch (its kernel and its encoded tensor maps at the batch's
 // window geometry WW x WH), checked before any work is issued; `fn` prefixes the messages.
 static int stochastic_validate(b200mppi_batch* b, const char* fn, int* WW, int* WH) {
   size_t smem;
   rollout_win_geometry(b->T, WW, WH, &smem);
   *WH = rollout_win_batch_height(b->T);
   CU(cudaSetDevice(b->device));
-  for (int i = 0; i < (int)b->pl.size(); ++i) {
+  for (int i = b->nmap; i < (int)b->pl.size(); ++i) {
     b200mppi_planner* p = b->pl[i];
     const std::string who = std::string(fn) + ": planner " + std::to_string(i);
     // the generic rollout kernel's costs differ from the windowed kernel's in the last bit: no stand-in
@@ -2472,18 +2505,19 @@ static int stochastic_validate(b200mppi_batch* b, const char* fn, int* WW, int* 
   return B200MPPI_OK;
 }
 
-// The per-planner descriptors of a stochastic batch's noise + controls, windowed rollout (+ tensor maps), CVaR and update
-// launches at byte offset 0 of `h` (the layout of b->h_desc); *masks01: every planner's masks are 0 / 1.
+// The MODE_TDM planners' (pl[nmap ..]) descriptors of the noise + controls, windowed rollout (+ tensor maps), CVaR and
+// update launches at byte offset 0 of `h` (the layout of b->h_desc), indexed from nmap except the update's; *masks01:
+// every planner's masks are 0 / 1.
 static void stochastic_descs(b200mppi_batch* b, unsigned char* h, int WW, int WH, bool* masks01) {
-  const int K = (int)b->pl.size(), T = b->T;
-  NoisePrepDesc* hn = reinterpret_cast<NoisePrepDesc*>(h);
+  const int K1 = b->nmap, K2 = (int)b->pl.size() - K1, T = b->T;
+  NoisePrepDesc* hn = reinterpret_cast<NoisePrepDesc*>(h + b->off_nprep);
   RolloutWinArgs* hw = reinterpret_cast<RolloutWinArgs*>(h + b->off_win);
   unsigned char* ht = h + b->off_tm;
   CvarDesc* hc = reinterpret_cast<CvarDesc*>(h + b->off_cvar);
   UpdateBatchDesc* hu = reinterpret_cast<UpdateBatchDesc*>(h + b->off_upd);
   *masks01 = true;
-  for (int i = 0; i < K; ++i) {
-    b200mppi_planner* p = b->pl[i];
+  for (int i = 0; i < K2; ++i) {
+    b200mppi_planner* p = b->pl[K1 + i];
     const b200mppi_params& q = p->prm;
     hn[i] = NoisePrepDesc{p->states, p->noise, p->u_cur, p->noiseT, p->ctrl, p->reach_d, p->reach_slot ^ 1,
                           q.u_std[0], q.u_std[1], q.lambda_weight, q.u_std[0] * q.u_std[0], q.u_std[1] * q.u_std[1],
@@ -2496,84 +2530,130 @@ static void stochastic_descs(b200mppi_batch* b, unsigned char* h, int WW, int WH
     std::memcpy(ht + (size_t)i * sizeof(b200mppi_planner::tmaps), p->tmaps, sizeof(b200mppi_planner::tmaps));
     hc[i] = CvarDesc{p->costs_nm, p->costs, p->n_local, p->n_local, p->M, cvar_numel(p->M, q.cvar_alpha), nullptr};
     // u_prev stays null: a stochastic solve does not alias it
-    fill_update_apply(p, hu[i], b->u_d + (size_t)i * T * 2, nullptr);
+    fill_update_apply(p, hu[K1 + i], b->u_d + (size_t)(K1 + i) * T * 2, nullptr);
   }
 }
 
-static int batch_solve_stochastic(b200mppi_batch* b) {
-  const int K = (int)b->pl.size(), T = b->T, N = b->N;
-  int WW, WH;
-  int rc = stochastic_validate(b, "batch_solve", &WW, &WH);
-  if (rc) return rc;
+// A solve's stochastic part (planners [nmap, K)): per iteration ONE noise + controls launch, [first iteration: every TDM
+// group's map sampling with the decisions of stage_sample_tdms], ONE windowed rollout launch over all (planner, map)
+// units and ONE CVaR launch.  The reach statistics of all planners are read back behind one event, so the host waits
+// once.
+struct StochasticSolve {
+  int WW = 0, WH = 0;                                  // the window geometry (stochastic_validate)
+  bool masks01 = true;
+  TdmGroups gr;
+  std::vector<SamplePlan> plans;
+  std::vector<b200mppi_planner*> ps;                   // planners by group
+};
+
+// the descriptors and sampler plans, one per TDM group (their host preparation may synchronise the stream), before the
+// solve's one upload
+static int stochastic_solve_plan(b200mppi_batch* b, StochasticSolve& ss) {
+  b200mppi_planner* const* sp = b->pl.data() + b->nmap;
+  const int K2 = (int)b->pl.size() - b->nmap;
+  stochastic_descs(b, b->h_desc, ss.WW, ss.WH, &ss.masks01);
+  ss.gr = batch_groups(b, b->nmap, (int)b->pl.size());
+  const int G = ss.gr.size();
+  ss.plans.resize(G);
+  ss.ps.resize(K2);
+  for (int j = 0; j < K2; ++j) ss.ps[j] = sp[ss.gr.members[j]];
+  for (int g = 0; g < G; ++g) {
+    const b200mppi_planner* p = sp[ss.gr.lead(g)];
+    const int rc = plan_sampling(p->lin, p->ang, sample_alpha(p), b->stream, &ss.plans[g]);
+    if (rc) return rc;
+  }
+  return B200MPPI_OK;
+}
+
+// the sampling of num_opt <= 0: the reference samples before its (empty) loop
+static int stochastic_solve_presample(b200mppi_batch* b, StochasticSolve& ss) {
+  const TdmGroups& gr = ss.gr;
+  std::vector<const float*> reach(ss.ps.size(), nullptr);
+  for (int g = 0; g < gr.size(); ++g) {
+    const int rc = sample_finish_group(&ss.ps[gr.first[g]], &reach[gr.first[g]], gr.count(g), ss.plans[g], false,
+                                       b->stream, &b->launches);
+    if (rc) return rc;
+  }
+  return B200MPPI_OK;
+}
+
+static int stochastic_solve_iteration(b200mppi_batch* b, StochasticSolve& ss, int k) {
+  b200mppi_planner* const* sp = b->pl.data() + b->nmap;
+  const int K2 = (int)b->pl.size() - b->nmap, G = ss.gr.size();
+  const TdmGroups& gr = ss.gr;
+  cudaStream_t st = b->stream;
+  int rc;
+  launch_noise_prepare_batch(reinterpret_cast<const NoisePrepDesc*>(b->d_desc + b->off_nprep), K2, b->N, b->T,
+                             sp[0]->npad, k, nullptr, st);
+  b->launches++;
+  CHECK_LAUNCH();
+  for (int i = 0; i < K2; ++i) {                       // stage_noise
+    sp[i]->reach_slot ^= 1;
+    sp[i]->prepared = true;
+    sp[i]->reach_valid = true;
+  }
+  if (k == 0) {                                        // stage_sample_tdms of every TDM group, one host wait
+    std::vector<char> reads(K2), advanced(G);
+    std::vector<const float*> reach(K2, nullptr);      // by group, as ps
+    bool any = false;
+    for (int i = 0; i < K2; ++i) {
+      b200mppi_planner* p = sp[i];
+      if (!(reads[i] = sample_reads_reach(p))) continue;
+      CU(cudaMemcpyAsync(sample_reach_host(p), p->reach_d + p->reach_slot, sizeof(float), cudaMemcpyDeviceToHost, st));
+      any = true;
+    }
+    if (any) CU(cudaEventRecord(b->ev, st));
+    for (int g = 0; g < G; ++g) {                      // a fused group's advance, if any member waits for its reach
+      bool wait = false;
+      for (int j = gr.first[g]; j < gr.first[g + 1]; ++j) wait = wait || reads[gr.members[j]];
+      if (!wait || !ss.plans[g].fused) continue;
+      launch_plan_advance(ss.plans[g], 0, st);
+      CHECK_LAUNCH();
+      b->launches++;
+      advanced[g] = 1;
+    }
+    if (any) CU(cudaEventSynchronize(b->ev));
+    for (int j = 0; j < K2; ++j) reach[j] = reads[gr.members[j]] ? sample_reach_host(ss.ps[j]) : nullptr;
+    for (int g = 0; g < G; ++g)
+      if ((rc = sample_finish_group(&ss.ps[gr.first[g]], &reach[gr.first[g]], gr.count(g), ss.plans[g],
+                                    advanced[g] != 0, st, &b->launches)))
+        return rc;
+  }
+  CU(launch_rollout_win_batch(*reinterpret_cast<const RolloutWinArgs*>(b->h_desc + b->off_win),
+                              reinterpret_cast<const RolloutWinArgs*>(b->d_desc + b->off_win), b->d_desc + b->off_tm,
+                              K2, ss.masks01, nullptr, st));
+  b->launches++;
+  for (int i = 0; i < K2; ++i) { sp[i]->prepared = false; sp[i]->pushed_direct = false; }
+  launch_cvar_batch(reinterpret_cast<const CvarDesc*>(b->d_desc + b->off_cvar), K2, b->N, b->M, st);
+  b->launches++;
+  CHECK_LAUNCH();
+  return B200MPPI_OK;
+}
+
+// Every batch's solve: num_opt x (the one-map part's launches, the stochastic part's, then ONE update launch over all K
+// planners), each part as described above; a batch of one kind issues only that kind's.  The descriptors of both parts
+// are built on the host for this solve and uploaded with ONE copy from pinned staging before the first launch.
+static int batch_solve_parts(b200mppi_batch* b) {
+  const int K = (int)b->pl.size(), K1 = b->nmap;
+  OnemapSolve os;
+  StochasticSolve ss;
+  int rc;
+  if (K1 < K && (rc = stochastic_validate(b, "batch_solve", &ss.WW, &ss.WH))) return rc;
+  CU(cudaSetDevice(b->device));
   cudaStream_t st = b->stream;
   if ((rc = batch_wait_members(b))) return rc;
-  const RolloutWinArgs* hw = reinterpret_cast<const RolloutWinArgs*>(b->h_desc + b->off_win);
-  bool masks01 = true;
-  stochastic_descs(b, b->h_desc, WW, WH, &masks01);
-  // the sampler plans, one per TDM group (their host preparation may synchronise the stream) before the one upload
-  const TdmGroups gr = batch_groups(b);
-  const int G = gr.size();
-  std::vector<SamplePlan> plans(G);
-  std::vector<b200mppi_planner*> ps(K);                // planners by group
-  for (int j = 0; j < K; ++j) ps[j] = b->pl[gr.members[j]];
-  for (int g = 0; g < G; ++g) {
-    const b200mppi_planner* p = b->pl[gr.lead(g)];
-    if ((rc = plan_sampling(p->lin, p->ang, sample_alpha(p), st, &plans[g]))) return rc;
-  }
+  if (K1 > 0 && (rc = onemap_solve_plan(b, os))) return rc;
+  if (K1 < K && (rc = stochastic_solve_plan(b, ss))) return rc;
   CU(cudaMemcpyAsync(b->d_desc, b->h_desc, b->desc_bytes, cudaMemcpyHostToDevice, st));
-  const NoisePrepDesc* dn = reinterpret_cast<const NoisePrepDesc*>(b->d_desc);
-  const RolloutWinArgs* dw = reinterpret_cast<const RolloutWinArgs*>(b->d_desc + b->off_win);
-  const void* dt = b->d_desc + b->off_tm;
-  const CvarDesc* dc = reinterpret_cast<const CvarDesc*>(b->d_desc + b->off_cvar);
-  const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(b->d_desc + b->off_upd);
   const int num_opt = b->pl[0]->prm.num_opt;
-  std::vector<const float*> reach(K, nullptr);         // by group, as ps
-  if (num_opt <= 0)                                    // the reference samples before its (empty) loop
-    for (int g = 0; g < G; ++g)
-      if ((rc = sample_finish_group(&ps[gr.first[g]], &reach[gr.first[g]], gr.count(g), plans[g], false, st,
-                                    &b->launches)))
-        return rc;
+  if (num_opt <= 0) {                                  // the reference samples before its (empty) loop
+    if (K1 > 0 && (rc = onemap_solve_sample(b, os))) return rc;
+    if (K1 < K && (rc = stochastic_solve_presample(b, ss))) return rc;
+  }
+  const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(b->d_desc + b->off_upd);
   for (int k = 0; k < num_opt; ++k) {
-    launch_noise_prepare_batch(dn, K, N, T, b->pl[0]->npad, k, nullptr, st);
-    b->launches++;
-    CHECK_LAUNCH();
-    for (b200mppi_planner* p : b->pl) {                // stage_noise
-      p->reach_slot ^= 1;
-      p->prepared = true;
-      p->reach_valid = true;
-    }
-    if (k == 0) {                                      // stage_sample_tdms of every TDM group, one host wait
-      std::vector<char> reads(K), advanced(G);
-      bool any = false;
-      for (int i = 0; i < K; ++i) {
-        b200mppi_planner* p = b->pl[i];
-        if (!(reads[i] = sample_reads_reach(p))) continue;
-        CU(cudaMemcpyAsync(sample_reach_host(p), p->reach_d + p->reach_slot, sizeof(float), cudaMemcpyDeviceToHost, st));
-        any = true;
-      }
-      if (any) CU(cudaEventRecord(b->ev, st));
-      for (int g = 0; g < G; ++g) {                    // a fused group's advance, if any member waits for its reach
-        bool wait = false;
-        for (int j = gr.first[g]; j < gr.first[g + 1]; ++j) wait = wait || reads[gr.members[j]];
-        if (!wait || !plans[g].fused) continue;
-        launch_plan_advance(plans[g], 0, st);
-        CHECK_LAUNCH();
-        b->launches++;
-        advanced[g] = 1;
-      }
-      if (any) CU(cudaEventSynchronize(b->ev));
-      for (int j = 0; j < K; ++j) reach[j] = reads[gr.members[j]] ? sample_reach_host(ps[j]) : nullptr;
-      for (int g = 0; g < G; ++g)
-        if ((rc = sample_finish_group(&ps[gr.first[g]], &reach[gr.first[g]], gr.count(g), plans[g], advanced[g] != 0,
-                                      st, &b->launches)))
-          return rc;
-    }
-    CU(launch_rollout_win_batch(hw[0], dw, dt, K, masks01, nullptr, st));
-    b->launches++;
-    for (b200mppi_planner* p : b->pl) { p->prepared = false; p->pushed_direct = false; }
-    launch_cvar_batch(dc, K, N, b->M, st);
-    b->launches++;
-    CHECK_LAUNCH();
+    if (K1 > 0 && (rc = onemap_solve_iteration(b, os, k))) return rc;
+    if (K1 < K && (rc = stochastic_solve_iteration(b, ss, k))) return rc;
     launch_update_partial_batch(du, K, b->pl[0]->num_ctas, nullptr, st);
     b->launches++;
     CHECK_LAUNCH();
@@ -2585,7 +2665,7 @@ extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
   int rc = batch_validate(b);
   if (rc) return rc;
-  if ((rc = b->stochastic ? batch_solve_stochastic(b) : batch_solve_onemap(b))) return rc;
+  if ((rc = batch_solve_parts(b))) return rc;
   const size_t n = (size_t)b->T * 2, ubytes = b->pl.size() * n * sizeof(float);
   if (b->pl[0]->prm.num_opt <= 0)                      // u unchanged
     for (size_t i = 0; i < b->pl.size(); ++i)
@@ -2680,8 +2760,9 @@ extern "C" int b200mppi_batch_get_state_rollout(b200mppi_batch* b, float* out, s
 // planners through pinned memory POLL steps behind the GPU and stops issuing once it reads zero.
 constexpr int TRIAL_POLL = 4;
 
-// one-map (MODE_DET_DYN, MODE_SPEED_MAP), stochastic (MODE_TDM) and barebone (MODE_BAREBONE, no map) trials
-enum class TrialKind { onemap, stochastic, barebone };
+// one-map (MODE_DET_DYN, MODE_SPEED_MAP), stochastic (MODE_TDM), barebone (MODE_BAREBONE, no map) and mixed (one-map
+// and MODE_TDM planners of a b200mppi_batch_create_mixed batch) trials
+enum class TrialKind { onemap, stochastic, barebone, mixed };
 
 // first: planner i's descriptors are tr[first[i] .. first[i + 1]): one each, or (seq) its episodes in a trial sequence
 static int trial_validate(b200mppi_batch* b, TrialKind kind, const b200mppi_trial_desc* tr, int32_t max_steps,
@@ -2766,19 +2847,20 @@ struct TrialClass {
   int mrows = 0, ncact = 0;
 };
 
-// A stochastic batch's trial sampler sets (set0: parity 0), launch classes and per-class launch sizes.  Every pair must
+// The MODE_TDM planners' trial sampler sets (set0: parity 0), launch classes and per-class launch sizes.  Every pair must
 // be fused (identical generator streams, well-formed PMF at its alpha, lin != ang).
 static int stochastic_trial_plans(b200mppi_batch* b, const TdmGroups& gr, const std::string& fn,
                                   std::vector<SamplePlan>& plans, std::vector<SampleGridsV2Args>& set0,
                                   LaunchClasses& lc, std::vector<TrialClass>& cls) {
-  const int K = (int)b->pl.size(), G = gr.size();
+  b200mppi_planner* const* sp = b->pl.data() + b->nmap;   // the MODE_TDM planners; gr counts from there
+  const int K = (int)b->pl.size() - b->nmap, G = gr.size();
   plans.resize(G);
   for (int g = 0; g < G; ++g) {                       // one plan per TDM group
-    b200mppi_planner* p = b->pl[gr.lead(g)];
+    b200mppi_planner* p = sp[gr.lead(g)];
     const int rc = plan_sampling(p->lin, p->ang, sample_alpha(p), b->stream, &plans[g]);
     if (rc) return rc;
     if (!plans[g].fused)
-      return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(gr.lead(g)) + ": its TDM pair cannot join the "
+      return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(b->nmap + gr.lead(g)) + ": its TDM pair cannot join the "
                                    "batch's one sampler launch (lin == ang, or map geometry, PMF or generator streams "
                                    "differ from planner 0's)");
   }
@@ -2791,7 +2873,7 @@ static int stochastic_trial_plans(b200mppi_batch* b, const TdmGroups& gr, const 
   std::vector<double> span(G, -1.0);                  // per pair: cells a side + margin (-1: no planner gets a box)
   for (int i = 0; i < K; ++i) {
     ReachBoxConst c;
-    fill_reach_const(b->pl[i], plans[gr.of[i]], &c);
+    fill_reach_const(sp[i], plans[gr.of[i]], &c);
     if (c.mode == 0) continue;
     const double w = (double)c.cols * (double)c.res, h = (double)c.rows * (double)c.res;
     const double A = std::fmax(std::fabs((double)c.pxl), std::fabs((double)c.pxl + w)) +
@@ -2821,13 +2903,13 @@ static int stochastic_trial_plans(b200mppi_batch* b, const TdmGroups& gr, const 
     std::vector<const SampleGridsV2Args*> mem;
     for (int j = lc.first[c]; j < lc.first[c + 1]; ++j) {
       const int g = lc.groups[j];
-      const b200mppi_tdm* l = b->pl[gr.lead(g)]->lin;
+      const b200mppi_tdm* l = sp[gr.lead(g)]->lin;
       set0[g] = plans[g].a[0];
       set0[g].segs = l->box_segs; set0[g].seg_rows = l->box_seg_rows; set0[g].jump = l->jump_box_d;
       set0[g].write_states = 0;
       set0[g].gm = gm_b;
       if (!sample_box_batch_fits(set0[g], tc.ncact))
-        return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(gr.lead(lc.groups[lc.first[c]])) +
+        return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(b->nmap + gr.lead(lc.groups[lc.first[c]])) +
                                      ": the batched sampler launch (" + std::to_string(tc.ncact) + " tile columns x " +
                                      std::to_string(gm_b) + " maps per CTA) does not fit a CTA");
       mem.push_back(&set0[g]);
@@ -2837,7 +2919,7 @@ static int stochastic_trial_plans(b200mppi_batch* b, const TdmGroups& gr, const 
   return B200MPPI_OK;
 }
 
-// A one-map batch's trial sampler sets (set0: parity 0, each pair's whole-map plan), launch classes and their shapes.
+// The one-map planners' trial sampler sets (set0: parity 0, each pair's whole-map plan), launch classes and their shapes.
 // Every pair must be fused.
 static int onemap_trial_plans(b200mppi_batch* b, const TdmGroups& gr, std::vector<SamplePlan>& plans,
                               std::vector<SampleGridsV2Args>& set0, LaunchClasses& lc, std::vector<TrialClass>& cls) {
@@ -2863,27 +2945,38 @@ static int onemap_trial_plans(b200mppi_batch* b, const TdmGroups& gr, std::vecto
   return B200MPPI_OK;
 }
 
-static const char* mode_name(int mode) {
-  return mode == B200MPPI_MODE_DET_DYN ? "MODE_DET_DYN" : mode == B200MPPI_MODE_SPEED_MAP ? "MODE_SPEED_MAP" :
-         mode == B200MPPI_MODE_BAREBONE ? "MODE_BAREBONE" : "MODE_TDM";
-}
+// The planners of one kind in a trial call: the one-map planners pl[0 .. nmap) or the MODE_TDM planners pl[nmap .. K).
+// Each kind's launches index its planners, groups and classes from lo (`active` too: active + lo).
+struct TrialPart {
+  int lo = 0, n = 0;
+  TdmGroups gr;
+  std::vector<SamplePlan> plans;
+  std::vector<SampleGridsV2Args> set0;                 // parity 0, one per TDM group
+  LaunchClasses lc;
+  std::vector<TrialClass> cls;
+  int G = 0, C = 0;                                    // groups whose pairs are sampled, sampler launch classes
+  bool grouped = false;                                // shared pairs: the group-aware sampler launches
+  size_t off_s0 = 0, off_s1 = 0, off_grp = 0, off_mem = 0, off_cls = 0;
+};
 
 // The closed-loop trials of every kind of batch.  Stochastic trials also move each planner's reach box with the robot;
 // with box_mode 2 and num_opt 1 it depends on the controls drawn, so the batched boxed sampler decides it on the device
 // (reach_box_decide, the function sample_finish calls) and a step needs no host round trip.  Per step: num_opt x
-// (noise [+ controls], [first iteration, not barebone: per launch class the sampler (stochastic: boxed, then the state
-// advance)], rollout [windowed, then CVaR], update) and the plant step, which for stochastic trials also moves each
-// planner's rollout window and for barebone trials counts obstacle contacts.  With C launch classes (launch_classes; 1
-// for a batch on one map geometry) that is 3 num_opt + 1 + C launches per one-map step, 4 num_opt + 1 + 2 C per
-// stochastic step and 3 num_opt + 1 per barebone step.
+// (one-map: noise, [first iteration, not barebone: per launch class the sampler], rollout; stochastic: noise + controls,
+// [first iteration: per launch class the boxed sampler, then the state advance], windowed rollout, CVaR; then ONE
+// update over all K planners) and the plant step, which for stochastic planners also moves the rollout window and for
+// barebone trials counts obstacle contacts.  With C launch classes (launch_classes; 1 for a batch on one map geometry)
+// that is 3 num_opt + 1 + C launches per one-map step, 4 num_opt + 1 + 2 C per stochastic step, 3 num_opt + 1 per
+// barebone step, and 6 num_opt + 1 + C1 + 2 C2 per step of a mixed batch holding both kinds (C1, C2: the one-map and the
+// stochastic classes).
 // record_every = n > 0 records the visualisation rollouts of every step s with s % n == 0, after the step's last update
-// and before the plant step (which shifts u_cur and overwrites x0): one batched launch, and for a stochastic batch first
-// one launch per launch class that completes maps [0, V) of every pair whose step sampled a box (the maps the rollouts
-// read).
-// Device buffer of a call: [descriptors (b->h_desc's layout; a one-map batch's parity-0 sampler set is its own section
-// there) | stochastic: the parity-0 sampler set | not barebone: the parity-1 set | stochastic: box descriptors, box
-// records | shared TDM pairs: group records (stochastic), group descriptors, members | not barebone: the launch classes'
-// pairs | states | barebone: contacts |
+// and before the plant step (which shifts u_cur and overwrites x0): one batched launch, and for stochastic planners first
+// one launch per stochastic launch class that completes maps [0, V) of every pair whose step sampled a box (the maps the
+// rollouts read).
+// Device buffer of a call: [descriptors (b->h_desc's layout; the one-map parity-0 sampler set is its own section there)
+// | stochastic: the parity-0 sampler set, the parity-1 set | one-map, not barebone: the parity-1 set | stochastic: box
+// descriptors, box records | shared TDM pairs: group records (stochastic), group descriptors, members (one-map, then
+// stochastic) | not barebone: the launch classes' pairs | states | barebone: contacts |
 // trials | active K + count | recording: vis descriptors | not barebone: the host grids | recording: the records (K, R,
 // V, T+1, 3) | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds
 // xhist and uhist: the float64 ground-truth grids (tens of MB for a batch of large maps) are copied straight from the
@@ -2898,9 +2991,10 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
                             int32_t record_every, float* rollouts, size_t rollout_bytes, int32_t* steps_issued,
                             const int32_t* episodes, int32_t reset_x0) {
   const bool stochastic = kind == TrialKind::stochastic, barebone = kind == TrialKind::barebone;
+  const bool mixed = kind == TrialKind::mixed;
   const bool seq = episodes != nullptr;
   const std::string fn = seq ? "run_trial_sequences" : stochastic ? "run_stochastic_trials"
-                         : barebone ? "run_barebone_trials" : "run_trials";
+                         : barebone ? "run_barebone_trials" : mixed ? "run_mixed_trials" : "run_trials";
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
   std::vector<int> first(b->pl.size() + 1, 0);        // planner i's slots: first[i] .. first[i + 1]
   int max_episodes = 1;
@@ -2915,6 +3009,12 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   }
   if ((int64_t)max_episodes * max_steps > INT32_MAX)
     return fail(B200MPPI_EINVAL, fn + ": max_steps x the largest episode count exceeds 2^31 - 1 steps");
+  if (b->mixed && !mixed)
+    return fail(B200MPPI_EINVAL, fn + ": a mixed batch (b200mppi_batch_create_mixed) runs its trials with "
+                                 "b200mppi_batch_run_mixed_trials (kind B200MPPI_TRIALS_MIXED)");
+  if (!b->mixed && mixed)
+    return fail(B200MPPI_EINVAL, fn + ": planner 0 is " + mode_name(b->mode) + " in a batch that is not mixed (mixed "
+                                 "trials run batches made by b200mppi_batch_create_mixed)");
   if (barebone && b->mode != B200MPPI_MODE_BAREBONE)
     return fail(B200MPPI_EINVAL, fn + ": planner 0 is " + mode_name(b->mode) + " (barebone trials run MODE_BAREBONE "
                                  "batches; b200mppi_batch_run_trials and b200mppi_batch_run_stochastic_trials run the "
@@ -2931,6 +3031,7 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   if (!xhist || !uhist || !results || (barebone && !contact_steps))
     return fail(B200MPPI_EINVAL, fn + ": null output buffer");
   const int K = (int)b->pl.size(), T = b->T, N = b->N, S = max_steps, nslot = first[K];
+  const int K1 = b->nmap, K2 = K - K1;                 // the one-map planners, then the MODE_TDM planners
   const bool record = record_every > 0;
   int V = 0, R = 0;
   size_t per = 0, rec_bytes = 0;                       // floats of one planner's record, bytes of all records
@@ -2944,38 +3045,50 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
                                    "(K, R, V, T+1, 3) float32 need " + std::to_string(rec_bytes));
   }
   int WW = 0, WH = 0;
-  if (stochastic && (rc = stochastic_validate(b, fn.c_str(), &WW, &WH))) return rc;
+  if (K2 > 0 && (rc = stochastic_validate(b, fn.c_str(), &WW, &WH))) return rc;
   CU(cudaSetDevice(b->device));
   cudaStream_t st = b->stream;
   // the sampler plans first (their host preparation may synchronise the stream): every TDM group's pair must join the
-  // one launch.  Groups of more than one planner (shared pairs) take the group-aware sampler launches.
-  const TdmGroups gr = batch_groups(b);
-  const int G = gr.size();
-  const bool grouped = !barebone && gr.shared();
-  std::vector<SamplePlan> plans;
-  std::vector<SampleGridsV2Args> set0(K);
-  LaunchClasses lc;
-  std::vector<TrialClass> cls;
-  if (stochastic) {
-    if ((rc = stochastic_trial_plans(b, gr, fn, plans, set0, lc, cls))) return rc;
-  } else if (!barebone) {
-    if ((rc = onemap_trial_plans(b, gr, plans, set0, lc, cls))) return rc;
+  // one launch of its kind.  Groups of more than one planner (shared pairs) take the group-aware sampler launches.
+  TrialPart P[2];                                      // one-map, stochastic
+  P[0].n = K1; P[1].lo = K1; P[1].n = K2;
+  for (TrialPart& q : P) {
+    q.gr = batch_groups(b, q.lo, q.lo + q.n);
+    q.set0.resize(q.n);
   }
-  const int C = barebone ? 0 : lc.size();             // sampler launch classes
+  if (K2 > 0 && (rc = stochastic_trial_plans(b, P[1].gr, fn, P[1].plans, P[1].set0, P[1].lc, P[1].cls))) return rc;
+  if (K1 > 0 && !barebone && (rc = onemap_trial_plans(b, P[0].gr, P[0].plans, P[0].set0, P[0].lc, P[0].cls))) return rc;
+  for (TrialPart& q : P) {
+    if (q.n == 0 || (barebone && &q == &P[0])) continue;
+    q.G = q.gr.size();
+    q.C = q.lc.size();
+    q.grouped = q.gr.shared();
+  }
   if ((rc = batch_wait_members(b))) return rc;
-  const size_t nbox = stochastic ? (size_t)K : 0;      // stochastic-only sections
-  const size_t nset = barebone ? 0 : (size_t)G;        // sections of TDM groups
-  const size_t ncon = barebone ? (size_t)K : 0;        // barebone-only section
-  const size_t ngrp = grouped ? (size_t)G : 0;         // shared pairs: group descriptors, group records, members
-  const size_t off_s0 = stochastic ? b->desc_bytes : b->off_sample;
-  const size_t off_s1 = b->desc_bytes + align256((stochastic ? nset : 0) * sizeof(SampleGridsV2Args));
-  const size_t off_box = off_s1 + align256(nset * sizeof(SampleGridsV2Args));
-  const size_t off_rec = off_box + align256(nbox * sizeof(SampleBoxDesc));
-  const size_t off_grec = off_rec + align256(nbox * 5 * sizeof(int));
-  const size_t off_grp = off_grec + align256(ngrp * 5 * sizeof(int));
+  const size_t ngrec = P[1].grouped ? (size_t)P[1].G : 0;   // stochastic shared pairs' group records
+  const size_t szs = sizeof(SampleGridsV2Args);
+  P[0].off_s0 = b->off_sample;
+  P[1].off_s0 = b->desc_bytes;
+  P[1].off_s1 = P[1].off_s0 + align256(P[1].G * szs);
+  P[0].off_s1 = P[1].off_s1 + align256(P[1].G * szs);
+  const size_t off_box = P[0].off_s1 + align256(P[0].G * szs);
+  const size_t off_rec = off_box + align256((size_t)K2 * sizeof(SampleBoxDesc));
+  const size_t off_grec = off_rec + align256((size_t)K2 * 5 * sizeof(int));
+  size_t off_grp = off_grec + align256(ngrec * 5 * sizeof(int)), ngrp = 0, nmem = 0, ncls = 0;
+  for (TrialPart& q : P) {
+    q.off_grp = ngrp; q.off_mem = nmem; q.off_cls = ncls;     // entries, made byte offsets below
+    if (q.grouped) { ngrp += q.G; nmem += q.n; }
+    ncls += q.G;
+  }
   const size_t off_mem = off_grp + align256(ngrp * sizeof(SampleGroupDesc));
-  const size_t off_cls = off_mem + align256((grouped ? (size_t)K : 0) * sizeof(int));
-  const size_t off_state = off_cls + align256(nset * sizeof(int));
+  const size_t off_cls = off_mem + align256(nmem * sizeof(int));
+  for (TrialPart& q : P) {
+    q.off_grp = off_grp + q.off_grp * sizeof(SampleGroupDesc);
+    q.off_mem = off_mem + q.off_mem * sizeof(int);
+    q.off_cls = off_cls + q.off_cls * sizeof(int);
+  }
+  const size_t ncon = barebone ? (size_t)K : 0;        // barebone-only section
+  const size_t off_state = off_cls + align256(ncls * sizeof(int));
   const size_t off_con = off_state + align256((size_t)K * sizeof(TrialState));
   const size_t nres = seq ? (size_t)nslot : 0;          // sequence-only sections: per-slot results and start poses
   const size_t off_res = off_con + align256(ncon * sizeof(int));
@@ -3013,10 +3126,8 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   unsigned char* d = buf.d;
   unsigned char* h = buf.h;
   bool masks01 = true;
-  if (stochastic) stochastic_descs(b, h, WW, WH, &masks01);
-  else onemap_descs(b, h);
-  SampleGridsV2Args* hs[2] = {reinterpret_cast<SampleGridsV2Args*>(h + off_s0),
-                              reinterpret_cast<SampleGridsV2Args*>(h + off_s1)};
+  if (K1 > 0) onemap_descs(b, h);
+  if (K2 > 0) stochastic_descs(b, h, WW, WH, &masks01);
   SampleBoxDesc* hb = reinterpret_cast<SampleBoxDesc*>(h + off_box);
   TrialState* hst = reinterpret_cast<TrialState*>(h + off_state);
   TrialDev* ht = reinterpret_cast<TrialDev*>(h + off_tr);
@@ -3030,8 +3141,10 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   float* drec = reinterpret_cast<float*>(d + off_vrec);
   for (int i = 0; i < K; ++i) {
     b200mppi_planner* p = b->pl[i];
+    const bool sto = i >= K1;
+    const int r = i - K1;                              // a stochastic planner's index in its kind's launches
     if (record)                                        // x0 from the record the plant step writes
-      hv[i] = vis_desc(p, stochastic ? &dw[i].p : &dr[i].p, drec + (size_t)i * R * per);
+      hv[i] = vis_desc(p, sto ? &dw[r].p : &dr[i].p, drec + (size_t)i * R * per);
     hst[i] = TrialState{};
     for (int c = 0; c < 3; ++c) hst[i].x[c] = trials[first[i]].x0[c];
     hact[i] = 1;
@@ -3053,20 +3166,20 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       t.H = q.height; t.W = q.width;
       t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res;
       t.pxlim[0] = q.pxlim[0]; t.pxlim[1] = q.pxlim[1]; t.pylim[0] = q.pylim[0]; t.pylim[1] = q.pylim[1];
-      if (!stochastic) {
+      if (!sto) {
         t.x0_out = dr[i].p.x0;                         // win stays null: one-map rollouts have no window
         continue;
       }
       const b200mppi_tdm* l = p->lin;
-      t.x0_out = dw[i].p.x0;
-      t.win = &dw[i].WW;
+      t.x0_out = dw[r].p.x0;
+      t.win = &dw[r].WW;
       t.win_pxl = l->pxl[0]; t.win_pyl = l->pyl[0]; t.win_res = l->res; t.win_rows = l->rows; t.win_cols = l->cols;
     }
-    if (!stochastic) continue;
-    reinterpret_cast<CvarDesc*>(h + b->off_cvar)[i].active = dact + i;
-    hb[i] = SampleBoxDesc{{}, dw[i].p.x0, p->reach_d, p->reach_slot ^ 1, reinterpret_cast<int*>(d + off_rec) + 5 * i,
+    if (!sto) continue;
+    reinterpret_cast<CvarDesc*>(h + b->off_cvar)[r].active = dact + i;
+    hb[r] = SampleBoxDesc{{}, dw[r].p.x0, p->reach_d, p->reach_slot ^ 1, reinterpret_cast<int*>(d + off_rec) + 5 * r,
                           p->lin->jump_tile_d};
-    fill_reach_const(p, plans[gr.of[i]], &hb[i].c);
+    fill_reach_const(p, P[1].plans[P[1].gr.of[r]], &hb[r].c);
   }
   TrialState* hres = reinterpret_cast<TrialState*>(h + off_res);
   SeqArgs sa{};
@@ -3084,26 +3197,40 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     sa = SeqArgs{dseq, dseq + K + 1, reinterpret_cast<const double*>(d + off_start),
                  reinterpret_cast<TrialState*>(d + off_res), reset_x0 ? 1 : 0};
   }
-  for (int g = 0; g < (int)nset; ++g) {
-    // parity 1: the pair samples from the buffers parity 0 wrote into
-    hs[0][g] = hs[1][g] = set0[g];
-    for (SampleTdm& td : hs[1][g].t) {
-      uint64_t* in = td.states_out;
-      td.states_out = const_cast<uint64_t*>(td.states);
-      td.states = in;
+  for (TrialPart& q : P) {
+    SampleGridsV2Args* hs0 = reinterpret_cast<SampleGridsV2Args*>(h + q.off_s0);
+    SampleGridsV2Args* hs1 = reinterpret_cast<SampleGridsV2Args*>(h + q.off_s1);
+    for (int g = 0; g < q.G; ++g) {
+      // parity 1: the pair samples from the buffers parity 0 wrote into
+      hs0[g] = hs1[g] = q.set0[g];
+      for (SampleTdm& td : hs1[g].t) {
+        uint64_t* in = td.states_out;
+        td.states_out = const_cast<uint64_t*>(td.states);
+        td.states = in;
+      }
     }
+    SampleGroupDesc* hg = reinterpret_cast<SampleGroupDesc*>(h + q.off_grp);
+    const bool sto = &q == &P[1];
+    for (int g = 0; g < q.G && q.grouped; ++g)
+      hg[g] = SampleGroupDesc{q.gr.first[g], q.gr.count(g), sto ? reinterpret_cast<int*>(d + off_grec) + 5 * g : nullptr};
+    if (q.grouped) std::copy(q.gr.members.begin(), q.gr.members.end(), reinterpret_cast<int*>(h + q.off_mem));
+    std::copy(q.lc.groups.begin(), q.lc.groups.end(), reinterpret_cast<int*>(h + q.off_cls));
   }
-  SampleGroupDesc* hg = reinterpret_cast<SampleGroupDesc*>(h + off_grp);
-  int* hmem = reinterpret_cast<int*>(h + off_mem);
-  for (int g = 0; g < (int)ngrp; ++g)
-    hg[g] = SampleGroupDesc{gr.first[g], gr.count(g), stochastic ? reinterpret_cast<int*>(d + off_grec) + 5 * g : nullptr};
-  if (grouped) std::copy(gr.members.begin(), gr.members.end(), hmem);
-  std::copy(lc.groups.begin(), lc.groups.end(), reinterpret_cast<int*>(h + off_cls));
-  const int* dcls = reinterpret_cast<const int*>(d + off_cls);     // class c's pairs: dcls + lc.first[c]
-  const SampleGroupDesc* dgrp = grouped ? reinterpret_cast<const SampleGroupDesc*>(d + off_grp) : nullptr;
-  const int* dmem = grouped ? reinterpret_cast<const int*>(d + off_mem) : nullptr;
+  // per kind: class c's pairs dcls[k] + lc.first[c], the group descriptors and members (null: no shared pair), and the
+  // sampler sets of each parity
+  const int* dcls[2];
+  const SampleGroupDesc* dgrp[2];
+  const int* dmem[2];
+  const SampleGridsV2Args* ds[2][2];
+  for (int k = 0; k < 2; ++k) {
+    dcls[k] = reinterpret_cast<const int*>(d + P[k].off_cls);
+    dgrp[k] = P[k].grouped ? reinterpret_cast<const SampleGroupDesc*>(d + P[k].off_grp) : nullptr;
+    dmem[k] = P[k].grouped ? reinterpret_cast<const int*>(d + P[k].off_mem) : nullptr;
+    ds[k][0] = reinterpret_cast<const SampleGridsV2Args*>(d + P[k].off_s0);
+    ds[k][1] = reinterpret_cast<const SampleGridsV2Args*>(d + P[k].off_s1);
+  }
   hact[K] = K;
-  const RolloutWinArgs g0 = stochastic ? *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win) : RolloutWinArgs{};
+  const RolloutWinArgs g0 = K2 > 0 ? *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win) : RolloutWinArgs{};
   CU(cudaMemcpyAsync(d, h, head, cudaMemcpyHostToDevice, st));
   for (int j = 0; j < nslot && !barebone; ++j) {      // pageable sources: staged by the driver before the call returns
     if (in_place[j]) continue;
@@ -3111,10 +3238,9 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     CU(cudaMemcpyAsync(d + off_grid[j], trials[j].lin, bytes, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(d + off_grid[j] + bytes, trials[j].ang, bytes, cudaMemcpyHostToDevice, st));
   }
-  const SampleGridsV2Args* ds[2] = {reinterpret_cast<const SampleGridsV2Args*>(d + off_s0),
-                                    reinterpret_cast<const SampleGridsV2Args*>(d + off_s1)};
   const SampleBoxDesc* db = reinterpret_cast<const SampleBoxDesc*>(d + off_box);
   const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(d + b->off_upd);
+  const int* dact2 = dact + K1;                        // the stochastic launches' active flags
   PlantArgs pa{reinterpret_cast<const TrialDev*>(d + off_tr), reinterpret_cast<TrialState*>(d + off_state), dact,
                dact + K, reinterpret_cast<double*>(d + off_xh), reinterpret_cast<float*>(d + off_uh), K, T, S, 0,
                barebone ? reinterpret_cast<int*>(d + off_con) : nullptr};
@@ -3122,6 +3248,9 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   int* hcount = reinterpret_cast<int*>(h);             // the polled counts, in the no longer needed head of the staging
   for (cudaEvent_t& e : buf.ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   const int num_opt = b->pl[0]->prm.num_opt, npad = b->pl[0]->npad;
+  const int C1 = P[0].C, C2 = P[1].C;
+  const LaunchClasses& lc1 = P[0].lc;
+  const LaunchClasses& lc2 = P[1].lc;
   int issued = 0;
   const int last_step = S * max_episodes;
   for (int s = 0; s < last_step; ++s) {
@@ -3130,31 +3259,34 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       if (hcount[s % TRIAL_POLL] == 0) break;
     }
     for (int k = 0; k < num_opt; ++k) {
-      if (stochastic) {
+      if (K1 > 0) {
+        launch_sample_noise_batch(reinterpret_cast<const NoiseDesc*>(d), K1, N, T, dact, st);
+        CHECK_LAUNCH();
+        for (int c = 0; c < C1 && k == 0; ++c) {
+          launch_sample_grids_v2_batch(P[0].cls[c].L, ds[0][s & 1], lc1.count(c), dcls[0] + lc1.first[c], dact, st,
+                                       dgrp[0], dmem[0]);
+          CHECK_LAUNCH();
+        }
+        launch_rollout_batch(dr, K1, b->mode, N, T, dact, st);
+        CHECK_LAUNCH();
+      }
+      if (K2 > 0) {
         const int iter = s * num_opt + k;             // every planner's reach slot toggles once per iteration
-        launch_noise_prepare_batch(reinterpret_cast<const NoisePrepDesc*>(d), K, N, T, npad, iter, dact, st);
+        launch_noise_prepare_batch(reinterpret_cast<const NoisePrepDesc*>(d + b->off_nprep), K2, N, T, npad, iter,
+                                   dact2, st);
         CHECK_LAUNCH();
-        for (int c = 0; c < C && k == 0; ++c) {
-          const TrialClass& tc = cls[c];
-          const SampleGridsV2Args& g0 = set0[lc.groups[lc.first[c]]];
-          launch_sample_grids_v2_box_batch(tc.L, ds[s & 1], db, lc.count(c), dcls + lc.first[c], dact, iter, tc.mrows,
-                                           tc.ncact, st, dgrp, dmem);
+        for (int c = 0; c < C2 && k == 0; ++c) {
+          const TrialClass& tc = P[1].cls[c];
+          const SampleGridsV2Args& g0c = P[1].set0[lc2.groups[lc2.first[c]]];
+          launch_sample_grids_v2_box_batch(tc.L, ds[1][s & 1], db, lc2.count(c), dcls[1] + lc2.first[c], dact2, iter,
+                                           tc.mrows, tc.ncact, st, dgrp[1], dmem[1]);
           CHECK_LAUNCH();
-          launch_advance_states_batch(ds[s & 1], db, lc.count(c), dcls + lc.first[c], g0.tx, g0.ty, g0.num_maps, dact,
-                                      st, dgrp, dmem);
-          CHECK_LAUNCH();
-        }
-        CU(launch_rollout_win_batch(g0, dw, d + b->off_tm, K, masks01, dact, st));
-        launch_cvar_batch(reinterpret_cast<const CvarDesc*>(d + b->off_cvar), K, N, b->M, st);
-        CHECK_LAUNCH();
-      } else {
-        launch_sample_noise_batch(reinterpret_cast<const NoiseDesc*>(d), K, N, T, dact, st);
-        CHECK_LAUNCH();
-        for (int c = 0; c < C && k == 0; ++c) {
-          launch_sample_grids_v2_batch(cls[c].L, ds[s & 1], lc.count(c), dcls + lc.first[c], dact, st, dgrp, dmem);
+          launch_advance_states_batch(ds[1][s & 1], db, lc2.count(c), dcls[1] + lc2.first[c], g0c.tx, g0c.ty,
+                                      g0c.num_maps, dact2, st, dgrp[1], dmem[1]);
           CHECK_LAUNCH();
         }
-        launch_rollout_batch(dr, K, b->mode, N, T, dact, st);
+        CU(launch_rollout_win_batch(g0, dw, d + b->off_tm, K2, masks01, dact2, st));
+        launch_cvar_batch(reinterpret_cast<const CvarDesc*>(d + b->off_cvar), K2, N, b->M, st);
         CHECK_LAUNCH();
       }
       launch_update_partial_batch(du, K, b->pl[0]->num_ctas, dact, st);
@@ -3162,10 +3294,10 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     }
     const bool rec_step = record && s % record_every == 0;
     if (rec_step) {
-      for (int c = 0; c < C && stochastic; ++c) {    // from the pre-call states this step's sampling read
-        const TrialClass& tc = cls[c];
-        launch_sample_grids_v2_complete_batch(tc.L, ds[s & 1], db, lc.count(c), dcls + lc.first[c], dact, V, tc.mrows,
-                                              tc.ncact, st, dgrp, dmem);
+      for (int c = 0; c < C2; ++c) {                  // from the pre-call states this step's sampling read
+        const TrialClass& tc = P[1].cls[c];
+        launch_sample_grids_v2_complete_batch(tc.L, ds[1][s & 1], db, lc2.count(c), dcls[1] + lc2.first[c], dact2, V,
+                                              tc.mrows, tc.ncact, st, dgrp[1], dmem[1]);
         CHECK_LAUNCH();
       }
       launch_state_rollout_batch(reinterpret_cast<const VisBatchDesc*>(d + off_vis), K, V, dact,
@@ -3176,8 +3308,8 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     if (seq) launch_plant_step_seq(pa, sa, st);
     else launch_plant_step(pa, st);
     CHECK_LAUNCH();
-    b->launches += stochastic ? 4 * num_opt + 1 + 2 * C : 3 * num_opt + 1 + C;
-    if (rec_step) b->launches += stochastic ? 1 + C : 1;
+    b->launches += num_opt + 1 + (K1 > 0 ? 2 * num_opt + C1 : 0) + (K2 > 0 ? 3 * num_opt + 2 * C2 : 0);
+    if (rec_step) b->launches += 1 + C2;
     ++issued;
     CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, dact + K, sizeof(int), cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(buf.ev[s % TRIAL_POLL], st));
@@ -3215,9 +3347,9 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     // box and x0 (the samplings of the pair below).  The last solve planned from the pose before the last step -- or,
     // when a later episode of a sequence without reset_x0 took one step, from the previous episode's final pose
     b200mppi_planner* p = b->pl[i];
-    const int* rec = hrec + 5 * i;
     const int n = ran[i];
-    if (stochastic) {
+    if (i >= K1) {
+      const int* rec = hrec + 5 * (i - K1);
       p->reach_slot ^= (n * num_opt) & 1;
       p->reach_valid = true;
       for (int c = 0; c < 5; ++c) p->last_box[c] = rec[c];
@@ -3232,13 +3364,18 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)x0[c];
   }
   // each TDM group's pair as after the samplings of its longest-running member (a group samples at every step while any
-  // member runs), the last one's kind from the group's record (a group of one: its planner's)
-  for (int g = 0; g < G && !barebone; ++g) {
-    int n = 0;
-    for (int j = gr.first[g]; j < gr.first[g + 1]; ++j) n = std::max(n, ran[gr.members[j]]);
-    const int* rec = grouped && stochastic ? reinterpret_cast<const int*>(h + off_grec) + 5 * g : hrec + 5 * gr.lead(g);
-    if (stochastic) plans[g].boxed[0] = plans[g].boxed[1] = rec[0] != 0;
-    for (int s = 0; s < n; ++s) { plan_commit(plans[g], 0); plan_commit(plans[g], 1); }
+  // member runs), a stochastic pair's last kind from the group's record (a group of one: its planner's)
+  for (TrialPart& q : P) {
+    const bool sto = &q == &P[1];
+    for (int g = 0; g < q.G; ++g) {
+      int n = 0;
+      for (int j = q.gr.first[g]; j < q.gr.first[g + 1]; ++j) n = std::max(n, ran[q.lo + q.gr.members[j]]);
+      if (sto) {
+        const int* rec = q.grouped ? reinterpret_cast<const int*>(h + off_grec) + 5 * g : hrec + 5 * q.gr.lead(g);
+        q.plans[g].boxed[0] = q.plans[g].boxed[1] = rec[0] != 0;
+      }
+      for (int s = 0; s < n; ++s) { plan_commit(q.plans[g], 0); plan_commit(q.plans[g], 1); }
+    }
   }
   if (record) {
     // record r belongs to step r * record_every.  Only the written ones are copied (records past a planner's last step
@@ -3273,6 +3410,19 @@ extern "C" int b200mppi_batch_run_stochastic_trials(b200mppi_batch* b, const b20
                           steps_issued, nullptr, 0);
 }
 
+extern "C" int b200mppi_batch_run_mixed_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials, int32_t max_steps,
+                                               double* xhist, float* uhist, b200mppi_trial_result* results,
+                                               int32_t* steps_issued) {
+  return batch_run_trials(b, TrialKind::mixed, trials, max_steps, xhist, uhist, results, nullptr, 0, nullptr, 0,
+                          steps_issued, nullptr, 0);
+}
+
+// the trial kind of B200MPPI_TRIALS_* `kind`
+static TrialKind trial_kind(int32_t kind) {
+  return kind == B200MPPI_TRIALS_STOCHASTIC ? TrialKind::stochastic : kind == B200MPPI_TRIALS_BAREBONE ?
+         TrialKind::barebone : kind == B200MPPI_TRIALS_MIXED ? TrialKind::mixed : TrialKind::onemap;
+}
+
 extern "C" int b200mppi_batch_run_barebone_trials(b200mppi_batch* b, const b200mppi_trial_desc* trials,
                                                   int32_t max_steps, double* xhist, float* uhist,
                                                   b200mppi_trial_result* results, int32_t* contact_steps,
@@ -3287,13 +3437,12 @@ extern "C" int b200mppi_batch_run_trials_recorded(b200mppi_batch* b, int32_t kin
                                                   int32_t record_every, float* rollouts, size_t rollout_bytes,
                                                   int32_t* steps_issued) {
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
-  if (kind != B200MPPI_TRIALS_MAP && kind != B200MPPI_TRIALS_STOCHASTIC && kind != B200MPPI_TRIALS_BAREBONE)
+  if (kind != B200MPPI_TRIALS_MAP && kind != B200MPPI_TRIALS_STOCHASTIC && kind != B200MPPI_TRIALS_BAREBONE &&
+      kind != B200MPPI_TRIALS_MIXED)
     return fail(B200MPPI_EINVAL, "run_trials_recorded: unknown trial kind " + std::to_string(kind));
   if (record_every < 1)
     return fail(B200MPPI_EINVAL, "run_trials_recorded: record_every " + std::to_string(record_every) + " < 1");
-  const TrialKind k = kind == B200MPPI_TRIALS_STOCHASTIC ? TrialKind::stochastic
-                      : kind == B200MPPI_TRIALS_BAREBONE ? TrialKind::barebone : TrialKind::onemap;
-  return batch_run_trials(b, k, trials, max_steps, xhist, uhist, results, contact_steps, record_every, rollouts,
+  return batch_run_trials(b, trial_kind(kind), trials, max_steps, xhist, uhist, results, contact_steps, record_every, rollouts,
                           rollout_bytes, steps_issued, nullptr, 0);
 }
 
@@ -3302,10 +3451,10 @@ extern "C" int b200mppi_batch_run_trial_sequences(b200mppi_batch* b, int32_t kin
                                                   double* xhist, float* uhist, b200mppi_trial_result* results,
                                                   int32_t* steps_issued) {
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
-  if (kind != B200MPPI_TRIALS_MAP && kind != B200MPPI_TRIALS_STOCHASTIC)
+  if (kind != B200MPPI_TRIALS_MAP && kind != B200MPPI_TRIALS_STOCHASTIC && kind != B200MPPI_TRIALS_MIXED)
     return fail(B200MPPI_EINVAL, "run_trial_sequences: trial kind " + std::to_string(kind) + " (sequences run "
-                                 "B200MPPI_TRIALS_MAP or B200MPPI_TRIALS_STOCHASTIC batches)");
+                                 "B200MPPI_TRIALS_MAP, B200MPPI_TRIALS_STOCHASTIC or B200MPPI_TRIALS_MIXED batches)");
   if (!episodes) return fail(B200MPPI_EINVAL, "run_trial_sequences: null episode counts");
-  return batch_run_trials(b, kind == B200MPPI_TRIALS_STOCHASTIC ? TrialKind::stochastic : TrialKind::onemap, trials,
+  return batch_run_trials(b, trial_kind(kind), trials,
                           max_steps, xhist, uhist, results, nullptr, 0, nullptr, 0, steps_issued, episodes, reset_x0);
 }

@@ -386,7 +386,9 @@ struct RolloutArgs {
 };
 // [emu:end rollout_args]
 void launch_rollout(const RolloutArgs& a, cudaStream_t st);
-// batched one-map solves (mode 1, 2, 3): descs = device array of `count` RolloutArgs of equal N and T (blockIdx.y)
+// batched one-map solves (mode 1, 2, 3): descs = device array of `count` RolloutArgs of equal N and T (blockIdx.y).
+// mode ROLLOUT_MODE_PER_DESC: det-dynamics and speed-map planners together, each rolled out in its descriptor's mode
+constexpr int ROLLOUT_MODE_PER_DESC = -1;
 void launch_rollout_batch(const RolloutArgs* descs, int count, int mode, int N, int T, const int* active,
                           cudaStream_t st);
 // windowed (TMA-staged) stochastic rollout kernel -- rollout_win.cu

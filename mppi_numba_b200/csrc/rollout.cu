@@ -210,6 +210,15 @@ __global__ void __launch_bounds__(128) rollout_batch_kernel(const RolloutArgs* _
   if constexpr (MODE == 3) rollout_barebone_body(descs[blockIdx.y]);
   else rollout_body<MODE>(descs[blockIdx.y]);
 }
+
+// mixed batches whose one-map planners mix det dynamics and speed map: each planner's rollout_body of its own mode
+// (descs[y].mode, 1 or 2), gated by `active` as above
+__global__ void __launch_bounds__(128) rollout_batch_mixed_kernel(const RolloutArgs* __restrict__ descs,
+                                                                  const int* __restrict__ active = nullptr) {
+  if (active && !active[blockIdx.y]) return;
+  if (descs[blockIdx.y].mode == 1) rollout_body<1>(descs[blockIdx.y]);
+  else rollout_body<2>(descs[blockIdx.y]);
+}
 // [emu:end rollout_batch]
 void launch_rollout(const RolloutArgs& a, cudaStream_t st) {
   const int threads = 128;
@@ -229,7 +238,8 @@ void launch_rollout_batch(const RolloutArgs* descs, int count, int mode, int N, 
   const int threads = 128;
   const dim3 grid((N + threads - 1) / threads, count);
   const size_t smem = (size_t)2 * T * sizeof(float);
-  if (mode == 1) rollout_batch_kernel<1><<<grid, threads, smem, st>>>(descs, active);
+  if (mode == ROLLOUT_MODE_PER_DESC) rollout_batch_mixed_kernel<<<grid, threads, smem, st>>>(descs, active);
+  else if (mode == 1) rollout_batch_kernel<1><<<grid, threads, smem, st>>>(descs, active);
   else if (mode == 2) rollout_batch_kernel<2><<<grid, threads, smem, st>>>(descs, active);
   else rollout_batch_kernel<3><<<grid, threads, smem, st>>>(descs, active);
 }
