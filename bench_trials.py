@@ -55,6 +55,13 @@ grids on twin planners (histories, steps, statuses and every planner's state bit
 alternating: "host_grids" (the helper's grids, uploaded by each call) and "device_grids" (one shared set, read in
 place); then the draw itself against the helper's sample, copy and convert.  The JSON line adds the grid bytes each call
 uploads, computed from the shapes.
+--episodes E --record-every n (c3, ref, gif) and --workload bb --episodes E [--record-every n]: recorded and barebone
+trial sequences (run_recorded_episodes below).  The parity check runs the benchmark's loop (no reset) with recording
+and replays the host sequence loop on twins with the device's trajectory, calling get_state_rollout() at each episode's
+steps t % n == 0: u[0], every record (NaN where nothing was recorded), bb's contact counts per episode and every
+planner's final state (state_rollout_batch_d included), bit for bit.  Then rounds of the legs, alternating, all with
+reset_x0: "recorded" (one recorded sequence call), "unrecorded" (the same call without recording, on twins; with
+--record-every) and "host" (the drawing host loop: the batch's solve() and, at recorded steps, get_state_rollout()).
 """
 import argparse
 import functools
@@ -676,6 +683,30 @@ def measure(args, emit, host_round, device_round, ba, bb, parity, dev, metric, c
     emit(json.dumps(line))
 
 
+def _bb_params(K):
+    """The bb workload's planner params (run_bb)."""
+    params = []
+    for k in range(K):
+        rng = np.random.default_rng(1000 + k)
+        x0 = np.array([0.0, 0.0, np.pi / 4]) + rng.uniform(-0.3, 0.3, 3)
+        xgoal = x0[:2] + np.array([0.3, 1.2]) if k % 2 == 0 else np.array([7.0, 5.0]) + rng.uniform(-0.3, 0.3, 2)
+        params.append(dict(dt=0.1, x0=x0, xgoal=xgoal, goal_tolerance=0.5, dist_weight=10, lambda_weight=1.0, num_opt=1,
+                           u_std=np.array([1.0, 1.0]), vrange=np.array([0.0, 2.0]), wrange=np.array([-np.pi, np.pi]),
+                           obstacle_positions=np.array([[5.0, 4.5], [2.0, 1.0]]) + rng.uniform(-0.2, 0.2, (2, 2)),
+                           obstacle_radius=np.array([1.5, 1.0]), obs_penalty=1e6))
+    return params
+
+
+def _bb_planners(params):
+    from mppi_numba_b200 import barebone as BB
+    pls = []
+    for k, q in enumerate(params):
+        p = BB.MPPI_Numba(BB.Config(T=5.0, dt=0.1, num_control_rollouts=1000, seed=k + 1))
+        p.setup(q)
+        pls.append(p)
+    return pls
+
+
 def run_bb(args, emit):
     """The bb workload: barebone planners of the notebook's shape (N 1000, T 50, dt 0.1, its two obstacles, vrange
     [0, 2], u_std [1, 1], dist_weight 10, obs_penalty 1e6, goal_tolerance 0.5), planner k with its own seed and seeded
@@ -691,24 +722,8 @@ def run_bb(args, emit):
     K, S = args.batch, args.closed_loop
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    params = []
-    for k in range(K):
-        rng = np.random.default_rng(1000 + k)
-        x0 = np.array([0.0, 0.0, np.pi / 4]) + rng.uniform(-0.3, 0.3, 3)
-        xgoal = x0[:2] + np.array([0.3, 1.2]) if k % 2 == 0 else np.array([7.0, 5.0]) + rng.uniform(-0.3, 0.3, 2)
-        params.append(dict(dt=0.1, x0=x0, xgoal=xgoal, goal_tolerance=0.5, dist_weight=10, lambda_weight=1.0, num_opt=1,
-                           u_std=np.array([1.0, 1.0]), vrange=np.array([0.0, 2.0]), wrange=np.array([-np.pi, np.pi]),
-                           obstacle_positions=np.array([[5.0, 4.5], [2.0, 1.0]]) + rng.uniform(-0.2, 0.2, (2, 2)),
-                           obstacle_radius=np.array([1.5, 1.0]), obs_penalty=1e6))
-
-    def planners():
-        pls = []
-        for k, q in enumerate(params):
-            p = BB.MPPI_Numba(BB.Config(T=5.0, dt=0.1, num_control_rollouts=1000, seed=k + 1))
-            p.setup(q)
-            pls.append(p)
-        return pls
-    A, Bs = planners(), planners()
+    params = _bb_params(K)
+    A, Bs = _bb_planners(params), _bb_planners(params)
     T = A[0].num_steps
 
     def reset(pls):
@@ -781,6 +796,197 @@ def run_bb(args, emit):
                          "the notebook's goal"})
 
 
+def run_recorded_episodes(args, emit):
+    """--episodes E with --record-every n (c3, ref, gif), or --workload bb --episodes E [--record-every n]: E episodes
+    per planner back to back, recording each episode's steps t with t % n == 0 (bb: counting contacts per episode)."""
+    import torch
+    import __graft_entry__
+    __graft_entry__.build_engine()
+    import mppi_numba_b200 as E
+    from bench_batch import gpu_info
+    K, S, n_ep, every = args.batch, args.closed_loop, args.episodes, args.record_every
+    bb = args.workload == "bb"
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    if bb:
+        from tests.barebone_trial_loop import goal_distance, in_contact, obstacles
+        from tests.barebone_trial_loop import plant_step as bb_step
+        params = _bb_params(K)
+        A, Bs, Hs, Cs = (_bb_planners(params) for _ in range(4))
+        Batch, seqs = E.MPPI_Batch, None
+
+        def reset(pls):
+            for p, q in zip(pls, params):
+                p.params["x0"] = q["x0"].copy()
+                p.u_cur_d.copy_to_device(np.zeros((p.num_steps, 2), np.float32))
+
+        def sequences(b, **kw):
+            return b.run_barebone_trial_sequences(n_ep, S, **kw)
+
+        def plant(k, e, x, u, p):
+            return bb_step(x, u, float(p.params["dt"]))
+
+        def stops(p, xn):
+            return goal_distance(p, xn) <= 0
+    else:
+        from tests.scenarios import make_scenario
+        from tests.trial_loop import plant_step, within
+        mode, N, M, T, H, res, B, da = LOCAL_WORKLOADS.get(args.workload) or WORKLOADS[args.workload]
+        W = MAP_WIDTH.get(args.workload, H)
+        scs = []
+        for k in range(K):
+            sc = make_scenario(mode, N=N, M=M, T=T, H=H, W=W, res=res, B=B, seed=k + 1, det_alpha=da, warm_start=True)
+            if args.workload in VIS_ROLLOUTS:
+                sc["cfg"]["num_vis_state_rollouts"] = VIS_ROLLOUTS[args.workload]
+            if k % 2 == 0:
+                sc["params"]["xgoal"] = sc["params"]["x0"][:2] + np.array([1.2, -0.9])
+            scs.append(sc)
+        rng = np.random.default_rng(7)
+        seqs = [[E.TractionGrid(rng.uniform(0.3, 1.0, (H, W)), rng.uniform(0.3, 1.0, (H, W)), res=res)
+                 for _ in range(n_ep)] for _ in range(K)]
+        with _quiet():
+            A, Bs, Hs, Cs = ([make_planner(E, sc, 0)[3] for sc in scs] for _ in range(4))
+        Batch = E.MPPI_StochasticBatch if mode == "tdm" else E.MPPI_Batch
+
+        def reset(pls):
+            for p, sc in zip(pls, scs):
+                p.params["x0"] = sc["params"]["x0"].copy()
+                p.u_cur_d.copy_to_device(sc["u0"])
+
+        def sequences(b, **kw):
+            return b.run_trial_sequences(seqs, S, **kw)
+
+        def plant(k, e, x, u, p):
+            return plant_step(seqs[k][e], x, u, float(p.params["dt"]))
+
+        def stops(p, xn):
+            return np.linalg.norm(xn[:2] - p.params["xgoal"]) - p.params["goal_tolerance"] <= 0 or not within(p, xn)
+    for pls in (A, Bs, Hs, Cs):
+        reset(pls)
+    ba, bh, bc = Batch(A), Batch(Hs), Batch(Cs)
+    rec_kw = {} if every is None else dict(record_every=every)
+
+    # ---- parity: the benchmark's loop (no reset) on the device == the host sequence loop replayed on twins with the
+    # device's trajectory, get_state_rollout() at each episode's recorded steps
+    with _quiet():
+        out = sequences(ba, **rec_kw)
+        ok_u = ok_rec = ok_con = True
+        for k, p in enumerate(Bs):
+            one = Batch([p])
+            for e in range(int(out["episodes_run"][k])):
+                n = int(out["steps"][k, e])
+                for t in range(n):
+                    useq = one.solve()[0]
+                    ok_u &= useq[0].tobytes() == out["uhist"][k, e, t].tobytes()
+                    if every is not None and t % every == 0:
+                        ok_rec &= p.get_state_rollout().tobytes() == out["state_rollouts"][k, e, t // every].tobytes()
+                    p.shift_and_update(out["xhist"][k, e, t + 1], useq, 1)
+                if every is not None:
+                    ok_rec &= bool(np.isnan(out["state_rollouts"][k, e, -(-n // every):]).all())
+                if bb:
+                    ok_con &= int(out["contact_steps"][k, e]) == sum(
+                        in_contact(out["xhist"][k, e, t], obstacles(p)) for t in range(1, n + 1))
+            if every is not None:
+                ok_rec &= bool(np.isnan(out["state_rollouts"][k, int(out["episodes_run"][k]):]).all())
+
+    def state(p):
+        d = [p.u_cur_d, p.u_prev_d, p.costs_d, p.weights_d, p.noise_samples_d, p.rng_states_d]
+        if not bb:
+            d += [p.lin_tdm.rng_states_d, p.ang_tdm.rng_states_d, p.lin_tdm.sample_grid_batch_d,
+                  p.ang_tdm.sample_grid_batch_d]
+        if every is not None:
+            d.append(p.state_rollout_batch_d)
+        return [a.copy_to_host().tobytes() for a in d] + [np.asarray(p.params["x0"]).tobytes()]
+    ok_state = all(state(a) == state(b) for a, b in zip(A, Bs))
+    parity = {"passed": bool(ok_u and ok_state and ok_rec and ok_con), "u_bitwise": bool(ok_u),
+              "state_bitwise": bool(ok_state), "planners": K, "episodes_run": out["episodes_run"].tolist(),
+              "steps": out["steps"].tolist(),
+              "against": "the host sequence loop replayed with the device's trajectory on identical twins"}
+    if every is not None:
+        parity["records_bitwise"] = bool(ok_rec)
+    if bb:
+        parity["contacts_exact"] = bool(ok_con)
+    if not parity["passed"]:
+        sys.stderr.write("bench_trials.py: PARITY CHECK FAILED: %s\n" % json.dumps(parity))
+        emit(json.dumps({"metric": "trial sequences", "error": "parity_check failed", "parity_check": parity}))
+        raise SystemExit(3)
+
+    def device_round(b, pls, **kw):
+        reset(pls)
+        o = sequences(b, reset_x0=True, **kw)
+        torch.cuda.synchronize(dev)
+        return int(o["steps"].sum()), b.steps_issued
+
+    def host_round():                                    # the drawing loop: the batch's solve and get_state_rollout
+        reset(Hs)
+        steps = issued = 0
+        starts = [np.asarray(p.params["x0"], dtype=np.float64).copy() for p in Hs]
+        for e in range(n_ep):
+            x = [s.copy() for s in starts]
+            for p, s in zip(Hs, starts):
+                p.params["x0"] = s.copy()
+            running = list(range(K))
+            for t in range(S):
+                u = bh.solve()
+                issued += 1
+                if every is not None and t % every == 0:
+                    bh.get_state_rollout()
+                still = []
+                for k in running:
+                    p = Hs[k]
+                    xn = plant(k, e, x[k], u[k, 0], p)
+                    p.shift_and_update(xn, u[k], 1)
+                    x[k] = xn
+                    steps += 1
+                    if not stops(p, xn):
+                        still.append(k)
+                running = still
+                if not running:
+                    break
+        torch.cuda.synchronize(dev)
+        return steps, issued
+
+    legs = [("recorded" if every is not None else "sequence", functools.partial(device_round, ba, A, **rec_kw), ba),
+            ("host", host_round, bh)]
+    if every is not None:
+        legs.insert(1, ("unrecorded", functools.partial(device_round, bc, Cs), bc))
+    with _quiet():
+        for _, fn, _ in legs:                            # warm-up of every path
+            fn()
+    res_ = {name: [] for name, _, _ in legs}
+    launches = {}
+    for _ in range(args.rounds):                         # alternate the legs
+        for name, fn, b in legs:
+            l0 = b.launch_count()
+            t0 = time.perf_counter()
+            with _quiet():
+                steps, issued = fn()
+            res_[name].append((time.perf_counter() - t0, steps, issued))
+            launches[name] = b.launch_count() - l0
+
+    def summary(name):
+        wall = [r[0] for r in res_[name]]
+        med = float(np.median(wall))
+        return {"s_per_round_wall": med, "s_per_round_wall_runs": wall, "control_steps_per_round": res_[name][0][1],
+                "steps_issued_per_round": res_[name][0][2], "episodes_per_s": K * n_ep / med,
+                "kernel_launches_per_round": launches[name]}
+    sums = {name: summary(name) for name, _, _ in legs}
+    lead = legs[0][0]
+    config = {"workload": ("bb" if bb else args.workload if args.workload in LOCAL_WORKLOADS
+                           else workload_name_of(args.workload)),
+              "batch": K, "max_steps": S, "episodes": n_ep, "record_every": every,
+              "legs": "reset_x0=True sequences on the device; host: the batch's solve()%s and a numpy plant step per "
+                      "running planner" % (" and get_state_rollout() at recorded steps" if every is not None else "")}
+    line = {"metric": "trial sequences%s: one device call vs the host loop" % (" with records" if every else ""),
+            "unit": "episodes/s", "value": sums[lead]["episodes_per_s"], "higher_is_better": True, "config": config,
+            "rounds": args.rounds, "gpu": gpu_info(dev), "parity_check": parity,
+            "speedup_wall_vs_host": sums["host"]["s_per_round_wall"] / sums[lead]["s_per_round_wall"]}
+    line.update(sums)
+    if every is not None:
+        line["recording_cost_wall"] = sums["recorded"]["s_per_round_wall"] / sums["unrecorded"]["s_per_round_wall"]
+    emit(json.dumps(line))
+
+
 def main():
     # one JSON line on stdout: everything else (the engine's allocation notices, ...) goes to stderr
     real_stdout = os.dup(1)
@@ -800,14 +1006,17 @@ def main():
     ap.add_argument("--share-tdms", action="store_true",
                     help="K planners on one map: K private TDM pairs against one pair shared by all (not bb)")
     ap.add_argument("--episodes", type=int, default=None, metavar="E",
-                    help="E ground-truth realisations per planner back to back (c2, c3, ref)")
+                    help="E ground-truth realisations per planner back to back (c2, c3, ref; with --record-every: "
+                         "c3, ref, gif; bb: E barebone episodes)")
     ap.add_argument("--device-grids", action="store_true",
                     help="with --episodes: the realisations drawn and read on the GPU against host grids (c4, ref)")
     args = ap.parse_args()
     if args.batch < 1 or args.closed_loop < 1 or args.rounds < 1:
         ap.error("--batch, --closed-loop and --rounds must be at least 1")
-    if args.record_every is not None and (args.record_every < 1 or args.workload == "bb"):
-        ap.error("--record-every must be at least 1, and the bb workload does not take it")
+    if args.record_every is not None and args.record_every < 1:
+        ap.error("--record-every must be at least 1")
+    if args.workload == "bb" and args.record_every is not None and args.episodes is None:
+        ap.error("the bb workload takes --record-every only with --episodes")
     if args.share_tdms and args.workload in ("bb", "mix"):
         ap.error("--share-tdms: barebone planners have no TDMs, and mix planners no common map")
     if args.device_grids:
@@ -818,8 +1027,15 @@ def main():
         run_device_grids(args, emit)
         return
     if args.episodes is not None:
-        if args.episodes < 1 or args.workload not in ("c2", "c3", "ref") or args.record_every is not None:
-            ap.error("--episodes must be at least 1, with workload c2, c3 or ref and without --record-every")
+        if args.episodes < 1:
+            ap.error("--episodes must be at least 1")
+        if args.workload == "bb" or args.record_every is not None:
+            if args.share_tdms or (args.workload != "bb" and args.workload not in ("c3", "ref", "gif")):
+                ap.error("--episodes with --record-every takes workload c3, ref or gif (or bb), without --share-tdms")
+            run_recorded_episodes(args, emit)
+            return
+        if args.workload not in ("c2", "c3", "ref"):
+            ap.error("--episodes takes workload c2, c3 or ref (with --record-every: c3, ref, gif; or bb)")
         run_episodes(args, emit)
         return
     (run_bb if args.workload == "bb" else run_shared if args.share_tdms else run)(args, emit)

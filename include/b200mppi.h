@@ -580,6 +580,31 @@ int b200mppi_batch_run_trial_sequences(b200mppi_batch* b, int32_t kind, const b2
                                        const int32_t* episodes, int32_t max_steps, int32_t reset_x0, double* xhist,
                                        float* uhist, b200mppi_trial_result* results, int32_t* steps_issued);
 
+/* b200mppi_batch_run_trial_sequences with every option: b200mppi_batch_run_trial_sequences_ex(..., contact_steps,
+ * record_every, rollouts, rollout_bytes, steps_issued) with contact_steps NULL and record_every 0 is
+ * b200mppi_batch_run_trial_sequences for kinds MAP, STOCHASTIC and MIXED: the same launches, buffers and results.
+ *   kind          : also B200MPPI_TRIALS_BAREBONE: episodes of b200mppi_batch_run_barebone_trials back to back on a
+ *                   MODE_BAREBONE batch, with reset_x0 as above.  Its plant has no map to leave, so every episode runs.
+ *   contact_steps : int32 (slots), per episode the steps whose new pose touched an obstacle: required for barebone
+ *                   sequences, NULL for the other kinds.
+ *   record_every  : 0, or n >= 1: each run episode records at each of its own steps t with t % n == 0 what
+ *                   b200mppi_batch_run_trials_recorded records there.  rollouts: float32 (K, Emax, R, V, T+1, 3),
+ *                   Emax = max_k episodes[k], R = ceil(max_steps / n), rollout_bytes its size; record r of (k, e)
+ *                   belongs to step r n of planner k's episode e, NaN after its last step and everywhere for an
+ *                   episode that did not run or that planner k does not have (e >= episodes[k]).  Each planner's
+ *                   state_rollout ends with the last record of its last run episode.  Whether a planner records at a
+ *                   step is decided on the device, so a recorded sequence issues the record launches (1 + C2, C2 the
+ *                   stochastic sampler launch classes) at every step; everything else is as without recording.
+ * Refused (B200MPPI_EINVAL) before any work is issued: what b200mppi_batch_run_trial_sequences refuses (bar the
+ * barebone kind), record_every < 0, contact_steps missing for barebone or given for another kind, a wrong
+ * rollout_bytes, unequal num_vis_state_rollouts when recording.  A record buffer that cannot be allocated:
+ * B200MPPI_ECUDA, nothing issued. */
+int b200mppi_batch_run_trial_sequences_ex(b200mppi_batch* b, int32_t kind, const b200mppi_trial_desc* trials,
+                                          const int32_t* episodes, int32_t max_steps, int32_t reset_x0, double* xhist,
+                                          float* uhist, b200mppi_trial_result* results, int32_t* contact_steps,
+                                          int32_t record_every, float* rollouts, size_t rollout_bytes,
+                                          int32_t* steps_issued);
+
 /* ------------------------------------------------------------------ mixed batches
  * The planners of a method comparison -- MODE_DET_DYN, MODE_SPEED_MAP and MODE_TDM planners on the same environments and
  * realisations -- solved and run through closed-loop trials in ONE batch, with one step loop, one host poll and one

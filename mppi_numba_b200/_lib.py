@@ -151,6 +151,8 @@ def _load():
                                                          C.POINTER(TrialResult), P, I32, P, SZ, C.POINTER(I32)]),
         "b200mppi_batch_run_trial_sequences": (C.c_int, [P, I32, C.POINTER(TrialDesc), P, I32, I32, P, P,
                                                          C.POINTER(TrialResult), C.POINTER(I32)]),
+        "b200mppi_batch_run_trial_sequences_ex": (C.c_int, [P, I32, C.POINTER(TrialDesc), P, I32, I32, P, P,
+                                                            C.POINTER(TrialResult), P, I32, P, SZ, C.POINTER(I32)]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)          # AttributeError here == ABI drift, fail loudly

@@ -326,7 +326,7 @@ class MPPI_Batch(object):
         return out
 
 
-    def run_trial_sequences(self, traction_grids, max_steps, dt=None, reset_x0=False):
+    def run_trial_sequences(self, traction_grids, max_steps, dt=None, reset_x0=False, record_every=None):
         """Several closed-loop episodes per planner, back to back on the GPU: planner k runs one episode of
         ``run_trials`` (``run_stochastic_trials`` for use_tdm planners) on each grid (``TractionGrid`` or
         ``DeviceTractionGrid``) of the non-empty list ``traction_grids[k]`` in turn, each starting its plant at
@@ -346,8 +346,17 @@ class MPPI_Batch(object):
         (K, Emax, max_steps+1, 3) and ``uhist`` float32 (K, Emax, max_steps, 2), NaN wherever nothing ran; ``steps``
         (K, Emax) int, 0 where nothing ran; ``status``, K lists of E_k of "goal" | "max_steps" | "left_map" |
         "not_run"; ``episodes_run`` (K,) int.  ``steps_issued`` is set as run_trials sets it.
-        Raises ValueError for barebone batches, a list count other than K, an empty list, and whatever run_trials
-        refuses for any of the grids; nothing is issued then."""
+        ``record_every=n`` records, in each run episode at each of its own steps ``t`` with ``t % n == 0``, what
+        run_trials records there (``get_state_rollout()`` after the step's solve and plant step, before
+        ``shift_and_update``); the dict gains ``state_rollouts`` float32 (K, Emax, R, V, T+1, 3), R = ceil(max_steps / n),
+        NaN after an episode's last step and everywhere for an episode that did not run or does not exist, and
+        ``rollout_steps`` (R,) = r n, steps of the episode.  Each planner's state_rollout_batch_d ends with the last
+        record of its last run episode; everything else is as without recording.  Which planners record at a step is
+        decided on the device, so a recorded sequence issues the record launches at every step: 1 + C2 per step more
+        than without recording (C2: the stochastic sampler launch classes, 0 for a batch without use_tdm planners).
+        Raises ValueError for barebone batches (run_barebone_trial_sequences runs them), a list count other than K, an
+        empty list, record_every < 1, unequal num_vis_state_rollouts when recording, and whatever run_trials refuses
+        for any of the grids; nothing is issued then."""
         name = "%s.run_trial_sequences" % type(self).__name__
         if self.kind == "barebone":
             raise ValueError("%s: planner 0 is a barebone planner (trial sequences run det-dynamics, speed-map and "
@@ -359,9 +368,48 @@ class MPPI_Batch(object):
         for i, g in enumerate(seqs):
             if not g:
                 raise ValueError("%s: planner %d: empty list of traction grids" % (name, self.order[i]))
+        kind = {"tdm": _lib.TRIALS_STOCHASTIC, "mixed": _lib.TRIALS_MIXED}.get(self.kind, _lib.TRIALS_MAP)
+        return self._sequences(name, seqs, max_steps, dt, reset_x0, record_every, kind)
+
+    def run_barebone_trial_sequences(self, episodes, max_steps, dt=None, reset_x0=False, record_every=None):
+        """Several episodes of run_barebone_trials per planner, back to back on the GPU: planner k runs ``episodes``
+        (an int, or K ints each >= 1) episodes of the barebone notebook's loop, each starting its plant at
+        ``x_start = params['x0']`` of the call.  Between episodes the planner keeps its warm start and RNG streams;
+        ``reset_x0`` as in run_trial_sequences.  A barebone plant has no map to leave, so every episode runs.
+        Afterwards every planner is exactly as after that host loop (tests/barebone_trial_loop.py per episode).
+        Returns run_trial_sequences' dict with barebone logs (each with its contact_steps), status "goal" |
+        "max_steps", and ``contact_steps`` (K, Emax) int, per episode the steps whose new pose touched an obstacle (0
+        where no episode exists); ``record_every`` as in run_trial_sequences (no completion launches: 1 per step).
+        Raises ValueError (naming the planner) for other batches, an episode count other than K or < 1, and whatever
+        run_barebone_trials refuses; nothing is issued then."""
+        name = "%s.run_barebone_trial_sequences" % type(self).__name__
+        if self.kind != "barebone":
+            raise ValueError("%s: planner 0 is a %s planner (barebone trial sequences run barebone planners; "
+                             "run_trial_sequences runs the others)" % (name, self.kind))
+        K = len(self.planners)
+        counts = [episodes] * K if np.ndim(episodes) == 0 else list(episodes)
+        if len(counts) != K:
+            raise ValueError("%s: %d episode counts for %d planners" % (name, len(counts), K))
+        for i, e in enumerate(counts):
+            if int(e) < 1:
+                raise ValueError("%s: planner %d: episode count %d < 1" % (name, self.order[i], int(e)))
+        return self._sequences(name, [[None] * int(e) for e in counts], max_steps, dt, reset_x0, record_every,
+                               _lib.TRIALS_BAREBONE)
+
+    def _sequences(self, name, seqs, max_steps, dt, reset_x0, record_every, kind):
+        """The marshalling of a trial-sequence call (``seqs``: per planner its grids, None for barebone episodes) through
+        b200mppi_batch_run_trial_sequences, or b200mppi_batch_run_trial_sequences_ex when recording or barebone, and
+        the dict built from its per-slot results; ``name`` prefixes the refusals."""
+        K = len(self.planners)
+        barebone = kind == _lib.TRIALS_BAREBONE
         max_steps = int(max_steps)
         if max_steps < 1:
             raise ValueError("%s: max_steps %d < 1" % (name, max_steps))
+        if record_every is not None:
+            record_every = int(record_every)
+            if record_every < 1:
+                raise ValueError("%s: record_every %d < 1" % (name, record_every))
+            V = self._vis_count(name)
         self._check_groups(name)
         E = np.array([len(g) for g in seqs], dtype=np.int32)
         first = np.concatenate([[0], np.cumsum(E)])
@@ -381,9 +429,19 @@ class MPPI_Batch(object):
         us = np.empty((slots, max_steps, 2), dtype=np.float32)
         res = (_lib.TrialResult * slots)()
         issued = C.c_int32()
-        kind = {"tdm": _lib.TRIALS_STOCHASTIC, "mixed": _lib.TRIALS_MIXED}.get(self.kind, _lib.TRIALS_MAP)
-        check(lib.b200mppi_batch_run_trial_sequences(self._handle, kind, descs, ptr(E), max_steps, int(bool(reset_x0)),
-                                                     ptr(xs), ptr(us), res, C.byref(issued)))
+        contacts = np.zeros(slots, dtype=np.int32)
+        if record_every is None and not barebone:
+            check(lib.b200mppi_batch_run_trial_sequences(self._handle, kind, descs, ptr(E), max_steps,
+                                                         int(bool(reset_x0)), ptr(xs), ptr(us), res, C.byref(issued)))
+        else:
+            if record_every is not None:                # written by the library in the returned layout
+                R = -(-max_steps // record_every)
+                recs = np.empty((K, int(E.max()), R, V, self.num_steps + 1, 3), dtype=np.float32)
+            check(lib.b200mppi_batch_run_trial_sequences_ex(
+                self._handle, kind, descs, ptr(E), max_steps, int(bool(reset_x0)), ptr(xs), ptr(us), res,
+                ptr(contacts) if barebone else None, record_every or 0,
+                ptr(recs) if record_every is not None else None, recs.nbytes if record_every is not None else 0,
+                C.byref(issued)))
         self.steps_issued = int(issued.value)
         Emax = int(E.max())
         xhist = np.full((K, Emax, max_steps + 1, 3), np.nan)
@@ -397,14 +455,25 @@ class MPPI_Batch(object):
             st = [TRIAL_STATUS[res[j].status] for j in range(first[i], first[i] + n)]
             run = sum(s != "not_run" for s in st)
             steps[i, :run] = [res[j].steps for j in range(first[i], first[i] + run)]
-            logs.append([_trial_log(res[first[i] + e], descs[first[i] + e], False) if e < run else None
+            logs.append([_trial_log(res[first[i] + e], descs[first[i] + e], barebone) if e < run else None
                          for e in range(n)])
+            if barebone:
+                for e in range(run):
+                    logs[i][e]["contact_steps"] = int(contacts[first[i] + e])
             status.append(st)
             episodes_run[i] = run
             if not self._tdm[i]:
                 p.u_prev_d = p._u_prev_buf             # as each planner's own solve() does (mppi.py:292,362)
             p.params["x0"] = xhist[i, run - 1, steps[i, run - 1]].copy()
-        return dict(logs=logs, xhist=xhist, uhist=uhist, steps=steps, status=status, episodes_run=episodes_run)
+        out = dict(logs=logs, xhist=xhist, uhist=uhist, steps=steps, status=status, episodes_run=episodes_run)
+        if barebone:
+            out["contact_steps"] = np.zeros((K, Emax), dtype=np.int64)
+            for i in range(K):
+                out["contact_steps"][i, :E[i]] = contacts[first[i]:first[i + 1]]
+        if record_every is not None:
+            out["state_rollouts"] = recs
+            out["rollout_steps"] = np.arange(R, dtype=np.int64) * record_every
+        return out
 
 
 def _fill_desc(who, p, g, dt, d, keep):
@@ -640,13 +709,18 @@ class MPPI_MixedBatch(MPPI_Batch):
                 out[key] = self._to_caller(out[key])
         return out
 
-    def run_trial_sequences(self, traction_grids, max_steps, dt=None, reset_x0=False):
+    def run_trial_sequences(self, traction_grids, max_steps, dt=None, reset_x0=False, record_every=None):
         """MPPI_Batch.run_trial_sequences for every planner, each by its kind; lists and the returned dict in the
         caller's order."""
-        out = super().run_trial_sequences(self._from_caller(traction_grids), max_steps, dt, reset_x0)
-        for key in ("logs", "xhist", "uhist", "steps", "status", "episodes_run"):
-            out[key] = self._to_caller(out[key])
+        out = super().run_trial_sequences(self._from_caller(traction_grids), max_steps, dt, reset_x0, record_every)
+        for key in ("logs", "xhist", "uhist", "steps", "status", "episodes_run", "state_rollouts"):
+            if key in out:
+                out[key] = self._to_caller(out[key])
         return out
+
+    def run_barebone_trial_sequences(self, episodes, max_steps, dt=None, reset_x0=False, record_every=None):
+        raise ValueError("MPPI_MixedBatch.run_barebone_trial_sequences: a mixed batch holds no barebone planners "
+                         "(MPPI_Batch runs barebone trial sequences)")
 
     def run_barebone_trials(self, max_steps, dt=None, record_every=None):
         raise ValueError("MPPI_MixedBatch.run_barebone_trials: a mixed batch holds no barebone planners (MPPI_Batch "

@@ -2976,9 +2976,9 @@ struct TrialPart {
 // Device buffer of a call: [descriptors (b->h_desc's layout; the one-map parity-0 sampler set is its own section there)
 // | stochastic: the parity-0 sampler set, the parity-1 set | one-map, not barebone: the parity-1 set | stochastic: box
 // descriptors, box records | shared TDM pairs: group records (stochastic), group descriptors, members (one-map, then
-// stochastic) | not barebone: the launch classes' pairs | states | barebone: contacts |
-// trials | active K + count | recording: vis descriptors | not barebone: the host grids | recording: the records (K, R,
-// V, T+1, 3) | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds
+// stochastic) | not barebone: the launch classes' pairs | states | barebone: contacts (per slot) |
+// trials | active K + count | recording: vis descriptors | recording sequences: the record flags (K) | not barebone: the
+// host grids | recording: the records (slots, R, V, T+1, 3) | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds
 // xhist and uhist: the float64 ground-truth grids (tens of MB for a batch of large maps) are copied straight from the
 // caller's arrays (a slot whose grids are planes of a realisation set has no grid section: the plant reads the planes), and the written records (of K * R * V * (T+1) * 12 bytes, 145 MB for K 8, 150 steps, V 100, T 100)
 // straight into the caller's array.
@@ -2986,6 +2986,9 @@ struct TrialPart {
 // back, descriptors, histories and results per slot (planner-major: planner i's are slots first[i] .. first[i + 1]),
 // through the same step loop for up to max_i episodes[i] * max_steps steps; the plant step (plant_step_seq_kernel)
 // moves a planner to its next episode without a launch, and the commit below follows each planner's total steps.
+// A recording sequence records at each episode's own steps t with t % record_every == 0: the plant step sets each
+// planner's record flag and record pointer for the next step (SeqArgs), and the record launches run at every step,
+// gated by those flags (1 + C2 launches per step more than without recording).
 static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_trial_desc* trials, int32_t max_steps,
                             double* xhist, float* uhist, b200mppi_trial_result* results, int32_t* contact_steps,
                             int32_t record_every, float* rollouts, size_t rollout_bytes, int32_t* steps_issued,
@@ -2993,7 +2996,7 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   const bool stochastic = kind == TrialKind::stochastic, barebone = kind == TrialKind::barebone;
   const bool mixed = kind == TrialKind::mixed;
   const bool seq = episodes != nullptr;
-  const std::string fn = seq ? "run_trial_sequences" : stochastic ? "run_stochastic_trials"
+  const std::string fn = seq ? (barebone ? "run_barebone_trial_sequences" : "run_trial_sequences") : stochastic ? "run_stochastic_trials"
                          : barebone ? "run_barebone_trials" : mixed ? "run_mixed_trials" : "run_trials";
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
   std::vector<int> first(b->pl.size() + 1, 0);        // planner i's slots: first[i] .. first[i + 1]
@@ -3034,15 +3037,20 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   const int K1 = b->nmap, K2 = K - K1;                 // the one-map planners, then the MODE_TDM planners
   const bool record = record_every > 0;
   int V = 0, R = 0;
-  size_t per = 0, rec_bytes = 0;                       // floats of one planner's record, bytes of all records
+  // floats of one record; bytes of the device's records (per slot) and of the caller's (K, max_episodes) slabs, so a
+  // sequence's records need no re-layout on the host (one episode per planner: the same two sizes)
+  size_t per = 0, rec_bytes = 0, out_bytes = 0;
   if (record) {
     if ((rc = batch_vis_validate(b, fn, &V))) return rc;
     R = (S + record_every - 1) / record_every;
     per = (size_t)V * (T + 1) * 3;
-    rec_bytes = (size_t)K * R * per * sizeof(float);
-    if (!rollouts || rollout_bytes != rec_bytes)
-      return fail(B200MPPI_EINVAL, fn + ": rollouts buffer of " + std::to_string(rollout_bytes) + " bytes, the records "
-                                   "(K, R, V, T+1, 3) float32 need " + std::to_string(rec_bytes));
+    if ((double)K * max_episodes * R * per * sizeof(float) > 4e18)
+      return fail(B200MPPI_EINVAL, fn + ": the records exceed 4e18 bytes");
+    rec_bytes = (size_t)nslot * R * per * sizeof(float);
+    out_bytes = (size_t)K * max_episodes * R * per * sizeof(float);
+    if (!rollouts || rollout_bytes != out_bytes)
+      return fail(B200MPPI_EINVAL, fn + ": rollouts buffer of " + std::to_string(rollout_bytes) + " bytes, the records " +
+                                   (seq ? "(K, Emax" : "(K") + ", R, V, T+1, 3) float32 need " + std::to_string(out_bytes));
   }
   int WW = 0, WH = 0;
   if (K2 > 0 && (rc = stochastic_validate(b, fn.c_str(), &WW, &WH))) return rc;
@@ -3087,7 +3095,7 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     q.off_mem = off_mem + q.off_mem * sizeof(int);
     q.off_cls = off_cls + q.off_cls * sizeof(int);
   }
-  const size_t ncon = barebone ? (size_t)K : 0;        // barebone-only section
+  const size_t ncon = barebone ? (size_t)nslot : 0;    // barebone-only section, per slot
   const size_t off_state = off_cls + align256(ncls * sizeof(int));
   const size_t off_con = off_state + align256((size_t)K * sizeof(TrialState));
   const size_t nres = seq ? (size_t)nslot : 0;          // sequence-only sections: per-slot results and start poses
@@ -3097,7 +3105,9 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   const size_t off_seq = off_act + align256((size_t)(K + 1) * sizeof(int));      // first (K + 1), episode (K)
   const size_t off_start = off_seq + align256((seq ? (size_t)(2 * K + 1) : 0) * sizeof(int));
   const size_t off_vis = off_start + align256(nres * 3 * sizeof(double));
-  size_t off = off_vis + align256((record ? (size_t)K : 0) * sizeof(VisBatchDesc));
+  const bool rec_seq = record && seq;                  // records gated per planner on the device (SeqArgs::rec_flag)
+  const size_t off_rflag = off_vis + align256((record ? (size_t)K : 0) * sizeof(VisBatchDesc));
+  size_t off = off_rflag + align256((rec_seq ? (size_t)K : 0) * sizeof(int));
   const size_t head = off;
   std::vector<size_t> off_grid(nslot);
   for (int j = 0; j < nslot; ++j) {
@@ -3118,7 +3128,11 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
     }
   } buf;
-  CU(cudaMalloc(&buf.d, total));
+  if (cudaMalloc(&buf.d, total) != cudaSuccess) {
+    buf.d = nullptr;
+    cudaGetLastError();                                // not sticky: later calls start clean
+    return fail(B200MPPI_ECUDA, fn + ": cudaMalloc of " + std::to_string(total) + " bytes");
+  }
   if (cudaMallocHost(&buf.h, head + (total - off_xh)) != cudaSuccess) {
     buf.h = nullptr;
     return fail(B200MPPI_ECUDA, fn + ": cudaMallocHost");
@@ -3143,14 +3157,15 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     b200mppi_planner* p = b->pl[i];
     const bool sto = i >= K1;
     const int r = i - K1;                              // a stochastic planner's index in its kind's launches
-    if (record)                                        // x0 from the record the plant step writes
-      hv[i] = vis_desc(p, sto ? &dw[r].p : &dr[i].p, drec + (size_t)i * R * per);
+    if (record)                                        // x0 from the record the plant step writes; record 0 of slot 0
+      hv[i] = vis_desc(p, sto ? &dw[r].p : &dr[i].p, drec + (size_t)first[i] * R * per);
+    if (rec_seq) reinterpret_cast<int*>(h + off_rflag)[i] = 1;
     hst[i] = TrialState{};
     for (int c = 0; c < 3; ++c) hst[i].x[c] = trials[first[i]].x0[c];
     hact[i] = 1;
-    if (barebone) hcon[i] = 0;
     for (int j = first[i]; j < first[i + 1]; ++j) {    // the planner's episodes: one, or its sequence
       const b200mppi_trial_desc& q = trials[j];
+      if (barebone) hcon[j] = 0;
       TrialDev& t = ht[j];
       t = TrialDev{};
       t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1]; t.tol = q.goal_tolerance;
@@ -3196,6 +3211,14 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     int* dseq = reinterpret_cast<int*>(d + off_seq);
     sa = SeqArgs{dseq, dseq + K + 1, reinterpret_cast<const double*>(d + off_start),
                  reinterpret_cast<TrialState*>(d + off_res), reset_x0 ? 1 : 0};
+    if (rec_seq) {
+      static_assert(sizeof(VisBatchDesc) % sizeof(float*) == 0, "rec_stride counts float* slots");
+      sa.rec_flag = reinterpret_cast<int*>(d + off_rflag);
+      sa.rec_out = &reinterpret_cast<VisBatchDesc*>(d + off_vis)->out;
+      sa.rec = drec;
+      sa.rec_per = (long long)per;
+      sa.rec_every = record_every; sa.rec_R = R; sa.rec_stride = (int)(sizeof(VisBatchDesc) / sizeof(float*));
+    }
   }
   for (TrialPart& q : P) {
     SampleGridsV2Args* hs0 = reinterpret_cast<SampleGridsV2Args*>(h + q.off_s0);
@@ -3292,16 +3315,19 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       launch_update_partial_batch(du, K, b->pl[0]->num_ctas, dact, st);
       CHECK_LAUNCH();
     }
-    const bool rec_step = record && s % record_every == 0;
+    // a sequence's episodes start at steps only the device knows: a recording sequence issues the record launches at
+    // every step, gated per planner by the flags the previous plant step set, each writing where its descriptor points
+    const bool rec_step = record && (seq || s % record_every == 0);
     if (rec_step) {
+      const int* rflag = seq ? sa.rec_flag : dact;
       for (int c = 0; c < C2; ++c) {                  // from the pre-call states this step's sampling read
         const TrialClass& tc = P[1].cls[c];
-        launch_sample_grids_v2_complete_batch(tc.L, ds[1][s & 1], db, lc2.count(c), dcls[1] + lc2.first[c], dact2, V,
-                                              tc.mrows, tc.ncact, st, dgrp[1], dmem[1]);
+        launch_sample_grids_v2_complete_batch(tc.L, ds[1][s & 1], db, lc2.count(c), dcls[1] + lc2.first[c], rflag + K1,
+                                              V, tc.mrows, tc.ncact, st, dgrp[1], dmem[1]);
         CHECK_LAUNCH();
       }
-      launch_state_rollout_batch(reinterpret_cast<const VisBatchDesc*>(d + off_vis), K, V, dact,
-                                 (size_t)(s / record_every) * per, st);
+      launch_state_rollout_batch(reinterpret_cast<const VisBatchDesc*>(d + off_vis), K, V, rflag,
+                                 seq ? 0 : (size_t)(s / record_every) * per, st);
       CHECK_LAUNCH();
     }
     pa.step = s;
@@ -3309,7 +3335,7 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     else launch_plant_step(pa, st);
     CHECK_LAUNCH();
     b->launches += num_opt + 1 + (K1 > 0 ? 2 * num_opt + C1 : 0) + (K2 > 0 ? 3 * num_opt + 2 * C2 : 0);
-    if (rec_step) b->launches += 1 + C2;
+    if (rec_step) b->launches += 1 + C2;          // every step of a recording sequence
     ++issued;
     CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, dact + K, sizeof(int), cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(buf.ev[s % TRIAL_POLL], st));
@@ -3341,8 +3367,8 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       for (size_t q = (size_t)n * 2; q < (size_t)S * 2; ++q) uo[q] = fnan;
       results[j] = b200mppi_trial_result{r.cum_obj, r.cum_dist, r.dist, n, r.status};
       ran[i] += n;
+      if (barebone) contact_steps[j] = hcon[j];
     }
-    if (barebone) contact_steps[i] = hcon[i];
     // host state as after ran[i] rounds of the host loop: the reach slot toggled once per iteration, the last solve's
     // box and x0 (the samplings of the pair below).  The last solve planned from the pose before the last step -- or,
     // when a later episode of a sequence without reset_x0 took one step, from the previous episode's final pose
@@ -3378,17 +3404,26 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
     }
   }
   if (record) {
-    // record r belongs to step r * record_every.  Only the written ones are copied (records past a planner's last step
-    // are never written, and an early stop leaves most of them so): the rest is NaN.  The last one is what the
-    // planner's state_rollout buffer holds after the host loop's last get_state_rollout.
+    // record r of a slot belongs to step r * record_every of its episode; slot first[i] + e goes to the caller's slab
+    // (i, e).  Only the written ones are copied (records past an episode's last step are never written, and an early
+    // stop leaves most of them so): the rest is NaN, as are the slabs of episodes a planner does not have.  The last one
+    // of a planner's last run episode is what its state_rollout buffer holds after the host loop's last
+    // get_state_rollout.
     for (int i = 0; i < K; ++i) {
-      const int done = (hst[i].steps + record_every - 1) / record_every;
-      float* slab = rollouts + (size_t)i * R * per;
-      CU(cudaMemcpyAsync(slab, drec + (size_t)i * R * per, (size_t)done * per * sizeof(float), cudaMemcpyDeviceToHost,
-                         st));
-      CU(cudaMemcpyAsync(b->pl[i]->state_rollout, drec + ((size_t)i * R + done - 1) * per, per * sizeof(float),
+      int last = first[i], last_done = 0;
+      float* planner_out = rollouts + (size_t)i * max_episodes * R * per;
+      std::fill(planner_out + (size_t)(first[i + 1] - first[i]) * R * per,
+                planner_out + (size_t)max_episodes * R * per, fnan);
+      for (int j = first[i]; j < first[i + 1]; ++j) {
+        const int done = (results[j].steps + record_every - 1) / record_every;
+        float* slab = planner_out + (size_t)(j - first[i]) * R * per;
+        CU(cudaMemcpyAsync(slab, drec + (size_t)j * R * per, (size_t)done * per * sizeof(float), cudaMemcpyDeviceToHost,
+                           st));
+        std::fill(slab + (size_t)done * per, slab + (size_t)R * per, fnan);
+        if (done > 0) { last = j; last_done = done; }
+      }
+      CU(cudaMemcpyAsync(b->pl[i]->state_rollout, drec + ((size_t)last * R + last_done - 1) * per, per * sizeof(float),
                          cudaMemcpyDeviceToDevice, st));
-      std::fill(slab + (size_t)done * per, slab + (size_t)R * per, fnan);
     }
     CU(cudaStreamSynchronize(st));
   }
@@ -3457,4 +3492,23 @@ extern "C" int b200mppi_batch_run_trial_sequences(b200mppi_batch* b, int32_t kin
   if (!episodes) return fail(B200MPPI_EINVAL, "run_trial_sequences: null episode counts");
   return batch_run_trials(b, trial_kind(kind), trials,
                           max_steps, xhist, uhist, results, nullptr, 0, nullptr, 0, steps_issued, episodes, reset_x0);
+}
+
+extern "C" int b200mppi_batch_run_trial_sequences_ex(b200mppi_batch* b, int32_t kind, const b200mppi_trial_desc* trials,
+                                                     const int32_t* episodes, int32_t max_steps, int32_t reset_x0,
+                                                     double* xhist, float* uhist, b200mppi_trial_result* results,
+                                                     int32_t* contact_steps, int32_t record_every, float* rollouts,
+                                                     size_t rollout_bytes, int32_t* steps_issued) {
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  if (kind != B200MPPI_TRIALS_MAP && kind != B200MPPI_TRIALS_STOCHASTIC && kind != B200MPPI_TRIALS_BAREBONE &&
+      kind != B200MPPI_TRIALS_MIXED)
+    return fail(B200MPPI_EINVAL, "run_trial_sequences_ex: unknown trial kind " + std::to_string(kind));
+  if (!episodes) return fail(B200MPPI_EINVAL, "run_trial_sequences_ex: null episode counts");
+  if (record_every < 0)
+    return fail(B200MPPI_EINVAL, "run_trial_sequences_ex: record_every " + std::to_string(record_every) + " < 0");
+  if (kind != B200MPPI_TRIALS_BAREBONE && contact_steps)
+    return fail(B200MPPI_EINVAL, "run_trial_sequences_ex: contact_steps given for a trial kind other than "
+                                 "B200MPPI_TRIALS_BAREBONE");
+  return batch_run_trials(b, trial_kind(kind), trials, max_steps, xhist, uhist, results, contact_steps, record_every,
+                          rollouts, rollout_bytes, steps_issued, episodes, reset_x0);
 }

@@ -577,7 +577,8 @@ struct PlantArgs {
   double* xhist;                          // (K, max_steps+1, 3)
   float* uhist;                           // (K, max_steps, 2)
   int K, T, max_steps, step;
-  int* contacts;                          // barebone trials: (K) steps whose new pose touches an obstacle; else null
+  int* contacts;                          // barebone trials: (K) steps whose new pose touches an obstacle (trial
+                                          // sequences: per slot); else null
 };
 // Trial sequences (b200mppi_batch_run_trial_sequences): planner k runs the episodes of slots first[k] .. first[k+1]-1
 // back to back.  PlantArgs::trials, xhist and uhist are then per slot, PlantArgs::state per planner (the running
@@ -589,6 +590,15 @@ struct SeqArgs {
   TrialState* results;                    // (slots) written when the episode stops
   int reset_x0;                           // 1: an episode's first solve plans from its start pose, and LEFT_MAP does
                                           // not end the sequence; 0: from the previous episode's final pose
+  // Recording sequences (record_every n > 0; rec_flag null: none).  After each step rec_flag[k] = 1 when planner k
+  // records at its next step (it runs, and its episode step then is a multiple of n), and then the planner's
+  // VisBatchDesc::out in the call's device descriptors (rec_out[k * rec_stride]) points at record step / n of that
+  // episode's slot: rec + (slot * rec_R + step / n) * rec_per.
+  int* rec_flag;                          // (K)
+  float** rec_out;                        // &VisBatchDesc::out of planner 0
+  float* rec;                             // (slots, rec_R, V, T+1, 3)
+  long long rec_per;                      // floats of one record
+  int rec_every, rec_R, rec_stride;       // rec_stride: sizeof(VisBatchDesc) / sizeof(float*)
 };
 // [emu:end trial_args]
 void launch_plant_step(const PlantArgs& a, cudaStream_t st);

@@ -381,15 +381,25 @@ __device__ __forceinline__ double py_floordiv(double vx, double wx) {
   return copysign(0.0, __ddiv_rn(vx, wx));
 }
 
+// Recording sequences: whether planner k records at its next step, step `step` of the episode of slot `slot`, and
+// where that record goes (SeqArgs).
+__device__ __forceinline__ void seq_record_next(const SeqArgs& q, int k, int slot, int step) {
+  if (!q.rec_flag) return;
+  const int on = step % q.rec_every == 0;
+  q.rec_flag[k] = on;
+  if (on) q.rec_out[(size_t)k * q.rec_stride] = q.rec + ((size_t)slot * q.rec_R + step / q.rec_every) * q.rec_per;
+}
+
 // One warp per planner (warp k of the grid = planner k): apply u_cur[0], shift u_cur by one row (the last row kept),
 // record the step, and stop the planner on the goal, on leaving the padded map or after max_steps steps.
 // Barebone trials (TrialDev::lin null) step the notebook's nominal unicycle (traction 1: dt * 1.0 == dt), have no map
-// to leave, and count in contacts[k] the steps whose new pose lies in one of the planner's obstacles.
+// to leave, and count in contacts[slot] the steps whose new pose lies in one of the planner's obstacles.
 // SEQ (trial sequences, SeqArgs): the planner steps its running episode e, slot first[k] + e of the descriptors and
 // histories.  When that episode stops and another follows (reset_x0, or a stop other than LEFT_MAP), its result is
 // written, the plant restarts from the next start pose with zero metrics, and the planner stays active; with reset_x0
 // the next solve also plans from that pose (x0_out and the window).  Without it x0_out keeps the final pose, as the
-// benchmark's planner keeps its params['x0'] across episodes.  active_count falls when the sequence ends.
+// benchmark's planner keeps its params['x0'] across episodes.  active_count falls when the sequence ends.  A recording
+// sequence also marks whether the planner records at its next step (seq_record_next; 0 once its sequence ends).
 template <bool SEQ = false>
 __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int lane, const SeqArgs& q = SeqArgs{}) {
   if (k >= a.K || !a.active[k]) return;
@@ -448,7 +458,7 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
       const double r = (double)d.obstacles[3 * j + 2];
       hit = __dadd_rn(__dmul_rn(ex, ex), __dmul_rn(ey, ey)) <= __dmul_rn(r, r);
     }
-    if (hit) a.contacts[k] += 1;
+    if (hit) a.contacts[slot] += 1;
   }
   int status = TRIAL_RUNNING;
   if (dist <= 0.0) status = TRIAL_GOAL;
@@ -471,12 +481,16 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
           d.x0_out[2] = __double2float_rn(x0[2]);
           if (d.win) win_origin(d.x0_out[0], d.x0_out[1], d.win_pxl, d.win_pyl, d.win_res, d.win_cols, d.win_rows, d.win);
         }
+        seq_record_next(q, k, slot + 1, 0);
         return;
       }
+      if (q.rec_flag) q.rec_flag[k] = 0;
     }
     s.status = status;
     a.active[k] = 0;
     atomicSub(a.active_count, 1);
+  } else if constexpr (SEQ) {
+    seq_record_next(q, k, slot, t + 1);
   }
 }
 
