@@ -1,4 +1,5 @@
-"""Directed one-step scenarios for the two float64 contractions of the unicycle step (TEST INFRASTRUCTURE).
+"""Directed one-step scenarios for the float64 contractions of the unicycle step and of the speed map's time cost (TEST
+INFRASTRUCTURE).
 
 Random scenarios cannot tell a float64 FMA from a product and a sum: the two differ by at most one float64 ulp, which
 moves the float32 state only when the value lies within ~1e-16 of a float32 rounding boundary.  These cases are built
@@ -12,6 +13,11 @@ differs between
 and then a goal and a tolerance that the exact x reaches and the other does not (or the reverse): a kernel that
 contracts differently reports a different goal flag, hence a different cost.  The start x0 is tiny (|x0| << one
 float32 ulp of dv * cos), which lets it place dv * cos + x0 between float64 grid points next to a float32 midpoint.
+
+``speed_map_boundary_case(A)`` (kind "speed") searches for traction bounds, a risk byte r and a float32 dt for which the
+speed map's time step RN32(dt / (eff + 1e-6)) differs between eff = fma(ratio, r, lo) and RN64(RN64(ratio * r) + lo).
+Its scenario stands still at the goal (v = 0), so the one step reaches it with d2 = 0 and the cost is that time step
+alone: a kernel that splits the contraction reports a cost one float32 ulp off.
 """
 import numpy as np
 
@@ -83,21 +89,58 @@ def fma_boundary_case(A, kind, lb=(0.2, 1.3), th0=0.6, y0=0.3, dt=0.1):
             continue
         return dict(kind=kind, lb=[float(lo), float(hi)], q=q, v=F32(v[idx[i // 7]]), x0=[float(x0[i]), float(F32(y0)), float(th)],
                     goal=[float(goal[0]), float(goal[1])], tol=float(tol), x1_exact=xe[i], x1_other=xm[i],
-                    exact_reaches=bool(d2e <= F32(tol * tol)))
+                    exact_reaches=bool(d2e <= F32(tol * tol)), dt=float(dt64))
     raise AssertionError("no %s boundary case found" % kind)
 
 
-def directed_scenario(case, N=33, M=2, T=2):
-    """Inputs of a case of fma_boundary_case: uniform maps (traction byte ``case['q']``), no masks, no noise, speed v, its
-    start, goal and tolerance -- the first step decides the goal flag by one float32 ulp of x."""
+def speed_map_boundary_case(A, seed=0, x0=(0.3, 0.3, 0.6), q=100):
+    """Bounds (lo, hi) drawn from ``seed``, risk byte r and dt: the first float32 dt in [1/16, 1/8) and the first byte of
+    the first bounds where the fused and the split eff give different float32 time steps.  Traction byte ``q``."""
+    dts = (F32(1 / 16) + np.arange(1 << 23, dtype=F64) * 2.0 ** -27).astype(F32)     # every float32 in [1/16, 1/8)
+    dt64 = dts.astype(F64)
+    qs = np.arange(0, 101, dtype=F64)
+    rng = np.random.default_rng(seed)
+    for _ in range(64):
+        lo, hi = F32(rng.uniform(0.05, 0.5)), F32(rng.uniform(0.8, 1.5))
+        ratio, lo64 = 0.01 * F64(F32(hi - lo)), F64(lo)
+        fused = A.fma64(np.full(101, ratio), qs, np.full(101, lo64))
+        split = ratio * qs + lo64
+        for r in np.nonzero(fused != split)[0]:
+            k = np.nonzero((dt64 / (fused[r] + 1e-6)).astype(F32) != (dt64 / (split[r] + 1e-6)).astype(F32))[0]
+            if not k.size:
+                continue
+            dt = dt64[k[0]]
+
+            def cost(eff):                       # one step at the goal: d2 = 0, cost = 0 + (sqrt(0) * w + dt_eff)
+                dt_eff = A.d2f(np.array([dt / (eff + 1e-6)]))
+                return F32(A.add32(F32(0), A.fma32(A.sqrt32(np.zeros(1, F32)), F32(1), dt_eff))[0])
+            ce, cm = cost(fused[r]), cost(split[r])
+            assert ce != cm, "speed case: the fused and the split time step give the same cost"
+            x = F32(x0[0])
+            return dict(kind="speed", lb=[float(lo), float(hi)], q=q, risk=int(r), v=F32(0), dt=float(dt),
+                        x0=[float(x), float(F32(x0[1])), float(F32(x0[2]))], goal=[float(x), float(F32(x0[1]))],
+                        tol=0.5, T=1, x1_exact=x, x1_other=x, exact_reaches=True, cost_exact=ce, cost_other=cm)
+    raise AssertionError("no speed boundary case found")
+
+
+def boundary_case(A, kind):
+    """The directed case of a kind: "state" and "traction" (fma_boundary_case) or "speed" (speed_map_boundary_case)."""
+    return speed_map_boundary_case(A) if kind == "speed" else fma_boundary_case(A, kind)
+
+
+def directed_scenario(case, N=33, M=2, T=None):
+    """Inputs of a directed case: uniform maps (traction byte ``case['q']``, risk byte ``case['risk']`` or the traction
+    byte), no masks, no noise, speed v, its start, goal, tolerance and dt -- the first step decides the goal flag by one
+    float32 ulp of x (or, kind "speed", the cost by one float32 ulp of the time step).  T: the case's, else 2."""
     R = Cc = 100
+    T = case.get("T", 2) if T is None else T
     s = dict(N=N, M=M, T=T, R=R, Cc=Cc, res=F32(0.1), xlo=F32(-5.0), ylo=F32(-5.0), lb=case["lb"], ab=[0.0, 1.0],
-             x0=case["x0"], goal=case["goal"], tol=case["tol"], shift=(0, 0))
+             x0=case["x0"], goal=case["goal"], tol=case["tol"], dt=case["dt"], shift=(0, 0))
     s["lin"] = np.full((M, R, Cc), case["q"], np.int8)
     s["ang"] = np.full((M, R, Cc), 50, np.int8)
     s["obs"] = np.zeros((R, Cc), np.int8)
     s["unk"] = np.zeros((R, Cc), np.int8)
-    s["risk"] = np.full((R, Cc), case["q"], np.int8)
+    s["risk"] = np.full((R, Cc), case.get("risk", case["q"]), np.int8)
     s["noise"] = np.zeros((N, T, 2), F32)
     s["u_cur"] = np.zeros((T, 2), F32)
     s["u_cur"][:, 0] = case["v"]

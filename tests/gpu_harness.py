@@ -200,8 +200,9 @@ class RawPlanner:
         self.L.check(getattr(self.lib, "b200mppi_planner_" + name)(self.pl, *args))
 
 
-def run_directed(eng, s, mode):
-    """A directed case (tests/directed_cases.py) through the C-ABI planner: uniform grids set directly, its bounds."""
+def run_directed(eng, s, mode, states=False):
+    """A directed case (tests/directed_cases.py) through the C-ABI planner: uniform grids set directly, its bounds.
+    ``states``: the planner's visualisation rollout instead (V = 1: u_cur without noise, on map 0), (1, T + 1, 3)."""
     N, T, R, Cc = s["N"], s["T"], s["R"], s["Cc"]
     rp = RawPlanner(eng, mode, N, s["M"], T, R, Cc)
     try:
@@ -214,7 +215,11 @@ def run_directed(eng, s, mode):
         rp.set_grids("ang", s["ang"][:rp.M])
         rp.copy_in(eng._lib.BUF_NOISE, s["noise"])
         rp.copy_in(eng._lib.BUF_U_CUR, s["u_cur"])
-        rp.set_params(x0=list(s["x0"]), xgoal=list(s["goal"]), goal_tolerance=s["tol"])
+        rp.set_params(x0=list(s["x0"]), xgoal=list(s["goal"]), goal_tolerance=s["tol"], dt=s["dt"])
+        if states:
+            out = np.empty((1, T + 1, 3), np.float32)
+            rp.call("get_state_rollout", eng._lib.ptr(out), out.nbytes)
+            return out
         rp.call("rollout")
         return rp.copy_out(eng._lib.BUF_COSTS_NM, (N, rp.M)) if mode == 0 else rp.copy_out(eng._lib.BUF_COSTS, (N,))[:, None]
     finally:
@@ -226,7 +231,7 @@ def directed_oracle(s, mode, arith):
     lim = [s["xlo"], s["xlo"] + s["Cc"] * s["res"]]
     return MR.rollout_costs(mode, s["lin"] if mode == 0 else s["lin"][:1], s["ang"] if mode == 0 else s["ang"][:1],
                             s["lb"], s["ab"], s["obs"], s["unk"], s["res"], lim, lim, [0, 3], [-np.pi, np.pi], s["goal"],
-                            0.01, 1e5, 1e2, s["tol"], 1.0, [2, 3], s["x0"], 0.1, 1.0, s["noise"], s["u_cur"],
+                            0.01, 1e5, 1e2, s["tol"], 1.0, [2, 3], s["x0"], s["dt"], 1.0, s["noise"], s["u_cur"],
                             risk_map=s["risk"][None], arith=arith, ctrl_order="presummed" if mode == 0 else "sequential",
                             wrap_clamp=True)
 

@@ -128,7 +128,7 @@ def _scenario(name):
     """Inputs of one edge scenario (dict): maps, masks, noise, controls, geometry, bounds, goal."""
     rng = np.random.default_rng(zlib.crc32(name.encode()))
     s = dict(N=300, M=2, T=30, R=300, Cc=280, res=F32(0.1), xlo=F32(0.0), ylo=F32(0.0), lb=[0, 1], ab=[0, 1],
-             x0=[14.03, 15.07, 0.7], goal=[17.0, 18.0], tol=0.5, shift=(0, 0), mask_lo=0, mask_hi=2)
+             x0=[14.03, 15.07, 0.7], goal=[17.0, 18.0], tol=0.5, dt=0.1, shift=(0, 0), mask_lo=0, mask_hi=2)
     if name == "lo_pos":
         s.update(lb=[0.2, 0.9], ab=[0.15, 1.3])
     elif name == "lo_neg":
@@ -186,7 +186,7 @@ def _scenario(name):
 def _run_all(emu, s, masks01=None):
     win, gen = emu
     N, M, T, R, Cc = s["N"], s["M"], s["T"], s["R"], s["Cc"]
-    f = _fparams(s["res"], s["xlo"], s["ylo"], 0.1, s["x0"], s["goal"], s["tol"], 0.01, 1.0, [2, 3], [0, 3],
+    f = _fparams(s["res"], s["xlo"], s["ylo"], s["dt"], s["x0"], s["goal"], s["tol"], 0.01, 1.0, [2, 3], [0, 3],
                  [-np.pi, np.pi], 1e5, 1e2, 1.0, s["lb"][0], s["ab"][0])
     ratios = _ratios(s["lb"], s["ab"])
     geo = _c([R, Cc, R, Cc, Cc, Cc, T, N, M], np.int32)
@@ -208,8 +208,8 @@ def _run_all(emu, s, masks01=None):
 def _oracle(s, mode, order="sequential"):
     return MR.rollout_costs(mode, s["lin"], s["ang"], s["lb"], s["ab"], s["obs"], s["unk"], s["res"],
                             [s["xlo"], 0], [s["ylo"], 0], [0, 3], [-np.pi, np.pi], s["goal"], 0.01, 1e5, 1e2, s["tol"],
-                            1.0, [2, 3], s["x0"], 0.1, 1.0, s["noise"], s["u_cur"], risk_map=s["risk"][None], wrap_clamp=True,
-                            arith=EXACT, ctrl_order=order)
+                            1.0, [2, 3], s["x0"], s["dt"], 1.0, s["noise"], s["u_cur"], risk_map=s["risk"][None],
+                            wrap_clamp=True, arith=EXACT, ctrl_order=order)
 
 
 def assert_equal(got, want, what):
@@ -287,27 +287,35 @@ def test_state_rollout_and_barebone_kernels_equal_exact_oracle(emu, name):
 
 
 # ----------------------------------------------------------------------------- directed: the float64 contractions
-@pytest.mark.parametrize("kind", ["state", "traction"])
+@pytest.mark.parametrize("kind", ["state", "traction", "speed"])
 def test_float64_contractions_on_a_float32_rounding_boundary(emu, kind):
     """The traction value fma(ratio, q, lo) and the state update fma(dv, cos, x), each rounded once: on inputs where
     rounding the product first moves the first step's float32 x by one ulp and flips the goal flag, every kernel
-    equals the exact oracle -- so a kernel (or an oracle) that split either contraction would differ here."""
-    from tests.directed_cases import directed_scenario, fma_boundary_case
-    case = fma_boundary_case(EXACT, kind)
-    assert case["x1_exact"] != case["x1_other"]
+    equals the exact oracle -- so a kernel (or an oracle) that split either contraction would differ here.  Kind
+    "speed": the speed map's eff = fma(ratio, risk, lo), on inputs where splitting it moves the time step dt / (eff +
+    1e-6), the whole cost of a one-step rollout that starts on its goal, by one float32 ulp."""
+    from tests.directed_cases import boundary_case, directed_scenario
+    case = boundary_case(EXACT, kind)
     s = directed_scenario(case)
     _, st = MR.rollout_costs(MR.MODE_STOCHASTIC, s["lin"], s["ang"], s["lb"], s["ab"], s["obs"], s["unk"], s["res"],
                              [s["xlo"], 0], [s["ylo"], 0], [0, 3], [-np.pi, np.pi], s["goal"], 0.01, 1e5, 1e2, s["tol"],
-                             1.0, [2, 3], s["x0"], 0.1, 1.0, s["noise"], s["u_cur"], return_states=True, arith=EXACT)
+                             1.0, [2, 3], s["x0"], s["dt"], 1.0, s["noise"], s["u_cur"], return_states=True, arith=EXACT)
     assert (st[:, :, 1, 0] == case["x1_exact"]).all()
-    assert (st[:, :, 2, 0] == 0).all() == case["exact_reaches"]      # reached at the first step: no second step ran
+    if kind == "speed":
+        assert s["T"] == 1 and case["risk"] != case["q"] and case["cost_exact"] != case["cost_other"]
+        assert (_oracle(s, MR.MODE_SPEED_MAP) == case["cost_exact"]).all()
+    else:
+        assert case["x1_exact"] != case["x1_other"]
+        assert (st[:, :, 2, 0] == 0).all() == case["exact_reaches"]      # reached at the first step: no second step ran
     out, gens = _run_all(emu, s)
     assert_equal(out, _oracle(s, MR.MODE_STOCHASTIC, "presummed"), "windowed kernel")
     for mode in (0, 1, 2):
         assert_equal(gens[mode], _oracle(s, mode), "generic kernel, mode %d" % mode)
+    if kind == "speed":
+        assert (gens[2] == case["cost_exact"]).all()
     _, gen = emu
-    f = _fparams(s["res"], s["xlo"], s["ylo"], 0.1, s["x0"], [0, 0], 0.0, 1.0, 1.0, [1, 1], [0, 3], [-np.pi, np.pi],
-                 0.0, 0.0, 1.0, s["lb"][0], s["ab"][0])
+    f = _fparams(s["res"], s["xlo"], s["ylo"], s["dt"], s["x0"], [0, 0], 0.0, 1.0, 1.0, [1, 1], [0, 3],
+                 [-np.pi, np.pi], 0.0, 0.0, 1.0, s["lb"][0], s["ab"][0])
     vis = np.zeros((1, s["T"] + 1, 3), F32)
     gen.emu_state_rollout(1, 1, _p(f), _p(_c([100, 100, 100, 100, 100, 100, s["T"], s["N"], 1], np.int32)),
                           _p(_ratios(s["lb"], s["ab"])), _p(_c(s["lin"], np.int8)), _p(_c(s["ang"], np.int8)),
