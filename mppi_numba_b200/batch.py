@@ -262,6 +262,37 @@ class MPPI_Batch(object):
         return self._trials("MPPI_Batch.run_barebone_trials", lib.b200mppi_batch_run_barebone_trials, None, max_steps,
                             dt, record_every, _lib.TRIALS_BAREBONE)
 
+    def _trial_descs(self, name, seqs, max_steps, dt, record_every, episodes):
+        """The checks every trial call makes before its C entry point (max_steps, record_every, V, the TDM groups, and
+        each planner's solve conditions and num_opt), and the trial descriptors of ``seqs`` (per planner its grids, one
+        per episode; None for barebone) planner-major, the refusals naming the episode when ``episodes``.  Returns
+        (max_steps, record_every, V, descs, first, keep): planner i's descriptors are descs[first[i]:first[i + 1]], and
+        ``keep`` holds what they point to."""
+        max_steps = int(max_steps)
+        if max_steps < 1:
+            raise ValueError("%s: max_steps %d < 1" % (name, max_steps))
+        V = None
+        if record_every is not None:
+            record_every = int(record_every)
+            if record_every < 1:
+                raise ValueError("%s: record_every %d < 1" % (name, record_every))
+            V = self._vis_count(name)
+        self._check_groups(name)
+        first = np.concatenate([[0], np.cumsum([len(g) for g in seqs], dtype=np.int64)])
+        descs = (_lib.TrialDesc * int(first[-1]))()
+        keep = []
+        for i, p in enumerate(self.planners):
+            who = "%s: planner %d" % (name, self.order[i])
+            if not p.check_solve_conditions():
+                raise ValueError("%s cannot solve (reason printed above)" % who)
+            if int(p.params["num_opt"]) < 1:
+                raise ValueError("%s has num_opt %d < 1" % (who, int(p.params["num_opt"])))
+            for e, g in enumerate(seqs[i]):
+                _fill_desc(who + (", episode %d" % e if episodes else ""), p, g, dt, descs[first[i] + e], keep)
+        for p in self.planners:
+            p.move_mppi_task_vars_to_device()
+        return max_steps, record_every, V, descs, first, keep
+
     def _trials(self, name, entry, traction_grids, max_steps, dt, record_every, kind):
         """The marshalling of a closed-loop trial call through the C entry point ``entry`` (with record_every set:
         b200mppi_batch_run_trials_recorded with trial kind ``kind``) and the logs built from its results (run_trials,
@@ -272,25 +303,8 @@ class MPPI_Batch(object):
         grids = [None] * K if barebone else list(traction_grids)
         if len(grids) != K:
             raise ValueError("%s: %d traction grids for %d planners" % (name, len(grids), K))
-        max_steps = int(max_steps)
-        if max_steps < 1:
-            raise ValueError("%s: max_steps %d < 1" % (name, max_steps))
-        if record_every is not None:
-            record_every = int(record_every)
-            if record_every < 1:
-                raise ValueError("%s: record_every %d < 1" % (name, record_every))
-            V = self._vis_count(name)
-        self._check_groups(name)
-        descs = (_lib.TrialDesc * K)()
-        keep = []
-        for i, (p, g) in enumerate(zip(self.planners, grids)):
-            if not p.check_solve_conditions():
-                raise ValueError("%s: planner %d cannot solve (reason printed above)" % (name, self.order[i]))
-            if int(p.params["num_opt"]) < 1:
-                raise ValueError("%s: planner %d has num_opt %d < 1" % (name, self.order[i], int(p.params["num_opt"])))
-            _fill_desc("%s: planner %d" % (name, self.order[i]), p, g, dt, descs[i], keep)
-        for p in self.planners:
-            p.move_mppi_task_vars_to_device()
+        max_steps, record_every, V, descs, _, keep = self._trial_descs(name, [[g] for g in grids], max_steps, dt,
+                                                                        record_every, False)
         xhist = np.empty((K, max_steps + 1, 3), dtype=np.float64)
         uhist = np.empty((K, max_steps, 2), dtype=np.float32)
         res = (_lib.TrialResult * K)()
@@ -402,28 +416,9 @@ class MPPI_Batch(object):
         the dict built from its per-slot results; ``name`` prefixes the refusals."""
         K = len(self.planners)
         barebone = kind == _lib.TRIALS_BAREBONE
-        max_steps = int(max_steps)
-        if max_steps < 1:
-            raise ValueError("%s: max_steps %d < 1" % (name, max_steps))
-        if record_every is not None:
-            record_every = int(record_every)
-            if record_every < 1:
-                raise ValueError("%s: record_every %d < 1" % (name, record_every))
-            V = self._vis_count(name)
-        self._check_groups(name)
-        E = np.array([len(g) for g in seqs], dtype=np.int32)
-        first = np.concatenate([[0], np.cumsum(E)])
-        descs = (_lib.TrialDesc * int(first[-1]))()
-        keep = []
-        for i, p in enumerate(self.planners):
-            if not p.check_solve_conditions():
-                raise ValueError("%s: planner %d cannot solve (reason printed above)" % (name, self.order[i]))
-            if int(p.params["num_opt"]) < 1:
-                raise ValueError("%s: planner %d has num_opt %d < 1" % (name, self.order[i], int(p.params["num_opt"])))
-            for e, g in enumerate(seqs[i]):
-                _fill_desc("%s: planner %d, episode %d" % (name, self.order[i], e), p, g, dt, descs[first[i] + e], keep)
-        for p in self.planners:
-            p.move_mppi_task_vars_to_device()
+        max_steps, record_every, V, descs, first, keep = self._trial_descs(name, seqs, max_steps, dt, record_every,
+                                                                            True)
+        E = np.diff(first).astype(np.int32)
         slots = int(first[-1])
         xs = np.empty((slots, max_steps + 1, 3), dtype=np.float64)
         us = np.empty((slots, max_steps, 2), dtype=np.float32)

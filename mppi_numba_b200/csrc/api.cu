@@ -2117,7 +2117,16 @@ struct b200mppi_batch {
   size_t off_nprep = 0;
 };
 
-static size_t align256(size_t v) { return (v + 255) / 256 * 256; }
+// Hands out 256-byte-aligned sections of one allocation, in order: take returns a section's offset.  An empty section
+// takes no bytes.
+struct Sections {
+  size_t end = 0;
+  size_t take(size_t bytes) {
+    const size_t at = end;
+    end += (bytes + 255) / 256 * 256;
+    return at;
+  }
+};
 
 extern "C" int b200mppi_batch_destroy(b200mppi_batch* b) {
   if (!b) return B200MPPI_OK;
@@ -2133,18 +2142,20 @@ extern "C" int b200mppi_batch_destroy(b200mppi_batch* b) {
 }
 
 static int batch_init(b200mppi_batch* b) {
-  const size_t K = b->pl.size(), K1 = b->nmap, K2 = K - K1;   // empty sections take no bytes
-  b->off_sample = align256(K1 * sizeof(NoiseDesc));
-  b->off_roll = b->off_sample + align256(K1 * sizeof(SampleGridsV2Args));
-  b->off_nprep = b->off_roll + align256(K1 * sizeof(RolloutArgs));
-  b->off_win = b->off_nprep + align256(K2 * sizeof(NoisePrepDesc));
-  b->off_tm = b->off_win + align256(K2 * sizeof(RolloutWinArgs));
-  b->off_cvar = b->off_tm + align256(K2 * sizeof(b200mppi_planner::tmaps));
-  b->off_upd = b->off_cvar + align256(K2 * sizeof(CvarDesc));
-  b->desc_bytes = b->off_upd + align256(K * sizeof(UpdateBatchDesc));
-  b->off_vis = b->desc_bytes;
-  b->off_visd = b->off_vis + align256(K * sizeof(RolloutParams));
-  b->vis_bytes = b->off_visd + align256(K * sizeof(VisBatchDesc)) - b->off_vis;
+  const size_t K = b->pl.size(), K1 = b->nmap, K2 = K - K1;
+  Sections s;
+  s.take(K1 * sizeof(NoiseDesc));                      // at 0
+  b->off_sample = s.take(K1 * sizeof(SampleGridsV2Args));
+  b->off_roll = s.take(K1 * sizeof(RolloutArgs));
+  b->off_nprep = s.take(K2 * sizeof(NoisePrepDesc));
+  b->off_win = s.take(K2 * sizeof(RolloutWinArgs));
+  b->off_tm = s.take(K2 * sizeof(b200mppi_planner::tmaps));
+  b->off_cvar = s.take(K2 * sizeof(CvarDesc));
+  b->off_upd = s.take(K * sizeof(UpdateBatchDesc));
+  b->desc_bytes = s.end;
+  b->off_vis = s.take(K * sizeof(RolloutParams));
+  b->off_visd = s.take(K * sizeof(VisBatchDesc));
+  b->vis_bytes = s.end - b->off_vis;
   CU(cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
   b->own_stream = true;
   CU(cudaEventCreateWithFlags(&b->ev, cudaEventDisableTiming));
@@ -2847,33 +2858,64 @@ struct TrialClass {
   int mrows = 0, ncact = 0;
 };
 
-// The MODE_TDM planners' trial sampler sets (set0: parity 0), launch classes and per-class launch sizes.  Every pair must
-// be fused (identical generator streams, well-formed PMF at its alpha, lin != ang).
-static int stochastic_trial_plans(b200mppi_batch* b, const TdmGroups& gr, const std::string& fn,
-                                  std::vector<SamplePlan>& plans, std::vector<SampleGridsV2Args>& set0,
-                                  LaunchClasses& lc, std::vector<TrialClass>& cls) {
-  b200mppi_planner* const* sp = b->pl.data() + b->nmap;   // the MODE_TDM planners; gr counts from there
-  const int K = (int)b->pl.size() - b->nmap, G = gr.size();
-  plans.resize(G);
-  for (int g = 0; g < G; ++g) {                       // one plan per TDM group
-    b200mppi_planner* p = sp[gr.lead(g)];
-    const int rc = plan_sampling(p->lin, p->ang, sample_alpha(p), b->stream, &plans[g]);
+// The planners of one kind in a trial call: the one-map planners pl[0 .. nmap) or the MODE_TDM planners pl[nmap .. K).
+// Each kind's launches index its planners, groups and classes from lo (`active` too: active + lo).
+struct TrialPart {
+  int lo = 0, n = 0;
+  TdmGroups gr;
+  std::vector<SamplePlan> plans;
+  std::vector<SampleGridsV2Args> set0;                 // parity 0, one per TDM group
+  LaunchClasses lc;
+  std::vector<TrialClass> cls;
+  int G = 0, C = 0;                                    // groups whose pairs are sampled, sampler launch classes
+  bool grouped = false;                                // shared pairs: the group-aware sampler launches
+  // in the call's device buffer: the sampler sets of each parity, class c's pairs cls_d + lc.first[c], and the group
+  // descriptors and members (null: no shared pair)
+  const SampleGridsV2Args* set_d[2] = {};
+  const int* cls_d = nullptr;
+  const SampleGroupDesc* grp_d = nullptr;
+  const int* mem_d = nullptr;
+};
+
+// A kind's trial sampler plans, one per TDM group (set0: parity 0, each pair's whole-map plan), and their launch classes.
+// Every pair must be fused (identical generator streams, well-formed PMF at its alpha, lin != ang): its samplings join
+// its class's one sampler launch.
+static int trial_plans(b200mppi_batch* b, TrialPart& q, bool stochastic, const std::string& fn) {
+  b200mppi_planner* const* pl = b->pl.data() + q.lo;
+  q.G = q.gr.size();
+  q.plans.resize(q.G);
+  q.set0.resize(q.G);
+  for (int g = 0; g < q.G; ++g) {
+    const b200mppi_planner* p = pl[q.gr.lead(g)];
+    const int rc = plan_sampling(p->lin, p->ang, stochastic ? sample_alpha(p) : BATCH_ALPHA, b->stream, &q.plans[g]);
     if (rc) return rc;
-    if (!plans[g].fused)
-      return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(b->nmap + gr.lead(g)) + ": its TDM pair cannot join the "
-                                   "batch's one sampler launch (lin == ang, or map geometry, PMF or generator streams "
-                                   "differ from planner 0's)");
+    if (!q.plans[g].fused)
+      return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(q.lo + q.gr.lead(g)) + ": its TDM pair cannot join "
+                                   "the batch's one sampler launch (" + (stochastic ? "lin == ang, or " : "") +
+                                   "map geometry, PMF or generator streams differ from planner 0's)");
+    q.set0[g] = q.plans[g].a[0];
   }
-  lc = launch_classes(plans);
+  q.lc = launch_classes(q.plans);
+  q.C = q.lc.size();
+  q.grouped = q.gr.shared();
+  q.cls.assign(q.C, TrialClass{});
+  return B200MPPI_OK;
+}
+
+// The MODE_TDM planners' per-class launch sizes, and their parity-0 sets made the boxed launch's.
+static int stochastic_trial_classes(b200mppi_batch* b, TrialPart& q, const std::string& fn) {
+  b200mppi_planner* const* sp = b->pl.data() + q.lo;
+  const TdmGroups& gr = q.gr;
+  const LaunchClasses& lc = q.lc;
   // a class's sampler launch is sized for the largest box the static bound allows (reach_box_decide: at most 2 R / res + 5
   // cells a side) over its planners that sample a box: mrows tile rows x ncact tile columns with the boxed launch's maps
   // per CTA, each the largest over the class's pairs of what the pair's own tile size needs.  Whole-map steps loop over
   // such groups.  x0 moves during a trial, so R's rounding terms take their bounds from the padded map's limits (a box
   // exists only for an x0 inside them).
-  std::vector<double> span(G, -1.0);                  // per pair: cells a side + margin (-1: no planner gets a box)
-  for (int i = 0; i < K; ++i) {
+  std::vector<double> span(q.G, -1.0);                // per pair: cells a side + margin (-1: no planner gets a box)
+  for (int i = 0; i < q.n; ++i) {
     ReachBoxConst c;
-    fill_reach_const(sp[i], plans[gr.of[i]], &c);
+    fill_reach_const(sp[i], q.plans[gr.of[i]], &c);
     if (c.mode == 0) continue;
     const double w = (double)c.cols * (double)c.res, h = (double)c.rows * (double)c.res;
     const double A = std::fmax(std::fabs((double)c.pxl), std::fabs((double)c.pxl + w)) +
@@ -2883,14 +2925,13 @@ static int stochastic_trial_plans(b200mppi_batch* b, const TdmGroups& gr, const 
     if (!(R >= 0.0)) continue;                        // that planner never gets a box
     span[gr.of[i]] = std::fmax(span[gr.of[i]], 2.0 * R / (double)c.res + 8.0);
   }
-  cls.assign(lc.size(), TrialClass{});
-  for (int c = 0; c < lc.size(); ++c) {
-    TrialClass& tc = cls[c];
-    const SampleGridsV2Args& sg0 = plans[lc.groups[lc.first[c]]].a[0];
+  for (int c = 0; c < q.C; ++c) {
+    TrialClass& tc = q.cls[c];
+    const SampleGridsV2Args& sg0 = q.plans[lc.groups[lc.first[c]]].a[0];
     for (int j = lc.first[c]; j < lc.first[c + 1]; ++j) {
       const int g = lc.groups[j];
       if (span[g] < 0.0) continue;
-      const SampleGridsV2Args& sg = plans[g].a[0];
+      const SampleGridsV2Args& sg = q.plans[g].a[0];
       const int nrow = (sg.rows + sg.tx - 1) / sg.tx, ncol = (sg.cols + sg.ty - 1) / sg.ty;
       const bool small = span[g] < (double)(sg.rows + sg.cols);
       tc.mrows = std::max(tc.mrows, small ? std::min(sg.tx, (int)span[g] / nrow + 2) : sg.tx);
@@ -2904,113 +2945,87 @@ static int stochastic_trial_plans(b200mppi_batch* b, const TdmGroups& gr, const 
     for (int j = lc.first[c]; j < lc.first[c + 1]; ++j) {
       const int g = lc.groups[j];
       const b200mppi_tdm* l = sp[gr.lead(g)]->lin;
-      set0[g] = plans[g].a[0];
-      set0[g].segs = l->box_segs; set0[g].seg_rows = l->box_seg_rows; set0[g].jump = l->jump_box_d;
-      set0[g].write_states = 0;
-      set0[g].gm = gm_b;
-      if (!sample_box_batch_fits(set0[g], tc.ncact))
-        return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(b->nmap + gr.lead(lc.groups[lc.first[c]])) +
+      SampleGridsV2Args& s0 = q.set0[g];
+      s0.segs = l->box_segs; s0.seg_rows = l->box_seg_rows; s0.jump = l->jump_box_d;
+      s0.write_states = 0;
+      s0.gm = gm_b;
+      if (!sample_box_batch_fits(s0, tc.ncact))
+        return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(q.lo + gr.lead(lc.groups[lc.first[c]])) +
                                      ": the batched sampler launch (" + std::to_string(tc.ncact) + " tile columns x " +
                                      std::to_string(gm_b) + " maps per CTA) does not fit a CTA");
-      mem.push_back(&set0[g]);
+      mem.push_back(&s0);
     }
     tc.L = sample_box_class_launch(mem.data(), (int)mem.size(), tc.mrows, tc.ncact);
   }
   return B200MPPI_OK;
 }
 
-// The one-map planners' trial sampler sets (set0: parity 0, each pair's whole-map plan), launch classes and their shapes.
-// Every pair must be fused.
-static int onemap_trial_plans(b200mppi_batch* b, const TdmGroups& gr, std::vector<SamplePlan>& plans,
-                              std::vector<SampleGridsV2Args>& set0, LaunchClasses& lc, std::vector<TrialClass>& cls) {
-  const int G = gr.size();
-  plans.resize(G);
-  for (int g = 0; g < G; ++g) {
-    const b200mppi_planner* p = b->pl[gr.lead(g)];
-    const int rc = plan_sampling(p->lin, p->ang, BATCH_ALPHA, b->stream, &plans[g]);
-    if (rc) return rc;
-    if (!plans[g].fused)
-      return fail(B200MPPI_EINVAL, "run_trials: planner " + std::to_string(gr.lead(g)) + ": its TDM pair cannot join "
-                                   "the batch's one sampler launch (map geometry, PMF or generator streams differ from "
-                                   "planner 0's)");
-    set0[g] = plans[g].a[0];
-  }
-  lc = launch_classes(plans);
-  cls.assign(lc.size(), TrialClass{});
-  for (int c = 0; c < lc.size(); ++c) {
+// The one-map planners' per-class launch shapes over their whole-map plans
+static void onemap_trial_classes(TrialPart& q) {
+  for (int c = 0; c < q.C; ++c) {
     std::vector<const SampleGridsV2Args*> mem;
-    for (int j = lc.first[c]; j < lc.first[c + 1]; ++j) mem.push_back(&set0[lc.groups[j]]);
-    cls[c].L = sample_class_launch(mem.data(), (int)mem.size());
+    for (int j = q.lc.first[c]; j < q.lc.first[c + 1]; ++j) mem.push_back(&q.set0[q.lc.groups[j]]);
+    q.cls[c].L = sample_class_launch(mem.data(), (int)mem.size());
   }
-  return B200MPPI_OK;
 }
 
-// The planners of one kind in a trial call: the one-map planners pl[0 .. nmap) or the MODE_TDM planners pl[nmap .. K).
-// Each kind's launches index its planners, groups and classes from lo (`active` too: active + lo).
-struct TrialPart {
-  int lo = 0, n = 0;
-  TdmGroups gr;
-  std::vector<SamplePlan> plans;
-  std::vector<SampleGridsV2Args> set0;                 // parity 0, one per TDM group
-  LaunchClasses lc;
-  std::vector<TrialClass> cls;
-  int G = 0, C = 0;                                    // groups whose pairs are sampled, sampler launch classes
-  bool grouped = false;                                // shared pairs: the group-aware sampler launches
-  size_t off_s0 = 0, off_s1 = 0, off_grp = 0, off_mem = 0, off_cls = 0;
+// Byte offsets into a trial call's one device allocation, in the order trial_layout takes them
+struct TrialLayout {
+  struct Part { size_t set[2] = {}, grp = 0, mem = 0, cls = 0; };   // a kind's sampler sets (by parity), group
+  Part part[2];                                                     // descriptors, members and class lists
+  size_t box = 0, rec = 0, grec = 0, state = 0, con = 0, res = 0, res_end = 0, tr = 0, act = 0, seq = 0, start = 0;
+  size_t vis = 0, rflag = 0, head = 0;                 // head: the sections staged and uploaded with one copy
+  std::vector<size_t> grid;                            // per slot
+  size_t vrec = 0, xh = 0, uh = 0, total = 0;
 };
 
-// The closed-loop trials of every kind of batch.  Stochastic trials also move each planner's reach box with the robot;
-// with box_mode 2 and num_opt 1 it depends on the controls drawn, so the batched boxed sampler decides it on the device
-// (reach_box_decide, the function sample_finish calls) and a step needs no host round trip.  Per step: num_opt x
-// (one-map: noise, [first iteration, not barebone: per launch class the sampler], rollout; stochastic: noise + controls,
-// [first iteration: per launch class the boxed sampler, then the state advance], windowed rollout, CVaR; then ONE
-// update over all K planners) and the plant step, which for stochastic planners also moves the rollout window and for
-// barebone trials counts obstacle contacts.  With C launch classes (launch_classes; 1 for a batch on one map geometry)
-// that is 3 num_opt + 1 + C launches per one-map step, 4 num_opt + 1 + 2 C per stochastic step, 3 num_opt + 1 per
-// barebone step, and 6 num_opt + 1 + C1 + 2 C2 per step of a mixed batch holding both kinds (C1, C2: the one-map and the
-// stochastic classes).
-// record_every = n > 0 records the visualisation rollouts of every step s with s % n == 0, after the step's last update
-// and before the plant step (which shifts u_cur and overwrites x0): one batched launch, and for stochastic planners first
-// one launch per stochastic launch class that completes maps [0, V) of every pair whose step sampled a box (the maps the
-// rollouts read).
-// Device buffer of a call: [descriptors (b->h_desc's layout; the one-map parity-0 sampler set is its own section there)
-// | stochastic: the parity-0 sampler set, the parity-1 set | one-map, not barebone: the parity-1 set | stochastic: box
-// descriptors, box records | shared TDM pairs: group records (stochastic), group descriptors, members (one-map, then
-// stochastic) | not barebone: the launch classes' pairs | states | barebone: contacts (per slot) |
-// trials | active K + count | recording: vis descriptors | recording sequences: the record flags (K) | not barebone: the
-// host grids | recording: the records (slots, R, V, T+1, 3) | xhist | uhist].  The pinned staging mirrors it up to the grids, then holds
-// xhist and uhist: the float64 ground-truth grids (tens of MB for a batch of large maps) are copied straight from the
-// caller's arrays (a slot whose grids are planes of a realisation set has no grid section: the plant reads the planes), and the written records (of K * R * V * (T+1) * 12 bytes, 145 MB for K 8, 150 steps, V 100, T 100)
-// straight into the caller's array.
-// Trial sequences (episodes non-null, b200mppi_batch_run_trial_sequences): planner i runs episodes[i] episodes back to
-// back, descriptors, histories and results per slot (planner-major: planner i's are slots first[i] .. first[i + 1]),
-// through the same step loop for up to max_i episodes[i] * max_steps steps; the plant step (plant_step_seq_kernel)
-// moves a planner to its next episode without a launch, and the commit below follows each planner's total steps.
-// A recording sequence records at each episode's own steps t with t % record_every == 0: the plant step sets each
-// planner's record flag and record pointer for the next step (SeqArgs), and the record launches run at every step,
-// gated by those flags (1 + C2 launches per step more than without recording).
-static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_trial_desc* trials, int32_t max_steps,
-                            double* xhist, float* uhist, b200mppi_trial_result* results, int32_t* contact_steps,
-                            int32_t record_every, float* rollouts, size_t rollout_bytes, int32_t* steps_issued,
-                            const int32_t* episodes, int32_t reset_x0) {
-  const bool stochastic = kind == TrialKind::stochastic, barebone = kind == TrialKind::barebone;
-  const bool mixed = kind == TrialKind::mixed;
-  const bool seq = episodes != nullptr;
-  const std::string fn = seq ? (barebone ? "run_barebone_trial_sequences" : "run_trial_sequences") : stochastic ? "run_stochastic_trials"
-                         : barebone ? "run_barebone_trials" : mixed ? "run_mixed_trials" : "run_trials";
-  if (!b) return fail(B200MPPI_EINVAL, "null batch");
-  std::vector<int> first(b->pl.size() + 1, 0);        // planner i's slots: first[i] .. first[i + 1]
-  int max_episodes = 1;
-  for (size_t i = 0; i < b->pl.size(); ++i) {
-    const int E = seq ? episodes[i] : 1;
+// One trial call passed through its phases: the request, both kinds' parts, the layout and the buffers
+struct TrialCall {
+  // the request: batch_run_trials' arguments (S: max_steps; episodes null: one episode per planner)
+  b200mppi_batch* b; TrialKind kind; const b200mppi_trial_desc* trials; int S;
+  double* xhist; float* uhist; b200mppi_trial_result* results; int32_t* contact_steps;
+  int record_every; float* rollouts; size_t rollout_bytes; const int32_t* episodes; bool reset_x0;
+  std::string fn;                                      // prefixes the refusals
+  bool barebone = false, seq = false, record = false, rec_seq = false;
+  int K = 0, K1 = 0, K2 = 0, nslot = 0, max_episodes = 1;   // the one-map planners, then the MODE_TDM planners
+  std::vector<int> first;                              // planner i's slots: first[i] .. first[i + 1]
+  std::vector<char> in_place;                          // slots whose grids are realisation planes, read where they are
+  int V = 0, R = 0;                                    // recording: rollouts per record, records per slot
+  size_t per = 0, rec_bytes = 0;                       // floats of one record, bytes of the device's records
+  int WW = 0, WH = 0;                                  // the stochastic planners' window geometry
+  bool masks01 = true;
+  TrialPart P[2];                                      // one-map, stochastic
+  TrialLayout L;
+  unsigned char* d = nullptr;                          // the device buffer (L)
+  unsigned char* h = nullptr;                          // its pinned staging: the head, then the histories
+  PlantArgs pa{};
+  SeqArgs sa{};
+  RolloutWinArgs g0{};                                 // the stochastic planners' first windowed rollout descriptor
+};
+
+// Everything a trial call checks before it allocates or issues anything
+static int trial_call_validate(TrialCall& t) {
+  b200mppi_batch* b = t.b;
+  const bool stochastic = t.kind == TrialKind::stochastic, mixed = t.kind == TrialKind::mixed;
+  t.barebone = t.kind == TrialKind::barebone;
+  t.seq = t.episodes != nullptr;
+  t.fn = t.seq ? (t.barebone ? "run_barebone_trial_sequences" : "run_trial_sequences") : stochastic ? "run_stochastic_trials"
+         : t.barebone ? "run_barebone_trials" : mixed ? "run_mixed_trials" : "run_trials";
+  const std::string& fn = t.fn;
+  t.K = (int)b->pl.size();
+  t.K1 = b->nmap;
+  t.K2 = t.K - t.K1;
+  t.first.assign(t.K + 1, 0);
+  for (int i = 0; i < t.K; ++i) {
+    const int E = t.seq ? t.episodes[i] : 1;
     if (E < 1)
       return fail(B200MPPI_EINVAL, fn + ": planner " + std::to_string(i) + ": episode count " + std::to_string(E) + " < 1");
-    if ((int64_t)first[i] + E > (1 << 24))
+    if ((int64_t)t.first[i] + E > (1 << 24))
       return fail(B200MPPI_EINVAL, fn + ": more than 2^24 episodes in all");
-    first[i + 1] = first[i] + E;
-    max_episodes = std::max(max_episodes, E);
+    t.first[i + 1] = t.first[i] + E;
+    t.max_episodes = std::max(t.max_episodes, E);
   }
-  if ((int64_t)max_episodes * max_steps > INT32_MAX)
+  if ((int64_t)t.max_episodes * t.S > INT32_MAX)
     return fail(B200MPPI_EINVAL, fn + ": max_steps x the largest episode count exceeds 2^31 - 1 steps");
   if (b->mixed && !mixed)
     return fail(B200MPPI_EINVAL, fn + ": a mixed batch (b200mppi_batch_create_mixed) runs its trials with "
@@ -3018,211 +3033,202 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
   if (!b->mixed && mixed)
     return fail(B200MPPI_EINVAL, fn + ": planner 0 is " + mode_name(b->mode) + " in a batch that is not mixed (mixed "
                                  "trials run batches made by b200mppi_batch_create_mixed)");
-  if (barebone && b->mode != B200MPPI_MODE_BAREBONE)
+  if (t.barebone && b->mode != B200MPPI_MODE_BAREBONE)
     return fail(B200MPPI_EINVAL, fn + ": planner 0 is " + mode_name(b->mode) + " (barebone trials run MODE_BAREBONE "
                                  "batches; b200mppi_batch_run_trials and b200mppi_batch_run_stochastic_trials run the "
                                  "others)");
-  if (b->stochastic && kind == TrialKind::onemap)
+  if (b->stochastic && t.kind == TrialKind::onemap)
     return fail(B200MPPI_EINVAL, "run_trials: planner 0 is MODE_TDM (trials run det-dynamics or speed-map batches: a "
                                  "stochastic solve sizes each planner's map-sampling box on the host)");
   if (!b->stochastic && stochastic)
     return fail(B200MPPI_EINVAL, fn + ": planner 0 is " + mode_name(b->mode) +
                                      " (stochastic trials run MODE_TDM batches; b200mppi_batch_run_trials runs the others)");
-  std::vector<char> in_place;                         // slots whose grids are realisation planes, read where they are
-  int rc = trial_validate(b, kind, trials, max_steps, fn.c_str(), first, seq, in_place);
+  int rc = trial_validate(b, t.kind, t.trials, t.S, fn.c_str(), t.first, t.seq, t.in_place);
   if (rc) return rc;
-  if (!xhist || !uhist || !results || (barebone && !contact_steps))
+  if (!t.xhist || !t.uhist || !t.results || (t.barebone && !t.contact_steps))
     return fail(B200MPPI_EINVAL, fn + ": null output buffer");
-  const int K = (int)b->pl.size(), T = b->T, N = b->N, S = max_steps, nslot = first[K];
-  const int K1 = b->nmap, K2 = K - K1;                 // the one-map planners, then the MODE_TDM planners
-  const bool record = record_every > 0;
-  int V = 0, R = 0;
-  // floats of one record; bytes of the device's records (per slot) and of the caller's (K, max_episodes) slabs, so a
-  // sequence's records need no re-layout on the host (one episode per planner: the same two sizes)
-  size_t per = 0, rec_bytes = 0, out_bytes = 0;
-  if (record) {
-    if ((rc = batch_vis_validate(b, fn, &V))) return rc;
-    R = (S + record_every - 1) / record_every;
-    per = (size_t)V * (T + 1) * 3;
-    if ((double)K * max_episodes * R * per * sizeof(float) > 4e18)
+  t.nslot = t.first[t.K];
+  t.record = t.record_every > 0;
+  t.rec_seq = t.record && t.seq;                       // records gated per planner on the device (SeqArgs::rec_flag)
+  if (t.record) {
+    // bytes of the device's records (per slot) and of the caller's (K, max_episodes) slabs, so a sequence's records
+    // need no re-layout on the host (one episode per planner: the same two sizes)
+    if ((rc = batch_vis_validate(b, fn, &t.V))) return rc;
+    t.R = (t.S + t.record_every - 1) / t.record_every;
+    t.per = (size_t)t.V * (b->T + 1) * 3;
+    if ((double)t.K * t.max_episodes * t.R * t.per * sizeof(float) > 4e18)
       return fail(B200MPPI_EINVAL, fn + ": the records exceed 4e18 bytes");
-    rec_bytes = (size_t)nslot * R * per * sizeof(float);
-    out_bytes = (size_t)K * max_episodes * R * per * sizeof(float);
-    if (!rollouts || rollout_bytes != out_bytes)
-      return fail(B200MPPI_EINVAL, fn + ": rollouts buffer of " + std::to_string(rollout_bytes) + " bytes, the records " +
-                                   (seq ? "(K, Emax" : "(K") + ", R, V, T+1, 3) float32 need " + std::to_string(out_bytes));
+    t.rec_bytes = (size_t)t.nslot * t.R * t.per * sizeof(float);
+    const size_t out_bytes = (size_t)t.K * t.max_episodes * t.R * t.per * sizeof(float);
+    if (!t.rollouts || t.rollout_bytes != out_bytes)
+      return fail(B200MPPI_EINVAL, fn + ": rollouts buffer of " + std::to_string(t.rollout_bytes) + " bytes, the records " +
+                                   (t.seq ? "(K, Emax" : "(K") + ", R, V, T+1, 3) float32 need " + std::to_string(out_bytes));
   }
-  int WW = 0, WH = 0;
-  if (K2 > 0 && (rc = stochastic_validate(b, fn.c_str(), &WW, &WH))) return rc;
+  if (t.K2 > 0 && (rc = stochastic_validate(b, fn.c_str(), &t.WW, &t.WH))) return rc;
+  return B200MPPI_OK;
+}
+
+// The sampler plans and launch classes of both kinds (their host preparation may synchronise the stream): every TDM
+// group's pair must join the one launch of its class.  Groups of more than one planner (shared pairs) take the
+// group-aware sampler launches.
+static int trial_call_plan(TrialCall& t) {
+  b200mppi_batch* b = t.b;
   CU(cudaSetDevice(b->device));
-  cudaStream_t st = b->stream;
-  // the sampler plans first (their host preparation may synchronise the stream): every TDM group's pair must join the
-  // one launch of its kind.  Groups of more than one planner (shared pairs) take the group-aware sampler launches.
-  TrialPart P[2];                                      // one-map, stochastic
-  P[0].n = K1; P[1].lo = K1; P[1].n = K2;
-  for (TrialPart& q : P) {
-    q.gr = batch_groups(b, q.lo, q.lo + q.n);
-    q.set0.resize(q.n);
+  t.P[0].n = t.K1; t.P[1].lo = t.K1; t.P[1].n = t.K2;
+  for (TrialPart& q : t.P) q.gr = batch_groups(b, q.lo, q.lo + q.n);
+  int rc;
+  if (t.K2 > 0 && ((rc = trial_plans(b, t.P[1], true, t.fn)) || (rc = stochastic_trial_classes(b, t.P[1], t.fn))))
+    return rc;
+  if (t.K1 > 0 && !t.barebone) {
+    if ((rc = trial_plans(b, t.P[0], false, "run_trials"))) return rc;
+    onemap_trial_classes(t.P[0]);
   }
-  if (K2 > 0 && (rc = stochastic_trial_plans(b, P[1].gr, fn, P[1].plans, P[1].set0, P[1].lc, P[1].cls))) return rc;
-  if (K1 > 0 && !barebone && (rc = onemap_trial_plans(b, P[0].gr, P[0].plans, P[0].set0, P[0].lc, P[0].cls))) return rc;
-  for (TrialPart& q : P) {
-    if (q.n == 0 || (barebone && &q == &P[0])) continue;
-    q.G = q.gr.size();
-    q.C = q.lc.size();
-    q.grouped = q.gr.shared();
-  }
-  if ((rc = batch_wait_members(b))) return rc;
-  const size_t ngrec = P[1].grouped ? (size_t)P[1].G : 0;   // stochastic shared pairs' group records
-  const size_t szs = sizeof(SampleGridsV2Args);
-  P[0].off_s0 = b->off_sample;
-  P[1].off_s0 = b->desc_bytes;
-  P[1].off_s1 = P[1].off_s0 + align256(P[1].G * szs);
-  P[0].off_s1 = P[1].off_s1 + align256(P[1].G * szs);
-  const size_t off_box = P[0].off_s1 + align256(P[0].G * szs);
-  const size_t off_rec = off_box + align256((size_t)K2 * sizeof(SampleBoxDesc));
-  const size_t off_grec = off_rec + align256((size_t)K2 * 5 * sizeof(int));
-  size_t off_grp = off_grec + align256(ngrec * 5 * sizeof(int)), ngrp = 0, nmem = 0, ncls = 0;
-  for (TrialPart& q : P) {
-    q.off_grp = ngrp; q.off_mem = nmem; q.off_cls = ncls;     // entries, made byte offsets below
-    if (q.grouped) { ngrp += q.G; nmem += q.n; }
-    ncls += q.G;
-  }
-  const size_t off_mem = off_grp + align256(ngrp * sizeof(SampleGroupDesc));
-  const size_t off_cls = off_mem + align256(nmem * sizeof(int));
-  for (TrialPart& q : P) {
-    q.off_grp = off_grp + q.off_grp * sizeof(SampleGroupDesc);
-    q.off_mem = off_mem + q.off_mem * sizeof(int);
-    q.off_cls = off_cls + q.off_cls * sizeof(int);
-  }
-  const size_t ncon = barebone ? (size_t)nslot : 0;    // barebone-only section, per slot
-  const size_t off_state = off_cls + align256(ncls * sizeof(int));
-  const size_t off_con = off_state + align256((size_t)K * sizeof(TrialState));
-  const size_t nres = seq ? (size_t)nslot : 0;          // sequence-only sections: per-slot results and start poses
-  const size_t off_res = off_con + align256(ncon * sizeof(int));
-  const size_t off_tr = off_res + align256(nres * sizeof(TrialState));
-  const size_t off_act = off_tr + align256((size_t)nslot * sizeof(TrialDev));
-  const size_t off_seq = off_act + align256((size_t)(K + 1) * sizeof(int));      // first (K + 1), episode (K)
-  const size_t off_start = off_seq + align256((seq ? (size_t)(2 * K + 1) : 0) * sizeof(int));
-  const size_t off_vis = off_start + align256(nres * 3 * sizeof(double));
-  const bool rec_seq = record && seq;                  // records gated per planner on the device (SeqArgs::rec_flag)
-  const size_t off_rflag = off_vis + align256((record ? (size_t)K : 0) * sizeof(VisBatchDesc));
-  size_t off = off_rflag + align256((rec_seq ? (size_t)K : 0) * sizeof(int));
-  const size_t head = off;
-  std::vector<size_t> off_grid(nslot);
-  for (int j = 0; j < nslot; ++j) {
-    off_grid[j] = off;
-    if (!barebone && !in_place[j]) off += align256((size_t)2 * trials[j].height * trials[j].width * sizeof(double));
-  }
-  const size_t off_vrec = off;
-  off += align256(rec_bytes);
-  const size_t off_xh = off, off_uh = off_xh + align256((size_t)nslot * (S + 1) * 3 * sizeof(double));
-  const size_t total = off_uh + align256((size_t)nslot * S * 2 * sizeof(float));
-  struct Buffers {                                     // freed on every return
-    unsigned char* d = nullptr;
-    unsigned char* h = nullptr;
-    cudaEvent_t ev[TRIAL_POLL] = {};
-    ~Buffers() {
-      cudaFree(d);
-      if (h) cudaFreeHost(h);
-      for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
-    }
-  } buf;
-  if (cudaMalloc(&buf.d, total) != cudaSuccess) {
-    buf.d = nullptr;
-    cudaGetLastError();                                // not sticky: later calls start clean
-    return fail(B200MPPI_ECUDA, fn + ": cudaMalloc of " + std::to_string(total) + " bytes");
-  }
-  if (cudaMallocHost(&buf.h, head + (total - off_xh)) != cudaSuccess) {
-    buf.h = nullptr;
-    return fail(B200MPPI_ECUDA, fn + ": cudaMallocHost");
-  }
-  unsigned char* d = buf.d;
-  unsigned char* h = buf.h;
-  bool masks01 = true;
+  return batch_wait_members(b);
+}
+
+static TrialLayout trial_layout(const TrialCall& t) {
+  const size_t K = t.K, K2 = t.K2, nslot = t.nslot, S = t.S, szs = sizeof(SampleGridsV2Args);
+  const size_t nres = t.seq ? nslot : 0;               // sequence-only sections: per-slot results and start poses
+  const TrialPart* P = t.P;
+  TrialLayout L;
+  TrialLayout::Part& om = L.part[0];
+  TrialLayout::Part& sto = L.part[1];
+  // the batch's descriptors in b->h_desc's layout, where the one-map parity-0 sampler set is a section of its own
+  Sections s{t.b->desc_bytes};
+  om.set[0] = t.b->off_sample;
+  sto.set[0] = s.take(P[1].G * szs);
+  sto.set[1] = s.take(P[1].G * szs);
+  om.set[1] = s.take(P[0].G * szs);
+  L.box = s.take(K2 * sizeof(SampleBoxDesc));
+  L.rec = s.take(K2 * 5 * sizeof(int));
+  L.grec = s.take((P[1].grouped ? P[1].G : 0) * 5 * sizeof(int));   // stochastic shared pairs' group records
+  // one section each of group descriptors, members and class lists, the one-map kind's entries first
+  const size_t ngrp0 = P[0].grouped ? P[0].G : 0, nmem0 = P[0].grouped ? P[0].n : 0;
+  om.grp = s.take((ngrp0 + (P[1].grouped ? P[1].G : 0)) * sizeof(SampleGroupDesc));
+  om.mem = s.take((nmem0 + (P[1].grouped ? P[1].n : 0)) * sizeof(int));
+  om.cls = s.take((size_t)(P[0].G + P[1].G) * sizeof(int));
+  sto.grp = om.grp + ngrp0 * sizeof(SampleGroupDesc);
+  sto.mem = om.mem + nmem0 * sizeof(int);
+  sto.cls = om.cls + P[0].G * sizeof(int);
+  L.state = s.take(K * sizeof(TrialState));
+  L.con = s.take((t.barebone ? nslot : 0) * sizeof(int));   // barebone contacts, per slot
+  L.res = s.take(nres * sizeof(TrialState));
+  L.res_end = s.end;
+  L.tr = s.take(nslot * sizeof(TrialDev));
+  L.act = s.take((K + 1) * sizeof(int));               // active (K), the count of running planners
+  L.seq = s.take((t.seq ? 2 * K + 1 : 0) * sizeof(int));     // first (K + 1), episode (K)
+  L.start = s.take(nres * 3 * sizeof(double));
+  L.vis = s.take((t.record ? K : 0) * sizeof(VisBatchDesc));
+  L.rflag = s.take((t.rec_seq ? K : 0) * sizeof(int));
+  L.head = s.end;
+  // The pinned staging holds the head and the histories only.  The float64 ground-truth grids (tens of MB for a batch
+  // of large maps) are copied straight from the caller's arrays, and a slot whose grids are planes of a realisation set
+  // has no grid section: the plant reads the planes.  The written records (of K * R * V * (T+1) * 12 bytes, 145 MB for
+  // K 8, 150 steps, V 100, T 100) are copied straight into the caller's array.
+  L.grid.resize(nslot);
+  for (size_t j = 0; j < nslot; ++j)
+    L.grid[j] = s.take(t.barebone || t.in_place[j] ? 0 : 2 * (size_t)t.trials[j].height * t.trials[j].width * sizeof(double));
+  L.vrec = s.take(t.rec_bytes);                        // (slots, R, V, T+1, 3)
+  L.xh = s.take(nslot * (S + 1) * 3 * sizeof(double));
+  L.uh = s.take(nslot * S * 2 * sizeof(float));
+  L.total = s.end;
+  return L;
+}
+
+// Fills the pinned staging's head (the batch's descriptors, per-planner and per-slot trial state, box, vis and sequence
+// descriptors, both parities' sampler sets, group descriptors and members) and uploads it and the host grids.
+static int trial_call_stage(TrialCall& t) {
+  b200mppi_batch* b = t.b;
+  const TrialLayout& L = t.L;
+  unsigned char* d = t.d;
+  unsigned char* h = t.h;
+  const int K = t.K, K1 = t.K1, R = t.R;
+  const std::vector<int>& first = t.first;
+  const b200mppi_trial_desc* trials = t.trials;
   if (K1 > 0) onemap_descs(b, h);
-  if (K2 > 0) stochastic_descs(b, h, WW, WH, &masks01);
-  SampleBoxDesc* hb = reinterpret_cast<SampleBoxDesc*>(h + off_box);
-  TrialState* hst = reinterpret_cast<TrialState*>(h + off_state);
-  TrialDev* ht = reinterpret_cast<TrialDev*>(h + off_tr);
-  int* hact = reinterpret_cast<int*>(h + off_act);
-  int* dact = reinterpret_cast<int*>(d + off_act);
+  if (t.K2 > 0) stochastic_descs(b, h, t.WW, t.WH, &t.masks01);
+  SampleBoxDesc* hb = reinterpret_cast<SampleBoxDesc*>(h + L.box);
+  TrialState* hst = reinterpret_cast<TrialState*>(h + L.state);
+  TrialDev* ht = reinterpret_cast<TrialDev*>(h + L.tr);
+  int* hact = reinterpret_cast<int*>(h + L.act);
+  int* dact = reinterpret_cast<int*>(d + L.act);
   // the rollout descriptors whose x0 the plant step writes: RolloutArgs (one-map), RolloutWinArgs (stochastic)
   RolloutArgs* dr = reinterpret_cast<RolloutArgs*>(d + b->off_roll);
   RolloutWinArgs* dw = reinterpret_cast<RolloutWinArgs*>(d + b->off_win);
-  int* hcon = reinterpret_cast<int*>(h + off_con);
-  VisBatchDesc* hv = reinterpret_cast<VisBatchDesc*>(h + off_vis);
-  float* drec = reinterpret_cast<float*>(d + off_vrec);
+  int* hcon = reinterpret_cast<int*>(h + L.con);
+  VisBatchDesc* hv = reinterpret_cast<VisBatchDesc*>(h + L.vis);
+  float* drec = reinterpret_cast<float*>(d + L.vrec);
   for (int i = 0; i < K; ++i) {
     b200mppi_planner* p = b->pl[i];
     const bool sto = i >= K1;
     const int r = i - K1;                              // a stochastic planner's index in its kind's launches
-    if (record)                                        // x0 from the record the plant step writes; record 0 of slot 0
-      hv[i] = vis_desc(p, sto ? &dw[r].p : &dr[i].p, drec + (size_t)first[i] * R * per);
-    if (rec_seq) reinterpret_cast<int*>(h + off_rflag)[i] = 1;
+    if (t.record)                                      // x0 from the record the plant step writes; record 0 of slot 0
+      hv[i] = vis_desc(p, sto ? &dw[r].p : &dr[i].p, drec + (size_t)first[i] * R * t.per);
+    if (t.rec_seq) reinterpret_cast<int*>(h + L.rflag)[i] = 1;
     hst[i] = TrialState{};
     for (int c = 0; c < 3; ++c) hst[i].x[c] = trials[first[i]].x0[c];
     hact[i] = 1;
     for (int j = first[i]; j < first[i + 1]; ++j) {    // the planner's episodes: one, or its sequence
       const b200mppi_trial_desc& q = trials[j];
-      if (barebone) hcon[j] = 0;
-      TrialDev& t = ht[j];
-      t = TrialDev{};
-      t.dt = q.dt; t.xgoal[0] = q.xgoal[0]; t.xgoal[1] = q.xgoal[1]; t.tol = q.goal_tolerance;
-      t.u_cur = p->u_cur;
-      if (barebone) {                                  // lin null: nominal unicycle, no map; contacts counted
-        t.x0_out = dr[i].p.x0;
-        t.obstacles = p->obstacles; t.num_obstacles = p->num_obstacles;
+      if (t.barebone) hcon[j] = 0;
+      TrialDev& td = ht[j];
+      td = TrialDev{};
+      td.dt = q.dt; td.xgoal[0] = q.xgoal[0]; td.xgoal[1] = q.xgoal[1]; td.tol = q.goal_tolerance;
+      td.u_cur = p->u_cur;
+      if (t.barebone) {                                // lin null: nominal unicycle, no map; contacts counted
+        td.x0_out = dr[i].p.x0;
+        td.obstacles = p->obstacles; td.num_obstacles = p->num_obstacles;
         continue;
       }
-      const double* dg = reinterpret_cast<const double*>(d + off_grid[j]);
-      t.lin = in_place[j] ? q.lin : dg;
-      t.ang = in_place[j] ? q.ang : dg + (size_t)q.height * q.width;
-      t.H = q.height; t.W = q.width;
-      t.xlo = q.xlo; t.ylo = q.ylo; t.res = q.res;
-      t.pxlim[0] = q.pxlim[0]; t.pxlim[1] = q.pxlim[1]; t.pylim[0] = q.pylim[0]; t.pylim[1] = q.pylim[1];
+      const double* dg = reinterpret_cast<const double*>(d + L.grid[j]);
+      td.lin = t.in_place[j] ? q.lin : dg;
+      td.ang = t.in_place[j] ? q.ang : dg + (size_t)q.height * q.width;
+      td.H = q.height; td.W = q.width;
+      td.xlo = q.xlo; td.ylo = q.ylo; td.res = q.res;
+      td.pxlim[0] = q.pxlim[0]; td.pxlim[1] = q.pxlim[1]; td.pylim[0] = q.pylim[0]; td.pylim[1] = q.pylim[1];
       if (!sto) {
-        t.x0_out = dr[i].p.x0;                         // win stays null: one-map rollouts have no window
+        td.x0_out = dr[i].p.x0;                        // win stays null: one-map rollouts have no window
         continue;
       }
       const b200mppi_tdm* l = p->lin;
-      t.x0_out = dw[r].p.x0;
-      t.win = &dw[r].WW;
-      t.win_pxl = l->pxl[0]; t.win_pyl = l->pyl[0]; t.win_res = l->res; t.win_rows = l->rows; t.win_cols = l->cols;
+      td.x0_out = dw[r].p.x0;
+      td.win = &dw[r].WW;
+      td.win_pxl = l->pxl[0]; td.win_pyl = l->pyl[0]; td.win_res = l->res; td.win_rows = l->rows; td.win_cols = l->cols;
     }
     if (!sto) continue;
     reinterpret_cast<CvarDesc*>(h + b->off_cvar)[r].active = dact + i;
-    hb[r] = SampleBoxDesc{{}, dw[r].p.x0, p->reach_d, p->reach_slot ^ 1, reinterpret_cast<int*>(d + off_rec) + 5 * r,
+    hb[r] = SampleBoxDesc{{}, dw[r].p.x0, p->reach_d, p->reach_slot ^ 1, reinterpret_cast<int*>(d + L.rec) + 5 * r,
                           p->lin->jump_tile_d};
-    fill_reach_const(p, P[1].plans[P[1].gr.of[r]], &hb[r].c);
+    fill_reach_const(p, t.P[1].plans[t.P[1].gr.of[r]], &hb[r].c);
   }
-  TrialState* hres = reinterpret_cast<TrialState*>(h + off_res);
-  SeqArgs sa{};
-  if (seq) {                                           // slots that never run keep NOT_RUN and 0 steps
-    int* hseq = reinterpret_cast<int*>(h + off_seq);
-    double* hstart = reinterpret_cast<double*>(h + off_start);
+  if (t.seq) {                                         // slots that never run keep NOT_RUN and 0 steps
+    int* hseq = reinterpret_cast<int*>(h + L.seq);
+    double* hstart = reinterpret_cast<double*>(h + L.start);
+    TrialState* hres = reinterpret_cast<TrialState*>(h + L.res);
     std::copy(first.begin(), first.end(), hseq);
     std::fill(hseq + K + 1, hseq + 2 * K + 1, 0);
-    for (int j = 0; j < nslot; ++j) {
+    for (int j = 0; j < t.nslot; ++j) {
       hres[j] = TrialState{};
       hres[j].status = B200MPPI_TRIAL_NOT_RUN;
       for (int c = 0; c < 3; ++c) hstart[3 * j + c] = trials[j].x0[c];
     }
-    int* dseq = reinterpret_cast<int*>(d + off_seq);
-    sa = SeqArgs{dseq, dseq + K + 1, reinterpret_cast<const double*>(d + off_start),
-                 reinterpret_cast<TrialState*>(d + off_res), reset_x0 ? 1 : 0};
-    if (rec_seq) {
+    int* dseq = reinterpret_cast<int*>(d + L.seq);
+    t.sa = SeqArgs{dseq, dseq + K + 1, reinterpret_cast<const double*>(d + L.start),
+                   reinterpret_cast<TrialState*>(d + L.res), t.reset_x0 ? 1 : 0};
+    if (t.rec_seq) {
       static_assert(sizeof(VisBatchDesc) % sizeof(float*) == 0, "rec_stride counts float* slots");
-      sa.rec_flag = reinterpret_cast<int*>(d + off_rflag);
-      sa.rec_out = &reinterpret_cast<VisBatchDesc*>(d + off_vis)->out;
-      sa.rec = drec;
-      sa.rec_per = (long long)per;
-      sa.rec_every = record_every; sa.rec_R = R; sa.rec_stride = (int)(sizeof(VisBatchDesc) / sizeof(float*));
+      t.sa.rec_flag = reinterpret_cast<int*>(d + L.rflag);
+      t.sa.rec_out = &reinterpret_cast<VisBatchDesc*>(d + L.vis)->out;
+      t.sa.rec = drec;
+      t.sa.rec_per = (long long)t.per;
+      t.sa.rec_every = t.record_every; t.sa.rec_R = R; t.sa.rec_stride = (int)(sizeof(VisBatchDesc) / sizeof(float*));
     }
   }
-  for (TrialPart& q : P) {
-    SampleGridsV2Args* hs0 = reinterpret_cast<SampleGridsV2Args*>(h + q.off_s0);
-    SampleGridsV2Args* hs1 = reinterpret_cast<SampleGridsV2Args*>(h + q.off_s1);
+  for (int k = 0; k < 2; ++k) {
+    TrialPart& q = t.P[k];
+    const TrialLayout::Part& o = L.part[k];
+    SampleGridsV2Args* hs0 = reinterpret_cast<SampleGridsV2Args*>(h + o.set[0]);
+    SampleGridsV2Args* hs1 = reinterpret_cast<SampleGridsV2Args*>(h + o.set[1]);
     for (int g = 0; g < q.G; ++g) {
       // parity 1: the pair samples from the buffers parity 0 wrote into
       hs0[g] = hs1[g] = q.set0[g];
@@ -3232,133 +3238,149 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
         td.states = in;
       }
     }
-    SampleGroupDesc* hg = reinterpret_cast<SampleGroupDesc*>(h + q.off_grp);
-    const bool sto = &q == &P[1];
+    SampleGroupDesc* hg = reinterpret_cast<SampleGroupDesc*>(h + o.grp);
     for (int g = 0; g < q.G && q.grouped; ++g)
-      hg[g] = SampleGroupDesc{q.gr.first[g], q.gr.count(g), sto ? reinterpret_cast<int*>(d + off_grec) + 5 * g : nullptr};
-    if (q.grouped) std::copy(q.gr.members.begin(), q.gr.members.end(), reinterpret_cast<int*>(h + q.off_mem));
-    std::copy(q.lc.groups.begin(), q.lc.groups.end(), reinterpret_cast<int*>(h + q.off_cls));
-  }
-  // per kind: class c's pairs dcls[k] + lc.first[c], the group descriptors and members (null: no shared pair), and the
-  // sampler sets of each parity
-  const int* dcls[2];
-  const SampleGroupDesc* dgrp[2];
-  const int* dmem[2];
-  const SampleGridsV2Args* ds[2][2];
-  for (int k = 0; k < 2; ++k) {
-    dcls[k] = reinterpret_cast<const int*>(d + P[k].off_cls);
-    dgrp[k] = P[k].grouped ? reinterpret_cast<const SampleGroupDesc*>(d + P[k].off_grp) : nullptr;
-    dmem[k] = P[k].grouped ? reinterpret_cast<const int*>(d + P[k].off_mem) : nullptr;
-    ds[k][0] = reinterpret_cast<const SampleGridsV2Args*>(d + P[k].off_s0);
-    ds[k][1] = reinterpret_cast<const SampleGridsV2Args*>(d + P[k].off_s1);
+      hg[g] = SampleGroupDesc{q.gr.first[g], q.gr.count(g), k == 1 ? reinterpret_cast<int*>(d + L.grec) + 5 * g : nullptr};
+    if (q.grouped) std::copy(q.gr.members.begin(), q.gr.members.end(), reinterpret_cast<int*>(h + o.mem));
+    std::copy(q.lc.groups.begin(), q.lc.groups.end(), reinterpret_cast<int*>(h + o.cls));
+    q.set_d[0] = reinterpret_cast<const SampleGridsV2Args*>(d + o.set[0]);
+    q.set_d[1] = reinterpret_cast<const SampleGridsV2Args*>(d + o.set[1]);
+    q.cls_d = reinterpret_cast<const int*>(d + o.cls);
+    q.grp_d = q.grouped ? reinterpret_cast<const SampleGroupDesc*>(d + o.grp) : nullptr;
+    q.mem_d = q.grouped ? reinterpret_cast<const int*>(d + o.mem) : nullptr;
   }
   hact[K] = K;
-  const RolloutWinArgs g0 = K2 > 0 ? *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win) : RolloutWinArgs{};
-  CU(cudaMemcpyAsync(d, h, head, cudaMemcpyHostToDevice, st));
-  for (int j = 0; j < nslot && !barebone; ++j) {      // pageable sources: staged by the driver before the call returns
-    if (in_place[j]) continue;
+  if (t.K2 > 0) t.g0 = *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win);
+  cudaStream_t st = b->stream;
+  CU(cudaMemcpyAsync(d, h, L.head, cudaMemcpyHostToDevice, st));
+  for (int j = 0; j < t.nslot && !t.barebone; ++j) {  // pageable sources: staged by the driver before the call returns
+    if (t.in_place[j]) continue;
     const size_t bytes = (size_t)trials[j].height * trials[j].width * sizeof(double);
-    CU(cudaMemcpyAsync(d + off_grid[j], trials[j].lin, bytes, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(d + off_grid[j] + bytes, trials[j].ang, bytes, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d + L.grid[j], trials[j].lin, bytes, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d + L.grid[j] + bytes, trials[j].ang, bytes, cudaMemcpyHostToDevice, st));
   }
-  const SampleBoxDesc* db = reinterpret_cast<const SampleBoxDesc*>(d + off_box);
-  const UpdateBatchDesc* du = reinterpret_cast<const UpdateBatchDesc*>(d + b->off_upd);
-  const int* dact2 = dact + K1;                        // the stochastic launches' active flags
-  PlantArgs pa{reinterpret_cast<const TrialDev*>(d + off_tr), reinterpret_cast<TrialState*>(d + off_state), dact,
-               dact + K, reinterpret_cast<double*>(d + off_xh), reinterpret_cast<float*>(d + off_uh), K, T, S, 0,
-               barebone ? reinterpret_cast<int*>(d + off_con) : nullptr};
+  t.pa = PlantArgs{reinterpret_cast<const TrialDev*>(d + L.tr), reinterpret_cast<TrialState*>(d + L.state), dact,
+                   dact + K, reinterpret_cast<double*>(d + L.xh), reinterpret_cast<float*>(d + L.uh), K, b->T, t.S, 0,
+                   t.barebone ? reinterpret_cast<int*>(d + L.con) : nullptr};
   CU(cudaStreamSynchronize(st));                      // the staging is read by the upload above
-  int* hcount = reinterpret_cast<int*>(h);             // the polled counts, in the no longer needed head of the staging
-  for (cudaEvent_t& e : buf.ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  const int num_opt = b->pl[0]->prm.num_opt, npad = b->pl[0]->npad;
-  const int C1 = P[0].C, C2 = P[1].C;
-  const LaunchClasses& lc1 = P[0].lc;
-  const LaunchClasses& lc2 = P[1].lc;
-  int issued = 0;
-  const int last_step = S * max_episodes;
-  for (int s = 0; s < last_step; ++s) {
-    if (s >= TRIAL_POLL) {                            // the count after step s - POLL
-      CU(cudaEventSynchronize(buf.ev[s % TRIAL_POLL]));
-      if (hcount[s % TRIAL_POLL] == 0) break;
-    }
-    for (int k = 0; k < num_opt; ++k) {
-      if (K1 > 0) {
-        launch_sample_noise_batch(reinterpret_cast<const NoiseDesc*>(d), K1, N, T, dact, st);
-        CHECK_LAUNCH();
-        for (int c = 0; c < C1 && k == 0; ++c) {
-          launch_sample_grids_v2_batch(P[0].cls[c].L, ds[0][s & 1], lc1.count(c), dcls[0] + lc1.first[c], dact, st,
-                                       dgrp[0], dmem[0]);
-          CHECK_LAUNCH();
-        }
-        launch_rollout_batch(dr, K1, b->mode, N, T, dact, st);
-        CHECK_LAUNCH();
-      }
-      if (K2 > 0) {
-        const int iter = s * num_opt + k;             // every planner's reach slot toggles once per iteration
-        launch_noise_prepare_batch(reinterpret_cast<const NoisePrepDesc*>(d + b->off_nprep), K2, N, T, npad, iter,
-                                   dact2, st);
-        CHECK_LAUNCH();
-        for (int c = 0; c < C2 && k == 0; ++c) {
-          const TrialClass& tc = P[1].cls[c];
-          const SampleGridsV2Args& g0c = P[1].set0[lc2.groups[lc2.first[c]]];
-          launch_sample_grids_v2_box_batch(tc.L, ds[1][s & 1], db, lc2.count(c), dcls[1] + lc2.first[c], dact2, iter,
-                                           tc.mrows, tc.ncact, st, dgrp[1], dmem[1]);
-          CHECK_LAUNCH();
-          launch_advance_states_batch(ds[1][s & 1], db, lc2.count(c), dcls[1] + lc2.first[c], g0c.tx, g0c.ty,
-                                      g0c.num_maps, dact2, st, dgrp[1], dmem[1]);
-          CHECK_LAUNCH();
-        }
-        CU(launch_rollout_win_batch(g0, dw, d + b->off_tm, K2, masks01, dact2, st));
-        launch_cvar_batch(reinterpret_cast<const CvarDesc*>(d + b->off_cvar), K2, N, b->M, st);
+  return B200MPPI_OK;
+}
+
+// The launches of step s, each counted where it is issued
+static int trial_call_step(TrialCall& t, int s) {
+  b200mppi_batch* b = t.b;
+  const unsigned char* d = t.d;
+  cudaStream_t st = b->stream;
+  const int K = t.K, K1 = t.K1, K2 = t.K2, N = b->N, T = b->T, num_opt = b->pl[0]->prm.num_opt;
+  const TrialPart& om = t.P[0];
+  const TrialPart& sto = t.P[1];
+  const int* dact = t.pa.active;
+  const int* dact2 = dact + K1;                        // the stochastic launches' active flags
+  const RolloutWinArgs* dw = reinterpret_cast<const RolloutWinArgs*>(d + b->off_win);
+  const SampleBoxDesc* db = reinterpret_cast<const SampleBoxDesc*>(d + t.L.box);
+  for (int k = 0; k < num_opt; ++k) {
+    if (K1 > 0) {
+      launch_sample_noise_batch(reinterpret_cast<const NoiseDesc*>(d), K1, N, T, dact, st);
+      b->launches++;
+      CHECK_LAUNCH();
+      for (int c = 0; c < om.C && k == 0; ++c) {
+        launch_sample_grids_v2_batch(om.cls[c].L, om.set_d[s & 1], om.lc.count(c), om.cls_d + om.lc.first[c], dact, st,
+                                     om.grp_d, om.mem_d);
+        b->launches++;
         CHECK_LAUNCH();
       }
-      launch_update_partial_batch(du, K, b->pl[0]->num_ctas, dact, st);
+      launch_rollout_batch(reinterpret_cast<const RolloutArgs*>(d + b->off_roll), K1, b->mode, N, T, dact, st);
+      b->launches++;
       CHECK_LAUNCH();
     }
-    // a sequence's episodes start at steps only the device knows: a recording sequence issues the record launches at
-    // every step, gated per planner by the flags the previous plant step set, each writing where its descriptor points
-    const bool rec_step = record && (seq || s % record_every == 0);
-    if (rec_step) {
-      const int* rflag = seq ? sa.rec_flag : dact;
-      for (int c = 0; c < C2; ++c) {                  // from the pre-call states this step's sampling read
-        const TrialClass& tc = P[1].cls[c];
-        launch_sample_grids_v2_complete_batch(tc.L, ds[1][s & 1], db, lc2.count(c), dcls[1] + lc2.first[c], rflag + K1,
-                                              V, tc.mrows, tc.ncact, st, dgrp[1], dmem[1]);
+    if (K2 > 0) {
+      const int iter = s * num_opt + k;               // every planner's reach slot toggles once per iteration
+      launch_noise_prepare_batch(reinterpret_cast<const NoisePrepDesc*>(d + b->off_nprep), K2, N, T, b->pl[0]->npad,
+                                 iter, dact2, st);
+      b->launches++;
+      CHECK_LAUNCH();
+      for (int c = 0; c < sto.C && k == 0; ++c) {
+        const TrialClass& tc = sto.cls[c];
+        const SampleGridsV2Args& g0c = sto.set0[sto.lc.groups[sto.lc.first[c]]];
+        const int* cls = sto.cls_d + sto.lc.first[c];
+        launch_sample_grids_v2_box_batch(tc.L, sto.set_d[s & 1], db, sto.lc.count(c), cls, dact2, iter, tc.mrows,
+                                         tc.ncact, st, sto.grp_d, sto.mem_d);
+        b->launches++;
+        CHECK_LAUNCH();
+        launch_advance_states_batch(sto.set_d[s & 1], db, sto.lc.count(c), cls, g0c.tx, g0c.ty, g0c.num_maps, dact2, st,
+                                    sto.grp_d, sto.mem_d);
+        b->launches++;
         CHECK_LAUNCH();
       }
-      launch_state_rollout_batch(reinterpret_cast<const VisBatchDesc*>(d + off_vis), K, V, rflag,
-                                 seq ? 0 : (size_t)(s / record_every) * per, st);
+      CU(launch_rollout_win_batch(t.g0, dw, d + b->off_tm, K2, t.masks01, dact2, st));
+      b->launches++;
+      launch_cvar_batch(reinterpret_cast<const CvarDesc*>(d + b->off_cvar), K2, N, b->M, st);
+      b->launches++;
       CHECK_LAUNCH();
     }
-    pa.step = s;
-    if (seq) launch_plant_step_seq(pa, sa, st);
-    else launch_plant_step(pa, st);
+    launch_update_partial_batch(reinterpret_cast<const UpdateBatchDesc*>(d + b->off_upd), K, b->pl[0]->num_ctas, dact,
+                                st);
+    b->launches++;
     CHECK_LAUNCH();
-    b->launches += num_opt + 1 + (K1 > 0 ? 2 * num_opt + C1 : 0) + (K2 > 0 ? 3 * num_opt + 2 * C2 : 0);
-    if (rec_step) b->launches += 1 + C2;          // every step of a recording sequence
-    ++issued;
-    CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, dact + K, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(buf.ev[s % TRIAL_POLL], st));
   }
-  // the box records (stochastic), the states and the contacts (barebone), then the histories
-  CU(cudaMemcpyAsync(h + off_rec, d + off_rec, off_tr - off_rec, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(h + head, d + off_xh, total - off_xh, cudaMemcpyDeviceToHost, st));
+  // a sequence's episodes start at steps only the device knows: a recording sequence issues the record launches at
+  // every step, gated per planner by the flags the previous plant step set, each writing where its descriptor points
+  if (t.record && (t.seq || s % t.record_every == 0)) {
+    const int* rflag = t.seq ? t.sa.rec_flag : dact;
+    for (int c = 0; c < sto.C; ++c) {                 // from the pre-call states this step's sampling read
+      const TrialClass& tc = sto.cls[c];
+      launch_sample_grids_v2_complete_batch(tc.L, sto.set_d[s & 1], db, sto.lc.count(c), sto.cls_d + sto.lc.first[c],
+                                            rflag + K1, t.V, tc.mrows, tc.ncact, st, sto.grp_d, sto.mem_d);
+      b->launches++;
+      CHECK_LAUNCH();
+    }
+    launch_state_rollout_batch(reinterpret_cast<const VisBatchDesc*>(d + t.L.vis), K, t.V, rflag,
+                               t.seq ? 0 : (size_t)(s / t.record_every) * t.per, st);
+    b->launches++;
+    CHECK_LAUNCH();
+  }
+  t.pa.step = s;
+  if (t.seq) launch_plant_step_seq(t.pa, t.sa, st);
+  else launch_plant_step(t.pa, st);
+  b->launches++;
+  CHECK_LAUNCH();
+  return B200MPPI_OK;
+}
+
+// Reads back the states and histories, and leaves the caller's outputs, every planner and every TDM group's pair as
+// after the host loop
+static int trial_call_commit(TrialCall& t) {
+  b200mppi_batch* b = t.b;
+  const TrialLayout& L = t.L;
+  const unsigned char* d = t.d;
+  unsigned char* h = t.h;
+  cudaStream_t st = b->stream;
+  const int K = t.K, K1 = t.K1, S = t.S, R = t.R, num_opt = b->pl[0]->prm.num_opt;
+  const size_t per = t.per;
+  const std::vector<int>& first = t.first;
+  b200mppi_trial_result* results = t.results;
+  // the box records (stochastic) through the results (sequences), then the histories
+  CU(cudaMemcpyAsync(h + L.rec, d + L.rec, L.res_end - L.rec, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(h + L.head, d + L.xh, L.total - L.xh, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  const int* hrec = reinterpret_cast<const int*>(h + off_rec);
-  const double* hx = reinterpret_cast<const double*>(h + head);
-  const float* hu = reinterpret_cast<const float*>(h + head + (off_uh - off_xh));
+  const int* hrec = reinterpret_cast<const int*>(h + L.rec);
+  const TrialState* hst = reinterpret_cast<const TrialState*>(h + L.state);
+  const TrialState* hres = reinterpret_cast<const TrialState*>(h + L.res);
+  const int* hcon = reinterpret_cast<const int*>(h + L.con);
+  const double* hx = reinterpret_cast<const double*>(h + L.head);
+  const float* hu = reinterpret_cast<const float*>(h + L.head + (L.uh - L.xh));
   const double dnan = std::nan("");
   const float fnan = std::nanf("");
   std::vector<int> ran(K, 0);                          // steps each planner ran, over all its episodes
   for (int i = 0; i < K; ++i) {
     int last = first[i];                               // the planner's last slot that ran
     for (int j = first[i]; j < first[i + 1]; ++j) {
-      const TrialState& r = seq ? hres[j] : hst[i];
+      const TrialState& r = t.seq ? hres[j] : hst[i];
       const int n = r.steps;                           // 0: an episode of a sequence that never ran
-      double* xo = xhist + (size_t)j * (S + 1) * 3;
-      float* uo = uhist + (size_t)j * S * 2;
+      double* xo = t.xhist + (size_t)j * (S + 1) * 3;
+      float* uo = t.uhist + (size_t)j * S * 2;
       if (n > 0) {
-        for (int c = 0; c < 3; ++c) xo[c] = trials[j].x0[c];
+        for (int c = 0; c < 3; ++c) xo[c] = t.trials[j].x0[c];
         last = j;
       }
       std::memcpy(xo + 3, hx + ((size_t)j * (S + 1) + 1) * 3, (size_t)n * 3 * sizeof(double));
@@ -3367,7 +3389,7 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       for (size_t q = (size_t)n * 2; q < (size_t)S * 2; ++q) uo[q] = fnan;
       results[j] = b200mppi_trial_result{r.cum_obj, r.cum_dist, r.dist, n, r.status};
       ran[i] += n;
-      if (barebone) contact_steps[j] = hcon[j];
+      if (t.barebone) t.contact_steps[j] = hcon[j];
     }
     // host state as after ran[i] rounds of the host loop: the reach slot toggled once per iteration, the last solve's
     // box and x0 (the samplings of the pair below).  The last solve planned from the pose before the last step -- or,
@@ -3379,54 +3401,116 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       p->reach_slot ^= (n * num_opt) & 1;
       p->reach_valid = true;
       for (int c = 0; c < 5; ++c) p->last_box[c] = rec[c];
-    } else if (!barebone) {
+    } else if (!t.barebone) {
       last_box_whole_map(p);
     }
     p->prepared = false;
     p->pushed_direct = false;
-    const double* x0 = xhist + ((size_t)last * (S + 1) + results[last].steps - 1) * 3;
-    if (results[last].steps == 1 && last > first[i] && !reset_x0)
-      x0 = xhist + ((size_t)(last - 1) * (S + 1) + results[last - 1].steps) * 3;
+    const double* x0 = t.xhist + ((size_t)last * (S + 1) + results[last].steps - 1) * 3;
+    if (results[last].steps == 1 && last > first[i] && !t.reset_x0)
+      x0 = t.xhist + ((size_t)(last - 1) * (S + 1) + results[last - 1].steps) * 3;
     for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)x0[c];
   }
   // each TDM group's pair as after the samplings of its longest-running member (a group samples at every step while any
   // member runs), a stochastic pair's last kind from the group's record (a group of one: its planner's)
-  for (TrialPart& q : P) {
-    const bool sto = &q == &P[1];
+  for (int k = 0; k < 2; ++k) {
+    TrialPart& q = t.P[k];
     for (int g = 0; g < q.G; ++g) {
       int n = 0;
       for (int j = q.gr.first[g]; j < q.gr.first[g + 1]; ++j) n = std::max(n, ran[q.lo + q.gr.members[j]]);
-      if (sto) {
-        const int* rec = q.grouped ? reinterpret_cast<const int*>(h + off_grec) + 5 * g : hrec + 5 * q.gr.lead(g);
+      if (k == 1) {
+        const int* rec = q.grouped ? reinterpret_cast<const int*>(h + L.grec) + 5 * g : hrec + 5 * q.gr.lead(g);
         q.plans[g].boxed[0] = q.plans[g].boxed[1] = rec[0] != 0;
       }
       for (int s = 0; s < n; ++s) { plan_commit(q.plans[g], 0); plan_commit(q.plans[g], 1); }
     }
   }
-  if (record) {
-    // record r of a slot belongs to step r * record_every of its episode; slot first[i] + e goes to the caller's slab
-    // (i, e).  Only the written ones are copied (records past an episode's last step are never written, and an early
-    // stop leaves most of them so): the rest is NaN, as are the slabs of episodes a planner does not have.  The last one
-    // of a planner's last run episode is what its state_rollout buffer holds after the host loop's last
-    // get_state_rollout.
-    for (int i = 0; i < K; ++i) {
-      int last = first[i], last_done = 0;
-      float* planner_out = rollouts + (size_t)i * max_episodes * R * per;
-      std::fill(planner_out + (size_t)(first[i + 1] - first[i]) * R * per,
-                planner_out + (size_t)max_episodes * R * per, fnan);
-      for (int j = first[i]; j < first[i + 1]; ++j) {
-        const int done = (results[j].steps + record_every - 1) / record_every;
-        float* slab = planner_out + (size_t)(j - first[i]) * R * per;
-        CU(cudaMemcpyAsync(slab, drec + (size_t)j * R * per, (size_t)done * per * sizeof(float), cudaMemcpyDeviceToHost,
-                           st));
-        std::fill(slab + (size_t)done * per, slab + (size_t)R * per, fnan);
-        if (done > 0) { last = j; last_done = done; }
-      }
-      CU(cudaMemcpyAsync(b->pl[i]->state_rollout, drec + ((size_t)last * R + last_done - 1) * per, per * sizeof(float),
-                         cudaMemcpyDeviceToDevice, st));
+  if (!t.record) return B200MPPI_OK;
+  // record r of a slot belongs to step r * record_every of its episode; slot first[i] + e goes to the caller's slab
+  // (i, e).  Only the written ones are copied (records past an episode's last step are never written, and an early
+  // stop leaves most of them so): the rest is NaN, as are the slabs of episodes a planner does not have.  The last one
+  // of a planner's last run episode is what its state_rollout buffer holds after the host loop's last
+  // get_state_rollout.
+  const float* drec = reinterpret_cast<const float*>(d + L.vrec);
+  for (int i = 0; i < K; ++i) {
+    int last = first[i], last_done = 0;
+    float* planner_out = t.rollouts + (size_t)i * t.max_episodes * R * per;
+    std::fill(planner_out + (size_t)(first[i + 1] - first[i]) * R * per,
+              planner_out + (size_t)t.max_episodes * R * per, fnan);
+    for (int j = first[i]; j < first[i + 1]; ++j) {
+      const int done = (results[j].steps + t.record_every - 1) / t.record_every;
+      float* slab = planner_out + (size_t)(j - first[i]) * R * per;
+      CU(cudaMemcpyAsync(slab, drec + (size_t)j * R * per, (size_t)done * per * sizeof(float), cudaMemcpyDeviceToHost,
+                         st));
+      std::fill(slab + (size_t)done * per, slab + (size_t)R * per, fnan);
+      if (done > 0) { last = j; last_done = done; }
     }
-    CU(cudaStreamSynchronize(st));
+    CU(cudaMemcpyAsync(b->pl[i]->state_rollout, drec + ((size_t)last * R + last_done - 1) * per, per * sizeof(float),
+                       cudaMemcpyDeviceToDevice, st));
   }
+  CU(cudaStreamSynchronize(st));
+  return B200MPPI_OK;
+}
+
+// The closed-loop trials of every kind of batch.  Stochastic trials also move each planner's reach box with the robot;
+// with box_mode 2 and num_opt 1 it depends on the controls drawn, so the batched boxed sampler decides it on the device
+// (reach_box_decide, the function sample_finish calls) and a step needs no host round trip (trial_call_step lists a
+// step's launches).  The plant step also moves stochastic planners' rollout windows and counts barebone contacts.
+// record_every = n > 0 records the visualisation rollouts of every step s with s % n == 0, after the step's last update
+// and before the plant step (which shifts u_cur and overwrites x0); stochastic planners first complete maps [0, V) of
+// every pair whose step sampled a box (the maps the rollouts read).
+// Trial sequences (episodes non-null, b200mppi_batch_run_trial_sequences): planner i runs episodes[i] episodes back to
+// back, descriptors, histories and results per slot (planner-major: planner i's are slots first[i] .. first[i + 1]),
+// through the same step loop for up to max_i episodes[i] * max_steps steps; the plant step (plant_step_seq_kernel)
+// moves a planner to its next episode without a launch, and the commit follows each planner's total steps.
+// A recording sequence records at each episode's own steps t with t % record_every == 0: the plant step sets each
+// planner's record flag and record pointer for the next step (SeqArgs).
+static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_trial_desc* trials, int32_t max_steps,
+                            double* xhist, float* uhist, b200mppi_trial_result* results, int32_t* contact_steps,
+                            int32_t record_every, float* rollouts, size_t rollout_bytes, int32_t* steps_issued,
+                            const int32_t* episodes, int32_t reset_x0) {
+  if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  TrialCall t{b, kind, trials, max_steps, xhist, uhist, results, contact_steps, record_every, rollouts, rollout_bytes,
+              episodes, reset_x0 != 0};
+  int rc;
+  if ((rc = trial_call_validate(t)) || (rc = trial_call_plan(t))) return rc;
+  t.L = trial_layout(t);
+  struct Buffers {                                     // freed on every return
+    unsigned char* d = nullptr;
+    unsigned char* h = nullptr;
+    cudaEvent_t ev[TRIAL_POLL] = {};
+    ~Buffers() {
+      cudaFree(d);
+      if (h) cudaFreeHost(h);
+      for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    }
+  } buf;
+  if (cudaMalloc(&buf.d, t.L.total) != cudaSuccess) {
+    buf.d = nullptr;
+    cudaGetLastError();                                // not sticky: later calls start clean
+    return fail(B200MPPI_ECUDA, t.fn + ": cudaMalloc of " + std::to_string(t.L.total) + " bytes");
+  }
+  if (cudaMallocHost(&buf.h, t.L.head + (t.L.total - t.L.xh)) != cudaSuccess) {
+    buf.h = nullptr;
+    return fail(B200MPPI_ECUDA, t.fn + ": cudaMallocHost");
+  }
+  t.d = buf.d;
+  t.h = buf.h;
+  if ((rc = trial_call_stage(t))) return rc;
+  int* hcount = reinterpret_cast<int*>(t.h);           // the polled counts, in the no longer needed head of the staging
+  for (cudaEvent_t& e : buf.ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  int issued = 0;
+  for (int s = 0; s < t.S * t.max_episodes; ++s) {
+    if (s >= TRIAL_POLL) {                            // the count after step s - POLL
+      CU(cudaEventSynchronize(buf.ev[s % TRIAL_POLL]));
+      if (hcount[s % TRIAL_POLL] == 0) break;
+    }
+    if ((rc = trial_call_step(t, s))) return rc;
+    ++issued;
+    CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, t.pa.active_count, sizeof(int), cudaMemcpyDeviceToHost, b->stream));
+    CU(cudaEventRecord(buf.ev[s % TRIAL_POLL], b->stream));
+  }
+  if ((rc = trial_call_commit(t))) return rc;
   if (steps_issued) *steps_issued = issued;
   return B200MPPI_OK;
 }
