@@ -636,6 +636,63 @@ int b200mppi_batch_run_mixed_trials(b200mppi_batch* b, const b200mppi_trial_desc
                                     double* xhist, float* uhist, b200mppi_trial_result* results,
                                     int32_t* steps_issued);
 
+/* ------------------------------------------------------------------ device loops
+ * A receding-horizon loop whose plant is the caller's: a simulator, a learned model or the robot's own state estimate in
+ * GPU memory.  A loop opened on a batch enqueues each solve and each shift_and_update on the batch's stream
+ * (b200mppi_batch_set_stream); they read poses from and write controls to device memory, and no call waits on the host.
+ * Per planner the loop is the host loop of the same calls, bit for bit:
+ *   b200mppi_loop_solve              == batch_solve of that planner (its trial kind's batch solve);
+ *   b200mppi_loop_shift_and_update   == set_u(u_cur shifted by one row, the last row kept) and set_params with x0 =
+ *                                      float32 of the pose, as shift_and_update(pose, u, 1) after that solve.
+ * The calls may come in any order (two solves, two shifts, a close right after a solve).  One planner: a batch of one.
+ * A loop issues what the trial of its kind issues, without the plant step: a solve issues one trial step's launches
+ * (num_opt x the solve stages, the sampler classes) and one export; a shift and a stop one launch each.
+ *
+ * b200mppi_batch_loop_open: kind as in b200mppi_batch_run_trials_recorded (the batch's own kind).  padded_limits: float64
+ * (count, 4) = padded x lo, x hi, y lo, y hi of each planner's map (the limits of the host's solve check; NULL for
+ * barebone).  rows: int32 (count), planner i's row in the caller's controls, poses and stop mask (a permutation of
+ * 0 .. count-1; NULL: row i).  The batch's descriptors are built from each planner's params as set now.  Refused
+ * (B200MPPI_EINVAL naming the planner) before any work: what batch_solve refuses, num_opt < 1, another kind, a NaN limit,
+ * bad rows, a loop already open; and what the trial of that kind refuses of the TDM pairs.
+ * While a loop is open, every planner and batch call that touches the state of the batch or its planners (solve, set_*,
+ * get_u, shift_u, copy_in / copy_out, the stage calls, get_state_rollout, the trial calls, share_tdms, set_stream and
+ * destroy) returns B200MPPI_EINVAL.
+ * b200mppi_loop_controls: the loop's own (count, T, 2) float32 device buffer, and the batch's stream.
+ * b200mppi_loop_solve: one solve of every running planner; row rows[i] of u_dev ((count, T, 2) float32 in device memory
+ *   of the batch's device) gets planner i's new u_cur, NaN for a planner that no longer runs.
+ * b200mppi_loop_shift_and_update: pose of planner i = row rows[i] of x_dev: 3 contiguous elements of dtype
+ *   B200MPPI_POSE_F64 or _F32 (widened exactly), rows row_stride_bytes apart.  Every running planner shifts u_cur by one
+ *   row and plans its next solve from float32 of the pose (a stochastic planner's rollout window moves with it).  A pose
+ *   outside its padded limits (float64 lo <= v <= hi for x and y; NaN fails), where the host's next solve would be
+ *   refused, stops that planner for good with status B200MPPI_TRIAL_LEFT_MAP (not for barebone planners: no map).
+ * b200mppi_loop_stop: mask_dev (count) of elem_bytes 4 (int32) or 1 (bool / uint8), indexed by row: a running planner
+ *   whose entry is nonzero stops for good (B200MPPI_LOOP_STOPPED).  A stopped planner never runs again, so every running
+ *   planner has solved equally often and one sampler parity serves them all.
+ * b200mppi_loop_wait_stream: the batch's stream waits (an event, not the host) for the work issued so far on stream.
+ * b200mppi_loop_active: the device's int32 (count) running flags, in the batch's order.
+ * b200mppi_loop_close: waits for the stream, commits and frees the loop (also on an error).  Every planner and TDM pair is
+ *   left as after the host loop: the reach slots, sample boxes and the samplings of shared pairs follow each planner's
+ *   solves (a pair's group: its longest-running member), and the C-side params keep the x0 of the last solve.
+ *   per_planner (may be NULL): count summaries in the batch's order. */
+typedef struct b200mppi_loop b200mppi_loop;
+enum { B200MPPI_POSE_F64 = 0, B200MPPI_POSE_F32 = 1 };
+enum { B200MPPI_LOOP_RUNNING = 0, B200MPPI_LOOP_STOPPED = 5 };   /* and B200MPPI_TRIAL_LEFT_MAP */
+typedef struct {
+  int32_t solves, shifts;       /* solves and shifts the planner took */
+  int32_t status;               /* B200MPPI_LOOP_RUNNING, B200MPPI_TRIAL_LEFT_MAP or B200MPPI_LOOP_STOPPED */
+  int32_t pad_;
+  double x[3];                  /* the last pose shift_and_update took (the params' x0 before the loop: shifts 0) */
+} b200mppi_loop_summary;
+int b200mppi_batch_loop_open(b200mppi_batch* b, int32_t kind, const double* padded_limits, const int32_t* rows,
+                             b200mppi_loop** out);
+int b200mppi_loop_controls(b200mppi_loop* loop, float** u_dev, void** stream);
+int b200mppi_loop_solve(b200mppi_loop* loop, float* u_dev);
+int b200mppi_loop_shift_and_update(b200mppi_loop* loop, const void* x_dev, int32_t dtype, int64_t row_stride_bytes);
+int b200mppi_loop_stop(b200mppi_loop* loop, const void* mask_dev, int32_t elem_bytes);
+int b200mppi_loop_wait_stream(b200mppi_loop* loop, void* stream);
+int b200mppi_loop_active(b200mppi_loop* loop, const int32_t** dev);
+int b200mppi_loop_close(b200mppi_loop* loop, b200mppi_loop_summary* per_planner);
+
 #ifdef __cplusplus
 }
 #endif

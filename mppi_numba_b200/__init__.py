@@ -9,7 +9,7 @@ planner or TDM needs a CUDA device.  There is no CPU fallback.
 from .config import Config
 from .terrain import DeviceTractionGrid, DeviceTractionGrids, TDM_Numba, TractionGrid, Terrain, draw_traction_grids
 from .mppi import MPPI_Numba
-from .batch import MPPI_Batch, MPPI_MixedBatch, MPPI_StochasticBatch
+from .batch import DeviceLoop, MPPI_Batch, MPPI_MixedBatch, MPPI_StochasticBatch
 from ._lib import B200MPPIError, device_count
 
-__all__ = ["Config", "TDM_Numba", "TractionGrid", "DeviceTractionGrid", "DeviceTractionGrids", "draw_traction_grids", "Terrain", "MPPI_Numba", "MPPI_Batch", "MPPI_StochasticBatch", "MPPI_MixedBatch", "B200MPPIError", "device_count"]
+__all__ = ["Config", "TDM_Numba", "TractionGrid", "DeviceTractionGrid", "DeviceTractionGrids", "draw_traction_grids", "Terrain", "MPPI_Numba", "MPPI_Batch", "MPPI_StochasticBatch", "MPPI_MixedBatch", "DeviceLoop", "B200MPPIError", "device_count"]

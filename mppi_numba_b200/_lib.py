@@ -59,6 +59,24 @@ TRIAL_GOAL, TRIAL_MAX_STEPS, TRIAL_LEFT_MAP, TRIAL_NOT_RUN = 1, 2, 3, 4
 TRIALS_MAP, TRIALS_STOCHASTIC, TRIALS_BAREBONE, TRIALS_MIXED = 0, 1, 2, 3
 
 
+class LoopSummary(C.Structure):
+    """b200mppi_loop_summary"""
+    _fields_ = [("solves", C.c_int32), ("shifts", C.c_int32), ("status", C.c_int32), ("pad_", C.c_int32),
+                ("x", C.c_double * 3)]
+
+
+POSE_F64, POSE_F32 = 0, 1
+LOOP_RUNNING, LOOP_STOPPED = 0, 5
+
+
+def refuse_in_loop(obj, name):
+    """ValueError when ``obj`` (a planner or TDM) belongs to the batch of an open device loop, naming the planner."""
+    held = getattr(obj, "_device_loop", None)
+    if held is not None:
+        raise ValueError("%s: planner %d is in an open device loop (its batch's DeviceLoop owns its state until it "
+                         "closes)" % (name, held))
+
+
 def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
@@ -153,6 +171,14 @@ def _load():
                                                          C.POINTER(TrialResult), C.POINTER(I32)]),
         "b200mppi_batch_run_trial_sequences_ex": (C.c_int, [P, I32, C.POINTER(TrialDesc), P, I32, I32, P, P,
                                                             C.POINTER(TrialResult), P, I32, P, SZ, C.POINTER(I32)]),
+        "b200mppi_batch_loop_open": (C.c_int, [P, I32, P, P, C.POINTER(P)]),
+        "b200mppi_loop_controls": (C.c_int, [P, C.POINTER(P), C.POINTER(P)]),
+        "b200mppi_loop_solve": (C.c_int, [P, P]),
+        "b200mppi_loop_shift_and_update": (C.c_int, [P, P, I32, I64]),
+        "b200mppi_loop_stop": (C.c_int, [P, P, I32]),
+        "b200mppi_loop_wait_stream": (C.c_int, [P, P]),
+        "b200mppi_loop_active": (C.c_int, [P, C.POINTER(P)]),
+        "b200mppi_loop_close": (C.c_int, [P, C.POINTER(LoopSummary)]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)          # AttributeError here == ABI drift, fail loudly
@@ -188,14 +214,16 @@ def c_floats(values, n):
 class DeviceArray(object):
     """Stand-in for numba's DeviceNDArray: ``.shape``, ``.dtype``, ``.copy_to_host()``,
     ``.copy_to_device(host_array)`` and ``__cuda_array_interface__`` (zero-copy views for torch /
-    numba / cupy).  The memory belongs to the planner / TDM handle that created it."""
+    numba / cupy).  The memory belongs to the planner / TDM handle that created it.  ``stream`` (a cudaStream_t as
+    int): the interface names it, so a consumer orders its work after the stream's (a device loop's controls)."""
 
-    def __init__(self, owner, shape, dtype, reader, writer=None, dev_ptr=None, strides=None):
+    def __init__(self, owner, shape, dtype, reader, writer=None, dev_ptr=None, strides=None, stream=None):
         self._owner = owner           # keeps the handle alive
         self.shape = tuple(int(s) for s in shape)
         self.dtype = np.dtype(dtype)
         self._reader, self._writer = reader, writer
         self._dev_ptr, self._strides = dev_ptr, strides
+        self._stream = stream
 
     @property
     def size(self):
@@ -225,5 +253,8 @@ class DeviceArray(object):
     def __cuda_array_interface__(self):
         if self._dev_ptr is None:
             raise AttributeError("no raw device view for this array")
-        return {"shape": self.shape, "typestr": self.dtype.str, "data": (int(self._dev_ptr()), False),
-                "version": 3, "strides": self._strides}
+        cai = {"shape": self.shape, "typestr": self.dtype.str, "data": (int(self._dev_ptr()), False),
+               "version": 3, "strides": self._strides}
+        if self._stream is not None:
+            cai["stream"] = int(self._stream) or 1      # the legacy default stream is 1 in the interface (0 is barred)
+        return cai

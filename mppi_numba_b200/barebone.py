@@ -101,9 +101,11 @@ class MPPI_Numba(object):
         print("MPPI planner has initialized GPU memory after {} s".format(time.time() - t0))
 
     def setup(self, params):
+        _lib.refuse_in_loop(self, "MPPI_Numba.setup")
         self.set_params(params)
 
     def set_params(self, params):
+        _lib.refuse_in_loop(self, "MPPI_Numba.set_params")
         self.params = copy.deepcopy(params)
         self.params_set = True
 
@@ -145,6 +147,7 @@ class MPPI_Numba(object):
         return pod
 
     def solve(self):
+        _lib.refuse_in_loop(self, "MPPI_Numba.solve")
         if not self.check_solve_conditions():
             print("MPPI solve condition not met. Cannot solve. Return")
             return None
@@ -158,6 +161,7 @@ class MPPI_Numba(object):
         return u
 
     def shift_and_update(self, new_x0, u_cur, num_shifts=1):
+        _lib.refuse_in_loop(self, "MPPI_Numba.shift_and_update")
         self.params["x0"] = new_x0.copy()
         self.shift_optimal_control_sequence(u_cur, num_shifts)
 
@@ -168,6 +172,7 @@ class MPPI_Numba(object):
         check(lib.b200mppi_planner_set_u(self._handle, ptr(shifted)))
 
     def get_state_rollout(self):
+        _lib.refuse_in_loop(self, "MPPI_Numba.get_state_rollout")
         assert self.params_set, "MPPI parameters are not set"
         if not self.device_var_initialized:
             print("Device variables not initialized. Cannot run mppi.")

@@ -38,13 +38,17 @@ pair would leave it (include/b200mppi.h, planners sharing TDM pairs).
 ``MPPI_MixedBatch(planners)`` holds det-dynamics, speed-map and use_tdm planners together -- the methods the reference
 benchmark compares -- and runs their solves, trials and trial sequences in one call each, every planner ending as the
 batch of its own kind would leave it (include/b200mppi.h, mixed batches).
+
+``device_loop()`` opens a ``DeviceLoop`` on any of these batches: the receding-horizon loop with the caller's own plant
+(a simulator, a learned model, a state estimate in GPU memory), whose ``solve()`` and ``shift_and_update(x)`` run on the
+batch's stream with no host wait (include/b200mppi.h, device loops).
 """
 import ctypes as C
 
 import numpy as np
 
 from . import _lib
-from ._lib import check, lib, ptr
+from ._lib import DeviceArray, check, lib, ptr
 from .terrain import DeviceTractionGrid
 
 TRIAL_STATUS = {_lib.TRIAL_GOAL: "goal", _lib.TRIAL_MAX_STEPS: "max_steps", _lib.TRIAL_LEFT_MAP: "left_map",
@@ -96,6 +100,7 @@ class MPPI_Batch(object):
         self.num_steps = planners[0].num_steps
         self.share_tdms = bool(share_tdms)
         self._handle = None
+        self._loop = None                              # the open DeviceLoop
         handles = (C.c_void_p * len(planners))(*[p._handle.value for p in planners])
         h = C.c_void_p()
         check(create(handles, len(planners), C.byref(h)))
@@ -133,6 +138,16 @@ class MPPI_Batch(object):
             except Exception:
                 pass
 
+    def _refuse_in_loop(self, name):
+        """ValueError while a device loop is open on the batch."""
+        if self._loop is not None:
+            raise ValueError("%s: a device loop is open on this batch (close it first)" % name)
+
+    def device_loop(self):
+        """Open a ``DeviceLoop`` on the batch: ``solve()`` and ``shift_and_update(x)`` enqueued on the batch's stream,
+        poses and controls in GPU memory, for a plant of the caller's own (see DeviceLoop)."""
+        return DeviceLoop(self)
+
     def __len__(self):
         return len(self.planners)
 
@@ -150,6 +165,7 @@ class MPPI_Batch(object):
         return u
 
     def _solve(self, name):
+        self._refuse_in_loop(name)
         for i, p in enumerate(self.planners):
             if not p.check_solve_conditions():
                 print("{}: planner {}: MPPI solve condition not met. Cannot solve. Return".format(name, self.order[i]))
@@ -163,6 +179,7 @@ class MPPI_Batch(object):
 
     def set_stream(self, cuda_stream):
         """Issue the batch's work on ``cuda_stream`` (a raw cudaStream_t as int, e.g. torch's ``stream.cuda_stream``)."""
+        self._refuse_in_loop("%s.set_stream" % type(self).__name__)
         check(lib.b200mppi_batch_set_stream(self._handle, C.c_void_p(int(cuda_stream))))
 
     def launch_count(self):
@@ -178,6 +195,7 @@ class MPPI_Batch(object):
         after planners[0].get_state_rollout(), planners[1].get_state_rollout(), ...  Raises ValueError (naming the
         planner) when a planner's params are not set or the planners' num_vis_state_rollouts differ; nothing is issued
         then."""
+        self._refuse_in_loop("%s.get_state_rollout" % type(self).__name__)
         V = self._vis_count("MPPI_Batch.get_state_rollout")
         for i, p in enumerate(self.planners):
             if not p.params_set:
@@ -268,6 +286,7 @@ class MPPI_Batch(object):
         per episode; None for barebone) planner-major, the refusals naming the episode when ``episodes``.  Returns
         (max_steps, record_every, V, descs, first, keep): planner i's descriptors are descs[first[i]:first[i + 1]], and
         ``keep`` holds what they point to."""
+        self._refuse_in_loop(name)
         max_steps = int(max_steps)
         if max_steps < 1:
             raise ValueError("%s: max_steps %d < 1" % (name, max_steps))
@@ -720,3 +739,190 @@ class MPPI_MixedBatch(MPPI_Batch):
     def run_barebone_trials(self, max_steps, dt=None, record_every=None):
         raise ValueError("MPPI_MixedBatch.run_barebone_trials: a mixed batch holds no barebone planners (MPPI_Batch "
                          "runs barebone trials)")
+
+
+LOOP_STATUS = {_lib.LOOP_RUNNING: "running", _lib.TRIAL_LEFT_MAP: "left_map", _lib.LOOP_STOPPED: "stopped"}
+
+
+class DeviceLoop(object):
+    """A receding-horizon loop on a batch whose plant is the caller's, on the GPU with no host wait between calls:
+
+        batch.set_stream(torch.cuda.current_stream().cuda_stream)    # optional; the loop runs on the batch's stream
+        with batch.device_loop() as loop:
+            for t in range(steps):
+                u = torch.as_tensor(loop.solve(), device="cuda")       # (K, T, 2) float32, NaN rows: not solved
+                x = my_plant(x, u[:, 0])                               # any GPU work on the same stream
+                loop.shift_and_update(x)                               # (K, 3) float64 or float32 on the device
+                loop.stop(done)                                        # optional: (K,) int32 / bool, nonzero stops k
+        loop.solves, loop.shifts, loop.status                         # per planner, read at close
+
+    Opened by ``device_loop()`` of an ``MPPI_Batch`` (det-dynamics, speed-map or barebone planners),
+    ``MPPI_StochasticBatch`` or ``MPPI_MixedBatch``, with or without share_tdms.  A single planner runs in a batch of
+    one.  Rows are in the caller's planner order.  Per planner the loop is the host loop of the same calls, bit for bit:
+    ``loop.solve()`` is ``u = p.solve()`` (a use_tdm planner: ``MPPI_StochasticBatch([p]).solve()``) and
+    ``loop.shift_and_update(x)`` is ``p.shift_and_update(x[k], u, 1)`` with ``u`` the planner's current controls (after
+    a solve: that solve's).  The calls may come in any order.  Each new pose goes into the next rollout as float32(x).
+
+    A pose outside the planner's padded map limits (float64 lo <= v <= hi; NaN fails), where its next host solve would be
+    refused, stops that planner for good with status "left_map"; barebone planners have no map, so never.  ``stop(done)``
+    stops planner k for good when done[k] is nonzero.  A stopped planner's rows of later ``solve()`` outputs are NaN and
+    it is left untouched by every later call.
+
+    While the loop is open, the batch's calls and every call that reads or writes a member's state on the host
+    (``solve``, ``setup`` / ``set_params``, ``shift_and_update``, ``get_state`` / ``set_state``,
+    ``get_state_rollout``, the TDM setters and ``sample_grids`` of its TDMs) raise ValueError naming the planner.
+    Closing (``close()``, or leaving the ``with`` block, also on an exception) waits for the stream and commits every
+    planner: afterwards each is exactly as after that host loop, ``params['x0']`` the float64 value of the last pose it
+    took (a float32 pose widened exactly), and ``solves``, ``shifts`` (K,) int and ``status`` (K,) of "running" |
+    "left_map" | "stopped" are set.  Launches: a solve issues what a trial step of the batch issues without its plant
+    step, plus one export; ``shift_and_update`` and ``stop`` one each."""
+
+    def __init__(self, batch):
+        name = "%s.device_loop" % type(batch).__name__
+        batch._refuse_in_loop(name)
+        batch._check_groups(name)
+        for i, p in enumerate(batch.planners):
+            who = "%s: planner %d" % (name, batch.order[i])
+            if not p.check_solve_conditions():
+                raise ValueError("%s cannot solve (reason printed above)" % who)
+            if int(p.params["num_opt"]) < 1:
+                raise ValueError("%s has num_opt %d < 1" % (who, int(p.params["num_opt"])))
+        for p in batch.planners:
+            p.move_mppi_task_vars_to_device()
+        self.batch = batch
+        self.K, self.T = len(batch.planners), batch.num_steps
+        self.device = int(getattr(batch.planners[0], "device", 0))
+        kind = {"barebone": _lib.TRIALS_BAREBONE, "tdm": _lib.TRIALS_STOCHASTIC,
+                "mixed": _lib.TRIALS_MIXED}.get(batch.kind, _lib.TRIALS_MAP)
+        limits = None
+        if batch.kind != "barebone":
+            limits = np.array([list(p.lin_tdm.padded_xlimits) + list(p.lin_tdm.padded_ylimits) for p in batch.planners],
+                              dtype=np.float64)
+        rows = np.array(batch.order, dtype=np.int32)
+        h = C.c_void_p()
+        check(lib.b200mppi_batch_loop_open(batch._handle, kind, ptr(limits) if limits is not None else None, ptr(rows),
+                                           C.byref(h)))
+        self._handle = h
+        u, st, act = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        check(lib.b200mppi_loop_controls(h, C.byref(u), C.byref(st)))
+        check(lib.b200mppi_loop_active(h, C.byref(act)))
+        self.stream = int(st.value or 0)
+
+        def unreadable(out):
+            raise _lib.B200MPPIError("a device loop's arrays are read through __cuda_array_interface__ (e.g. "
+                                     "torch.as_tensor(a, device='cuda'))")
+        self._u = DeviceArray(self, (self.K, self.T, 2), np.float32, unreadable, dev_ptr=lambda: u.value,
+                              stream=self.stream)
+        self.active = DeviceArray(self, (self.K,), np.int32, unreadable, dev_ptr=lambda: act.value, stream=self.stream)
+        """(K,) int32 running flags on the device, in ``batch.planners`` order"""
+        self.solves = self.shifts = self.status = None
+        batch._loop = self
+        for i, p in enumerate(batch.planners):
+            for obj in (p, getattr(p, "lin_tdm", None), getattr(p, "ang_tdm", None)):
+                if obj is not None:
+                    obj._device_loop = batch.order[i]
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+        return False
+
+    def __del__(self):
+        if getattr(self, "_handle", None) is not None:
+            try:
+                self.close()
+            except Exception:
+                pass
+
+    def _live(self, fn):
+        if self._handle is None:
+            raise ValueError("DeviceLoop.%s: the loop is closed" % fn)
+
+    def _array(self, obj, fn, what, shape, typestrs, strided_rows=False):
+        """Pointer, typestr and row stride of ``obj``'s __cuda_array_interface__ (v3) after checking its shape, dtype,
+        strides and device; if it names a stream, the batch's stream waits for that stream's work (an event)."""
+        name = "DeviceLoop.%s" % fn
+        try:
+            cai = obj.__cuda_array_interface__
+        except AttributeError:
+            raise TypeError("%s: %s has no __cuda_array_interface__ (a torch or CuPy array, or a DeviceArray, in GPU "
+                            "memory)" % (name, what))
+        shape_o, typestr = tuple(int(v) for v in cai["shape"]), cai["typestr"]
+        if shape_o != shape:
+            raise ValueError("%s: %s of shape %s, expected %s" % (name, what, shape_o, shape))
+        if typestr not in typestrs:
+            raise ValueError("%s: %s of dtype %s, expected one of %s" % (name, what, typestr, ", ".join(typestrs)))
+        item = int(typestr[2:])
+        dense = tuple(int(np.prod(shape[d + 1:])) * item for d in range(len(shape)))
+        strides = cai.get("strides")
+        strides = dense if strides is None else tuple(int(v) for v in strides)
+        row = strides[0] if len(shape) > 1 else item
+        ok = strides[1:] == dense[1:] and (shape[0] == 1 or (row >= dense[0] if strided_rows else row == dense[0]))
+        if not ok:
+            raise ValueError("%s: %s with strides %s (%s)" % (name, what, strides, "rows may be strided, their elements "
+                             "must be contiguous" if strided_rows else "must be C-contiguous"))
+        if shape[0] == 1:
+            row = dense[0]
+        dev = getattr(obj, "device", None)
+        if dev is not None:
+            dtype_, index = getattr(dev, "type", "cuda"), getattr(dev, "index", getattr(dev, "id", None))
+            if dtype_ != "cuda" or (index is not None and int(index) != self.device):
+                raise ValueError("%s: %s is on device %s, the batch on cuda:%d" % (name, what, dev, self.device))
+        stream = cai.get("stream")
+        if stream is not None:
+            check(lib.b200mppi_loop_wait_stream(self._handle, C.c_void_p(int(stream))))
+        return C.c_void_p(int(cai["data"][0])), typestr, row
+
+    def solve(self, out=None):
+        """One solve of every running planner.  Returns a DeviceArray, a (K, T, 2) float32 view of the loop's own buffer
+        (its __cuda_array_interface__ names the batch's stream) that the next solve() overwrites; with ``out``, a
+        caller's (K, T, 2) float32 C-contiguous device array, the controls go there and ``out`` is returned.  Row k is
+        planner k's new controls, NaN once it has stopped."""
+        self._live("solve")
+        if out is None:
+            check(lib.b200mppi_loop_solve(self._handle, C.c_void_p(self._u._dev_ptr())))
+            return self._u
+        p, _, _ = self._array(out, "solve", "out", (self.K, self.T, 2), ("<f4",))
+        check(lib.b200mppi_loop_solve(self._handle, p))
+        return out
+
+    def shift_and_update(self, x):
+        """Every running planner takes its new pose x[k] ((K, 3) float64 or float32 on the batch's device; rows may be
+        strided, their elements not): its controls shift by one row and its next solve plans from float32(x[k])."""
+        self._live("shift_and_update")
+        p, typestr, row = self._array(x, "shift_and_update", "x", (self.K, 3), ("<f8", "<f4"), strided_rows=True)
+        check(lib.b200mppi_loop_shift_and_update(self._handle, p, _lib.POSE_F64 if typestr == "<f8" else _lib.POSE_F32,
+                                                 row))
+
+    def stop(self, done):
+        """Planner k stops for good where done[k] ((K,) int32, bool or uint8 on the device) is nonzero."""
+        self._live("stop")
+        p, typestr, _ = self._array(done, "stop", "done", (self.K,), ("<i4", "|b1", "|u1"))
+        check(lib.b200mppi_loop_stop(self._handle, p, 4 if typestr == "<i4" else 1))
+
+    def close(self):
+        """Wait for the stream, commit every planner (as after the host loop) and free the loop.  Idempotent."""
+        h, self._handle = getattr(self, "_handle", None), None
+        if h is None:
+            return
+        b = self.batch
+        S = (_lib.LoopSummary * self.K)()
+        try:
+            check(lib.b200mppi_loop_close(h, S))
+        finally:
+            b._loop = None
+            for p in b.planners:
+                for obj in (p, getattr(p, "lin_tdm", None), getattr(p, "ang_tdm", None)):
+                    if obj is not None:
+                        obj._device_loop = None
+        solves, shifts, status = np.zeros(self.K, np.int64), np.zeros(self.K, np.int64), [None] * self.K
+        for j, p in enumerate(b.planners):
+            s, i = S[j], b.order[j]
+            solves[i], shifts[i], status[i] = s.solves, s.shifts, LOOP_STATUS[s.status]
+            if s.solves > 0 and not b._tdm[j]:
+                p.u_prev_d = p._u_prev_buf             # as each planner's own solve() does (mppi.py:292,362)
+            if s.shifts > 0:
+                p.params["x0"] = np.array(s.x[:], dtype=np.float64)     # shift_and_update(x[k], ...)
+        self.solves, self.shifts, self.status = solves, shifts, status

@@ -965,7 +965,13 @@ struct b200mppi_planner {
   cudaEvent_t ev_reach = nullptr;   // after the reach read-back copy (stage_sample_tdms)
   float last_ms[B200MPPI_T_COUNT] = {};
   int64_t launches = 0;
+  const b200mppi_loop* loop = nullptr;   // the open device loop of a batch holding this planner (b200mppi_batch_loop_open)
 };
+
+// The refusal of a call on a planner or batch whose device loop is open: the loop's kernels own its state until it closes
+static int loop_busy(const char* fn) {
+  return fail(B200MPPI_EINVAL, std::string(fn) + ": a device loop is open on its batch (b200mppi_loop_close it first)");
+}
 
 static int planner_check_ready(b200mppi_planner* p) {
   if (p->cfg.mode == B200MPPI_MODE_BAREBONE)
@@ -1113,6 +1119,7 @@ extern "C" int b200mppi_planner_create(const b200mppi_config* cfg, b200mppi_plan
 
 extern "C" int b200mppi_planner_destroy(b200mppi_planner* p) {
   if (!p) return B200MPPI_OK;
+  if (p->loop) return loop_busy("planner_destroy");
   cudaSetDevice(p->cfg.device);
   if (p->stream) cudaStreamSynchronize(p->stream);
   cudaFree(p->noise); cudaFree(p->u_cur); cudaFree(p->u_prev); cudaFree(p->costs); cudaFree(p->weights);
@@ -1131,6 +1138,7 @@ extern "C" int b200mppi_planner_destroy(b200mppi_planner* p) {
 }
 
 extern "C" int b200mppi_planner_set_stream(b200mppi_planner* p, void* s) {
+  if (p && p->loop) return loop_busy("planner_set_stream");
   if (!p) return fail(B200MPPI_EINVAL, "null planner");
   if (p->own_stream && p->stream) { cudaStreamSynchronize(p->stream); cudaStreamDestroy(p->stream); }
   p->stream = (cudaStream_t)s;
@@ -1139,6 +1147,7 @@ extern "C" int b200mppi_planner_set_stream(b200mppi_planner* p, void* s) {
 }
 
 extern "C" int b200mppi_planner_set_tdms(b200mppi_planner* p, b200mppi_tdm* lin, b200mppi_tdm* ang) {
+  if (p && p->loop) return loop_busy("planner_set_tdms");
   if (!p || !lin || !ang) return fail(B200MPPI_EINVAL, "set_tdms: null argument");
   if (lin->cfg.device != p->cfg.device || ang->cfg.device != p->cfg.device)
     return fail(B200MPPI_EINVAL, "set_tdms: TDMs live on another device");
@@ -1155,6 +1164,7 @@ extern "C" int b200mppi_planner_set_tdms(b200mppi_planner* p, b200mppi_tdm* lin,
 }
 
 extern "C" int b200mppi_planner_set_params(b200mppi_planner* p, const b200mppi_params* q) {
+  if (p && p->loop) return loop_busy("planner_set_params");
   if (!p || !q) return fail(B200MPPI_EINVAL, "set_params: null argument");
   if (!(q->dt > 0) || q->num_opt < 0) return fail(B200MPPI_EINVAL, "set_params: bad dt/num_opt");
   p->prm = *q;
@@ -1163,6 +1173,7 @@ extern "C" int b200mppi_planner_set_params(b200mppi_planner* p, const b200mppi_p
 }
 
 extern "C" int b200mppi_planner_set_u(b200mppi_planner* p, const float* u) {
+  if (p && p->loop) return loop_busy("planner_set_u");
   if (!p || !u) return fail(B200MPPI_EINVAL, "set_u: null argument");
   CU(cudaSetDevice(p->cfg.device));
   std::memcpy(p->h_u, u, (size_t)p->T * 2 * sizeof(float));
@@ -1173,6 +1184,7 @@ extern "C" int b200mppi_planner_set_u(b200mppi_planner* p, const float* u) {
 }
 
 extern "C" int b200mppi_planner_get_u(b200mppi_planner* p, float* u) {
+  if (p && p->loop) return loop_busy("planner_get_u");
   if (!p || !u) return fail(B200MPPI_EINVAL, "get_u: null argument");
   CU(cudaSetDevice(p->cfg.device));
   CU(cudaMemcpyAsync(p->h_u, p->u_cur, (size_t)p->T * 2 * sizeof(float), cudaMemcpyDeviceToHost, p->stream));
@@ -1182,6 +1194,7 @@ extern "C" int b200mppi_planner_get_u(b200mppi_planner* p, float* u) {
 }
 
 extern "C" int b200mppi_planner_shift_u(b200mppi_planner* p, int32_t shifts) {
+  if (p && p->loop) return loop_busy("planner_shift_u");
   if (!p) return fail(B200MPPI_EINVAL, "null planner");
   CU(cudaSetDevice(p->cfg.device));
   launch_shift_u(p->u_cur, p->T, shifts, p->stream);
@@ -1408,6 +1421,7 @@ static int stage_update_finish(b200mppi_planner* p, const float* gathered, int c
 }
 
 extern "C" int b200mppi_planner_set_obstacles(b200mppi_planner* p, const float* xy, const float* rad, int32_t count) {
+  if (p && p->loop) return loop_busy("planner_set_obstacles");
   if (!p || count < 0 || (count > 0 && (!xy || !rad))) return fail(B200MPPI_EINVAL, "set_obstacles: bad argument");
   CU(cudaSetDevice(p->cfg.device));
   if (count > p->obstacles_cap) {
@@ -1599,6 +1613,7 @@ static int iteration_rollouts(b200mppi_planner* p, bool first) {
 }
 
 extern "C" int b200mppi_planner_solve(b200mppi_planner* p, float* u_out) {
+  if (p && p->loop) return loop_busy("planner_solve");
   if (!p) return fail(B200MPPI_EINVAL, "null planner");
   if (p->cfg.world_size != 1) return fail(B200MPPI_ESTATE, "solve: world_size > 1, use solve_local/solve_finish");
   int rc = planner_check_ready(p);
@@ -1627,6 +1642,7 @@ extern "C" int b200mppi_planner_solve(b200mppi_planner* p, float* u_out) {
 }
 
 extern "C" int b200mppi_planner_solve_local(b200mppi_planner* p, int32_t first_iteration) {
+  if (p && p->loop) return loop_busy("planner_solve_local");
   if (!p) return fail(B200MPPI_EINVAL, "null planner");
   int rc = planner_check_ready(p);
   if (rc) return rc;
@@ -1639,6 +1655,7 @@ extern "C" int b200mppi_planner_solve_local(b200mppi_planner* p, int32_t first_i
 }
 
 extern "C" int b200mppi_planner_solve_reduce(b200mppi_planner* p, const float* exchanged_dev) {
+  if (p && p->loop) return loop_busy("planner_solve_reduce");
   if (!p || !exchanged_dev) return fail(B200MPPI_EINVAL, "solve_reduce: null argument");
   if (!p->shard_maps) return fail(B200MPPI_ESTATE, "solve_reduce: only for MODE_TDM with world_size > 1");
   CU(cudaSetDevice(p->cfg.device));
@@ -1652,6 +1669,7 @@ extern "C" int b200mppi_planner_solve_reduce(b200mppi_planner* p, const float* e
 }
 
 extern "C" int b200mppi_planner_solve_finish(b200mppi_planner* p, const float* gathered_dev, float* u_out) {
+  if (p && p->loop) return loop_busy("planner_solve_finish");
   if (!p || !gathered_dev) return fail(B200MPPI_EINVAL, "solve_finish: null argument");
   if (p->cfg.world_size > 512) return fail(B200MPPI_EINVAL, "solve_finish: world_size > 512");
   CU(cudaSetDevice(p->cfg.device));
@@ -1825,6 +1843,7 @@ extern "C" int b200mppi_planner_p2p_finish(b200mppi_planner* p, float* u_out) {
 }
 
 extern "C" int b200mppi_planner_solve_p2p(b200mppi_planner* p, float* u_out) {
+  if (p && p->loop) return loop_busy("planner_solve_p2p");
   int rc = p2p_check(p, "solve_p2p");
   if (rc) return rc;
   if (!u_out) return fail(B200MPPI_EINVAL, "solve_p2p: null output");
@@ -1866,6 +1885,7 @@ extern "C" int b200mppi_combine_partials_host(const float* g, int32_t ws, int32_
 
 // ---- stage-level entry points
 extern "C" int b200mppi_planner_sample_noise(b200mppi_planner* p) {
+  if (p && p->loop) return loop_busy("planner_sample_noise");
   if (!p) return fail(B200MPPI_EINVAL, "null planner");
   if (!p->params_set) return fail(B200MPPI_ESTATE, "sample_noise: params not set");
   CU(cudaSetDevice(p->cfg.device));
@@ -1876,6 +1896,7 @@ extern "C" int b200mppi_planner_sample_noise(b200mppi_planner* p) {
 }
 
 extern "C" int b200mppi_planner_rollout(b200mppi_planner* p) {
+  if (p && p->loop) return loop_busy("planner_rollout");
   if (!p) return fail(B200MPPI_EINVAL, "null planner");
   int rc = planner_check_ready(p);
   if (rc) return rc;
@@ -1890,6 +1911,7 @@ extern "C" int b200mppi_planner_rollout(b200mppi_planner* p) {
 }
 
 extern "C" int b200mppi_planner_cvar(b200mppi_planner* p) {
+  if (p && p->loop) return loop_busy("planner_cvar");
   if (!p) return fail(B200MPPI_EINVAL, "null planner");
   if (!p->params_set) return fail(B200MPPI_ESTATE, "cvar: params not set");
   if (p->cfg.mode != B200MPPI_MODE_TDM) return fail(B200MPPI_ESTATE, "cvar: only MODE_TDM has per-(n,m) costs");
@@ -1904,6 +1926,7 @@ extern "C" int b200mppi_planner_cvar(b200mppi_planner* p) {
 }
 
 extern "C" int b200mppi_planner_update(b200mppi_planner* p, const float* costs_host) {
+  if (p && p->loop) return loop_busy("planner_update");
   if (!p) return fail(B200MPPI_EINVAL, "null planner");
   if (!p->params_set) return fail(B200MPPI_ESTATE, "update: params not set");
   CU(cudaSetDevice(p->cfg.device));
@@ -1916,6 +1939,7 @@ extern "C" int b200mppi_planner_update(b200mppi_planner* p, const float* costs_h
 }
 
 extern "C" int b200mppi_planner_get_state_rollout(b200mppi_planner* p, float* out, size_t bytes) {
+  if (p && p->loop) return loop_busy("planner_get_state_rollout");
   if (!p || !out) return fail(B200MPPI_EINVAL, "null argument");
   int rc = planner_check_ready(p);
   if (rc) return rc;
@@ -1980,6 +2004,7 @@ static void costs_logical(const b200mppi_planner* p, const float* dev_layout, fl
 }
 
 extern "C" int b200mppi_planner_copy_out(b200mppi_planner* p, int32_t id, void* dst, size_t bytes) {
+  if (p && p->loop) return loop_busy("planner_copy_out");
   void* d; size_t b;
   int rc = b200mppi_planner_buffer(p, id, &d, &b);
   if (rc) return rc;
@@ -1998,6 +2023,7 @@ extern "C" int b200mppi_planner_copy_out(b200mppi_planner* p, int32_t id, void* 
 }
 
 extern "C" int b200mppi_planner_copy_in(b200mppi_planner* p, int32_t id, const void* src, size_t bytes) {
+  if (p && p->loop) return loop_busy("planner_copy_in");
   void* d; size_t b;
   int rc = b200mppi_planner_buffer(p, id, &d, &b);
   if (rc) return rc;
@@ -2017,6 +2043,7 @@ extern "C" int b200mppi_planner_copy_in(b200mppi_planner* p, int32_t id, const v
 }
 
 extern "C" int b200mppi_planner_set_noise(b200mppi_planner* p, const float* noise, size_t bytes) {
+  if (p && p->loop) return loop_busy("planner_set_noise");
   return b200mppi_planner_copy_in(p, B200MPPI_BUF_NOISE, noise, bytes);
 }
 
@@ -2115,6 +2142,7 @@ struct b200mppi_batch {
   bool mixed = false;
   int nmap = 0;
   size_t off_nprep = 0;
+  const b200mppi_loop* loop = nullptr;   // its open device loop (b200mppi_batch_loop_open)
 };
 
 // Hands out 256-byte-aligned sections of one allocation, in order: take returns a section's offset.  An empty section
@@ -2129,6 +2157,7 @@ struct Sections {
 };
 
 extern "C" int b200mppi_batch_destroy(b200mppi_batch* b) {
+  if (b && b->loop) return loop_busy("batch_destroy");
   if (!b) return B200MPPI_OK;
   cudaSetDevice(b->device);
   if (b->stream) cudaStreamSynchronize(b->stream);
@@ -2261,6 +2290,7 @@ extern "C" int b200mppi_batch_create_mixed(b200mppi_planner* const* planners, in
 }
 
 extern "C" int b200mppi_batch_set_stream(b200mppi_batch* b, void* s) {
+  if (b && b->loop) return loop_busy("batch_set_stream");
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
   if (b->own_stream && b->stream) { cudaStreamSynchronize(b->stream); cudaStreamDestroy(b->stream); }
   b->stream = (cudaStream_t)s;
@@ -2275,6 +2305,7 @@ extern "C" int b200mppi_batch_launch_count(b200mppi_batch* b, int64_t* out) {
 }
 
 extern "C" int b200mppi_batch_share_tdms(b200mppi_batch* b, int32_t enable) {
+  if (b && b->loop) return loop_busy("batch_share_tdms");
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
   b->share = enable != 0;
   return B200MPPI_OK;
@@ -2673,6 +2704,7 @@ static int batch_solve_parts(b200mppi_batch* b) {
 }
 
 extern "C" int b200mppi_batch_solve(b200mppi_batch* b, float* u_out) {
+  if (b && b->loop) return loop_busy("batch_solve");
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
   int rc = batch_validate(b);
   if (rc) return rc;
@@ -2727,6 +2759,7 @@ static VisBatchDesc vis_desc(const b200mppi_planner* p, const RolloutParams* dp,
 }
 
 extern "C" int b200mppi_batch_get_state_rollout(b200mppi_batch* b, float* out, size_t bytes) {
+  if (b && b->loop) return loop_busy("batch_get_state_rollout");
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
   if (!out) return fail(B200MPPI_EINVAL, "batch_get_state_rollout: null output");
   int V = 0;
@@ -2973,10 +3006,11 @@ static void onemap_trial_classes(TrialPart& q) {
 struct TrialLayout {
   struct Part { size_t set[2] = {}, grp = 0, mem = 0, cls = 0; };   // a kind's sampler sets (by parity), group
   Part part[2];                                                     // descriptors, members and class lists
-  size_t box = 0, rec = 0, grec = 0, state = 0, con = 0, res = 0, res_end = 0, tr = 0, act = 0, seq = 0, start = 0;
+  size_t box = 0, rec = 0, grec = 0, state = 0, con = 0, res = 0, loop = 0, res_end = 0, tr = 0, act = 0, seq = 0,
+         start = 0;
   size_t vis = 0, rflag = 0, head = 0;                 // head: the sections staged and uploaded with one copy
   std::vector<size_t> grid;                            // per slot
-  size_t vrec = 0, xh = 0, uh = 0, total = 0;
+  size_t vrec = 0, xh = 0, uh = 0, lu = 0, total = 0;
 };
 
 // One trial call passed through its phases: the request, both kinds' parts, the layout and the buffers
@@ -3001,7 +3035,35 @@ struct TrialCall {
   PlantArgs pa{};
   SeqArgs sa{};
   RolloutWinArgs g0{};                                 // the stochastic planners' first windowed rollout descriptor
+  // a device loop (b200mppi_batch_loop_open) instead of a trial: no descriptors, grids, histories or plant step; per
+  // planner its padded limits (K x 4, null for barebone) and its row in the caller's arrays (null: its index)
+  bool loop = false;
+  const double* limits = nullptr;
+  const int32_t* rows = nullptr;
 };
+
+// What a device loop checks in place of trial_validate: a batch that can solve, num_opt >= 1, padded limits for every
+// planner that has a map, and rows that are a permutation of 0 .. K-1
+static int loop_validate(TrialCall& t) {
+  b200mppi_batch* b = t.b;
+  if (!t.barebone && b->mode == B200MPPI_MODE_BAREBONE)
+    return fail(B200MPPI_EINVAL, t.fn + ": planner 0 is MODE_BAREBONE (its loops are of kind B200MPPI_TRIALS_BAREBONE)");
+  int rc = batch_validate(b);
+  if (rc) return rc;
+  if (!t.barebone && !t.limits) return fail(B200MPPI_EINVAL, t.fn + ": null padded limits");
+  std::vector<char> seen(t.K, 0);
+  for (int i = 0; i < t.K; ++i) {
+    const std::string who = t.fn + ": planner " + std::to_string(i);
+    if (b->pl[i]->prm.num_opt < 1) return fail(B200MPPI_EINVAL, who + " has num_opt < 1");
+    for (int c = 0; c < 4 && !t.barebone; ++c)
+      if (std::isnan(t.limits[4 * i + c])) return fail(B200MPPI_EINVAL, who + ": padded limit is NaN");
+    const int r = t.rows ? t.rows[i] : i;
+    if (r < 0 || r >= t.K || seen[r]) return fail(B200MPPI_EINVAL, who + ": row " + std::to_string(r) + " out of range "
+                                                                 "or taken twice (rows must be a permutation of 0 .. K-1)");
+    seen[r] = 1;
+  }
+  return B200MPPI_OK;
+}
 
 // Everything a trial call checks before it allocates or issues anything
 static int trial_call_validate(TrialCall& t) {
@@ -3009,7 +3071,7 @@ static int trial_call_validate(TrialCall& t) {
   const bool stochastic = t.kind == TrialKind::stochastic, mixed = t.kind == TrialKind::mixed;
   t.barebone = t.kind == TrialKind::barebone;
   t.seq = t.episodes != nullptr;
-  t.fn = t.seq ? (t.barebone ? "run_barebone_trial_sequences" : "run_trial_sequences") : stochastic ? "run_stochastic_trials"
+  t.fn = t.loop ? "loop_open" : t.seq ? (t.barebone ? "run_barebone_trial_sequences" : "run_trial_sequences") : stochastic ? "run_stochastic_trials"
          : t.barebone ? "run_barebone_trials" : mixed ? "run_mixed_trials" : "run_trials";
   const std::string& fn = t.fn;
   t.K = (int)b->pl.size();
@@ -3043,9 +3105,9 @@ static int trial_call_validate(TrialCall& t) {
   if (!b->stochastic && stochastic)
     return fail(B200MPPI_EINVAL, fn + ": planner 0 is " + mode_name(b->mode) +
                                      " (stochastic trials run MODE_TDM batches; b200mppi_batch_run_trials runs the others)");
-  int rc = trial_validate(b, t.kind, t.trials, t.S, fn.c_str(), t.first, t.seq, t.in_place);
+  int rc = t.loop ? loop_validate(t) : trial_validate(b, t.kind, t.trials, t.S, fn.c_str(), t.first, t.seq, t.in_place);
   if (rc) return rc;
-  if (!t.xhist || !t.uhist || !t.results || (t.barebone && !t.contact_steps))
+  if (!t.loop && (!t.xhist || !t.uhist || !t.results || (t.barebone && !t.contact_steps)))
     return fail(B200MPPI_EINVAL, fn + ": null output buffer");
   t.nslot = t.first[t.K];
   t.record = t.record_every > 0;
@@ -3113,6 +3175,7 @@ static TrialLayout trial_layout(const TrialCall& t) {
   L.state = s.take(K * sizeof(TrialState));
   L.con = s.take((t.barebone ? nslot : 0) * sizeof(int));   // barebone contacts, per slot
   L.res = s.take(nres * sizeof(TrialState));
+  L.loop = s.take((t.loop ? K : 0) * sizeof(LoopState));   // a loop's per-planner counters and poses
   L.res_end = s.end;
   L.tr = s.take(nslot * sizeof(TrialDev));
   L.act = s.take((K + 1) * sizeof(int));               // active (K), the count of running planners
@@ -3127,10 +3190,11 @@ static TrialLayout trial_layout(const TrialCall& t) {
   // K 8, 150 steps, V 100, T 100) are copied straight into the caller's array.
   L.grid.resize(nslot);
   for (size_t j = 0; j < nslot; ++j)
-    L.grid[j] = s.take(t.barebone || t.in_place[j] ? 0 : 2 * (size_t)t.trials[j].height * t.trials[j].width * sizeof(double));
+    L.grid[j] = s.take(t.barebone || t.loop || t.in_place[j] ? 0 : 2 * (size_t)t.trials[j].height * t.trials[j].width * sizeof(double));
   L.vrec = s.take(t.rec_bytes);                        // (slots, R, V, T+1, 3)
-  L.xh = s.take(nslot * (S + 1) * 3 * sizeof(double));
+  L.xh = s.take((t.loop ? 0 : nslot * (S + 1) * 3) * sizeof(double));
   L.uh = s.take(nslot * S * 2 * sizeof(float));
+  L.lu = s.take((t.loop ? K * t.b->T * 2 : 0) * sizeof(float));   // a loop's own (K, T, 2) controls
   L.total = s.end;
   return L;
 }
@@ -3166,9 +3230,29 @@ static int trial_call_stage(TrialCall& t) {
       hv[i] = vis_desc(p, sto ? &dw[r].p : &dr[i].p, drec + (size_t)first[i] * R * t.per);
     if (t.rec_seq) reinterpret_cast<int*>(h + L.rflag)[i] = 1;
     hst[i] = TrialState{};
-    for (int c = 0; c < 3; ++c) hst[i].x[c] = trials[first[i]].x0[c];
+    for (int c = 0; c < 3; ++c) hst[i].x[c] = t.loop ? (double)p->prm.x0[c] : trials[first[i]].x0[c];
     hact[i] = 1;
-    for (int j = first[i]; j < first[i + 1]; ++j) {    // the planner's episodes: one, or its sequence
+    if (t.loop) {                                      // from the pose of the params the batch's descriptors were built from
+      LoopState& ls = reinterpret_cast<LoopState*>(h + L.loop)[i];
+      ls = LoopState{};
+      for (int c = 0; c < 3; ++c) { ls.x[c] = p->prm.x0[c]; ls.x0[c] = p->prm.x0[c]; }
+      ls.bounded = !t.barebone;
+      if (ls.bounded) {
+        const double* lim = t.limits + 4 * i;
+        ls.pxlim[0] = lim[0]; ls.pxlim[1] = lim[1]; ls.pylim[0] = lim[2]; ls.pylim[1] = lim[3];
+      }
+      ls.row = t.rows ? t.rows[i] : i;
+      TrialDev& td = ht[i];                            // what the loop kernels read: the shift, the next x0 and window
+      td = TrialDev{};
+      td.u_cur = p->u_cur;
+      td.x0_out = sto ? dw[r].p.x0 : dr[i].p.x0;
+      if (sto) {
+        const b200mppi_tdm* l = p->lin;
+        td.win = &dw[r].WW;
+        td.win_pxl = l->pxl[0]; td.win_pyl = l->pyl[0]; td.win_res = l->res; td.win_rows = l->rows; td.win_cols = l->cols;
+      }
+    }
+    for (int j = first[i]; j < first[i + 1] && !t.loop; ++j) {    // the planner's episodes: one, or its sequence
       const b200mppi_trial_desc& q = trials[j];
       if (t.barebone) hcon[j] = 0;
       TrialDev& td = ht[j];
@@ -3253,7 +3337,7 @@ static int trial_call_stage(TrialCall& t) {
   if (t.K2 > 0) t.g0 = *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win);
   cudaStream_t st = b->stream;
   CU(cudaMemcpyAsync(d, h, L.head, cudaMemcpyHostToDevice, st));
-  for (int j = 0; j < t.nslot && !t.barebone; ++j) {  // pageable sources: staged by the driver before the call returns
+  for (int j = 0; j < t.nslot && !t.barebone && !t.loop; ++j) {  // pageable sources: staged by the driver before the call returns
     if (t.in_place[j]) continue;
     const size_t bytes = (size_t)trials[j].height * trials[j].width * sizeof(double);
     CU(cudaMemcpyAsync(d + L.grid[j], trials[j].lin, bytes, cudaMemcpyHostToDevice, st));
@@ -3266,7 +3350,8 @@ static int trial_call_stage(TrialCall& t) {
   return B200MPPI_OK;
 }
 
-// The launches of step s, each counted where it is issued
+// The launches of step s but its plant step (trial_call_plant; a device loop runs the caller's plant), each counted where
+// it is issued
 static int trial_call_step(TrialCall& t, int s) {
   b200mppi_batch* b = t.b;
   const unsigned char* d = t.d;
@@ -3339,12 +3424,60 @@ static int trial_call_step(TrialCall& t, int s) {
     b->launches++;
     CHECK_LAUNCH();
   }
+  return B200MPPI_OK;
+}
+
+// The plant step that ends trial step s
+static int trial_call_plant(TrialCall& t, int s) {
+  cudaStream_t st = t.b->stream;
   t.pa.step = s;
   if (t.seq) launch_plant_step_seq(t.pa, t.sa, st);
   else launch_plant_step(t.pa, st);
-  b->launches++;
+  t.b->launches++;
   CHECK_LAUNCH();
   return B200MPPI_OK;
+}
+
+// Leaves every planner and every TDM group's pair as after the host loop in which planner i solved ran[i] times, the
+// last time from x0[3 i ..]; t.h holds the box records read back.  A planner that never solved is left as it was.
+static void trial_commit_planners(TrialCall& t, const std::vector<int>& ran, const std::vector<float>& x0) {
+  const TrialLayout& L = t.L;
+  const unsigned char* h = t.h;
+  const int K1 = t.K1, num_opt = t.b->pl[0]->prm.num_opt;
+  const int* hrec = reinterpret_cast<const int*>(h + L.rec);
+  for (int i = 0; i < t.K; ++i) {
+    // host state as after ran[i] solves: the reach slot toggled once per iteration, the last solve's box and x0 (the
+    // samplings of the pair below)
+    b200mppi_planner* p = t.b->pl[i];
+    const int n = ran[i];
+    p->prepared = false;
+    p->pushed_direct = false;
+    if (n == 0) continue;
+    if (i >= K1) {
+      const int* rec = hrec + 5 * (i - K1);
+      p->reach_slot ^= (n * num_opt) & 1;
+      p->reach_valid = true;
+      for (int c = 0; c < 5; ++c) p->last_box[c] = rec[c];
+    } else if (!t.barebone) {
+      last_box_whole_map(p);
+    }
+    for (int c = 0; c < 3; ++c) p->prm.x0[c] = x0[3 * i + c];
+  }
+  // each TDM group's pair as after the samplings of its longest-running member (a group samples at every solve while any
+  // member runs), a stochastic pair's last kind from the group's record (a group of one: its planner's)
+  for (int k = 0; k < 2; ++k) {
+    TrialPart& q = t.P[k];
+    for (int g = 0; g < q.G; ++g) {
+      int n = 0;
+      for (int j = q.gr.first[g]; j < q.gr.first[g + 1]; ++j) n = std::max(n, ran[q.lo + q.gr.members[j]]);
+      if (n == 0) continue;
+      if (k == 1) {
+        const int* rec = q.grouped ? reinterpret_cast<const int*>(h + L.grec) + 5 * g : hrec + 5 * q.gr.lead(g);
+        q.plans[g].boxed[0] = q.plans[g].boxed[1] = rec[0] != 0;
+      }
+      for (int s = 0; s < n; ++s) { plan_commit(q.plans[g], 0); plan_commit(q.plans[g], 1); }
+    }
+  }
 }
 
 // Reads back the states and histories, and leaves the caller's outputs, every planner and every TDM group's pair as
@@ -3355,7 +3488,7 @@ static int trial_call_commit(TrialCall& t) {
   const unsigned char* d = t.d;
   unsigned char* h = t.h;
   cudaStream_t st = b->stream;
-  const int K = t.K, K1 = t.K1, S = t.S, R = t.R, num_opt = b->pl[0]->prm.num_opt;
+  const int K = t.K, S = t.S, R = t.R;
   const size_t per = t.per;
   const std::vector<int>& first = t.first;
   b200mppi_trial_result* results = t.results;
@@ -3363,7 +3496,6 @@ static int trial_call_commit(TrialCall& t) {
   CU(cudaMemcpyAsync(h + L.rec, d + L.rec, L.res_end - L.rec, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(h + L.head, d + L.xh, L.total - L.xh, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  const int* hrec = reinterpret_cast<const int*>(h + L.rec);
   const TrialState* hst = reinterpret_cast<const TrialState*>(h + L.state);
   const TrialState* hres = reinterpret_cast<const TrialState*>(h + L.res);
   const int* hcon = reinterpret_cast<const int*>(h + L.con);
@@ -3372,6 +3504,7 @@ static int trial_call_commit(TrialCall& t) {
   const double dnan = std::nan("");
   const float fnan = std::nanf("");
   std::vector<int> ran(K, 0);                          // steps each planner ran, over all its episodes
+  std::vector<float> x0(3 * (size_t)K);                // the x0 of each planner's last solve
   for (int i = 0; i < K; ++i) {
     int last = first[i];                               // the planner's last slot that ran
     for (int j = first[i]; j < first[i + 1]; ++j) {
@@ -3391,40 +3524,14 @@ static int trial_call_commit(TrialCall& t) {
       ran[i] += n;
       if (t.barebone) t.contact_steps[j] = hcon[j];
     }
-    // host state as after ran[i] rounds of the host loop: the reach slot toggled once per iteration, the last solve's
-    // box and x0 (the samplings of the pair below).  The last solve planned from the pose before the last step -- or,
-    // when a later episode of a sequence without reset_x0 took one step, from the previous episode's final pose
-    b200mppi_planner* p = b->pl[i];
-    const int n = ran[i];
-    if (i >= K1) {
-      const int* rec = hrec + 5 * (i - K1);
-      p->reach_slot ^= (n * num_opt) & 1;
-      p->reach_valid = true;
-      for (int c = 0; c < 5; ++c) p->last_box[c] = rec[c];
-    } else if (!t.barebone) {
-      last_box_whole_map(p);
-    }
-    p->prepared = false;
-    p->pushed_direct = false;
-    const double* x0 = t.xhist + ((size_t)last * (S + 1) + results[last].steps - 1) * 3;
+    // the last solve planned from the pose before the last step -- or, when a later episode of a sequence without
+    // reset_x0 took one step, from the previous episode's final pose
+    const double* xl = t.xhist + ((size_t)last * (S + 1) + results[last].steps - 1) * 3;
     if (results[last].steps == 1 && last > first[i] && !t.reset_x0)
-      x0 = t.xhist + ((size_t)(last - 1) * (S + 1) + results[last - 1].steps) * 3;
-    for (int c = 0; c < 3; ++c) p->prm.x0[c] = (float)x0[c];
+      xl = t.xhist + ((size_t)(last - 1) * (S + 1) + results[last - 1].steps) * 3;
+    for (int c = 0; c < 3; ++c) x0[3 * i + c] = (float)xl[c];
   }
-  // each TDM group's pair as after the samplings of its longest-running member (a group samples at every step while any
-  // member runs), a stochastic pair's last kind from the group's record (a group of one: its planner's)
-  for (int k = 0; k < 2; ++k) {
-    TrialPart& q = t.P[k];
-    for (int g = 0; g < q.G; ++g) {
-      int n = 0;
-      for (int j = q.gr.first[g]; j < q.gr.first[g + 1]; ++j) n = std::max(n, ran[q.lo + q.gr.members[j]]);
-      if (k == 1) {
-        const int* rec = q.grouped ? reinterpret_cast<const int*>(h + L.grec) + 5 * g : hrec + 5 * q.gr.lead(g);
-        q.plans[g].boxed[0] = q.plans[g].boxed[1] = rec[0] != 0;
-      }
-      for (int s = 0; s < n; ++s) { plan_commit(q.plans[g], 0); plan_commit(q.plans[g], 1); }
-    }
-  }
+  trial_commit_planners(t, ran, x0);
   if (!t.record) return B200MPPI_OK;
   // record r of a slot belongs to step r * record_every of its episode; slot first[i] + e goes to the caller's slab
   // (i, e).  Only the written ones are copied (records past an episode's last step are never written, and an early
@@ -3470,6 +3577,7 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
                             int32_t record_every, float* rollouts, size_t rollout_bytes, int32_t* steps_issued,
                             const int32_t* episodes, int32_t reset_x0) {
   if (!b) return fail(B200MPPI_EINVAL, "null batch");
+  if (b->loop) return loop_busy("run_trials");
   TrialCall t{b, kind, trials, max_steps, xhist, uhist, results, contact_steps, record_every, rollouts, rollout_bytes,
               episodes, reset_x0 != 0};
   int rc;
@@ -3505,7 +3613,7 @@ static int batch_run_trials(b200mppi_batch* b, TrialKind kind, const b200mppi_tr
       CU(cudaEventSynchronize(buf.ev[s % TRIAL_POLL]));
       if (hcount[s % TRIAL_POLL] == 0) break;
     }
-    if ((rc = trial_call_step(t, s))) return rc;
+    if ((rc = trial_call_step(t, s)) || (rc = trial_call_plant(t, s))) return rc;
     ++issued;
     CU(cudaMemcpyAsync(hcount + s % TRIAL_POLL, t.pa.active_count, sizeof(int), cudaMemcpyDeviceToHost, b->stream));
     CU(cudaEventRecord(buf.ev[s % TRIAL_POLL], b->stream));
@@ -3595,4 +3703,166 @@ extern "C" int b200mppi_batch_run_trial_sequences_ex(b200mppi_batch* b, int32_t 
                                  "B200MPPI_TRIALS_BAREBONE");
   return batch_run_trials(b, trial_kind(kind), trials, max_steps, xhist, uhist, results, contact_steps, record_every,
                           rollouts, rollout_bytes, steps_issued, episodes, reset_x0);
+}
+
+// --------------------------------------------------------------------------------------------- device loops
+// A trial call without its plant step, driven one call at a time: the phases of batch_run_trials (validation, plans,
+// layout, staging, step and the planner and TDM commit) over one device buffer that lives while the loop is open.  The
+// caller's plant runs between the calls on the batch's stream; the loop kernels (reduce.cu) take its poses and stops.
+struct b200mppi_loop {
+  TrialCall t{};
+  LoopArgs la{};
+  cudaEvent_t ev = nullptr;            // orders the batch's stream after work on the stream of a caller's array
+  int solves = 0;                      // solves issued: every running planner has solved exactly this many times
+  ~b200mppi_loop() {
+    cudaFree(t.d);
+    if (t.h) cudaFreeHost(t.h);
+    if (ev) cudaEventDestroy(ev);
+  }
+};
+
+// a caller's array at p must lie in device memory of the batch's device
+static int loop_device_ptr(const b200mppi_loop* lp, const void* p, const char* fn, const char* what) {
+  cudaPointerAttributes at{};
+  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(B200MPPI_EINVAL, std::string(fn) + ": " + what + " is not a CUDA pointer");
+  }
+  if ((at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) || at.device != lp->t.b->device)
+    return fail(B200MPPI_EINVAL, std::string(fn) + ": " + what + " is not in memory of device " +
+                                 std::to_string(lp->t.b->device));
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_batch_loop_open(b200mppi_batch* b, int32_t kind, const double* padded_limits,
+                                        const int32_t* rows, b200mppi_loop** out) {
+  if (!b || !out) return fail(B200MPPI_EINVAL, "loop_open: null argument");
+  if (b->loop) return loop_busy("loop_open");
+  if (kind != B200MPPI_TRIALS_MAP && kind != B200MPPI_TRIALS_STOCHASTIC && kind != B200MPPI_TRIALS_BAREBONE &&
+      kind != B200MPPI_TRIALS_MIXED)
+    return fail(B200MPPI_EINVAL, "loop_open: unknown trial kind " + std::to_string(kind));
+  std::unique_ptr<b200mppi_loop> lp(new b200mppi_loop());
+  TrialCall& t = lp->t;
+  t.b = b; t.kind = trial_kind(kind); t.S = 0;
+  t.loop = true; t.limits = padded_limits; t.rows = rows;
+  int rc;
+  if ((rc = trial_call_validate(t)) || (rc = trial_call_plan(t))) return rc;
+  t.L = trial_layout(t);
+  if (cudaMalloc(&t.d, t.L.total) != cudaSuccess) {
+    t.d = nullptr;
+    cudaGetLastError();
+    return fail(B200MPPI_ECUDA, "loop_open: cudaMalloc of " + std::to_string(t.L.total) + " bytes");
+  }
+  if (cudaMallocHost(&t.h, t.L.head) != cudaSuccess) {
+    t.h = nullptr;
+    return fail(B200MPPI_ECUDA, "loop_open: cudaMallocHost");
+  }
+  if ((rc = trial_call_stage(t))) return rc;
+  CU(cudaEventCreateWithFlags(&lp->ev, cudaEventDisableTiming));
+  lp->la = LoopArgs{reinterpret_cast<const TrialDev*>(t.d + t.L.tr), reinterpret_cast<LoopState*>(t.d + t.L.loop),
+                    t.pa.active, t.pa.active_count, t.K, b->T};
+  b->loop = lp.get();
+  for (b200mppi_planner* p : b->pl) p->loop = lp.get();
+  *out = lp.release();
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_loop_controls(b200mppi_loop* lp, float** u_dev, void** stream) {
+  if (!lp || !u_dev || !stream) return fail(B200MPPI_EINVAL, "loop_controls: null argument");
+  *u_dev = reinterpret_cast<float*>(lp->t.d + lp->t.L.lu);
+  *stream = lp->t.b->stream;
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_loop_wait_stream(b200mppi_loop* lp, void* stream) {
+  if (!lp) return fail(B200MPPI_EINVAL, "loop_wait_stream: null loop");
+  cudaStream_t s = (cudaStream_t)stream, st = lp->t.b->stream;
+  if (s == st) return B200MPPI_OK;
+  CU(cudaSetDevice(lp->t.b->device));
+  CU(cudaEventRecord(lp->ev, s));
+  CU(cudaStreamWaitEvent(st, lp->ev, 0));
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_loop_solve(b200mppi_loop* lp, float* u_dev) {
+  if (!lp || !u_dev) return fail(B200MPPI_EINVAL, "loop_solve: null argument");
+  int rc;
+  if ((rc = loop_device_ptr(lp, u_dev, "loop_solve", "u_dev"))) return rc;
+  b200mppi_batch* b = lp->t.b;
+  CU(cudaSetDevice(b->device));
+  if (lp->solves == INT32_MAX) return fail(B200MPPI_EINVAL, "loop_solve: 2^31 - 1 solves issued");
+  if ((rc = trial_call_step(lp->t, lp->solves))) return rc;
+  launch_loop_export(lp->la, u_dev, b->stream);
+  b->launches++;
+  CHECK_LAUNCH();
+  lp->solves++;
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_loop_shift_and_update(b200mppi_loop* lp, const void* x_dev, int32_t dtype,
+                                              int64_t row_stride_bytes) {
+  if (!lp || !x_dev) return fail(B200MPPI_EINVAL, "loop_shift_and_update: null argument");
+  if (dtype != B200MPPI_POSE_F64 && dtype != B200MPPI_POSE_F32)
+    return fail(B200MPPI_EINVAL, "loop_shift_and_update: unknown pose dtype " + std::to_string(dtype));
+  const int64_t e = dtype == B200MPPI_POSE_F64 ? 8 : 4;
+  if (row_stride_bytes < 3 * e || row_stride_bytes % e != 0 || reinterpret_cast<uintptr_t>(x_dev) % e != 0)
+    return fail(B200MPPI_EINVAL, "loop_shift_and_update: row stride of " + std::to_string(row_stride_bytes) +
+                                 " bytes or a pointer not aligned to the element (rows of 3 contiguous elements)");
+  int rc;
+  if ((rc = loop_device_ptr(lp, x_dev, "loop_shift_and_update", "x_dev"))) return rc;
+  b200mppi_batch* b = lp->t.b;
+  CU(cudaSetDevice(b->device));
+  launch_loop_ingest(lp->la, x_dev, dtype, row_stride_bytes, b->stream);
+  b->launches++;
+  CHECK_LAUNCH();
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_loop_stop(b200mppi_loop* lp, const void* mask_dev, int32_t elem_bytes) {
+  if (!lp || !mask_dev) return fail(B200MPPI_EINVAL, "loop_stop: null argument");
+  if (elem_bytes != 1 && elem_bytes != 4)
+    return fail(B200MPPI_EINVAL, "loop_stop: mask elements of " + std::to_string(elem_bytes) + " bytes (1 or 4)");
+  if (reinterpret_cast<uintptr_t>(mask_dev) % elem_bytes != 0)
+    return fail(B200MPPI_EINVAL, "loop_stop: mask not aligned to its elements");
+  int rc;
+  if ((rc = loop_device_ptr(lp, mask_dev, "loop_stop", "mask_dev"))) return rc;
+  b200mppi_batch* b = lp->t.b;
+  CU(cudaSetDevice(b->device));
+  launch_loop_stop(lp->la, mask_dev, elem_bytes, b->stream);
+  b->launches++;
+  CHECK_LAUNCH();
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_loop_active(b200mppi_loop* lp, const int32_t** dev) {
+  if (!lp || !dev) return fail(B200MPPI_EINVAL, "loop_active: null argument");
+  *dev = lp->t.pa.active;
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_loop_close(b200mppi_loop* lp, b200mppi_loop_summary* per_planner) {
+  if (!lp) return fail(B200MPPI_EINVAL, "loop_close: null loop");
+  std::unique_ptr<b200mppi_loop> own(lp);
+  TrialCall& t = lp->t;
+  b200mppi_batch* b = t.b;
+  b->loop = nullptr;                                   // closed whatever follows: the batch and planners are free again
+  for (b200mppi_planner* p : b->pl) p->loop = nullptr;
+  CU(cudaSetDevice(b->device));
+  // the box records through the loop's counters and poses, in one copy
+  CU(cudaMemcpyAsync(t.h + t.L.rec, t.d + t.L.rec, t.L.res_end - t.L.rec, cudaMemcpyDeviceToHost, b->stream));
+  CU(cudaStreamSynchronize(b->stream));
+  const LoopState* ls = reinterpret_cast<const LoopState*>(t.h + t.L.loop);
+  std::vector<int> ran(t.K);
+  std::vector<float> x0(3 * (size_t)t.K);
+  for (int i = 0; i < t.K; ++i) {
+    ran[i] = ls[i].solves;
+    for (int c = 0; c < 3; ++c) x0[3 * i + c] = ls[i].x0[c];
+    if (per_planner) {
+      b200mppi_loop_summary& s = per_planner[i];
+      s.solves = ls[i].solves; s.shifts = ls[i].shifts; s.status = ls[i].status;
+      for (int c = 0; c < 3; ++c) s.x[c] = ls[i].x[c];
+    }
+  }
+  trial_commit_planners(t, ran, x0);
+  return B200MPPI_OK;
 }

@@ -604,6 +604,29 @@ struct SeqArgs {
 void launch_plant_step(const PlantArgs& a, cudaStream_t st);
 void launch_plant_step_seq(const PlantArgs& a, const SeqArgs& q, cudaStream_t st);
 
+// device loops of a batch (b200mppi_batch_loop_open): the caller's plant between solves, one launch per call
+// [emu:begin loop_args]
+enum { LOOP_STOPPED = 5 };                // LoopState::status besides TRIAL_RUNNING and TRIAL_LEFT_MAP
+enum { LOOP_POSE_F64 = 0, LOOP_POSE_F32 = 1 };
+struct LoopState {
+  double x[3];                            // the last pose shift_and_update took (a float32 pose widened)
+  double pxlim[2], pylim[2];              // the padded map limits of the planner's solve check
+  float x0[3];                            // the x0 its last solve planned from
+  int solves, shifts, status;
+  int bounded;                            // 1: the padded-limit rule applies (0: barebone, no map)
+  int row;                                // the planner's row in the caller's controls, poses and stop mask
+};
+struct LoopArgs {
+  const TrialDev* dev;                    // per planner: u_cur, x0_out and (stochastic) the window; the rest unused
+  LoopState* state;
+  int* active; int* active_count;
+  int K, T;
+};
+// [emu:end loop_args]
+void launch_loop_export(const LoopArgs& a, float* u_out, cudaStream_t st);
+void launch_loop_ingest(const LoopArgs& a, const void* x, int dtype, long long row_stride, cudaStream_t st);
+void launch_loop_stop(const LoopArgs& a, const void* mask, int elem_bytes, cudaStream_t st);
+
 // visualisation rollouts (mppi.py:1194-1351)
 // [emu:begin vis_args]
 struct VisArgs {

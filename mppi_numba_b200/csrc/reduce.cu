@@ -381,6 +381,25 @@ __device__ __forceinline__ double py_floordiv(double vx, double wx) {
   return copysign(0.0, __ddiv_rn(vx, wx));
 }
 
+// u[:-1] = u[1:] in place by one warp, the last row kept (shift_and_update with num_shifts 1): chunk c reads floats
+// [c+2, c+34) before any lane writes [c, c+32)
+__device__ __forceinline__ void warp_shift_u(float* u, int T, int lane) {
+  const int n = 2 * (T - 1);
+  for (int c = 0; c < n; c += 32) {
+    const int i = c + lane;
+    const float x = i < n ? u[i + 2] : 0.0f;
+    __syncwarp();
+    if (i < n) u[i] = x;
+  }
+}
+
+// The x0 the planner's next rollout starts from, as set_params passes it (float32), and for a windowed (stochastic)
+// rollout the window around it
+__device__ __forceinline__ void set_next_x0(const TrialDev& d, float x, float y, float th) {
+  d.x0_out[0] = x; d.x0_out[1] = y; d.x0_out[2] = th;
+  if (d.win) win_origin(x, y, d.win_pxl, d.win_pyl, d.win_res, d.win_cols, d.win_rows, d.win);
+}
+
 // Recording sequences: whether planner k records at its next step, step `step` of the episode of slot `slot`, and
 // where that record goes (SeqArgs).
 __device__ __forceinline__ void seq_record_next(const SeqArgs& q, int k, int slot, int step) {
@@ -409,14 +428,7 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
   float v = 0.0f, w = 0.0f;
   if (lane == 0) { v = u[0]; w = u[1]; }
   __syncwarp();
-  // u[:-1] = u[1:] in place: chunk c reads floats [c+2, c+34) before any lane writes [c, c+32)
-  const int n = 2 * (a.T - 1);
-  for (int c = 0; c < n; c += 32) {
-    const int i = c + lane;
-    const float x = i < n ? u[i + 2] : 0.0f;
-    __syncwarp();
-    if (i < n) u[i] = x;
-  }
+  warp_shift_u(u, a.T, lane);
   if (lane != 0) return;
   TrialState& s = a.state[k];
   const int t = SEQ ? s.steps : a.step;
@@ -441,8 +453,7 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
   double* xh = a.xhist + ((size_t)slot * (a.max_steps + 1) + t + 1) * 3;
   xh[0] = xn; xh[1] = yn; xh[2] = thn;
   // the next rollout starts from float32(x_next), as set_params would pass it
-  d.x0_out[0] = __double2float_rn(xn); d.x0_out[1] = __double2float_rn(yn); d.x0_out[2] = __double2float_rn(thn);
-  if (d.win) win_origin(d.x0_out[0], d.x0_out[1], d.win_pxl, d.win_pyl, d.win_res, d.win_cols, d.win_rows, d.win);
+  set_next_x0(d, __double2float_rn(xn), __double2float_rn(yn), __double2float_rn(thn));
   const double dx = __dsub_rn(xn, d.xgoal[0]), dy = __dsub_rn(yn, d.xgoal[1]);
   const double dist = __dsub_rn(__dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy))), d.tol);
   s.cum_obj = __dadd_rn(s.cum_obj, __dadd_rn(d.dt, dist));
@@ -477,9 +488,7 @@ __device__ __forceinline__ void plant_step_body(const PlantArgs& a, int k, int l
         s.steps = 0;
         q.episode[k] += 1;
         if (q.reset_x0) {
-          d.x0_out[0] = __double2float_rn(x0[0]); d.x0_out[1] = __double2float_rn(x0[1]);
-          d.x0_out[2] = __double2float_rn(x0[2]);
-          if (d.win) win_origin(d.x0_out[0], d.x0_out[1], d.win_pxl, d.win_pyl, d.win_res, d.win_cols, d.win_rows, d.win);
+          set_next_x0(d, __double2float_rn(x0[0]), __double2float_rn(x0[1]), __double2float_rn(x0[2]));
         }
         seq_record_next(q, k, slot + 1, 0);
         return;
@@ -502,6 +511,99 @@ __global__ void __launch_bounds__(128) plant_step_seq_kernel(const PlantArgs a, 
   plant_step_body<true>(a, (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), (int)(threadIdx.x & 31), q);
 }
 // [emu:end trial]
+
+// ---------------------------------------------------------------------------------------------
+// Device loops (b200mppi_batch_loop_open): the solve's controls out, the caller's pose in, and stops.  A planner whose
+// active flag is 0 is left untouched by all three.
+// [emu:begin loop]
+// One CTA per planner: its u_cur into row `row` of the caller's (K, T, 2) controls, NaN for a planner that no longer
+// runs.  A running planner counts the solve and keeps the x0 it planned from.
+__device__ __forceinline__ void loop_export_body(const LoopArgs& a, float* __restrict__ out, int k) {
+  LoopState& s = a.state[k];
+  const TrialDev& d = a.dev[k];
+  const bool on = a.active[k] != 0;
+  float* o = out + (size_t)s.row * 2 * a.T;
+  for (int j = threadIdx.x; j < 2 * a.T; j += blockDim.x) o[j] = on ? d.u_cur[j] : __int_as_float(0x7fc00000);
+  if (on && threadIdx.x == 0) {
+    s.solves += 1;
+    for (int c = 0; c < 3; ++c) s.x0[c] = d.x0_out[c];
+  }
+}
+
+__global__ void __launch_bounds__(128) loop_export_kernel(const LoopArgs a, float* __restrict__ out) {
+  loop_export_body(a, out, (int)blockIdx.x);
+}
+
+// One warp per planner (warp k of the grid = planner k), as the plant step: shift u_cur by one row, take the pose of row
+// `row` of x (float64, or float32 widened; row_stride bytes apart) and count the shift.  A pose outside the padded map
+// limits (float64 lo <= v <= hi; NaN fails), where the planner's next solve would be refused, stops the planner
+// (TRIAL_LEFT_MAP); otherwise its next rollout plans from float32 of the pose (set_next_x0).
+__device__ __forceinline__ void loop_ingest_body(const LoopArgs& a, const unsigned char* __restrict__ x, int dtype,
+                                                 long long row_stride, int k, int lane) {
+  if (k >= a.K || !a.active[k]) return;
+  const TrialDev& d = a.dev[k];
+  warp_shift_u(d.u_cur, a.T, lane);
+  if (lane != 0) return;
+  LoopState& s = a.state[k];
+  const unsigned char* r = x + (long long)s.row * row_stride;
+  double p[3];
+  float f[3];
+  for (int c = 0; c < 3; ++c) {
+    if (dtype == LOOP_POSE_F32) {
+      f[c] = reinterpret_cast<const float*>(r)[c];
+      p[c] = (double)f[c];
+    } else {
+      p[c] = reinterpret_cast<const double*>(r)[c];
+      f[c] = __double2float_rn(p[c]);
+    }
+    s.x[c] = p[c];
+  }
+  s.shifts += 1;
+  if (s.bounded && !(p[0] >= s.pxlim[0] && p[0] <= s.pxlim[1] && p[1] >= s.pylim[0] && p[1] <= s.pylim[1])) {
+    s.status = TRIAL_LEFT_MAP;
+    a.active[k] = 0;
+    atomicSub(a.active_count, 1);
+    return;
+  }
+  set_next_x0(d, f[0], f[1], f[2]);
+}
+
+__global__ void __launch_bounds__(128) loop_ingest_kernel(const LoopArgs a, const unsigned char* __restrict__ x, int dtype,
+                                                          long long row_stride) {
+  loop_ingest_body(a, x, dtype, row_stride, (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5),
+                   (int)(threadIdx.x & 31));
+}
+
+// One thread per planner: a running planner whose entry of the caller's mask (int32, or one byte: bool / uint8) is
+// nonzero stops for good (LOOP_STOPPED)
+__device__ __forceinline__ void loop_stop_body(const LoopArgs& a, const void* __restrict__ mask, int elem_bytes, int k) {
+  if (k >= a.K || !a.active[k]) return;
+  LoopState& s = a.state[k];
+  const bool stop = elem_bytes == 1 ? reinterpret_cast<const unsigned char*>(mask)[s.row] != 0
+                                    : reinterpret_cast<const int*>(mask)[s.row] != 0;
+  if (!stop) return;
+  s.status = LOOP_STOPPED;
+  a.active[k] = 0;
+  atomicSub(a.active_count, 1);
+}
+
+__global__ void __launch_bounds__(128) loop_stop_kernel(const LoopArgs a, const void* __restrict__ mask, int elem_bytes) {
+  loop_stop_body(a, mask, elem_bytes, (int)(blockIdx.x * blockDim.x + threadIdx.x));
+}
+// [emu:end loop]
+
+void launch_loop_export(const LoopArgs& a, float* u_out, cudaStream_t st) {
+  loop_export_kernel<<<(unsigned)a.K, 128, 0, st>>>(a, u_out);
+}
+
+void launch_loop_ingest(const LoopArgs& a, const void* x, int dtype, long long row_stride, cudaStream_t st) {
+  loop_ingest_kernel<<<(unsigned)((a.K + 3) / 4), 128, 0, st>>>(a, reinterpret_cast<const unsigned char*>(x), dtype,
+                                                                 row_stride);
+}
+
+void launch_loop_stop(const LoopArgs& a, const void* mask, int elem_bytes, cudaStream_t st) {
+  loop_stop_kernel<<<(unsigned)((a.K + 127) / 128), 128, 0, st>>>(a, mask, elem_bytes);
+}
 
 void launch_plant_step(const PlantArgs& a, cudaStream_t st) {
   plant_step_kernel<<<(unsigned)((a.K + 3) / 4), 128, 0, st>>>(a);

@@ -134,6 +134,7 @@ class MPPI_Numba(object):
 
     # ------------------------------------------------------------------ task set-up
     def setup(self, params, lin_tdm, ang_tdm):
+        _lib.refuse_in_loop(self, "MPPI_Numba.setup")
         self.set_tdm(lin_tdm, ang_tdm)
         self.set_params(params)
 
@@ -141,6 +142,7 @@ class MPPI_Numba(object):
         return v >= vbounds[0] and v <= vbounds[1]
 
     def set_params(self, params):
+        _lib.refuse_in_loop(self, "MPPI_Numba.set_params")
         for axis, limits, label in ((0, self.lin_tdm.xlimits, "xlimits"), (1, self.lin_tdm.ylimits, "ylimits")):
             if not self.is_within_bound(params['x0'][axis], limits):
                 print("ERROR: When setting mppi params, x0[{}] is not within {}!".format(axis, label))
@@ -149,6 +151,7 @@ class MPPI_Numba(object):
         self.params_set = True
 
     def set_tdm(self, lin_tdm, ang_tdm):
+        _lib.refuse_in_loop(self, "MPPI_Numba.set_tdm")
         self.lin_tdm, self.ang_tdm = lin_tdm, ang_tdm
         self.tdm_set = True
 
@@ -201,6 +204,7 @@ class MPPI_Numba(object):
     def solve(self):
         """One MPPI solve: sample both TDMs, then num_opt x (noise, rollouts, CVaR, update).
         Returns the optimised control sequence (T, 2) float32, or None if a precondition fails."""
+        _lib.refuse_in_loop(self, "MPPI_Numba.solve")
         if not self.check_solve_conditions():
             print("MPPI solve condition not met. Cannot solve. Return")
             return None
@@ -328,6 +332,7 @@ class MPPI_Numba(object):
 
     # ------------------------------------------------------------------ receding horizon
     def shift_and_update(self, new_x0, u_cur, num_shifts=1):
+        _lib.refuse_in_loop(self, "MPPI_Numba.shift_and_update")
         self.params["x0"] = new_x0.copy()
         self.shift_optimal_control_sequence(u_cur, num_shifts)
 
@@ -343,6 +348,7 @@ class MPPI_Numba(object):
     def get_state_rollout(self):
         """State sequences (V, T+1, 3) of the current optimal controls: over the first V sampled maps
         (use_tdm) or, for the deterministic modes, the optimal sequence plus V-1 noisy samples."""
+        _lib.refuse_in_loop(self, "MPPI_Numba.get_state_rollout")
         assert self.params_set, "MPPI parameters are not set"
         assert self.tdm_set, "MPPI has not received TDMs"
         if not self.device_var_initialized:
@@ -387,6 +393,7 @@ class MPPI_Numba(object):
 
     def get_state(self):
         """Checkpoint: warm-start controls + noise RNG streams (+ both TDM streams if attached)."""
+        _lib.refuse_in_loop(self, "MPPI_Numba.get_state")
         st = dict(u_cur=self.u_cur_d.copy_to_host(), rng=self.rng_states_d.copy_to_host())
         if self.tdm_set:
             st["lin_rng"] = self.lin_tdm.rng_states_d.copy_to_host()
@@ -394,6 +401,7 @@ class MPPI_Numba(object):
         return st
 
     def set_state(self, st):
+        _lib.refuse_in_loop(self, "MPPI_Numba.set_state")
         self.u_cur_d.copy_to_device(st["u_cur"])
         self.rng_states_d.copy_to_device(st["rng"])
         if self.tdm_set and "lin_rng" in st:

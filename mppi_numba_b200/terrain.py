@@ -228,6 +228,7 @@ class TDM_Numba(object):
     def set_TDM_from_PMF_grid(self, pmf_grid, tdm_dict, obstacle_map=None, unknown_map=None):
         """``pmf_grid``: int (num_bins, rows, cols), each column summing to 100.  ``tdm_dict`` keys:
         res, xlimits, ylimits, bin_values, bin_values_bounds, det_dynamics_cvar_alpha."""
+        _lib.refuse_in_loop(self, "TDM_Numba.set_TDM_from_PMF_grid")
         alpha = tdm_dict["det_dynamics_cvar_alpha"]
         if not (0 < alpha <= 1.0):
             print("WARNING: TDM cannot be setup since alpha is not in (0,1]")
@@ -289,6 +290,7 @@ class TDM_Numba(object):
         """Simulation-benchmark entry: ``sg`` holds semantic ids, ``terrain2pmf[terrain]`` is
         ``(values, pmf)`` with pmf summing to 1.  One PMF column per terrain class is computed and
         broadcast over the cells of that class (the reference loops over cells, terrain.py:226-324)."""
+        _lib.refuse_in_loop(self, "TDM_Numba.set_TDM_from_semantic_grid")
         if det_dynamics_cvar_alpha is None:
             assert self.use_tdm or self.use_costmap
         else:
@@ -357,6 +359,7 @@ class TDM_Numba(object):
     def sample_grids(self, alpha_dyn=1.0):
         """Sample M (or 1) traction maps from the PMF on the GPU; returns the persistent device array
         (M|1, Rmax, Cmax) int8.  Bit-exact with the reference's generator layout (terrain.py:633-694)."""
+        _lib.refuse_in_loop(self, "TDM_Numba.sample_grids")
         check(lib.b200mppi_tdm_sample_grids(self._handle, float(alpha_dyn)))
         return self.sample_grid_batch_d
 
