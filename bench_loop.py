@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench_loop.py -- the receding-horizon loop with the caller's plant: the device loop against the host loop.
 
-    python bench_loop.py --workload c2|c3|bb|ref --batch K --closed-loop S [--rounds R]
+    python bench_loop.py --workload c2|c3|bb|ref --batch K --closed-loop S [--rounds R] [--graph-steps G]
 
 A user whose plant is not the built-in one (a simulator, a learned model, a state estimate in GPU memory) drives the
 planners with batch.device_loop(): solve() and shift_and_update(x) on the batch's stream, poses and controls in GPU
@@ -9,15 +9,20 @@ memory.  Here the plant is the benchmark's unicycle on a ground-truth traction g
 nominal unicycle), written in torch on the device.  c2 is one-map (MPPI_Batch), c3 and ref are stochastic
 (MPPI_StochasticBatch; ref is bench_trials.py's reference shape), bb is barebone (bench_trials.py's bb planners).
 
-First the parity check: the device loop with the torch plant on one set of planners; on identical twins the host loop
-replayed with the loop's poses (u = MPPI_*Batch([p]).solve()[0], p.shift_and_update(x[k], u, 1)): u of every solve and
-every planner's final state bit for bit; a mismatch exits non-zero.  Then R rounds of three legs, alternating, every
-round from the same start (params, warm start), S steps each:
+First the parity check, for the device loop and for the graph-replayed loop: the loop with the torch plant on one set
+of planners; on identical twins the host loop replayed with the loop's poses (u = MPPI_*Batch([p]).solve()[0],
+p.shift_and_update(x[k], u, 1)): u of every solve and every planner's final state bit for bit; a mismatch exits
+non-zero.  Then R rounds of four legs, alternating, every round from the same start (params, warm start), S steps each:
   device_loop: S x (loop.solve(), the torch plant, loop.stop(at goal), loop.shift_and_update(x)); no host wait inside;
+  graph:       the device_loop step on a side stream: one eager step, then G steps of it captured into one CUDA graph
+               (torch.cuda.CUDAGraph) and replayed ceil((S - 1) / G) times; the loop's open, capture and close included
+               (each timed round's capture, instantiation included, is also reported on its own);
   host:        S x (batch.solve(), per running planner the numpy plant step and shift_and_update) until all stopped;
   run_trials:  one run_trials(grids, S) (run_stochastic_trials, run_barebone_trials), the built-in plant: the floor.
-Wall clock per round (each ends in a host synchronisation) and kernel launches per round.  Prints one JSON line with
-the card's name, power limit and maximum SM clock; writes nothing to the tree."""
+Planners stop at the goal on the device, so steps after that do nothing in every leg but the host's, which stops
+issuing.  Wall clock per round (each ends in a host synchronisation) and kernel launches per round (issued from the
+host: a replay adds none).  Prints one JSON line with the card's name, power limit and maximum SM clock; writes
+nothing to the tree."""
 import argparse
 import contextlib
 import io
@@ -68,7 +73,10 @@ def main():
     ap.add_argument("--closed-loop", type=int, default=40)
     ap.add_argument("--parity-steps", type=int, default=8)
     ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--graph-steps", type=int, default=1)
     args = ap.parse_args()
+    if args.graph_steps < 1:
+        ap.error("--graph-steps must be >= 1")
     import torch
     import __graft_entry__
     __graft_entry__.build_engine()
@@ -143,14 +151,63 @@ def main():
         torch.cuda.synchronize(dev)
         return loop
 
+    G = args.graph_steps
+    main_stream, side = torch.cuda.current_stream(dev), torch.cuda.Stream(dev)   # a capture needs a stream of its own
+    U = [torch.empty((K, A[0].num_steps, 2), dtype=torch.float32, device=dev) for _ in range(G)]
+    xs = torch.empty((K, 3), **f64)
+    done = [torch.empty(K, dtype=torch.bool, device=dev) for _ in range(G)]
+    xrec = [torch.empty((K, 3), **f64) for _ in range(G)]
+    capture_seconds = []                                   # host time of each capture, instantiation included
+
+    def graph_round(steps, record=None):
+        """The device_loop leg's step with static tensors: one eager step, then G of them captured and replayed."""
+        reset(A)
+        ba.set_stream(side.cuda_stream)
+        with torch.cuda.stream(side):
+            xs.copy_(torch.tensor(np.stack([np.asarray(p.params["x0"], np.float64)[:3] for p in A]), **f64))
+
+            def step(loop, j):
+                loop.solve(out=U[j])
+                xn, d = torch_plant(torch, xs, U[j][:, 0], dt, tg, xlo, ylo, gres, goal, tol)
+                xs.copy_(xn)
+                done[j].copy_(d)
+                loop.stop(done[j])
+                loop.shift_and_update(xs)
+                if record is not None:
+                    xrec[j].copy_(xs)
+
+            def keep(n):
+                for j in range(n):
+                    record.append(("solve", U[j].cpu().numpy().copy()))
+                    record.append(("stop", done[j].cpu().numpy()))
+                    record.append(("shift", xrec[j].cpu().numpy()))
+
+            with ba.device_loop() as loop:
+                step(loop, 0)
+                if record is not None:
+                    keep(1)
+                g = torch.cuda.CUDAGraph()
+                t0 = time.perf_counter()
+                g.capture_begin()
+                for j in range(G):
+                    step(loop, j)
+                g.capture_end()
+                capture_seconds.append(time.perf_counter() - t0)
+                for _ in range(-(-(steps - 1) // G)):
+                    g.replay()
+                    if record is not None:
+                        keep(G)
+        torch.cuda.synchronize(dev)
+        ba.set_stream(main_stream.cuda_stream)
+        return loop
+
     ba, bh = Batch(A), Batch(Bs)
     for b in (ba, bh):                                     # the torch plant, the loop and torch's reads on one stream
-        b.set_stream(torch.cuda.current_stream(dev).cuda_stream)
+        b.set_stream(main_stream.cuda_stream)
 
-    # ---- parity: the device loop == the host loop replayed with the loop's poses on identical twins
-    calls = []
-    with contextlib.redirect_stdout(io.StringIO()):
-        loop = loop_round(args.parity_steps, calls)
+    # ---- parity: the device loop (then the graph-replayed loop) == the host loop replayed with the loop's poses on
+    # identical twins
+    def replayed_on_twins(calls):
         reset(Bs)
         ok_u = True
         for k, p in enumerate(Bs):
@@ -167,6 +224,7 @@ def main():
                 elif what == "shift" and running:
                     p.shift_and_update(v[k].copy(), p.u_cur_d.copy_to_host(), 1)
                     running = bb or within(p, v[k])
+        return ok_u
 
     def state(p):
         d = [p.u_cur_d, p.u_prev_d, p.costs_d, p.weights_d, p.noise_samples_d, p.rng_states_d]
@@ -176,10 +234,18 @@ def main():
         if stochastic:
             d.append(p.costs_nm_d)
         return [a.copy_to_host() for a in d] + [np.asarray(p.params["x0"], np.float64)]
-    ok_state = all(all(np.array_equal(x, y) for x, y in zip(state(a), state(b))) for a, b in zip(A, Bs))
-    parity = {"passed": bool(ok_u and ok_state), "u_bitwise": bool(ok_u), "state_bitwise": bool(ok_state),
-              "planners": K, "steps": args.parity_steps, "solves": loop.solves.tolist(), "status": loop.status,
-              "against": "the host loop replayed with the device loop's poses on identical twins"}
+
+    parity = {"planners": K, "steps": args.parity_steps,
+              "against": "the host loop replayed with the loop's poses on identical twins"}
+    for name, fn in (("device_loop", loop_round), ("graph", graph_round)):
+        calls = []
+        with contextlib.redirect_stdout(io.StringIO()):
+            loop = fn(args.parity_steps, calls)
+            ok_u = replayed_on_twins(calls)
+        ok_state = all(all(np.array_equal(x, y) for x, y in zip(state(a), state(b))) for a, b in zip(A, Bs))
+        parity[name] = {"passed": bool(ok_u and ok_state), "u_bitwise": bool(ok_u), "state_bitwise": bool(ok_state),
+                        "solves": loop.solves.tolist(), "status": loop.status}
+    parity["passed"] = parity["device_loop"]["passed"] and parity["graph"]["passed"]
     if not parity["passed"]:
         sys.stderr.write("bench_loop.py: PARITY CHECK FAILED: %s\n" % json.dumps(parity))
         print(json.dumps({"metric": "device loop", "error": "parity_check failed", "parity_check": parity}))
@@ -215,12 +281,14 @@ def main():
         trials(ba)
         torch.cuda.synchronize(dev)
 
-    legs = [("device_loop", lambda: loop_round(S), ba), ("host", host_round, bh), ("run_trials", trials_round, ba)]
+    legs = [("device_loop", lambda: loop_round(S), ba), ("graph", lambda: graph_round(S), ba), ("host", host_round, bh),
+            ("run_trials", trials_round, ba)]
     times = {name: [] for name, _, _ in legs}
     launches = {}
     with contextlib.redirect_stdout(io.StringIO()):
         for _, fn, _ in legs:                              # warm-up
             fn()
+        del capture_seconds[:]
         for _ in range(args.rounds):
             for name, fn, b in legs:
                 n0 = b.launch_count()
@@ -232,12 +300,17 @@ def main():
     out = {"metric": "device loop: caller's torch plant vs host loop vs run_trials",
            "config": {"workload": args.workload, "batch": K, "steps": S, "rounds": args.rounds,
                       "plant": "unicycle on a float64 traction grid in torch" if not bb else "nominal unicycle in torch",
-                      "device_loop": "S solves, plant, stop at goal, shift: no host poll, all S steps issued"},
+                      "device_loop": "S solves, plant, stop at goal, shift: no host poll, all S steps issued",
+                      "graph_steps": G,
+                      "graph": "one eager step, G steps captured, ceil((S - 1) / G) replays; open, capture, close "
+                               "included"},
            "gpu": gpu_info(dev), "parity_check": parity,
            "round_seconds": {name: [round(t, 4) for t in v] for name, v in times.items()},
            "median_seconds": {name: round(t, 4) for name, t in med.items()},
            "host_over_device_loop": round(med["host"] / med["device_loop"], 3),
            "device_loop_over_run_trials": round(med["device_loop"] / med["run_trials"], 3),
+           "device_loop_over_graph": round(med["device_loop"] / med["graph"], 3),
+           "graph_capture_seconds": [round(t, 4) for t in capture_seconds],
            "launches_per_round": launches}
     print(json.dumps(out))
 

@@ -647,6 +647,11 @@ int b200mppi_batch_run_mixed_trials(b200mppi_batch* b, const b200mppi_trial_desc
  * The calls may come in any order (two solves, two shifts, a close right after a solve).  One planner: a batch of one.
  * A loop issues what the trial of its kind issues, without the plant step: a solve issues one trial step's launches
  * (num_opt x the solve stages, the sampler classes) and one export; a shift and a stop one launch each.
+ * CUDA graphs: the loop counts its solves on the device (the export that ends a solve prepares the next one's sampler
+ * parity and reach slots), so no launch depends on how many solves came before.  Solve, shift_and_update and stop may
+ * be captured (cudaStreamCaptureModeGlobal included) on the batch's stream and replayed any number of times, mixed
+ * with eager calls: each replay is those calls at that point of the loop, bit for bit, reading the arrays captured.
+ * Launches count where they are issued from the host: a capture counts once, a replay adds nothing.
  *
  * b200mppi_batch_loop_open: kind as in b200mppi_batch_run_trials_recorded (the batch's own kind).  padded_limits: float64
  * (count, 4) = padded x lo, x hi, y lo, y hi of each planner's map (the limits of the host's solve check; NULL for
@@ -669,11 +674,16 @@ int b200mppi_batch_run_mixed_trials(b200mppi_batch* b, const b200mppi_trial_desc
  *   whose entry is nonzero stops for good (B200MPPI_LOOP_STOPPED).  A stopped planner never runs again, so every running
  *   planner has solved equally often and one sampler parity serves them all.
  * b200mppi_loop_wait_stream: the batch's stream waits (an event, not the host) for the work issued so far on stream.
+ *   While the batch's stream captures a graph, B200MPPI_EINVAL unless stream is part of the same capture (an event
+ *   recorded outside it would invalidate the capture).
  * b200mppi_loop_active: the device's int32 (count) running flags, in the batch's order.
  * b200mppi_loop_close: waits for the stream, commits and frees the loop (also on an error).  Every planner and TDM pair is
  *   left as after the host loop: the reach slots, sample boxes and the samplings of shared pairs follow each planner's
  *   solves (a pair's group: its longest-running member), and the C-side params keep the x0 of the last solve.
- *   per_planner (may be NULL): count summaries in the batch's order. */
+ *   per_planner (may be NULL): count summaries in the batch's order.
+ *   While the batch's stream captures a graph: B200MPPI_EINVAL before any work, the loop left open and usable (close
+ *   waits for the stream).  More than 2^31 - 1 solves issued: B200MPPI_ESTATE, the loop freed and the planners' counts
+ *   not committed.  Any other error: the loop is freed. */
 typedef struct b200mppi_loop b200mppi_loop;
 enum { B200MPPI_POSE_F64 = 0, B200MPPI_POSE_F32 = 1 };
 enum { B200MPPI_LOOP_RUNNING = 0, B200MPPI_LOOP_STOPPED = 5 };   /* and B200MPPI_TRIAL_LEFT_MAP */

@@ -67,6 +67,7 @@ class LoopSummary(C.Structure):
 
 POSE_F64, POSE_F32 = 0, 1
 LOOP_RUNNING, LOOP_STOPPED = 0, 5
+EINVAL = -1
 
 
 def refuse_in_loop(obj, name):

@@ -44,6 +44,7 @@ batch of its own kind would leave it (include/b200mppi.h, mixed batches).
 batch's stream with no host wait (include/b200mppi.h, device loops).
 """
 import ctypes as C
+import sys
 
 import numpy as np
 
@@ -775,7 +776,34 @@ class DeviceLoop(object):
     planner: afterwards each is exactly as after that host loop, ``params['x0']`` the float64 value of the last pose it
     took (a float32 pose widened exactly), and ``solves``, ``shifts`` (K,) int and ``status`` (K,) of "running" |
     "left_map" | "stopped" are set.  Launches: a solve issues what a trial step of the batch issues without its plant
-    step, plus one export; ``shift_and_update`` and ``stop`` one each."""
+    step, plus one export; ``shift_and_update`` and ``stop`` one each.
+
+    CUDA graphs.  Nothing a loop call passes to the GPU changes from one call to the next (the loop counts its solves on
+    the device), so a whole step, the caller's plant included, can be captured once and replayed:
+
+        s = torch.cuda.Stream()
+        batch.set_stream(s.cuda_stream)                               # before the loop opens
+        u = torch.empty((K, T, 2), dtype=torch.float32, device="cuda")   # static tensors: out, pose, done
+        with batch.device_loop() as loop:
+            def step():
+                loop.solve(out=u)
+                x.copy_(my_plant(x, u[:, 0]))
+                loop.stop(done_of(x, done))                           # optional: a device-computed stop
+                loop.shift_and_update(x)
+            with torch.cuda.stream(s):
+                step()                                                # warm-up: the loop's first step, eager
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=s):
+                step()                                                # captured, not run
+            for t in range(steps - 1):
+                g.replay()                                            # stopped planners do nothing
+
+    Replays, eager calls and more captures mix freely on one loop: each replay is the captured calls at that point of
+    the loop, bit for bit.  A replay reads the arrays captured (their pointers, dtype and row stride are fixed at
+    capture), so refill them in place.  ``batch.launch_count()`` counts the launches issued from the host: captured
+    calls count once, replays add nothing.  While the batch's stream captures, ``close()`` raises and the loop stays
+    open, and a call while torch captures on a stream other than the loop's raises ValueError before anything is
+    enqueued (its launches would run at once, outside the caller's graph)."""
 
     def __init__(self, batch):
         name = "%s.device_loop" % type(batch).__name__
@@ -839,6 +867,17 @@ class DeviceLoop(object):
     def _live(self, fn):
         if self._handle is None:
             raise ValueError("DeviceLoop.%s: the loop is closed" % fn)
+        self._refuse_foreign_capture(fn)
+
+    def _refuse_foreign_capture(self, fn):
+        """ValueError while torch (if imported) captures a CUDA graph on a stream other than the loop's."""
+        torch = sys.modules.get("torch")
+        if torch is None or not torch.cuda.is_initialized() or not torch.cuda.is_current_stream_capturing():
+            return
+        cur = int(torch.cuda.current_stream().cuda_stream)
+        if cur != self.stream:
+            raise ValueError("DeviceLoop.%s: torch is capturing a CUDA graph on stream 0x%x, the loop runs on 0x%x "
+                             "(batch.set_stream() to the capturing stream before the loop opens)" % (fn, cur, self.stream))
 
     def _array(self, obj, fn, what, shape, typestrs, strided_rows=False):
         """Pointer, typestr and row stride of ``obj``'s __cuda_array_interface__ (v3) after checking its shape, dtype,
@@ -903,14 +942,20 @@ class DeviceLoop(object):
         check(lib.b200mppi_loop_stop(self._handle, p, 4 if typestr == "<i4" else 1))
 
     def close(self):
-        """Wait for the stream, commit every planner (as after the host loop) and free the loop.  Idempotent."""
-        h, self._handle = getattr(self, "_handle", None), None
+        """Wait for the stream, commit every planner (as after the host loop) and free the loop.  Idempotent.  Raises,
+        with the loop left open, while the batch's stream captures a CUDA graph."""
+        h = getattr(self, "_handle", None)
         if h is None:
             return
+        self._refuse_foreign_capture("close")
         b = self.batch
         S = (_lib.LoopSummary * self.K)()
+        rc = lib.b200mppi_loop_close(h, S)
+        if rc == _lib.EINVAL:                          # refused before any work: the loop stays open
+            check(rc)
+        self._handle = None
         try:
-            check(lib.b200mppi_loop_close(h, S))
+            check(rc)
         finally:
             b._loop = None
             for p in b.planners:

@@ -2905,6 +2905,7 @@ struct TrialPart {
   // in the call's device buffer: the sampler sets of each parity, class c's pairs cls_d + lc.first[c], and the group
   // descriptors and members (null: no shared pair)
   const SampleGridsV2Args* set_d[2] = {};
+  const SampleGridsV2Args* set_cur_d = nullptr;        // a loop's current set (LoopArgs::set_cur), read at every solve
   const int* cls_d = nullptr;
   const SampleGroupDesc* grp_d = nullptr;
   const int* mem_d = nullptr;
@@ -3004,10 +3005,11 @@ static void onemap_trial_classes(TrialPart& q) {
 
 // Byte offsets into a trial call's one device allocation, in the order trial_layout takes them
 struct TrialLayout {
-  struct Part { size_t set[2] = {}, grp = 0, mem = 0, cls = 0; };   // a kind's sampler sets (by parity), group
-  Part part[2];                                                     // descriptors, members and class lists
-  size_t box = 0, rec = 0, grec = 0, state = 0, con = 0, res = 0, loop = 0, res_end = 0, tr = 0, act = 0, seq = 0,
-         start = 0;
+  struct Part { size_t set[2] = {}, grp = 0, mem = 0, cls = 0, cur = 0; };   // a kind's sampler sets (by parity),
+  Part part[2];                                                     // group descriptors, members, class lists and
+                                                                    // (loop) current set
+  size_t box = 0, rec = 0, grec = 0, state = 0, con = 0, res = 0, loop = 0, clock = 0, res_end = 0, tr = 0, act = 0,
+         seq = 0, start = 0, slot0 = 0;
   size_t vis = 0, rflag = 0, head = 0;                 // head: the sections staged and uploaded with one copy
   std::vector<size_t> grid;                            // per slot
   size_t vrec = 0, xh = 0, uh = 0, lu = 0, total = 0;
@@ -3176,6 +3178,7 @@ static TrialLayout trial_layout(const TrialCall& t) {
   L.con = s.take((t.barebone ? nslot : 0) * sizeof(int));   // barebone contacts, per slot
   L.res = s.take(nres * sizeof(TrialState));
   L.loop = s.take((t.loop ? K : 0) * sizeof(LoopState));   // a loop's per-planner counters and poses
+  L.clock = s.take((t.loop ? 2 : 0) * sizeof(int));   // a loop's solve clock (LoopClock)
   L.res_end = s.end;
   L.tr = s.take(nslot * sizeof(TrialDev));
   L.act = s.take((K + 1) * sizeof(int));               // active (K), the count of running planners
@@ -3183,6 +3186,9 @@ static TrialLayout trial_layout(const TrialCall& t) {
   L.start = s.take(nres * 3 * sizeof(double));
   L.vis = s.take((t.record ? K : 0) * sizeof(VisBatchDesc));
   L.rflag = s.take((t.rec_seq ? K : 0) * sizeof(int));
+  om.cur = s.take((t.loop ? P[0].G : 0) * szs);        // a loop's current sampler sets and staged reach slots
+  sto.cur = s.take((t.loop ? P[1].G : 0) * szs);
+  L.slot0 = s.take((t.loop ? 2 * K2 : 0) * sizeof(int));
   L.head = s.end;
   // The pinned staging holds the head and the histories only.  The float64 ground-truth grids (tens of MB for a batch
   // of large maps) are copied straight from the caller's arrays, and a slot whose grids are planes of a realisation set
@@ -3329,11 +3335,21 @@ static int trial_call_stage(TrialCall& t) {
     std::copy(q.lc.groups.begin(), q.lc.groups.end(), reinterpret_cast<int*>(h + o.cls));
     q.set_d[0] = reinterpret_cast<const SampleGridsV2Args*>(d + o.set[0]);
     q.set_d[1] = reinterpret_cast<const SampleGridsV2Args*>(d + o.set[1]);
+    if (t.loop) {                                      // the current set of solve 0: parity 0
+      std::copy(hs0, hs0 + q.G, reinterpret_cast<SampleGridsV2Args*>(h + o.cur));
+      q.set_cur_d = reinterpret_cast<const SampleGridsV2Args*>(d + o.cur);
+    }
     q.cls_d = reinterpret_cast<const int*>(d + o.cls);
     q.grp_d = q.grouped ? reinterpret_cast<const SampleGroupDesc*>(d + o.grp) : nullptr;
     q.mem_d = q.grouped ? reinterpret_cast<const int*>(d + o.mem) : nullptr;
   }
   hact[K] = K;
+  if (t.loop) {                                        // the clock at 0, and the staged slots the clock rewrites from
+    std::fill_n(reinterpret_cast<int*>(h + L.clock), 2, 0);
+    int* slot0 = reinterpret_cast<int*>(h + L.slot0);
+    const NoisePrepDesc* hn = reinterpret_cast<const NoisePrepDesc*>(h + b->off_nprep);
+    for (int r = 0; r < t.K2; ++r) { slot0[r] = hn[r].slot; slot0[t.K2 + r] = hb[r].slot; }
+  }
   if (t.K2 > 0) t.g0 = *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win);
   cudaStream_t st = b->stream;
   CU(cudaMemcpyAsync(d, h, L.head, cudaMemcpyHostToDevice, st));
@@ -3363,13 +3379,17 @@ static int trial_call_step(TrialCall& t, int s) {
   const int* dact2 = dact + K1;                        // the stochastic launches' active flags
   const RolloutWinArgs* dw = reinterpret_cast<const RolloutWinArgs*>(d + b->off_win);
   const SampleBoxDesc* db = reinterpret_cast<const SampleBoxDesc*>(d + t.L.box);
+  // a loop's solves read the current sets and slots its solve clock prepares (LoopClock): nothing of solve s is
+  // passed by value, so a captured solve replays as any later one
+  const SampleGridsV2Args* om_set = t.loop ? om.set_cur_d : om.set_d[s & 1];
+  const SampleGridsV2Args* sto_set = t.loop ? sto.set_cur_d : sto.set_d[s & 1];
   for (int k = 0; k < num_opt; ++k) {
     if (K1 > 0) {
       launch_sample_noise_batch(reinterpret_cast<const NoiseDesc*>(d), K1, N, T, dact, st);
       b->launches++;
       CHECK_LAUNCH();
       for (int c = 0; c < om.C && k == 0; ++c) {
-        launch_sample_grids_v2_batch(om.cls[c].L, om.set_d[s & 1], om.lc.count(c), om.cls_d + om.lc.first[c], dact, st,
+        launch_sample_grids_v2_batch(om.cls[c].L, om_set, om.lc.count(c), om.cls_d + om.lc.first[c], dact, st,
                                      om.grp_d, om.mem_d);
         b->launches++;
         CHECK_LAUNCH();
@@ -3379,7 +3399,7 @@ static int trial_call_step(TrialCall& t, int s) {
       CHECK_LAUNCH();
     }
     if (K2 > 0) {
-      const int iter = s * num_opt + k;               // every planner's reach slot toggles once per iteration
+      const int iter = (t.loop ? 0 : s * num_opt) + k;   // every planner's reach slot toggles once per iteration
       launch_noise_prepare_batch(reinterpret_cast<const NoisePrepDesc*>(d + b->off_nprep), K2, N, T, b->pl[0]->npad,
                                  iter, dact2, st);
       b->launches++;
@@ -3388,11 +3408,11 @@ static int trial_call_step(TrialCall& t, int s) {
         const TrialClass& tc = sto.cls[c];
         const SampleGridsV2Args& g0c = sto.set0[sto.lc.groups[sto.lc.first[c]]];
         const int* cls = sto.cls_d + sto.lc.first[c];
-        launch_sample_grids_v2_box_batch(tc.L, sto.set_d[s & 1], db, sto.lc.count(c), cls, dact2, iter, tc.mrows,
+        launch_sample_grids_v2_box_batch(tc.L, sto_set, db, sto.lc.count(c), cls, dact2, iter, tc.mrows,
                                          tc.ncact, st, sto.grp_d, sto.mem_d);
         b->launches++;
         CHECK_LAUNCH();
-        launch_advance_states_batch(sto.set_d[s & 1], db, sto.lc.count(c), cls, g0c.tx, g0c.ty, g0c.num_maps, dact2, st,
+        launch_advance_states_batch(sto_set, db, sto.lc.count(c), cls, g0c.tx, g0c.ty, g0c.num_maps, dact2, st,
                                     sto.grp_d, sto.mem_d);
         b->launches++;
         CHECK_LAUNCH();
@@ -3709,11 +3729,14 @@ extern "C" int b200mppi_batch_run_trial_sequences_ex(b200mppi_batch* b, int32_t 
 // A trial call without its plant step, driven one call at a time: the phases of batch_run_trials (validation, plans,
 // layout, staging, step and the planner and TDM commit) over one device buffer that lives while the loop is open.  The
 // caller's plant runs between the calls on the batch's stream; the loop kernels (reduce.cu) take its poses and stops.
+// The loop's solve clock lives on the device (LoopClock) and no call passes anything that changes from one call
+// to the next, so the calls may be captured into a CUDA graph and replayed, mixed freely with eager calls.  Every call
+// a loop call makes while the batch's stream captures is legal under cudaStreamCaptureModeGlobal; close refuses.
 struct b200mppi_loop {
   TrialCall t{};
   LoopArgs la{};
+  LoopClock lc{};
   cudaEvent_t ev = nullptr;            // orders the batch's stream after work on the stream of a caller's array
-  int solves = 0;                      // solves issued: every running planner has solved exactly this many times
   ~b200mppi_loop() {
     cudaFree(t.d);
     if (t.h) cudaFreeHost(t.h);
@@ -3761,6 +3784,19 @@ extern "C" int b200mppi_batch_loop_open(b200mppi_batch* b, int32_t kind, const d
   CU(cudaEventCreateWithFlags(&lp->ev, cudaEventDisableTiming));
   lp->la = LoopArgs{reinterpret_cast<const TrialDev*>(t.d + t.L.tr), reinterpret_cast<LoopState*>(t.d + t.L.loop),
                     t.pa.active, t.pa.active_count, t.K, b->T};
+  LoopClock& lc = lp->lc;
+  lc.clock = reinterpret_cast<int*>(t.d + t.L.clock);
+  for (int k = 0; k < 2; ++k) {
+    lc.set_cur[k] = reinterpret_cast<SampleGridsV2Args*>(t.d + t.L.part[k].cur);
+    lc.set_par[k][0] = t.P[k].set_d[0];
+    lc.set_par[k][1] = t.P[k].set_d[1];
+    lc.G[k] = t.P[k].G;
+  }
+  lc.nprep = reinterpret_cast<NoisePrepDesc*>(t.d + b->off_nprep);
+  lc.box = reinterpret_cast<SampleBoxDesc*>(t.d + t.L.box);
+  lc.slot0 = reinterpret_cast<const int*>(t.d + t.L.slot0);
+  lc.K2 = t.K2;
+  lc.num_opt = b->pl[0]->prm.num_opt;
   b->loop = lp.get();
   for (b200mppi_planner* p : b->pl) p->loop = lp.get();
   *out = lp.release();
@@ -3774,11 +3810,29 @@ extern "C" int b200mppi_loop_controls(b200mppi_loop* lp, float** u_dev, void** s
   return B200MPPI_OK;
 }
 
+// The capture sequence id of stream s (0: s is not capturing)
+static int capture_id(cudaStream_t s, unsigned long long* id) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  *id = 0;
+  CU(cudaStreamGetCaptureInfo(s, &cs, id));
+  if (cs != cudaStreamCaptureStatusActive) *id = 0;
+  return B200MPPI_OK;
+}
+
 extern "C" int b200mppi_loop_wait_stream(b200mppi_loop* lp, void* stream) {
   if (!lp) return fail(B200MPPI_EINVAL, "loop_wait_stream: null loop");
   cudaStream_t s = (cudaStream_t)stream, st = lp->t.b->stream;
   if (s == st) return B200MPPI_OK;
   CU(cudaSetDevice(lp->t.b->device));
+  // while the batch's stream captures, an event recorded on a stream outside that capture would invalidate it (the
+  // legacy default stream is never part of one, and is not even queried then)
+  unsigned long long id_st = 0, id_s = 0;
+  int rc;
+  if ((rc = capture_id(st, &id_st))) return rc;
+  if (id_st && s != nullptr && s != cudaStreamLegacy && (rc = capture_id(s, &id_s))) return rc;
+  if (id_st && id_s != id_st)
+    return fail(B200MPPI_EINVAL, "loop_wait_stream: the batch's stream is capturing a CUDA graph and the stream is not "
+                                 "part of that capture");
   CU(cudaEventRecord(lp->ev, s));
   CU(cudaStreamWaitEvent(st, lp->ev, 0));
   return B200MPPI_OK;
@@ -3790,12 +3844,10 @@ extern "C" int b200mppi_loop_solve(b200mppi_loop* lp, float* u_dev) {
   if ((rc = loop_device_ptr(lp, u_dev, "loop_solve", "u_dev"))) return rc;
   b200mppi_batch* b = lp->t.b;
   CU(cudaSetDevice(b->device));
-  if (lp->solves == INT32_MAX) return fail(B200MPPI_EINVAL, "loop_solve: 2^31 - 1 solves issued");
-  if ((rc = trial_call_step(lp->t, lp->solves))) return rc;
-  launch_loop_export(lp->la, u_dev, b->stream);
+  if ((rc = trial_call_step(lp->t, 0))) return rc;   // s unused: the loop's solves read what its clock prepared
+  launch_loop_export(lp->la, lp->lc, u_dev, b->stream);
   b->launches++;
   CHECK_LAUNCH();
-  lp->solves++;
   return B200MPPI_OK;
 }
 
@@ -3842,15 +3894,24 @@ extern "C" int b200mppi_loop_active(b200mppi_loop* lp, const int32_t** dev) {
 
 extern "C" int b200mppi_loop_close(b200mppi_loop* lp, b200mppi_loop_summary* per_planner) {
   if (!lp) return fail(B200MPPI_EINVAL, "loop_close: null loop");
-  std::unique_ptr<b200mppi_loop> own(lp);
   TrialCall& t = lp->t;
   b200mppi_batch* b = t.b;
+  // close waits for the stream, which a capture forbids: refused with the loop left open and usable
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(b->stream, &cs) == cudaSuccess && cs != cudaStreamCaptureStatusNone)
+    return fail(B200MPPI_EINVAL, "loop_close: the batch's stream is capturing a CUDA graph (close the loop after the "
+                                 "capture ends)");
+  std::unique_ptr<b200mppi_loop> own(lp);
   b->loop = nullptr;                                   // closed whatever follows: the batch and planners are free again
   for (b200mppi_planner* p : b->pl) p->loop = nullptr;
   CU(cudaSetDevice(b->device));
-  // the box records through the loop's counters and poses, in one copy
+  // the box records through the loop's counters, poses and solve clock, in one copy
   CU(cudaMemcpyAsync(t.h + t.L.rec, t.d + t.L.rec, t.L.res_end - t.L.rec, cudaMemcpyDeviceToHost, b->stream));
   CU(cudaStreamSynchronize(b->stream));
+  if (reinterpret_cast<const int*>(t.h + t.L.clock)[1]) {
+    for (b200mppi_planner* p : b->pl) { p->prepared = false; p->pushed_direct = false; }
+    return fail(B200MPPI_ESTATE, "loop_close: more than 2^31 - 1 solves issued; the planners' counts are not committed");
+  }
   const LoopState* ls = reinterpret_cast<const LoopState*>(t.h + t.L.loop);
   std::vector<int> ran(t.K);
   std::vector<float> x0(3 * (size_t)t.K);

@@ -623,7 +623,22 @@ struct LoopArgs {
   int K, T;
 };
 // [emu:end loop_args]
-void launch_loop_export(const LoopArgs& a, float* u_out, cudaStream_t st);
+// [emu:begin loop_clock_args]
+// A loop's solve clock (clock null: none, and nothing else is read): clock[0] counts the solves issued to the loop,
+// clock[1] is set once a solve was issued past 2^31 - 1.  The export launch that ends solve s prepares solve s + 1
+// (loop_clock_body), so no launch of a loop solve takes anything from the host that changes between solves.
+struct LoopClock {
+  int* clock;
+  SampleGridsV2Args* set_cur[2];          // per kind (one-map, stochastic): the sampler set of the next solve
+  const SampleGridsV2Args* set_par[2][2]; // per kind: the staged sets of parity 0 and 1, G[kind] each
+  int G[2];
+  NoisePrepDesc* nprep;                   // the stochastic planners' descriptors whose slot the next solve reads
+  SampleBoxDesc* box;
+  const int* slot0;                       // their staged slots: nprep's (K2), then box's (K2)
+  int K2, num_opt;
+};
+// [emu:end loop_clock_args]
+void launch_loop_export(const LoopArgs& a, const LoopClock& c, float* u_out, cudaStream_t st);
 void launch_loop_ingest(const LoopArgs& a, const void* x, int dtype, long long row_stride, cudaStream_t st);
 void launch_loop_stop(const LoopArgs& a, const void* mask, int elem_bytes, cudaStream_t st);
 

@@ -530,10 +530,6 @@ __device__ __forceinline__ void loop_export_body(const LoopArgs& a, float* __res
   }
 }
 
-__global__ void __launch_bounds__(128) loop_export_kernel(const LoopArgs a, float* __restrict__ out) {
-  loop_export_body(a, out, (int)blockIdx.x);
-}
-
 // One warp per planner (warp k of the grid = planner k), as the plant step: shift u_cur by one row, take the pose of row
 // `row` of x (float64, or float32 widened; row_stride bytes apart) and count the shift.  A pose outside the padded map
 // limits (float64 lo <= v <= hi; NaN fails), where the planner's next solve would be refused, stops the planner
@@ -592,8 +588,47 @@ __global__ void __launch_bounds__(128) loop_stop_kernel(const LoopArgs a, const 
 }
 // [emu:end loop]
 
-void launch_loop_export(const LoopArgs& a, float* u_out, cudaStream_t st) {
-  loop_export_kernel<<<(unsigned)a.K, 128, 0, st>>>(a, u_out);
+// [emu:begin loop_clock]
+// The solve clock (LoopClock), run by one CTA of the export launch that ends solve s = clock[0]: it prepares
+// solve s + 1.  Only two inputs of a loop solve change from one solve to the next, and both move here:
+//   - each kind's sampler set: the staged set of parity (s + 1) & 1 is copied into the current set, which the solve's
+//     sampler launches read (every running planner has sampled its pair exactly s + 1 times before that solve);
+//   - the reach slot of every stochastic planner's noise and box descriptor becomes the slot of the solve's first
+//     iteration, staged slot ^ (((s + 1) * num_opt) & 1): iteration k then reads slot ^ (k & 1), the slot the by-value
+//     iteration index (s + 1) * num_opt + k selects.
+// The clock advances last, after the CTA's barrier.  At 2^31 - 1 solves it stops and sets clock[1] instead of wrapping.
+__device__ __forceinline__ void loop_clock_body(const LoopClock& a) {
+  if (!a.clock) return;
+  const int s = a.clock[0];
+  const unsigned next = (unsigned)s + 1u;
+  static_assert(sizeof(SampleGridsV2Args) % sizeof(unsigned long long) == 0, "sampler sets copied in 8-byte words");
+  constexpr int words = (int)(sizeof(SampleGridsV2Args) / sizeof(unsigned long long));
+  for (int k = 0; k < 2; ++k) {
+    const unsigned long long* src = reinterpret_cast<const unsigned long long*>(a.set_par[k][next & 1u]);
+    unsigned long long* dst = reinterpret_cast<unsigned long long*>(a.set_cur[k]);
+    for (int j = threadIdx.x; j < a.G[k] * words; j += blockDim.x) dst[j] = src[j];
+  }
+  const int flip = (int)((next * (unsigned)a.num_opt) & 1u);
+  for (int r = threadIdx.x; r < a.K2; r += blockDim.x) {
+    a.nprep[r].slot = a.slot0[r] ^ flip;
+    a.box[r].slot = a.slot0[a.K2 + r] ^ flip;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (s == 0x7fffffff) a.clock[1] = 1;
+    else a.clock[0] = s + 1;
+  }
+}
+// [emu:end loop_clock]
+
+// the export of a loop solve, and (CTA 0) the preparation of the next
+__global__ void __launch_bounds__(128) loop_export_kernel(const LoopArgs a, float* __restrict__ out, const LoopClock c) {
+  loop_export_body(a, out, (int)blockIdx.x);
+  if (blockIdx.x == 0) loop_clock_body(c);
+}
+
+void launch_loop_export(const LoopArgs& a, const LoopClock& c, float* u_out, cudaStream_t st) {
+  loop_export_kernel<<<(unsigned)a.K, 128, 0, st>>>(a, u_out, c);
 }
 
 void launch_loop_ingest(const LoopArgs& a, const void* x, int dtype, long long row_stride, cudaStream_t st) {
