@@ -2,6 +2,7 @@
 """bench_loop.py -- the receding-horizon loop with the caller's plant: the device loop against the host loop.
 
     python bench_loop.py --workload c2|c3|bb|ref --batch K --closed-loop S [--rounds R] [--graph-steps G]
+    python bench_loop.py --workload swarm --batch K --closed-loop S [--rounds R] [--graph-steps G] [--profile]
 
 A user whose plant is not the built-in one (a simulator, a learned model, a state estimate in GPU memory) drives the
 planners with batch.device_loop(): solve() and shift_and_update(x) on the batch's stream, poses and controls in GPU
@@ -22,7 +23,19 @@ non-zero.  Then R rounds of four legs, alternating, every round from the same st
 Planners stop at the goal on the device, so steps after that do nothing in every leg but the host's, which stops
 issuing.  Wall clock per round (each ends in a host synchronisation) and kernel launches per round (issued from the
 host: a replay adds none).  Prints one JSON line with the card's name, power limit and maximum SM clock; writes
-nothing to the tree."""
+nothing to the tree.
+
+swarm: K barebone robots of the notebook's shape (N 1000, T 50, dt 0.1, its two obstacles) in one arena, started on a
+circle around it and each cycling through its own waypoints across the arena, so their paths cross.  Every step, each
+robot's obstacles are the two static ones plus the other K - 1 robots' current positions (radius 0.3), and a robot
+within 0.5 of its goal moves on to its next waypoint: the task changes at every step, from GPU memory
+(loop.set_goals, loop.set_obstacles).  The parity check is as above, with the goal and obstacle calls replayed through
+params['xgoal'], params['obstacle_positions'] and params['obstacle_radius'].  Legs: device_loop, graph (the goals and
+obstacles computed and set inside the graph) and host (batch.solve(), then per robot the numpy plant step,
+shift_and_update and the new params); no run_trials leg, as the built-in plant has no moving obstacles.  --profile
+instead runs the device loop under torch.profiler (a run of its own) and reports each kernel's GPU time per step, with
+the robots as obstacles and with the two static obstacles only: whether the barebone rollout's per-step obstacle loop
+bounds the step."""
 import argparse
 import contextlib
 import io
@@ -68,15 +81,18 @@ def torch_plant(torch, x, u0, dt, grids, xlo, ylo, res, goal, tol):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", default="c2", choices=["c2", "c3", "bb", "ref"])
+    ap.add_argument("--workload", default="c2", choices=["c2", "c3", "bb", "ref", "swarm"])
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--closed-loop", type=int, default=40)
     ap.add_argument("--parity-steps", type=int, default=8)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--graph-steps", type=int, default=1)
+    ap.add_argument("--profile", action="store_true", help="swarm: kernel times per step under torch.profiler")
     args = ap.parse_args()
     if args.graph_steps < 1:
         ap.error("--graph-steps must be >= 1")
+    if args.workload == "swarm":
+        return run_swarm(args)
     import torch
     import __graft_entry__
     __graft_entry__.build_engine()
@@ -312,6 +328,261 @@ def main():
            "device_loop_over_graph": round(med["device_loop"] / med["graph"], 3),
            "graph_capture_seconds": [round(t, 4) for t in capture_seconds],
            "launches_per_round": launches}
+    print(json.dumps(out))
+
+
+SWARM_STATIC = [[5.0, 4.5, 1.5], [2.0, 1.0, 1.0]]     # the notebook's two obstacles
+SWARM_R, SWARM_CENTRE, SWARM_RADIUS, SWARM_WAYPOINTS = 0.3, (3.5, 2.75), 6.0, 3
+
+
+def swarm_params(K):
+    """Robot k starts on a circle of radius 6 around the arena's centre, heading in, and its waypoints are the points of
+    the circle 90, 180 and 270 degrees on; the notebook's planner otherwise (the bb workload's params)."""
+    cx, cy = SWARM_CENTRE
+    params, ways = [], []
+    for k in range(K):
+        a = 2 * np.pi * k / K
+        x0 = np.array([cx + SWARM_RADIUS * np.cos(a), cy + SWARM_RADIUS * np.sin(a), a + np.pi])
+        w = [[cx + SWARM_RADIUS * np.cos(a + np.pi * (j + 1) / 2), cy + SWARM_RADIUS * np.sin(a + np.pi * (j + 1) / 2)]
+             for j in range(SWARM_WAYPOINTS)]
+        ways.append(w)
+        params.append(dict(dt=0.1, x0=x0, xgoal=np.array(w[0]), goal_tolerance=0.5, dist_weight=10, lambda_weight=1.0,
+                           num_opt=1, u_std=np.array([1.0, 1.0]), vrange=np.array([0.0, 2.0]),
+                           wrange=np.array([-np.pi, np.pi]), obstacle_positions=np.array(SWARM_STATIC)[:, :2],
+                           obstacle_radius=np.array(SWARM_STATIC)[:, 2], obs_penalty=1e6))
+    return params, np.array(ways)
+
+
+def run_swarm(args):
+    import torch
+    import __graft_entry__
+    __graft_entry__.build_engine()
+    import mppi_numba_b200 as E
+    from bench_batch import gpu_info
+    K, S, G = args.batch, args.closed_loop, args.graph_steps
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    params, ways = swarm_params(K)
+    with contextlib.redirect_stdout(io.StringIO()):
+        A, Bs = _bb_planners(params), _bb_planners(params)
+    Op = 2 + K - 1
+    f64 = dict(dtype=torch.float64, device=dev)
+    dt = torch.full((K,), 0.1, **f64)
+    W = torch.tensor(ways, **f64)                          # (K, P, 2)
+    rows = torch.arange(K, device=dev)
+    others = torch.tensor([[j for j in range(K) if j != k] for k in range(K)], device=dev)
+    static = torch.tensor(SWARM_STATIC, **f64).expand(K, 2, 3)
+    radius = torch.full((K, K - 1, 1), SWARM_R, **f64)
+    main_stream, side = torch.cuda.current_stream(dev), torch.cuda.Stream(dev)
+
+    def reset(pls):
+        for p, q in zip(pls, params):
+            p.params["x0"] = q["x0"].copy()
+            p.params["xgoal"] = q["xgoal"].copy()
+            p.params["obstacle_positions"] = q["obstacle_positions"].copy()
+            p.params["obstacle_radius"] = q["obstacle_radius"].copy()
+            p.u_cur_d.copy_to_device(np.zeros((p.num_steps, 2), np.float32))
+
+    class State(object):
+        """The device-side step: plant, waypoint switch, obstacles from the robots' positions (static tensors)."""
+
+        def __init__(self, static_only=False):
+            self.x = torch.tensor(np.stack([q["x0"] for q in params]), **f64)
+            self.widx = torch.zeros(K, dtype=torch.int64, device=dev)
+            self.g = W[rows, self.widx].clone()
+            self.obs = torch.zeros((K, Op, 3), **f64)
+            self.counts = torch.full((K,), 2 if static_only else Op, dtype=torch.int32, device=dev)
+
+        def step(self, loop, u, record=None):
+            v, w = torch.nan_to_num(u[:, 0, 0].double()), torch.nan_to_num(u[:, 0, 1].double())
+            th = self.x[:, 2]
+            self.x.copy_(torch.stack([self.x[:, 0] + dt * torch.cos(th) * v, self.x[:, 1] + dt * torch.sin(th) * v,
+                                      th + dt * w], dim=1))
+            loop.shift_and_update(self.x)
+            near = torch.linalg.norm(self.x[:, :2] - self.g, dim=1) <= 0.5
+            self.widx.copy_((self.widx + near.long()) % SWARM_WAYPOINTS)
+            self.g.copy_(W[rows, self.widx])
+            loop.set_goals(self.g)
+            self.obs.copy_(torch.cat([static, torch.cat([self.x[others, :2], radius], dim=2)], dim=1))
+            loop.set_obstacles(self.obs, self.counts)
+            if record is not None:
+                record.append(("shift", self.x.cpu().numpy()))
+                record.append(("goals", self.g.cpu().numpy()))
+                record.append(("obstacles", self.obs.cpu().numpy(), self.counts.cpu().numpy()))
+
+    ba, bh = E.MPPI_Batch(A), E.MPPI_Batch(Bs)
+    for b in (ba, bh):
+        b.set_stream(main_stream.cuda_stream)
+
+    def loop_round(steps, record=None, static_only=False):
+        reset(A)
+        st = State(static_only)
+        with ba.device_loop(max_obstacles=Op) as loop:
+            for _ in range(steps):
+                u = torch.as_tensor(loop.solve(), device=dev)
+                if record is not None:
+                    record.append(("solve", u.cpu().numpy().copy()))
+                st.step(loop, u, record)
+        torch.cuda.synchronize(dev)
+        return loop
+
+    U = [torch.empty((K, A[0].num_steps, 2), dtype=torch.float32, device=dev) for _ in range(G)]
+    capture_seconds = []
+
+    def graph_round(steps, record=None):
+        reset(A)
+        ba.set_stream(side.cuda_stream)
+        with torch.cuda.stream(side):
+            st = State()
+
+            def step(loop, j):
+                loop.solve(out=U[j])
+                st.step(loop, U[j])
+
+            def keep(j):
+                record.append(("solve", U[j].cpu().numpy().copy()))
+                record.append(("shift", st.x.cpu().numpy()))
+                record.append(("goals", st.g.cpu().numpy()))
+                record.append(("obstacles", st.obs.cpu().numpy(), st.counts.cpu().numpy()))
+
+            with ba.device_loop(max_obstacles=Op) as loop:
+                step(loop, 0)
+                if record is not None:
+                    keep(0)
+                g = torch.cuda.CUDAGraph()
+                t0 = time.perf_counter()
+                g.capture_begin()
+                for j in range(G):
+                    step(loop, j)
+                g.capture_end()
+                capture_seconds.append(time.perf_counter() - t0)
+                for _ in range(-(-(steps - 1) // G)):
+                    g.replay()
+                    if record is not None:                 # G 1 in the parity check: the step's own state
+                        keep(0)
+        torch.cuda.synchronize(dev)
+        ba.set_stream(main_stream.cuda_stream)
+        return loop
+
+    def replayed_on_twins(calls):
+        reset(Bs)
+        ok = True
+        for k, p in enumerate(Bs):
+            one = E.MPPI_Batch([p])
+            for c in calls:
+                if c[0] == "solve":
+                    ok &= one.solve()[0].tobytes() == c[1][k].tobytes()
+                elif c[0] == "shift":
+                    p.shift_and_update(c[1][k].copy(), p.u_cur_d.copy_to_host(), 1)
+                elif c[0] == "goals":
+                    p.params["xgoal"] = c[1][k].copy()
+                else:
+                    n = int(c[2][k])
+                    p.params["obstacle_positions"] = c[1][k, :n, :2].copy()
+                    p.params["obstacle_radius"] = c[1][k, :n, 2].copy()
+        return ok
+
+    def state(p):
+        return [a.copy_to_host() for a in (p.u_cur_d, p.u_prev_d, p.costs_d, p.weights_d, p.noise_samples_d,
+                                           p.rng_states_d)] + [np.asarray(p.params[q], np.float64) for q in
+                                                               ("x0", "xgoal", "obstacle_positions", "obstacle_radius")]
+
+    if args.profile:
+        return swarm_profile(torch, dev, K, S, loop_round, gpu_info)
+
+    parity = {"planners": K, "steps": args.parity_steps,
+              "against": "the host loop replayed with the loop's poses, goals and obstacles on identical twins"}
+    for name, fn in (("device_loop", loop_round), ("graph", graph_round)):
+        if name == "graph" and G != 1:
+            continue                                       # the parity record keeps one step's state per replay
+        calls = []
+        with contextlib.redirect_stdout(io.StringIO()):
+            fn(args.parity_steps, calls)
+            ok_u = replayed_on_twins(calls)
+        ok_state = all(all(np.array_equal(x, y) for x, y in zip(state(a), state(b))) for a, b in zip(A, Bs))
+        parity[name] = {"passed": bool(ok_u and ok_state), "u_bitwise": bool(ok_u), "state_bitwise": bool(ok_state)}
+    parity["passed"] = all(v["passed"] for k, v in parity.items() if isinstance(v, dict))
+    if not parity["passed"]:
+        sys.stderr.write("bench_loop.py: PARITY CHECK FAILED: %s\n" % json.dumps(parity))
+        print(json.dumps({"metric": "device loop swarm", "error": "parity_check failed", "parity_check": parity}))
+        raise SystemExit(3)
+
+    def host_round():
+        reset(Bs)
+        x = [q["x0"].copy() for q in params]
+        widx = [0] * K
+        for _ in range(S):
+            u = bh.solve()
+            for k, p in enumerate(Bs):
+                th = x[k][2]
+                x[k] = np.array([x[k][0] + 0.1 * np.cos(th) * float(u[k, 0, 0]),
+                                 x[k][1] + 0.1 * np.sin(th) * float(u[k, 0, 0]), th + 0.1 * float(u[k, 0, 1])])
+                p.shift_and_update(x[k], u[k], 1)
+            for k, p in enumerate(Bs):
+                if np.linalg.norm(x[k][:2] - ways[k][widx[k]]) <= 0.5:
+                    widx[k] = (widx[k] + 1) % SWARM_WAYPOINTS
+                p.params["xgoal"] = ways[k][widx[k]].copy()
+                pos = np.array([x[j][:2] for j in range(K) if j != k]).reshape(-1, 2)
+                p.params["obstacle_positions"] = np.concatenate([np.array(SWARM_STATIC)[:, :2], pos])
+                p.params["obstacle_radius"] = np.concatenate([np.array(SWARM_STATIC)[:, 2], np.full(K - 1, SWARM_R)])
+        torch.cuda.synchronize(dev)
+
+    legs = [("device_loop", lambda: loop_round(S), ba), ("graph", lambda: graph_round(S), ba), ("host", host_round, bh)]
+    times = {name: [] for name, _, _ in legs}
+    launches = {}
+    with contextlib.redirect_stdout(io.StringIO()):
+        for _, fn, _ in legs:                              # warm-up
+            fn()
+        del capture_seconds[:]
+        for _ in range(args.rounds):
+            for name, fn, b in legs:
+                n0 = b.launch_count()
+                t0 = time.perf_counter()
+                fn()
+                times[name].append(time.perf_counter() - t0)
+                launches[name] = b.launch_count() - n0
+    med = {name: float(np.median(v)) for name, v in times.items()}
+    print(json.dumps({
+        "metric": "device loop swarm: goals and obstacles from GPU memory every step vs the host loop",
+        "config": {"workload": "swarm", "batch": K, "steps": S, "rounds": args.rounds, "obstacles_per_robot": Op,
+                   "N": A[0].num_control_rollouts, "T": A[0].num_steps, "graph_steps": G,
+                   "device_loop": "S x (solve, torch plant, shift, waypoint switch, set_goals, set_obstacles)",
+                   "graph": "one eager step, G steps captured, ceil((S - 1) / G) replays; open, capture, close included",
+                   "host": "S x (batch.solve(), numpy plant, shift_and_update, params xgoal and obstacles)"},
+        "gpu": gpu_info(dev), "parity_check": parity,
+        "round_seconds": {name: [round(t, 4) for t in v] for name, v in times.items()},
+        "median_seconds": {name: round(t, 4) for name, t in med.items()},
+        "host_over_device_loop": round(med["host"] / med["device_loop"], 3),
+        "device_loop_over_graph": round(med["device_loop"] / med["graph"], 3),
+        "graph_capture_seconds": [round(t, 4) for t in capture_seconds],
+        "launches_per_round": launches}))
+
+
+def swarm_profile(torch, dev, K, S, loop_round, gpu_info):
+    """Each kernel's GPU time per step of the swarm's device loop under torch.profiler, with the K + 1 obstacles and
+    with the two static ones only (counts 2), and the step's wall time without the profiler."""
+    from torch.profiler import ProfilerActivity, profile
+    out = {"metric": "device loop swarm: kernel time per step (torch.profiler)", "gpu": gpu_info(dev),
+           "config": {"batch": K, "steps": S, "obstacles_per_robot": {"robots": K + 1, "static_only": 2}}}
+    with contextlib.redirect_stdout(io.StringIO()):
+        for static_only in (False, True):
+            loop_round(S, static_only=static_only)        # warm-up
+            t0 = time.perf_counter()
+            loop_round(S, static_only=static_only)
+            wall = (time.perf_counter() - t0) / S
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                loop_round(S, static_only=static_only)
+            kern = {}
+            for e in prof.key_averages():
+                t = getattr(e, "device_time_total", None)
+                if t is None:
+                    t = e.cuda_time_total
+                if t > 0:
+                    kern[e.key] = round(t / S, 2)         # microseconds per step
+            total = sum(v for k, v in kern.items() if "Memcpy" not in k and "Memset" not in k)
+            top = dict(sorted(kern.items(), key=lambda kv: -kv[1])[:8])
+            out["static_only" if static_only else "robots"] = {
+                "step_wall_us": round(wall * 1e6, 1), "kernel_us_per_step": round(total, 1), "top_kernels_us": top}
     print(json.dumps(out))
 
 

@@ -652,6 +652,9 @@ int b200mppi_batch_run_mixed_trials(b200mppi_batch* b, const b200mppi_trial_desc
  * be captured (cudaStreamCaptureModeGlobal included) on the batch's stream and replayed any number of times, mixed
  * with eager calls: each replay is those calls at that point of the loop, bit for bit, reading the arrays captured.
  * Launches count where they are issued from the host: a capture counts once, a replay adds nothing.
+ * Task updates: b200mppi_loop_set_goals and (barebone loops) b200mppi_loop_set_obstacles give every running planner a new
+ * goal or obstacle set from device memory between solves, one launch each and capturable like the other calls.  Per
+ * planner they are set_params with that goal and set_obstacles with that set before its later solves, bit for bit.
  *
  * b200mppi_batch_loop_open: kind as in b200mppi_batch_run_trials_recorded (the batch's own kind).  padded_limits: float64
  * (count, 4) = padded x lo, x hi, y lo, y hi of each planner's map (the limits of the host's solve check; NULL for
@@ -659,6 +662,12 @@ int b200mppi_batch_run_mixed_trials(b200mppi_batch* b, const b200mppi_trial_desc
  * 0 .. count-1; NULL: row i).  The batch's descriptors are built from each planner's params as set now.  Refused
  * (B200MPPI_EINVAL naming the planner) before any work: what batch_solve refuses, num_opt < 1, another kind, a NaN limit,
  * bad rows, a loop already open; and what the trial of that kind refuses of the TDM pairs.
+ * b200mppi_batch_loop_open_ex: the same with an obstacle capacity O = max(max_obstacles, the largest obstacle count of
+ *   the batch's planners) per planner, allocated at open (a barebone loop can always set as many obstacles as it started
+ *   with).  max_obstacles outside [0, 2^24], or above 0 for a loop that is not barebone: B200MPPI_EINVAL.  A barebone
+ *   loop's rollouts read each planner's obstacles from its slice of the loop's buffer, filled at open with the planner's
+ *   current ones.  b200mppi_batch_loop_open is b200mppi_batch_loop_open_ex with max_obstacles 0.
+ * b200mppi_loop_obstacle_capacity: O.
  * While a loop is open, every planner and batch call that touches the state of the batch or its planners (solve, set_*,
  * get_u, shift_u, copy_in / copy_out, the stage calls, get_state_rollout, the trial calls, share_tdms, set_stream and
  * destroy) returns B200MPPI_EINVAL.
@@ -673,6 +682,16 @@ int b200mppi_batch_run_mixed_trials(b200mppi_batch* b, const b200mppi_trial_desc
  * b200mppi_loop_stop: mask_dev (count) of elem_bytes 4 (int32) or 1 (bool / uint8), indexed by row: a running planner
  *   whose entry is nonzero stops for good (B200MPPI_LOOP_STOPPED).  A stopped planner never runs again, so every running
  *   planner has solved equally often and one sampler parity serves them all.
+ * b200mppi_loop_set_goals: goal of planner i = row rows[i] of g_dev: 2 contiguous elements of dtype B200MPPI_POSE_F64 or
+ *   _F32 (widened exactly), rows row_stride_bytes apart.  Every running planner's later solves plan toward float32 of
+ *   it, as set_params with that goal.  Not checked, as set_params does not check the goal (NaN and inf pass).
+ * b200mppi_loop_set_obstacles: barebone loops only.  obs_dev: rows of count (O' <= O) triples [x, y, r], contiguous, of
+ *   dtype B200MPPI_POSE_F64 or _F32, rows row_stride_bytes apart (may be NULL when count is 0).  counts_dev: int32 (count)
+ *   by row, or NULL for O' each.  Every running planner's later solves take the first counts[rows[i]] triples of its
+ *   row as float32, as set_obstacles with that set (0: no obstacles).  A count outside [0, O'], which set_obstacles
+ *   refuses, stops that planner for good with status B200MPPI_LOOP_BAD_OBSTACLES; it keeps its last set.
+ *   Refused with B200MPPI_EINVAL before any work: a loop that is not barebone, O' > O, a null pointer, a bad dtype,
+ *   stride or alignment, an array outside the batch's device.
  * b200mppi_loop_wait_stream: the batch's stream waits (an event, not the host) for the work issued so far on stream.
  *   While the batch's stream captures a graph, B200MPPI_EINVAL unless stream is part of the same capture (an event
  *   recorded outside it would invalidate the capture).
@@ -683,25 +702,46 @@ int b200mppi_batch_run_mixed_trials(b200mppi_batch* b, const b200mppi_trial_desc
  *   per_planner (may be NULL): count summaries in the batch's order.
  *   While the batch's stream captures a graph: B200MPPI_EINVAL before any work, the loop left open and usable (close
  *   waits for the stream).  More than 2^31 - 1 solves issued: B200MPPI_ESTATE, the loop freed and the planners' counts
- *   not committed.  Any other error: the loop is freed. */
+ *   not committed.  Any other error: the loop is freed.
+ * b200mppi_loop_close_ex: b200mppi_loop_close that also commits the task updates and returns them per planner in the
+ *   batch's order (tasks, obstacles: may be NULL).  A planner that took a goal keeps its float32 in the C-side params; one
+ *   that took an obstacle set keeps that set (float32) as its own obstacles, the buffer grown if needed.  tasks[i]: what
+ *   planner i took; obstacles: (count, O, 3) float64, planner i's last set in its first tasks[i].num_obstacles triples.
+ *   A planner that never took a call is left as it was. */
 typedef struct b200mppi_loop b200mppi_loop;
 enum { B200MPPI_POSE_F64 = 0, B200MPPI_POSE_F32 = 1 };
-enum { B200MPPI_LOOP_RUNNING = 0, B200MPPI_LOOP_STOPPED = 5 };   /* and B200MPPI_TRIAL_LEFT_MAP */
+enum { B200MPPI_LOOP_RUNNING = 0, B200MPPI_LOOP_STOPPED = 5, B200MPPI_LOOP_BAD_OBSTACLES = 6 };   /* and B200MPPI_TRIAL_LEFT_MAP */
 typedef struct {
   int32_t solves, shifts;       /* solves and shifts the planner took */
-  int32_t status;               /* B200MPPI_LOOP_RUNNING, B200MPPI_TRIAL_LEFT_MAP or B200MPPI_LOOP_STOPPED */
+  int32_t status;               /* B200MPPI_LOOP_RUNNING, B200MPPI_TRIAL_LEFT_MAP, B200MPPI_LOOP_STOPPED or
+                                   B200MPPI_LOOP_BAD_OBSTACLES */
   int32_t pad_;
   double x[3];                  /* the last pose shift_and_update took (the params' x0 before the loop: shifts 0) */
 } b200mppi_loop_summary;
+typedef struct {
+  int32_t took_goal;            /* 1: the planner took a goal (b200mppi_loop_set_goals) */
+  int32_t took_obstacles;       /* 1: it took an obstacle set (b200mppi_loop_set_obstacles) */
+  int32_t num_obstacles;        /* the count of the last set it took */
+  int32_t pad_;
+  double goal[2];               /* the last goal it took, float64 (a float32 goal widened) */
+} b200mppi_loop_task;
 int b200mppi_batch_loop_open(b200mppi_batch* b, int32_t kind, const double* padded_limits, const int32_t* rows,
                              b200mppi_loop** out);
+int b200mppi_batch_loop_open_ex(b200mppi_batch* b, int32_t kind, const double* padded_limits, const int32_t* rows,
+                                int32_t max_obstacles, b200mppi_loop** out);
+int b200mppi_loop_obstacle_capacity(b200mppi_loop* loop, int32_t* capacity);
 int b200mppi_loop_controls(b200mppi_loop* loop, float** u_dev, void** stream);
 int b200mppi_loop_solve(b200mppi_loop* loop, float* u_dev);
 int b200mppi_loop_shift_and_update(b200mppi_loop* loop, const void* x_dev, int32_t dtype, int64_t row_stride_bytes);
 int b200mppi_loop_stop(b200mppi_loop* loop, const void* mask_dev, int32_t elem_bytes);
+int b200mppi_loop_set_goals(b200mppi_loop* loop, const void* g_dev, int32_t dtype, int64_t row_stride_bytes);
+int b200mppi_loop_set_obstacles(b200mppi_loop* loop, const void* obs_dev, int32_t dtype, int32_t count,
+                                int64_t row_stride_bytes, const int32_t* counts_dev);
 int b200mppi_loop_wait_stream(b200mppi_loop* loop, void* stream);
 int b200mppi_loop_active(b200mppi_loop* loop, const int32_t** dev);
 int b200mppi_loop_close(b200mppi_loop* loop, b200mppi_loop_summary* per_planner);
+int b200mppi_loop_close_ex(b200mppi_loop* loop, b200mppi_loop_summary* per_planner, b200mppi_loop_task* tasks,
+                           double* obstacles);
 
 #ifdef __cplusplus
 }

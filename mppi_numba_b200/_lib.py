@@ -65,8 +65,14 @@ class LoopSummary(C.Structure):
                 ("x", C.c_double * 3)]
 
 
+class LoopTask(C.Structure):
+    """b200mppi_loop_task"""
+    _fields_ = [("took_goal", C.c_int32), ("took_obstacles", C.c_int32), ("num_obstacles", C.c_int32),
+                ("pad_", C.c_int32), ("goal", C.c_double * 2)]
+
+
 POSE_F64, POSE_F32 = 0, 1
-LOOP_RUNNING, LOOP_STOPPED = 0, 5
+LOOP_RUNNING, LOOP_STOPPED, LOOP_BAD_OBSTACLES = 0, 5, 6
 EINVAL = -1
 
 
@@ -180,6 +186,11 @@ def _load():
         "b200mppi_loop_wait_stream": (C.c_int, [P, P]),
         "b200mppi_loop_active": (C.c_int, [P, C.POINTER(P)]),
         "b200mppi_loop_close": (C.c_int, [P, C.POINTER(LoopSummary)]),
+        "b200mppi_batch_loop_open_ex": (C.c_int, [P, I32, P, P, I32, C.POINTER(P)]),
+        "b200mppi_loop_obstacle_capacity": (C.c_int, [P, C.POINTER(I32)]),
+        "b200mppi_loop_set_goals": (C.c_int, [P, P, I32, I64]),
+        "b200mppi_loop_set_obstacles": (C.c_int, [P, P, I32, I32, I64, P]),
+        "b200mppi_loop_close_ex": (C.c_int, [P, C.POINTER(LoopSummary), C.POINTER(LoopTask), P]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)          # AttributeError here == ABI drift, fail loudly

@@ -144,10 +144,12 @@ class MPPI_Batch(object):
         if self._loop is not None:
             raise ValueError("%s: a device loop is open on this batch (close it first)" % name)
 
-    def device_loop(self):
-        """Open a ``DeviceLoop`` on the batch: ``solve()`` and ``shift_and_update(x)`` enqueued on the batch's stream,
-        poses and controls in GPU memory, for a plant of the caller's own (see DeviceLoop)."""
-        return DeviceLoop(self)
+    def device_loop(self, max_obstacles=0):
+        """Open a ``DeviceLoop`` on the batch: ``solve()``, ``shift_and_update(x)``, ``set_goals(g)`` and (barebone)
+        ``set_obstacles(obs)`` enqueued on the batch's stream, in GPU memory, for a plant of the caller's own (see
+        DeviceLoop).  ``max_obstacles``: a barebone loop's obstacle capacity per planner, at least the largest obstacle
+        count of its planners."""
+        return DeviceLoop(self, max_obstacles)
 
     def __len__(self):
         return len(self.planners)
@@ -742,7 +744,8 @@ class MPPI_MixedBatch(MPPI_Batch):
                          "runs barebone trials)")
 
 
-LOOP_STATUS = {_lib.LOOP_RUNNING: "running", _lib.TRIAL_LEFT_MAP: "left_map", _lib.LOOP_STOPPED: "stopped"}
+LOOP_STATUS = {_lib.LOOP_RUNNING: "running", _lib.TRIAL_LEFT_MAP: "left_map", _lib.LOOP_STOPPED: "stopped",
+               _lib.LOOP_BAD_OBSTACLES: "bad_obstacles"}
 
 
 class DeviceLoop(object):
@@ -769,14 +772,29 @@ class DeviceLoop(object):
     stops planner k for good when done[k] is nonzero.  A stopped planner's rows of later ``solve()`` outputs are NaN and
     it is left untouched by every later call.
 
+    The task can change between solves, from GPU memory, one launch per call (waypoints, a moving target, robots that
+    avoid each other):
+
+        loop.set_goals(g)                                             # (K, 2) float64 / float32 on the device
+        loop.set_obstacles(obs, counts)                               # barebone: (K, O', 3) [x, y, r], counts (K,) int32
+
+    ``set_goals(g)`` is ``p.params['xgoal'] = g[k]`` before planner k's later solves: they plan toward float32(g[k]).
+    ``set_obstacles(obs, counts)`` (barebone loops only) is ``p.params['obstacle_positions'] = obs[k, :n, :2]`` and
+    ``p.params['obstacle_radius'] = obs[k, :n, 2]`` with n = counts[k] (default O').  O' is at most the loop's
+    ``max_obstacles``: ``device_loop(max_obstacles=O)`` sets it, and it is never below the largest obstacle count of the
+    planners at open.  A count outside [0, O'], which the host's set_obstacles refuses, stops that planner for good with
+    status "bad_obstacles"; its rollouts keep the last set it took.
+
     While the loop is open, the batch's calls and every call that reads or writes a member's state on the host
     (``solve``, ``setup`` / ``set_params``, ``shift_and_update``, ``get_state`` / ``set_state``,
     ``get_state_rollout``, the TDM setters and ``sample_grids`` of its TDMs) raise ValueError naming the planner.
     Closing (``close()``, or leaving the ``with`` block, also on an exception) waits for the stream and commits every
     planner: afterwards each is exactly as after that host loop, ``params['x0']`` the float64 value of the last pose it
-    took (a float32 pose widened exactly), and ``solves``, ``shifts`` (K,) int and ``status`` (K,) of "running" |
-    "left_map" | "stopped" are set.  Launches: a solve issues what a trial step of the batch issues without its plant
-    step, plus one export; ``shift_and_update`` and ``stop`` one each.
+    took (a float32 pose widened exactly), ``params['xgoal']``, ``params['obstacle_positions']`` and
+    ``params['obstacle_radius']`` the float64 values of the last goal and obstacle set it took (a planner that took
+    none keeps its own), and ``solves``, ``shifts`` (K,) int and ``status`` (K,) of "running" | "left_map" | "stopped"
+    | "bad_obstacles" are set.  Launches: a solve issues what a trial step of the batch issues without its plant step,
+    plus one export; ``shift_and_update``, ``stop``, ``set_goals`` and ``set_obstacles`` one each.
 
     CUDA graphs.  Nothing a loop call passes to the GPU changes from one call to the next (the loop counts its solves on
     the device), so a whole step, the caller's plant included, can be captured once and replayed:
@@ -790,6 +808,8 @@ class DeviceLoop(object):
                 x.copy_(my_plant(x, u[:, 0]))
                 loop.stop(done_of(x, done))                           # optional: a device-computed stop
                 loop.shift_and_update(x)
+                goal.copy_(next_waypoint(x, goal))                    # optional: goals computed on the device
+                loop.set_goals(goal)
             with torch.cuda.stream(s):
                 step()                                                # warm-up: the loop's first step, eager
             g = torch.cuda.CUDAGraph()
@@ -805,9 +825,15 @@ class DeviceLoop(object):
     open, and a call while torch captures on a stream other than the loop's raises ValueError before anything is
     enqueued (its launches would run at once, outside the caller's graph)."""
 
-    def __init__(self, batch):
+    def __init__(self, batch, max_obstacles=0):
         name = "%s.device_loop" % type(batch).__name__
         batch._refuse_in_loop(name)
+        max_obstacles = int(max_obstacles)
+        if max_obstacles < 0:
+            raise ValueError("%s: max_obstacles %d < 0" % (name, max_obstacles))
+        if max_obstacles > 0 and batch.kind != "barebone":
+            raise ValueError("%s: max_obstacles %d for a %s batch (only barebone planners take obstacles)"
+                             % (name, max_obstacles, batch.kind))
         batch._check_groups(name)
         for i, p in enumerate(batch.planners):
             who = "%s: planner %d" % (name, batch.order[i])
@@ -828,9 +854,17 @@ class DeviceLoop(object):
                               dtype=np.float64)
         rows = np.array(batch.order, dtype=np.int32)
         h = C.c_void_p()
-        check(lib.b200mppi_batch_loop_open(batch._handle, kind, ptr(limits) if limits is not None else None, ptr(rows),
-                                           C.byref(h)))
+        lim = ptr(limits) if limits is not None else None
+        if max_obstacles:
+            check(lib.b200mppi_batch_loop_open_ex(batch._handle, kind, lim, ptr(rows), max_obstacles, C.byref(h)))
+        else:                                          # open_ex with 0
+            check(lib.b200mppi_batch_loop_open(batch._handle, kind, lim, ptr(rows), C.byref(h)))
         self._handle = h
+        cap = C.c_int32()
+        check(lib.b200mppi_loop_obstacle_capacity(h, C.byref(cap)))
+        self.max_obstacles = int(cap.value)
+        """the obstacle capacity O per planner: max(max_obstacles, the largest obstacle count of the planners at open)"""
+        self._tasks = False                            # a set_goals / set_obstacles call was issued
         u, st, act = C.c_void_p(), C.c_void_p(), C.c_void_p()
         check(lib.b200mppi_loop_controls(h, C.byref(u), C.byref(st)))
         check(lib.b200mppi_loop_active(h, C.byref(act)))
@@ -941,6 +975,43 @@ class DeviceLoop(object):
         p, typestr, _ = self._array(done, "stop", "done", (self.K,), ("<i4", "|b1", "|u1"))
         check(lib.b200mppi_loop_stop(self._handle, p, 4 if typestr == "<i4" else 1))
 
+    def set_goals(self, g):
+        """Every running planner's later solves plan toward float32(g[k]) ((K, 2) float64 or float32 on the batch's
+        device; rows may be strided, their elements not), as ``p.params['xgoal'] = g[k]`` before them.  Not checked:
+        NaN and inf pass, as the host passes them."""
+        self._live("set_goals")
+        p, typestr, row = self._array(g, "set_goals", "g", (self.K, 2), ("<f8", "<f4"), strided_rows=True)
+        self._tasks = True
+        check(lib.b200mppi_loop_set_goals(self._handle, p, _lib.POSE_F64 if typestr == "<f8" else _lib.POSE_F32, row))
+
+    def set_obstacles(self, obs, counts=None):
+        """Barebone loops: every running planner's later solves avoid the first counts[k] obstacles [x, y, r] of
+        obs[k] ((K, O', 3) float64 or float32 on the device, O' <= ``max_obstacles``; planner rows may be strided, the
+        triples of a planner C-contiguous; counts (K,) int32 on the device, default O'), as
+        ``p.params['obstacle_positions'] = obs[k, :n, :2]`` and ``p.params['obstacle_radius'] = obs[k, :n, 2]``
+        before them.  A count outside [0, O'] stops that planner for good with status "bad_obstacles"."""
+        self._live("set_obstacles")
+        name = "DeviceLoop.set_obstacles"
+        if self.batch.kind != "barebone":
+            raise ValueError("%s: a %s loop (only barebone planners take obstacles)" % (name, self.batch.kind))
+        try:
+            shape = tuple(int(v) for v in obs.__cuda_array_interface__["shape"])
+        except AttributeError:
+            shape = None                               # refused by _array
+        if shape is not None and (len(shape) != 3 or shape[0] != self.K or shape[2] != 3):
+            raise ValueError("%s: obs of shape %s, expected (%d, O', 3)" % (name, shape, self.K))
+        O = shape[1] if shape is not None else 0
+        if O > self.max_obstacles:
+            raise ValueError("%s: %d obstacles per planner, the loop's capacity is %d (device_loop(max_obstacles=...))"
+                             % (name, O, self.max_obstacles))
+        p, typestr, row = self._array(obs, "set_obstacles", "obs", (self.K, O, 3), ("<f8", "<f4"), strided_rows=True)
+        c = None
+        if counts is not None:
+            c, _, _ = self._array(counts, "set_obstacles", "counts", (self.K,), ("<i4",))
+        self._tasks = True
+        check(lib.b200mppi_loop_set_obstacles(self._handle, p, _lib.POSE_F64 if typestr == "<f8" else _lib.POSE_F32, O,
+                                              row, c))
+
     def close(self):
         """Wait for the stream, commit every planner (as after the host loop) and free the loop.  Idempotent.  Raises,
         with the loop left open, while the batch's stream captures a CUDA graph."""
@@ -950,7 +1021,13 @@ class DeviceLoop(object):
         self._refuse_foreign_capture("close")
         b = self.batch
         S = (_lib.LoopSummary * self.K)()
-        rc = lib.b200mppi_loop_close(h, S)
+        tasks, obs = None, None
+        if self._tasks:                                # the task updates' commit: close_ex
+            tasks = (_lib.LoopTask * self.K)()
+            obs = np.zeros((self.K, self.max_obstacles, 3), np.float64)
+            rc = lib.b200mppi_loop_close_ex(h, S, tasks, ptr(obs) if self.max_obstacles else None)
+        else:
+            rc = lib.b200mppi_loop_close(h, S)
         if rc == _lib.EINVAL:                          # refused before any work: the loop stays open
             check(rc)
         self._handle = None
@@ -970,4 +1047,10 @@ class DeviceLoop(object):
                 p.u_prev_d = p._u_prev_buf             # as each planner's own solve() does (mppi.py:292,362)
             if s.shifts > 0:
                 p.params["x0"] = np.array(s.x[:], dtype=np.float64)     # shift_and_update(x[k], ...)
+            if tasks is not None and tasks[j].took_goal:
+                p.params["xgoal"] = np.array(tasks[j].goal[:], dtype=np.float64)
+            if tasks is not None and tasks[j].took_obstacles:
+                n = int(tasks[j].num_obstacles)
+                p.params["obstacle_positions"] = obs[j, :n, :2].copy()
+                p.params["obstacle_radius"] = obs[j, :n, 2].copy()
         self.solves, self.shifts, self.status = solves, shifts, status

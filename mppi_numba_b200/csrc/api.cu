@@ -3008,11 +3008,11 @@ struct TrialLayout {
   struct Part { size_t set[2] = {}, grp = 0, mem = 0, cls = 0, cur = 0; };   // a kind's sampler sets (by parity),
   Part part[2];                                                     // group descriptors, members, class lists and
                                                                     // (loop) current set
-  size_t box = 0, rec = 0, grec = 0, state = 0, con = 0, res = 0, loop = 0, clock = 0, res_end = 0, tr = 0, act = 0,
-         seq = 0, start = 0, slot0 = 0;
+  size_t box = 0, rec = 0, grec = 0, state = 0, con = 0, res = 0, loop = 0, clock = 0, task = 0, obs64 = 0, res_end = 0,
+         tr = 0, act = 0, seq = 0, start = 0, slot0 = 0;
   size_t vis = 0, rflag = 0, head = 0;                 // head: the sections staged and uploaded with one copy
   std::vector<size_t> grid;                            // per slot
-  size_t vrec = 0, xh = 0, uh = 0, lu = 0, total = 0;
+  size_t vrec = 0, xh = 0, uh = 0, lu = 0, obs = 0, total = 0;
 };
 
 // One trial call passed through its phases: the request, both kinds' parts, the layout and the buffers
@@ -3042,6 +3042,7 @@ struct TrialCall {
   bool loop = false;
   const double* limits = nullptr;
   const int32_t* rows = nullptr;
+  int O = 0;                                           // a loop's obstacle capacity per planner (barebone)
 };
 
 // What a device loop checks in place of trial_validate: a batch that can solve, num_opt >= 1, padded limits for every
@@ -3179,6 +3180,8 @@ static TrialLayout trial_layout(const TrialCall& t) {
   L.res = s.take(nres * sizeof(TrialState));
   L.loop = s.take((t.loop ? K : 0) * sizeof(LoopState));   // a loop's per-planner counters and poses
   L.clock = s.take((t.loop ? 2 : 0) * sizeof(int));   // a loop's solve clock (LoopClock)
+  L.task = s.take((t.loop ? K : 0) * sizeof(LoopTask));   // a loop's task updates (LoopTaskArgs) and their float64
+  L.obs64 = s.take((t.loop ? K * t.O * 3 : 0) * sizeof(double));   // obstacle triples: read back at close
   L.res_end = s.end;
   L.tr = s.take(nslot * sizeof(TrialDev));
   L.act = s.take((K + 1) * sizeof(int));               // active (K), the count of running planners
@@ -3201,8 +3204,14 @@ static TrialLayout trial_layout(const TrialCall& t) {
   L.xh = s.take((t.loop ? 0 : nslot * (S + 1) * 3) * sizeof(double));
   L.uh = s.take(nslot * S * 2 * sizeof(float));
   L.lu = s.take((t.loop ? K * t.b->T * 2 : 0) * sizeof(float));   // a loop's own (K, T, 2) controls
+  L.obs = s.take((t.loop ? K * t.O * 3 : 0) * sizeof(float));      // the obstacles a barebone loop's rollouts read
   L.total = s.end;
   return L;
+}
+
+// A barebone loop's (O, 3) obstacle slice of planner i
+static float* loop_obstacles(const TrialCall& t, int i) {
+  return reinterpret_cast<float*>(t.d + t.L.obs) + (size_t)i * t.O * 3;
 }
 
 // Fills the pinned staging's head (the batch's descriptors, per-planner and per-slot trial state, box, vis and sequence
@@ -3256,6 +3265,15 @@ static int trial_call_stage(TrialCall& t) {
         const b200mppi_tdm* l = p->lin;
         td.win = &dw[r].WW;
         td.win_pxl = l->pxl[0]; td.win_pyl = l->pyl[0]; td.win_res = l->res; td.win_rows = l->rows; td.win_cols = l->cols;
+      }
+      // where the goal and obstacle calls write; a barebone planner reads its obstacles from its slice of the loop's
+      // buffer, filled with its current ones below (no capacity: the descriptor is left as it is, with no obstacles)
+      LoopTask& lt = reinterpret_cast<LoopTask*>(h + L.task)[i];
+      lt = LoopTask{};
+      lt.xgoal_out = sto ? dw[r].p.xgoal : dr[i].p.xgoal;
+      if (t.barebone) {
+        lt.num_obstacles_out = &dr[i].num_obstacles;
+        if (t.O > 0) reinterpret_cast<RolloutArgs*>(h + b->off_roll)[i].obstacles = loop_obstacles(t, i);
       }
     }
     for (int j = first[i]; j < first[i + 1] && !t.loop; ++j) {    // the planner's episodes: one, or its sequence
@@ -3349,10 +3367,17 @@ static int trial_call_stage(TrialCall& t) {
     int* slot0 = reinterpret_cast<int*>(h + L.slot0);
     const NoisePrepDesc* hn = reinterpret_cast<const NoisePrepDesc*>(h + b->off_nprep);
     for (int r = 0; r < t.K2; ++r) { slot0[r] = hn[r].slot; slot0[t.K2 + r] = hb[r].slot; }
+    std::memset(h + L.obs64, 0, (size_t)K * t.O * 3 * sizeof(double));
   }
   if (t.K2 > 0) t.g0 = *reinterpret_cast<const RolloutWinArgs*>(h + b->off_win);
   cudaStream_t st = b->stream;
   CU(cudaMemcpyAsync(d, h, L.head, cudaMemcpyHostToDevice, st));
+  for (int i = 0; i < K && t.loop && t.O > 0; ++i) {
+    const b200mppi_planner* p = b->pl[i];
+    if (p->num_obstacles > 0)
+      CU(cudaMemcpyAsync(loop_obstacles(t, i), p->obstacles, (size_t)p->num_obstacles * 3 * sizeof(float),
+                         cudaMemcpyDeviceToDevice, st));
+  }
   for (int j = 0; j < t.nslot && !t.barebone && !t.loop; ++j) {  // pageable sources: staged by the driver before the call returns
     if (t.in_place[j]) continue;
     const size_t bytes = (size_t)trials[j].height * trials[j].width * sizeof(double);
@@ -3736,6 +3761,7 @@ struct b200mppi_loop {
   TrialCall t{};
   LoopArgs la{};
   LoopClock lc{};
+  LoopTaskArgs ta{};
   cudaEvent_t ev = nullptr;            // orders the batch's stream after work on the stream of a caller's array
   ~b200mppi_loop() {
     cudaFree(t.d);
@@ -3757,19 +3783,29 @@ static int loop_device_ptr(const b200mppi_loop* lp, const void* p, const char* f
   return B200MPPI_OK;
 }
 
-extern "C" int b200mppi_batch_loop_open(b200mppi_batch* b, int32_t kind, const double* padded_limits,
-                                        const int32_t* rows, b200mppi_loop** out) {
+constexpr int LOOP_MAX_OBSTACLES = 1 << 24;
+
+extern "C" int b200mppi_batch_loop_open_ex(b200mppi_batch* b, int32_t kind, const double* padded_limits,
+                                           const int32_t* rows, int32_t max_obstacles, b200mppi_loop** out) {
   if (!b || !out) return fail(B200MPPI_EINVAL, "loop_open: null argument");
   if (b->loop) return loop_busy("loop_open");
   if (kind != B200MPPI_TRIALS_MAP && kind != B200MPPI_TRIALS_STOCHASTIC && kind != B200MPPI_TRIALS_BAREBONE &&
       kind != B200MPPI_TRIALS_MIXED)
     return fail(B200MPPI_EINVAL, "loop_open: unknown trial kind " + std::to_string(kind));
+  if (max_obstacles < 0 || max_obstacles > LOOP_MAX_OBSTACLES)
+    return fail(B200MPPI_EINVAL, "loop_open: max_obstacles " + std::to_string(max_obstacles) + " outside [0, 2^24]");
+  if (max_obstacles > 0 && kind != B200MPPI_TRIALS_BAREBONE)
+    return fail(B200MPPI_EINVAL, "loop_open: max_obstacles " + std::to_string(max_obstacles) + " for a loop that is not "
+                                 "barebone (only barebone planners take obstacles)");
   std::unique_ptr<b200mppi_loop> lp(new b200mppi_loop());
   TrialCall& t = lp->t;
   t.b = b; t.kind = trial_kind(kind); t.S = 0;
   t.loop = true; t.limits = padded_limits; t.rows = rows;
   int rc;
   if ((rc = trial_call_validate(t)) || (rc = trial_call_plan(t))) return rc;
+  // the capacity: a barebone loop can always set again as many obstacles as any of its planners has now
+  t.O = max_obstacles;
+  for (int i = 0; i < t.K && t.barebone; ++i) t.O = std::max(t.O, b->pl[i]->num_obstacles);
   t.L = trial_layout(t);
   if (cudaMalloc(&t.d, t.L.total) != cudaSuccess) {
     t.d = nullptr;
@@ -3797,9 +3833,22 @@ extern "C" int b200mppi_batch_loop_open(b200mppi_batch* b, int32_t kind, const d
   lc.slot0 = reinterpret_cast<const int*>(t.d + t.L.slot0);
   lc.K2 = t.K2;
   lc.num_opt = b->pl[0]->prm.num_opt;
+  lp->ta = LoopTaskArgs{reinterpret_cast<LoopTask*>(t.d + t.L.task), reinterpret_cast<float*>(t.d + t.L.obs),
+                        reinterpret_cast<double*>(t.d + t.L.obs64), t.O};
   b->loop = lp.get();
   for (b200mppi_planner* p : b->pl) p->loop = lp.get();
   *out = lp.release();
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_batch_loop_open(b200mppi_batch* b, int32_t kind, const double* padded_limits,
+                                        const int32_t* rows, b200mppi_loop** out) {
+  return b200mppi_batch_loop_open_ex(b, kind, padded_limits, rows, 0, out);
+}
+
+extern "C" int b200mppi_loop_obstacle_capacity(b200mppi_loop* lp, int32_t* capacity) {
+  if (!lp || !capacity) return fail(B200MPPI_EINVAL, "loop_obstacle_capacity: null argument");
+  *capacity = lp->t.O;
   return B200MPPI_OK;
 }
 
@@ -3886,13 +3935,67 @@ extern "C" int b200mppi_loop_stop(b200mppi_loop* lp, const void* mask_dev, int32
   return B200MPPI_OK;
 }
 
+// A caller's (count, n) array of dtype B200MPPI_POSE_F64 / _F32, rows row_stride_bytes apart: the stride holds a row
+// and is a whole number of elements, and the pointer is aligned to the element
+static int loop_rows_ok(const void* p, int32_t dtype, int64_t n, int64_t row_stride_bytes, const char* fn,
+                        const char* what) {
+  if (dtype != B200MPPI_POSE_F64 && dtype != B200MPPI_POSE_F32)
+    return fail(B200MPPI_EINVAL, std::string(fn) + ": unknown " + what + " dtype " + std::to_string(dtype));
+  const int64_t e = dtype == B200MPPI_POSE_F64 ? 8 : 4;
+  if (row_stride_bytes < n * e || row_stride_bytes % e != 0 || reinterpret_cast<uintptr_t>(p) % e != 0)
+    return fail(B200MPPI_EINVAL, std::string(fn) + ": row stride of " + std::to_string(row_stride_bytes) + " bytes or a " +
+                                 "pointer not aligned to the element (rows of " + std::to_string(n) +
+                                 " contiguous elements)");
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_loop_set_goals(b200mppi_loop* lp, const void* g_dev, int32_t dtype, int64_t row_stride_bytes) {
+  if (!lp || !g_dev) return fail(B200MPPI_EINVAL, "loop_set_goals: null argument");
+  int rc;
+  if ((rc = loop_rows_ok(g_dev, dtype, 2, row_stride_bytes, "loop_set_goals", "goal"))) return rc;
+  if ((rc = loop_device_ptr(lp, g_dev, "loop_set_goals", "g_dev"))) return rc;
+  b200mppi_batch* b = lp->t.b;
+  CU(cudaSetDevice(b->device));
+  launch_loop_goal(lp->la, lp->ta, g_dev, dtype, row_stride_bytes, b->stream);
+  b->launches++;
+  CHECK_LAUNCH();
+  return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_loop_set_obstacles(b200mppi_loop* lp, const void* obs_dev, int32_t dtype, int32_t count,
+                                           int64_t row_stride_bytes, const int32_t* counts_dev) {
+  if (!lp || (!obs_dev && count > 0)) return fail(B200MPPI_EINVAL, "loop_set_obstacles: null argument");
+  if (!lp->t.barebone)
+    return fail(B200MPPI_EINVAL, "loop_set_obstacles: the loop is not barebone (only barebone planners take obstacles)");
+  if (count < 0 || count > lp->t.O)
+    return fail(B200MPPI_EINVAL, "loop_set_obstacles: " + std::to_string(count) + " obstacles per planner, the loop's "
+                                 "capacity is " + std::to_string(lp->t.O) + " (b200mppi_batch_loop_open_ex's "
+                                 "max_obstacles)");
+  int rc;
+  if ((rc = loop_rows_ok(obs_dev, dtype, 3 * (int64_t)count, row_stride_bytes, "loop_set_obstacles", "obstacle")))
+    return rc;
+  if (count > 0 && (rc = loop_device_ptr(lp, obs_dev, "loop_set_obstacles", "obs_dev"))) return rc;
+  if (counts_dev) {
+    if (reinterpret_cast<uintptr_t>(counts_dev) % 4 != 0)
+      return fail(B200MPPI_EINVAL, "loop_set_obstacles: counts not aligned to its int32 elements");
+    if ((rc = loop_device_ptr(lp, counts_dev, "loop_set_obstacles", "counts_dev"))) return rc;
+  }
+  b200mppi_batch* b = lp->t.b;
+  CU(cudaSetDevice(b->device));
+  launch_loop_obstacles(lp->la, lp->ta, obs_dev, dtype, count, row_stride_bytes, counts_dev, b->stream);
+  b->launches++;
+  CHECK_LAUNCH();
+  return B200MPPI_OK;
+}
+
 extern "C" int b200mppi_loop_active(b200mppi_loop* lp, const int32_t** dev) {
   if (!lp || !dev) return fail(B200MPPI_EINVAL, "loop_active: null argument");
   *dev = lp->t.pa.active;
   return B200MPPI_OK;
 }
 
-extern "C" int b200mppi_loop_close(b200mppi_loop* lp, b200mppi_loop_summary* per_planner) {
+extern "C" int b200mppi_loop_close_ex(b200mppi_loop* lp, b200mppi_loop_summary* per_planner,
+                                      b200mppi_loop_task* tasks, double* obstacles) {
   if (!lp) return fail(B200MPPI_EINVAL, "loop_close: null loop");
   TrialCall& t = lp->t;
   b200mppi_batch* b = t.b;
@@ -3905,7 +4008,7 @@ extern "C" int b200mppi_loop_close(b200mppi_loop* lp, b200mppi_loop_summary* per
   b->loop = nullptr;                                   // closed whatever follows: the batch and planners are free again
   for (b200mppi_planner* p : b->pl) p->loop = nullptr;
   CU(cudaSetDevice(b->device));
-  // the box records through the loop's counters, poses and solve clock, in one copy
+  // the box records through the loop's counters, poses, solve clock and task updates, in one copy
   CU(cudaMemcpyAsync(t.h + t.L.rec, t.d + t.L.rec, t.L.res_end - t.L.rec, cudaMemcpyDeviceToHost, b->stream));
   CU(cudaStreamSynchronize(b->stream));
   if (reinterpret_cast<const int*>(t.h + t.L.clock)[1]) {
@@ -3925,5 +4028,37 @@ extern "C" int b200mppi_loop_close(b200mppi_loop* lp, b200mppi_loop_summary* per
     }
   }
   trial_commit_planners(t, ran, x0);
+  // the C-side params and obstacles as set_params and set_obstacles of the last goal and obstacle set would leave them
+  const LoopTask* lt = reinterpret_cast<const LoopTask*>(t.h + t.L.task);
+  const double* o64 = reinterpret_cast<const double*>(t.h + t.L.obs64);
+  bool copied = false;
+  for (int i = 0; i < t.K; ++i) {
+    b200mppi_planner* p = b->pl[i];
+    if (tasks) {
+      tasks[i] = b200mppi_loop_task{lt[i].took_goal, lt[i].took_obstacles, lt[i].num_obstacles, 0,
+                                    {lt[i].goal[0], lt[i].goal[1]}};
+    }
+    if (lt[i].took_goal)
+      for (int c = 0; c < 2; ++c) p->prm.xgoal[c] = (float)lt[i].goal[c];
+    if (!lt[i].took_obstacles) continue;
+    const int n = lt[i].num_obstacles;
+    if (n > p->obstacles_cap) {
+      cudaFree(p->obstacles); p->obstacles = nullptr; p->obstacles_cap = 0; p->num_obstacles = 0;
+      CU(cudaMalloc(&p->obstacles, (size_t)n * 3 * sizeof(float)));
+      p->obstacles_cap = n;
+    }
+    if (n > 0) {
+      CU(cudaMemcpyAsync(p->obstacles, loop_obstacles(t, i), (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToDevice,
+                         b->stream));
+      copied = true;
+    }
+    p->num_obstacles = n;
+  }
+  if (obstacles) std::memcpy(obstacles, o64, (size_t)t.K * t.O * 3 * sizeof(double));
+  if (copied) CU(cudaStreamSynchronize(b->stream));   // before the loop's buffer is freed
   return B200MPPI_OK;
+}
+
+extern "C" int b200mppi_loop_close(b200mppi_loop* lp, b200mppi_loop_summary* per_planner) {
+  return b200mppi_loop_close_ex(lp, per_planner, nullptr, nullptr);
 }

@@ -638,9 +638,32 @@ struct LoopClock {
   int K2, num_opt;
 };
 // [emu:end loop_clock_args]
+// [emu:begin loop_task_args]
+// A loop's task updates (b200mppi_loop_set_goals / _set_obstacles): per planner where its rollout descriptor in the
+// loop's buffer keeps the goal and the obstacle count, and what it took, read back at close.
+enum { LOOP_BAD_OBSTACLES = 6 };          // LoopState::status: an obstacle count outside [0, O']
+struct LoopTask {
+  double goal[2];                         // the last goal taken, float64 (a float32 goal widened)
+  float* xgoal_out;                       // RolloutParams::xgoal of the planner (RolloutArgs or RolloutWinArgs)
+  int* num_obstacles_out;                 // RolloutArgs::num_obstacles of a barebone planner, else null
+  int took_goal, took_obstacles;          // 1 once the planner took a goal / an obstacle set
+  int num_obstacles;                      // the count of the last obstacle set taken
+  int pad_;
+};
+struct LoopTaskArgs {
+  LoopTask* task;                         // (K), in the batch's order
+  float* obs;                             // (K, O, 3): planner k's slice is what its RolloutArgs::obstacles points at
+  double* obs64;                          // (K, O, 3): the triples as taken, float64
+  int O;                                  // the loop's obstacle capacity
+};
+// [emu:end loop_task_args]
 void launch_loop_export(const LoopArgs& a, const LoopClock& c, float* u_out, cudaStream_t st);
 void launch_loop_ingest(const LoopArgs& a, const void* x, int dtype, long long row_stride, cudaStream_t st);
 void launch_loop_stop(const LoopArgs& a, const void* mask, int elem_bytes, cudaStream_t st);
+void launch_loop_goal(const LoopArgs& a, const LoopTaskArgs& ta, const void* g, int dtype, long long row_stride,
+                      cudaStream_t st);
+void launch_loop_obstacles(const LoopArgs& a, const LoopTaskArgs& ta, const void* obs, int dtype, int count,
+                           long long row_stride, const int* counts, cudaStream_t st);
 
 // visualisation rollouts (mppi.py:1194-1351)
 // [emu:begin vis_args]

@@ -621,6 +621,86 @@ __device__ __forceinline__ void loop_clock_body(const LoopClock& a) {
 }
 // [emu:end loop_clock]
 
+// [emu:begin loop_task]
+// Element c of a caller's row r: float64, or float32 widened exactly; *f is what set_params would pass (float32)
+__device__ __forceinline__ double loop_elem(const unsigned char* r, int dtype, int c, float* f) {
+  if (dtype == LOOP_POSE_F32) {
+    *f = reinterpret_cast<const float*>(r)[c];
+    return (double)*f;
+  }
+  const double v = reinterpret_cast<const double*>(r)[c];
+  *f = __double2float_rn(v);
+  return v;
+}
+
+// One thread per planner: a running planner takes the goal of row `row` of g (2 elements, float64 or float32; rows
+// row_stride bytes apart).  Its rollout descriptor's goal becomes float32 of it, as set_params passes it, and the
+// float64 value is kept for the commit.  Nothing is checked: set_params takes any goal.
+__device__ __forceinline__ void loop_goal_body(const LoopArgs& a, const LoopTaskArgs& ta,
+                                               const unsigned char* __restrict__ g, int dtype, long long row_stride,
+                                               int k) {
+  if (k >= a.K || !a.active[k]) return;
+  LoopTask& q = ta.task[k];
+  const unsigned char* r = g + (long long)a.state[k].row * row_stride;
+  for (int c = 0; c < 2; ++c) {
+    float f;
+    q.goal[c] = loop_elem(r, dtype, c, &f);
+    q.xgoal_out[c] = f;
+  }
+  q.took_goal = 1;
+}
+
+__global__ void __launch_bounds__(128) loop_goal_kernel(const LoopArgs a, const LoopTaskArgs ta,
+                                                        const unsigned char* __restrict__ g, int dtype,
+                                                        long long row_stride) {
+  loop_goal_body(a, ta, g, dtype, row_stride, (int)(blockIdx.x * blockDim.x + threadIdx.x));
+}
+
+// One warp per planner (warp k of the grid = planner k): a running planner takes the first n triples [x, y, r] of row
+// `row` of obs (count = O' triples per row, contiguous, float64 or float32; rows row_stride bytes apart), n =
+// counts[row] (counts null: O').  Float32 of each element goes into the planner's slice of the loop's buffer, which
+// its rollout descriptor reads, the float64 values into the shadow for the commit, and the descriptor's obstacle count
+// becomes n.  A count outside [0, O'], which the host's set_obstacles refuses, stops the planner for good
+// (LOOP_BAD_OBSTACLES); its rollouts keep the last set it took.
+__device__ __forceinline__ void loop_obstacles_body(const LoopArgs& a, const LoopTaskArgs& ta,
+                                                    const unsigned char* __restrict__ obs, int dtype, int count,
+                                                    long long row_stride, const int* __restrict__ counts, int k,
+                                                    int lane) {
+  if (k >= a.K || !a.active[k]) return;
+  LoopState& s = a.state[k];
+  const int n = counts ? counts[s.row] : count;
+  if (n < 0 || n > count) {
+    if (lane == 0) {
+      s.status = LOOP_BAD_OBSTACLES;
+      a.active[k] = 0;
+      atomicSub(a.active_count, 1);
+    }
+    return;
+  }
+  const unsigned char* r = obs + (long long)s.row * row_stride;
+  float* o = ta.obs + (size_t)k * ta.O * 3;
+  double* o64 = ta.obs64 + (size_t)k * ta.O * 3;
+  for (int j = lane; j < 3 * n; j += 32) {
+    float f;
+    o64[j] = loop_elem(r, dtype, j, &f);
+    o[j] = f;
+  }
+  if (lane != 0) return;
+  LoopTask& q = ta.task[k];
+  *q.num_obstacles_out = n;
+  q.num_obstacles = n;
+  q.took_obstacles = 1;
+}
+
+__global__ void __launch_bounds__(128) loop_obstacles_kernel(const LoopArgs a, const LoopTaskArgs ta,
+                                                             const unsigned char* __restrict__ obs, int dtype,
+                                                             int count, long long row_stride,
+                                                             const int* __restrict__ counts) {
+  loop_obstacles_body(a, ta, obs, dtype, count, row_stride, counts,
+                      (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), (int)(threadIdx.x & 31));
+}
+// [emu:end loop_task]
+
 // the export of a loop solve, and (CTA 0) the preparation of the next
 __global__ void __launch_bounds__(128) loop_export_kernel(const LoopArgs a, float* __restrict__ out, const LoopClock c) {
   loop_export_body(a, out, (int)blockIdx.x);
@@ -638,6 +718,18 @@ void launch_loop_ingest(const LoopArgs& a, const void* x, int dtype, long long r
 
 void launch_loop_stop(const LoopArgs& a, const void* mask, int elem_bytes, cudaStream_t st) {
   loop_stop_kernel<<<(unsigned)((a.K + 127) / 128), 128, 0, st>>>(a, mask, elem_bytes);
+}
+
+void launch_loop_goal(const LoopArgs& a, const LoopTaskArgs& ta, const void* g, int dtype, long long row_stride,
+                      cudaStream_t st) {
+  loop_goal_kernel<<<(unsigned)((a.K + 127) / 128), 128, 0, st>>>(a, ta, reinterpret_cast<const unsigned char*>(g),
+                                                                  dtype, row_stride);
+}
+
+void launch_loop_obstacles(const LoopArgs& a, const LoopTaskArgs& ta, const void* obs, int dtype, int count,
+                           long long row_stride, const int* counts, cudaStream_t st) {
+  loop_obstacles_kernel<<<(unsigned)((a.K + 3) / 4), 128, 0, st>>>(a, ta, reinterpret_cast<const unsigned char*>(obs),
+                                                                    dtype, count, row_stride, counts);
 }
 
 void launch_plant_step(const PlantArgs& a, cudaStream_t st) {
